@@ -58,18 +58,17 @@ def bench_config(args, world):
                         "glorot random-init parameters" % (which, B),
             "global_batch": world * B, "trajectory": T, "parallelism": "dp%d" % world,
             "scaling_mode": args.scaling,
-            "l2": "inputs+activations+params ~%d MB/step %s 126 MB L2; two staging slots alternate"
-                  % (int(7.2 * B), ">" if 7.2 * B > 126 else "<"),
-            "arms": "ours: hand-written sm_100a kernels behind the C-ABI (csrc/libdrl_b200.so); reference: float32 "
+            "l2": "inputs+activations+params ~%d MB/step %s 50 MB L2; two staging slots alternate"
+                  % (int(7.2 * B), ">" if 7.2 * B > 50 else "<"),
+            "arms": "ours: hand-written sm_90a kernels behind the C-ABI (csrc/libdrl_b200.so); reference: float32 "
                     "torch-CPU restatement of the TF1 graph on the host cores (TF 1.14 is not installable), a bounded "
                     "sample of min(global_batch, 32) trajectories per step"}
 
 
 MATH_MODES = {1: "FP32 FFMA (CUDA cores)",
-              2: "tcgen05 kind::tf32, 3xTF32 split (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi), fp32 TMEM accumulate",
-              3: "tcgen05 kind::tf32 3xTF32, persistent warp-specialised kernels (dedicated epilogue warps)",
-              4: "tcgen05 kind::tf32 3xTF32 with TMA-fed conv2/conv3 forward (tensor loads of value + tf32-remainder planes)",
-              5: "tcgen05 kind::f16 with 16-bit split operands (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi, fp32 TMEM accumulate; "
+              2: "wgmma tf32, 3xTF32 split (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi), fp32 register accumulate",
+              3: "wgmma tf32 3xTF32, persistent warp-specialised kernels",
+              5: "wgmma f16/bf16 with 16-bit split operands (A_lo*B_hi + A_hi*B_lo + A_hi*B_hi, fp32 register accumulate; "
                  "bf16 hi/lo planes, uint8 frames exact in fp16)"}
 
 
@@ -100,10 +99,10 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, src="H100 SXM data sheet (dense bf16), not measured")
 
 
-# ---- clocks sampling (B200_PROFILING.md) -------------------------------------------------------
+# ---- clocks sampling -------------------------------------------------------
 class ClockSampler:
     """SM clock / throttle reasons sampled DURING the timed region.  The timed region of the default run is
     only tens of milliseconds, shorter than one `nvidia-smi -lms` period, so NVML is polled directly from a
@@ -208,20 +207,6 @@ def kernel_flops(name, M, Mb):
     return tbl.get(name)
 
 
-# DRAM bytes (dram__bytes_read.sum + dram__bytes_write.sum) per launch at B=32, T=20 from the ncu --set full
-# capture summarised in profiles/r01_ncu_umma_full.md (tcgen05 path; conv*_dgrad = the dCol GEMM part only).
-NCU_TRAFFIC_B32 = {"lstm_fwd": 38.70e6, "lstm_wgrad": 10.25e6, "lstm_dgrad": 37.94e6, "conv1_fwd": 18.18e6,
-                   "conv2_fwd": 33.09e6, "conv3_fwd": 13.62e6, "conv1_wgrad": 46.14e6, "conv2_wgrad": 41.79e6,
-                   "conv3_wgrad": 19.22e6, "conv2_dgrad": 49.42e6, "conv3_dgrad": 16.57e6}
-
-
-# the same for the split-16 kernels (math mode 5), from profiles/r02_ncu_umma16_full.md
-# (+ profiles/r02_ncu_conv1_tma.md for the two frame-resident conv1 kernels; lstm_wgrad is the bulk-fed kernel now: not captured)
-NCU_TRAFFIC_B32_M5 = {"conv2_fwd": 32.95e6, "conv3_fwd": 13.47e6, "lstm_fwd": 23.68e6,
-                      "lstm_dgrad": 23.78e6, "conv3_wgrad": 19.21e6, "conv3_dgrad": 16.60e6, "conv2_wgrad": 41.74e6,
-                      "conv2_dgrad": 50.96e6, "conv1_fwd": 18.21e6, "conv1_wgrad": 46.13e6}
-
-
 def step_flops(B):
     M, Mb = B * T, B * (T - 2)
     return 2.0 * 11810048 * M + 2.0 * 2.0 * 11810048 * Mb       # SURVEY.md App. B (upper bound incl. conv1 dgrad)
@@ -291,6 +276,19 @@ def run_reference(args):
 
 
 # ---- our arm ----------------------------------------------------------------------------------------
+def dump_outputs(d, eng, out):
+    """What the last timed step handed its caller, as float32 / float64 .npy files under `d` (~33 MB at B = 32): the
+    step's scalars, its V-trace taps, the gradient of total_loss and the parameters after the update.  The inputs are
+    fixed seeded batches and the parameters start from init_params(seed=0), so two builds compare output for output."""
+    os.makedirs(d, exist_ok=True)
+    keys = ("pi_loss", "baseline_loss", "entropy", "learning_rate", "grad_norm", "total_loss", "step")
+    np.save(os.path.join(d, "step_scalars.npy"), np.array([out[k] for k in keys], np.float64))
+    for k, v in eng.taps().items():
+        np.save(os.path.join(d, "%s.npy" % k), v.astype(np.float32))
+    np.save(os.path.join(d, "grads.npy"), eng.get_grads().astype(np.float32))
+    np.save(os.path.join(d, "params.npy"), eng.get_params().astype(np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -385,6 +383,8 @@ def run_ours(args):
     barrier()
     ms_dev = max_over_ranks(e0.elapsed_time(e1))
     launches = eng.launches_per_step() * K
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, out)
 
     # ---------------- end to end through host buffers (`e2e`) ----------------
     for i in range(2):       # warm the copy path
@@ -442,13 +442,8 @@ def run_ours(args):
                 "kernel": name, "bound": "tensor", "achieved": ach, "peak": peaks["tf_sus"], "unit": "TFLOP/s",
                 "frac": ach / peaks["tf_sus"],
                 # fp32-grade results cost 3 tf32 MMAs per product and tf32 runs at half the bf16 rate:
-                "frac_of_3xtf32_ceiling": ach / (peaks["tf_sus"] / 6.0) if args.math_mode in (2, 3, 4) else None,
+                "frac_of_3xtf32_ceiling": ach / (peaks["tf_sus"] / 6.0) if args.math_mode in (2, 3) else None,
                 "frac_of_3x16bit_ceiling": ach / (peaks["tf_sus"] / 3.0) if args.math_mode == 5 else None,
-                "traffic": (NCU_TRAFFIC_B32.get(name) if args.math_mode == 2 else
-                            NCU_TRAFFIC_B32_M5.get(name) if args.math_mode == 5 else None) if B == 32 else None,
-                "traffic_source": (("profiles/r02_ncu_conv1_tma.md" if name.startswith("conv1") else
-                                    "profiles/r02_ncu_umma16_full.md") if args.math_mode == 5 else
-                                   "profiles/r01_ncu_umma_full.md") + " (ncu --set full, dram read + write per launch)",
                 "peak_source": peaks["src"] + " bf16 sustained",
                 "math_mode": MATH_MODES[args.math_mode] + "; achieved = algorithmic 2MNK flops (counted once, "
                              "not x3) / CUDA-event time",
@@ -506,8 +501,6 @@ def run_ours(args):
 
 
 # dram__bytes_read.sum + dram__bytes_write.sum per launch of vtrace_from_softmax_pipe_kernel at [65536,18,18], from the
-# ncu --set full capture summarised in profiles/r02_ncu_vtrace.md
-NCU_TRAFFIC_VTRACE = 201.4e6
 
 
 def vtrace_roofline(torch, peaks, Bv=65536, Tv=18, reps=20):
@@ -563,14 +556,14 @@ def vtrace_roofline(torch, peaks, Bv=65536, Tv=18, reps=20):
     nbytes = Bv * Tv * (2 * A * 4 + 4 * 4 + 8) + Bv * 4
     ach = nbytes / (ms * 1e-3) / 1e9
     single = float(np.median(ts))
-    big = nbytes > (126 << 20)
+    big = nbytes > (50 << 20)
     return {"kernel": "vtrace_from_softmax_pipe_kernel", "bound": "hbm", "achieved": ach, "peak": peaks["hbm"],
             "unit": "GB/s", "frac": ach / peaks["hbm"],
-            "traffic": NCU_TRAFFIC_VTRACE if (big and Bv == 65536) else None, "peak_source": peaks["src"],
+            "peak_source": peaks["src"],
             "bytes_per_launch": nbytes, "bytes_per_element": 168, "kernel_ms": ms, "kernel_ms_single_flushed": single,
             "achieved_single_flushed": nbytes / (single * 1e-3) / 1e9,
             "frac_single_flushed": nbytes / (single * 1e-3) / 1e9 / peaks["hbm"],
-            "l2": ("%.0f MB streamed per launch > 126 MB L2" % (nbytes / 1e6) if big else
+            "l2": ("%.0f MB streamed per launch > 50 MB L2" % (nbytes / 1e6) if big else
                    "%.0f KB per launch: L2-resident, launch-latency bound (reported for the learner's own size)"
                    % (nbytes / 1e3)) + "; %d back-to-back launches between one event pair; single = one launch after "
                   "an explicit 256 MB L2 flush" % REPS,
@@ -658,8 +651,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-graph", action="store_true", help="launch kernels directly instead of CUDA graphs")
-    ap.add_argument("--math-mode", type=int, default=5, choices=[1, 2, 3, 4, 5],
-                    help="1 = FP32 FFMA contractions, 2 = tcgen05 3xTF32, 5 = tcgen05 kind::f16 with 16-bit split operands (default)")
+    ap.add_argument("--math-mode", type=int, default=5, choices=[1, 2, 3, 5],
+                    help="1 = FP32 FFMA contractions, 2 = wgmma 3xTF32, 3 = same, persistent kernels, "
+                         "5 = wgmma with 16-bit split operands (default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (scalars, V-trace taps, gradient, "
+                         "updated parameters) as DIR/<name>.npy")
     ap.add_argument("--no-cpu-baseline", dest="cpu_baseline", action="store_false")
     ap.add_argument("--no-agent-api", dest="agent_api", action="store_false",
                     help="skip the e2e_agent_api leg (the unchanged train_impala.py loop body on impala.Agent)")

@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``agent/a3c.py``: same constructor kwargs, methods and return values (the
+"""H100-native stand-in for the reference's ``agent/a3c.py``: same constructor kwargs, methods and return values (the
 learner branch of ``train_a3c.py`` runs on it unchanged), with the TF1 graph replaced by ``drl_a3c_*``.
 
   Agent.__init__               agent/a3c.py:11-83

@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``agent/apex.py``: same constructor kwargs, same methods, same return
+"""H100-native stand-in for the reference's ``agent/apex.py``: same constructor kwargs, same methods, same return
 values -- so the learner branch of ``train_apex.py:82-155`` runs on it unchanged -- with the TF1 graph +
 ``tf.Session`` replaced by the CUDA Ape-X learner behind the C-ABI (``drl_apex_*``).
 

@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``agent/impala.py``: same constructor kwargs, same
+"""H100-native stand-in for the reference's ``agent/impala.py``: same constructor kwargs, same
 methods, same return values -- so the learner branch of ``train_impala.py:89-113`` runs on it
 unchanged -- with the TF1 graph + ``tf.Session`` replaced by the CUDA learner behind the C-ABI.
 

@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``agent/r2d2.py``: same constructor kwargs, methods and return values, so
+"""H100-native stand-in for the reference's ``agent/r2d2.py``: same constructor kwargs, methods and return values, so
 the learner branch of ``train_r2d2.py:87-165`` runs on it unchanged, with the TF1 graph replaced by ``drl_r2d2_*``.
 
   Agent.__init__       agent/r2d2.py:13-95

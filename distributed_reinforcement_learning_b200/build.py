@@ -1,7 +1,7 @@
-"""In-tree build of the C-ABI library ``csrc/libdrl_b200.so`` with nvcc for sm_100a.
+"""In-tree build of the C-ABI library ``csrc/libdrl_b200.so`` with nvcc for sm_90a (H100).
 
 ``python -m distributed_reinforcement_learning_b200.build`` (or ``__graft_entry__.build()``)
-cross-compiles without a GPU.  The .so is git-ignored but travels with gpurun snapshots.
+cross-compiles without a GPU.  The .so and the objects under csrc/build are build products (git-ignored).
 """
 import concurrent.futures
 import hashlib
@@ -16,7 +16,7 @@ OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(CSRC, "libdrl_b200.so")
 SOURCES = ["learner.cu", "layers.cu", "apex.cu", "r2d2.cu", "elementwise.cu", "vtrace.cu", "optimizer.cu", "ring.cu", "per.cu", "debug.cu",
            "peer.cu"]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -43,7 +43,7 @@ def _stamp():
 
 
 def build(force=False, verbose=False):
-    """Compile all CUDA sources for sm_100a and link the shared library.  Returns its path."""
+    """Compile all CUDA sources for sm_90a and link the shared library.  Returns its path."""
     os.makedirs(OBJ, exist_ok=True)
     stamp_file = os.path.join(OBJ, "stamp")
     stamp = _stamp()
@@ -70,7 +70,7 @@ def build(force=False, verbose=False):
     if verbose:
         for _, log in results:
             sys.stderr.write(log)
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lpthread"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lpthread"]
     p = subprocess.run(cmd, capture_output=True, text=True)
     if p.returncode != 0:
         raise RuntimeError("link failed:\n" + p.stdout + p.stderr)

@@ -854,7 +854,7 @@ int drl_apex_create(const drl_apex_config* cfg, drl_apex** out) {
   }
   if (cfg->num_action < 2 || cfg->num_action > 32) { set_error("num_action must be in [2,32]"); return DRL_ERR_INVALID; }
   if (cfg->batch < 1) { set_error("batch must be >= 1"); return DRL_ERR_INVALID; }
-  if (cfg->math_mode < 0 || cfg->math_mode > 2) { set_error("math_mode must be 0 (default), 1 (FP32 FFMA) or 2 (tcgen05 3xTF32)"); return DRL_ERR_INVALID; }
+  if (cfg->math_mode < 0 || cfg->math_mode > 2) { set_error("math_mode must be 0 (default), 1 (FP32 FFMA) or 2 (wgmma 3xTF32)"); return DRL_ERR_INVALID; }
   if (drl_device_count() <= cfg->device) { set_error("CUDA device %d not available (no CPU fallback)", cfg->device); return DRL_ERR_CUDA; }
   drl_apex* h = new drl_apex();
   h->cfg = *cfg;
@@ -935,7 +935,7 @@ int drl_apex_create(const drl_apex_config* cfg, drl_apex** out) {
     for (size_t i = 0; i < B; ++i) h->h_ones[i] = 1.0f;
     AdamState& o = h->opt;
     o.params = h->params; o.m = h->adam_m; o.v = h->adam_v; o.grads = h->grads; o.n = (int64_t)NP;
-    o.nblk = 148 * 4;
+    o.nblk = 132 * 4;
     DRL_TRY(dev_alloc(h, &o.norm_partials, o.nblk));
     o.step = h->d_step; o.lr_cur = h->d_lr; o.alpha = h->d_alpha; o.b1p = h->d_b1p; o.b2p = h->d_b2p;
     o.out = h->d_out; o.loss = h->loss;

@@ -1,8 +1,8 @@
 // conv1_tma.cuh -- conv1 of the attention_CNN (model/impala_actor_critic.py:6: 8x8 stride 4 over 84x84x4 uint8 frames ->
-// 20x20x32, ReLU) as a FRAME-RESIDENT, TMA-fed, warp-specialised tcgen05 kernel (math mode 5).
+// 20x20x32, ReLU) as a FRAME-RESIDENT, TMA-fed, warp-specialised wgmma kernel (math mode 5).
 //
 // The generic gather-GEMM spends conv1's time in per-CTA fixed costs: 2000 CTAs of one 128-row tile each (K = 256 only),
-// every one paying barrier/TMEM set-up, a cold first gather and a serial epilogue, and every frame byte is gathered 4x
+// every one paying barrier set-up, a cold first gather and a serial epilogue, and every frame byte is gathered 4x
 // through the LSU (8x8 windows at stride 4 overlap).  Here one persistent CTA per SM walks over whole frames:
 //
 //   TMA warp      one tensor load per frame: the raw 84x84x4 bytes (28,224 B) -> shared memory, double-buffered
@@ -12,13 +12,12 @@
 //   warps         turns them into 32 fp16 (exact: PRMT + HSUB2) and writes 4 swizzled 16-byte chunks of a K-major
 //                 SWIZZLE_128B operand stage [128 pixels x 64 features]; 16 stages per frame (4 M tiles x 4 K chunks)
 //                 through a ring of 6; four groups of two warps, group g owns chunk g (4 tasks per thread and stage)
-//   MMA warp      4 tcgen05.mma (kind::f16, M128 N64 K16) per stage: the B tile is [W_hi ; W_lo] stacked along N (the two
-//                 planes of the weight image are adjacent, i.e. ONE 64-row K-major tile), so A x W_hi lands in columns
-//                 0-31 and A x W_lo in columns 32-63 of one of two TMEM accumulators and the epilogue adds the halves --
-//                 half the instructions of issuing the two products separately (an N = 32 MMA costs 44 cycles, an N = 64
-//                 one 48: tools/microbench/mma_rate.cu); tcgen05.commit frees the stage / publishes the accumulator
-//   4 epilogue    TMEM -> registers -> /255 (true fp32 divide, agent/impala.py:133) + bias + ReLU -> coalesced stores of
-//   warps         the a1 rows, overlapped with the next tile's conversion and MMAs
+//   consumer      one warpgroup (warps 8-11): per stage 2 x 4 wgmma (f16, M64 N64 K16) for the two 64-pixel halves of the
+//   warpgroup     tile; the B tile is [W_hi ; W_lo] stacked along N (the two planes of the weight image are adjacent, i.e.
+//                 ONE 64-row K-major tile), so A x W_hi lands in columns 0-31 and A x W_lo in columns 32-63 of the
+//                 register accumulator and the epilogue adds the halves -- half the instructions of issuing the two
+//                 products separately.  After the 4 stages of a tile: /255 (true fp32 divide, agent/impala.py:133) + bias
+//                 + ReLU -> coalesced stores of the a1 rows, while the converters already fill the ring for the next tile
 //
 // Algorithmic traffic per frame: 28,224 B read once (TMA) + 51,200 B of a1 written; shared memory sees the 4x im2col
 // amplification instead of L2 (102 KB read, 205 KB written, 205 KB read by the tensor core per frame).
@@ -55,21 +54,20 @@ struct Conv1Tma {
   static constexpr int RAW_STRIDE = 28672;            // frame buffer pitch (128-byte multiple)
   static constexpr int W_BYTES = 4 * 2 * 32 * 128;    // 4 K tiles x [hi | lo] x 32 rows x 128 B = 32 KB
   static constexpr int CONV_WARPS = 8, EPI_WARPS = 4;
-  static constexpr int W_TMA = CONV_WARPS + EPI_WARPS, W_MMA = W_TMA + 1;   // warps 0-7 convert, 8-11 epilogue, 12 TMA, 13 MMA
-  static constexpr int NT = (W_MMA + 1) * 32;         // 448 threads
+  static constexpr int W_TMA = CONV_WARPS + EPI_WARPS;   // warps 0-7 convert, 8-11 MMA + epilogue (one warpgroup), 12 TMA
+  static constexpr int NT = (W_TMA + 1) * 32;         // 416 threads
   static constexpr int OFF_RAW = NS * STAGE_BYTES;
   static constexpr int OFF_W = OFF_RAW + 2 * RAW_STRIDE;
   static constexpr int OFF_EPI = OFF_W + W_BYTES;
-  static constexpr int OFF_AUX = OFF_EPI + EPI_WARPS * kEpiStageBytes;
+  static constexpr int OFF_AUX = OFF_EPI + EPI_WARPS * wg::kEpiWarpBytes;
   static constexpr int OFF_DBG = OFF_AUX + 512;        // 4 roles x 96 clock samples (debug timeline, tools/conv1_timeline.py)
   static constexpr int SMEM_BYTES = OFF_DBG + 4 * 96 * 8 + 1024;
-  static constexpr int TMEM_COLS = 128;               // two accumulators of 64 columns ([A x W_hi | A x W_lo])
 };
 
 template <class EP>
 __global__ void __launch_bounds__(Conv1Tma::NT, 1)
 conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __restrict__ wimage,
-                     const float* __restrict__ wf32, const EP ep, RowMap map, int nframes, int flags) {
+                     const float* __restrict__ wf32, const EP ep, RowMap map, int nframes) {
   pdl_prologue();
   using C = Conv1Tma;
   using TA = Umma16Tile<128, true>;
@@ -82,10 +80,7 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
   uint64_t* a_empty = a_full + C::NS;                                  // [NS]
   uint64_t* raw_full = a_empty + C::NS;                                // [2]
   uint64_t* raw_empty = raw_full + 2;                                  // [2]
-  uint64_t* acc_full = raw_empty + 2;                                  // [2]
-  uint64_t* acc_empty = acc_full + 2;                                  // [2]
-  uint64_t* w_full = acc_empty + 2;                                    // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(w_full + 1);
+  uint64_t* w_full = raw_empty + 2;                                    // [1]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // debug timeline: when the trace buffer is armed with magic 0xC0171 in word 8001, lane 0 of each role keeps clock64()
@@ -104,8 +99,6 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
     for (int b = 0; b < 2; ++b) {
       umma::mbar_init(&raw_full[b], 1);
       umma::mbar_init(&raw_empty[b], C::CONV_WARPS * 32);
-      umma::mbar_init(&acc_full[b], 1);
-      umma::mbar_init(&acc_empty[b], C::EPI_WARPS * 32);
     }
     // weights: either ONE bulk copy of the pre-tiled image (expect_tx), or -- wf32 != nullptr -- the epilogue warps
     // build the image from the fp32 HWIO weights themselves while the first frame slab is in flight: the step's first
@@ -113,11 +106,7 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
     umma::mbar_init(w_full, wf32 ? C::EPI_WARPS * 32 : 1);
     umma::fence_barrier_init();
   }
-  if (warp == C::W_MMA) umma::tmem_alloc<C::TMEM_COLS>(tmem_ptr);
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < C::CONV_WARPS) {
     // ================= CONVERTERS: raw frame bytes -> fp16 K-major operand stages =================
@@ -176,9 +165,9 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
       umma::mbar_arrive(&raw_empty[slot]);        // this thread no longer reads the frame buffer
     }
   } else if (warp < C::W_TMA) {
-    // ================= EPILOGUE (warps 8..11: TMEM lane quarter = warp & 3) =================
-    const int quarter = warp & 3;
-    uint8_t* stg = smem + C::OFF_EPI + quarter * kEpiStageBytes;
+    // ================= MMA + EPILOGUE (warps 8..11: one warpgroup) =================
+    const int cwarp = warp & 3;
+    uint8_t* stg = smem + C::OFF_EPI + cwarp * wg::kEpiWarpBytes;
     if (wf32) {
       // [K = 256][N = 32] fp32 -> per K tile of 64: rows 0..31 = fp16(w), rows 32..63 = fp16(w - hi) (K-major, swizzled):
       // 1024 units of 8 consecutive k of one n; lanes = consecutive n (coalesced 128-byte rows of the HWIO matrix)
@@ -198,53 +187,46 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
       umma::fence_proxy_async();
       umma::mbar_arrive(w_full);
     }
-    uint32_t tile = 0;
+    umma::mbar_wait(w_full, 0);
+    const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO), db_base = umma::make_desc(0, TB::LBO, TB::SBO);
+    float acc0[32], acc1[32];   // pixels 0-63 / 64-127 of the tile x [A W_hi | A W_lo]
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    uint32_t it = 0;
     for (int mf = blockIdx.x; mf < nframes; mf += gridDim.x) {
       const int row_base = mf * C::PIX, row_end = row_base + C::PIX;
-      for (int mt = 0; mt < C::MT; ++mt, ++tile) {
-        const int buf = tile & 1;
-        umma::mbar_wait(&acc_full[buf], (tile >> 1) & 1);
-        umma::tc_fence_after();
-        if (warp == C::CONV_WARPS && lane == 0) C1_TR(2);
-        float v[32], w[32];
-        umma::tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 64), v);
-        umma::tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 64 + 32), w);
+      for (int mt = 0; mt < C::MT; ++mt) {
+        for (int c = 0; c < C::KC; ++c, ++it) {
+          const int s = it % C::NS;
+          umma::mbar_wait(&a_full[s], (it / C::NS) & 1);
+          if (cwarp == 0 && lane == 0) C1_TR(1);
+          const uint32_t sa = umma::smem_u32(smem + s * C::STAGE_BYTES);
+          const uint64_t a0 = umma::desc_at(da_base, sa), a1 = umma::desc_at(da_base, sa + 64 * 128);
+          const uint64_t b = umma::desc_at(db_base, umma::smem_u32(wsm + c * (2 * TB::BYTES)));   // [W_hi ; W_lo]: 64 rows
+          wg::fence_operand(acc0);
+          wg::fence_operand(acc1);
+          wg::fence();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] += w[i];     // hi product + lo product
-        umma::tc_fence_before();
-        umma::mbar_arrive(&acc_empty[buf]);
-        if (flags & 1) {
-          // experiment: no output at all
-        } else if (flags & 48) {   // experiments: 16 = multiply by 1/255 instead of dividing; 32 = compute but do not store
-          const int m = row_base + mt * 128 + quarter * 32 + lane;
-          if (m < row_end) {
-            float acc = 0.f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float o[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float x = v[4 * j + q];
-                const float y = (flags & 16) ? x * (1.0f / 255.0f) : x / 255.0f;
-                o[q] = fmaxf(y + __ldg(ep.bias + 4 * j + q), 0.f);
-                acc += o[q];
-              }
-              if (!(flags & 32)) *reinterpret_cast<float4*>(ep.c + (size_t)m * 32 + 4 * j) = make_float4(o[0], o[1], o[2], o[3]);
-            }
-            if ((flags & 32) && acc == 123456.789f) ep.c[0] = acc;     // keep the arithmetic alive
+          for (int j = 0; j < 4; ++j) {
+            const uint64_t ko = (uint64_t)(j * 32 >> 4);
+            umma16::mma16<64, umma16::F16, 0, 0>(acc0, a0 + ko, b + ko, (c > 0 || j > 0) ? 1u : 0u);
+            umma16::mma16<64, umma16::F16, 0, 0>(acc1, a1 + ko, b + ko, (c > 0 || j > 0) ? 1u : 0u);
           }
-        } else if (flags & 4) {   // experiment: every lane stores its own row, no staging through shared memory
-          const int m = row_base + mt * 128 + quarter * 32 + lane;
-          if (m < row_end) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float o[4] = {v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]};
-              ep.template store<4>(0, m, 4 * j, o);
-            }
-          }
-        } else
-        epilogue_store_32x32(ep, stg, lane, 0, row_base + mt * 128 + quarter * 32, 0, row_end, 32, v);
-        if (warp == C::CONV_WARPS && lane == 0) C1_TR(2);
+          wg::commit();
+          wg::wait<1>();                               // the MMAs of the previous stage are complete: hand it back
+          wg::fence_operand(acc0);
+          wg::fence_operand(acc1);
+          if (c > 0 && tid == C::CONV_WARPS * 32) umma::mbar_arrive(&a_empty[(it - 1) % C::NS]);
+        }
+        wg::wait<0>();
+        wg::fence_operand(acc0);
+        wg::fence_operand(acc1);
+        if (tid == C::CONV_WARPS * 32) umma::mbar_arrive(&a_empty[(it - 1) % C::NS]);
+        if (cwarp == 0 && lane == 0) C1_TR(2);
+        const int r0 = row_base + mt * 128 + cwarp * 16;
+        wg_epilogue<64, true>(ep, acc0, stg, lane, 0, r0, 0, row_end, 32);
+        wg_epilogue<64, true>(ep, acc1, stg, lane, 0, r0 + 64, 0, row_end, 32);
+        if (cwarp == 0 && lane == 0) C1_TR(2);
       }
     }
   } else if (warp == C::W_TMA) {
@@ -264,50 +246,12 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
         umma::tma_load_4d(raw + slot * C::RAW_STRIDE, &fmap, 0, 0, 0, map.src(mf), &raw_full[slot]);
       }
     }
-  } else {
-    // ================= MMA ISSUER =================
-    constexpr uint32_t idesc = umma16::make_idesc16(64, umma16::F16::kFormat, umma16::F16::kFormat, false, false);
-    umma::mbar_wait(w_full, 0);
-    uint32_t it = 0, tile = 0;
-    for (int mf = blockIdx.x; mf < nframes; mf += gridDim.x) {
-      for (int mt = 0; mt < C::MT; ++mt, ++tile) {
-        const int buf = tile & 1;
-        umma::mbar_wait(&acc_empty[buf], ((tile >> 1) & 1) ^ 1);
-        umma::tc_fence_after();
-        const uint32_t d = tmem_base + (uint32_t)(buf * 64);
-        for (int c = 0; c < C::KC; ++c, ++it) {
-          const int s = it % C::NS;
-          umma::mbar_wait(&a_full[s], (it / C::NS) & 1);
-          umma::tc_fence_after();
-          if (lane == 0) C1_TR(1);
-          if (umma::elect_one()) {
-            const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-            const uint64_t db_base = umma::make_desc(0, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-            const uint64_t a = umma::desc_at(da_base, umma::smem_u32(smem + s * C::STAGE_BYTES));
-            const uint64_t b = umma::desc_at(db_base, umma::smem_u32(wsm + c * (2 * TB::BYTES)));   // [W_hi ; W_lo]: 64 rows
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint64_t ko = (uint64_t)(j * 32 >> 4);
-              umma16::mma_f16(d, a + ko, b + ko, idesc, (c > 0 || j > 0) ? 1u : 0u);
-            }
-            umma::mma_commit(&a_empty[s]);
-            if (c == C::KC - 1) umma::mma_commit(&acc_full[buf]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-    umma::tc_fence_before();
   }
   __syncthreads();
   if (tracing) {
     for (int i = tid; i < 4 * 96; i += blockDim.x) trbuf[8002 + i] = (unsigned long long)dbg[i];
   }
 #undef C1_TR
-  if (warp == C::W_MMA) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<C::TMEM_COLS>(tmem_base);
-  }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------
@@ -345,8 +289,7 @@ inline int launch_conv1_fwd_tma(cudaStream_t s, const uint8_t* frames, int nfram
     attr_done = true;
   }
   const int grid = std::min(nframes, device_sm_count());
-  static const int flags = getenv("DRL_C1_FLAGS") ? atoi(getenv("DRL_C1_FLAGS")) : 0;   // experiments (see the kernel)
-  DRL_CUDA_CHECK((launch_k(kern, grid, Conv1Tma::NT, Conv1Tma::SMEM_BYTES, s, it->second, wimage, wf32, ep, map, nframes, flags)));
+  DRL_CUDA_CHECK((launch_k(kern, grid, Conv1Tma::NT, Conv1Tma::SMEM_BYTES, s, it->second, wimage, wf32, ep, map, nframes)));
   return DRL_OK;
 }
 
@@ -361,10 +304,10 @@ inline int launch_conv1_fwd_tma(cudaStream_t s, const uint8_t* frames, int nfram
 //                    MN-major SWIZZLE_128B operand (M = feature contiguous, K = pixel) of the transposed product;
 //                 B: dA1 [64 px][32] fp32 -> bf16 hi / lo, TRANSPOSED into one K-major tile of 64 rows [hi n | lo n] x 64 px
 //                    (each thread: 8 consecutive pixels of one n = one 16-byte chunk per plane); column sums for db
-//   MMA warp      per tile 2 feature tiles x 4 K slices of tcgen05.mma (M128 N64 K16, A MN-major, B K-major); the two
-//                 accumulators [X^T dA1_hi | X^T dA1_lo] stay in TMEM over ALL tiles of all frames of the CTA
-//   4 epilogue    once: hi + lo halves, x 1/255, partial slab [257 x 32] of this CTA; a fixed-order reduce over the CTAs
-//   warps         follows (splitk_reduce)
+//   2 consumer    warpgroup h (warps 8-11 / 12-15) owns features 128 h .. 128 h + 127: per tile 2 x 4 wgmma (bf16, M64
+//   warpgroups    N64 K16, A MN-major, B K-major); the accumulators [X^T dA1_hi | X^T dA1_lo] stay in registers over ALL
+//                 tiles of all frames of the CTA.  Once at the end: hi + lo halves, x 1/255, partial slab [257 x 32] of
+//                 this CTA; a fixed-order reduce over the CTAs follows (splitk_reduce)
 // =====================================================================================================================
 struct Conv1WgTma {
   static constexpr int FRAME = Geo::FRAME, PIX = 400;
@@ -374,15 +317,14 @@ struct Conv1WgTma {
   static constexpr int B_SLOT = 64 * 128;              // 64 rows (32 hi + 32 lo) x 64 px bf16 = 8 KB
   static constexpr int D_SLOT = TPX * 32 * 4;          // raw dA1 rows of a tile, fp32: 8 KB
   static constexpr int RAW_STRIDE = 28672;
-  static constexpr int CONV_WARPS = 8, EPI_WARPS = 4;
-  static constexpr int W_TMA = CONV_WARPS + EPI_WARPS, W_MMA = W_TMA + 1;
-  static constexpr int NT = (W_MMA + 1) * 32;
+  static constexpr int CONV_WARPS = 8, MMA_WARPS = 8;
+  static constexpr int W_TMA = CONV_WARPS + MMA_WARPS;   // warps 0-7 convert, 8-15 two consumer warpgroups, 16 TMA
+  static constexpr int NT = (W_TMA + 1) * 32;
   static constexpr int OFF_B = 2 * A_SLOT;
   static constexpr int OFF_RAW = OFF_B + 2 * B_SLOT;
   static constexpr int OFF_D = OFF_RAW + 2 * RAW_STRIDE;
   static constexpr int OFF_AUX = OFF_D + 2 * D_SLOT;
   static constexpr int SMEM_BYTES = OFF_AUX + 512 + 1024;
-  static constexpr int TMEM_COLS = 128;                // 2 feature tiles x [hi | lo] x 32
   static constexpr int SLAB = 257 * 32;                // floats per CTA partial: dW [256 x 32] + db [32]
 };
 
@@ -412,8 +354,6 @@ conv1_wgrad_tma_kernel(const __grid_constant__ CUtensorMap fmap, const float* __
   uint64_t* raw_empty = raw_full + 2;                                  // [2]
   uint64_t* d_full = raw_empty + 2;                                    // [2] raw dA1 rows of a tile
   uint64_t* d_empty = d_full + 2;                                      // [2]
-  uint64_t* acc_done = d_empty + 2;                                    // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_done + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // operand slots start as zeros: rows of a partial tile keep stale (finite) values that meet zero B columns
@@ -421,21 +361,16 @@ conv1_wgrad_tma_kernel(const __grid_constant__ CUtensorMap fmap, const float* __
   if (tid == 0) {
     for (int b = 0; b < 2; ++b) {
       umma::mbar_init(&t_full[b], C::CONV_WARPS * 32);
-      umma::mbar_init(&t_empty[b], 1);
+      umma::mbar_init(&t_empty[b], wg::kConsumerWGs);
       umma::mbar_init(&raw_full[b], 1);
       umma::mbar_init(&raw_empty[b], C::CONV_WARPS * 32);
       umma::mbar_init(&d_full[b], 1);
       umma::mbar_init(&d_empty[b], C::CONV_WARPS * 32);
     }
-    umma::mbar_init(acc_done, 1);
     umma::fence_barrier_init();
   }
-  if (warp == C::W_MMA) umma::tmem_alloc<C::TMEM_COLS>(tmem_ptr);
   umma::fence_proxy_async();
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   float* slab = partial + (size_t)blockIdx.x * C::SLAB;
 
   if (warp < C::CONV_WARPS) {
@@ -507,23 +442,57 @@ conv1_wgrad_tma_kernel(const __grid_constant__ CUtensorMap fmap, const float* __
     colsum += __shfl_xor_sync(0xffffffffu, colsum, 4);
     if (bj == 0) slab[256 * 32 + bn] = colsum;
   } else if (warp < C::W_TMA) {
-    // ================= EPILOGUE (once) =================
-    const int quarter = warp & 3;
-    umma::mbar_wait(acc_done, 0);
-    umma::tc_fence_after();
-#pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-      float v[32], w[32];
-      umma::tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(h * 64), v);
-      umma::tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(h * 64 + 32), w);
-      float* dst = slab + (size_t)(h * 128 + quarter * 32 + lane) * 32;
+    // ================= MMA (warpgroup h: features 128 h ..), epilogue once =================
+    // A: MN-major (M = feature, K = pixel): atom = 8 px x 64 features = 1024 B; next 64 features = next chunk (LBO = 8 KB);
+    //    next 8 pixels SBO = 1024; a K = 16 slice = 2 atoms = 2048 B.   B: K-major, 64 rows of 128 B.
+    const int ct = tid - C::CONV_WARPS * 32, h = ct >> 7, cwarp = (ct >> 5) & 3;
+    const uint64_t da_base = umma::make_desc(0, C::TPX * 128, 1024), db_base = umma::make_desc(0, 16, 1024);
+    float acc0[32], acc1[32];   // features 128 h + [0, 64) / [64, 128) x [dA1_hi | dA1_lo]
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(dst + 4 * j) =
-            make_float4((v[4 * j] + w[4 * j]) * (1.0f / 255.0f), (v[4 * j + 1] + w[4 * j + 1]) * (1.0f / 255.0f),
-                        (v[4 * j + 2] + w[4 * j + 2]) * (1.0f / 255.0f), (v[4 * j + 3] + w[4 * j + 3]) * (1.0f / 255.0f));
+    for (int i = 0; i < 32; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    uint32_t it = 0;
+    for (int mf = blockIdx.x; mf < nframes; mf += gridDim.x) {
+      for (int pt = 0; pt < C::NTILE; ++pt, ++it) {
+        const int ts = it & 1;
+        umma::mbar_wait(&t_full[ts], (it >> 1) & 1);
+        const uint64_t b = umma::desc_at(db_base, umma::smem_u32(bsm + ts * C::B_SLOT));
+        const uint32_t sa = umma::smem_u32(smem + ts * C::A_SLOT + h * 2 * (C::TPX * 128));
+        const uint64_t a0 = umma::desc_at(da_base, sa), a1 = umma::desc_at(da_base, sa + C::TPX * 128);
+        wg::fence_operand(acc0);
+        wg::fence_operand(acc1);
+        wg::fence();
+#pragma unroll
+        for (int j = 0; j < C::TPX / 16; ++j) {
+          const uint64_t ao = (uint64_t)(j * 2048 >> 4), bo = (uint64_t)(j * 32 >> 4);
+          umma16::mma16<64, umma16::BF16, 1, 0>(acc0, a0 + ao, b + bo, (it > 0 || j > 0) ? 1u : 0u);
+          umma16::mma16<64, umma16::BF16, 1, 0>(acc1, a1 + ao, b + bo, (it > 0 || j > 0) ? 1u : 0u);
+        }
+        wg::commit();
+        wg::wait<1>();                                 // the previous tile's MMAs are complete: hand its slot back
+        wg::fence_operand(acc0);
+        wg::fence_operand(acc1);
+        if (it > 0 && (ct & 127) == 0) umma::mbar_arrive(&t_empty[(it - 1) & 1]);
+      }
     }
-    umma::tc_fence_before();
+    wg::wait<0>();
+    wg::fence_operand(acc0);
+    wg::fence_operand(acc1);
+    // fragment: acc[4c + e] = feature row lane/4 (+8 for e >= 2), column 8c + 2 (lane % 4) + (e & 1); c < 4: x dA1_hi,
+    // c >= 4: the same column x dA1_lo
+    const int r = lane >> 2, q = lane & 3;
+#pragma unroll
+    for (int sub = 0; sub < 2; ++sub) {
+      const float* acc = sub ? acc1 : acc0;
+      const int f0 = h * 128 + sub * 64 + cwarp * 16 + r;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const int n = 8 * c + 2 * q, i = 4 * c;
+        *reinterpret_cast<float2*>(slab + (size_t)f0 * 32 + n) =
+            make_float2((acc[i] + acc[i + 16]) * (1.0f / 255.0f), (acc[i + 1] + acc[i + 17]) * (1.0f / 255.0f));
+        *reinterpret_cast<float2*>(slab + (size_t)(f0 + 8) * 32 + n) =
+            make_float2((acc[i + 2] + acc[i + 18]) * (1.0f / 255.0f), (acc[i + 3] + acc[i + 19]) * (1.0f / 255.0f));
+      }
+    }
   } else if (warp == C::W_TMA) {
     // ================= TMA PRODUCER =================
     if (lane == 0) {
@@ -544,44 +513,6 @@ conv1_wgrad_tma_kernel(const __grid_constant__ CUtensorMap fmap, const float* __
         }
       }
     }
-  } else {
-    // ================= MMA ISSUER =================
-    // A: MN-major (M = feature, K = pixel): atom = 8 px x 64 features = 1024 B; next 64 features = next chunk (LBO = 8 KB);
-    //    next 8 pixels SBO = 1024; a K = 16 slice = 2 atoms = 2048 B.   B: K-major, 64 rows of 128 B.
-    constexpr uint32_t idesc = umma16::make_idesc16(64, umma16::BF16::kFormat, umma16::BF16::kFormat, true, false);
-    uint32_t it = 0;
-    bool any = false;
-    for (int mf = blockIdx.x; mf < nframes; mf += gridDim.x) {
-      for (int pt = 0; pt < C::NTILE; ++pt, ++it) {
-        const int ts = it & 1;
-        umma::mbar_wait(&t_full[ts], (it >> 1) & 1);
-        umma::tc_fence_after();
-        if (umma::elect_one()) {
-          const uint64_t da_base = umma::make_desc(0, C::TPX * 128, 1024, 2);
-          const uint64_t db_base = umma::make_desc(0, 16, 1024, 2);
-          const uint64_t b = umma::desc_at(db_base, umma::smem_u32(bsm + ts * C::B_SLOT));
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint64_t a = umma::desc_at(da_base, umma::smem_u32(smem + ts * C::A_SLOT + h * 2 * (C::TPX * 128)));
-#pragma unroll
-            for (int j = 0; j < C::TPX / 16; ++j)
-              umma16::mma_f16(tmem_base + (uint32_t)(h * 64), a + (uint64_t)(j * 2048 >> 4), b + (uint64_t)(j * 32 >> 4), idesc,
-                              (it > 0 || j > 0) ? 1u : 0u);
-          }
-          umma::mma_commit(&t_empty[ts]);
-        }
-        __syncwarp();
-        any = true;
-      }
-    }
-    if (any && umma::elect_one()) umma::mma_commit(acc_done);
-    __syncwarp();
-    umma::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == C::W_MMA) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<C::TMEM_COLS>(tmem_base);
   }
 }
 

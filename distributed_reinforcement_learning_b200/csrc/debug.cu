@@ -1,6 +1,6 @@
 // debug.cu -- drl_debug_gemm: runs ONE plain GEMM  C[M,N] = A * B  on either contraction core
-// (FP32-FFMA gather-GEMM or tcgen05 3xTF32 UMMA) with every operand-major combination the layers use,
-// so the shared-memory layouts / UMMA descriptors can be validated in isolation against NumPy.
+// (FP32-FFMA gather-GEMM or wgmma 3xTF32) with every operand-major combination the layers use,
+// so the shared-memory layouts / wgmma descriptors can be validated in isolation against NumPy.
 #include <vector>
 
 #include "gemm_simt.cuh"
@@ -19,10 +19,10 @@ static int run_fmt16(bool pretiled, int bn, cudaStream_t s, const AL& al, const 
   if (!pretiled) {
     if (!BL::kContigK && bn < 64) { set_error("debug_gemm: MN-major 16-bit B tiles need bn >= 64"); return DRL_ERR_INVALID; }
     switch (bn) {
-      case 32: if constexpr (BL::kContigK) return launch_gemm_umma16<Umma16Cfg<32, 2, 2, 4, 0, F, F>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk); else break;
-      case 64: return launch_gemm_umma16<Umma16Cfg<64, 2, 2, 4, 0, F, F>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
+      case 32: if constexpr (BL::kContigK) return launch_gemm_umma16<Umma16Cfg<32, 2, 1, 4, 0, F, F>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk); else break;
+      case 64: return launch_gemm_umma16<Umma16Cfg<64, 2, 1, 4, 0, F, F>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
       case 128: return launch_gemm_umma16<Umma16Cfg<128, 3, 1, 8, 0, F, F>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
-      case 256: return launch_gemm_umma16<Umma16Cfg<256, 2, 1, 8, 0, F, F>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
+      case 256: return launch_gemm_umma16<Umma16Cfg<256, 2, 1, 4, 0, F, F>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
     }
     set_error("debug_gemm: bn must be 32 (K-major B), 64, 128 or 256");
     return DRL_ERR_INVALID;
@@ -34,7 +34,7 @@ static int run_fmt16(bool pretiled, int bn, cudaStream_t s, const AL& al, const 
     DRL_CUDA_CHECK(cudaMalloc(&img, weight_image16_bytes<BN>(N, K) + 1024));
     DRL_TRY((launch_retile_b16<BN, F>(s, bl, N, K, img)));
     PretiledB<BL> blp{img, cdiv(K, 64)};
-    using Cfg = Umma16Cfg<BN, (BN == 256 ? 2 : 3), (BN <= 64 ? 2 : 1), (BN <= 64 ? 4 : 8), 1, F, F>;
+    using Cfg = Umma16Cfg<BN, (BN == 256 ? 2 : 3), 1, (BN == 128 ? 8 : 4), (BN == 256 ? 0 : 1), F, F>;
     return launch_gemm_umma16<Cfg>(s, al, blp, ep, M, N, K, nz, kchunk, kchunk);
   };
   switch (bn) {
@@ -69,10 +69,10 @@ static int run_one(int core, int bn, cudaStream_t s, const AL& al, const BL& bl,
   if (core == 1) return launch_gemm_simt<CfgMid>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
   if (core >= 5) return run_one16(core, bn, s, al, bl, ep, M, N, K, nz, kchunk);
   switch (bn) {
-    case 32: return launch_gemm_umma<UmmaCfg<32, 2, 2>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
-    case 64: return launch_gemm_umma<UmmaCfg<64, 2, 2>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
+    case 32: return launch_gemm_umma<UmmaCfg<32, 2, 1>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
+    case 64: return launch_gemm_umma<UmmaCfg<64, 2, 1>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
     case 128: return launch_gemm_umma<UmmaCfg<128, 3, 1, 8>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
-    case 256: return launch_gemm_umma<UmmaCfg<256, 2, 1, 8>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
+    case 256: return launch_gemm_umma<UmmaCfg<256, 2, 1, 4>>(s, al, bl, ep, M, N, K, nz, kchunk, kchunk);
     default: set_error("debug_gemm: bn must be 32, 64, 128 or 256"); return DRL_ERR_INVALID;
   }
 }
@@ -81,7 +81,7 @@ static int run_one(int core, int bn, cudaStream_t s, const AL& al, const BL& bl,
 
 using namespace drl;
 
-// core: 1 = FFMA, 2 = tcgen05.  a_kmajor: A given as [M,K] row-major (1) or as [K,M] row-major (0).
+// core: 1 = FFMA, 2 = wgmma 3xTF32, 5-8 = wgmma 16-bit split (see run_one16).  a_kmajor: A given as [M,K] row-major (1) or as [K,M] row-major (0).
 // b_kmajor: B given as [N,K] row-major (1) or [K,N] row-major (0).  C out: [splits][(M+1), N] host floats
 // (row M of each slab = column sums of B over that split's K range when B is N-major, else untouched).
 extern "C" int drl_debug_gemm(int32_t core, int32_t bn, int32_t a_kmajor, int32_t b_kmajor, int32_t M, int32_t N,

@@ -370,7 +370,7 @@ int col2im_conv2(cudaStream_t s, const float* dcol, const float* a1, float* da1,
 // ------------------------------------------------------------------------------------------
 // 256 threads = 32 consecutive outputs (one 128-byte line per slab) x 8 slab groups: group g sums slabs g, g+8, ... with
 // four independent accumulators, the eight group sums are then added in the fixed order 0..7 -- the serial chain per
-// thread is nsplit/8 loads instead of nsplit (conv1's 148 per-CTA slabs: 10 us -> ~3 us on the critical path).
+// thread is nsplit/8 loads instead of nsplit (many per-CTA slabs: fewer dependent loads on the critical path).
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ part, size_t slab, int nsplit,
                                                              float* __restrict__ out, size_t n) {
   pdl_prologue();

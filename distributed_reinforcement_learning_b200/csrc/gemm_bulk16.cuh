@@ -1,4 +1,4 @@
-// gemm_bulk16.cuh -- tcgen05 GEMM whose BOTH operands are pre-tiled 16-bit images: no producer warps at all.
+// gemm_bulk16.cuh -- wgmma GEMM whose BOTH operands are pre-tiled 16-bit images: no producer warps at all.
 //
 // The gather-GEMMs of gemm_umma16.cuh feed the tensor core through producer warps (LDG fp32 -> split into bf16 hi/lo ->
 // STS).  For the three LSTM contractions of model/impala_actor_critic.py:18-25 (forward z = [a3|emb|h0] W, data
@@ -6,34 +6,31 @@
 // the eight producer warps ~3 us, while the 64 KB weight tile next to it arrived by ONE cp.async.bulk in a fraction of
 // that.  Here the activation-side operand is ALSO written once as an image (retile_b16_kernel over the activation
 // loader: x as rows x K, x^T, dz, dz^T -- 2.4-9.3 MB each, written once, read by 4-29 CTAs each), so a K tile of a CTA is
-// two bulk copies that complete on the stage's mbarrier (expect_tx) and twelve tcgen05.mma:
+// two bulk copies that complete on the stage's mbarrier (expect_tx) and twelve wgmma per consumer warpgroup:
 //
 //     image tile (row tile rt, k tile kt) = [hi plane | lo plane], each ROWS x 128 bytes K-major SWIZZLE_128B
 //     (byte for byte what a stage holds; Umma16Tile<ROWS, true>), at image + (rt * ktiles + kt) * 2 * ROWS * 128
 //
 //   warp 0      loader: one lane, per K tile arrive.expect_tx + 2 bulk copies (A tile 32 KB, B tile BN x 256 B)
-//   warp 1      TMEM allocation + MMA issue (A_lo B_hi + A_hi B_lo + A_hi B_hi per K = 16 slice), commit -> empty / acc_full
-//   warps 2..   epilogue (4 or 8 warps): tcgen05.ld of their lane quarter / column half, transposed through the dead
-//               stages (epilogue_store_32x32), epilogue functor
+//               (warps 1-3 idle: the consumers must start on a warpgroup boundary)
+//   warps 4-11  two consumer warpgroups (rows 0-63 / 64-127): MMA issue (A_lo B_hi + A_hi B_lo + A_hi B_hi per K = 16
+//               slice) into the register accumulator, stage hand-back (empty), then the epilogue through the dead
+//               stages (wg_epilogue)
 // Rows beyond M / N and k beyond K are zero in the images, so no masking is needed before the epilogue.
 #pragma once
 #include "gemm_umma16.cuh"
 
 namespace drl {
 
-template <int BN_, int STAGES_, int EW_ = 8>
+template <int BN_, int STAGES_>
 struct Bulk16Cfg {
-  static constexpr int BM = 128, BN = BN_, BK = 64, STAGES = STAGES_, EW = EW_;
-  static constexpr int NT = 64 + 32 * EW;
+  static constexpr int BM = 128, BN = BN_, BK = 64, STAGES = STAGES_;
+  static constexpr int NT = 128 + wg::kConsumerThreads;                  // loader warpgroup + two consumer warpgroups
   static constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128;            // one plane
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 1024;   // stages + barriers / tmem pointer + alignment
-  static constexpr int TMEM_COLS = BN;
-  static constexpr int EPI_COLS = BN / (EW / 4);
-  static_assert(EW == 4 || EW == 8, "4 or 8 epilogue warps");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 1024;   // stages + barriers + alignment
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
-  static_assert(EPI_COLS % 32 == 0, "epilogue reads 32 columns at a time");
-  static_assert(STAGES * STAGE_BYTES >= EW * kEpiStageBytes, "epilogue staging tiles live in the dead stages");
+  static_assert(STAGES * STAGE_BYTES >= 8 * wg::kEpiWarpBytes, "epilogue staging tiles live in the dead stages");
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
@@ -56,8 +53,6 @@ gemm_bulk16_kernel(const ImageOp a, const ImageOp b, const EP ep, int M, int N, 
   uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_full + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int z = blockIdx.z;
@@ -70,16 +65,11 @@ gemm_bulk16_kernel(const ImageOp a, const ImageOp b, const EP ep, int M, int N, 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       umma::mbar_init(&full[s], 1);
-      umma::mbar_init(&empty[s], 1);
+      umma::mbar_init(&empty[s], wg::kConsumerWGs);
     }
-    umma::mbar_init(acc_full, 1);
     umma::fence_barrier_init();
   }
-  if (warp == 1) umma::tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   if (tid == 0) TR(2);
 
   if (warp == 0) {
@@ -98,57 +88,45 @@ gemm_bulk16_kernel(const ImageOp a, const ImageOp b, const EP ep, int M, int N, 
         umma::bulk_g2s(st + 2 * Cfg::A_BYTES, bsrc + (size_t)t * (2 * Cfg::B_BYTES), 2 * Cfg::B_BYTES, &full[s]);
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA ISSUER =================
-    constexpr uint32_t idesc = umma16::make_idesc16(BN, umma16::BF16::kFormat, umma16::BF16::kFormat, false, false);
+  } else if (warp >= 4) {
+    // ================= CONSUMERS (warps 4..11: warpgroup cw = rows 64 cw .. 64 cw + 63) =================
+    const int ct = tid - 128, cw = ct >> 7, cwarp = (ct >> 5) & 3;
+    const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO), db_base = umma::make_desc(0, TB::LBO, TB::SBO);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int t = 0; t < ntiles; ++t) {
       const int s = t % STAGES;
       umma::mbar_wait(&full[s], (t / STAGES) & 1);
-      umma::tc_fence_after();
-      if (umma::elect_one()) {
-        TR(3000 + t);
-        const uint32_t st = umma::smem_u32(smem + s * Cfg::STAGE_BYTES);
-        const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-        const uint64_t db_base = umma::make_desc(0, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-        const uint64_t a_hi = umma::desc_at(da_base, st), a_lo = umma::desc_at(da_base, st + Cfg::A_BYTES);
-        const uint64_t b_hi = umma::desc_at(db_base, st + 2 * Cfg::A_BYTES);
-        const uint64_t b_lo = umma::desc_at(db_base, st + 2 * Cfg::A_BYTES + Cfg::B_BYTES);
+      if (ct == 0) TR(3000 + t);
+      const uint32_t st = umma::smem_u32(smem + s * Cfg::STAGE_BYTES);
+      const uint64_t a_hi = umma::desc_at(da_base, st + cw * 64 * 128);
+      const uint64_t a_lo = umma::desc_at(da_base, st + Cfg::A_BYTES + cw * 64 * 128);
+      const uint64_t b_hi = umma::desc_at(db_base, st + 2 * Cfg::A_BYTES);
+      const uint64_t b_lo = umma::desc_at(db_base, st + 2 * Cfg::A_BYTES + Cfg::B_BYTES);
+      wg::fence_operand(acc);
+      wg::fence();
 #pragma unroll
-        for (int j = 0; j < BK / 16; ++j) {
-          const uint64_t ao = (uint64_t)(TA::kslice_off(j) >> 4), bo = (uint64_t)(TB::kslice_off(j) >> 4);
-          umma16::mma_f16(tmem_base, a_lo + ao, b_hi + bo, idesc, (t > 0 || j > 0) ? 1u : 0u);   // small terms first
-          umma16::mma_f16(tmem_base, a_hi + ao, b_lo + bo, idesc, 1u);
-          umma16::mma_f16(tmem_base, a_hi + ao, b_hi + bo, idesc, 1u);
-        }
-        umma::mma_commit(&empty[s]);
-        if (t == ntiles - 1) umma::mma_commit(acc_full);
-        TR(4000 + t);
+      for (int j = 0; j < BK / 16; ++j) {
+        const uint64_t ao = (uint64_t)(TA::kslice_off(j) >> 4), bo = (uint64_t)(TB::kslice_off(j) >> 4);
+        umma16::mma16<BN, umma16::BF16, 0, 0>(acc, a_lo + ao, b_hi + bo, (t > 0 || j > 0) ? 1u : 0u);   // small terms first
+        umma16::mma16<BN, umma16::BF16, 0, 0>(acc, a_hi + ao, b_lo + bo, 1u);
+        umma16::mma16<BN, umma16::BF16, 0, 0>(acc, a_hi + ao, b_hi + bo, 1u);
       }
-      __syncwarp();
+      wg::commit();
+      wg::wait<1>();
+      wg::fence_operand(acc);
+      if (t > 0 && (ct & 127) == 0) umma::mbar_arrive(&empty[(t - 1) % STAGES]);
+      if (ct == 0) TR(4000 + t);
     }
-    umma::tc_fence_before();
-  } else {
+    wg::wait<0>();
+    wg::fence_operand(acc);
     // ================= EPILOGUE =================
-    const int e = warp - 2, quarter = warp & 3;
-    umma::mbar_wait(acc_full, 0);
-    umma::tc_fence_after();
-    if (e == 0 && lane == 0) TR(6000);
-    uint8_t* stg = smem + e * kEpiStageBytes;       // all stages are dead once the accumulator is complete
-    const int row0 = m0 + quarter * 32;
-    const int cbeg = (e >> 2) * Cfg::EPI_COLS;
-#pragma unroll 1
-    for (int c0 = cbeg; c0 < cbeg + Cfg::EPI_COLS; c0 += 32) {
-      float v[32];
-      umma::tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c0, v);
-      epilogue_store_32x32(ep, stg, lane, z, row0, n0 + c0, M, N, v);
-    }
-    if (e == 0 && lane == 0) TR(6001);
-    umma::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+    wg::consumer_sync();                               // all stages are dead once both accumulators are complete
+    if (ct == 0) TR(6000);
+    uint8_t* stg = smem + (ct >> 5) * wg::kEpiWarpBytes;
+    wg_epilogue<BN>(ep, acc, stg, lane, z, m0 + cw * 64 + cwarp * 16, n0, M, N);
+    if (ct == 0) TR(6001);
   }
 }
 

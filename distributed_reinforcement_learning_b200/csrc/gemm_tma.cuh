@@ -1,4 +1,4 @@
-// gemm_tma.cuh -- TMA-fed tcgen05 convolution forward (conv2 / conv3 of model/impala_actor_critic.py:7-8).
+// gemm_tma.cuh -- TMA-fed wgmma convolution forward (conv2 / conv3 of model/impala_actor_critic.py:7-8).
 //
 // The software-producer core (gemm_umma.cuh) spends its time in the LSU pipe: every A element is fetched with LDG,
 // split into hi/lo in registers and written to shared memory with STS.  For the NHWC convolutions this im2col
@@ -8,7 +8,7 @@
 //     tap (kh, kw):  base = act + ((kh*IH + kw)*CIN) floats
 //                    dims {CIN, OH, OH, images, plane}, strides {S*CIN, S*IH*CIN, IH*IH*CIN, plane} floats
 //                    box  {32, OH, OH, IMGS, 1}  ->  IMGS*OH*OH rows of 128 bytes, written with SWIZZLE_128B:
-//                    byte for byte the K-major UMMA operand tile (rows = output pixels of IMGS whole images).
+//                    byte for byte the K-major wgmma operand tile (rows = output pixels of IMGS whole images).
 //
 // The hi/lo split of 3xTF32 is done by the PRODUCING kernel's epilogue instead: plane 0 is the activation itself
 // (the tensor core reads the upper 19 bits of each 32-bit word, i.e. hi = trunc_tf32(x)), plane 1 holds
@@ -19,9 +19,10 @@
 // ignored by the epilogue):
 //   warps 0..5  TMA producers (one lane each): per K tile two tensor loads (planes 0/1) + one bulk copy, each issued
 //               by its own warp with arrive.expect_tx on full[stage]; two groups of three warps alternate K tiles
-//   warp 6      TMEM allocation + MMA issuer (12 tcgen05.mma per K tile), tcgen05.commit -> empty[stage] / acc_full
-//   warps 7..10 epilogue: tcgen05.ld of their TMEM lane quarter, bias + ReLU, coalesced stores of the activation
-//               and its lo plane (the next layer's TMA operand); two accumulator buffers overlap it with the MMAs
+//               (warps 6, 7 idle: the consumers start on a warpgroup boundary)
+//   warps 8..15 two consumer warpgroups (rows 0-63 / 64-127): 12 wgmma per K tile into the register accumulator,
+//               stage hand-back (empty), then bias + ReLU and coalesced stores of the activation and its lo plane (the
+//               next layer's TMA operand) while the producers already load the next tile
 #pragma once
 #include <cuda.h>
 
@@ -61,10 +62,11 @@ struct ConvTmaCfg {
   static constexpr int BOX_BYTES = ROWS * 128;           // bytes one tensor load delivers
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   static constexpr int PGROUPS = 2, PWARPS = 3 * PGROUPS;   // producer warps (one issuing lane each)
-  static constexpr int NT = (PWARPS + 1 + 4) * 32;
+  static constexpr int CW0 = 8;                          // first consumer warp (warpgroup aligned)
+  static constexpr int NT = CW0 * 32 + wg::kConsumerThreads;
   static constexpr int AUX_BYTES = 1024;
-  static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + AUX_BYTES + 4 * kEpiStageBytes + 1024;
-  static constexpr int TMEM_COLS = 2 * BN;
+  static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + AUX_BYTES + 8 * wg::kEpiWarpBytes + 1024;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
 template <int TAPS>
@@ -79,34 +81,23 @@ conv_fwd_tma_kernel(const __grid_constant__ ConvTmaMaps<Cfg::TAPS> maps, const u
   pdl_prologue();
   constexpr int NSTAGE = Cfg::NSTAGE, NKT = Cfg::NKT, BN = Cfg::BN;
   using TA = UmmaTile<128, true>;
-  using TB = UmmaTile<BN, false>;    // the weight image of a [K, N] row-major matrix is MN-major
+  using TB = UmmaTile<BN, false>;    // the weight image of a [K, N] row-major matrix (stored K-major by retile_b_kernel)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* aux = smem + NSTAGE * Cfg::STAGE_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty = full + NSTAGE;
-  uint64_t* acc_full = empty + NSTAGE;   // [2]
-  uint64_t* acc_empty = acc_full + 2;    // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 2);
   uint8_t* stg_base = aux + Cfg::AUX_BYTES;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
     for (int s = 0; s < NSTAGE; ++s) {
       umma::mbar_init(&full[s], 3);     // hi plane, lo plane, weight tile: one arrive.expect_tx each
-      umma::mbar_init(&empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      umma::mbar_init(&acc_full[b], 1);
-      umma::mbar_init(&acc_empty[b], 128);
+      umma::mbar_init(&empty[s], wg::kConsumerWGs);
     }
     umma::fence_barrier_init();
   }
-  if (warp == Cfg::PWARPS) umma::tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < Cfg::PWARPS) {
     // ================= TMA PRODUCERS =================
@@ -135,70 +126,35 @@ conv_fwd_tma_kernel(const __grid_constant__ ConvTmaMaps<Cfg::TAPS> maps, const u
         }
       }
     }
-  } else if (warp == Cfg::PWARPS) {
-    // ================= MMA ISSUER =================
-    constexpr uint32_t idesc = umma::make_idesc(BN, false, true);
+  } else if (warp >= Cfg::CW0) {
+    // ================= CONSUMERS (warpgroup cw = rows 64 cw .. 64 cw + 63 of the tile) =================
+    const int ct = tid - Cfg::CW0 * 32, cw = ct >> 7, cwarp = (ct >> 5) & 3;
+    uint8_t* stg = stg_base + (ct >> 5) * wg::kEpiWarpBytes;
     uint32_t it = 0;
-    int i = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++i) {
-      const int buf = i & 1;
-      umma::mbar_wait(&acc_empty[buf], (((uint32_t)i >> 1) & 1) ^ 1);
-      umma::tc_fence_after();
-      const uint32_t d = tmem_base + (uint32_t)(buf * BN);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       for (int kt = 0; kt < NKT; ++kt, ++it) {
         const int s = it % NSTAGE;
         umma::mbar_wait(&full[s], (it / NSTAGE) & 1);
-        umma::tc_fence_after();
-        if (umma::elect_one()) {
-          const uint32_t st = umma::smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint32_t a_hi = st, a_lo = st + Cfg::A_BYTES, b_hi = st + 2 * Cfg::A_BYTES, b_lo = b_hi + Cfg::B_BYTES;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t ao = TA::kslice_off(j), bo = TB::kslice_off(j);
-            const uint64_t dah = umma::make_desc(a_hi + ao, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-            const uint64_t dal = umma::make_desc(a_lo + ao, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-            const uint64_t dbh = umma::make_desc(b_hi + bo, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-            const uint64_t dbl = umma::make_desc(b_lo + bo, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-            umma::mma_tf32(d, dal, dbh, idesc, (kt > 0 || j > 0) ? 1u : 0u);   // small terms first
-            umma::mma_tf32(d, dah, dbl, idesc, 1u);
-            umma::mma_tf32(d, dah, dbh, idesc, 1u);
-          }
-          umma::mma_commit(&empty[s]);
-          if (kt == NKT - 1) umma::mma_commit(&acc_full[buf]);
-        }
-        __syncwarp();
+        const uint32_t st = umma::smem_u32(smem + s * Cfg::STAGE_BYTES);
+        const uint32_t a_hi = st + cw * 64 * 128, b_hi = st + 2 * Cfg::A_BYTES;
+        wg::fence_operand(acc);
+        wg::fence();
+        tf32_stage_mmas<BN, false, 32, TA, TB>(acc, a_hi, a_hi + Cfg::A_BYTES, b_hi, b_hi + Cfg::B_BYTES, kt == 0);
+        wg::commit();
+        wg::wait<1>();
+        wg::fence_operand(acc);
+        if (kt > 0 && (ct & 127) == 0) umma::mbar_arrive(&empty[(it - 1) % NSTAGE]);
       }
-    }
-    umma::tc_fence_before();
-  } else {
-    // ================= EPILOGUE (4 warps) =================
-    const int quarter = warp & 3;     // TMEM lanes 32*quarter .. +31
-    uint8_t* stg = stg_base + quarter * kEpiStageBytes;
-    int i = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++i) {
-      const int buf = i & 1;
-      const int img0 = tile * Cfg::IMGS;
-      const int row_base = img0 * Cfg::PIX;
+      wg::wait<0>();
+      wg::fence_operand(acc);
+      if ((ct & 127) == 0) umma::mbar_arrive(&empty[(it - 1) % NSTAGE]);
+      const int row_base = tile * Cfg::IMGS * Cfg::PIX;
       const int row_end = min(nimg * Cfg::PIX, row_base + Cfg::ROWS);
-      umma::mbar_wait(&acc_full[buf], ((uint32_t)i >> 1) & 1);
-      umma::tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        umma::tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN + c0), v);
-        if (c0 + 32 >= BN) {
-          umma::tc_fence_before();
-          umma::mbar_arrive(&acc_empty[buf]);
-        }
-        epilogue_store_32x32(ep, stg, lane, 0, row_base + quarter * 32, c0, row_end, BN, v);
-      }
+      wg_epilogue<BN>(ep, acc, stg, lane, 0, row_base + cw * 64 + cwarp * 16, 0, row_end, BN);
     }
-    umma::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == Cfg::PWARPS) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 

@@ -1,37 +1,36 @@
-// gemm_umma.cuh -- gather-GEMM on the 5th-generation tensor cores (tcgen05.mma, kind::tf32) with
-// fp32-grade accuracy by operand splitting ("3xTF32"):
+// gemm_umma.cuh -- gather-GEMM on the Hopper tensor cores (wgmma.mma_async, tf32 operands) with fp32-grade accuracy
+// by operand splitting ("3xTF32"):
 //
 //     x = hi + lo,  hi = rna_tf32(x),  lo = x - hi      (lo is exact in fp32, |lo| <= 2^-11 |x|)
 //     A*B ~= A_lo*B_hi + A_hi*B_lo + A_hi*B_hi           (dropped term A_lo*B_lo ~ 2^-22 relative)
 //
-// all three products accumulate in fp32 in ONE TMEM accumulator.  Same loader / epilogue functor
-// concepts as gemm_simt.cuh, so every layer of layers.cu can run on either core.
+// all three products accumulate in fp32 in ONE register accumulator.  Same loader / epilogue functor concepts as
+// gemm_simt.cuh, so every layer of layers.cu can run on either core.
 //
-// Structure (one 128 x BN output tile per CTA; 160-320 threads; 1-3 CTAs per SM depending on the configuration):
-//   warps 0..PW-1 (PW = 4 or 8): PRODUCERS, then EPILOGUE.  Each thread gathers float4 groups of A and B through the
-//               loader functors (im2col, concat, transposes, uint8 -> fp32 happen here), splits them into hi/lo and
-//               writes both into the stage's shared-memory operand tiles in the canonical swizzled UMMA layout
-//               (K-major for kContigK loaders, MN-major otherwise), then fence.proxy.async and mbarrier-arrive on
-//               full[stage].  A weight operand may instead arrive as a pre-split, pre-tiled image with one
-//               cp.async.bulk per stage (PretiledB; issued by warp PW+1 when Cfg::LW).
-//   warp PW   : TMEM allocation + MMA ISSUER: waits full[stage], one lane issues 3 x (BK/8)
-//               tcgen05.mma (M=128, N=BN, K=8) from shared-memory descriptors, then tcgen05.commit ->
-//               empty[stage]; after the last K tile tcgen05.commit -> acc_full.
-//   epilogue  : the producer warps read their 32 TMEM lanes (tcgen05.ld 32x32b.x32), transpose each 32x32 block
-//               through a swizzled shared tile (epilogue_store_32x32) and hand row segments to the epilogue
-//               functor (bias/ReLU/mask/split-K partial ...).
+// Structure (one 128 x BN output tile per CTA):
+//   warps 0..PW-1 (PW = 4 or 8): PRODUCERS.  Each thread gathers float4 groups of A and B through the loader functors
+//               (im2col, concat, transposes, uint8 -> fp32 happen here), splits them into hi/lo and writes both into
+//               the stage's shared-memory operand tiles in the canonical K-major SWIZZLE_128B layout (a loader whose
+//               contiguous dimension is M or N is transposed on the way: wgmma reads tf32 operands K-major only), then
+//               fence.proxy.async and mbarrier-arrive on full[stage].  A weight operand may instead arrive as a
+//               pre-split, pre-tiled image with one cp.async.bulk per stage (PretiledB; issued by warp PW+8 when
+//               Cfg::LW, else by producer thread 0).
+//   warps PW..PW+7: two CONSUMER warpgroups, rows 0-63 and 64-127 of the tile.  Each waits full[stage], issues
+//               3 x (BK/8) wgmma.mma_async (M=64, N=BN, K=8) from shared-memory descriptors into its fp32 register
+//               accumulator, keeps one stage of MMAs in flight and hands the previous stage back (empty[stage]).
+//               After the last K tile it drains the accumulator through a swizzled shared tile (wg_epilogue) into the
+//               epilogue functor (bias/ReLU/mask/split-K partial ...).
 // gemm_tma.cuh holds the TMA-fed variant (cp.async.bulk.tensor im2col boxes) for the conv2/conv3 forward.
 //
-// Canonical SWIZZLE_128B layouts (CuTe mma_traits_sm100.hpp::make_umma_desc), BK = 32 floats:
-//   K-major : row r is 128 contiguous bytes (32 floats of K) at r*128; the 16-byte chunk c of row r is
-//             stored at chunk position c ^ (r & 7)  (Swizzle<3,4,3>: address bits [4,7) ^= bits [7,10)).
-//             8-row groups are 1024 bytes apart (SBO = 1024).  A K=8 MMA slice j starts at +32*j bytes.
-//   MN-major: SWIZZLE_128B_BASE32B, atoms of 32 (mn) x 4 (k) -- see UmmaTile below.
-// All operand tiles are 1024-byte aligned (base_offset = 0).
+// Canonical SWIZZLE_128B K-major layout (CuTe GMMA::Layout_K_SW128_Atom), BK = 32 floats: row r is 128 contiguous
+// bytes (32 floats of K) at r*128; the 16-byte chunk c of row r is stored at chunk position c ^ (r & 7)
+// (Swizzle<3,4,3>: address bits [4,7) ^= bits [7,10)).  8-row groups are 1024 bytes apart (SBO = 1024).  A K=8 MMA
+// slice j starts at +32*j bytes.  All operand tiles are 1024-byte aligned (base_offset = 0).
 #pragma once
 #include <type_traits>
 
 #include "common.cuh"
+#include "wgmma_ops.cuh"
 
 namespace drl {
 namespace umma {
@@ -58,58 +57,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by one thread
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive columns (one 32-bit word each) -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// One lane of a converged warp, chosen by the hardware (elect.sync).  Unlike `lane == 0`, the compiler knows the branch
-// holds exactly one thread and keeps the tcgen05 operands (descriptors, TMEM address) in uniform registers with a plain
-// R2UR; with `lane == 0` it wrapped EVERY tcgen05.mma in an ELECT / R2UR.BROADCAST / BRA.U.ANY loop (cuobjdump), which
-// together with the per-MMA descriptor arithmetic cost ~120-165 cycles per MMA against 44-128 for the instruction itself
-// (tools/microbench/mma_rate.cu).
+// One lane of a converged warp, chosen by the hardware (elect.sync).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -118,27 +67,15 @@ __device__ __forceinline__ bool elect_one() {
 // descriptor = constant part (everything but the start address) + (shared-memory byte address >> 4)
 __device__ __forceinline__ uint64_t desc_at(uint64_t base, uint32_t saddr) { return base + (uint64_t)(saddr >> 4); }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): descriptor version 1 (sm_100), base_offset 0,
-// layout_type 2 = SWIZZLE_128B, 1 = SWIZZLE_128B_BASE32B
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                              uint32_t layout_type) {
+// shared-memory matrix descriptor of wgmma (cute::GMMA::GmmaDescriptor): start address, leading / stride byte offsets,
+// base_offset 0, layout type 1 = SWIZZLE_128B (bits 62-63)
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;   // version
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=F32, A=B=TF32, dense, no negate; M=128
-__host__ __device__ constexpr uint32_t make_idesc(int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4)                        // c_format  = F32
-         | (2u << 7)                      // a_format  = TF32
-         | (2u << 10)                     // b_format  = TF32
-         | ((a_mn_major ? 1u : 0u) << 15) // a_major
-         | ((b_mn_major ? 1u : 0u) << 16) // b_major
-         | ((uint32_t)(N >> 3) << 17)     // n_dim
-         | ((uint32_t)(128 >> 4) << 24);  // m_dim
 }
 
 __device__ __forceinline__ float tf32_hi(float x) {
@@ -153,44 +90,69 @@ __device__ __forceinline__ void split4(const float4& x, float4& h, float4& l) {
 
 }  // namespace umma
 
-// One operand tile of a stage: ROWS (128 for A, BN for B) x 32 floats.
-//   K-major : SWIZZLE_128B (layout type 2), rows of 128 bytes, 16-byte chunks XOR (row & 7).
-//   MN-major: SWIZZLE_128B_BASE32B (layout type 1) -- the ONLY shared-memory layout the hardware accepts for
-//             MN-major tf32 operands (cutlass sm100_common.inl:92).  Atoms of 32 (mn) x 4 (k) = 512 bytes:
-//             k-row kr is 128 contiguous bytes (32 mn values), its four 32-byte chunks XOR kr
-//             (Swizzle<2,5,2>: byte-address bits [5,7) ^= bits [7,9)).  Atom (g = mn/32, kg = k/4) sits at
-//             (kg*(ROWS/32) + g)*512: LBO (mn-group stride) = 512, SBO (k-group stride) = (ROWS/32)*512.
-//             A K=8 MMA slice j covers k-groups 2j, 2j+1 and starts at j*2*SBO.
+// ---- warpgroup MMA plumbing shared by every tensor-core kernel ----------------------------------------------------------
+namespace wg {
+constexpr int kConsumerWGs = 2;                       // two consumer warpgroups: rows 0-63 and 64-127 of a 128-row tile
+constexpr int kConsumerThreads = 128 * kConsumerWGs;
+constexpr int kEpiWarpBytes = 16 * 128;               // per consumer warp: one 16-row x 32-column staging tile
+
+__device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_operand(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// named barrier over the consumer warpgroups only (id 2; id 1 is the producers' column-sum barrier)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 2, %0;" ::"n"(kConsumerThreads) : "memory"); }
+}  // namespace wg
+
+// One operand tile of a stage: ROWS (128 for A, BN for B) x 32 floats, K-major SWIZZLE_128B, rows of 128 bytes, 16-byte
+// chunks XOR (row & 7).  KMAJOR says how the LOADER delivers the operand: K-major loaders hand over 4 consecutive k of
+// one row (one 16-byte chunk); the others hand over 4 consecutive rows of one k, which put() scatters into the four rows
+// (tf32 wgmma has no transposed operand mode).
 template <int ROWS, bool KMAJOR>
 struct UmmaTile {
   static constexpr int BK = 32;
   static constexpr int BYTES = ROWS * BK * 4;
-  static constexpr int LBO = KMAJOR ? 16 : 512;                       // K-major: unused by hw (canonical value 1 unit)
-  static constexpr int SBO = KMAJOR ? 1024 : (ROWS / 32) * 512;
-  static constexpr int LAYOUT_TYPE = KMAJOR ? 2 : 1;
-  // byte offset of the 16-byte chunk a loader group writes.
-  //   K-major : idx = row, k multiple of 4      MN-major : idx = row (multiple of 4), single k
+  static constexpr int LBO = 16;                       // unused by the hardware for swizzled K-major tiles
+  static constexpr int SBO = 1024;
+  // K-major: byte offset of the chunk holding [k, k+4) of row idx (k multiple of 4).  Otherwise: byte offset of element
+  // (row idx, k) with idx a multiple of 4 -- put() derives the other three rows from it.
   __device__ static __forceinline__ int chunk_off(int idx, int k) {
-    if (KMAJOR) return idx * 128 + ((((k >> 2) ^ idx) & 7) << 4);
-    const int kr = k & 3, c32 = (idx & 31) >> 3, half = (idx & 7) >> 2;
-    return ((k >> 2) * (ROWS / 32) + (idx >> 5)) * 512 + kr * 128 + ((c32 ^ kr) << 5) + (half << 4);
+    const int c = idx * 128 + ((((k >> 2) ^ idx) & 7) << 4);
+    return KMAJOR ? c : c + (k & 3) * 4;
+  }
+  __device__ static __forceinline__ void put(uint8_t* base, int off, const float4& v) {
+    if (KMAJOR) {
+      *reinterpret_cast<float4*>(base + off) = v;
+    } else {
+      // rows idx+j (idx % 4 == 0): chunk c ^ j, same offset inside the chunk
+      const int c = (off >> 4) & 7, b = off & ~0x70;
+      *reinterpret_cast<float*>(base + b + ((c ^ 0) << 4)) = v.x;
+      *reinterpret_cast<float*>(base + b + 128 + ((c ^ 1) << 4)) = v.y;
+      *reinterpret_cast<float*>(base + b + 256 + ((c ^ 2) << 4)) = v.z;
+      *reinterpret_cast<float*>(base + b + 384 + ((c ^ 3) << 4)) = v.w;
+    }
   }
   // descriptor start offset of the j-th K=8 slice
-  __device__ static __forceinline__ int kslice_off(int j) { return KMAJOR ? j * 32 : j * 2 * SBO; }
+  __device__ static __forceinline__ int kslice_off(int j) { return j * 32; }
 };
 
 template <int BN_, int STAGES_, int MINB_ = 1, int PW_ = 4, int LW_ = 0>
 struct UmmaCfg {
   static constexpr int BM = 128, BN = BN_, BK = 32, STAGES = STAGES_, MINB = MINB_;
-  static constexpr int PW = PW_;            // producer / epilogue warps (4 or 8), warps 0..PW-1
-  static constexpr int LW = LW_;            // 1: warp PW+1 issues the bulk copies of a pre-tiled B (see the kernel)
+  static constexpr int PW = PW_;            // producer warps (4 or 8), warps 0..PW-1
+  static constexpr int LW = LW_;            // 1: warp PW+8 issues the bulk copies of a pre-tiled B (see the kernel)
   static constexpr int NPROD = PW * 32;
-  static constexpr int NT = NPROD + 32 + 32 * LW;   // + the MMA warp (warp PW) [+ the B loader warp]
-  static constexpr int EPI_COLS = BN / (PW / 4);   // accumulator columns each producer warp drains
+  static constexpr int NT = NPROD + wg::kConsumerThreads + 32 * LW;   // + two consumer warpgroups [+ the B loader warp]
   static_assert(PW == 4 || PW == 8, "4 or 8 producer warps");
-  static_assert(EPI_COLS % 32 == 0, "epilogue reads 32 columns at a time");
-  static constexpr int TMEM_COLS = BN;
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
+  // the BN / 2 accumulator registers of a consumer thread must fit the per-thread register budget of the launch
+  static_assert(BN / 2 + 40 <= 65536 / (NT * MINB), "accumulator does not fit the register budget: fewer threads or CTAs");
 };
 
 // A loader may declare `static constexpr bool kExactTf32 = true` when its values are exactly representable in
@@ -241,29 +203,18 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 }
 }  // namespace umma
 
-// Epilogue store of one 32x32 accumulator block.  tcgen05.ld hands every lane one ROW (v[j] = D[row0 + lane][col0 + j]);
-// storing that directly makes each 128-bit store instruction touch 32 different 128-byte lines (ncu: the LSU data
-// pipe was the busiest unit of the epilogue-heavy kernels).  The block is transposed through a per-warp 4 KB
-// shared-memory tile instead (16-byte chunks XOR-swizzled by row & 7: conflict-free both ways), so that 8 lanes
-// cover one 128-byte row segment and an instruction touches 4 lines.  The functor sees the same (m, n) pairs.
-constexpr int kEpiStageBytes = 32 * 32 * 4;
 // An epilogue functor may provide `bias4(z, n)` + `store4b(z, m, n, o, bias)`: the per-column bias of a lane is the same
-// for all 8 rows it stores, so it is fetched ONCE per 32x32 block instead of once per element.  (Measured on the conv1
-// kernel: the streaming stores of the output evict the bias line from L1, each of the 8 row iterations then paid an L2
-// round trip for it, and the epilogue of one 128x32 tile took 11,000 cycles -- tools/conv1_timeline.py.)
+// for all rows it stores, so it is fetched ONCE per block instead of once per element.
 template <class EP, class = void>
 struct ep_has_bias4 : std::false_type {};
 template <class EP>
 struct ep_has_bias4<EP, std::void_t<decltype(std::declval<const EP&>().bias4(0, 0))>> : std::true_type {};
 
-template <class EP>
-__device__ __forceinline__ void epilogue_store_32x32(const EP& ep, uint8_t* stg, int lane, int z, int row0, int col0,
-                                                     int M, int N, const float (&v)[32]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-    *reinterpret_cast<float4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-        make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-  __syncwarp();
+// Second half of an epilogue store: a ROWS x 32 block staged in shared memory (row r = 128 bytes, 16-byte chunks XOR
+// (r & 7)) is read back row-wise, 8 lanes per 128-byte row segment, and handed to the functor (coalesced stores).
+template <int ROWS, class EP>
+__device__ __forceinline__ void epilogue_drain(const EP& ep, const uint8_t* stg, int lane, int z, int row0, int col0,
+                                               int M, int N) {
   const int c = lane & 7, rr = lane >> 3;
   const int n = col0 + c * 4;
   float4 bias = zero4();
@@ -271,7 +222,7 @@ __device__ __forceinline__ void epilogue_store_32x32(const EP& ep, uint8_t* stg,
     if (n + 3 < N) bias = ep.bias4(z, n);
   }
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
+  for (int i = 0; i < ROWS / 4; ++i) {
     const int r = i * 4 + rr;
     const float4 o4 = *reinterpret_cast<const float4*>(stg + r * 128 + ((c ^ (r & 7)) << 4));
     const int m = row0 + r;
@@ -290,7 +241,34 @@ __device__ __forceinline__ void epilogue_store_32x32(const EP& ep, uint8_t* stg,
       }
     }
   }
-  __syncwarp();
+}
+
+// Epilogue of one consumer warp: its 16 rows (row0 ..) of a 64 x BN wgmma accumulator (fragment: d[4c + e] holds row
+// lane/4 (+8 for e >= 2), column 8c + 2 (lane % 4) + (e & 1)), 32 columns at a time through its 2 KB staging tile.
+// FOLD: the accumulator holds [X | Y] of width BN and the epilogue sees X + Y (width BN / 2).
+template <int BN, bool FOLD = false, class EP>
+__device__ __forceinline__ void wg_epilogue(const EP& ep, const float (&acc)[BN / 2], uint8_t* stg, int lane, int z,
+                                            int row0, int n0, int M, int N) {
+  constexpr int W = FOLD ? BN / 2 : BN;
+  const int r = lane >> 2, q = lane & 3;
+#pragma unroll 1
+  for (int cb = 0; cb < W / 32; ++cb) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int i = (cb * 4 + c) * 4;
+      float2 lo = make_float2(acc[i], acc[i + 1]), hi = make_float2(acc[i + 2], acc[i + 3]);
+      if constexpr (FOLD) {
+        constexpr int H = BN / 4;   // the Y half starts BN / 2 columns = BN / 16 column groups = BN / 4 registers later
+        lo.x += acc[i + H]; lo.y += acc[i + H + 1]; hi.x += acc[i + H + 2]; hi.y += acc[i + H + 3];
+      }
+      const int chunk = 2 * c + (q >> 1), in = (q & 1) * 8;
+      *reinterpret_cast<float2*>(stg + r * 128 + ((chunk ^ (r & 7)) << 4) + in) = lo;
+      *reinterpret_cast<float2*>(stg + (r + 8) * 128 + ((chunk ^ (r & 7)) << 4) + in) = hi;
+    }
+    __syncwarp();
+    epilogue_drain<16>(ep, stg, lane, z, row0, n0 + cb * 32, M, N);
+    __syncwarp();
+  }
 }
 
 template <class Cfg, class AL, class BL>
@@ -300,9 +278,29 @@ struct UmmaSmem {
   static constexpr bool AEX = loader_exact<AL>::value;
   static constexpr int A_BYTES = TA::BYTES, B_BYTES = TB::BYTES;       // multiples of 1024
   static constexpr int STAGE_BYTES = (AEX ? 1 : 2) * A_BYTES + 2 * B_BYTES;   // hi (and lo) copies of the operands
-  static constexpr int AUX_BYTES = 1024 + (BL::kContigK ? 0 : Cfg::NPROD * 16);   // barriers, tmem ptr, colsum scratch
+  static constexpr int AUX_BYTES = 1024 + (BL::kContigK ? 0 : Cfg::NPROD * 16);   // barriers, colsum scratch
   static constexpr int BYTES = Cfg::STAGES * STAGE_BYTES + AUX_BYTES + 1024;      // + alignment slack
+  static_assert(Cfg::STAGES * STAGE_BYTES >= 8 * wg::kEpiWarpBytes, "epilogue staging tiles live in the dead stages");
 };
+
+// The 3xTF32 MMAs of one stage for consumer warpgroup `cw` (A rows 64 cw ..): 3 (2 for an exact A) products per K=8 slice.
+template <int BN, bool AEX, int BK, class TA, class TB>
+__device__ __forceinline__ void tf32_stage_mmas(float (&acc)[BN / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+                                                uint32_t b_lo, bool first_tile) {
+  const uint64_t da = umma::make_desc(0, TA::LBO, TA::SBO), db = umma::make_desc(0, TB::LBO, TB::SBO);
+#pragma unroll
+  for (int j = 0; j < BK / 8; ++j) {
+    const uint32_t ao = TA::kslice_off(j), bo = TB::kslice_off(j);
+    const uint32_t first = (!first_tile || j > 0) ? 1u : 0u;
+    if (!AEX) {                                                    // small terms first
+      wg::WgTf32<BN>::mma(acc, umma::desc_at(da, a_lo + ao), umma::desc_at(db, b_hi + bo), first);
+      wg::WgTf32<BN>::mma(acc, umma::desc_at(da, a_hi + ao), umma::desc_at(db, b_lo + bo), 1u);
+    } else {
+      wg::WgTf32<BN>::mma(acc, umma::desc_at(da, a_hi + ao), umma::desc_at(db, b_lo + bo), first);
+    }
+    wg::WgTf32<BN>::mma(acc, umma::desc_at(da, a_hi + ao), umma::desc_at(db, b_hi + bo), 1u);
+  }
+}
 
 template <class Cfg, class AL, class BL, class EP>
 __global__ void __launch_bounds__(Cfg::NT, Cfg::MINB)
@@ -317,9 +315,8 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
   constexpr int NGA = BM * BK / 4, NGB = BN * BK / 4;       // float4 groups per stage
   constexpr bool A16 = loader_vec16<AL>::value;              // 16-element (one 128-bit load) A groups
   constexpr bool BPT = loader_pretiled<BL>::value;           // B arrives as pre-split stage images via cp.async.bulk
-  // A cp.async.bulk blocks its issuing thread for ~0.24 us whatever its size (tools/microbench/tma_box_bw.cu).  Issued
-  // by producer thread 0 that delay sits in front of its own gathers and so of every stage's full barrier; with
-  // Cfg::LW a dedicated warp (PW+1) issues the copies instead and arrives on the barrier itself.
+  // with Cfg::LW a dedicated warp (PW+8) issues the bulk copies and arrives on the barrier itself; otherwise producer
+  // thread 0 does, in front of its own gathers
   constexpr bool LWB = BPT && Cfg::LW;
   constexpr int GA = (A16 ? NGA / 4 : NGA) / NPROD, GB = BPT ? 1 : NGB / NPROD;   // groups per producer thread
   static_assert((A16 ? NGA / 4 : NGA) % NPROD == 0 && NGB % NPROD == 0, "groups must divide among producers");
@@ -333,8 +330,6 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
   uint8_t* aux = smem + STAGES * SM::STAGE_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_full + 1);
   float4* cs_scratch = reinterpret_cast<float4*>(aux + 1024);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -347,23 +342,18 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       umma::mbar_init(&full[s], NPROD + (LWB ? 1 : 0));
-      umma::mbar_init(&empty[s], 1);
+      umma::mbar_init(&empty[s], wg::kConsumerWGs);
     }
-    umma::mbar_init(acc_full, 1);
     umma::fence_barrier_init();
   }
-  if (warp == Cfg::PW) umma::tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < Cfg::PW) {
     // ================= PRODUCERS =================
     // K-major operand : group g -> row g/8, chunk g%8  (8 lanes cover one 128-byte row: coalesced global
     //                   read of 128 contiguous bytes, conflict-free swizzled 16-byte stores)
     // MN-major operand: group g -> k = g/(ROWS/4), quad q = g%(ROWS/4)  (8 lanes cover 32 contiguous mn
-    //                   values of one k: coalesced, conflict-free)
+    //                   values of one k: coalesced)
     typename AL::Row arow[GA];
     typename BL::Row brow[GB];
     int a_k[GA], a_o[GA], b_k[GB], b_o[GB];
@@ -371,7 +361,7 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
     for (int i = 0; i < GA; ++i) {
       const int g = tid + i * NPROD;
       if (A16) {
-        if (AK) {   // group = (row, 16-k half): 32 lanes = 32 consecutive rows -> coalesced, conflict-free stores
+        if (AK) {   // group = (row, 16-k half): 32 lanes = 32 consecutive rows
           const int r = g % BM, half = g / BM;
           arow[i] = al.row(z, (m0 + r < M) ? m0 + r : -1);
           a_k[i] = half * 16;
@@ -454,15 +444,15 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const int off = AK ? TA::chunk_off(a_o[i], a_k[i] + 4 * j) : TA::chunk_off(a_o[i] + 4 * j, a_k[i]);
-            *reinterpret_cast<float4*>(st + off) = f[j];
+            TA::put(st, off, f[j]);
           }
         } else if constexpr (AEX) {
-          *reinterpret_cast<float4*>(st + a_o[i]) = ra[i];
+          TA::put(st, a_o[i], ra[i]);
         } else {
           float4 h, l;
           umma::split4(ra[i], h, l);
-          *reinterpret_cast<float4*>(st + a_o[i]) = h;
-          *reinterpret_cast<float4*>(st + OFF_ALO + a_o[i]) = l;
+          TA::put(st, a_o[i], h);
+          TA::put(st + OFF_ALO, a_o[i], l);
         }
       }
       if constexpr (!BPT) {
@@ -470,8 +460,8 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
         for (int i = 0; i < GB; ++i) {
           float4 h, l;
           umma::split4(rb[i], h, l);
-          *reinterpret_cast<float4*>(st + OFF_BHI + b_o[i]) = h;
-          *reinterpret_cast<float4*>(st + OFF_BLO + b_o[i]) = l;
+          TB::put(st + OFF_BHI, b_o[i], h);
+          TB::put(st + OFF_BLO, b_o[i], l);
           if (kColSum) { csum[i].x += rb[i].x; csum[i].y += rb[i].y; csum[i].z += rb[i].z; csum[i].w += rb[i].w; }
         }
       }
@@ -480,9 +470,10 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
     };
 
     // register prefetch ring of depth PF: the gathers of tiles t+1 .. t+PF-1 are in flight while tile t is split
-    // and stored (these kernels are bound by per-K-tile latency, not by producer throughput).  The uint8 operand
-    // needs 8 registers per tile, and a pre-tiled B needs none, so those cases afford a deeper ring.
-    constexpr int PF = A16 ? 4 : (BPT ? 3 : 2);
+    // and stored.  The accumulators live in registers of the same CTA, so the ring is capped at ~96 registers.
+    constexpr int RPT = 4 * (GA + (BPT ? 0 : GB));             // registers one gathered tile occupies
+    constexpr int PF0 = A16 ? 4 : (BPT ? 3 : 2);
+    constexpr int PF = (PF0 * RPT <= 96) ? PF0 : (96 / RPT >= 1 ? 96 / RPT : 1);
     ARaw ra[PF][GA];
     float4 rb[PF][GB];
 #pragma unroll
@@ -521,24 +512,8 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
         if (n + 3 < N) ep.store_colsum(z, n + 3, tot.w);
       }
     }
-
-    // ================= EPILOGUE =================
-    umma::mbar_wait(acc_full, 0);
-    umma::tc_fence_after();
-    // warp w may only touch TMEM lanes 32*(w%4)..+31; with 8 warps the two warps of a lane quarter split the columns.
-    // Every MMA has completed, so the pipeline stages are dead: their first bytes become the per-warp staging tiles.
-    uint8_t* stg = smem + warp * kEpiStageBytes;
-    const int row0 = m0 + (warp & 3) * 32;
-    const int cbeg = (warp >> 2) * Cfg::EPI_COLS;
-#pragma unroll 1
-    for (int c0 = cbeg; c0 < cbeg + Cfg::EPI_COLS; c0 += 32) {
-      float v[32];
-      umma::tmem_ld32(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)c0, v);
-      epilogue_store_32x32(ep, stg, lane, z, row0, n0 + c0, M, N, v);
-    }
-    umma::tc_fence_before();
-  } else if (warp > Cfg::PW) {
-    // ================= B LOADER (warp PW+1, Cfg::LW) =================
+  } else if (warp >= Cfg::PW + 8) {
+    // ================= B LOADER (warp PW+8, Cfg::LW) =================
     if constexpr (LWB) {
       if (lane == 0) {
         for (int t = 0; t < ntiles; ++t) {
@@ -554,43 +529,31 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
       }
     }
   } else {
-    // ================= MMA ISSUER (warp PW) =================
-    constexpr uint32_t idesc = umma::make_idesc(BN, !AK, !BKc);
+    // ================= CONSUMERS (warps PW .. PW+7: warpgroup cw = rows 64 cw .. 64 cw + 63) =================
+    const int ct = tid - NPROD, cw = ct >> 7, cwarp = (ct >> 5) & 3;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int t = 0; t < ntiles; ++t) {
       const int s = t % STAGES;
-      const uint32_t ph = (t / STAGES) & 1;
-      umma::mbar_wait(&full[s], ph);
-      umma::tc_fence_after();
-      if (umma::elect_one()) {
-        const uint32_t st = umma::smem_u32(smem + s * SM::STAGE_BYTES);
-        const uint32_t a_hi = st, a_lo = st + OFF_ALO, b_hi = st + OFF_BHI, b_lo = st + OFF_BLO;
-#pragma unroll
-        for (int j = 0; j < BK / 8; ++j) {
-          const uint32_t ao = TA::kslice_off(j), bo = TB::kslice_off(j);
-          const uint64_t dah = umma::make_desc(a_hi + ao, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-          const uint64_t dbh = umma::make_desc(b_hi + bo, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-          const uint64_t dbl = umma::make_desc(b_lo + bo, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-          const uint32_t first = (t > 0 || j > 0) ? 1u : 0u;
-          if (!AEX) {                                                    // small terms first
-            const uint64_t dal = umma::make_desc(a_lo + ao, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-            umma::mma_tf32(tmem_base, dal, dbh, idesc, first);
-            umma::mma_tf32(tmem_base, dah, dbl, idesc, 1u);
-          } else {
-            umma::mma_tf32(tmem_base, dah, dbl, idesc, first);
-          }
-          umma::mma_tf32(tmem_base, dah, dbh, idesc, 1u);
-        }
-        umma::mma_commit(&empty[s]);            // frees the smem slot once these MMAs have read it
-        if (t == ntiles - 1) umma::mma_commit(acc_full);
-      }
-      __syncwarp();
+      umma::mbar_wait(&full[s], (t / STAGES) & 1);
+      const uint32_t st = umma::smem_u32(smem + s * SM::STAGE_BYTES);
+      const uint32_t a_hi = st + cw * 64 * 128;
+      wg::fence_operand(acc);
+      wg::fence();
+      tf32_stage_mmas<BN, AEX, BK, TA, TB>(acc, a_hi, a_hi + OFF_ALO, st + OFF_BHI, st + OFF_BLO, t == 0);
+      wg::commit();
+      wg::wait<1>();                                   // the MMAs of stage t-1 are complete: hand it back
+      wg::fence_operand(acc);
+      if (t > 0 && (ct & 127) == 0) umma::mbar_arrive(&empty[(t - 1) % STAGES]);
     }
-    umma::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == Cfg::PW) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+    wg::wait<0>();
+    wg::fence_operand(acc);
+    // ================= EPILOGUE =================
+    // both warpgroups' MMAs are complete, so the pipeline stages are dead: their first bytes become the staging tiles
+    wg::consumer_sync();
+    uint8_t* stg = smem + (ct >> 5) * wg::kEpiWarpBytes;
+    wg_epilogue<BN>(ep, acc, stg, lane, z, m0 + cw * 64 + cwarp * 16, n0, M, N);
   }
 }
 
@@ -619,8 +582,8 @@ __global__ void __launch_bounds__(256) retile_b_kernel(const BL bl, int N, int K
   float4 h, l;
   umma::split4(v, h, l);
   uint8_t* dst = image + (size_t)tile * (2 * TB::BYTES);
-  *reinterpret_cast<float4*>(dst + off) = h;
-  *reinterpret_cast<float4*>(dst + TB::BYTES + off) = l;
+  TB::put(dst, off, h);
+  TB::put(dst + TB::BYTES, off, l);
 }
 
 template <int BN>
@@ -651,6 +614,7 @@ inline int launch_gemm_umma(cudaStream_t s, const AL& al, const BL& bl, const EP
     return DRL_ERR_INVALID;
   }
   if (kchunk < 1 || K < 1) { set_error("gemm_umma: empty K range"); return DRL_ERR_INVALID; }
+  static_assert(Cfg::STAGES >= 2, "consumers hand a stage back only after the next stage's MMAs are issued");
   dim3 grid(cdiv(M, Cfg::BM), cdiv(N, Cfg::BN), zcount);
   DRL_CUDA_CHECK((launch_k(kern, grid, Cfg::NT, SM::BYTES, s, al, bl, ep, M, N, K, kchunk, kstep)));
   return DRL_OK;

@@ -1,5 +1,5 @@
-// gemm_umma16.cuh -- gather-GEMM on the 5th-generation tensor cores with 16-BIT SPLIT operands (tcgen05.mma kind::f16,
-// fp32 accumulation in TMEM): fp32-grade results from half-width operand tiles.
+// gemm_umma16.cuh -- gather-GEMM on the Hopper tensor cores with 16-BIT SPLIT operands (wgmma.mma_async f16 / bf16,
+// fp32 accumulation in registers): fp32-grade results from half-width operand tiles.
 //
 //     x = hi + lo + e,   hi = rn16(x),  lo = rn16(x - hi)          (x - hi is exact in fp32)
 //     A*B ~= A_lo*B_hi + A_hi*B_lo + A_hi*B_hi                     (dropped: A_lo*B_lo and the e terms)
@@ -8,16 +8,15 @@
 //   bf16     8 bits     2^-17       2^-16               fp32's own (no overflow / underflow concerns)
 //   fp16     11 bits    2^-22       2^-22               6e-8 .. 65504 (lo underflows gradually below |x| ~ 1e-4:
 //                                                       absolute error <= 3e-8; conversion saturates, never inf)
-// Both operands of one GEMM must use the SAME format: the instruction descriptor has separate a_format / b_format
-// fields, but f16 x bf16 traps with "illegal instruction" on the B200 (measured: tools/diag_mode5b.py, cores 9 / 10).
-// The format is therefore chosen per GEMM.  Compared with the 3xTF32
-// core (gemm_umma.cuh): an operand element costs 4 bytes of shared memory (hi + lo) instead of 8, so a pipeline stage
-// of the same size covers K = 64 instead of 32, the tensor core reads half the bytes per product, and each MMA
-// instruction retires K = 16 instead of 8 at the same issue cost.  ncu showed the 3xTF32 kernels bound by exactly that
-// shared-memory traffic (producer writes + 3 operand reads per K tile), with the tensor pipe 13-37 % busy.
+// Both operands of one GEMM use the SAME format (wgmma has one type for A and B); the format is chosen per GEMM.
+// Compared with the 3xTF32 core (gemm_umma.cuh): an operand element costs 4 bytes of shared memory (hi + lo) instead
+// of 8, so a pipeline stage of the same size covers K = 64 instead of 32, the tensor core reads half the bytes per
+// product, each MMA instruction retires K = 16 instead of 8, and 16-bit operands may be MN-major (no transposing
+// stores in the producers).
 //
-// Same structure as gemm_umma_kernel (producer / epilogue warps 0..PW-1, MMA warp PW, optional bulk-copy loader warp
-// PW+1 for pre-tiled weight images), same loader / epilogue functors.  Differences:
+// Same structure as gemm_umma_kernel (producer warps 0..PW-1, two consumer warpgroups PW..PW+7 that issue the MMAs and
+// run the epilogue, optional bulk-copy loader warp PW+8 for pre-tiled weight images), same loader / epilogue functors.
+// Differences:
 //   * a stage is filled in two SUB-TILES of K = 32 (so the per-thread register footprint of the gathers stays that of
 //     the 3xTF32 kernel); a producer "unit" is 8 consecutive elements of the loader's contiguous dimension = two float4
 //     loads -> one 16-byte chunk of hi and one of lo;
@@ -25,7 +24,7 @@
 //                     8-row groups 1024 bytes apart; a K = 16 slice j starts at +32 j bytes;
 //     MN-major tiles: SWIZZLE_128B atoms of 64 (mn) x 8 (k) = 1024 bytes (k-row kr = 128 contiguous bytes, chunk ^ kr);
 //                     atom (g = mn / 64, kg = k / 8) at (kg * (ROWS / 64) + g) * 1024: LBO = 1024, SBO = (ROWS/64)*1024;
-//                     a K = 16 slice j covers k-groups 2j, 2j+1 and starts at 2 j SBO   (cute: make_umma_desc<Major::MN>);
+//                     a K = 16 slice j covers k-groups 2j, 2j+1 and starts at 2 j SBO   (cute: make_gmma_desc<Major::MN>);
 //   * uint8 operands (the frames) are exact in fp16: one plane, two products, 16 bytes -> 16 halves with PRMT + HSUB2;
 //   * pre-tiled weight images are always K-major (retile_b16_kernel), whatever the weight's own layout.
 #pragma once
@@ -35,7 +34,8 @@ namespace drl {
 namespace umma16 {
 
 struct BF16 {
-  static constexpr uint32_t kFormat = 1;   // InstrDescriptor a_format / b_format for kind::f16
+  static constexpr uint32_t kFormat = 1;
+  static constexpr bool kBf16 = true;
   __device__ static __forceinline__ uint32_t pack2(float lo_elem, float hi_elem) {
     uint32_t r;
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));   // d = {a (upper), b (lower)}
@@ -47,6 +47,7 @@ struct BF16 {
 };
 struct F16 {
   static constexpr uint32_t kFormat = 0;
+  static constexpr bool kBf16 = false;
   __device__ static __forceinline__ uint32_t pack2(float lo_elem, float hi_elem) {
     uint32_t r;
     asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
@@ -83,19 +84,10 @@ __device__ __forceinline__ uint2 u8x4_to_h4(uint32_t w) {
   return make_uint2(r0, r1);
 }
 
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// instruction descriptor for kind::f16: D = F32, A/B = F16 (0) or BF16 (1), dense, no negate; M = 128
-__host__ __device__ constexpr uint32_t make_idesc16(int N, uint32_t afmt, uint32_t bfmt, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (afmt << 7) | (bfmt << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+// D (+)= A * B for one warpgroup (M = 64, N, K = 16); F: BF16 / F16, TA / TB: 1 for an MN-major A / B tile
+template <int N, class F, int TA, int TB>
+__device__ __forceinline__ void mma16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  wg::Wg16<N, F::kBf16, TA, TB>::mma(d, adesc, bdesc, accumulate);
 }
 
 }  // namespace umma16
@@ -107,7 +99,6 @@ struct Umma16Tile {
   static constexpr int BYTES = ROWS * 128;
   static constexpr int LBO = KMAJOR ? 16 : 1024;
   static constexpr int SBO = KMAJOR ? 1024 : (ROWS / 64) * 1024;
-  static constexpr int LAYOUT_TYPE = 2;   // SWIZZLE_128B for both majors (the BASE32B restriction is tf32-only)
   static_assert(KMAJOR || ROWS % 64 == 0, "MN-major 16-bit tiles are built from 64-element atoms");
   // byte offset of the 16-byte chunk holding elements [k, k+8) of row `idx` (K-major; k multiple of 8) or elements
   // [idx, idx+8) of k-row `k` (MN-major; idx multiple of 8)
@@ -125,12 +116,10 @@ struct Umma16Cfg {
   static constexpr int BM = 128, BN = BN_, BK = 64, SUBK = 32, STAGES = STAGES_, MINB = MINB_;
   static constexpr int PW = PW_, LW = LW_;
   static constexpr int NPROD = PW * 32;
-  static constexpr int NT = NPROD + 32 + 32 * LW;
-  static constexpr int EPI_COLS = BN / (PW / 4);
+  static constexpr int NT = NPROD + wg::kConsumerThreads + 32 * LW;   // producers + two consumer warpgroups [+ loader]
   static_assert(PW == 4 || PW == 8, "4 or 8 producer warps");
-  static_assert(EPI_COLS % 32 == 0, "epilogue reads 32 columns at a time");
-  static constexpr int TMEM_COLS = BN;
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
+  static_assert(BN / 2 + 40 <= 65536 / (NT * MINB), "accumulator does not fit the register budget: fewer threads or CTAs");
   using AF = AF_;   // 16-bit format of the A operand (uint8 operands are always fp16: exact)
   using BF = BF_;
 };
@@ -142,8 +131,8 @@ struct Umma16Smem {
   static constexpr bool AEX = loader_exact<AL>::value;
   static constexpr int A_BYTES = TA::BYTES, B_BYTES = TB::BYTES;
   static constexpr int STAGE_BYTES = (AEX ? 1 : 2) * A_BYTES + 2 * B_BYTES;
-  static constexpr int AUX_BYTES = 1024 + Cfg::NPROD * 32;   // barriers, tmem ptr, column-sum scratch (8 floats / thread)
-  static constexpr int EPI_BYTES = Cfg::PW * kEpiStageBytes; // the dead stages are reused; never larger than one stage
+  static constexpr int AUX_BYTES = 1024 + Cfg::NPROD * 32;   // barriers, column-sum scratch (8 floats / thread)
+  static constexpr int EPI_BYTES = 8 * wg::kEpiWarpBytes;    // the dead stages are reused
   static constexpr int BYTES = Cfg::STAGES * STAGE_BYTES + AUX_BYTES + 1024;
   static_assert(Cfg::STAGES * STAGE_BYTES >= EPI_BYTES, "epilogue staging tiles must fit into the pipeline stages");
 };
@@ -207,8 +196,6 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
   uint8_t* aux = smem + STAGES * SM::STAGE_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_full + 1);
   float4* cs_scratch = reinterpret_cast<float4*>(aux + 1024);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -221,16 +208,11 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       umma::mbar_init(&full[s], NPROD + (LWB ? 1 : 0));
-      umma::mbar_init(&empty[s], 1);
+      umma::mbar_init(&empty[s], wg::kConsumerWGs);
     }
-    umma::mbar_init(acc_full, 1);
     umma::fence_barrier_init();
   }
-  if (warp == Cfg::PW) umma::tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   if (tid == 0) TR(2);
 
   if (warp < Cfg::PW) {
@@ -380,7 +362,10 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
       if (tid == 0) TR(2000 + g);
     };
 
-    constexpr int PF = Cfg::PFD > 0 ? Cfg::PFD : (A16 ? 4 : (BPT ? 3 : 2));   // register prefetch ring, in sub-tiles
+    // register prefetch ring, in sub-tiles; the accumulators live in registers of the same CTA, so it is capped at ~96
+    constexpr int RPS = 4 * UA * AR + (BPT ? 0 : 8 * UB);      // registers one gathered sub-tile occupies
+    constexpr int PF0 = Cfg::PFD > 0 ? Cfg::PFD : (A16 ? 4 : (BPT ? 3 : 2));
+    constexpr int PF = (PF0 * RPS <= 96) ? PF0 : (96 / RPS >= 1 ? 96 / RPS : 1);
     const int nsub = 2 * ntiles;
     ARaw ra[PF][UA][AR];
     float4 rb[PF][UB][2];
@@ -426,23 +411,8 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
       }
     }
 
-    // ================= EPILOGUE =================
-    umma::mbar_wait(acc_full, 0);
-    umma::tc_fence_after();
-    if (tid == 0) TR(6000);
-    uint8_t* stg = smem + warp * kEpiStageBytes;
-    const int row0 = m0 + (warp & 3) * 32;
-    const int cbeg = (warp >> 2) * Cfg::EPI_COLS;
-#pragma unroll 1
-    for (int c0 = cbeg; c0 < cbeg + Cfg::EPI_COLS; c0 += 32) {
-      float v[32];
-      umma::tmem_ld32(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)c0, v);
-      epilogue_store_32x32(ep, stg, lane, z, row0, n0 + c0, M, N, v);
-    }
-    if (tid == 0) TR(6001);
-    umma::tc_fence_before();
-  } else if (warp > Cfg::PW) {
-    // ================= B LOADER (warp PW+1, Cfg::LW) =================
+  } else if (warp >= Cfg::PW + 8) {
+    // ================= B LOADER (warp PW+8, Cfg::LW) =================
     if constexpr (LWB) {
       if (lane == 0) {
         for (int t = 0; t < ntiles; ++t) {
@@ -459,44 +429,50 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
       }
     }
   } else {
-    // ================= MMA ISSUER (warp PW) =================
-    constexpr uint32_t idesc = umma16::make_idesc16(BN, AF::kFormat, BF::kFormat, !AK, !BKc);
+    // ================= CONSUMERS (warps PW .. PW+7: warpgroup cw = rows 64 cw .. 64 cw + 63) =================
+    const int ct = tid - NPROD, cw = ct >> 7, cwarp = (ct >> 5) & 3;
+    // A rows of this warpgroup: K-major +64 rows of 128 bytes; MN-major the second 64-element atom of every k-group
+    const uint32_t a_off = AK ? (uint32_t)(cw * 64 * 128) : (uint32_t)(cw * 1024);
+    const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO), db_base = umma::make_desc(0, TB::LBO, TB::SBO);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int t = 0; t < ntiles; ++t) {
       const int s = t % STAGES;
       umma::mbar_wait(&full[s], (t / STAGES) & 1);
-      umma::tc_fence_after();
-      if (umma::elect_one()) {
-        TR(3000 + t);
-        const uint32_t st = umma::smem_u32(smem + s * SM::STAGE_BYTES);
-        // descriptors: constant part + (address >> 4); all offsets are multiples of 16 bytes
-        const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-        const uint64_t db_base = umma::make_desc(0, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-        const uint64_t a_hi = umma::desc_at(da_base, st), a_lo = umma::desc_at(da_base, st + OFF_ALO);
-        const uint64_t b_hi = umma::desc_at(db_base, st + OFF_BHI), b_lo = umma::desc_at(db_base, st + OFF_BLO);
+      if (ct == 0) TR(3000 + t);
+      const uint32_t st = umma::smem_u32(smem + s * SM::STAGE_BYTES);
+      const uint64_t a_hi = umma::desc_at(da_base, st + a_off), a_lo = umma::desc_at(da_base, st + OFF_ALO + a_off);
+      const uint64_t b_hi = umma::desc_at(db_base, st + OFF_BHI), b_lo = umma::desc_at(db_base, st + OFF_BLO);
+      constexpr int TAm = AK ? 0 : 1, TBm = BKc ? 0 : 1;
+      wg::fence_operand(acc);
+      wg::fence();
 #pragma unroll
-        for (int j = 0; j < BK / 16; ++j) {
-          const uint64_t ao = (uint64_t)(TA::kslice_off(j) >> 4), bo = (uint64_t)(TB::kslice_off(j) >> 4);
-          const uint32_t first = (t > 0 || j > 0) ? 1u : 0u;
-          if (!AEX) {                                                    // small terms first
-            umma16::mma_f16(tmem_base, a_lo + ao, b_hi + bo, idesc, first);
-            umma16::mma_f16(tmem_base, a_hi + ao, b_lo + bo, idesc, 1u);
-          } else {
-            umma16::mma_f16(tmem_base, a_hi + ao, b_lo + bo, idesc, first);
-          }
-          umma16::mma_f16(tmem_base, a_hi + ao, b_hi + bo, idesc, 1u);
+      for (int j = 0; j < BK / 16; ++j) {
+        const uint64_t ao = (uint64_t)(TA::kslice_off(j) >> 4), bo = (uint64_t)(TB::kslice_off(j) >> 4);
+        const uint32_t first = (t > 0 || j > 0) ? 1u : 0u;
+        if (!AEX) {                                                    // small terms first
+          umma16::mma16<BN, AF, TAm, TBm>(acc, a_lo + ao, b_hi + bo, first);
+          umma16::mma16<BN, AF, TAm, TBm>(acc, a_hi + ao, b_lo + bo, 1u);
+        } else {
+          umma16::mma16<BN, AF, TAm, TBm>(acc, a_hi + ao, b_lo + bo, first);
         }
-        umma::mma_commit(&empty[s]);
-        if (t == ntiles - 1) umma::mma_commit(acc_full);
-        TR(4000 + t);
+        umma16::mma16<BN, AF, TAm, TBm>(acc, a_hi + ao, b_hi + bo, 1u);
       }
-      __syncwarp();
+      wg::commit();
+      wg::wait<1>();                                   // the MMAs of stage t-1 are complete: hand it back
+      wg::fence_operand(acc);
+      if (t > 0 && (ct & 127) == 0) umma::mbar_arrive(&empty[(t - 1) % STAGES]);
+      if (ct == 0) TR(4000 + t);
     }
-    umma::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == Cfg::PW) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+    wg::wait<0>();
+    wg::fence_operand(acc);
+    // ================= EPILOGUE =================
+    wg::consumer_sync();                               // both warpgroups are done with the stages: reuse them
+    if (ct == 0) TR(6000);
+    uint8_t* stg = smem + (ct >> 5) * wg::kEpiWarpBytes;
+    wg_epilogue<BN>(ep, acc, stg, lane, z, m0 + cw * 64 + cwarp * 16, n0, M, N);
+    if (ct == 0) TR(6001);
   }
 }
 
@@ -619,6 +595,11 @@ inline int launch_gemm_umma16(cudaStream_t s, const AL& al, const BL& bl, const 
     return DRL_ERR_INVALID;
   }
   if (kchunk < 1 || K < 1) { set_error("gemm_umma16: empty K range"); return DRL_ERR_INVALID; }
+  // consumers hand a stage back only after the MMAs of the NEXT stage are issued: one stage holds one K tile at most
+  if (Cfg::STAGES < 2 && (kchunk > Cfg::BK || (zcount == 1 && K > Cfg::BK))) {
+    set_error("gemm_umma16: a single-stage configuration takes K <= %d per split (kchunk %d, K %d)", Cfg::BK, kchunk, K);
+    return DRL_ERR_INVALID;
+  }
   dim3 grid(cdiv(M, Cfg::BM), cdiv(N, Cfg::BN), zcount);
   DRL_CUDA_CHECK((launch_k(kern, grid, Cfg::NT, SM::BYTES, s, al, bl, ep, M, N, K, kchunk, kstep)));
   return DRL_OK;

@@ -1,14 +1,13 @@
-// gemm_umma_persist.cuh -- persistent, fully warp-specialised variant of the tcgen05 3xTF32 gather-GEMM
+// gemm_umma_persist.cuh -- persistent, warp-specialised variant of the wgmma 3xTF32 gather-GEMM
 // (same operand layouts / loaders / epilogues as gemm_umma.cuh; see there for the math and the layouts).
 //
 //   grid = one CTA per SM; every CTA walks the tile list  tile = blockIdx.x, += gridDim.x  (m fastest)
 //   warps 0..PW-1   PRODUCERS   gather -> hi/lo split -> swizzled smem stage (ring continues across tiles,
 //                               register double buffering continues across tile boundaries)
-//   warp  PW        MMA ISSUER  tcgen05.mma into TMEM accumulator buffer (tile & 1); tcgen05.commit frees the
-//                               smem stage, and after the last K tile signals acc_full[buf]
-//   warps PW+1..+4  EPILOGUE    wait acc_full[buf], tcgen05.ld their lane quarter, release the buffer
-//                               (acc_empty[buf]) and run the epilogue functor -- overlapping the next
-//                               tile's gathers and MMAs (two accumulator buffers of BN columns each)
+//   warps PW..PW+7  CONSUMERS   two warpgroups (rows 0-63 / 64-127): wgmma into the register accumulator, hand each
+//                               stage back once its MMAs are complete, then run the epilogue of the tile through
+//                               their own staging tiles -- while the producers already fill the ring for the next
+//                               tile
 #pragma once
 #include <algorithm>
 
@@ -20,10 +19,11 @@ template <int BN_, int STAGES_, int PW_ = 8>
 struct UmmaPCfg {
   static constexpr int BM = 128, BN = BN_, BK = 32, STAGES = STAGES_, PW = PW_;
   static constexpr int NPROD = PW * 32;
-  static constexpr int NT = (PW + 5) * 32;          // producers + MMA warp + 4 epilogue warps
-  static constexpr int TMEM_COLS = 2 * BN;          // two accumulator buffers
+  static constexpr int NT = NPROD + wg::kConsumerThreads;   // producers + two consumer warpgroups
   static constexpr int MINB = 1;
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
+  static_assert(STAGES >= 2, "consumers hand a stage back only after the next stage's MMAs are issued");
+  static_assert(BN / 2 + 40 <= 65536 / NT, "accumulator does not fit the register budget: fewer producer warps");
 };
 
 struct PTile {
@@ -57,9 +57,6 @@ gemm_umma_persist_kernel(const AL al, const BL bl, const EP ep, int M, int N, in
   uint8_t* aux = smem + STAGES * SM::STAGE_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;      // [2]
-  uint64_t* acc_empty = acc_full + 2;       // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 2);
   float4* cs_scratch = reinterpret_cast<float4*>(aux + 1024);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -86,19 +83,11 @@ gemm_umma_persist_kernel(const AL al, const BL bl, const EP ep, int M, int N, in
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       umma::mbar_init(&full[s], NPROD);
-      umma::mbar_init(&empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      umma::mbar_init(&acc_full[b], 1);
-      umma::mbar_init(&acc_empty[b], 128);
+      umma::mbar_init(&empty[s], wg::kConsumerWGs);
     }
     umma::fence_barrier_init();
   }
-  if (warp == PW) umma::tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < PW) {
     // ================= PRODUCERS =================
@@ -169,15 +158,15 @@ gemm_umma_persist_kernel(const AL al, const BL bl, const EP ep, int M, int N, in
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const int off = AK ? TA::chunk_off(a_o[i], a_k[i] + 4 * j) : TA::chunk_off(a_o[i] + 4 * j, a_k[i]);
-            *reinterpret_cast<float4*>(st + off) = f[j];
+            TA::put(st, off, f[j]);
           }
         } else if constexpr (AEX) {
-          *reinterpret_cast<float4*>(st + a_o[i]) = ra[i];
+          TA::put(st, a_o[i], ra[i]);
         } else {
           float4 h, l;
           umma::split4(ra[i], h, l);
-          *reinterpret_cast<float4*>(st + a_o[i]) = h;
-          *reinterpret_cast<float4*>(st + OFF_ALO + a_o[i]) = l;
+          TA::put(st, a_o[i], h);
+          TA::put(st + OFF_ALO, a_o[i], l);
         }
       }
       const bool cs_tile = kColSum && p.mt == 0;
@@ -186,8 +175,8 @@ gemm_umma_persist_kernel(const AL al, const BL bl, const EP ep, int M, int N, in
         for (int i = 0; i < GB; ++i) {
           float4 h, l;
           umma::split4(rb[i], h, l);
-          *reinterpret_cast<float4*>(st + OFF_BHI + b_o[i]) = h;
-          *reinterpret_cast<float4*>(st + OFF_BLO + b_o[i]) = l;
+          TB::put(st + OFF_BHI, b_o[i], h);
+          TB::put(st + OFF_BLO, b_o[i], l);
           if (cs_tile) { csum[i].x += rb[i].x; csum[i].y += rb[i].y; csum[i].z += rb[i].z; csum[i].w += rb[i].w; }
         }
       }
@@ -233,81 +222,37 @@ gemm_umma_persist_kernel(const AL al, const BL bl, const EP ep, int M, int N, in
       publish(pb, q, ra1, rb1);
       advance(pb); ++q;
     }
-  } else if (warp == PW) {
-    // ================= MMA ISSUER =================
-    constexpr uint32_t idesc = umma::make_idesc(BN, !AK, !BKc);
+  } else {
+    // ================= CONSUMERS (warps PW .. PW+7: warpgroup cw = rows 64 cw .. 64 cw + 63) =================
+    const int ct = tid - NPROD, cw = ct >> 7, cwarp = (ct >> 5) & 3;
+    uint8_t* stg = aux + SM::AUX_BYTES + (ct >> 5) * wg::kEpiWarpBytes;   // dedicated staging: the stages stay live here
     PTile p;
     setup(p, blockIdx.x);
-    int q = 0, i = 0;
+    int q = 0;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     while (p.valid) {
-      const int buf = i & 1;
-      umma::mbar_wait(&acc_empty[buf], (((uint32_t)i >> 1) & 1) ^ 1);
-      umma::tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(buf * BN);
       const int ntl = p.ntl;
       for (int t = 0; t < ntl; ++t, ++q) {
         const int s = q % STAGES;
-        const uint32_t ph = (q / STAGES) & 1;
-        umma::mbar_wait(&full[s], ph);
-        umma::tc_fence_after();
-        if (umma::elect_one()) {
-          const uint32_t st = umma::smem_u32(smem + s * SM::STAGE_BYTES);
-          const uint32_t a_hi = st, a_lo = st + OFF_ALO, b_hi = st + OFF_BHI, b_lo = st + OFF_BLO;
-#pragma unroll
-          for (int j = 0; j < BK / 8; ++j) {
-            const uint32_t ao = TA::kslice_off(j), bo = TB::kslice_off(j);
-            const uint64_t dah = umma::make_desc(a_hi + ao, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-            const uint64_t dbh = umma::make_desc(b_hi + bo, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-            const uint64_t dbl = umma::make_desc(b_lo + bo, TB::LBO, TB::SBO, TB::LAYOUT_TYPE);
-            const uint32_t first = (t > 0 || j > 0) ? 1u : 0u;
-            if (!AEX) {
-              const uint64_t dal = umma::make_desc(a_lo + ao, TA::LBO, TA::SBO, TA::LAYOUT_TYPE);
-              umma::mma_tf32(tmem_d, dal, dbh, idesc, first);
-              umma::mma_tf32(tmem_d, dah, dbl, idesc, 1u);
-            } else {
-              umma::mma_tf32(tmem_d, dah, dbl, idesc, first);
-            }
-            umma::mma_tf32(tmem_d, dah, dbh, idesc, 1u);
-          }
-          umma::mma_commit(&empty[s]);
-          if (t == ntl - 1) umma::mma_commit(&acc_full[buf]);
-        }
-        __syncwarp();
+        umma::mbar_wait(&full[s], (q / STAGES) & 1);
+        const uint32_t st = umma::smem_u32(smem + s * SM::STAGE_BYTES);
+        const uint32_t a_hi = st + cw * 64 * 128;
+        wg::fence_operand(acc);
+        wg::fence();
+        tf32_stage_mmas<BN, AEX, BK, TA, TB>(acc, a_hi, a_hi + OFF_ALO, st + OFF_BHI, st + OFF_BLO, t == 0);
+        wg::commit();
+        wg::wait<1>();                                 // the MMAs of the previous stage are complete: hand it back
+        wg::fence_operand(acc);
+        if (t > 0 && (ct & 127) == 0) umma::mbar_arrive(&empty[(q - 1) % STAGES]);
       }
+      wg::wait<0>();
+      wg::fence_operand(acc);
+      if ((ct & 127) == 0) umma::mbar_arrive(&empty[(q - 1) % STAGES]);
+      wg_epilogue<BN>(ep, acc, stg, lane, p.z, p.m0 + cw * 64 + cwarp * 16, p.n0, M, N);
       setup(p, p.tile + gridDim.x);
-      ++i;
     }
-    umma::tc_fence_before();
-  } else {
-    // ================= EPILOGUE (warps PW+1 .. PW+4) =================
-    const int quarter = warp & 3;            // TMEM lanes 32*quarter .. +31
-    uint8_t* stg = aux + SM::AUX_BYTES + quarter * kEpiStageBytes;   // dedicated staging: the stages stay live here
-    PTile p;
-    setup(p, blockIdx.x);
-    int i = 0;
-    while (p.valid) {
-      const int buf = i & 1;
-      umma::mbar_wait(&acc_full[buf], ((uint32_t)i >> 1) & 1);
-      umma::tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        umma::tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN + c0), v);
-        if (c0 + 32 >= BN) {                 // last read of this buffer: hand it back to the MMA warp
-          umma::tc_fence_before();
-          umma::mbar_arrive(&acc_empty[buf]);
-        }
-        epilogue_store_32x32(ep, stg, lane, p.z, p.m0 + quarter * 32, p.n0 + c0, M, N, v);
-      }
-      setup(p, p.tile + gridDim.x);
-      ++i;
-    }
-    umma::tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == PW) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -316,7 +261,7 @@ inline int device_sm_count() {
   if (sms == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -328,7 +273,7 @@ inline int launch_gemm_umma_persist(cudaStream_t s, const AL& al, const BL& bl, 
   static bool attr_done = false;
   auto kern = gemm_umma_persist_kernel<Cfg, AL, BL, EP>;
   if (!attr_done) {
-    DRL_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::BYTES + 4 * kEpiStageBytes));
+    DRL_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::BYTES + 8 * wg::kEpiWarpBytes));
     attr_done = true;
   }
   if ((AL::kContigK || BL::kContigK) && (K % 4 != 0 || kchunk % 4 != 0)) {
@@ -340,7 +285,7 @@ inline int launch_gemm_umma_persist(cudaStream_t s, const AL& al, const BL& bl, 
   const long long total = (long long)mtiles * ntn * zcount;
   if (total > 0x7fffffffLL) { set_error("gemm_umma_persist: too many tiles"); return DRL_ERR_INVALID; }
   const int grid = (int)std::min<long long>(total, device_sm_count());
-  DRL_CUDA_CHECK((launch_k(kern, grid, Cfg::NT, SM::BYTES + 4 * kEpiStageBytes, s, al, bl, ep, M, N, K, kchunk, kstep,
+  DRL_CUDA_CHECK((launch_k(kern, grid, Cfg::NT, SM::BYTES + 8 * wg::kEpiWarpBytes, s, al, bl, ep, M, N, K, kchunk, kstep,
                            mtiles, ntn, (int)total)));
   return DRL_OK;
 }

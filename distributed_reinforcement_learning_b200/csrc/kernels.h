@@ -89,7 +89,7 @@ struct VtraceOut {       // parity taps, batch-major [B, T-2]
 
 constexpr int kLstmSplits = 8;   // slabs allocated for the LSTM split-K partial sums (4 or 7 are used)
 
-// math_mode 0 in drl_learner_config resolves to this (1 = FP32 FFMA, 2 = tcgen05 3xTF32)
+// math_mode 0 in drl_learner_config resolves to this (1 = FP32 FFMA, 2 = wgmma 3xTF32)
 #ifndef DRL_DEFAULT_PDL_LEVEL
 #define DRL_DEFAULT_PDL_LEVEL 0   // programmatic dependent launch (common.cuh); see DESIGN.md for the measurements
 #endif
@@ -97,7 +97,7 @@ constexpr int kLstmSplits = 8;   // slabs allocated for the LSTM split-K partial
 #define DRL_DEFAULT_MATH_MODE 2          // Ape-X / A3C / R2D2 handles
 #endif
 #ifndef DRL_DEFAULT_MATH_MODE_IMPALA
-#define DRL_DEFAULT_MATH_MODE_IMPALA 5   // IMPALA handle: tcgen05 kind::f16 with 16-bit split operands (gemm_umma16.cuh)
+#define DRL_DEFAULT_MATH_MODE_IMPALA 5   // IMPALA handle: wgmma with 16-bit split operands (gemm_umma16.cuh)
 #endif
 
 // Per-kernel device timing (learner.cu): when a profile run is active, prof_mark records a CUDA event
@@ -133,7 +133,7 @@ struct Streams {
   cudaEvent_t ev_lstm_grads = nullptr;   // backward: recorded on the side stream once the head and LSTM weight gradients
                                          // are in the bucket (the early part of the peer exchange waits for it)
 };
-// mode: 1 = FP32-FFMA gather-GEMM, 2 = tcgen05 3xTF32 gather-GEMM for the large contractions
+// mode: 1 = FP32-FFMA gather-GEMM, 2 = wgmma 3xTF32 gather-GEMM for the large contractions
 int net_forward(const Streams& st, const ParamLayout& pl, const float* params, const WeightImages& wi, const Inputs& in,
                 const Acts& act, int B, int T, int mode, bool retile);
 int net_backward(const Streams& st, const ParamLayout& pl, const float* params, const WeightImages& wi, float* grads,

@@ -23,10 +23,9 @@ using Conv1A = ConvFwdA<uint8_t, 84, 84, 4, 20, 20, 8, 4, true>;
 using Conv2A = ConvFwdA<float, 20, 20, 32, 9, 9, 4, 2, false>;
 using Conv3A = ConvFwdA<float, 9, 9, 64, 7, 7, 3, 1, false>;
 // math mode 4: TMA-fed forward of conv2 / conv3 (gemm_tma.cuh): tiles of 1 image (81 rows) / 2 images (98 rows), 4 stages.
-// Correct and tested, but measured SLOWER than the software producers on this network (conv2 59 vs 46 us, conv3 41 vs
-// 33 us at B=32, T=20): with 32/64 input channels a K tile is one filter tap, so every activation byte is fetched
-// 4x (conv2) / 9x (conv3) from L2 for each of the two planes plus a 16 KB weight tile per tap and image -- 2.3x the
-// L2->SM bytes of the LDG path, which reads raw fp32 once per tap and splits in registers.
+// With 32/64 input channels a K tile is one filter tap, so every activation byte is fetched 4x (conv2) / 9x (conv3) from
+// L2 for each of the two planes plus a weight tile per tap and image: more L2->SM bytes than the LDG path, which reads
+// raw fp32 once per tap and splits in registers.
 using Conv2Tma = ConvTmaCfg<32, 20, 9, 4, 2, 1, 4>;
 using Conv3Tma = ConvTmaCfg<64, 9, 7, 3, 1, 2, 4>;
 using Conv1WA = ConvWgradA<uint8_t, 84, 84, 4, 20, 20, 8, 4, true>;
@@ -39,14 +38,17 @@ using Conv2DA = ConvDgradA<9, 9, 64, 2, 4, 4, 10, 10>;
 using Conv2DB = ConvDgradB<32, 64, 2, 4, 4>;
 using Conv2DE = EpConvDx<20, 20, 32, 2, 10, 10>;
 
-using U32 = UmmaCfg<32, 2, 3>;   // 24 KB / stage (A exact: conv1 only), 3 CTAs per SM
-using U64 = UmmaCfg<64, 2, 2>;   // 48 KB / stage, 2 CTAs per SM
-using U128 = UmmaCfg<128, 3, 1, 8>;   // 64 KB / stage, 1 CTA per SM, 8 producer warps
-using U256 = UmmaCfg<256, 2, 1, 8>;   // 96 KB / stage, 1 CTA per SM, 8 producer warps
-// the same with a B-loader warp, for GEMMs whose B operand is a pre-tiled weight image
-using U64L = UmmaCfg<64, 2, 2, 4, 1>;
+// Every tensor-core configuration has two consumer warpgroups (256 threads) whose wgmma accumulators hold BN / 2 fp32
+// registers per thread, next to the producer warps, in one CTA per SM: BN = 256 (128 accumulator registers) leaves
+// room for 4 producer warps and no loader warp within the 65,536 registers of an H100 SM.
+using U32 = UmmaCfg<32, 2, 1>;   // 24 KB / stage (A exact: conv1 only)
+using U64 = UmmaCfg<64, 2, 1>;   // 48 KB / stage
+using U128 = UmmaCfg<128, 3, 1, 8>;   // 64 KB / stage, 8 producer warps
+using U256 = UmmaCfg<256, 2, 1, 4>;   // 96 KB / stage, 4 producer warps
+// the same for GEMMs whose B operand is a pre-tiled weight image (B-loader warp where the registers allow it)
+using U64L = UmmaCfg<64, 2, 1, 4, 1>;
 using U128L = UmmaCfg<128, 3, 1, 8, 1>;
-using U256L = UmmaCfg<256, 2, 1, 8, 1>;
+using U256L = U256;                    // (no loader warp: the same configuration as U256)
 
 // math mode 5: 16-bit split operands (gemm_umma16.cuh).  One format per GEMM (f16 x bf16 traps).  bf16 keeps fp32's
 // exponent range (gradients span many decades); fp16 has three more mantissa bits but underflows gradually below ~1e-4
@@ -54,32 +56,30 @@ using U256L = UmmaCfg<256, 2, 1, 8, 1>;
 // an O(0.1) weight.
 using Fmt16 = umma16::BF16;     // every GEMM whose operands are fp32 activations / gradients / weights
 using FmtC1 = umma16::F16;      // conv1: uint8 frames (exact) x weights
-using X32L = Umma16Cfg<32, 4, 2, 4, 1, FmtC1, FmtC1>;        // conv1 fwd: whole K = 256 resident
-using X64L = Umma16Cfg<64, 2, 2, 4, 1, Fmt16, Fmt16>;        // conv2 / conv3 fwd: 48 KB per K = 64 stage, 2 CTAs per SM
-using X64L8x2 = Umma16Cfg<64, 2, 2, 8, 1, Fmt16, Fmt16>;     // conv2 / conv3 fwd (default): two CTAs per SM x 8 producer warps = twice the loads
-                                                             // in flight of X64L (conv2_fwd 41 -> 33 us: the gathers are latency-bound); DRL_B200_C2F=0: X64L
-using X64W8x2 = Umma16Cfg<64, 2, 2, 8, 0, Fmt16, Fmt16>;     // conv2 / conv3 weight gradients (default; 39 -> 33, 30 -> 27 us); DRL_B200_CW8=0: X64W
-using X64W = Umma16Cfg<64, 2, 2, 4, 0, Fmt16, Fmt16>;        // conv2 / conv3 weight gradients (both operands gathered)
+using X32L = Umma16Cfg<32, 4, 1, 4, 1, FmtC1, FmtC1>;        // conv1 fwd: whole K = 256 resident
+using X64L = Umma16Cfg<64, 2, 1, 4, 1, Fmt16, Fmt16>;        // conv2 / conv3 fwd: 48 KB per K = 64 stage
+using X64L8x2 = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16>;     // conv2 / conv3 fwd (default): 8 producer warps = twice the loads in flight of
+                                                             // X64L (the gathers are latency-bound); DRL_B200_C2F=0: X64L
+using X64W8x2 = Umma16Cfg<64, 2, 1, 8, 0, Fmt16, Fmt16>;     // conv2 / conv3 weight gradients (default); DRL_B200_CW8=0: X64W
+using X64W = Umma16Cfg<64, 2, 1, 4, 0, Fmt16, Fmt16>;        // conv2 / conv3 weight gradients (both operands gathered)
 using XH = Umma16Cfg<64, 4, 1, 8, 0, Fmt16, Fmt16>;          // head layers (K = 256 = all four stages in flight), DRL_B200_HEADS_TC=1
 // bulk-fed LSTM weight gradient (gemm_bulk16.cuh): both operands are pre-tiled images, no producer warps
-using BK256 = Bulk16Cfg<256, 2, 8>;    // 96 KB per stage (A 32 KB + B 64 KB), 2 stages
-using X256L = Umma16Cfg<256, 2, 1, 8, 1, Fmt16, Fmt16>;      // lstm fwd: 96 KB per stage
-using X256W = Umma16Cfg<256, 2, 1, 8, 0, Fmt16, Fmt16>;      // lstm weight gradient
+using BK256 = Bulk16Cfg<256, 2>;       // 96 KB per stage (A 32 KB + B 64 KB), 2 stages
+using X256L = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm fwd: 96 KB per stage
+using X256W = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm weight gradient
 using X128D = Umma16Cfg<128, 3, 1, 8, 1, Fmt16, Fmt16>;      // lstm data gradient: 64 KB per stage
-using X256D = Umma16Cfg<256, 1, 2, 8, 1, Fmt16, Fmt16>;      // dCol GEMMs (K = 64 = ONE stage of 96 KB): two CTAs per SM, so that
-                                                             // the 128 KB epilogue of one overlaps the load + MMAs of the other
-using X64G = Umma16Cfg<64, 2, 2, 4, 0, Fmt16, Fmt16>;        // conv3 data gradient, gather form (K = 9 taps x 64)
-using X32G = Umma16Cfg<32, 3, 2, 4, 0, Fmt16, Fmt16>;        // conv2 data gradient, gather form (4 parity classes, K = 4 taps x 64)
+using X256D = Umma16Cfg<256, 1, 1, 4, 0, Fmt16, Fmt16>;      // dCol GEMMs (K = 64 = ONE stage of 96 KB)
+using X64G = Umma16Cfg<64, 2, 1, 4, 0, Fmt16, Fmt16>;        // conv3 data gradient, gather form (K = 9 taps x 64)
+using X32G = Umma16Cfg<32, 3, 1, 4, 0, Fmt16, Fmt16>;        // conv2 data gradient, gather form (4 parity classes, K = 4 taps x 64)
 
 // math mode 3 (experimental): the persistent, fully warp-specialised variant of each tensor-core configuration
 template <class U> struct PersistOf;
 template <> struct PersistOf<U32> { using type = UmmaPCfg<32, 5, 8>; };
 template <> struct PersistOf<U64> { using type = UmmaPCfg<64, 4, 8>; };
 template <> struct PersistOf<U128> { using type = UmmaPCfg<128, 3, 8>; };
-template <> struct PersistOf<U256> { using type = UmmaPCfg<256, 2, 8>; };
+template <> struct PersistOf<U256> { using type = UmmaPCfg<256, 2, 4>; };
 template <> struct PersistOf<U64L> { using type = UmmaPCfg<64, 4, 8>; };
 template <> struct PersistOf<U128L> { using type = UmmaPCfg<128, 3, 8>; };
-template <> struct PersistOf<U256L> { using type = UmmaPCfg<256, 2, 8>; };
 
 
 // name the launch for the per-kernel profile, run it on the selected core, count it
@@ -138,10 +138,10 @@ template <> struct PersistOf<U256L> { using type = UmmaPCfg<256, 2, 8>; };
     n += (cnt);                                              \
   } while (0)
 
-// split-K plan: about `waves` waves of CTAs on 148 SMs
+// split-K plan: about `waves` waves of CTAs on the 132 SMs of an H100
 struct SplitPlan { int splits, kchunk; };
 static SplitPlan plan_split(int K, int tiles_mn, int bk, int waves) {
-  int target = (waves * 148 + tiles_mn - 1) / tiles_mn;
+  int target = (waves * 132 + tiles_mn - 1) / tiles_mn;
   if (target < 1) target = 1;
   int kchunk = (K + target - 1) / target;
   kchunk = (kchunk + bk - 1) / bk * bk;

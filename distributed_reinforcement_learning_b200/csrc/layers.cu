@@ -2,7 +2,7 @@
 // over M = B*T independent rows (the LSTM is a single step from fed state, :18-25 / :73-82, so
 // time is embarrassingly parallel; only T distinct forwards exist, SURVEY.md section 0.3).
 // Every dense contraction is one launch of a gather-GEMM: the FP32-FFMA core (gemm_simt.cuh, math
-// mode 1) or the tcgen05 3xTF32 tensor-core core (gemm_umma.cuh, math mode 2) -- same loaders and
+// mode 1) or the wgmma 3xTF32 tensor-core core (gemm_umma.cuh, math mode 2) -- same loaders and
 // epilogues.  The small head layers (M x 256 x 256) always use the FFMA core.
 #include <stdlib.h>
 
@@ -106,7 +106,7 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
   // for them behind conv1), the LSTM / dgrad ones behind the embedding table (joined before lstm_fwd)
   const bool m16 = mode == 5;
   bool c3_event = false;   // conv3's weight image has its own event (math mode 5)
-  static const bool heads_tc = !(getenv("DRL_B200_HEADS_TC") && atoi(getenv("DRL_B200_HEADS_TC")) == 0);   // head layers on tcgen05 (0: FFMA)
+  static const bool heads_tc = !(getenv("DRL_B200_HEADS_TC") && atoi(getenv("DRL_B200_HEADS_TC")) == 0);   // head layers on tensor cores (0: FFMA)
   // math mode 5: conv1 is the frame-resident TMA kernel (conv1_tma.cuh), which builds its 32 KB weight image itself;
   // DRL_B200_CONV1_GATHER=1 keeps the generic gather-GEMM, DRL_B200_C1_WIMG=1 the pre-tiled image (one more kernel in
   // front of the step's first kernel)
@@ -218,7 +218,7 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     LstmA al{act.a3, act.table, in.pa, in.h0, map};
     PlainB bl{P + pl.lstm_w, Geo::G4, 0};
     EpRaw<false> ep{act.zpart, Geo::G4, (size_t)M * Geo::G4, 1.0f, 0, Geo::G4};
-    // FFMA: 4 splits of 57 x 16.  tcgen05: 128 x 256 tiles -> 5 x 4 output tiles x 7 splits of 17 x 32 = 140 CTAs (one wave)
+    // FFMA: 4 splits of 57 x 16.  Tensor cores: 128 x 256 tiles -> 5 x 4 output tiles x 7 splits of 17 x 32 (B = 32, T = 20)
     nsplit = (mode >= 2) ? 7 : 4;
     const int kchunk = m16 ? 576 : (mode >= 2) ? 544 : Geo::XK / 4;      // 16-bit: 9 K tiles of 64 per split
     PretiledB<PlainB> blp{wi.img[3], m16 ? Geo::XK / 64 : Geo::XK / 32};
@@ -265,7 +265,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
   PdlRegionOff pdl_region;   // DRL_B200_PDL=2: no early launches while the side stream competes for the same SMs
   if (mode == 4) mode = 2;
   const bool m16 = mode == 5;
-  static const bool heads_tc = !(getenv("DRL_B200_HEADS_TC") && atoi(getenv("DRL_B200_HEADS_TC")) == 0);   // head layers on tcgen05 (0: FFMA)
+  static const bool heads_tc = !(getenv("DRL_B200_HEADS_TC") && atoi(getenv("DRL_B200_HEADS_TC")) == 0);   // head layers on tensor cores (0: FFMA)
   cudaStream_t s = st.main;
   const cudaStream_t side = st.par ? st.side : st.main;
   const int M = B * T;
@@ -423,8 +423,8 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     PlainA al{bw.da3, 64, 0};
     PlainBT bl{P + pl.conv3_w, 64, 0};               // B(k = co, n = (ky,kx,ci)) = W[n*64 + co]
     EpRaw<false> ep{bw.dcol, 576, 0, 1.0f, 0, 576};
-    // K = 64 (two K tiles) and 128 x 256 outputs per tile: epilogue-dominated, so the persistent kernel with
-    // dedicated epilogue warps wins here (measured 0.067 vs 0.073 ms); elsewhere two CTAs per SM win.
+    // K = 64 (two K tiles) and 128 x 256 outputs per tile: epilogue-dominated, so the persistent kernel whose
+    // dedicated epilogue warps wins here while the producers gather the next tile.
     prof_mark(s, "conv3_dgrad");
     PretiledB<PlainBT> blp{wi.img[5], m16 ? 1 : 2};
     if (m16) DRL_TRY((launch_gemm_umma16<X256D>(s, al, blp, ep, Mb * 49, 576, 64, 1, 64, 0)));

@@ -157,7 +157,7 @@ struct drl_learner {
   std::vector<cudaGraphExec_t> graph_step;   // forward+backward+[exchange]+apply in one graph
   // gradient exchange over NVLink peer memory (peer.cu); off until drl_learner_peer_import
   bool peer_on = false;
-  int peer_nblk = 148 * 4;
+  int peer_nblk = 132 * 4;
   uint8_t* comm = nullptr;                   // [reduced | partials | flags | epochs | err], own cudaMalloc (IPC-exported)
   size_t comm_bytes = 0, off_partials = 0, off_flags = 0, off_epoch = 0, off_err = 0;
   PeerPlan plan{};                           // peer table + the update's OptState on the reduced buffer
@@ -284,7 +284,7 @@ int enqueue_apply(drl_learner* h, int out_row, bool local_only = false, bool ear
       } else {
         DRL_TRY(peer_exchange(h->compute, h->plan, 0, split4, end4, false, h->peer_early_ctas));
       }
-      DRL_TRY(peer_exchange(h->compute, h->plan, 1, 0, split4, true, 148));
+      DRL_TRY(peer_exchange(h->compute, h->plan, 1, 0, split4, true, 132));
     }
     prof_mark(h->compute, "optimizer(rmsprop)");
     NvtxRange r("drl:update");
@@ -404,7 +404,7 @@ int drl_debug_trace(void* dev_buf) {
   DRL_CUDA_CHECK(cudaDeviceSynchronize());
   return DRL_OK;
 }
-const char* drl_version(void) { return "drl_b200 0.4 (sm_100a; tcgen05 kind::f16 split-16 / 3xTF32 gather-GEMMs, FP32-FFMA core, NVLink peer exchange; IMPALA, Ape-X, R2D2, A3C learners)"; }
+const char* drl_version(void) { return "drl_b200 0.5 (sm_90a; wgmma split-16 / 3xTF32 gather-GEMMs, FP32-FFMA core, NVLink peer exchange; IMPALA, Ape-X, R2D2, A3C learners)"; }
 
 int drl_device_count(void) {
   int n = 0;
@@ -429,8 +429,8 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     return DRL_ERR_INVALID;
   }
   if (cfg->math_mode < 0 || cfg->math_mode > 5) {
-    set_error("math_mode must be 0 (default), 1 (FP32 FFMA), 2 (tcgen05 3xTF32), 3 (same, persistent kernels), "
-              "4 (same as 2 with TMA-fed conv2/conv3 forward) or 5 (tcgen05 kind::f16 with 16-bit split operands)");
+    set_error("math_mode must be 0 (default), 1 (FP32 FFMA), 2 (wgmma 3xTF32), 3 (same, persistent kernels), "
+              "4 (same as 2 with TMA-fed conv2/conv3 forward) or 5 (wgmma with 16-bit split operands)");
     return DRL_ERR_INVALID;
   }
   if (drl_device_count() <= cfg->device) { set_error("CUDA device %d not available (no CPU fallback)", cfg->device); return DRL_ERR_CUDA; }
@@ -538,7 +538,7 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     memset(h->h_out, 0, out_rows * 8 * sizeof(float));
     OptState& o = h->opt;
     o.params = h->params; o.ms = h->ms; o.grads = h->bucket; o.n = (int64_t)NP;
-    o.nblk = 148 * 4;
+    o.nblk = 132 * 4;
     o.npart = o.nblk;
     o.wait_flags = nullptr; o.wait_epoch = nullptr; o.wait_world = 0; o.wait_err = nullptr; o.wait_parts = 0;
     o.wait_err_host = nullptr; o.wait_timeout_ns = 0;

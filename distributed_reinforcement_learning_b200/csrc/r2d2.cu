@@ -123,7 +123,7 @@ static SplitPlan plan_r2_x(int M, int mode) {
   return mode >= 2 ? plan_split(kR2Cat, cdiv(M, 128), 32, 1) : plan_split(kR2Cat, cdiv(M, CfgMid::BM) * (kR2G / CfgMid::BN), 16, 1);
 }
 // conv1 weight gradient with single-channel frames is a [64 x 32] output with K = M*400: half of a 128-row MMA tile
-// would be padding and the producers, not the tensor pipe, set the pace (measured 0.20 ms at M = 1280 on the tcgen05
+// would be padding and the producers, not the tensor pipe, set the pace on the 128-row tensor-core
 // core).  A 64 x 32 FFMA tile with the reduction split over ~4 CTAs per SM fits the shape in both math modes.
 using CfgWgC1 = TileCfg<64, 32, 16, 4, 4>;
 static SplitPlan plan_r2_conv1_wgrad(int M, int) { return plan_split(M * 400, 1, 16, 4); }
@@ -924,7 +924,7 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
     set_error("need seq_len >= 2 and 0 <= burn_in <= seq_len - 2 (got seq_len %d, burn_in %d)", cfg->seq_len, cfg->burn_in);
     return DRL_ERR_INVALID;
   }
-  if (cfg->math_mode < 0 || cfg->math_mode > 2) { set_error("math_mode must be 0 (default), 1 (FP32 FFMA) or 2 (tcgen05 3xTF32)"); return DRL_ERR_INVALID; }
+  if (cfg->math_mode < 0 || cfg->math_mode > 2) { set_error("math_mode must be 0 (default), 1 (FP32 FFMA) or 2 (wgmma 3xTF32)"); return DRL_ERR_INVALID; }
   if (drl_device_count() <= cfg->device) { set_error("CUDA device %d not available (no CPU fallback)", cfg->device); return DRL_ERR_CUDA; }
   drl_r2d2* h = new drl_r2d2();
   h->cfg = *cfg;
@@ -1007,7 +1007,7 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
     for (size_t i = 0; i < M; ++i) h->h_ones[i] = 1.0f;
     AdamState& o = h->opt;
     o.params = h->params; o.m = h->adam_m; o.v = h->adam_v; o.grads = h->grads; o.n = (int64_t)NP;
-    o.nblk = 148 * 4;
+    o.nblk = 132 * 4;
     DRL_TRY(dev_alloc(h, &o.norm_partials, o.nblk));
     o.step = h->d_step; o.lr_cur = h->d_lr; o.alpha = h->d_alpha; o.b1p = h->d_b1p; o.b2p = h->d_b2p;
     o.out = h->d_out; o.loss = h->loss;

@@ -361,7 +361,7 @@ static int launch_fs(cudaStream_t s, const float* mu, const float* pi, const int
   // learner-shaped fast path: persistent warps with a cp.async pipeline
   const size_t smem_pipe = (size_t)kFsWarps * 4 * T * A * sizeof(float);
   if (T <= 32 && ((T * A) & 3) == 0 && ((((size_t)mu | (size_t)pi)) & 15) == 0 && smem_pipe <= 48 * 1024) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(12, (200 * 1024) / std::max<size_t>(smem_pipe, 1)));

@@ -1,4 +1,4 @@
-"""B200-native stand-ins for ``distributed_queue/buffer_queue.py``: ``FIFOQueue`` (reference :418-512, the IMPALA
+"""H100-native stand-ins for ``distributed_queue/buffer_queue.py``: ``FIFOQueue`` (reference :418-512, the IMPALA
 trajectory queue) and ``SumTree`` / ``Memory`` (reference :326-416, the Ape-X prioritized replay memory).
 
 The reference keeps a ``tf.FIFOQueue`` of 9-field trajectories on the learner's CPU and dequeues a

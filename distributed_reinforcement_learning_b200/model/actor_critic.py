@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``model/actor_critic.py`` (the A3C network): parameter inventory of scope
+"""H100-native stand-in for the reference's ``model/actor_critic.py`` (the A3C network): parameter inventory of scope
 'a3c' in TF layouts / TF variable order -- conv2d x3, dense x2 (action embedding), dense x3 (actor 3392 -> 256 -> 256 -> A,
 softmax), dense x3 (critic 3392 -> 256 -> 256 -> 1).  The same body as ``model/apex_value.py`` with the two streams named
 actor / critic; the graph (``network`` :28-39, ``build_network`` :41-56) is evaluated by ``drl_a3c_*`` through

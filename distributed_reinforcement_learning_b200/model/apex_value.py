@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``model/apex_value.py`` (the Ape-X dueling network).
+"""H100-native stand-in for the reference's ``model/apex_value.py`` (the Ape-X dueling network).
 
 Reference graph (model/apex_value.py:4-41): conv 8x8s4/32 -> 4x4s2/64 -> 3x3s1/64 -> flatten(3136) ||
 one_hot(previous_action) -> dense256 -> dense256; concat (3392) -> value stream [256, 256, A] and a SEPARATE

@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``model/impala_actor_critic.py``.
+"""H100-native stand-in for the reference's ``model/impala_actor_critic.py``.
 
 The reference builds a TF1 graph: conv 8x8s4/32 -> 4x4s2/64 -> 3x3s1/64 -> flatten(3136) ||
 one_hot(prev_action) -> dense256 -> dense256 || one LSTMCell(256) step from FED (h, c) ->

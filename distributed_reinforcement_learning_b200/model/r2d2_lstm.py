@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``model/r2d2_lstm.py``: parameter inventory / initialisation of one scope
+"""H100-native stand-in for the reference's ``model/r2d2_lstm.py``: parameter inventory / initialisation of one scope
 ('main' or 'target') in TF layouts and TF variable-creation order (conv2d x3, dense x2 (action embedding),
 rnn/lstm_cell kernel [3136 + 256 + L, 4L] gate order i,j,f,o + bias, dense 128, dense A (value), dense 1 (mean)).
 The graph itself (``network`` :28-53, ``build_network`` :55-116) is evaluated by ``drl_r2d2_*`` through

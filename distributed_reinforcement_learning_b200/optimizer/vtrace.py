@@ -1,4 +1,4 @@
-"""B200-native stand-in for the reference's ``optimizer/vtrace.py`` (same names, argument order,
+"""H100-native stand-in for the reference's ``optimizer/vtrace.py`` (same names, argument order,
 layouts and error behaviour; NumPy arrays in and out, CUDA kernels underneath via the C-ABI).
 
   split_data                          optimizer/vtrace.py:3-14   (views, no compute)

@@ -1,5 +1,5 @@
 /*
- * drl_b200.h -- C-ABI of the B200-native learner hot paths: IMPALA (the headline path), then the Ape-X DQN, R2D2 and
+ * drl_b200.h -- C-ABI of the H100-native learner hot paths: IMPALA (the headline path), then the Ape-X DQN, R2D2 and
  * A3C learner steps and the prioritized-replay index (SURVEY.md section 8(f)).
  *
  * The reference (chagmgang/distributed_reinforcement_learning @ 1890ce4) has no FFI: its hot
@@ -36,7 +36,7 @@ extern "C" {
 
 /* Last error text of the calling thread ("" if none). */
 const char* drl_last_error(void);
-/* Library version string, e.g. "drl_b200 0.1 sm_100a". */
+/* Library version string, e.g. "drl_b200 0.5 (sm_90a; ...)". */
 const char* drl_version(void);
 /* Number of CUDA devices visible (0 when there is none / no driver). */
 int drl_device_count(void);
@@ -64,10 +64,9 @@ typedef struct drl_learner_config {
   int32_t device;             /* CUDA device ordinal                                            */
   int32_t num_slots;          /* device staging slots for stream-overlapped H2D (>=1, default 2) */
   int32_t use_cuda_graph;     /* 1: capture forward+backward(+apply) into CUDA graphs           */
-  int32_t math_mode;          /* 0 = default (5); 1 = FP32 FFMA; 2 = tcgen05 3xTF32; 3 = same, persistent kernels;
-                                 4 = as 2 with TMA-fed conv2/conv3 forward (experimental); 5 = tcgen05 kind::f16 on
-                                 bf16 hi/lo split operands (three products, fp32-grade) + TMA-fed conv1 kernels +
-                                 bulk-fed LSTM weight gradient */
+  int32_t math_mode;          /* 0 = default (5); 1 = FP32 FFMA; 2 = wgmma 3xTF32; 3 = same, persistent kernels;
+                                 4 = rejected (former TMA-fed conv experiment); 5 = wgmma on bf16 hi/lo split
+                                 operands (three products, fp32-grade) + bulk-fed LSTM weight gradient */
 } drl_learner_config;
 
 /* Results of one step: the 4 floats Agent.train returns (agent/impala.py:144-148) + grad norm. */
@@ -173,7 +172,7 @@ int drl_learner_act(drl_learner* h, int32_t n, const uint8_t* state, const int32
  * '\n'-joined list (names_len bytes available), ms[i] the time from launch i to launch i+1. */
 int drl_learner_profile_step(drl_learner* h, int32_t slot, char* names, int64_t names_len, float* ms,
                              int32_t max_kernels, int32_t* count);
-/* Test aid: one plain GEMM C[M,N] = A*B on a chosen contraction core (1 = FP32 FFMA, 2 = tcgen05 3xTF32) and
+/* Test aid: one plain GEMM C[M,N] = A*B on a chosen contraction core (1 = FP32 FFMA, 2 = wgmma 3xTF32, 5-8 = wgmma 16-bit split) and
  * operand-major combination, to validate shared-memory layouts / UMMA descriptors in isolation.
  * a_kmajor: A is [M,K] row-major (1) or [K,M] row-major (0); b_kmajor: B is [N,K] (1) or [K,N] (0).
  * C: `splits` slabs of [(M+1), N] floats (split-K partials; row M = column sums of B for N-major B). */
@@ -290,7 +289,7 @@ typedef struct drl_apex_config {
   int32_t device;             /* CUDA device ordinal                                                    */
   int32_t num_slots;          /* device staging slots for stream-overlapped H2D (>=1, default 2)        */
   int32_t use_cuda_graph;     /* 1: capture the whole step into one CUDA graph per slot                 */
-  int32_t math_mode;          /* 0 = default (2); 1 = FP32 FFMA; 2 = tcgen05 3xTF32 convolutions        */
+  int32_t math_mode;          /* 0 = default (2); 1 = FP32 FFMA; 2 = wgmma 3xTF32 convolutions          */
 } drl_apex_config;
 
 typedef struct drl_apex_out {
@@ -407,7 +406,7 @@ typedef struct drl_r2d2_config {
   int32_t device;
   int32_t num_slots;
   int32_t use_cuda_graph;
-  int32_t math_mode;          /* 0 = default (2); 1 = FP32 FFMA; 2 = tcgen05 3xTF32 for the large contractions */
+  int32_t math_mode;          /* 0 = default (2); 1 = FP32 FFMA; 2 = wgmma 3xTF32 for the large contractions */
 } drl_r2d2_config;
 
 typedef struct drl_r2d2_out {

@@ -1,6 +1,6 @@
 """-m gpu: the reference-facing Python surface.  The learner branch of train_impala.py:89-113 -- queue size
 gate, sample_batch, eight np.stack calls, learner.train, five scalars -- is replayed here against the
-B200-native Agent / FIFOQueue with the reference's config.json values, and its results are checked against
+H100-native Agent / FIFOQueue with the reference's config.json values, and its results are checked against
 the CPU oracle stepping on the same trajectories."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""-m gpu: the tcgen05 3xTF32 contraction core (csrc/gemm_umma.cuh).
+"""-m gpu: the wgmma 3xTF32 contraction core (csrc/gemm_umma.cuh).
 (1) drl_debug_gemm: one plain GEMM per operand-major combination (K-major / MN-major A and B -- the
     128-byte-swizzled shared-memory layouts and UMMA descriptors), tile width and split-K setting, against
     NumPy float64; the FP32-FFMA core runs the same cases as a cross-check.
@@ -89,8 +89,8 @@ def test_two_steps_cuda_graph_tensor_core_path(native):
 @pytest.mark.parametrize("B,T,A,kw", [(4, 20, 18, {}), (32, 20, 18, {"layers": False}), (5, 32, 18, {}), (1, 3, 2, {}),
                                       (4, 20, 18, {"layers": False, "steps": 2, "use_cuda_graph": True})])
 def test_step_persistent_tensor_core_kernels(native, B, T, A, kw):
-    """math_mode=3: the persistent, fully warp-specialised tcgen05 kernels (dedicated epilogue warps, two TMEM
-    accumulator buffers) reach the same 1e-4 bar."""
+    """math_mode=3: the persistent, warp-specialised wgmma kernels (the epilogue of one tile overlaps the
+    gathers of the next) reach the same 1e-4 bar."""
     _assert_all(parity.compare_step(B, T=T, A=A, math_mode=3, **kw))
 
 

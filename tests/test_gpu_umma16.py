@@ -1,4 +1,4 @@
-"""-m gpu: the tcgen05 kind::f16 contraction core with 16-bit split operands (csrc/gemm_umma16.cuh, math_mode 5).
+"""-m gpu: the wgmma f16 / bf16 contraction core with 16-bit split operands (csrc/gemm_umma16.cuh, math_mode 5).
 (1) drl_debug_gemm cores 5 (bf16 split) / 6 (fp16 split) / 7, 8 (same with B from a pre-tiled K-major image fetched by
     the bulk-copy loader warp): every operand-major combination, tile width, split-K and ragged shapes against NumPy
     float64.  Expected error of hi*hi + hi*lo + lo*hi: ~2^-16 per product for bf16 (random sign: ~1e-6 .. 1e-5 of the

@@ -20,14 +20,14 @@ def test_library_exports_every_declared_symbol(native):
     missing = [n for n in declared if not hasattr(native.lib, n)]
     assert not missing, missing
     assert set(native.EXPORTS) == set(declared), set(native.EXPORTS) ^ set(declared)
-    assert b"sm_100a" in native.lib.drl_version()
+    assert b"sm_90a" in native.lib.drl_version()
 
 
-def test_built_for_sm_100a_only(native):
+def test_built_for_sm_90a_only(native):
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", native.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_compute_fails_loudly_without_a_device(native):

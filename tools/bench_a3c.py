@@ -1,5 +1,5 @@
 """A3C learner bench leg (`python bench.py --workload a3c`): transitions/s of ``a3c.Agent.train`` on one unroll of
-trajectory = 32 synthetic 84x84x4 transitions (config.json:2-41), one B200.  Same structure as tools/bench_apex.py."""
+trajectory = 32 synthetic 84x84x4 transitions (config.json:2-41), one H100.  Same structure as tools/bench_apex.py."""
 import json
 import os
 import sys

@@ -1,5 +1,5 @@
 """Ape-X learner bench leg (BASELINE.json configs[3]; `python bench.py --workload apex`): transitions/s of
-``apex.Agent.distributed_train`` on synthetic 84x84x4 minibatches, B=32 (config.json:154), one B200.
+``apex.Agent.distributed_train`` on synthetic 84x84x4 minibatches, B=32 (config.json:154), one H100.
 
   value : device-resident (two staged slots alternate, the whole step is one CUDA graph)
   e2e   : through the C-ABI with HOST buffers: every step copies that step's minibatch (2 x B frames + scalars) from

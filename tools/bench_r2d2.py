@@ -1,6 +1,6 @@
 """R2D2 learner bench leg (BASELINE.json configs[4]; `python bench.py --workload r2d2`): frames/s of
 ``r2d2.Agent.train`` on synthetic sequences -- B=16 sequences (config.json:94) of seq_len=80 with burn_in=40 (the sizes
-BASELINE.json names; the reference ships 15/7), 84x84x1 frames, LSTM 64, 4 actions, one B200.
+BASELINE.json names; the reference ships 15/7), 84x84x1 frames, LSTM 64, 4 actions, one H100.
 
   value : device-resident (two staged slots alternate, the whole step is one CUDA graph)
   e2e   : through the C-ABI with HOST buffers (per-step H2D of the sequences, host reads loss + B priorities)

@@ -3,7 +3,7 @@
 // of [A tile | B tile] into a STAGES-deep shared-memory ring with cp.async.bulk, a consumer thread "using" a stage for
 // `hold` ns before it frees it.  Variants: tiles SHARED between CTAs as in the GEMM (A tile by all CTAs of an m row, B tile
 // by all CTAs of an n column) or PRIVATE per CTA; one or two issuing lanes; chunked copies.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o bulk_gemm_feed bulk_gemm_feed.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o bulk_gemm_feed bulk_gemm_feed.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

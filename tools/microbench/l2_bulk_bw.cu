@@ -2,7 +2,7 @@
 //   mode 0: cp.async.bulk (global -> shared, mbarrier complete_tx), CHUNK bytes per copy, 2..4 stages in flight
 //   mode 1: LDG.128 by 256 threads per CTA (registers only, no shared-memory store)
 // The window (default 16 MB) is re-read many times, so after the first pass every byte comes from L2.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o l2_bulk_bw l2_bulk_bw.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o l2_bulk_bw l2_bulk_bw.cu
 // Usage: ./l2_bulk_bw [window_MB=16] [chunk_KB=32] [stages=3] [ctas_per_sm=1]
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,6 +1,6 @@
 // p2p_bw.cu -- NVLink peer-memory bandwidth seen by a kernel on GPU 0 that reads / writes GPU 1's memory with
 // 128-bit accesses (the access pattern of csrc/peer.cu), for a slice-sized (8 MB) and a large (128 MB) buffer.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o p2p_bw p2p_bw.cu     Usage: ./p2p_bw
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o p2p_bw p2p_bw.cu     Usage: ./p2p_bw
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>

@@ -4,7 +4,7 @@
 //   mode 0: 4-D box {32, W, W, 1} over dims {32, W, W, N} with strides {sx*128 B, sy*ROWPITCH, IMG} (conv gather)
 //   mode 1: 2-D box {32, W*W} over a dense [rows, 32] fp32 matrix (contiguous 128-byte rows)
 //   mode 2: cp.async.bulk of W*W*128 contiguous bytes
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tma_box_bw tma_box_bw.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tma_box_bw tma_box_bw.cu
 // Usage: ./tma_box_bw [W=9] [stride=2] [stages=4] [ctas_per_sm=1]
 #include <cuda.h>
 #include <cuda_runtime.h>

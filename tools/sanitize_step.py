@@ -1,4 +1,4 @@
-"""One tiny learner step per math mode for compute-sanitizer (memcheck / racecheck / synccheck of the mbarrier + tcgen05
+"""One tiny learner step per math mode for compute-sanitizer (memcheck / racecheck / synccheck of the mbarrier + wgmma
 pipelines), and with --peer under torchrun the 2-GPU fused exchange (flag protocol over NVLink peer memory).
 
     compute-sanitizer --tool memcheck  python tools/sanitize_step.py --modes 2 3
