@@ -109,17 +109,22 @@ struct Umma16Tile {
   __device__ static __forceinline__ int kslice_off(int j) { return KMAJOR ? j * 32 : j * 2 * SBO; }
 };
 
+// TAPSUM: every K tile of 64 starts a fresh accumulator, which is added in fp32 to a running sum in K-tile order once its
+// MMAs are complete (two register sets).  For the conv data gradients, whose K tiles are filter taps, this rounds and
+// sums exactly as a per-tap GEMM followed by a fixed-order tap sum would.
 template <int BN_, int STAGES_, int MINB_ = 1, int PW_ = 4, int LW_ = 0, class AF_ = umma16::BF16, class BF_ = umma16::BF16,
-          int PFD_ = 0>
+          int PFD_ = 0, bool TAPSUM_ = false>
 struct Umma16Cfg {
   static constexpr int PFD = PFD_;   // register prefetch ring depth in 32-wide K sub-tiles (0: 4 / 3 / 2 by operand kind)
   static constexpr int BM = 128, BN = BN_, BK = 64, SUBK = 32, STAGES = STAGES_, MINB = MINB_;
   static constexpr int PW = PW_, LW = LW_;
+  static constexpr bool TAPSUM = TAPSUM_;
   static constexpr int NPROD = PW * 32;
   static constexpr int NT = NPROD + wg::kConsumerThreads + 32 * LW;   // producers + two consumer warpgroups [+ loader]
   static_assert(PW == 4 || PW == 8, "4 or 8 producer warps");
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
-  static_assert(BN / 2 + 40 <= 65536 / (NT * MINB), "accumulator does not fit the register budget: fewer threads or CTAs");
+  static_assert((TAPSUM ? BN : BN / 2) + 40 <= 65536 / (NT * MINB),
+                "accumulator does not fit the register budget: fewer threads or CTAs");
   using AF = AF_;   // 16-bit format of the A operand (uint8 operands are always fp16: exact)
   using BF = BF_;
 };
@@ -435,8 +440,11 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
     const uint32_t a_off = AK ? (uint32_t)(cw * 64 * 128) : (uint32_t)(cw * 1024);
     const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO), db_base = umma::make_desc(0, TB::LBO, TB::SBO);
     float acc[BN / 2];
+    float tsum[Cfg::TAPSUM ? BN / 2 : 1];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < (Cfg::TAPSUM ? BN / 2 : 1); ++i) tsum[i] = 0.f;
     for (int t = 0; t < ntiles; ++t) {
       const int s = t % STAGES;
       umma::mbar_wait(&full[s], (t / STAGES) & 1);
@@ -450,7 +458,7 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
 #pragma unroll
       for (int j = 0; j < BK / 16; ++j) {
         const uint64_t ao = (uint64_t)(TA::kslice_off(j) >> 4), bo = (uint64_t)(TB::kslice_off(j) >> 4);
-        const uint32_t first = (t > 0 || j > 0) ? 1u : 0u;
+        const uint32_t first = ((t > 0 && !Cfg::TAPSUM) || j > 0) ? 1u : 0u;
         if (!AEX) {                                                    // small terms first
           umma16::mma16<BN, AF, TAm, TBm>(acc, a_lo + ao, b_hi + bo, first);
           umma16::mma16<BN, AF, TAm, TBm>(acc, a_hi + ao, b_lo + bo, 1u);
@@ -460,9 +468,17 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
         umma16::mma16<BN, AF, TAm, TBm>(acc, a_hi + ao, b_hi + bo, 1u);
       }
       wg::commit();
-      wg::wait<1>();                                   // the MMAs of stage t-1 are complete: hand it back
-      wg::fence_operand(acc);
-      if (t > 0 && (ct & 127) == 0) umma::mbar_arrive(&empty[(t - 1) % STAGES]);
+      if constexpr (Cfg::TAPSUM) {
+        wg::wait<0>();                                 // this tile's partial sum is complete: add it, hand the stage back
+        wg::fence_operand(acc);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) tsum[i] += acc[i];
+        if ((ct & 127) == 0) umma::mbar_arrive(&empty[s]);
+      } else {
+        wg::wait<1>();                                 // the MMAs of stage t-1 are complete: hand it back
+        wg::fence_operand(acc);
+        if (t > 0 && (ct & 127) == 0) umma::mbar_arrive(&empty[(t - 1) % STAGES]);
+      }
       if (ct == 0) TR(4000 + t);
     }
     wg::wait<0>();
@@ -471,7 +487,8 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
     wg::consumer_sync();                               // both warpgroups are done with the stages: reuse them
     if (ct == 0) TR(6000);
     uint8_t* stg = smem + (ct >> 5) * wg::kEpiWarpBytes;
-    wg_epilogue<BN>(ep, acc, stg, lane, z, m0 + cw * 64 + cwarp * 16, n0, M, N);
+    if constexpr (Cfg::TAPSUM) wg_epilogue<BN>(ep, tsum, stg, lane, z, m0 + cw * 64 + cwarp * 16, n0, M, N);
+    else wg_epilogue<BN>(ep, acc, stg, lane, z, m0 + cw * 64 + cwarp * 16, n0, M, N);
     if (ct == 0) TR(6001);
   }
 }

@@ -74,7 +74,8 @@ struct Bwd {             // backward workspace, Mb = B*(T-2) rows
   float* da1;            // [Mb,20,20,32]
   float* wg_part;        // split-K partial slabs for the conv3/conv2 weight gradients (side stream) + emb scratch
   float* wg_part2;       // split-K partial slabs for the conv1 weight gradient (main stream)
-  float* dcol;           // [Mb*81, 512] (conv2) / [Mb*49, 576] (conv3): per-output-pixel tap gradients before col2im
+  float* dcol = nullptr; // [Mb*81, 512] (conv2) / [Mb*49, 576] (conv3): per-output-pixel tap gradients before col2im
+                         // (math modes 2-4; math mode 5 computes the conv data gradients without it)
   size_t wg_part_floats;
   float* emb_scratch = nullptr;   // own scratch of emb_backward (16 * 32 * 256 floats): lets it run on the second side lane
                                   // beside the conv weight gradients; nullptr: it borrows wg_part on `side`

@@ -37,6 +37,8 @@ using Conv3DE = EpConvDx<9, 9, 64, 1, 9, 9>;
 using Conv2DA = ConvDgradA<9, 9, 64, 2, 4, 4, 10, 10>;
 using Conv2DB = ConvDgradB<32, 64, 2, 4, 4>;
 using Conv2DE = EpConvDx<20, 20, 32, 2, 10, 10>;
+using Conv2DBm = ConvDgradBMerged<32, 64, 2, 4, 4>;     // math mode 5: the four parity classes as one GEMM, N = 128
+using Conv2DEm = EpConvDxMerged<20, 20, 32, 2, 10, 10>;
 
 // Every tensor-core configuration has two consumer warpgroups (256 threads) whose wgmma accumulators hold BN / 2 fp32
 // registers per thread, next to the producer warps, in one CTA per SM: BN = 256 (128 accumulator registers) leaves
@@ -68,9 +70,11 @@ using BK256 = Bulk16Cfg<256, 2>;       // 96 KB per stage (A 32 KB + B 64 KB), 2
 using X256L = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm fwd: 96 KB per stage
 using X256W = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm weight gradient
 using X128D = Umma16Cfg<128, 3, 1, 8, 1, Fmt16, Fmt16>;      // lstm data gradient: 64 KB per stage
-using X256D = Umma16Cfg<256, 1, 1, 4, 0, Fmt16, Fmt16>;      // dCol GEMMs (K = 64 = ONE stage of 96 KB)
-using X64G = Umma16Cfg<64, 2, 1, 4, 0, Fmt16, Fmt16>;        // conv3 data gradient, gather form (K = 9 taps x 64)
-using X32G = Umma16Cfg<32, 3, 1, 4, 0, Fmt16, Fmt16>;        // conv2 data gradient, gather form (4 parity classes, K = 4 taps x 64)
+// conv data gradients (pre-tiled B, one K tile of 64 co per filter tap): per-tap partial sums added in tap order, the
+// rounding of the dCol GEMM + col2im of math modes 2-4.  The second register set costs conv2 (BN = 128) its loader warp
+// and half its producer warps (384 threads: 170 registers each).
+using X64T = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16, 0, true>;    // conv3: K = 9 taps x 64 co, N = 64 ci
+using X128T = Umma16Cfg<128, 3, 1, 4, 0, Fmt16, Fmt16, 0, true>;  // conv2: K = 4 taps x 64 co, N = 4 parity classes x 32 ci
 
 // math mode 3 (experimental): the persistent, fully warp-specialised variant of each tensor-core configuration
 template <class U> struct PersistOf;

@@ -64,21 +64,26 @@ void weight_image_sizes(size_t (&b)[WeightImages::kCount]) {
   b[2] = weight_image_bytes<64>(64, 576);
   b[3] = weight_image_bytes<256>(Geo::G4, Geo::XK);
   b[4] = weight_image_bytes<128>(Geo::FLAT + Geo::EMB, Geo::G4);
-  b[5] = weight_image_bytes<256>(576, 64);
-  b[6] = weight_image_bytes<256>(512, 64);
+  b[5] = weight_image_bytes<256>(576, 64);   // the dCol operands of math modes 2-4; larger than the 16-bit dgrad images
+  b[6] = weight_image_bytes<256>(512, 64);   // of math mode 5 (weight_image16_bytes<64>(64, 576), <128>(128, 256))
 }
 
 // Refresh the weight images (4 launches on the side stream + 1 for the two conv-forward images; ~60 MB written).
 // Must run after every parameter change.  Image 0 (conv1) is unused: conv1 is the first kernel of the step and its
 // weight tile is 1/5 of a stage.
-// math mode 5: the same seven images in the 16-bit K-major form (gemm_umma16.cuh); they fit into the same buffers
+// math mode 5: the same seven images in the 16-bit K-major form (gemm_umma16.cuh); they fit into the same buffers.
+// Images 5 / 6 are the B operands of the conv3 / conv2 data gradients (gather form: B(k = (tap, co), n = ci)).
+static int retile_dgrad16(cudaStream_t s, const ParamLayout& pl, const float* P, const WeightImages& wi) {
+  DRL_TRY((launch_retile_b16<64, Fmt16>(s, Conv3DB{P + pl.conv3_w}, 64, 576, wi.img[5])));
+  DRL_TRY((launch_retile_b16<128, Fmt16>(s, Conv2DBm{{P + pl.conv2_w}}, 128, 256, wi.img[6])));
+  return DRL_OK;
+}
+
 int net_retile16(cudaStream_t s_rest, const ParamLayout& pl, const float* P, const WeightImages& wi) {
   prof_mark(s_rest, "weight_retile");
   DRL_TRY((launch_retile_b16<256, Fmt16>(s_rest, PlainB{P + pl.lstm_w, Geo::G4, 0}, Geo::G4, Geo::XK, wi.img[3])));
   DRL_TRY((launch_retile_b16<128, Fmt16>(s_rest, PlainBT{P + pl.lstm_w, Geo::G4, 0}, Geo::FLAT + Geo::EMB, Geo::G4, wi.img[4])));
-  DRL_TRY((launch_retile_b16<256, Fmt16>(s_rest, PlainBT{P + pl.conv3_w, 64, 0}, 576, 64, wi.img[5])));
-  DRL_TRY((launch_retile_b16<256, Fmt16>(s_rest, PlainBT{P + pl.conv2_w, 64, 0}, 512, 64, wi.img[6])));
-  return DRL_OK;
+  return retile_dgrad16(s_rest, pl, P, wi);
 }
 
 int net_retile(cudaStream_t, cudaStream_t s_rest, const ParamLayout& pl, const float* P, const WeightImages& wi) {
@@ -139,11 +144,11 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
   if (retile && mode >= 2) {
     if (m16 && st.par) {
       // the LSTM forward image first; lstm_fwd waits for it (and the embedding table) only -- the three images of the
-      // backward pass (LSTM dgrad, two dCol) are joined at the end of the forward pass, long after they are done
+      // backward pass (LSTM dgrad, conv3 / conv2 dgrad) are joined at the end of the forward pass, long after they are done
       prof_mark(side, "weight_retile");
       DRL_TRY((launch_retile_b16<256, Fmt16>(side, PlainB{P + pl.lstm_w, Geo::G4, 0}, Geo::G4, Geo::XK, wi.img[3])));
       DRL_CUDA_CHECK(cudaEventRecord(st.ev[1], side));
-      late_images = true;   // LSTM dgrad + two dCol images: behind lstm_gates_fwd, in the shadow of the small head kernels
+      late_images = true;   // LSTM dgrad + two conv dgrad images: behind lstm_gates_fwd, in the shadow of the small head kernels
     } else if (m16) {
       DRL_TRY(net_retile16(side, pl, P, wi));
     } else {
@@ -235,8 +240,7 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     // for the SMs if launched with the others; the head layers that follow leave most of the GPU idle
     DRL_TRY(fork_to_side(st, 3));
     DRL_TRY((launch_retile_b16<128, Fmt16>(side, PlainBT{P + pl.lstm_w, Geo::G4, 0}, Geo::FLAT + Geo::EMB, Geo::G4, wi.img[4])));
-    DRL_TRY((launch_retile_b16<256, Fmt16>(side, PlainBT{P + pl.conv3_w, 64, 0}, 576, 64, wi.img[5])));
-    DRL_TRY((launch_retile_b16<256, Fmt16>(side, PlainBT{P + pl.conv2_w, 64, 0}, 512, 64, wi.img[6])));
+    DRL_TRY(retile_dgrad16(side, pl, P, wi));
   }
   {
     PlainA al{act.h1, Geo::L, 0};
@@ -409,14 +413,14 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     KERNEL("conv3_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv3_w, slab), 1);
   }
   s = st.main;
-  // DRL_B200_DGRAD_GATHER=1 (math mode 5): the data gradients of conv3 / conv2 as gather-GEMMs over the input pixels
-  // (K = taps x 64 output channels, ReLU mask in the epilogue) instead of dCol GEMM + col2im
-  static const bool dgrad_gather = getenv("DRL_B200_DGRAD_GATHER") != nullptr;
-  if (m16 && dgrad_gather) {
+  if (m16) {
+    // gather form: rows = input pixels, K = 9 taps x 64 output channels (taps outside the output are zero), ReLU mask of
+    // a2 in the epilogue; each tap's partial sum is rounded to fp32 and the taps are added in (ky, kx) order, as
+    // col2im_conv3 adds the dCol of math modes 2-4: the same da2, bit for bit
     Conv3DA al{bw.da3};
-    Conv3DB bl{P + pl.conv3_w};
+    PretiledB<Conv3DB> blp{wi.img[5], 576 / 64};
     Conv3DE ep{bw.da2, act.a2};
-    GEMM16("conv3_dgrad", X64G, al, bl, ep, Mb * 81, 64, 576, 1, 576, 0);
+    GEMM16("conv3_dgrad", X64T, al, blp, ep, Mb * 81, 64, 576, 1, 576, 0);
   } else if (mode >= 2) {
     // "dCol" form: one plain GEMM with K = 64 output channels (instead of gathering every dY value 9 times
     // through the producers), then a gather of <= 9 taps per input pixel with the ReLU mask.
@@ -426,9 +430,8 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     // K = 64 (two K tiles) and 128 x 256 outputs per tile: epilogue-dominated, so the persistent kernel whose
     // dedicated epilogue warps wins here while the producers gather the next tile.
     prof_mark(s, "conv3_dgrad");
-    PretiledB<PlainBT> blp{wi.img[5], m16 ? 1 : 2};
-    if (m16) DRL_TRY((launch_gemm_umma16<X256D>(s, al, blp, ep, Mb * 49, 576, 64, 1, 64, 0)));
-    else DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 49, 576, 64, 1, 64, 0)));
+    PretiledB<PlainBT> blp{wi.img[5], 2};
+    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 49, 576, 64, 1, 64, 0)));
     prof_mark(s, "conv3_col2im");
     DRL_TRY(col2im_conv3(s, bw.dcol, act.a2, bw.da2, Mb));
     n += 2;
@@ -454,19 +457,21 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     KERNEL("conv2_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv2_w, slab), 1);
   }
   s = st.main;
-  if (m16 && dgrad_gather) {
+  if (m16) {
+    // merged-phase gather form: row = the 2 x 2 block of input pixels (2i + py, 2j + px); all four parity classes read
+    // the same dY taps (i - a, j - b), so K = (a, b, co) = 256 and N = (py, px, ci) = 128; ReLU mask of a1 in the epilogue;
+    // per-tap partial sums added in (a, b) order, as in col2im_conv2
     Conv2DA al{bw.da2};
-    Conv2DB bl{P + pl.conv2_w};
-    Conv2DE ep{bw.da1, act.a1};
-    GEMM16("conv2_dgrad", X32G, al, bl, ep, Mb * 100, 32, 256, 4, 256, 0);
+    PretiledB<Conv2DBm> blp{wi.img[6], 256 / 64};
+    Conv2DEm ep{{bw.da1, act.a1}};
+    GEMM16("conv2_dgrad", X128T, al, blp, ep, Mb * 100, 128, 256, 1, 256, 0);
   } else if (mode >= 2) {
     PlainA al{bw.da2, 64, 0};
     PlainBT bl{P + pl.conv2_w, 64, 0};               // B(k = co, n = (ky,kx,ci)) = W[n*64 + co]
     EpRaw<false> ep{bw.dcol, 512, 0, 1.0f, 0, 512};
     prof_mark(s, "conv2_dgrad");                      // persistent kernel: 0.079 vs 0.091 ms
-    PretiledB<PlainBT> blp{wi.img[6], m16 ? 1 : 2};
-    if (m16) DRL_TRY((launch_gemm_umma16<X256D>(s, al, blp, ep, Mb * 81, 512, 64, 1, 64, 0)));
-    else DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 81, 512, 64, 1, 64, 0)));
+    PretiledB<PlainBT> blp{wi.img[6], 2};
+    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 81, 512, 64, 1, 64, 0)));
     prof_mark(s, "conv2_col2im");
     DRL_TRY(col2im_conv2(s, bw.dcol, act.a1, bw.da1, Mb));
     n += 2;

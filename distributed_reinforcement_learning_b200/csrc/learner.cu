@@ -512,7 +512,7 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     DRL_TRY(dev_alloc(h, &b.wg_part, b.wg_part_floats));
     DRL_TRY(dev_alloc(h, &b.wg_part2, b.wg_part_floats));
     DRL_TRY(dev_alloc(h, &b.emb_scratch, (size_t)16 * 32 * 256));
-    DRL_TRY(dev_alloc(h, &b.dcol, Mb * 81 * 512));
+    if (h->mode != 5) DRL_TRY(dev_alloc(h, &b.dcol, Mb * 81 * 512));
     {
       size_t wb[WeightImages::kCount];
       weight_image_sizes(wb);

@@ -172,6 +172,17 @@ struct ConvDgradB {
     return __ldg(reinterpret_cast<const float4*>(w + ((size_t)((ky * KW + kx) * CI + r.n)) * CO + co));
   }
 };
+// All S*S parity classes side by side along N: n = (z, ci), B(k, n) = class z's B(k, ci).  Every class of the S x S block
+// of input pixels at (yy, xx) reads the same dY taps, so the whole data gradient is ONE GEMM with N = S*S*CI whose A
+// operand (ConvDgradA) is gathered once per row instead of once per class.
+template <int CI, int CO, int S, int KH, int KW>
+struct ConvDgradBMerged {
+  static constexpr bool kContigK = true;
+  ConvDgradB<CI, CO, S, KH, KW> b;
+  using Row = typename ConvDgradB<CI, CO, S, KH, KW>::Row;
+  __device__ __forceinline__ Row row(int, int n) const { return n < 0 ? b.row(0, -1) : b.row(n / CI, n % CI); }
+  __device__ __forceinline__ float4 load(const Row& r, int k) const { return b.load(r, k); }
+};
 
 // --------------------------------------------------------------------------------------------
 // LSTM operand: x_m = [flatten(a3_m) | emb[prev_action_m] | h0_m]  (model/impala_actor_critic.py:35-38,
@@ -538,6 +549,18 @@ struct EpConvDx {
 #pragma unroll
       for (int j = 0; j < V; ++j) dx[o + j] = (__ldg(act + o + j) > 0.f) ? v[j] : 0.f;
     }
+  }
+  __device__ __forceinline__ void store_colsum(int, int, float) const {}
+};
+// The same for the merged-phase GEMM (ConvDgradBMerged): column n = (z, ci).  The 4 columns of a store never straddle
+// two classes (CI is a multiple of 4), and the 32 columns of an epilogue block are CI = 32 channels of one pixel.
+template <int IH, int IW, int CI, int S, int RH, int RW>
+struct EpConvDxMerged {
+  static constexpr bool kColSum = false;
+  EpConvDx<IH, IW, CI, S, RH, RW> e;
+  template <int V>
+  __device__ __forceinline__ void store(int, int m, int n, const float (&v)[V]) const {
+    e.template store<V>(n / CI, m, n % CI, v);
   }
   __device__ __forceinline__ void store_colsum(int, int, float) const {}
 };
