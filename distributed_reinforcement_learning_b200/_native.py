@@ -246,3 +246,11 @@ def as_c(arr, dtype, shape=None, name="array"):
 
 def ptr(a):
     return C.c_void_p(a.ctypes.data)
+
+
+def as_u8(done):
+    """A done / boolean array as uint8 (a bool array is viewed, not converted)."""
+    d = np.asarray(done)
+    if d.dtype == np.bool_:
+        return np.ascontiguousarray(d).view(np.uint8)
+    return d.astype(np.uint8, copy=False)

@@ -5,11 +5,13 @@ import ctypes as C
 import numpy as np
 
 from . import _native as N
-from . import dp
-from .apex_learner import _as_u8
+from .adam_learner import AdamLearnerHandle
 
 
-class NativeA3CLearner:
+class NativeA3CLearner(AdamLearnerHandle):
+    family = "a3c"
+    last_step_ms = None      # the A3C C-ABI has no step timer
+
     def __init__(self, batch, num_action=4, input_shape=(84, 84, 4), discount_factor=0.997, start_learning_rate=1e-4,
                  end_learning_rate=0.0, learning_frame=1000000000, baseline_loss_coef=1.0, entropy_coef=0.05,
                  gradient_clip_norm=40.0, reward_clipping="abs_one", device=0, num_slots=2, use_cuda_graph=False,
@@ -23,26 +25,9 @@ class NativeA3CLearner:
                           float(learning_frame), baseline_loss_coef, entropy_coef, gradient_clip_norm,
                           N.REWARD_CLIPPING[reward_clipping], int(device), int(num_slots), int(bool(use_cuda_graph)),
                           int(math_mode))
-        self._h = C.c_void_p()
-        N.check(N.lib.drl_a3c_create(C.byref(cfg), C.byref(self._h)))
-        n = C.c_int64()
-        N.check(N.lib.drl_a3c_param_count(self._h, C.byref(n)))
-        self.param_count = int(n.value)
-        self.num_slots = int(num_slots)
-        self._keep = [None] * self.num_slots
-        self._dp = dp.BucketAllReduce("a3c", self._h, int(device))
+        self._create(cfg, device, num_slots)
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value:
-            N.lib.drl_a3c_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
+    # one network: no `which`
     def set_params(self, flat):
         a = N.as_c(flat, np.float32, (self.param_count,), "params")
         N.check(N.lib.drl_a3c_set_params(self._h, N.ptr(a), a.size))
@@ -52,38 +37,16 @@ class NativeA3CLearner:
         N.check(N.lib.drl_a3c_get_params(self._h, N.ptr(a), a.size))
         return a
 
-    def set_opt_state(self, m, v, step, beta1_power=0.9, beta2_power=0.999):
-        am = N.as_c(m, np.float32, (self.param_count,), "m")
-        av = N.as_c(v, np.float32, (self.param_count,), "v")
-        N.check(N.lib.drl_a3c_set_opt_state(self._h, N.ptr(am), N.ptr(av), am.size, int(step), float(beta1_power),
-                                            float(beta2_power)))
-
-    def get_opt_state(self):
-        m = np.empty(self.param_count, np.float32)
-        v = np.empty(self.param_count, np.float32)
-        st, b1, b2 = C.c_int64(), C.c_float(), C.c_float()
-        N.check(N.lib.drl_a3c_get_opt_state(self._h, N.ptr(m), N.ptr(v), m.size, C.byref(st), C.byref(b1), C.byref(b2)))
-        return dict(m=m, v=v, step=int(st.value), beta1_power=float(b1.value), beta2_power=float(b2.value))
-
-    def get_grads(self):
-        a = np.empty(self.param_count, np.float32)
-        N.check(N.lib.drl_a3c_get_grads(self._h, N.ptr(a), a.size))
-        return a
-
     def stage(self, slot, state, next_state, previous_action, action, reward, done):
         B = self.B
         arrs = (N.as_c(state, np.uint8, (B,) + self.input_shape, "state"),
                 N.as_c(next_state, np.uint8, (B,) + self.input_shape, "next_state"),
                 N.as_c(previous_action, np.int32, (B,), "previous_action"), N.as_c(action, np.int32, (B,), "action"),
-                N.as_c(reward, np.float32, (B,), "reward"), N.as_c(_as_u8(done), np.uint8, (B,), "done"))
+                N.as_c(reward, np.float32, (B,), "reward"), N.as_c(N.as_u8(done), np.uint8, (B,), "done"))
         self._keep[slot] = arrs
         N.check(N.lib.drl_a3c_stage(self._h, slot, *[N.ptr(a) for a in arrs]))
 
-    def step(self, slot=0):
-        if dp.distributed():
-            self._dp.step_async(slot)           # data parallel: see dp.py
-        else:
-            N.check(N.lib.drl_a3c_step_async(self._h, slot))
+    def wait(self):
         o = N.A3cOut()
         N.check(N.lib.drl_a3c_wait(self._h, C.byref(o)))
         return dict(pi_loss=o.pi_loss, baseline_loss=o.baseline_loss, entropy=o.entropy, learning_rate=o.learning_rate,
@@ -104,8 +67,3 @@ class NativeA3CLearner:
         out = [np.empty((B, self.A), np.float32), np.empty(B, np.float32), np.empty(B, np.float32), np.empty(B, np.float32)]
         N.check(N.lib.drl_a3c_taps(self._h, *[N.ptr(a) for a in out]))
         return dict(policy=out[0], value=out[1], next_value=out[2], advantage=out[3])
-
-    def read_buffer(self, name, count):
-        a = np.empty(int(count), np.float32)
-        N.check(N.lib.drl_a3c_read_buffer(self._h, name.encode(), N.ptr(a), a.size))
-        return a

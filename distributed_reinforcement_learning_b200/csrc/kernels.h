@@ -1,28 +1,75 @@
-// kernels.h -- internal interface between the learner orchestration (learner.cu) and the kernel
-// launchers (layers.cu, elementwise.cu, vtrace.cu, optimizer.cu).  Not part of the C-ABI.
+// kernels.h -- internal interface between the learner orchestration (learner.cu; adam_learner.cu with apex.cu and
+// r2d2.cu) and the kernel launchers (layers.cu, elementwise.cu, vtrace.cu, optimizer.cu).  Not part of the C-ABI.
 #pragma once
 #include "common.cuh"
 
 namespace drl {
 
-// Offsets (in floats) of each tensor inside the padded flat parameter / gradient / slot vectors.
+// Offsets (in floats) of each tensor inside the padded flat parameter / gradient / slot vectors of one network.
 // Order = TF1 variable-creation order (SURVEY.md App. A.6); every bias directly follows its
 // kernel (kernel sizes are multiples of 4) and is padded up to a multiple of 4 floats so that all
 // kernels start 16-byte aligned.  [w ; b] therefore forms one contiguous [(K+1), N] matrix, which
 // is what the weight-gradient GEMMs write (bias gradient = column sum of dY in row K).
-struct ParamLayout {
+// The C-ABI exchanges the packed (TF-flat) vector; the device holds the padded one.
+struct FlatLayout {
+  static constexpr int kMaxTensors = 24;
+  int num_tensors = 0;
+  int64_t padded_total = 0;   // floats in the padded vector (multiple of 4)
+  int64_t packed_total = 0;   // floats in the TF-flat (API) vector
+  int64_t packed_off[kMaxTensors], padded_off[kMaxTensors], count[kMaxTensors];
+  // offsets of the tensors of sizes[] (kernel, bias, kernel, bias, ...); *named[i] receives padded_off[i]
+  template <int N>
+  void set(const int64_t (&sizes)[N], int64_t* const (&named)[N]) {
+    static_assert(N <= kMaxTensors, "too many tensors");
+    set(N, sizes, named);
+  }
+  void set(int n, const int64_t* sizes, int64_t* const* named);
+};
+
+struct ParamLayout : FlatLayout {   // IMPALA network
   int A;
   int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b;
   int64_t emb1_w, emb1_b, emb2_w, emb2_b;
   int64_t lstm_w, lstm_b;
   int64_t actor1_w, actor1_b, actor2_w, actor2_b, actor3_w, actor3_b;
   int64_t critic1_w, critic1_b, critic2_w, critic2_b, critic3_w, critic3_b;
-  int64_t padded_total;   // floats in the padded vector (multiple of 4)
-  int64_t packed_total;   // floats in the TF-flat (API) vector
-  static constexpr int kNumTensors = 24;
-  int64_t packed_off[kNumTensors], padded_off[kNumTensors], count[kNumTensors];
   void init(int num_action);
 };
+
+// packed (API) <-> padded (device) copies through the pinned staging buffer `h_flat` (padded_total floats) on stream
+// `s`; both return once the copy is complete.  upload fills the padding with pad_value.
+int upload_flat(cudaStream_t s, float* h_flat, const FlatLayout& pl, float* dev_padded, const float* host_packed,
+                float pad_value);
+int download_flat(cudaStream_t s, float* h_flat, const FlatLayout& pl, const float* dev_padded, float* host_packed);
+
+// cudaMalloc + memset of count elements plus 256 bytes of slack (kernels may read a vector's tail past its end);
+// the handle's `allocs` list owns the memory
+template <class H, class T>
+int dev_alloc(H* h, T** p, size_t count, int fill_byte = 0) {
+  void* q = nullptr;
+  DRL_CUDA_CHECK(cudaMalloc(&q, count * sizeof(T) + 256));
+  DRL_CUDA_CHECK(cudaMemset(q, fill_byte, count * sizeof(T) + 256));
+  h->allocs.push_back(q);
+  *p = static_cast<T*>(q);
+  return DRL_OK;
+}
+
+inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Captures what enqueue() (-> DRL_OK or an error code) issues on stream s into an instantiated graph.  A failing
+// enqueue or capture leaves *exec untouched.
+template <class F>
+int capture_graph(cudaStream_t s, F&& enqueue, cudaGraphExec_t* exec) {
+  cudaGraph_t g = nullptr;
+  DRL_CUDA_CHECK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+  const int r = enqueue();
+  const cudaError_t e = cudaStreamEndCapture(s, &g);
+  if (r != DRL_OK) { if (g) cudaGraphDestroy(g); return r; }
+  if (e != cudaSuccess) { set_error("graph capture failed: %s", cudaGetErrorString(e)); return DRL_ERR_CUDA; }
+  DRL_CUDA_CHECK(cudaGraphInstantiate(exec, g, 0));
+  cudaGraphDestroy(g);
+  return DRL_OK;
+}
 
 struct Inputs {          // one device staging slot, caller's batch-major layout
   const uint8_t* frames; // [B,T,84,84,4]
@@ -194,7 +241,7 @@ struct OptState {
 int optimizer_apply(cudaStream_t s, const OptState& o);
 int optimizer_update_only(cudaStream_t s, const OptState& o);   // clip + RMSProp from already reduced partials
 
-// ---- apex.cu: TF1 Adam (shared by the Ape-X and the R2D2 learner) -------------------------------------------------
+// ---- adam_learner.cu: TF1 Adam (the Ape-X / A3C and the R2D2 learner) -------------------------------------------
 // clip_norm <= 0: no clipping (optimizer.minimize, agent/r2d2.py:92); start_lr == end_lr: constant learning rate
 struct AdamState {
   float* params; float* m; float* v; const float* grads; int64_t n;

@@ -106,6 +106,23 @@ int prof_end(cudaStream_t s, int rc, char* names, int64_t names_len, float* ms, 
   return DRL_OK;
 }
 
+int upload_flat(cudaStream_t s, float* h_flat, const FlatLayout& pl, float* dev_padded, const float* host_packed,
+                float pad_value) {
+  for (int64_t i = 0; i < pl.padded_total; ++i) h_flat[i] = pad_value;
+  for (int i = 0; i < pl.num_tensors; ++i)
+    memcpy(h_flat + pl.padded_off[i], host_packed + pl.packed_off[i], pl.count[i] * sizeof(float));
+  DRL_CUDA_CHECK(cudaMemcpyAsync(dev_padded, h_flat, pl.padded_total * sizeof(float), cudaMemcpyHostToDevice, s));
+  DRL_CUDA_CHECK(cudaStreamSynchronize(s));
+  return DRL_OK;
+}
+int download_flat(cudaStream_t s, float* h_flat, const FlatLayout& pl, const float* dev_padded, float* host_packed) {
+  DRL_CUDA_CHECK(cudaMemcpyAsync(h_flat, dev_padded, pl.padded_total * sizeof(float), cudaMemcpyDeviceToHost, s));
+  DRL_CUDA_CHECK(cudaStreamSynchronize(s));
+  for (int i = 0; i < pl.num_tensors; ++i)
+    memcpy(host_packed + pl.packed_off[i], h_flat + pl.padded_off[i], pl.count[i] * sizeof(float));
+  return DRL_OK;
+}
+
 struct Slot {
   uint8_t* base = nullptr;   // one allocation, fields at 256-byte aligned offsets
   Inputs in{};
@@ -175,18 +192,6 @@ struct drl_learner {
 
 namespace {
 
-template <class T>
-int dev_alloc(drl_learner* h, T** p, size_t count, int fill_byte = 0) {
-  void* q = nullptr;
-  DRL_CUDA_CHECK(cudaMalloc(&q, count * sizeof(T) + 256));
-  DRL_CUDA_CHECK(cudaMemset(q, fill_byte, count * sizeof(T) + 256));
-  h->allocs.push_back(q);
-  *p = static_cast<T*>(q);
-  return DRL_OK;
-}
-
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 int check_handle(const drl_learner* h) {
   if (!h) { set_error("null learner handle"); return DRL_ERR_INVALID; }
   return DRL_OK;
@@ -202,25 +207,6 @@ int check_not_failed(const drl_learner* h) {
 
 int set_device(const drl_learner* h) {
   DRL_CUDA_CHECK(cudaSetDevice(h->cfg.device));
-  return DRL_OK;
-}
-
-// packed (TF-flat, API) <-> padded (device) copies through the pinned scratch
-int upload_flat(drl_learner* h, float* dev_padded, const float* host_packed, float pad_value) {
-  for (int64_t i = 0; i < h->pl.padded_total; ++i) h->h_flat[i] = pad_value;
-  for (int i = 0; i < ParamLayout::kNumTensors; ++i)
-    memcpy(h->h_flat + h->pl.padded_off[i], host_packed + h->pl.packed_off[i], h->pl.count[i] * sizeof(float));
-  DRL_CUDA_CHECK(cudaMemcpyAsync(dev_padded, h->h_flat, h->pl.padded_total * sizeof(float), cudaMemcpyHostToDevice,
-                                 h->compute));
-  DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
-  return DRL_OK;
-}
-int download_flat(drl_learner* h, const float* dev_padded, float* host_packed) {
-  DRL_CUDA_CHECK(cudaMemcpyAsync(h->h_flat, dev_padded, h->pl.padded_total * sizeof(float), cudaMemcpyDeviceToHost,
-                                 h->compute));
-  DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
-  for (int i = 0; i < ParamLayout::kNumTensors; ++i)
-    memcpy(host_packed + h->pl.packed_off[i], h->h_flat + h->pl.padded_off[i], h->pl.count[i] * sizeof(float));
   return DRL_OK;
 }
 
@@ -311,14 +297,7 @@ int run_forward_backward(drl_learner* h, int slot) {
       // one eager pass first: sets the per-kernel shared-memory attributes outside of stream capture
       // (idempotent: every buffer it writes is fully overwritten by the captured pass)
       DRL_TRY(enqueue_forward_backward(h, slot));
-      cudaGraph_t g = nullptr;
-      DRL_CUDA_CHECK(cudaStreamBeginCapture(h->compute, cudaStreamCaptureModeThreadLocal));
-      int r = enqueue_forward_backward(h, slot);
-      cudaError_t e = cudaStreamEndCapture(h->compute, &g);
-      if (r != DRL_OK) { if (g) cudaGraphDestroy(g); return r; }
-      if (e != cudaSuccess) { set_error("graph capture failed: %s", cudaGetErrorString(e)); return DRL_ERR_CUDA; }
-      DRL_CUDA_CHECK(cudaGraphInstantiate(&h->graph_fb[slot], g, 0));
-      cudaGraphDestroy(g);
+      DRL_TRY(capture_graph(h->compute, [&] { return enqueue_forward_backward(h, slot); }, &h->graph_fb[slot]));
     }
     DRL_CUDA_CHECK(cudaGraphLaunch(h->graph_fb[slot], h->compute));
   } else {
@@ -330,16 +309,8 @@ int run_forward_backward(drl_learner* h, int slot) {
 
 int run_apply(drl_learner* h) {
   if (h->cfg.use_cuda_graph) {
-    if (!h->graph_apply) {
-      cudaGraph_t g = nullptr;
-      DRL_CUDA_CHECK(cudaStreamBeginCapture(h->compute, cudaStreamCaptureModeThreadLocal));
-      int r = enqueue_apply(h, (int)h->slots.size());
-      cudaError_t e = cudaStreamEndCapture(h->compute, &g);
-      if (r != DRL_OK) { if (g) cudaGraphDestroy(g); return r; }
-      if (e != cudaSuccess) { set_error("graph capture failed: %s", cudaGetErrorString(e)); return DRL_ERR_CUDA; }
-      DRL_CUDA_CHECK(cudaGraphInstantiate(&h->graph_apply, g, 0));
-      cudaGraphDestroy(g);
-    }
+    if (!h->graph_apply)
+      DRL_TRY(capture_graph(h->compute, [&] { return enqueue_apply(h, (int)h->slots.size()); }, &h->graph_apply));
     DRL_CUDA_CHECK(cudaGraphLaunch(h->graph_apply, h->compute));
   } else {
     DRL_TRY(enqueue_apply(h, (int)h->slots.size()));
@@ -363,15 +334,10 @@ int run_step(drl_learner* h, int slot) {
   if (h->cfg.use_cuda_graph) {
     if (!h->graph_step[slot]) {
       DRL_TRY(enqueue_forward_backward(h, slot));   // eager pass: per-kernel attributes are set outside of capture
-      cudaGraph_t g = nullptr;
-      DRL_CUDA_CHECK(cudaStreamBeginCapture(h->compute, cudaStreamCaptureModeThreadLocal));
-      int r = enqueue_forward_backward(h, slot);
-      if (r == DRL_OK) r = enqueue_apply(h, slot, false, h->peer_on && h->par && h->peer_early_ctas > 0);
-      cudaError_t e = cudaStreamEndCapture(h->compute, &g);
-      if (r != DRL_OK) { if (g) cudaGraphDestroy(g); return r; }
-      if (e != cudaSuccess) { set_error("graph capture failed: %s", cudaGetErrorString(e)); return DRL_ERR_CUDA; }
-      DRL_CUDA_CHECK(cudaGraphInstantiate(&h->graph_step[slot], g, 0));
-      cudaGraphDestroy(g);
+      DRL_TRY(capture_graph(h->compute, [&] {
+        DRL_TRY(enqueue_forward_backward(h, slot));
+        return enqueue_apply(h, slot, false, h->peer_on && h->par && h->peer_early_ctas > 0);
+      }, &h->graph_step[slot]));
     }
     NvtxRange r("drl:step(graph)");
     DRL_CUDA_CHECK(cudaGraphLaunch(h->graph_step[slot], h->compute));
@@ -634,7 +600,7 @@ int drl_learner_set_params(drl_learner* h, const float* host_flat, int64_t n) {
   DRL_LOCK(const_cast<drl_learner*>(h));
   if (!host_flat || n != h->pl.packed_total) { set_error("set_params: expected %lld floats, got %lld", (long long)h->pl.packed_total, (long long)n); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  DRL_TRY(upload_flat(h, h->params, host_flat, 0.0f));
+  DRL_TRY(upload_flat(h->compute, h->h_flat, h->pl, h->params, host_flat, 0.0f));
   h->images_stale = true;
   return DRL_OK;
 }
@@ -644,14 +610,14 @@ int drl_learner_get_params(drl_learner* h, float* host_flat, int64_t n) {
   DRL_TRY(check_not_failed(h));
   if (!host_flat || n != h->pl.packed_total) { set_error("get_params: expected %lld floats", (long long)h->pl.packed_total); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  return download_flat(h, h->params, host_flat);
+  return download_flat(h->compute, h->h_flat, h->pl, h->params, host_flat);
 }
 int drl_learner_set_opt_state(drl_learner* h, const float* host_ms_flat, int64_t n, int64_t step) {
   DRL_TRY(check_handle(h));
   DRL_LOCK(const_cast<drl_learner*>(h));
   if (!host_ms_flat || n != h->pl.packed_total) { set_error("set_opt_state: expected %lld floats", (long long)h->pl.packed_total); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  DRL_TRY(upload_flat(h, h->ms, host_ms_flat, 1.0f));
+  DRL_TRY(upload_flat(h->compute, h->h_flat, h->pl, h->ms, host_ms_flat, 1.0f));
   long long st = step;
   DRL_CUDA_CHECK(cudaMemcpy(h->d_step, &st, sizeof(st), cudaMemcpyHostToDevice));
   return DRL_OK;
@@ -662,7 +628,7 @@ int drl_learner_get_opt_state(drl_learner* h, float* host_ms_flat, int64_t n, in
   DRL_TRY(check_not_failed(h));
   if (n != h->pl.packed_total) { set_error("get_opt_state: expected %lld floats", (long long)h->pl.packed_total); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  if (host_ms_flat) DRL_TRY(download_flat(h, h->ms, host_ms_flat));
+  if (host_ms_flat) DRL_TRY(download_flat(h->compute, h->h_flat, h->pl, h->ms, host_ms_flat));
   if (step) {
     long long st = 0;
     DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
@@ -677,7 +643,8 @@ int drl_learner_get_grads(drl_learner* h, float* host_flat, int64_t n) {
   DRL_TRY(check_not_failed(h));
   if (!host_flat || n != h->pl.packed_total) { set_error("get_grads: expected %lld floats", (long long)h->pl.packed_total); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  return download_flat(h, h->peer_on ? reinterpret_cast<float*>(h->comm) : h->bucket, host_flat);
+  return download_flat(h->compute, h->h_flat, h->pl, h->peer_on ? reinterpret_cast<float*>(h->comm) : h->bucket,
+                       host_flat);
 }
 
 int drl_learner_stage(drl_learner* h, int32_t slot, const uint8_t* state, const float* reward, const int32_t* action,

@@ -17,13 +17,6 @@ from . import _native as N
 H, W, CH, LSTM = 84, 84, 4, 256
 
 
-def _as_u8(done):
-    d = np.asarray(done)
-    if d.dtype == np.bool_:
-        return np.ascontiguousarray(d).view(np.uint8)      # bool is one byte, 0/1: no copy
-    return d.astype(np.uint8, copy=False)
-
-
 class NativeLearner:
     def __init__(self, batch, trajectory=20, num_action=18, lstm_hidden_size=256, input_shape=(84, 84, 4),
                  discount_factor=0.99, start_learning_rate=0.0006, end_learning_rate=0.0,
@@ -96,7 +89,7 @@ class NativeLearner:
         arrs = (N.as_c(state, np.uint8, (B, T) + self.input_shape, "state"),
                 N.as_c(reward, np.float32, (B, T), "reward"),
                 N.as_c(action, np.int32, (B, T), "action"),
-                N.as_c(_as_u8(done), np.uint8, (B, T), "done"),
+                N.as_c(N.as_u8(done), np.uint8, (B, T), "done"),
                 N.as_c(behavior_policy, np.float32, (B, T, A), "behavior_policy"),
                 N.as_c(previous_action, np.int32, (B, T), "previous_action"),
                 N.as_c(initial_h, np.float32, (B, T, L), "initial_h"),

@@ -10,19 +10,12 @@ import ctypes as C
 import numpy as np
 
 from . import _native as N
-from . import dp
-
-MAIN, TARGET = 0, 1
+from .adam_learner import MAIN, TARGET, AdamLearnerHandle  # noqa: F401  (MAIN / TARGET: the `which` of set/get_params)
 
 
-def _as_u8(done):
-    d = np.asarray(done)
-    if d.dtype == np.bool_:
-        return np.ascontiguousarray(d).view(np.uint8)
-    return d.astype(np.uint8, copy=False)
+class NativeR2D2Learner(AdamLearnerHandle):
+    family = "r2d2"
 
-
-class NativeR2D2Learner:
     def __init__(self, batch, seq_len=15, burn_in=7, num_action=4, lstm_size=64, input_shape=(84, 84, 1),
                  discount_factor=0.997, learning_rate=1e-4, device=0, num_slots=2, use_cuda_graph=False, math_mode=0):
         h, w, c = input_shape
@@ -32,52 +25,7 @@ class NativeR2D2Learner:
         self.device = int(device)
         cfg = N.R2d2Config(self.B, self.S, self.bi, h, w, c, self.A, self.L, discount_factor, learning_rate,
                            self.device, int(num_slots), int(bool(use_cuda_graph)), int(math_mode))
-        self._h = C.c_void_p()
-        N.check(N.lib.drl_r2d2_create(C.byref(cfg), C.byref(self._h)))
-        n = C.c_int64()
-        N.check(N.lib.drl_r2d2_param_count(self._h, C.byref(n)))
-        self.param_count = int(n.value)
-        self.num_slots = int(num_slots)
-        self._keep = [None] * self.num_slots
-        self._dp = dp.BucketAllReduce("r2d2", self._h, self.device)
-
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value:
-            N.lib.drl_r2d2_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def set_params(self, flat, which=MAIN):
-        a = N.as_c(flat, np.float32, (self.param_count,), "params")
-        N.check(N.lib.drl_r2d2_set_params(self._h, int(which), N.ptr(a), a.size))
-
-    def get_params(self, which=MAIN):
-        a = np.empty(self.param_count, np.float32)
-        N.check(N.lib.drl_r2d2_get_params(self._h, int(which), N.ptr(a), a.size))
-        return a
-
-    def set_opt_state(self, m, v, step, beta1_power=0.9, beta2_power=0.999):
-        am = N.as_c(m, np.float32, (self.param_count,), "m")
-        av = N.as_c(v, np.float32, (self.param_count,), "v")
-        N.check(N.lib.drl_r2d2_set_opt_state(self._h, N.ptr(am), N.ptr(av), am.size, int(step), float(beta1_power),
-                                             float(beta2_power)))
-
-    def get_opt_state(self):
-        m = np.empty(self.param_count, np.float32)
-        v = np.empty(self.param_count, np.float32)
-        st, b1, b2 = C.c_int64(), C.c_float(), C.c_float()
-        N.check(N.lib.drl_r2d2_get_opt_state(self._h, N.ptr(m), N.ptr(v), m.size, C.byref(st), C.byref(b1), C.byref(b2)))
-        return dict(m=m, v=v, step=int(st.value), beta1_power=float(b1.value), beta2_power=float(b2.value))
-
-    def get_grads(self):
-        a = np.empty(self.param_count, np.float32)
-        N.check(N.lib.drl_r2d2_get_grads(self._h, N.ptr(a), a.size))
-        return a
+        self._create(cfg, self.device, num_slots)
 
     def main_to_target(self):
         N.check(N.lib.drl_r2d2_main_to_target(self._h))
@@ -88,7 +36,7 @@ class NativeR2D2Learner:
                 N.as_c(previous_action, np.int32, (n, S), "previous_action"),
                 N.as_c(action, np.int32, (n, S), "action"),
                 N.as_c(h0, np.float32, (n, self.L), "h0"), N.as_c(c0, np.float32, (n, self.L), "c0"),
-                N.as_c(reward, np.float32, (n, S), "reward"), N.as_c(_as_u8(done), np.uint8, (n, S), "done"))
+                N.as_c(reward, np.float32, (n, S), "reward"), N.as_c(N.as_u8(done), np.uint8, (n, S), "done"))
 
     def stage(self, slot, state, previous_action, action, h0, c0, reward, done, weight=None):
         arrs = self._arrays(self.B, state, previous_action, action, h0, c0, reward, done)
@@ -99,16 +47,6 @@ class NativeR2D2Learner:
     @staticmethod
     def _out(o):
         return dict(loss=o.loss, grad_norm=o.grad_norm, step=o.step)
-
-    def step(self, slot=0):
-        self.step_async(slot)
-        return self.wait()
-
-    def step_async(self, slot=0):
-        if dp.distributed():
-            self._dp.step_async(slot)           # data parallel: see dp.py
-        else:
-            N.check(N.lib.drl_r2d2_step_async(self._h, slot))
 
     def wait(self):
         o = N.R2d2Out()
@@ -144,31 +82,3 @@ class NativeR2D2Learner:
         sv = np.empty((n, self.Nt), np.float32)
         N.check(N.lib.drl_r2d2_taps(self._h, N.ptr(mq), N.ptr(tq), N.ptr(tv), N.ptr(sv)))
         return dict(main_q=mq, target_q=tq, target_value=tv, state_action_value=sv)
-
-    def read_buffer(self, name, count):
-        a = np.empty(int(count), np.float32)
-        N.check(N.lib.drl_r2d2_read_buffer(self._h, name.encode(), N.ptr(a), a.size))
-        return a
-
-    def profile_step(self, slot=0, max_kernels=128):
-        names = C.create_string_buffer(8192)
-        ms = np.zeros(max_kernels, np.float32)
-        cnt = C.c_int32()
-        N.check(N.lib.drl_r2d2_profile_step(self._h, slot, names, len(names), N.ptr(ms), max_kernels, C.byref(cnt)))
-        nm = names.value.decode().split("\n") if cnt.value else []
-        return list(zip(nm, [float(x) for x in ms[:cnt.value]]))
-
-    def last_step_ms(self):
-        ms = C.c_float()
-        N.check(N.lib.drl_r2d2_last_step_ms(self._h, C.byref(ms)))
-        return float(ms.value)
-
-    def launches_per_step(self):
-        n = C.c_int32()
-        N.check(N.lib.drl_r2d2_launches_per_step(self._h, C.byref(n)))
-        return int(n.value)
-
-    def stream_ptr(self):
-        s = C.c_void_p()
-        N.check(N.lib.drl_r2d2_stream(self._h, C.byref(s)))
-        return int(s.value or 0)
