@@ -20,7 +20,7 @@ namespace drl {
 constexpr float kBeta1 = 0.9f, kBeta2 = 0.999f, kAdamEps = 1e-8f;
 
 __global__ void __launch_bounds__(256) adam_prepare_kernel(AdamState o) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8];
   const int64_t n4 = o.n / 4;
   const float4* g4 = reinterpret_cast<const float4*>(o.grads);
@@ -54,7 +54,7 @@ __global__ void __launch_bounds__(256) adam_prepare_kernel(AdamState o) {
 }
 
 __global__ void __launch_bounds__(256) adam_apply_kernel(AdamState o) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8];
   __shared__ float s_scale;
   float acc = 0.f;
@@ -244,7 +244,6 @@ int refresh_target_images(AdamLearner* h) {
 
 int enqueue_step(AdamLearner* h, int slot, int* launches) {
   DRL_TRY(h->fwd_bwd(h, slot, launches));
-  pdl_break(h->compute);
   AdamState o = h->opt;
   o.out = h->d_out + 8 * slot;
   prof_mark(h->compute, "optimizer(norm+adam)");
@@ -391,7 +390,6 @@ int adam_main_to_target(AdamLearner* h, const char* family) {
   DRL_TRY(set_device(h));
   DRL_CUDA_CHECK(cudaMemcpyAsync(h->target, h->params, h->layout->padded_total * sizeof(float), cudaMemcpyDeviceToDevice,
                                  h->compute));
-  pdl_break(h->compute);
   h->target_images_stale = true;
   return DRL_OK;
 }
@@ -435,7 +433,6 @@ int adam_apply(AdamLearner* h, const char* family, float grad_scale) {
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   if (!(grad_scale > 0.f)) { set_error("apply: grad_scale must be > 0"); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  pdl_break(h->compute);
   AdamState o = h->opt;
   o.out = h->d_out + 8 * h->last_slot;
   o.grad_scale = grad_scale;

@@ -70,7 +70,7 @@ static SplitPlan plan_head1(int M) { return plan_split(kCat, cdiv(M, CfgMid::BM)
 __global__ void __launch_bounds__(256) apex_hid1_kernel(const float* __restrict__ zpart, int nsplit, size_t slab,
                                                          const float* __restrict__ bv, const float* __restrict__ bm,
                                                          float* __restrict__ hid1, int M) {
-  pdl_prologue();
+  kernel_prologue();
   const int m = blockIdx.x, j = threadIdx.x;
 #pragma unroll
   for (int z = 0; z < 2; ++z) {
@@ -104,7 +104,7 @@ struct TdArgs {
 };
 
 __global__ void __launch_bounds__(256) apex_td_kernel(TdArgs a) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8];
   float part = 0.f;
   for (int b = threadIdx.x; b < a.n; b += blockDim.x) {
@@ -172,7 +172,7 @@ struct A3cArgs {
   float* loss;                                  // [3] pi, baseline, entropy
 };
 __global__ void __launch_bounds__(256) a3c_loss_kernel(A3cArgs a) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[3][8];
   float s_pi = 0.f, s_bl = 0.f, s_en = 0.f;
   const float inv_n = 1.0f / (float)a.n;
@@ -252,13 +252,10 @@ static int apex_forward(const Streams& st, const ApexLayout& pl, const float* P,
   {  // conv1: u8 frames -> a1 (model/apex_value.py:5)
     Conv1A al{frames, map};
     PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b, nullptr};
+    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
     GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
   }
-  if (st.par) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
-    pdl_break(st.main);
-  }
+  if (st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
   {  // conv2 (:6)
     Conv2A al{act.a1, map};
     PlainB bl{P + pl.conv2_w, 64, 0};
@@ -306,7 +303,6 @@ static int apex_forward(const Streams& st, const ApexLayout& pl, const float* P,
 static int apex_backward(const Streams& st, const ApexLayout& pl, const float* P, const WeightImages& wi, float* G,
                          const uint8_t* frames, const int32_t* pa, const ApexActs& act, const ApexBwd& bw, int M, int Mb,
                          int mode, int* launches) {
-  PdlRegionOff pdl_region;
   cudaStream_t s = st.main;
   const cudaStream_t side = st.par ? st.side : st.main;
   const RowMap map{M, 1};
@@ -482,8 +478,6 @@ int alloc_acts(drl_apex* h, ApexActs& a, int cap) {
 
 // forward passes + TD kernel over n transitions held by `sl`; train = also head gradients and the loss
 int enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* td_host, int* launches) {
-  pdl_break(h->compute);
-  pdl_break(h->side);
   const Streams st = h->streams(), tst = h->target_streams();
   if (h->algo == 1) {      // A3C: one scope; rows [0, n) = network(s, prev_a), rows [n, 2n) = network(s', a)
     DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, sl.frames, sl.pa2, h->act, 2 * n, h->mode, h->main_images_stale,
@@ -505,8 +499,6 @@ int enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* 
   if (h->par) {
     DRL_CUDA_CHECK(cudaEventRecord(h->ev_tfork, h->compute));
     DRL_CUDA_CHECK(cudaStreamWaitEvent(h->tmain, h->ev_tfork, 0));
-    pdl_break(h->tmain);
-    pdl_break(h->tside);
   }
   DRL_TRY(apex_forward(tst, h->pl, h->target, h->twi, sl.frames + (size_t)n * Geo::FRAME, sl.pa2 + n, h->tact, n, h->mode,
                        h->target_images_stale, false, true, launches));
@@ -516,10 +508,7 @@ int enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* 
   DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, sl.frames, sl.pa2, h->act, 2 * n, h->mode, h->main_images_stale,
                        h->main_images_stale, false, launches));
   h->main_images_stale = false;
-  if (h->par) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, h->ev_tjoin, 0));
-    pdl_break(h->compute);
-  }
+  if (h->par) DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, h->ev_tjoin, 0));
   TdArgs a{};
   a.vstream = h->act.vstream; a.mstream = h->act.mstream;
   a.tvstream = h->tact.vstream; a.tmstream = h->tact.mstream;
@@ -568,7 +557,6 @@ int forward_main(drl_apex* h, int n, const uint8_t* state, const int32_t* previo
   const ApexIn& s = h->in[h->num_slots];
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   DRL_TRY(stage_into(h, s, h->compute, n, n, state, nullptr, previous_action, nullptr, nullptr, nullptr, nullptr));
-  pdl_break(h->compute);
   DRL_TRY(apex_forward(h->streams(), h->pl, h->params, h->wi, s.frames, s.pa2, h->act, n, h->mode, h->main_images_stale,
                        h->main_images_stale, false, nullptr));
   h->main_images_stale = false;
@@ -732,7 +720,6 @@ int drl_apex_td_error(drl_apex* h, int32_t n, const uint8_t* state, const uint8_
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   // rows [0, n) = s, rows [n, 2n) = s' (packed, so that one main-network forward covers both)
   DRL_TRY(stage_into(h, s, h->compute, n, n, state, next_state, previous_action, action, reward, done, nullptr));
-  pdl_break(h->compute);
   const Streams st = h->streams();
   DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, s.frames, s.pa2, h->act, 2 * n, h->mode, h->main_images_stale,
                        h->main_images_stale, false, nullptr));

@@ -42,23 +42,13 @@ const char* get_error();
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// ---- programmatic dependent launch ----------------------------------------------------
-// The learner step is a chain of ~45 short dependent kernels; between two of them the GPU otherwise idles for the
-// launch latency.  Every kernel of the step starts with pdl_prologue(): `griddepcontrol.wait` blocks until the grid
-// it depends on has completed and flushed (so the usual stream-order semantics hold, including write-after-read),
-// `griddepcontrol.launch_dependents` then lets the NEXT kernel of the stream be scheduled while this one runs, so
-// its CTAs are already resident (parked in their own wait) when this grid drains.  Kernels are launched through
-// launch_k(), which sets the programmatic-stream-serialization attribute only when the previous operation on the
-// stream was another such kernel (pdl_break() marks event waits, copies and API entry points).  Under stream
-// capture the attribute becomes a programmatic edge of the CUDA graph.  DRL_B200_PDL=0 turns the attribute off.
-// Optional start-time trace (drl_debug_trace): when armed, CTA (0,0,0) of every kernel appends
-// {globaltimer ns, grid size << 32 | block size} to a device buffer, which gives the true kernel timeline inside a
+// ---- kernel start-time trace ----------------------------------------------------------
+// Every kernel of the learners starts with kernel_prologue().  When the trace is armed (drl_debug_trace), CTA (0,0,0)
+// appends {globaltimer ns, grid size << 32 | block size} to a device buffer, which gives the true kernel timeline inside a
 // CUDA-graph replay (both streams), something CUDA events cannot do without serialising the graph.  The pointer is a
 // per-translation-unit device global (no relocatable device code); every TU registers a setter at load time.
 static __device__ unsigned long long* g_trace_tu = nullptr;
-__device__ __forceinline__ void pdl_prologue() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+__device__ __forceinline__ void kernel_prologue() {
   unsigned long long* tr = g_trace_tu;
   if (tr != nullptr && threadIdx.x == 0 && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) {
     unsigned long long t;
@@ -74,16 +64,6 @@ typedef void (*TraceSetter)(unsigned long long*);
 int register_trace_setter(TraceSetter f);            // learner.cu
 static void trace_set_tu(unsigned long long* p) { cudaMemcpyToSymbol(g_trace_tu, &p, sizeof(p)); }
 static const int g_trace_registered = register_trace_setter(&trace_set_tu);
-bool& pdl_chain_ok(cudaStream_t s);   // per calling thread: was the last thing enqueued on s a pdl-aware kernel?
-int pdl_level();                      // DRL_B200_PDL: 0 off, 1 every chained launch, 2 outside the backward pass,
-                                      // 3 only launches without dynamic shared memory (the elementwise kernels)
-bool& pdl_region_on();                // per calling thread: false inside the backward pass
-inline void pdl_break(cudaStream_t s) { pdl_chain_ok(s) = false; }
-struct PdlRegionOff {                 // RAII: marks the backward pass
-  bool prev;
-  PdlRegionOff() : prev(pdl_region_on()) { pdl_region_on() = false; }
-  ~PdlRegionOff() { pdl_region_on() = prev; }
-};
 
 template <class... KA, class... A>
 inline cudaError_t launch_k(void (*kern)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, A&&... args) {
@@ -92,16 +72,6 @@ inline cudaError_t launch_k(void (*kern)(KA...), dim3 grid, dim3 block, size_t s
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  bool& ok = pdl_chain_ok(s);
-  const int level = pdl_level();
-  if (ok && (level == 1 || (level == 2 && pdl_region_on()) || (level == 3 && smem == 0))) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-  }
-  ok = true;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KA>(args)...);
 }
 

@@ -7,7 +7,7 @@
 //
 //   TMA warp      one tensor load per frame: the raw 84x84x4 bytes (28,224 B) -> shared memory, double-buffered
 //                 (tensor map {16 B, 21, 84, frames}, box = one frame; the (t,b) -> b*T+t remap of the caller's batch-major
-//                 trajectory buffer is just the box coordinate); the fp16 hi/lo weight image (32 KB) is fetched once
+//                 trajectory buffer is just the box coordinate)
 //   8 converter   expand the im2col FROM SHARED MEMORY: a task (pixel, ky) reads the 32 contiguous bytes of one window row,
 //   warps         turns them into 32 fp16 (exact: PRMT + HSUB2) and writes 4 swizzled 16-byte chunks of a K-major
 //                 SWIZZLE_128B operand stage [128 pixels x 64 features]; 16 stages per frame (4 M tiles x 4 K chunks)
@@ -28,13 +28,19 @@
 #include <map>
 #include <tuple>
 
-#include "gemm_tma.cuh"
 #include "gemm_umma16.cuh"
+#include "gemm_umma_persist.cuh"
 #include "loaders.cuh"
 
 namespace drl {
 
 namespace umma {
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
+}
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
                                             uint64_t* bar) {
   asm volatile(
@@ -66,9 +72,9 @@ struct Conv1Tma {
 
 template <class EP>
 __global__ void __launch_bounds__(Conv1Tma::NT, 1)
-conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __restrict__ wimage,
-                     const float* __restrict__ wf32, const EP ep, RowMap map, int nframes) {
-  pdl_prologue();
+conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const float* __restrict__ wf32, const EP ep, RowMap map,
+                     int nframes) {
+  kernel_prologue();
   using C = Conv1Tma;
   using TA = Umma16Tile<128, true>;
   using TB = Umma16Tile<32, true>;
@@ -100,10 +106,9 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
       umma::mbar_init(&raw_full[b], 1);
       umma::mbar_init(&raw_empty[b], C::CONV_WARPS * 32);
     }
-    // weights: either ONE bulk copy of the pre-tiled image (expect_tx), or -- wf32 != nullptr -- the epilogue warps
-    // build the image from the fp32 HWIO weights themselves while the first frame slab is in flight: the step's first
-    // kernel then has no weight-image kernel in front of it (5 us at the head of every step)
-    umma::mbar_init(w_full, wf32 ? C::EPI_WARPS * 32 : 1);
+    // weights: the epilogue warps build the image from the fp32 HWIO weights themselves while the first frame slab is in
+    // flight: the step's first kernel then has no weight-image kernel in front of it (5 us at the head of every step)
+    umma::mbar_init(w_full, C::EPI_WARPS * 32);
     umma::fence_barrier_init();
   }
   __syncthreads();
@@ -168,25 +173,22 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
     // ================= MMA + EPILOGUE (warps 8..11: one warpgroup) =================
     const int cwarp = warp & 3;
     uint8_t* stg = smem + C::OFF_EPI + cwarp * wg::kEpiWarpBytes;
-    if (wf32) {
-      // [K = 256][N = 32] fp32 -> per K tile of 64: rows 0..31 = fp16(w), rows 32..63 = fp16(w - hi) (K-major, swizzled):
-      // 1024 units of 8 consecutive k of one n; lanes = consecutive n (coalesced 128-byte rows of the HWIO matrix)
-      const int et = tid - C::CONV_WARPS * 32;
-      for (int u = et; u < 32 * 32; u += C::EPI_WARPS * 32) {
-        const int n = u & 31, kb = (u >> 5) * 8;
-        float x[8];
+    // [K = 256][N = 32] fp32 -> per K tile of 64: rows 0..31 = fp16(w), rows 32..63 = fp16(w - hi) (K-major, swizzled):
+    // 1024 units of 8 consecutive k of one n; lanes = consecutive n (coalesced 128-byte rows of the HWIO matrix)
+    for (int u = tid - C::CONV_WARPS * 32; u < 32 * 32; u += C::EPI_WARPS * 32) {
+      const int n = u & 31, kb = (u >> 5) * 8;
+      float x[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) x[i] = __ldg(wf32 + (size_t)(kb + i) * 32 + n);
-        uint4 h, l;
-        umma16::split8<umma16::F16>(make_float4(x[0], x[1], x[2], x[3]), make_float4(x[4], x[5], x[6], x[7]), h, l);
-        uint8_t* dst = wsm + (kb >> 6) * (2 * TB::BYTES);
-        const int off = TB::chunk_off(n, kb & 63);
-        *reinterpret_cast<uint4*>(dst + off) = h;
-        *reinterpret_cast<uint4*>(dst + TB::BYTES + off) = l;
-      }
-      umma::fence_proxy_async();
-      umma::mbar_arrive(w_full);
+      for (int i = 0; i < 8; ++i) x[i] = __ldg(wf32 + (size_t)(kb + i) * 32 + n);
+      uint4 h, l;
+      umma16::split8<umma16::F16>(make_float4(x[0], x[1], x[2], x[3]), make_float4(x[4], x[5], x[6], x[7]), h, l);
+      uint8_t* dst = wsm + (kb >> 6) * (2 * TB::BYTES);
+      const int off = TB::chunk_off(n, kb & 63);
+      *reinterpret_cast<uint4*>(dst + off) = h;
+      *reinterpret_cast<uint4*>(dst + TB::BYTES + off) = l;
     }
+    umma::fence_proxy_async();
+    umma::mbar_arrive(w_full);
     umma::mbar_wait(w_full, 0);
     const uint64_t da_base = umma::make_desc(0, TA::LBO, TA::SBO), db_base = umma::make_desc(0, TB::LBO, TB::SBO);
     float acc0[32], acc1[32];   // pixels 0-63 / 64-127 of the tile x [A W_hi | A W_lo]
@@ -233,10 +235,6 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
     // ================= TMA PRODUCER =================
     if (lane == 0) {
       umma::prefetch_tensormap(&fmap);
-      if (!wf32) {
-        umma::mbar_arrive_expect_tx(w_full, C::W_BYTES);
-        umma::bulk_g2s(wsm, wimage, C::W_BYTES, w_full);
-      }
       int fi = 0;
       for (int mf = blockIdx.x; mf < nframes; mf += gridDim.x, ++fi) {
         const int slot = fi & 1;
@@ -255,6 +253,21 @@ conv1_fwd_tma_kernel(const __grid_constant__ CUtensorMap fmap, const uint8_t* __
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------
+typedef CUresult (*TmaEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline TmaEncodeTiledFn tma_encode_fn() {
+  static TmaEncodeTiledFn fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      p = nullptr;
+    return reinterpret_cast<TmaEncodeTiledFn>(p);
+  }();
+  return fn;
+}
+
 // frames: the staging slot's uint8 [nframes, 84, 84, 4] buffer (caller's batch-major order)
 inline int conv1_frame_map(const uint8_t* frames, int nframes, CUtensorMap* out) {
   TmaEncodeTiledFn enc = tma_encode_fn();
@@ -271,8 +284,8 @@ inline int conv1_frame_map(const uint8_t* frames, int nframes, CUtensorMap* out)
 }
 
 template <class EP>
-inline int launch_conv1_fwd_tma(cudaStream_t s, const uint8_t* frames, int nframes, const RowMap& map, const uint8_t* wimage,
-                                const float* wf32, const EP& ep) {
+inline int launch_conv1_fwd_tma(cudaStream_t s, const uint8_t* frames, int nframes, const RowMap& map, const float* wf32,
+                                const EP& ep) {
   using Key = std::tuple<const uint8_t*, int>;
   static thread_local std::map<Key, CUtensorMap> cache;
   const Key key{frames, nframes};
@@ -289,7 +302,7 @@ inline int launch_conv1_fwd_tma(cudaStream_t s, const uint8_t* frames, int nfram
     attr_done = true;
   }
   const int grid = std::min(nframes, device_sm_count());
-  DRL_CUDA_CHECK((launch_k(kern, grid, Conv1Tma::NT, Conv1Tma::SMEM_BYTES, s, it->second, wimage, wf32, ep, map, nframes)));
+  DRL_CUDA_CHECK((launch_k(kern, grid, Conv1Tma::NT, Conv1Tma::SMEM_BYTES, s, it->second, wf32, ep, map, nframes)));
   return DRL_OK;
 }
 
@@ -341,7 +354,7 @@ __device__ __forceinline__ uint2 u8x4_to_bf4(uint32_t w) {
 static __global__ void __launch_bounds__(Conv1WgTma::NT, 1)
 conv1_wgrad_tma_kernel(const __grid_constant__ CUtensorMap fmap, const float* __restrict__ da1, float* __restrict__ partial,
                        RowMap map, int nframes) {
-  pdl_prologue();
+  kernel_prologue();
   using C = Conv1WgTma;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);

@@ -88,7 +88,6 @@ extern "C" int drl_debug_gemm(int32_t core, int32_t bn, int32_t a_kmajor, int32_
                               int32_t K, int32_t splits, const float* A, const float* B, float* C) {
   if (!A || !B || !C || M < 1 || N < 1 || K < 1 || splits < 1) { set_error("debug_gemm: bad argument"); return DRL_ERR_INVALID; }
   if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
-  pdl_break(0);
   float *dA = nullptr, *dB = nullptr, *dC = nullptr;
   const size_t nA = (size_t)M * K, nB = (size_t)N * K, nC = (size_t)splits * (M + 1) * N;
   DRL_CUDA_CHECK(cudaMalloc(&dA, nA * 4 + 64));

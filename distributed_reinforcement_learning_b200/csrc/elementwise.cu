@@ -17,7 +17,7 @@ namespace drl {
 __global__ void __launch_bounds__(256) emb_forward_kernel(const float* __restrict__ w1, const float* __restrict__ b1,
                                                            const float* __restrict__ w2, const float* __restrict__ b2,
                                                            float* __restrict__ e1, float* __restrict__ table) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float se[Geo::EMB];
   __shared__ float part[4][64];
   const int a = blockIdx.x, tid = threadIdx.x;
@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(256) lstm_gates_forward_kernel(
     const float* __restrict__ zpart, int nsplit, size_t split_stride, const float* __restrict__ bias,
     const float* __restrict__ c0, float* __restrict__ gates, float* __restrict__ c1, float* __restrict__ tc1,
     float* __restrict__ h1, int M, int B, int T) {
-  pdl_prologue();
+  kernel_prologue();
   const int m = blockIdx.x, u = threadIdx.x;
   if (m >= M) return;
   const int t = m / B, b = m - t * B;
@@ -93,7 +93,7 @@ int lstm_gates_forward(cudaStream_t s, const float* zpart, int nsplit, const flo
 __global__ void __launch_bounds__(256) lstm_gates_backward_kernel(
     const float* __restrict__ dh_part, size_t part_stride, const float* __restrict__ gates,
     const float* __restrict__ tc1, const float* __restrict__ c0, float* __restrict__ dz, int Mb, int B, int T) {
-  pdl_prologue();
+  kernel_prologue();
   const int m = blockIdx.x, u = threadIdx.x;
   if (m >= Mb) return;
   const int t = m / B, b = m - t * B;
@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(128) heads_out_forward_kernel(
     const float* __restrict__ ha, const float* __restrict__ hc, const float* __restrict__ w5,
     const float* __restrict__ b5, const float* __restrict__ w8, const float* __restrict__ b8,
     float* __restrict__ logits, float* __restrict__ policy, float* __restrict__ value, int M, int A) {
-  pdl_prologue();
+  kernel_prologue();
   extern __shared__ __align__(16) float sw[];   // W5 [256*A] then w8 [256]
   // Weight staging with every load in flight at once: as a scalar loop this was 36 loads per thread that the compiler
   // issued four at a time -- nine dependent round trips to L2 (~6 us) in front of 2 us of arithmetic.
@@ -210,7 +210,7 @@ __global__ void __launch_bounds__(256) heads_out_backward_kernel(
     const float* __restrict__ dlogits, const float* __restrict__ dv, const float* __restrict__ w5,
     const float* __restrict__ w8, const float* __restrict__ ha, const float* __restrict__ hc,
     float* __restrict__ dha, float* __restrict__ dhc, int Mb, int A) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float sd[kMaxA];
   __shared__ float sdv;
   const int m = blockIdx.x, k = threadIdx.x;
@@ -239,7 +239,7 @@ int heads_out_backward(cudaStream_t s, const float* dlogits, const float* dv, co
 constexpr int kEmbChunks = 16;
 __global__ void __launch_bounds__(256) emb_segsum_kernel(const float* __restrict__ du, const int32_t* __restrict__ pa,
                                                           float* __restrict__ part, int Mb, int B, int T, int A) {
-  pdl_prologue();
+  kernel_prologue();
   const int a = blockIdx.x, c = blockIdx.y, j = threadIdx.x;
   const int per = (Mb + kEmbChunks - 1) / kEmbChunks;
   const int lo = c * per, hi = min(Mb, lo + per);
@@ -253,7 +253,7 @@ __global__ void __launch_bounds__(256) emb_segsum_kernel(const float* __restrict
 // (1b) dpre2[a,j] = relu'(table[a,j]) * sum_c part[c][a][j]   (fixed order)           grid A, 256 threads
 __global__ void __launch_bounds__(256) emb_dpre2_kernel(const float* __restrict__ part, const float* __restrict__ table,
                                                          float* __restrict__ dpre2, int A) {
-  pdl_prologue();
+  kernel_prologue();
   const int a = blockIdx.x, j = threadIdx.x;
   float acc = 0.f;
 #pragma unroll
@@ -263,7 +263,7 @@ __global__ void __launch_bounds__(256) emb_dpre2_kernel(const float* __restrict_
 // (2) g_w2[k,j] = sum_a e1[a,k] dpre2[a,j] ; g_b2[j] = sum_a dpre2[a,j]             grid 256 (k), 256 threads (j)
 __global__ void __launch_bounds__(256) emb_bwd2_kernel(const float* __restrict__ e1, const float* __restrict__ dpre2,
                                                         float* __restrict__ g_w2, float* __restrict__ g_b2, int A) {
-  pdl_prologue();
+  kernel_prologue();
   const int k = blockIdx.x, j = threadIdx.x;
   float acc = 0.f, bs = 0.f;
   for (int a = 0; a < A; ++a) {
@@ -279,7 +279,7 @@ __global__ void __launch_bounds__(256) emb_bwd2_kernel(const float* __restrict__
 __global__ void __launch_bounds__(256) emb_bwd1_kernel(const float* __restrict__ e1, const float* __restrict__ dpre2,
                                                         const float* __restrict__ w2, float* __restrict__ dpre1,
                                                         float* __restrict__ g_w1, float* __restrict__ g_b1, int A) {
-  pdl_prologue();
+  kernel_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k = blockIdx.x * 8 + warp;
   float w[8];
@@ -322,7 +322,7 @@ template <int IH, int IW, int CI, int OH, int OW, int KH, int KW, int S>
 __global__ void __launch_bounds__(256) col2im_relu_kernel(const float* __restrict__ dcol,
                                                            const float* __restrict__ act, float* __restrict__ dx,
                                                            int nimg) {
-  pdl_prologue();
+  kernel_prologue();
   constexpr int C4 = CI / 4, NCOL = KH * KW * CI;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)nimg * IH * IW * C4;
@@ -373,7 +373,7 @@ int col2im_conv2(cudaStream_t s, const float* dcol, const float* a1, float* da1,
 // thread is nsplit/8 loads instead of nsplit (many per-CTA slabs: fewer dependent loads on the critical path).
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ part, size_t slab, int nsplit,
                                                              float* __restrict__ out, size_t n) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8][32];
   const int lane = threadIdx.x & 31, g = threadIdx.x >> 5;
   const size_t j = (size_t)blockIdx.x * 32 + lane;

@@ -42,7 +42,7 @@ struct ImageOp {
 template <class Cfg, class EP>
 __global__ void __launch_bounds__(Cfg::NT, 1)
 gemm_bulk16_kernel(const ImageOp a, const ImageOp b, const EP ep, int M, int N, int K, int kchunk, int kstep) {
-  pdl_prologue();
+  kernel_prologue();
   const Trace16 TR = trace16_arm();   // tools/umma16_timeline.py: same tags as gemm_umma16_kernel
   if (threadIdx.x == 0) TR((1ull << 40) | ((unsigned long long)gridDim.x << 20) | (gridDim.y * gridDim.z * 1024 + (Cfg::BN & 1023)));
   constexpr int BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES;

@@ -50,7 +50,7 @@ struct SmemLayout {
 template <class Cfg, class AL, class BL, class EP, int KS = 1>
 __global__ void __launch_bounds__(Cfg::NT * KS)
 gemm_simt_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int kchunk, int kstep) {
-  pdl_prologue();
+  kernel_prologue();
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, TM = Cfg::TM, TN = Cfg::TN;
   constexpr int NT = Cfg::NT, TX = Cfg::TX, QM = Cfg::QM, QN = Cfg::QN;
   constexpr bool AK = AL::kContigK, BKc = BL::kContigK;

@@ -20,7 +20,6 @@
 //               accumulator, keeps one stage of MMAs in flight and hands the previous stage back (empty[stage]).
 //               After the last K tile it drains the accumulator through a swizzled shared tile (wg_epilogue) into the
 //               epilogue functor (bias/ReLU/mask/split-K partial ...).
-// gemm_tma.cuh holds the TMA-fed variant (cp.async.bulk.tensor im2col boxes) for the conv2/conv3 forward.
 //
 // Canonical SWIZZLE_128B K-major layout (CuTe GMMA::Layout_K_SW128_Atom), BK = 32 floats: row r is 128 contiguous
 // bytes (32 floats of K) at r*128; the 16-byte chunk c of row r is stored at chunk position c ^ (r & 7)
@@ -305,7 +304,7 @@ __device__ __forceinline__ void tf32_stage_mmas(float (&acc)[BN / 2], uint32_t a
 template <class Cfg, class AL, class BL, class EP>
 __global__ void __launch_bounds__(Cfg::NT, Cfg::MINB)
 gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int kchunk, int kstep) {
-  pdl_prologue();
+  kernel_prologue();
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES, NPROD = Cfg::NPROD;
   constexpr bool AK = AL::kContigK, BKc = BL::kContigK;
   using SM = UmmaSmem<Cfg, AL, BL>;
@@ -562,7 +561,7 @@ gemm_umma_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int
 template <int BN, class BL>
 __global__ void __launch_bounds__(256) retile_b_kernel(const BL bl, int N, int K, int ktiles, int ntn,
                                                         uint8_t* __restrict__ image) {
-  pdl_prologue();
+  kernel_prologue();
   using TB = UmmaTile<BN, BL::kContigK>;
   constexpr int GPT = BN * 8;                         // float4 groups per tile (BN rows x 32 floats)
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;

@@ -170,7 +170,7 @@ __device__ __forceinline__ Trace16 trace16_arm() {
 template <class Cfg, class AL, class BL, class EP>
 __global__ void __launch_bounds__(Cfg::NT, Cfg::MINB)
 gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int kchunk, int kstep) {
-  pdl_prologue();
+  kernel_prologue();
   const Trace16 TR = trace16_arm();
   if (threadIdx.x == 0) TR((1ull << 40) | ((unsigned long long)gridDim.x << 20) | (gridDim.y * gridDim.z * 1024 + Cfg::BN));
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, SUBK = Cfg::SUBK, STAGES = Cfg::STAGES, NPROD = Cfg::NPROD;
@@ -511,7 +511,7 @@ __device__ __forceinline__ float b_elem(const BL& bl, int n, int k) {
 template <int BN, class F, class BL>
 __global__ void __launch_bounds__(256) retile_b16_kernel(const BL bl, int N, int K, int ktiles, int ntn,
                                                           uint8_t* __restrict__ image) {
-  pdl_prologue();
+  kernel_prologue();
   using TB = Umma16Tile<BN, true>;
   constexpr int UPT = BN * 8;                        // 8-element units per tile (BN rows x 64 elements)
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -541,7 +541,7 @@ template <int BN, class F, class BL>
 __global__ void __launch_bounds__(256) retile_t16_kernel(const BL bl, int N, int K, int ktiles, int ntn,
                                                           uint8_t* __restrict__ image) {
   static_assert(!BL::kContigK, "transposing variant: the loader's row index is contiguous in memory");
-  pdl_prologue();
+  kernel_prologue();
   using TB = Umma16Tile<BN, true>;
   constexpr int UPT = (BN / 4) * 8;                  // (4-row group, 8-k group) units per tile
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;

@@ -35,7 +35,7 @@ template <class Cfg, class AL, class BL, class EP>
 __global__ void __launch_bounds__(Cfg::NT, 1)
 gemm_umma_persist_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, int kchunk, int kstep,
                          int mtiles, int ntn, int total_tiles) {
-  pdl_prologue();
+  kernel_prologue();
   constexpr int BM = Cfg::BM, BN = Cfg::BN, BK = Cfg::BK, STAGES = Cfg::STAGES, NPROD = Cfg::NPROD, PW = Cfg::PW;
   constexpr bool AK = AL::kContigK, BKc = BL::kContigK;
   using SM = UmmaSmem<Cfg, AL, BL>;

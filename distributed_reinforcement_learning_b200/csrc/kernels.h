@@ -84,9 +84,7 @@ struct Inputs {          // one device staging slot, caller's batch-major layout
 
 struct Acts {            // forward activations, time-major rows m = t*B + b, M = B*T rows
   float* a1;             // [M,20,20,32]
-  float* a1_lo;          // tf32 remainder plane of a1 (same shape), allocated right behind a1: TMA operand of conv2
   float* a2;             // [M,9,9,64]
-  float* a2_lo;          // same for a2 (conv3)
   float* a3;             // [M,3136]
   float* e1;             // [A,256]  relu(emb1)
   float* table;          // [A,256]  action-embedding table
@@ -100,9 +98,8 @@ struct Acts {            // forward activations, time-major rows m = t*B + b, M 
   float* logits;         // [M,A]
   float* policy;         // [M,A]
   float* value;          // [M]
-  // math mode 5, bulk-fed lstm_wgrad (gemm_bulk16.cuh): x^T = [a3|emb|h0]^T as a 16-bit operand image, nullptr = gather path
+  // math mode 5, bulk-fed lstm_wgrad (gemm_bulk16.cuh): x^T = [a3|emb|h0]^T as a 16-bit operand image
   uint8_t* img_xt = nullptr;   // x^T : rows = features (3648) x K = Mb rows -- A operand of lstm_wgrad
-  int img_rows = 0;            // M the images were sized for
 };
 
 struct Bwd {             // backward workspace, Mb = B*(T-2) rows
@@ -122,7 +119,7 @@ struct Bwd {             // backward workspace, Mb = B*(T-2) rows
   float* wg_part;        // split-K partial slabs for the conv3/conv2 weight gradients (side stream) + emb scratch
   float* wg_part2;       // split-K partial slabs for the conv1 weight gradient (main stream)
   float* dcol = nullptr; // [Mb*81, 512] (conv2) / [Mb*49, 576] (conv3): per-output-pixel tap gradients before col2im
-                         // (math modes 2-4; math mode 5 computes the conv data gradients without it)
+                         // (math modes 2 and 3; math mode 5 computes the conv data gradients without it)
   size_t wg_part_floats;
   float* emb_scratch = nullptr;   // own scratch of emb_backward (16 * 32 * 256 floats): lets it run on the second side lane
                                   // beside the conv weight gradients; nullptr: it borrows wg_part on `side`
@@ -138,9 +135,6 @@ struct VtraceOut {       // parity taps, batch-major [B, T-2]
 constexpr int kLstmSplits = 8;   // slabs allocated for the LSTM split-K partial sums (4 or 7 are used)
 
 // math_mode 0 in drl_learner_config resolves to this (1 = FP32 FFMA, 2 = wgmma 3xTF32)
-#ifndef DRL_DEFAULT_PDL_LEVEL
-#define DRL_DEFAULT_PDL_LEVEL 0   // programmatic dependent launch (common.cuh); see DESIGN.md for the measurements
-#endif
 #ifndef DRL_DEFAULT_MATH_MODE
 #define DRL_DEFAULT_MATH_MODE 2          // Ape-X / A3C / R2D2 handles
 #endif
@@ -160,7 +154,9 @@ int prof_end(cudaStream_t s, int rc, char* names, int64_t names_len, float* ms, 
 // tensor-core GEMMs (gemm_umma.cuh: PretiledB / retile_b_kernel); refreshed after every parameter update.
 struct WeightImages {
   static constexpr int kCount = 7;
-  uint8_t* img[kCount];   // 0 conv1 fwd, 1 conv2 fwd, 2 conv3 fwd, 3 lstm fwd, 4 lstm dgrad, 5 conv3 dCol, 6 conv2 dCol
+  // 0 conv1 fwd (no reader: every conv1 kernel reads the fp32 weights; kept because the Ape-X / R2D2 handles size their
+  // images with the same weight_image_sizes), 1 conv2 fwd, 2 conv3 fwd, 3 lstm fwd, 4 lstm dgrad, 5 conv3 dCol, 6 conv2 dCol
+  uint8_t* img[kCount];
 };
 void weight_image_sizes(size_t (&bytes)[WeightImages::kCount]);
 int net_retile(cudaStream_t s_conv, cudaStream_t s_rest, const ParamLayout& pl, const float* params,

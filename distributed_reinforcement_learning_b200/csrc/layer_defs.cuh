@@ -9,7 +9,6 @@
 #include "gemm_umma16.cuh"
 #include "conv1_tma.cuh"
 #include "gemm_bulk16.cuh"
-#include "gemm_tma.cuh"
 #include "gemm_umma_persist.cuh"
 #include "kernels.h"
 #include "loaders.cuh"
@@ -22,12 +21,6 @@ namespace drl {
 using Conv1A = ConvFwdA<uint8_t, 84, 84, 4, 20, 20, 8, 4, true>;
 using Conv2A = ConvFwdA<float, 20, 20, 32, 9, 9, 4, 2, false>;
 using Conv3A = ConvFwdA<float, 9, 9, 64, 7, 7, 3, 1, false>;
-// math mode 4: TMA-fed forward of conv2 / conv3 (gemm_tma.cuh): tiles of 1 image (81 rows) / 2 images (98 rows), 4 stages.
-// With 32/64 input channels a K tile is one filter tap, so every activation byte is fetched 4x (conv2) / 9x (conv3) from
-// L2 for each of the two planes plus a weight tile per tap and image: more L2->SM bytes than the LDG path, which reads
-// raw fp32 once per tap and splits in registers.
-using Conv2Tma = ConvTmaCfg<32, 20, 9, 4, 2, 1, 4>;
-using Conv3Tma = ConvTmaCfg<64, 9, 7, 3, 1, 2, 4>;
 using Conv1WA = ConvWgradA<uint8_t, 84, 84, 4, 20, 20, 8, 4, true>;
 using Conv2WA = ConvWgradA<float, 20, 20, 32, 9, 9, 4, 2, false>;
 using Conv3WA = ConvWgradA<float, 9, 9, 64, 7, 7, 3, 1, false>;
@@ -54,24 +47,19 @@ using U256L = U256;                    // (no loader warp: the same configuratio
 
 // math mode 5: 16-bit split operands (gemm_umma16.cuh).  One format per GEMM (f16 x bf16 traps).  bf16 keeps fp32's
 // exponent range (gradients span many decades); fp16 has three more mantissa bits but underflows gradually below ~1e-4
-// and saturates at 65504 -- it is used where one operand is EXACT in it (the uint8 frames of conv1) and the other is
-// an O(0.1) weight.
+// and saturates at 65504 -- conv1 (conv1_tma.cuh) uses it because one operand is EXACT in it (the uint8 frames) and the
+// other is an O(0.1) weight.
 using Fmt16 = umma16::BF16;     // every GEMM whose operands are fp32 activations / gradients / weights
-using FmtC1 = umma16::F16;      // conv1: uint8 frames (exact) x weights
-using X32L = Umma16Cfg<32, 4, 1, 4, 1, FmtC1, FmtC1>;        // conv1 fwd: whole K = 256 resident
-using X64L = Umma16Cfg<64, 2, 1, 4, 1, Fmt16, Fmt16>;        // conv2 / conv3 fwd: 48 KB per K = 64 stage
-using X64L8x2 = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16>;     // conv2 / conv3 fwd (default): 8 producer warps = twice the loads in flight of
-                                                             // X64L (the gathers are latency-bound); DRL_B200_C2F=0: X64L
-using X64W8x2 = Umma16Cfg<64, 2, 1, 8, 0, Fmt16, Fmt16>;     // conv2 / conv3 weight gradients (default); DRL_B200_CW8=0: X64W
-using X64W = Umma16Cfg<64, 2, 1, 4, 0, Fmt16, Fmt16>;        // conv2 / conv3 weight gradients (both operands gathered)
-using XH = Umma16Cfg<64, 4, 1, 8, 0, Fmt16, Fmt16>;          // head layers (K = 256 = all four stages in flight), DRL_B200_HEADS_TC=1
+using X64L8x2 = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16>;     // conv2 / conv3 fwd: 48 KB per K = 64 stage, 8 producer warps
+                                                             // (the gathers are latency-bound)
+using X64W8x2 = Umma16Cfg<64, 2, 1, 8, 0, Fmt16, Fmt16>;     // conv2 / conv3 weight gradients (both operands gathered)
+using XH = Umma16Cfg<64, 4, 1, 8, 0, Fmt16, Fmt16>;          // head layers (K = 256 = all four stages in flight)
 // bulk-fed LSTM weight gradient (gemm_bulk16.cuh): both operands are pre-tiled images, no producer warps
 using BK256 = Bulk16Cfg<256, 2>;       // 96 KB per stage (A 32 KB + B 64 KB), 2 stages
 using X256L = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm fwd: 96 KB per stage
-using X256W = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm weight gradient
 using X128D = Umma16Cfg<128, 3, 1, 8, 1, Fmt16, Fmt16>;      // lstm data gradient: 64 KB per stage
 // conv data gradients (pre-tiled B, one K tile of 64 co per filter tap): per-tap partial sums added in tap order, the
-// rounding of the dCol GEMM + col2im of math modes 2-4.  The second register set costs conv2 (BN = 128) its loader warp
+// rounding of the dCol GEMM + col2im of math modes 2 and 3.  The second register set costs conv2 (BN = 128) its loader warp
 // and half its producer warps (384 threads: 170 registers each).
 using X64T = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16, 0, true>;    // conv3: K = 9 taps x 64 co, N = 64 ci
 using X128T = Umma16Cfg<128, 3, 1, 4, 0, Fmt16, Fmt16, 0, true>;  // conv2: K = 4 taps x 64 co, N = 4 parity classes x 32 ci
@@ -125,14 +113,11 @@ template <> struct PersistOf<U128L> { using type = UmmaPCfg<128, 3, 8>; };
     DRL_TRY((launch_gemm_simt<SCfg>(s, __VA_ARGS__)));       \
     ++n;                                                     \
   } while (0)
-// the small dense layers of the heads: in-CTA split-K (KS groups work on the K tiles of one output tile concurrently);
-// DRL_B200_HEADS_KS=1 restores the one-group kernel
+// the small dense layers of the heads: in-CTA split-K (KS groups work on the K tiles of one output tile concurrently)
 #define GEMM_FFMA_KS(name, SCfg, KS, ...)                      \
   do {                                                       \
-    static const int ks_env = getenv("DRL_B200_HEADS_KS") ? atoi(getenv("DRL_B200_HEADS_KS")) : 0; \
     prof_mark(s, name);                                      \
-    if (ks_env == 1) DRL_TRY((launch_gemm_simt<SCfg>(s, __VA_ARGS__)));  \
-    else DRL_TRY((launch_gemm_simt<SCfg, KS>(s, __VA_ARGS__)));        \
+    DRL_TRY((launch_gemm_simt<SCfg, KS>(s, __VA_ARGS__)));   \
     ++n;                                                     \
   } while (0)
 #define KERNEL(name, call, cnt)                              \
@@ -175,7 +160,6 @@ static inline int fork_to_side(const Streams& st, int i) {
   if (!st.par) return DRL_OK;
   DRL_CUDA_CHECK(cudaEventRecord(st.ev[i], st.main));
   DRL_CUDA_CHECK(cudaStreamWaitEvent(st.side, st.ev[i], 0));
-  pdl_break(st.side);   // the next side-stream kernel depends on a kernel of another stream: full dependency
   return DRL_OK;
 }
 // main -> side2 edge (ev2[i]); side2 -> other stream edge
@@ -183,21 +167,18 @@ static inline int fork_to_side2(const Streams& st, int i) {
   if (!st.par || !st.side2) return DRL_OK;
   DRL_CUDA_CHECK(cudaEventRecord(st.ev2[i], st.main));
   DRL_CUDA_CHECK(cudaStreamWaitEvent(st.side2, st.ev2[i], 0));
-  pdl_break(st.side2);
   return DRL_OK;
 }
 static inline int join_side2_into(const Streams& st, int i, cudaStream_t into) {
   if (!st.par || !st.side2) return DRL_OK;
   DRL_CUDA_CHECK(cudaEventRecord(st.ev2[i], st.side2));
   DRL_CUDA_CHECK(cudaStreamWaitEvent(into, st.ev2[i], 0));
-  pdl_break(into);
   return DRL_OK;
 }
 static inline int join_from_side(const Streams& st, int i) {
   if (!st.par) return DRL_OK;
   DRL_CUDA_CHECK(cudaEventRecord(st.ev[i], st.side));
   DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[i], 0));
-  pdl_break(st.main);
   return DRL_OK;
 }
 

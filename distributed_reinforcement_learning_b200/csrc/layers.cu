@@ -3,9 +3,7 @@
 // time is embarrassingly parallel; only T distinct forwards exist, SURVEY.md section 0.3).
 // Every dense contraction is one launch of a gather-GEMM: the FP32-FFMA core (gemm_simt.cuh, math
 // mode 1) or the wgmma 3xTF32 tensor-core core (gemm_umma.cuh, math mode 2) -- same loaders and
-// epilogues.  The small head layers (M x 256 x 256) always use the FFMA core.
-#include <stdlib.h>
-
+// epilogues.  Outside math mode 5 the small head layers (M x 256 x 256) use the FFMA core.
 #include "layer_defs.cuh"
 
 namespace drl {
@@ -69,7 +67,7 @@ void weight_image_sizes(size_t (&b)[WeightImages::kCount]) {
   b[2] = weight_image_bytes<64>(64, 576);
   b[3] = weight_image_bytes<256>(Geo::G4, Geo::XK);
   b[4] = weight_image_bytes<128>(Geo::FLAT + Geo::EMB, Geo::G4);
-  b[5] = weight_image_bytes<256>(576, 64);   // the dCol operands of math modes 2-4; larger than the 16-bit dgrad images
+  b[5] = weight_image_bytes<256>(576, 64);   // the dCol operands of math modes 2 and 3; larger than the 16-bit dgrad images
   b[6] = weight_image_bytes<256>(512, 64);   // of math mode 5 (weight_image16_bytes<64>(64, 576), <128>(128, 256))
 }
 
@@ -105,8 +103,6 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
   const int M = B * T;
   const RowMap map{B, T};
   int n = 0, nsplit = 4;
-  const bool tma = mode == 4;
-  if (mode == 4) mode = 2;
   cudaStream_t s = st.main;
   const cudaStream_t side = st.par ? st.side : st.main;
   // action embedding table (:12-16): only A distinct inputs exist; depends on parameters only -> side stream
@@ -116,19 +112,9 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
   // for them behind conv1), the LSTM / dgrad ones behind the embedding table (joined before lstm_fwd)
   const bool m16 = mode == 5;
   bool c3_event = false;   // conv3's weight image has its own event (math mode 5)
-  static const bool heads_tc = !(getenv("DRL_B200_HEADS_TC") && atoi(getenv("DRL_B200_HEADS_TC")) == 0);   // head layers on tensor cores (0: FFMA)
-  // math mode 5: conv1 is the frame-resident TMA kernel (conv1_tma.cuh), which builds its 32 KB weight image itself;
-  // DRL_B200_CONV1_GATHER=1 keeps the generic gather-GEMM, DRL_B200_C1_WIMG=1 the pre-tiled image (one more kernel in
-  // front of the step's first kernel)
-  static const bool c1_gather = getenv("DRL_B200_CONV1_GATHER") != nullptr;
-  static const bool c1_wimg = c1_gather || getenv("DRL_B200_C1_WIMG") != nullptr;
+  // math mode 5: conv1 is the frame-resident TMA kernel (conv1_tma.cuh), which builds its 32 KB weight image itself
   if (retile && m16) {
     prof_mark(s, "weight_retile");
-    if (c1_wimg) {
-      DRL_TRY((launch_retile_b16<32, FmtC1>(s, PlainB{P + pl.conv1_w, 32, 0}, 32, 256, wi.img[0])));
-      if (st.par) DRL_CUDA_CHECK(cudaEventRecord(st.ev[2], side));        // conv1 waits for its (tiny) image
-      ++n;
-    }
     DRL_TRY((launch_retile_b16<64, Fmt16>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, wi.img[1])));
     if (st.par) DRL_CUDA_CHECK(cudaEventRecord(st.ev[7], side));          // conv2 image (main waits behind conv1)
     DRL_TRY((launch_retile_b16<64, Fmt16>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, wi.img[2])));
@@ -161,68 +147,41 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     }
     n += 4;
   }
-  if (retile && m16 && st.par && c1_wimg) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[2], 0));
-    pdl_break(st.main);
-  }
   // conv1: u8 frames -> a1 [M,20,20,32]   (attention_CNN, model/impala_actor_critic.py:6)
   {
-    Conv1A al{in.frames, map};
-    PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b, tma ? act.a1_lo : nullptr};
-    if (m16 && !c1_gather) {
+    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
+    if (m16) {
       prof_mark(s, "conv1_fwd");
-      DRL_TRY(launch_conv1_fwd_tma(s, in.frames, M, map, wi.img[0], c1_wimg ? nullptr : P + pl.conv1_w, ep));
+      DRL_TRY(launch_conv1_fwd_tma(s, in.frames, M, map, P + pl.conv1_w, ep));
       ++n;
-    } else if (m16) {
-      PretiledB<PlainB> blp{wi.img[0], 256 / 64};
-      GEMM16("conv1_fwd", X32L, al, blp, ep, M * 400, 32, 256, 1, 256, 0);
     } else {
+      Conv1A al{in.frames, map};
+      PlainB bl{P + pl.conv1_w, 32, 0};
       GEMM("conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
     }
   }
-  if (retile && mode >= 2 && st.par) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
-    pdl_break(st.main);
-  }
+  if (retile && mode >= 2 && st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
   // conv2 -> a2 [M,9,9,64]   (:7)
-  if (tma) {
-    EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f, act.a2_lo};
-    KERNEL("conv2_fwd", (launch_conv_fwd_tma<Conv2Tma>(s, act.a1, (size_t)(act.a1_lo - act.a1), M, wi.img[1], ep)), 1);
-  } else {
+  {
     Conv2A al{act.a1, map};
     PlainB bl{P + pl.conv2_w, 64, 0};
     PretiledB<PlainB> blp{wi.img[1], m16 ? 512 / 64 : 512 / 32};
     EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    static const int c2f = getenv("DRL_B200_C2F") ? atoi(getenv("DRL_B200_C2F")) : 2;
-    if (m16 && c2f == 2) GEMM16("conv2_fwd", X64L8x2, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
-    else if (m16) GEMM16("conv2_fwd", X64L, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
+    if (m16) GEMM16("conv2_fwd", X64L8x2, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
     else GEMM_W("conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
   }
-  if (c3_event) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[4], 0));
-    pdl_break(st.main);
-  }
+  if (c3_event) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[4], 0));
   // conv3 -> a3 [M,7,7,64] = flatten HWC [M,3136]   (:8-10)
-  if (tma) {
-    EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    KERNEL("conv3_fwd", (launch_conv_fwd_tma<Conv3Tma>(s, act.a2, (size_t)(act.a2_lo - act.a2), M, wi.img[2], ep)), 1);
-  } else {
+  {
     Conv3A al{act.a2, map};
     PlainB bl{P + pl.conv3_w, 64, 0};
     PretiledB<PlainB> blp{wi.img[2], m16 ? 576 / 64 : 576 / 32};
     EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    static const int c3f = getenv("DRL_B200_C2F") ? atoi(getenv("DRL_B200_C2F")) : 2;
-    if (m16 && c3f == 2) GEMM16("conv3_fwd", X64L8x2, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
-    else if (m16) GEMM16("conv3_fwd", X64L, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
+    if (m16) GEMM16("conv3_fwd", X64L8x2, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
     else GEMM_W("conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
   }
-  if (late_images) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[1], 0));
-    pdl_break(st.main);
-  } else {
-    DRL_TRY(join_from_side(st, 1));
-  }
+  if (late_images) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[1], 0));
+  else DRL_TRY(join_from_side(st, 1));
   // LSTM pre-activation z = [a3 | emb | h0] W  (split-K partial sums; bias added in the gate kernel) (:18-25)
   {
     LstmA al{act.a3, act.table, in.pa, in.h0, map};
@@ -251,14 +210,14 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     PlainA al{act.h1, Geo::L, 0};
     PlainB bl{P + pl.actor1_w, Geo::HID, head_stride};
     EpBiasAct<true, true> ep{act.hid1, Geo::HID, (size_t)M * Geo::HID, P + pl.actor1_b, head_stride, 1.0f};
-    if (m16 && heads_tc) GEMM16("heads_l1_fwd", XH, al, bl, ep, M, Geo::HID, Geo::L, 2, Geo::L, 0);
+    if (m16) GEMM16("heads_l1_fwd", XH, al, bl, ep, M, Geo::HID, Geo::L, 2, Geo::L, 0);
     else GEMM_FFMA("heads_l1_fwd", CfgSmall, al, bl, ep, M, Geo::HID, Geo::L, 2, Geo::L, 0);
   }
   {
     PlainA al{act.hid1, Geo::HID, (size_t)M * Geo::HID};
     PlainB bl{P + pl.actor2_w, Geo::HID, head_stride};
     EpBiasAct<true, true> ep{act.hid2, Geo::HID, (size_t)M * Geo::HID, P + pl.actor2_b, head_stride, 1.0f};
-    if (m16 && heads_tc) GEMM16("heads_l2_fwd", XH, al, bl, ep, M, Geo::HID, Geo::HID, 2, Geo::HID, 0);
+    if (m16) GEMM16("heads_l2_fwd", XH, al, bl, ep, M, Geo::HID, Geo::HID, 2, Geo::HID, 0);
     else GEMM_FFMA("heads_l2_fwd", CfgSmall, al, bl, ep, M, Geo::HID, Geo::HID, 2, Geo::HID, 0);
   }
   KERNEL("heads_out_fwd",
@@ -271,10 +230,7 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
 
 int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const WeightImages& wi, float* G,
                  const Inputs& in, const Acts& act, const Bwd& bw, int B, int T, int mode) {
-  PdlRegionOff pdl_region;   // DRL_B200_PDL=2: no early launches while the side stream competes for the same SMs
-  if (mode == 4) mode = 2;
   const bool m16 = mode == 5;
-  static const bool heads_tc = !(getenv("DRL_B200_HEADS_TC") && atoi(getenv("DRL_B200_HEADS_TC")) == 0);   // head layers on tensor cores (0: FFMA)
   cudaStream_t s = st.main;
   const cudaStream_t side = st.par ? st.side : st.main;
   const int M = B * T;
@@ -288,8 +244,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
   KERNEL("heads_out_bwd",
          heads_out_backward(s, bw.dlogits, bw.dv, P + pl.actor3_w, P + pl.critic3_w, act.hid2,
                             act.hid2 + (size_t)M * Geo::HID, bw.dhid2, bw.dhid2 + (size_t)Mb * Geo::HID, Mb, A), 1);
-  const bool lbulk = m16 && act.img_xt != nullptr && bw.img_dzt != nullptr && M <= act.img_rows;   // bulk-fed lstm_wgrad
-  if (lbulk) {
+  if (m16) {
     // x^T as an operand image (A of lstm_wgrad): depends on the forward pass only -> side stream, in the shadow of the
     // small head kernels
     DRL_TRY(fork_to_side(st, 0));
@@ -326,7 +281,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     PlainA al{bw.dhid2, Geo::HID, (size_t)Mb * Geo::HID};
     PlainBT bl{P + pl.actor2_w, Geo::HID, head_stride};
     EpReluMask ep{bw.dhid1, act.hid1, Geo::HID, (size_t)Mb * Geo::HID, (size_t)M * Geo::HID};
-    if (m16 && heads_tc) GEMM16("heads_l2_dgrad", XH, al, bl, ep, Mb, Geo::HID, Geo::HID, 2, Geo::HID, 0);
+    if (m16) GEMM16("heads_l2_dgrad", XH, al, bl, ep, Mb, Geo::HID, Geo::HID, 2, Geo::HID, 0);
     else GEMM_FFMA_KS("heads_l2_dgrad", CfgSmall, 4, al, bl, ep, Mb, Geo::HID, Geo::HID, 2, Geo::HID, 0);
   }
   if (lane2) DRL_TRY(fork_to_side2(st, 1));
@@ -343,7 +298,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     PlainA al{bw.dhid1, Geo::HID, (size_t)Mb * Geo::HID};
     PlainBT bl{P + pl.actor1_w, Geo::HID, head_stride};
     EpRaw<false> ep{bw.dh_part, Geo::L, (size_t)Mb * Geo::L, 1.0f, 0, Geo::L};
-    if (m16 && heads_tc) GEMM16("heads_l1_dgrad", XH, al, bl, ep, Mb, Geo::L, Geo::HID, 2, Geo::HID, 0);
+    if (m16) GEMM16("heads_l1_dgrad", XH, al, bl, ep, Mb, Geo::L, Geo::HID, 2, Geo::HID, 0);
     else GEMM_FFMA_KS("heads_l1_dgrad", CfgSmall, 4, al, bl, ep, Mb, Geo::L, Geo::HID, 2, Geo::HID, 0);
   }
   // ---- LSTM cell ---------------------------------------------------------------------------
@@ -352,10 +307,8 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
   DRL_TRY(fork_to_side(st, 3));
   s = side;
   {  // d lstm kernel [3648(+1), 1024] = x^T dz ; bias gradient = column sums of dz
-    LstmAT al{act.a3, act.table, in.pa, in.h0, map};
     PlainB bl{bw.dz, Geo::G4, 0};
-    EpRaw<true> ep{G + pl.lstm_w, Geo::G4, 0, 1.0f, Geo::XK, Geo::G4};
-    if (lbulk) {
+    if (m16) {
       const int ktm = cdiv(Mb, 64);
       prof_mark(s, "lstm_dzt_image");
       DRL_TRY((launch_retile_t16<256, Fmt16>(s, bl, Geo::G4, Mb, bw.img_dzt)));
@@ -366,8 +319,11 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
       DRL_TRY((launch_gemm_bulk16<BK256>(s, ImageOp{act.img_xt, ktm}, ImageOp{bw.img_dzt, ktm}, epw, Geo::XK, Geo::G4, Mb,
                                          1, Mb, 0)));
       n += 3;
-    } else if (m16) GEMM16("lstm_wgrad", X256W, al, bl, ep, Geo::XK, Geo::G4, Mb, 1, Mb, 0);
-    else GEMM("lstm_wgrad", CfgBig, U256, al, bl, ep, Geo::XK, Geo::G4, Mb, 1, Mb, 0);   // 29 x 4 = 116 CTAs: one wave
+    } else {
+      LstmAT al{act.a3, act.table, in.pa, in.h0, map};
+      EpRaw<true> ep{G + pl.lstm_w, Geo::G4, 0, 1.0f, Geo::XK, Geo::G4};
+      GEMM("lstm_wgrad", CfgBig, U256, al, bl, ep, Geo::XK, Geo::G4, Mb, 1, Mb, 0);   // 29 x 4 = 116 CTAs: one wave
+    }
     // the head gradients (earlier on this stream, or on the second lane: joined here) and the LSTM gradient are now
     // in the bucket: [lstm_w .. end)
     if (lane2) DRL_TRY(join_side2_into(st, 2, side));
@@ -387,10 +343,8 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
   // in the graph).  On one GPU they stay in front of conv3_wgrad on `side` (the second lane measured 0.4 % slower: the
   // backward pass is throughput-bound, earlier weight gradients only take SMs from the main chain).  With the fused peer
   // exchange the side stream IS the tail of the step (the early exchange part competes with it), and moving them to the
-  // second lane (own scratch) gains 1 % at 2 GPUs.  DRL_B200_EMB_SIDE2=0/1 forces either.
-  static const int emb_lane2_env = getenv("DRL_B200_EMB_SIDE2") ? atoi(getenv("DRL_B200_EMB_SIDE2")) : -1;
-  const bool emb2 = lane2 && bw.emb_scratch != nullptr &&
-                    (emb_lane2_env == 1 || (emb_lane2_env < 0 && st.ev_lstm_grads != nullptr));
+  // second lane (own scratch) gains 1 % at 2 GPUs.
+  const bool emb2 = lane2 && bw.emb_scratch != nullptr && st.ev_lstm_grads != nullptr;
   if (emb2) {
     DRL_TRY(fork_to_side2(st, 3));
     s = st.side2;
@@ -411,9 +365,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     Conv3WA al{act.a2, map};
     PlainB bl{bw.da3, 64, 0};
     EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 576, 64};
-    static const int cw8 = getenv("DRL_B200_CW8") ? atoi(getenv("DRL_B200_CW8")) : 1;
-    if (m16 && cw8) GEMM16("conv3_wgrad", X64W8x2, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
-    else if (m16) GEMM16("conv3_wgrad", X64W, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
+    if (m16) GEMM16("conv3_wgrad", X64W8x2, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
     else GEMM("conv3_wgrad", CfgBig, U64, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
     KERNEL("conv3_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv3_w, slab), 1);
   }
@@ -421,7 +373,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
   if (m16) {
     // gather form: rows = input pixels, K = 9 taps x 64 output channels (taps outside the output are zero), ReLU mask of
     // a2 in the epilogue; each tap's partial sum is rounded to fp32 and the taps are added in (ky, kx) order, as
-    // col2im_conv3 adds the dCol of math modes 2-4: the same da2, bit for bit
+    // col2im_conv3 adds the dCol of math modes 2 and 3: the same da2, bit for bit
     Conv3DA al{bw.da3};
     PretiledB<Conv3DB> blp{wi.img[5], 576 / 64};
     Conv3DE ep{bw.da2, act.a2};
@@ -455,9 +407,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     Conv2WA al{act.a1, map};
     PlainB bl{bw.da2, 64, 0};
     EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 512, 64};
-    static const int cw8 = getenv("DRL_B200_CW8") ? atoi(getenv("DRL_B200_CW8")) : 1;
-    if (m16 && cw8) GEMM16("conv2_wgrad", X64W8x2, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
-    else if (m16) GEMM16("conv2_wgrad", X64W, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
+    if (m16) GEMM16("conv2_wgrad", X64W8x2, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
     else GEMM("conv2_wgrad", CfgBig, U64, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
     KERNEL("conv2_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv2_w, slab), 1);
   }
@@ -487,8 +437,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     GEMM_FFMA("conv2_dgrad", CfgN32, al, bl, ep, Mb * 100, 32, 256, 4, 256, 0);
   }
   // ---- conv1 (input is data: weight gradient only) -----------------------------------------
-  static const bool c1w_gather = getenv("DRL_B200_CONV1_GATHER") != nullptr;
-  if (m16 && !c1w_gather) {
+  if (m16) {
     // frame-resident TMA kernel (conv1_tma.cuh): one partial slab per CTA, then the fixed-order reduce
     const size_t slab = 257 * 32;
     int splits = 0;

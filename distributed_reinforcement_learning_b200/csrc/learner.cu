@@ -8,7 +8,6 @@
 
 #include <mutex>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: no link dependency, a no-op unless a profiler injects itself
@@ -34,18 +33,6 @@ void set_error(const char* fmt, ...) {
 }
 const char* get_error() { return g_err; }
 
-// programmatic-dependent-launch bookkeeping (common.cuh): per thread, per stream
-bool& pdl_chain_ok(cudaStream_t s) {
-  static thread_local std::unordered_map<cudaStream_t, bool> chain;
-  return chain[s];
-}
-int pdl_level() {
-  static const int level = [] {
-    const char* e = getenv("DRL_B200_PDL");
-    return e ? atoi(e) : DRL_DEFAULT_PDL_LEVEL;
-  }();
-  return level;
-}
 static std::vector<TraceSetter>& trace_setters() {
   static std::vector<TraceSetter> v;
   return v;
@@ -53,10 +40,6 @@ static std::vector<TraceSetter>& trace_setters() {
 int register_trace_setter(TraceSetter f) {
   trace_setters().push_back(f);
   return (int)trace_setters().size();
-}
-bool& pdl_region_on() {
-  static thread_local bool on = true;
-  return on;
 }
 
 // ---- per-kernel profiler -------------------------------------------------------------------
@@ -71,7 +54,6 @@ void prof_mark(cudaStream_t s, const char* name) {
   cudaEvent_t e = nullptr;
   if (cudaEventCreate(&e) != cudaSuccess) return;
   cudaEventRecord(e, s);
-  pdl_break(s);
   g_prof.ev.push_back(e);
   g_prof.names.push_back(name);
 }
@@ -144,7 +126,7 @@ struct drl_learner {
   int peer_early_ctas = 64;   // grid of the early exchange instance (DRL_B200_PEER_EARLY_CTAS; 0 = no early part)
   cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_done = nullptr;
   cudaEvent_t fj[8] = {};    // fork/join events between the compute and the side stream
-  cudaStream_t side2 = nullptr;   // second side lane (small head weight gradients), DRL_B200_SIDE2=0 disables
+  cudaStream_t side2 = nullptr;   // second side lane (small head weight gradients)
   cudaEvent_t fj2[4] = {};
   bool par = true;           // run off-critical-path kernels on the side stream
   bool images_stale = true;  // weight images do not match the parameters (forward-only entry points rebuild them)
@@ -225,8 +207,6 @@ Streams streams_of(const drl_learner* h) {
 // retile = true: (re)build the weight images first.  A training step always does (the parameters changed in the
 // previous apply); the forward-only entry points only when the images are stale.
 int enqueue_forward(drl_learner* h, const Inputs& in, int B, int T, bool retile) {
-  pdl_break(h->compute);   // whatever precedes (event waits, copies) is not a pdl-aware kernel
-  pdl_break(h->side);
   return net_forward(streams_of(h), h->pl, h->params, h->wimg, in, h->act, B, T, h->mode, retile);
 }
 
@@ -251,7 +231,6 @@ int enqueue_forward_backward(drl_learner* h, int slot) {
 // local_only: the single-replica update on the local bucket even when the peer exchange is on (profiling on one rank)
 // early: the backward pass of THIS enqueue recorded ev_lstm_grads (one-graph step): part 0 of the exchange overlaps it
 int enqueue_apply(drl_learner* h, int out_row, bool local_only = false, bool early = false) {
-  pdl_break(h->compute);
   OptState o_local = h->opt, o_peer = h->plan.o;
   o_local.out = o_peer.out = h->d_out + 8 * out_row;
   if (h->peer_on && !local_only) {
@@ -362,7 +341,7 @@ extern "C" {
 const char* drl_last_error(void) { return get_error(); }
 
 // debug: arm (dev_buf = device buffer of >= 8001 uint64, word 0 = entry counter) or disarm (NULL) the kernel
-// start-time trace of common.cuh::pdl_prologue
+// start-time trace of common.cuh::kernel_prologue
 int drl_debug_trace(void* dev_buf) {
   if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
   DRL_CUDA_CHECK(cudaDeviceSynchronize());
@@ -394,9 +373,9 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     set_error("reward_clipping must be DRL_REWARD_ABS_ONE or DRL_REWARD_SOFT_ASYMMETRIC");   // utils.py:45
     return DRL_ERR_INVALID;
   }
-  if (cfg->math_mode < 0 || cfg->math_mode > 5) {
-    set_error("math_mode must be 0 (default), 1 (FP32 FFMA), 2 (wgmma 3xTF32), 3 (same, persistent kernels), "
-              "4 (same as 2 with TMA-fed conv2/conv3 forward) or 5 (wgmma with 16-bit split operands)");
+  if (cfg->math_mode < 0 || cfg->math_mode > 5 || cfg->math_mode == 4) {
+    set_error("math_mode must be 0 (default), 1 (FP32 FFMA), 2 (wgmma 3xTF32), 3 (same, persistent kernels) "
+              "or 5 (wgmma with 16-bit split operands)");
     return DRL_ERR_INVALID;
   }
   if (drl_device_count() <= cfg->device) { set_error("CUDA device %d not available (no CPU fallback)", cfg->device); return DRL_ERR_CUDA; }
@@ -418,13 +397,8 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_xchg_done, cudaEventDisableTiming));
     if (const char* e = getenv("DRL_B200_PEER_EARLY_CTAS")) h->peer_early_ctas = atoi(e);
     for (int i = 0; i < 8; ++i) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->fj[i], cudaEventDisableTiming));
-    {
-      const char* e = getenv("DRL_B200_SIDE2");
-      if (!(e && atoi(e) == 0)) {
-        DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side2, cudaStreamNonBlocking));
-        for (int i = 0; i < 4; ++i) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->fj2[i], cudaEventDisableTiming));
-      }
-    }
+    DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side2, cudaStreamNonBlocking));
+    for (int i = 0; i < 4; ++i) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->fj2[i], cudaEventDisableTiming));
     DRL_CUDA_CHECK(cudaEventCreate(&h->ev_start));
     DRL_CUDA_CHECK(cudaEventCreate(&h->ev_stop));
     DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_done, cudaEventDisableTiming));
@@ -437,11 +411,8 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
       DRL_CUDA_CHECK(cudaMemcpy(h->ms, ones.data(), NP * sizeof(float), cudaMemcpyHostToDevice));
     }
     Acts& a = h->act;
-    const size_t planes = (h->mode == 4) ? 2 : 1;      // math mode 4: [value plane | tf32 remainder plane]
-    DRL_TRY(dev_alloc(h, &a.a1, planes * M * 400 * 32));
-    a.a1_lo = (planes == 2) ? a.a1 + M * 400 * 32 : nullptr;
-    DRL_TRY(dev_alloc(h, &a.a2, planes * M * 81 * 64));
-    a.a2_lo = (planes == 2) ? a.a2 + M * 81 * 64 : nullptr;
+    DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
+    DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
     DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
     DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
     DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
@@ -455,11 +426,9 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     DRL_TRY(dev_alloc(h, &a.logits, M * A));
     DRL_TRY(dev_alloc(h, &a.policy, M * A));
     DRL_TRY(dev_alloc(h, &a.value, M));
-    if (h->mode == 5 && !(getenv("DRL_B200_LSTM_BULK") && atoi(getenv("DRL_B200_LSTM_BULK")) == 0)) {
-      const size_t Mbr = (size_t)h->B * (h->T - 2);
-      DRL_TRY(dev_alloc(h, &a.img_xt, lstm_image_bytes(1, (int)M, (int)Mbr)));
-      DRL_TRY(dev_alloc(h, &h->bwd.img_dzt, lstm_image_bytes(3, (int)M, (int)Mbr)));
-      a.img_rows = (int)M;
+    if (h->mode == 5) {
+      DRL_TRY(dev_alloc(h, &a.img_xt, lstm_image_bytes(1, (int)M, (int)Mb)));
+      DRL_TRY(dev_alloc(h, &h->bwd.img_dzt, lstm_image_bytes(3, (int)M, (int)Mb)));
     }
     Bwd& b = h->bwd;
     DRL_TRY(dev_alloc(h, &b.dlogits, Mb * 32));

@@ -364,10 +364,6 @@ struct PlainBT {   // B(k, n) = W[z][n][k], K-contiguous (used for dX = dY W^T)
 // --------------------------------------------------------------------------------------------
 // Epilogues
 // --------------------------------------------------------------------------------------------
-// x - trunc_tf32(x): what the tensor core does NOT see when it reads x as a tf32 operand (it uses the upper 19 bits of
-// the word).  Exact in fp32.  Stored next to an activation, it is the A_lo operand of the 3xTF32 split.
-__device__ __forceinline__ float tf32_rem(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
-
 // C[z][m][n] = act(v * scale + bias[z][n])
 template <bool RELU, bool BIAS>
 struct EpBiasAct {
@@ -375,7 +371,6 @@ struct EpBiasAct {
   float* c; int ldc; size_t sz;
   const float* bias; size_t sbias;
   float scale;
-  float* lo = nullptr;   // optional tf32 remainder plane of C (operand of a TMA-fed consumer, gemm_tma.cuh)
   template <int V>
   __device__ __forceinline__ void store(int z, int m, int n, const float (&v)[V]) const {
     float o[V];
@@ -388,11 +383,6 @@ struct EpBiasAct {
     const size_t off = z * sz + (size_t)m * ldc + n;
     if constexpr (V == 4) *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
     else c[off] = o[0];
-    if (lo) {
-      if constexpr (V == 4)
-        *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_rem(o[0]), tf32_rem(o[1]), tf32_rem(o[2]), tf32_rem(o[3]));
-      else lo[off] = tf32_rem(o[0]);
-    }
   }
   // hoisted-bias form used by the tensor-core epilogues (epilogue_store_32x32)
   __device__ __forceinline__ float4 bias4(int z, int n) const {
@@ -408,7 +398,6 @@ struct EpBiasAct {
     }
     const size_t off = z * sz + (size_t)m * ldc + n;
     *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
-    if (lo) *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_rem(o[0]), tf32_rem(o[1]), tf32_rem(o[2]), tf32_rem(o[3]));
   }
   __device__ __forceinline__ void store_colsum(int, int, float) const {}
 };
@@ -427,7 +416,6 @@ struct EpConv1 {
   static constexpr bool kColSum = false;
   float* c; int ldc;
   const float* bias;
-  float* lo = nullptr;   // optional tf32 remainder plane (see EpBiasAct)
   template <int V>
   __device__ __forceinline__ void store(int, int m, int n, const float (&v)[V]) const {
     float o[V];
@@ -436,11 +424,6 @@ struct EpConv1 {
     const size_t off = (size_t)m * ldc + n;
     if constexpr (V == 4) *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
     else c[off] = o[0];
-    if (lo) {
-      if constexpr (V == 4)
-        *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_rem(o[0]), tf32_rem(o[1]), tf32_rem(o[2]), tf32_rem(o[3]));
-      else lo[off] = tf32_rem(o[0]);
-    }
   }
   __device__ __forceinline__ float4 bias4(int, int n) const { return __ldg(reinterpret_cast<const float4*>(bias + n)); }
   __device__ __forceinline__ void store4b(int, int m, int n, const float (&v)[4], const float4& b) const {
@@ -450,7 +433,6 @@ struct EpConv1 {
     for (int j = 0; j < 4; ++j) o[j] = fmaxf(div255(v[j]) + bb[j], 0.f);
     const size_t off = (size_t)m * ldc + n;
     *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
-    if (lo) *reinterpret_cast<float4*>(lo + off) = make_float4(tf32_rem(o[0]), tf32_rem(o[1]), tf32_rem(o[2]), tf32_rem(o[3]));
   }
   __device__ __forceinline__ void store_colsum(int, int, float) const {}
 };

@@ -15,7 +15,7 @@
 namespace drl {
 
 __global__ void __launch_bounds__(256) sqnorm_partial_kernel(OptState o) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8];
   const int64_t n4 = o.n / 4;
   const float4* g4 = reinterpret_cast<const float4*>(o.grads);
@@ -45,7 +45,7 @@ __global__ void __launch_bounds__(256) sqnorm_partial_kernel(OptState o) {
 }
 
 __global__ void __launch_bounds__(256) rmsprop_apply_kernel(OptState o) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8];
   __shared__ float s_scale;
   // data-parallel: barrier 1 of the peer exchange -- every peer has delivered its slice of the summed gradients and

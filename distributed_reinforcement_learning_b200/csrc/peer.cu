@@ -37,7 +37,7 @@ namespace drl {
 //             peer "my slice and my partials have been delivered to you"; the update kernel waits for those flags.
 __global__ void __launch_bounds__(kPeerThreads) peer_reduce_kernel(PeerTable t, OptState o, int rank, int world, int nblk_r,
                                                           int part, int64_t beg4, int64_t end4, int do_lr) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8];
   __shared__ bool last_s;
   uint32_t* epoch = t.epoch[rank] + 4 * part; // [0], [1]: epochs completed; [2]: ticket counter

@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(kR2G) r2d2_lstm_fwd_kernel(
     const float* __restrict__ Wh, const float* __restrict__ h0, const float* __restrict__ c0,
     const uint8_t* __restrict__ done, float* __restrict__ gates, float* __restrict__ tc, float* __restrict__ hout,
     float* __restrict__ hin, float* __restrict__ cin, float* __restrict__ c_last, int B, int S) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ __align__(16) float sh[kR2L];
   __shared__ float sz[kR2G];
   const int b = blockIdx.x, j = threadIdx.x;
@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(kR2G) r2d2_lstm_bwd_kernel(
     const float* __restrict__ dhout, const float* __restrict__ gates, const float* __restrict__ tc,
     const float* __restrict__ cin, const float* __restrict__ Wh, const uint8_t* __restrict__ done,
     float* __restrict__ dz, int B, int S) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ __align__(16) float sdz[kR2G];
   __shared__ float sdh[kR2L];
   __shared__ float spart[4 * kR2L];
@@ -267,7 +267,7 @@ __global__ void __launch_bounds__(kR2G) r2d2_lstm_bwd_kernel(
 __global__ void __launch_bounds__(128) r2d2_out_kernel(const float* __restrict__ q1, const float* __restrict__ wv,
                                                         const float* __restrict__ bv, const float* __restrict__ wm,
                                                         const float* __restrict__ bm, float* __restrict__ q, int M, int A) {
-  pdl_prologue();
+  kernel_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m = blockIdx.x * 4 + warp;
   if (m >= M) return;
@@ -291,7 +291,7 @@ __global__ void __launch_bounds__(128) r2d2_out_kernel(const float* __restrict__
 __global__ void __launch_bounds__(kR2H) r2d2_out_bwd_kernel(const float* __restrict__ dq, const float* __restrict__ dmean,
                                                              const float* __restrict__ wv, const float* __restrict__ wm,
                                                              const float* __restrict__ q1, float* __restrict__ dq1, int A) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float sd[32];
   __shared__ float sdm;
   const int m = blockIdx.x, k = threadIdx.x;
@@ -331,7 +331,7 @@ __device__ __forceinline__ double r2_hinv(double x) {
   return s * (r * r - 1.0);
 }
 __global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[8];
   const int Nt = a.S - a.burn_in - 1;
   const int M = a.B * a.S;
@@ -431,18 +431,15 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
   if (pl.C == 1) {
     Conv1A1 al{in.frames, map};
     PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b, nullptr};
+    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
     GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 64, 1, 64, 0);
   } else {
     Conv1A al{in.frames, map};
     PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b, nullptr};
+    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
     GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
   }
-  if (st.par) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
-    pdl_break(st.main);
-  }
+  if (st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
   {
     Conv2A al{act.a1, map};
     PlainB bl{P + pl.conv2_w, 64, 0};
@@ -489,7 +486,6 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
 
 static int r2_backward(const Streams& st, const R2Layout& pl, const float* P, const WeightImages& wi, float* G,
                        const R2In& in, const R2Acts& act, const R2Bwd& bw, int B, int S, int mode, int* launches) {
-  PdlRegionOff pdl_region;
   const int M = B * S;
   const RowMap map{B, S};
   cudaStream_t s = st.main;
@@ -668,16 +664,12 @@ int alloc_acts(drl_r2d2* h, R2Acts& a) {
 
 // both unrolls + TD kernel over nb sequences held by `in`
 int enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, float* td_host, int* launches) {
-  pdl_break(h->compute);
-  pdl_break(h->side);
   const Streams st = h->streams(), tst = h->target_streams();
   // the two unrolls are independent (and each recurrence kernel only occupies nb SMs): the target scope runs on its
   // own stream pair beside the main scope and joins before the TD kernel
   if (h->par) {
     DRL_CUDA_CHECK(cudaEventRecord(h->ev_tfork, h->compute));
     DRL_CUDA_CHECK(cudaStreamWaitEvent(h->tmain, h->ev_tfork, 0));
-    pdl_break(h->tmain);
-    pdl_break(h->tside);
   }
   DRL_TRY(r2_forward(tst, h->pl, h->target, h->twi, in, h->tact, nullptr, nb, h->S, h->mode, h->target_images_stale, false,
                      true, launches));
@@ -686,10 +678,7 @@ int enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, float* t
   DRL_TRY(r2_forward(st, h->pl, h->params, h->wi, in, h->act, nullptr, nb, h->S, h->mode, h->main_images_stale,
                      h->main_images_stale, false, launches));
   h->main_images_stale = false;
-  if (h->par) {
-    DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, h->ev_tjoin, 0));
-    pdl_break(h->compute);
-  }
+  if (h->par) DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, h->ev_tjoin, 0));
   R2TdArgs a{};
   a.mq = h->act.q; a.tq = h->tact.q;
   a.action = in.action; a.reward = in.reward; a.done = in.done; a.weight = train ? in.weight : nullptr;
@@ -909,8 +898,6 @@ int drl_r2d2_act(drl_r2d2* h, int32_t n, const uint8_t* state, const int32_t* pr
   R2In in = h->in[h->num_slots];
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   DRL_TRY(stage_into(h, in, h->compute, n, 1, state, previous_action, nullptr, h_in, c_in, nullptr, nullptr, nullptr));
-  pdl_break(h->compute);
-  pdl_break(h->side);
   in.done = nullptr;                                     // a single step: nothing is carried
   DRL_TRY(r2_forward(h->streams(), h->pl, h->params, h->wi, in, h->act, h->c_last, n, 1, h->mode, h->main_images_stale,
                      h->main_images_stale, false, nullptr));

@@ -109,7 +109,7 @@ __device__ __forceinline__ void vtrace_trajectory(const VtraceCfg& cfg, const fl
 __global__ void __launch_bounds__(128) vtrace_losses_kernel(
     VtraceCfg cfg, const float* __restrict__ policy, const float* __restrict__ value, Inputs in, VtraceOut out,
     float* __restrict__ dlogits, float* __restrict__ dv, int B, int T, int A) {
-  pdl_prologue();
+  kernel_prologue();
   __shared__ float red[4][3];
   __shared__ bool is_last;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;

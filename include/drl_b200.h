@@ -65,8 +65,8 @@ typedef struct drl_learner_config {
   int32_t num_slots;          /* device staging slots for stream-overlapped H2D (>=1, default 2) */
   int32_t use_cuda_graph;     /* 1: capture forward+backward(+apply) into CUDA graphs           */
   int32_t math_mode;          /* 0 = default (5); 1 = FP32 FFMA; 2 = wgmma 3xTF32; 3 = same, persistent kernels;
-                                 4 = rejected (former TMA-fed conv experiment); 5 = wgmma on bf16 hi/lo split
-                                 operands (three products, fp32-grade) + bulk-fed LSTM weight gradient */
+                                 5 = wgmma on bf16 hi/lo split operands (three products, fp32-grade) + bulk-fed
+                                 LSTM weight gradient; any other value (4 included) is DRL_ERR_INVALID */
 } drl_learner_config;
 
 /* Results of one step: the 4 floats Agent.train returns (agent/impala.py:144-148) + grad norm. */

@@ -93,38 +93,3 @@ def test_step_persistent_tensor_core_kernels(native, B, T, A, kw):
     gathers of the next) reach the same 1e-4 bar."""
     _assert_all(parity.compare_step(B, T=T, A=A, math_mode=3, **kw))
 
-
-@pytest.mark.parametrize("B,T", [(4, 20), (3, 5), (32, 20)])
-def test_tma_fed_conv_forward_matches_ffma_path(native, B, T):
-    """math_mode=4: conv2 / conv3 forward are fed by TMA tensor loads of the activation's value plane and its
-    tf32-remainder plane (gemm_tma.cuh).  Their outputs must agree with the FP32-FFMA kernels to fp32 rounding
-    (3xTF32 with a truncated hi part drops lo*lo ~ 2^-20 per product), for odd image counts (partial last tile of
-    two images) as well."""
-    from distributed_reinforcement_learning_b200.learner import NativeLearner
-    from oracle import impala_torch as it
-    from oracle import synthetic
-    batch = synthetic.make_batch(B, T=T, seed=5)
-    flat = it.flatten_params(it.init_params(0))
-    outs = {}
-    for mode in (1, 4):
-        eng = NativeLearner(batch=B, trajectory=T, num_action=18, math_mode=mode)
-        eng.set_params(flat)
-        eng.stage(0, *[batch[f] for f in synthetic.TRAIN_FIELDS])
-        eng.forward(0)
-        M = B * T
-        outs[mode] = {"a1": eng.read_buffer("a1", M * 400 * 32), "a2": eng.read_buffer("a2", M * 81 * 64),
-                      "a3": eng.read_buffer("a3", M * 3136)}
-        del eng
-    for name in ("a1", "a2", "a3"):
-        ref, got = outs[1][name].astype(np.float64), outs[4][name].astype(np.float64)
-        assert np.all(np.isfinite(got))
-        err = np.max(np.abs(got - ref)) / np.max(np.abs(ref))
-        assert err < (5e-6 if name != "a3" else 2e-5), (name, err)
-        # ReLU zeros must be the same set up to borderline pre-activations
-        assert np.mean((ref > 0) != (got > 0)) < 1e-4, name
-
-
-def test_step_tma_fed_conv_forward(native):
-    """the whole learner step in math_mode=4 against the float64 oracle"""
-    _assert_all(parity.compare_step(4, T=20, math_mode=4))
-    _assert_all(parity.compare_step(3, T=5, A=6, math_mode=4))

@@ -43,6 +43,18 @@ def test_compute_fails_loudly_without_a_device(native):
         vtrace.from_importance_weights(z, z, z, z, np.zeros(2, np.float32))
 
 
+def test_learner_rejects_math_mode_4(native):
+    """math_mode 4 is not a mode: create fails as invalid, before it looks for a device, and names the accepted modes."""
+    from distributed_reinforcement_learning_b200.learner import NativeLearner
+    with pytest.raises(native.DrlError) as ei:
+        NativeLearner(batch=2, trajectory=5, math_mode=4)
+    assert ei.value.code == native.DRL_ERR_INVALID
+    msg = str(ei.value)
+    for accepted in ("0 (default)", "1 (FP32 FFMA)", "2 (wgmma 3xTF32)", "3 (", "5 (wgmma with 16-bit split operands)"):
+        assert accepted in msg, msg
+    assert "4 (" not in msg, msg
+
+
 def test_product_package_never_imports_the_oracle():
     pkg = os.path.join(ROOT, "distributed_reinforcement_learning_b200")
     for dp, _, fs in os.walk(pkg):

@@ -2,8 +2,8 @@
 
     python tools/timeline.py [--math-mode 2] [--no-graph]
 
-Arms drl_debug_trace: CTA 0 of every kernel records {globaltimer, grid, block} when it starts (after its
-griddepcontrol.wait).  Prints the start times relative to the first kernel, the gap to the next start on the device
+Arms drl_debug_trace: CTA 0 of every kernel records {globaltimer, grid, block} when it starts.
+Prints the start times relative to the first kernel, the gap to the next start on the device
 and the launch geometry, so each kernel can be recognised (conv1_fwd = 2000 CTAs x 160 threads, ...)."""
 import argparse
 import ctypes as C
