@@ -133,7 +133,7 @@ def unroll(p, state, previous_action, done, h0, c0, num_action, pattern=False):
 
 
 DEFAULT_CFG = dict(seq_len=15, burn_in=7, input_shape=(84, 84, 1), num_action=4, lstm_size=64,
-                   discount_factor=0.997)                      # config.json:84-101
+                   discount_factor=0.997, learning_rate=LR)    # config.json:84-101; agent/r2d2.py's fixed Adam rate
 
 
 class Learner:
@@ -226,7 +226,7 @@ class Learner:
         out, g = self.gradients(state, previous_action, action, h, c, reward, done, weight=weight,
                                 next_action=next_action)
         b1p, b2p = float(self.beta1_power), float(self.beta2_power)
-        alpha = float(np.float32(LR)) * np.sqrt(1.0 - b2p) / (1.0 - b1p)
+        alpha = float(np.float32(self.cfg["learning_rate"])) * np.sqrt(1.0 - b2p) / (1.0 - b1p)
         with torch.no_grad():
             for n, p in self.params.items():
                 self.m[n] += (g[n] - self.m[n]) * (1.0 - BETA1)

@@ -53,12 +53,44 @@ def adam_expected(p0, g, m0, v0, gn, clip, lr, b1p, b2p):
     return p0 - m * alpha / (np.sqrt(v) + ax.ADAM_EPS), m, v
 
 
-def compare_step(B, A=4, seed=4321, steps=1, reward_clipping="abs_one", sync_target_at=None, **kw):
+OPT_KEYS = ("gradient_clip_norm", "start_learning_rate", "end_learning_rate", "learning_frame")
+
+
+def check_opt(opt, keys=OPT_KEYS):
+    opt = dict(opt or {})
+    if set(opt) - set(keys):
+        raise ValueError("unknown optimizer settings %s" % sorted(set(opt) - set(keys)))
+    return opt
+
+
+def load_adam_state(eng, L, st, unflatten):
+    """Restore the Adam state ``st`` (flat float32 m, v; step; beta powers) into the CUDA learner and the oracle."""
+    eng.set_opt_state(st["m"], st["v"], int(st["step"]), st["beta1_power"], st["beta2_power"])
+    md, vd = unflatten(st["m"]), unflatten(st["v"])
+    with torch.no_grad():
+        for n in L.params:
+            L.m[n].copy_(md[n])
+            L.v[n].copy_(vd[n])
+    L.beta1_power, L.beta2_power = np.float32(st["beta1_power"]), np.float32(st["beta2_power"])
+    L.step = int(st["step"])
+    return int(st["step"])
+
+
+def compare_step(B, A=4, seed=4321, steps=1, reward_clipping="abs_one", sync_target_at=None, opt=None,
+                 init_state=None, trace=None, **kw):
+    """``opt``: optimizer settings (keys of OPT_KEYS) given to both the CUDA learner and the oracle; ``init_state``: an
+    Adam state (see load_adam_state) loaded into both before the first step; ``trace``: a list that receives the
+    scalars of every GPU step."""
+    opt = check_opt(opt)
     params = ax.init_params(0, torch.float32, num_action=A)
     target = ax.init_params(1, torch.float32, num_action=A)
     cfg = dict(num_action=A, reward_clipping=reward_clipping)
-    L = ax.Learner(params, target, torch.float64, **cfg)
-    eng = native_apex(B, A, params, target, reward_clipping=reward_clipping, **kw)
+    L = ax.Learner(params, target, torch.float64, **cfg, **opt)
+    eng = native_apex(B, A, params, target, reward_clipping=reward_clipping, **opt, **kw)
+    step0 = 0
+    if init_state is not None:
+        step0 = load_adam_state(eng, L, init_state,
+                                lambda f: ax.unflatten_params(f, torch.float64, num_action=A))
     errs = {}
     flips = elems = 0
     max_abs = 0.0
@@ -76,6 +108,8 @@ def compare_step(B, A=4, seed=4321, steps=1, reward_clipping="abs_one", sync_tar
             slot = s % eng.num_slots
             eng.stage(slot, *args)
             out, td = eng.step(slot)
+            if trace is not None:
+                trace.append(out)
             taps = eng.taps()
             masks = gpu_masks(eng, B, A)
             # double-DQN argmax at the GPU's choice; disagreements are only allowed at float32-level ties
@@ -94,7 +128,7 @@ def compare_step(B, A=4, seed=4321, steps=1, reward_clipping="abs_one", sync_tar
             errs["td_error" + tag] = rel_err(td, res[1])
             errs["lr" + tag] = abs(out["learning_rate"] - lr)
             errs["grad_norm" + tag] = rel_err(out["grad_norm"], gn)
-            if out["step"] != s + 1:
+            if out["step"] != step0 + s + 1:
                 errs["step" + tag] = float("inf")
             for k in ("main_q", "next_main_q", "target_q", "target_value", "state_action_value"):
                 errs["tap/" + k + tag] = rel_err(taps[k], o[k].detach().numpy())
@@ -119,8 +153,8 @@ def compare_step(B, A=4, seed=4321, steps=1, reward_clipping="abs_one", sync_tar
             gn_gpu = float(np.sqrt(np.sum(g_gpu_flat.astype(np.float64) ** 2)))
             exp_p, exp_m, exp_v = adam_expected(p0.astype(np.float64), g_gpu_flat.astype(np.float64),
                                                 st0["m"].astype(np.float64), st0["v"].astype(np.float64), gn_gpu,
-                                                40.0, float(out["learning_rate"]), st0["beta1_power"],
-                                                st0["beta2_power"])
+                                                L.cfg["gradient_clip_norm"], float(out["learning_rate"]),
+                                                st0["beta1_power"], st0["beta2_power"])
             floor = 4.0 * np.finfo(np.float32).eps * np.max(np.abs(p0)) / TOL
             errs["update/adam" + tag] = float(np.max(np.abs(p1 - exp_p)) / (np.max(np.abs(exp_p - p0)) + floor))
             errs["adam/m" + tag] = rel_err(st1["m"], exp_m)

@@ -83,13 +83,33 @@ def gpu_activation_pattern(eng, B, T, A):
     return masks
 
 
-def compare_step(B, T=20, A=18, seed=1234, steps=1, reward_clipping="abs_one", layers=True, **kw):
+OPT_KEYS = ("gradient_clip_norm", "start_learning_rate", "end_learning_rate", "learning_frame")
+
+
+def compare_step(B, T=20, A=18, seed=1234, steps=1, reward_clipping="abs_one", layers=True, opt=None,
+                 init_state=None, trace=None, **kw):
     """Returns {name: rel_err} for activations, taps, losses, every parameter gradient, and the applied
     update / RMSProp slots after each of `steps` updates (GPU step first, then the float64 oracle step
-    evaluated at the GPU's ReLU activation pattern)."""
+    evaluated at the GPU's ReLU activation pattern).
+
+    ``opt``: optimizer settings (keys of OPT_KEYS) given to both the CUDA learner and the oracle.
+    ``init_state``: dict(ms=flat float32 RMSProp slots, step=global step) loaded into both before the first step.
+    ``trace``: a list that receives the scalars of every GPU step (learning rate, grad norm, ...)."""
+    opt = dict(opt or {})
+    if set(opt) - set(OPT_KEYS):
+        raise ValueError("unknown optimizer settings %s" % sorted(set(opt) - set(OPT_KEYS)))
     batch, params, cfg = make_case(B, T, A, seed, reward_clipping=reward_clipping)
-    L = it.Learner(params, torch.float64, "dedup", **cfg)
-    eng = native_learner(batch, params, cfg, **kw)
+    L = it.Learner(params, torch.float64, "dedup", **cfg, **opt)
+    eng = native_learner(batch, params, cfg, **opt, **kw)
+    step0 = 0
+    if init_state is not None:
+        step0 = int(init_state["step"])
+        eng.set_opt_state(init_state["ms"], step0)
+        ms0 = it.unflatten_params(init_state["ms"], torch.float64, num_action=A)
+        with torch.no_grad():
+            for n in L.ms:
+                L.ms[n].copy_(ms0[n])
+        L.step = step0
     args = [batch[k] for k in synthetic.TRAIN_FIELDS]
     M, Mb = B * T, B * (T - 2)
     errs = {}
@@ -101,6 +121,8 @@ def compare_step(B, T=20, A=18, seed=1234, steps=1, reward_clipping="abs_one", l
             p_before = {n: v.detach().clone() for n, v in L.params.items()}
             eng.stage(s % eng.num_slots, *args)
             out = eng.step(s % eng.num_slots)
+            if trace is not None:
+                trace.append(out)
             masks = gpu_activation_pattern(eng, B, T, A)
             with it.activation_pattern(masks) as st:
                 res, o, grads, gn = L.train(*args, return_all=True)
@@ -109,7 +131,7 @@ def compare_step(B, T=20, A=18, seed=1234, steps=1, reward_clipping="abs_one", l
                 errs["loss/" + k + tag] = rel_err(out[k], float(o[k].detach()))
             errs["lr" + tag] = abs(out["learning_rate"] - res[3])
             errs["grad_norm" + tag] = rel_err(out["grad_norm"], gn)
-            if out["step"] != s + 1:
+            if out["step"] != step0 + s + 1:
                 errs["step" + tag] = float("inf")
             taps = eng.taps()
             for k in ("vs", "clipped_rho", "vs_plus_1", "pg_advantage"):
@@ -150,7 +172,7 @@ def compare_step(B, T=20, A=18, seed=1234, steps=1, reward_clipping="abs_one", l
         md = it.unflatten_params(ms, torch.float64, num_action=A)
         for n in L.params:
             errs["ms/" + n] = rel_err(md[n].numpy(), L.ms[n].detach().numpy())
-        if st_ != steps:
+        if st_ != step0 + steps:
             errs["opt_step"] = float("inf")
         errs["kink/flip_fraction"] = flips / max(elems, 1)
         errs["kink/max_abs_at_flip"] = max_abs

@@ -4,7 +4,7 @@ handling and Adam check as tests/apex_parity.py."""
 import numpy as np
 import torch
 
-from apex_parity import adam_expected
+from apex_parity import adam_expected, check_opt, load_adam_state
 from oracle import impala_torch as it
 from oracle import r2d2_torch as rt
 from parity import TOL, failures, rel_err   # noqa: F401
@@ -29,12 +29,30 @@ def gpu_masks(eng, B, S, A):
             "emb": torch.from_numpy(eng.read_buffer("emb", A * 256).reshape(A, 256) > 0)}
 
 
-def compare_step(B, S=15, bi=7, A=4, C=1, seed=2468, steps=1, sync_target_at=None, **kw):
+def make_batch(B, S, A, C, seed, done_rate=None, done_ends=False):
+    """rt.make_sequences, optionally with its dones redrawn at ``done_rate`` and, with ``done_ends``, forced at the
+    first and the last step of every sequence."""
+    b = rt.make_sequences(B, S=S, A=A, input_shape=(84, 84, C), seed=seed)
+    if done_rate is not None:
+        b["done"] = np.random.default_rng(seed + 7919).random((B, S)) < done_rate
+    if done_ends:
+        b["done"][:, 0] = b["done"][:, S - 1] = True
+    return b
+
+
+def compare_step(B, S=15, bi=7, A=4, C=1, seed=2468, steps=1, sync_target_at=None, opt=None, init_state=None,
+                 trace=None, done_rate=None, done_ends=False, **kw):
+    """``opt``: dict(learning_rate=...) given to both the CUDA learner and the oracle (R2D2 does not clip);
+    ``init_state`` and ``trace`` as in apex_parity.compare_step; ``done_rate`` / ``done_ends`` as in make_batch."""
+    opt = check_opt(opt, ("learning_rate",))
     kwp = dict(num_action=A, lstm_size=64, input_shape=(84, 84, C))
     params = rt.init_params(0, torch.float32, **kwp)
     target = rt.init_params(1, torch.float32, **kwp)
-    L = rt.Learner(params, target, torch.float64, seq_len=S, burn_in=bi, **kwp)
-    eng = native_r2d2(B, S, bi, A, C, params, target, **kw)
+    L = rt.Learner(params, target, torch.float64, seq_len=S, burn_in=bi, **kwp, **opt)
+    eng = native_r2d2(B, S, bi, A, C, params, target, **opt, **kw)
+    step0 = 0
+    if init_state is not None:
+        step0 = load_adam_state(eng, L, init_state, lambda f: rt.unflatten_params(f, torch.float64, **kwp))
     errs = {}
     flips = elems = 0
     max_abs = 0.0
@@ -45,7 +63,7 @@ def compare_step(B, S=15, bi=7, A=4, C=1, seed=2468, steps=1, sync_target_at=Non
             if sync_target_at is not None and s == sync_target_at:
                 eng.main_to_target()
                 L.main_to_target()
-            b = rt.make_sequences(B, S=S, A=A, input_shape=(84, 84, C), seed=seed + s)
+            b = make_batch(B, S, A, C, seed + s, done_rate, done_ends)
             args = [b[k] for k in rt.TRAIN_FIELDS]
             st0 = eng.get_opt_state()
             p0 = eng.get_params()
@@ -53,6 +71,8 @@ def compare_step(B, S=15, bi=7, A=4, C=1, seed=2468, steps=1, sync_target_at=Non
             eng.stage(slot, b["state"], b["previous_action"], b["action"], b["h"][:, 0], b["c"][:, 0], b["reward"],
                       b["done"], b["weight"])
             out, td = eng.step(slot)
+            if trace is not None:
+                trace.append(out)
             taps = eng.taps()
             masks = gpu_masks(eng, B, S, A)
             with torch.no_grad():
@@ -67,7 +87,7 @@ def compare_step(B, S=15, bi=7, A=4, C=1, seed=2468, steps=1, sync_target_at=Non
             errs["loss" + tag] = rel_err(out["loss"], res[0])
             errs["td_error" + tag] = rel_err(td, res[1])
             errs["grad_norm" + tag] = rel_err(out["grad_norm"], gn)
-            if out["step"] != s + 1:
+            if out["step"] != step0 + s + 1:
                 errs["step" + tag] = float("inf")
             for k in ("main_q", "target_q", "target_value", "state_action_value"):
                 errs["tap/" + k + tag] = rel_err(taps[k], o[k].detach().numpy())
@@ -85,7 +105,8 @@ def compare_step(B, S=15, bi=7, A=4, C=1, seed=2468, steps=1, sync_target_at=Non
             g64 = g_gpu.astype(np.float64)
             exp_p, exp_m, exp_v = adam_expected(p0.astype(np.float64), g64, st0["m"].astype(np.float64),
                                                 st0["v"].astype(np.float64), float(np.sqrt(np.sum(g64 ** 2))), 1e30,
-                                                float(np.float32(1e-4)), st0["beta1_power"], st0["beta2_power"])
+                                                float(np.float32(L.cfg["learning_rate"])), st0["beta1_power"],
+                                                st0["beta2_power"])
             floor = 4.0 * np.finfo(np.float32).eps * np.max(np.abs(p0)) / TOL
             errs["update/adam" + tag] = float(np.max(np.abs(p1 - exp_p)) / (np.max(np.abs(exp_p - p0)) + floor))
             errs["adam/m" + tag] = rel_err(st1["m"], exp_m)

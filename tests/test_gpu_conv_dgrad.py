@@ -30,6 +30,10 @@ def _dgrad(dy_nhwc, w_hwio, act_nhwc, stride):
 
 @pytest.mark.parametrize("B,T,A", [(32, 20, 18), (3, 7, 6), (5, 32, 18)])
 def test_conv_data_gradients_mode5(native, B, T, A):
+    check_conv_data_gradients(B, T, A)
+
+
+def check_conv_data_gradients(B, T, A):
     batch, params, cfg = parity.make_case(B, T, A)
     eng = parity.native_learner(batch, params, cfg, math_mode=5)
     M, Mb = B * T, B * (T - 2)

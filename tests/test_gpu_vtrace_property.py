@@ -125,8 +125,10 @@ def test_golden_reference_executed_vector_on_the_cuda_kernel(native):
 def test_fused_learner_vtrace_kernel_property(native, B, T, A, seed, clipping):
     """The fused kernel of the learner step (both V-trace windows, pg_advantage, the three loss sums): its taps and
     losses against optimizer/vtrace.py (NumPy oracle, float64) evaluated on the ENGINE'S OWN policy / value outputs."""
-    import torch
+    check_fused_learner_vtrace(B, T, A, seed, clipping)
 
+
+def check_fused_learner_vtrace(B, T, A, seed, clipping):
     import parity
     from oracle import impala_torch as it
     from oracle import synthetic
