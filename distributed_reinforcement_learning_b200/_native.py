@@ -77,6 +77,12 @@ class R2d2Out(C.Structure):
     _fields_ = [("loss", C.c_float), ("grad_norm", C.c_float), ("step", C.c_int64)]
 
 
+class PolicyConfig(C.Structure):
+    _fields_ = [("max_batch", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32),
+                ("num_action", C.c_int32), ("lstm_size", C.c_int32), ("device", C.c_int32),
+                ("use_cuda_graph", C.c_int32)]
+
+
 class RingBatch(C.Structure):
     _fields_ = [("state", C.c_void_p), ("reward", C.c_void_p), ("done", C.c_void_p),
                 ("behavior_policy", C.c_void_p), ("action", C.c_void_p), ("previous_action", C.c_void_p),
@@ -124,6 +130,14 @@ def _load():
         "drl_debug_trace": (C.c_int, [vp]),
         "drl_learner_last_step_ms": (C.c_int, [vp, C.POINTER(f32)]),
         "drl_learner_launches_per_step": (C.c_int, [vp, C.POINTER(i32)]),
+        "drl_policy_create": (C.c_int, [C.POINTER(PolicyConfig), C.POINTER(vp)]),
+        "drl_policy_destroy": (C.c_int, [vp]),
+        "drl_policy_param_count": (C.c_int, [vp, C.POINTER(i64)]),
+        "drl_policy_set_params": (C.c_int, [vp, vp, i64]),
+        "drl_policy_get_params": (C.c_int, [vp, vp, i64]),
+        "drl_policy_sync_from_learner": (C.c_int, [vp, vp]),
+        "drl_policy_act": (C.c_int, [vp, i32] + [vp] * 9),
+        "drl_policy_last_act_ms": (C.c_int, [vp, C.POINTER(f32)]),
         "drl_vtrace_from_importance_weights": (C.c_int, [vp] * 5 + [i32, i32, f32, vp, vp]),
         "drl_vtrace_from_importance_weights_dev": (C.c_int, [vp] * 5 + [i32, i32, f32, vp, vp, vp]),
         "drl_vtrace_from_softmax": (C.c_int, [vp] * 7 + [i32, i32, i32, f32, vp, vp]),

@@ -1,0 +1,93 @@
+"""Vector actor: the actor branch of ``train_impala.py:117-194`` for N environments in lockstep on one NativePolicy.
+
+Each environment is its own actor task ``i`` (what ``FLAGS.task`` selects in the reference).  Per unroll:
+
+  - one parameter sync through ``learner.sync_policy(policy)`` (the learner-side ``impala.Agent``; device to device
+    when it has a CUDA learner);
+  - ``trajectory`` batched ``policy.act`` calls: one forward over all N environments, the actions drawn on the GPU
+    from the same global ``np.random`` stream the reference's ``np.random.choice`` reads;
+  - every environment steps with ``action % available_action[i]``; the trajectory stores the action unmodified
+    (SURVEY.md App. D);
+  - a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True; the score keeps the raw reward;
+  - at an episode's end the environment is reset, and previous action, h and c go back to 0;
+  - every environment's ``utils.UnrolledTrajectory`` goes to ``queue.append_to_queue(task=i, ...)``.
+"""
+import numpy as np
+
+from . import utils
+
+START_LIVES = 5   # the reference actor's life counter starts (and restarts after every episode) at 5
+
+
+class VectorActor:
+    def __init__(self, policy, envs, queue, trajectory, available_action, learner=None):
+        self.policy, self.envs, self.queue, self.learner = policy, list(envs), queue, learner
+        self.trajectory = int(trajectory)
+        self.available_action = [int(a) for a in available_action]
+        n = len(self.envs)
+        if not 1 <= n <= policy.max_batch:
+            raise ValueError("%d environments, the policy serves 1..%d per call" % (n, policy.max_batch))
+        if len(self.available_action) != n:
+            raise ValueError("available_action has %d entries for %d environments" % (len(self.available_action), n))
+        L = policy.L
+        self.states = [env.reset() for env in self.envs]
+        self.previous_action = np.zeros(n, np.int32)
+        self.h = np.zeros((n, L), np.float32)
+        self.c = np.zeros((n, L), np.float32)
+        self.lives = [START_LIVES] * n
+        self.episode = [0] * n
+        self.score = [0.0] * n
+        self.episode_step = [0] * n
+        self.total_max_prob = [0.0] * n
+
+    def run_unroll(self):
+        """One unroll of `trajectory` steps for every environment, pushed to the queue.  Returns the episodes that
+        finished during it: dicts of task, episode, score, episode_step and prob (mean max probability), the values
+        train_impala.py:170-172 logs."""
+        if self.learner is not None:
+            self.learner.sync_policy(self.policy)
+        n = len(self.envs)
+        trajs = [utils.UnrolledTrajectory() for _ in range(n)]
+        for t in trajs:
+            t.initialize()
+        finished = []
+        for _ in range(self.trajectory):
+            out = self.policy.act(np.stack(self.states), self.previous_action, self.h, self.c)
+            action, policy, max_prob = out["action"], out["policy"], out["max_prob"]
+            # fresh copies: rows already stored in a trajectory, and the arrays act returned, are never written again
+            next_pa, next_h, next_c = action.astype(np.int32), out["h"].copy(), out["c"].copy()
+            for i, env in enumerate(self.envs):
+                a = int(action[i])
+                self.episode_step[i] += 1
+                self.total_max_prob[i] += float(max_prob[i])
+                next_state, reward, done, info = env.step(a % self.available_action[i])
+                self.score[i] += reward
+                if self.lives[i] != info["ale.lives"]:
+                    r, d = -1.0, True
+                else:
+                    r, d = reward, False
+                trajs[i].append(state=self.states[i], next_state=next_state, reward=r, done=d, action=a,
+                                behavior_policy=policy[i], previous_action=int(self.previous_action[i]),
+                                initial_h=self.h[i], initial_c=self.c[i])
+                self.states[i] = next_state
+                self.lives[i] = info["ale.lives"]
+                if done:
+                    finished.append(dict(task=i, episode=self.episode[i], score=self.score[i],
+                                         episode_step=self.episode_step[i],
+                                         prob=self.total_max_prob[i] / self.episode_step[i]))
+                    self.episode[i] += 1
+                    self.score[i], self.episode_step[i], self.total_max_prob[i] = 0.0, 0, 0.0
+                    self.states[i] = env.reset()
+                    self.lives[i] = START_LIVES
+                    next_pa[i] = 0
+                    next_h[i] = 0.0
+                    next_c[i] = 0.0
+            self.previous_action, self.h, self.c = next_pa, next_h, next_c
+        for i, t in enumerate(trajs):
+            u = t.extract()
+            self.queue.append_to_queue(
+                task=i, unrolled_state=u["state"], unrolled_next_state=u["next_state"], unrolled_reward=u["reward"],
+                unrolled_done=u["done"], unrolled_behavior_policy=u["behavior_policy"], unrolled_action=u["action"],
+                unrolled_previous_action=u["previous_action"], unrolled_previous_h=u["initial_h"],
+                unrolled_previous_c=u["initial_c"])
+        return finished

@@ -7,6 +7,7 @@ unchanged -- with the TF1 graph + ``tf.Session`` replaced by the CUDA learner be
   Agent.train               agent/impala.py:132-148  -> stage + one fused device step
   Agent.get_policy_and_action  agent/impala.py:118-130
   Agent.parameter_sync      agent/impala.py:111-112  (learner -> this agent's variables)
+  Agent.sync_policy         (new) parameter_sync into a NativePolicy (policy.py), device to device from the learner
   Agent.save_weights / load_weights   agent/impala.py:105-109
 
 The graph attributes the reference exposes (``vs``, ``clipped_rho``, ``vs_plus_1``, ``pg_advantage``,
@@ -140,6 +141,16 @@ class Agent:
                 self._ms = np.ones_like(self._params)
             if self._engine is not None:
                 self._engine.set_params(self._params)
+
+    def sync_policy(self, policy):
+        """parameter_sync into a NativePolicy (the actor side of VectorActor): device to device from this agent's
+        learner when it has one, otherwise from the host copy of the parameters."""
+        with self._lock:
+            if self._engine is not None:
+                policy.sync_from(self._engine)
+            else:
+                self._ensure_init()
+                policy.set_params(self._params)
 
     def set_session(self, sess):
         """Stores the session object (unused) and (re-)initialises every variable, as

@@ -187,6 +187,20 @@ size_t wgrad_partial_floats(int B, int T);
 size_t lstm_image_bytes(int which, int M, int Mb);
 int forward_launch_count();
 int backward_launch_count();
+// the policy engine's convolutions (policy.cu): the math-mode-5 conv1 / conv2 / conv3 forward of net_forward over n
+// single frames on one stream, and the build of its conv2 / conv3 weight images (WeightImages slots 1 and 2 sizes)
+int conv_images16(cudaStream_t s, const ParamLayout& pl, const float* params, uint8_t* img_conv2, uint8_t* img_conv3);
+int conv_forward16(cudaStream_t s, const ParamLayout& pl, const float* params, const uint8_t* img_conv2,
+                   const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3);
+
+// ---- learner.cu: parameter snapshot for the policy engine (drl_policy_sync_from_learner) ---------------------------
+// Under the learner's lock: records ev_ready on the learner's compute stream (after everything enqueued so far, a step
+// in flight included), makes `dst_stream` wait for it, copies the padded parameter vector device to device into `dst`
+// on `dst_stream`, records ev_copied there and makes the compute stream wait for it, so that the learner's next update
+// cannot overwrite the parameters while they are read.  DRL_ERR_INVALID for a learner on another device or with another
+// num_action, DRL_ERR_STATE for a learner in the failed state.
+int learner_params_snapshot(drl_learner* h, int device, int num_action, cudaStream_t dst_stream, float* dst,
+                            cudaEvent_t ev_ready, cudaEvent_t ev_copied);
 
 // ---- elementwise.cu -----------------------------------------------------------------------
 int emb_forward(cudaStream_t s, const float* w1, const float* b1, const float* w2, const float* b2, float* e1,

@@ -228,6 +228,34 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
   return DRL_OK;
 }
 
+// The convolutions of the policy engine (policy.cu): the math-mode-5 kernels and launch configurations of net_forward
+// over n single frames (B = n, T = 1), on one stream.  The conv2 / conv3 weight images are the engine's own and are
+// rebuilt by conv_images16 whenever its parameters change.
+int conv_images16(cudaStream_t s, const ParamLayout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3) {
+  DRL_TRY((launch_retile_b16<64, Fmt16>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, img_conv2)));
+  DRL_TRY((launch_retile_b16<64, Fmt16>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, img_conv3)));
+  return DRL_OK;
+}
+
+int conv_forward16(cudaStream_t s, const ParamLayout& pl, const float* P, const uint8_t* img_conv2,
+                   const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3) {
+  const RowMap map{n, 1};
+  DRL_TRY(launch_conv1_fwd_tma(s, frames, n, map, P + pl.conv1_w, EpConv1{a1, 32, P + pl.conv1_b}));
+  {
+    Conv2A al{a1, map};
+    PretiledB<PlainB> blp{img_conv2, 512 / 64};
+    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
+    DRL_TRY((launch_gemm_umma16<X64L8x2>(s, al, blp, ep, n * 81, 64, 512, 1, 512, 0)));
+  }
+  {
+    Conv3A al{a2, map};
+    PretiledB<PlainB> blp{img_conv3, 576 / 64};
+    EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
+    DRL_TRY((launch_gemm_umma16<X64L8x2>(s, al, blp, ep, n * 49, 64, 576, 1, 576, 0)));
+  }
+  return DRL_OK;
+}
+
 int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const WeightImages& wi, float* G,
                  const Inputs& in, const Acts& act, const Bwd& bw, int B, int T, int mode) {
   const bool m16 = mode == 5;

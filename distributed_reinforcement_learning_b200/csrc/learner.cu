@@ -336,6 +336,32 @@ int run_step(drl_learner* h, int slot) {
 
 }  // namespace
 
+namespace drl {
+int learner_params_snapshot(drl_learner* h, int device, int num_action, cudaStream_t dst_stream, float* dst,
+                            cudaEvent_t ev_ready, cudaEvent_t ev_copied) {
+  DRL_TRY(check_handle(h));
+  DRL_LOCK(h);
+  DRL_TRY(check_not_failed(h));
+  if (h->cfg.device != device) {
+    set_error("sync: the learner is on device %d, the policy on device %d (no cross-device sync)", h->cfg.device, device);
+    return DRL_ERR_INVALID;
+  }
+  if (h->A != num_action) {
+    set_error("sync: the learner has num_action %d, the policy %d", h->A, num_action);
+    return DRL_ERR_INVALID;
+  }
+  DRL_TRY(set_device(h));
+  NvtxRange r("drl:learner_snapshot");
+  DRL_CUDA_CHECK(cudaEventRecord(ev_ready, h->compute));
+  DRL_CUDA_CHECK(cudaStreamWaitEvent(dst_stream, ev_ready, 0));
+  DRL_CUDA_CHECK(cudaMemcpyAsync(dst, h->params, (size_t)h->pl.padded_total * sizeof(float), cudaMemcpyDeviceToDevice,
+                                 dst_stream));
+  DRL_CUDA_CHECK(cudaEventRecord(ev_copied, dst_stream));
+  DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, ev_copied, 0));
+  return DRL_OK;
+}
+}  // namespace drl
+
 extern "C" {
 
 const char* drl_last_error(void) { return get_error(); }

@@ -188,6 +188,47 @@ int drl_learner_last_step_ms(drl_learner* h, float* ms);
 int drl_learner_launches_per_step(const drl_learner* h, int32_t* n);
 
 /* ------------------------------------------------------------------------------------------
+ * IMPALA policy engine (new): the actor side of train_impala.py:132-194 (the actor loop's batched forward and
+ * sampling; the loop itself is distributed_reinforcement_learning_b200/actor.py).  A forward-only handle that serves
+ * Agent.get_policy_and_action (agent/impala.py:118-130) for up to 64 environments per call, on its own stream next to a
+ * training learner, and takes the learner's parameters device to device (parameter_sync, agent/impala.py:111-112).
+ * It holds no optimizer state, gradients or backward buffers.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_policy drl_policy;
+
+typedef struct drl_policy_config {
+  int32_t max_batch;                 /* 1..64 rows (environments) per drl_policy_act call             */
+  int32_t height, width, channels;   /* 84,84,4 -- only this geometry is supported (as the learner)   */
+  int32_t num_action;                /* A, 2..32                                                      */
+  int32_t lstm_size;                 /* 256 -- only this size is supported                            */
+  int32_t device;                    /* CUDA device ordinal                                           */
+  int32_t use_cuda_graph;            /* 1: one CUDA graph per row count n (input copy + 5 kernels)    */
+} drl_policy_config;
+
+int drl_policy_create(const drl_policy_config* cfg, drl_policy** out);
+int drl_policy_destroy(drl_policy* h);
+/* Same inventory and flat TF order as drl_learner_param_count / _set_params / _get_params. */
+int drl_policy_param_count(const drl_policy* h, int64_t* n);
+int drl_policy_set_params(drl_policy* h, const float* host_flat, int64_t n);
+int drl_policy_get_params(drl_policy* h, float* host_flat, int64_t n);
+/* parameter_sync (agent/impala.py:111-112) without a host round trip: the snapshot is the learner's parameters after
+ * all work enqueued on it so far (a step in flight included), copied device to device on the policy's stream; the
+ * learner's next update waits for the copy.  The learner must be on the same device and have the same num_action
+ * (DRL_ERR_INVALID otherwise); a learner in the failed state is DRL_ERR_STATE.  Returns without waiting for the copy. */
+int drl_policy_sync_from_learner(drl_policy* h, drl_learner* learner);
+/* Agent.get_policy_and_action (agent/impala.py:118-130) for n <= max_batch environments, with the sampling on the GPU.
+ * state u8 [n,H,W,C]; previous_action i32 [n] in [0, A); h_in, c_in f32 [n,L]; uniform f64 [n] in [0, 1) or NULL ->
+ * policy f32 [n,A] (the actor head's softmax), h_out, c_out f32 [n,L], action i32 [n].  Per row the action is the
+ * number of entries of cdf = cumsum(float64(policy)) / cdf[A-1] that are <= uniform, clamped to A-1: exactly what
+ * numpy's legacy RandomState.choice(A, p=policy) picks from u = random_sample().  Synchronous (the outputs are in the
+ * caller's memory on return); any output pointer may be NULL; `action` without `uniform` is DRL_ERR_INVALID. */
+int drl_policy_act(drl_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action, const float* h_in,
+                   const float* c_in, const double* uniform, int32_t* action, float* policy, float* h_out,
+                   float* c_out);
+/* Device time of the most recent drl_policy_act (input copy + kernels; CUDA events on the policy's stream), ms. */
+int drl_policy_last_act_ms(drl_policy* h, float* ms);
+
+/* ------------------------------------------------------------------------------------------
  * Stand-alone V-trace (optimizer/vtrace.py), host-pointer convenience forms + device forms.
  * ------------------------------------------------------------------------------------------ */
 /* vtrace.from_importance_weights (optimizer/vtrace.py:71-103): time-major [T,B] float32 inputs,
