@@ -1,6 +1,7 @@
-"""Vector actor: the actor branch of ``train_impala.py:117-194`` for N environments in lockstep on one NativePolicy.
+"""Vector actors: the actor branches of ``train_impala.py:117-194`` (VectorActor, on one NativePolicy) and of
+``train_r2d2.py:167-251`` (R2D2VectorActor, on one NativeR2D2Policy) for N environments in lockstep.
 
-Each environment is its own actor task ``i`` (what ``FLAGS.task`` selects in the reference).  Per unroll:
+VectorActor: each environment is its own actor task ``i`` (what ``FLAGS.task`` selects in the reference).  Per unroll:
 
   - one parameter sync through ``learner.sync_policy(policy)`` (the learner-side ``impala.Agent``; device to device
     when it has a CUDA learner);
@@ -15,6 +16,7 @@ Each environment is its own actor task ``i`` (what ``FLAGS.task`` selects in the
 import numpy as np
 
 from . import utils
+from .distributed_queue import buffer_queue
 
 START_LIVES = 5   # the reference actor's life counter starts (and restarts after every episode) at 5
 
@@ -90,4 +92,92 @@ class VectorActor:
                 unrolled_done=u["done"], unrolled_behavior_policy=u["behavior_policy"], unrolled_action=u["action"],
                 unrolled_previous_action=u["previous_action"], unrolled_previous_h=u["initial_h"],
                 unrolled_previous_c=u["initial_c"])
+        return finished
+
+
+class R2D2VectorActor:
+    """The actor branch of ``train_r2d2.py:167-251`` for N environments in lockstep on one NativeR2D2Policy; each
+    environment is its own actor task ``i``.  Per unroll:
+
+      - every environment's ``R2D2TrajectoryBuffer.init()``, then one ``learner.sync_policy(policy)`` (the
+        learner-side ``r2d2.Agent``; device to device when it has a CUDA learner);
+      - ``seq_len`` batched ``policy.act`` calls with each environment's epsilon: the explore draws of environments
+        0..n-1 from the global ``np.random`` stream, in that order, then ``env.step(action)`` for 0..n-1 with the raw
+        action (the R2D2 actor applies no ``% available_action``);
+      - ``lives`` is only ever set back to 5 by an episode reset, never after a life loss, so every step after the
+        first life loss of an episode is stored as reward -1 and done=True (the reference's behaviour, SURVEY.md
+        App. D); the score keeps the raw reward;
+      - at an episode's end epsilon becomes 1 / (0.01 episode + 1), and the environment, the previous action, h, c
+        and lives are reset.  episode_step and the summed q of the logged average are never reset, as in the
+        reference;
+      - every environment's trajectory goes to ``queue.append_to_queue(task=i, ...)``.
+    At n = 1 this is the reference actor's loop, including the order of its ``np.random`` draws.
+    """
+
+    def __init__(self, policy, envs, queue, seq_len, learner=None):
+        self.policy, self.envs, self.queue, self.learner = policy, list(envs), queue, learner
+        self.seq_len = int(seq_len)
+        n = len(self.envs)
+        if not 1 <= n <= policy.max_batch:
+            raise ValueError("%d environments, the policy serves 1..%d per call" % (n, policy.max_batch))
+        L = policy.L
+        self.buffers = [buffer_queue.R2D2TrajectoryBuffer(seq_len=self.seq_len) for _ in range(n)]
+        self.states = [env.reset() for env in self.envs]
+        self.previous_action = np.zeros(n, np.int32)
+        self.h = np.zeros((n, L), np.float32)
+        self.c = np.zeros((n, L), np.float32)
+        self.lives = [START_LIVES] * n
+        self.episode = [0] * n
+        self.epsilon = [1.0] * n
+        self.score = [0.0] * n
+        self.episode_step = [0] * n
+        self.episode_q_value = [0.0] * n
+
+    def run_unroll(self):
+        """One unroll of `seq_len` steps for every environment, pushed to the queue.  Returns the episodes that
+        finished during it: dicts of task, episode, score, epsilon, episode_step and avg_q_value, the values
+        train_r2d2.py:227-230 logs."""
+        for b in self.buffers:
+            b.init()
+        if self.learner is not None:
+            self.learner.sync_policy(self.policy)
+        finished = []
+        for _ in range(self.seq_len):
+            out = self.policy.act(np.stack(self.states), self.previous_action, self.h, self.c,
+                                  epsilon=np.array(self.epsilon))
+            action, q_action = out["action"], out["q_action"]
+            # fresh copies: rows already stored in a trajectory, and the arrays act returned, are never written again
+            next_pa, next_h, next_c = action.astype(np.int32), out["h"].copy(), out["c"].copy()
+            for i, env in enumerate(self.envs):
+                a = int(action[i])
+                self.episode_q_value[i] += float(q_action[i])
+                self.episode_step[i] += 1
+                next_state, reward, done, info = env.step(a)
+                self.score[i] += reward
+                if self.lives[i] != info["ale.lives"]:
+                    r, d = -1, True
+                else:
+                    r, d = reward, False
+                self.buffers[i].append(state=self.states[i], previous_action=int(self.previous_action[i]), action=a,
+                                       reward=r, done=d, initial_h=self.h[i], initial_c=self.c[i])
+                self.states[i] = next_state
+                if done:
+                    finished.append(dict(task=i, episode=self.episode[i], score=self.score[i],
+                                         epsilon=self.epsilon[i], episode_step=self.episode_step[i],
+                                         avg_q_value=self.episode_q_value[i] / self.episode_step[i]))
+                    self.episode[i] += 1
+                    self.score[i] = 0
+                    self.epsilon[i] = 1.0 / (0.01 * self.episode[i] + 1)
+                    self.states[i] = env.reset()
+                    next_pa[i] = 0
+                    next_h[i] = 0.0
+                    next_c[i] = 0.0
+                    self.lives[i] = START_LIVES
+            self.previous_action, self.h, self.c = next_pa, next_h, next_c
+        for i, b in enumerate(self.buffers):
+            u = b.extract()
+            self.queue.append_to_queue(
+                task=i, unrolled_state=u["state"], unrolled_previous_action=u["previous_action"],
+                unrolled_action=u["action"], unrolled_reward=u["reward"], unrolled_done=u["done"],
+                unrolled_previous_h=u["initial_h"], unrolled_previous_c=u["initial_c"])
         return finished

@@ -6,6 +6,7 @@ the learner branch of ``train_r2d2.py:87-165`` runs on it unchanged, with the TF
   Agent.train          agent/r2d2.py:132-159 -> (loss, td_error [B])
   Agent.parameter_sync agent/r2d2.py:161-162 ; Agent.main_to_target :164-165 ; Agent.set_session :167-169
   Agent.get_action     agent/r2d2.py:171-191 -> (action, q_value[action], h', c')
+  Agent.sync_policy    (new) parameter_sync into a NativeR2D2Policy (r2d2_policy.py), device to device from the learner
   Agent.main_q_value_test / target_q_value_test   agent/r2d2.py:193-217
 """
 import os
@@ -123,6 +124,16 @@ class Agent:
             if self._engine is not None:
                 self._engine.set_params(self._main, MAIN)
                 self._engine.set_params(self._target, TARGET)
+
+    def sync_policy(self, policy):
+        """parameter_sync into a NativeR2D2Policy (the actor side of R2D2VectorActor): device to device from this
+        agent's learner when it has one, otherwise from the host copy of the main parameters."""
+        with self._lock:
+            if self._engine is not None:
+                policy.sync_from(self._engine)
+            else:
+                self._ensure_init()
+                policy.set_params(self._main)
 
     def main_to_target(self):
         self._ensure_init()

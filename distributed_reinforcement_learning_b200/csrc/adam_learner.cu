@@ -394,6 +394,24 @@ int adam_main_to_target(AdamLearner* h, const char* family) {
   return DRL_OK;
 }
 
+int adam_params_snapshot(AdamLearner* h, const char* family, int device, cudaStream_t dst_stream, float* dst,
+                         cudaEvent_t ev_ready, cudaEvent_t ev_copied) {
+  DRL_TRY(check_handle(h, family));
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  if (h->device != device) {
+    set_error("sync: the learner is on device %d, the policy on device %d (no cross-device sync)", h->device, device);
+    return DRL_ERR_INVALID;
+  }
+  DRL_TRY(set_device(h));
+  DRL_CUDA_CHECK(cudaEventRecord(ev_ready, h->compute));
+  DRL_CUDA_CHECK(cudaStreamWaitEvent(dst_stream, ev_ready, 0));
+  DRL_CUDA_CHECK(cudaMemcpyAsync(dst, h->params, (size_t)h->layout->padded_total * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, dst_stream));
+  DRL_CUDA_CHECK(cudaEventRecord(ev_copied, dst_stream));
+  DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, ev_copied, 0));
+  return DRL_OK;
+}
+
 int adam_step_async(AdamLearner* h, const char* family, int slot) {
   DRL_TRY(check_handle(h, family));
   std::lock_guard<std::recursive_mutex> lk(h->mu);

@@ -81,6 +81,13 @@ int adam_get_opt_state(AdamLearner* h, const char* family, float* host_m, float*
                        float* beta1_power, float* beta2_power);
 int adam_get_grads(AdamLearner* h, const char* family, float* host_flat, int64_t n);
 int adam_main_to_target(AdamLearner* h, const char* family);
+// Parameter snapshot for a policy engine, under the learner's lock: records ev_ready on the compute stream (after
+// everything enqueued so far, a step in flight included), makes dst_stream wait for it, copies the padded main
+// parameters device to device into dst on dst_stream, records ev_copied there and makes the compute stream wait for it,
+// so that the next update cannot overwrite the parameters while they are read.  Does not block the host.
+// DRL_ERR_INVALID for a learner on another device; the family checks that the networks match.
+int adam_params_snapshot(AdamLearner* h, const char* family, int device, cudaStream_t dst_stream, float* dst,
+                         cudaEvent_t ev_ready, cudaEvent_t ev_copied);
 int adam_step_async(AdamLearner* h, const char* family, int slot);
 int adam_forward_backward(AdamLearner* h, const char* family, int slot);
 int adam_grad_bucket(AdamLearner* h, const char* family, void** dev_ptr, int64_t* count);

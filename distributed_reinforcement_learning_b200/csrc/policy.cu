@@ -18,8 +18,8 @@
 
 #include <nvtx3/nvToolsExt.h>
 
-#include "gemm_umma.cuh"   // umma:: mbarrier / bulk-copy helpers
 #include "kernels.h"
+#include "policy_lstm.cuh"
 
 namespace drl {
 namespace {
@@ -31,102 +31,10 @@ struct PolicyNvtx {
 
 constexpr int kMaxPolicyRows = 64;
 
-// ---- policy_lstm_fwd --------------------------------------------------------------------------------------------
+// ---- policy_lstm_fwd (policy_lstm.cuh) --------------------------------------------------------------------------
 // grid (1024 / kLN column chunks) x (kLSplits K splits) = 8 x 16 = 128 CTAs: one wave on the 132 SMs of an H100, each
-// streaming its 228 x 128 fp32 slab of W (114 KB) once.  The slab arrives by 228 row-wise cp.async.bulk copies of 512 B
-// (all in flight at once, completing on kLStages mbarriers so the FFMA loop starts on the first third); the CTA's
-// [R x 228] slice of x is gathered into shared memory meanwhile.  Thread (c, g): columns c and c + 64 for the rows
-// [g R/4, (g+1) R/4) -- per 4 k: 8 conflict-free LDS of W and R/4 broadcast LDS.128 of x for 2 R FFMA.
-constexpr int kLN = 128;
+// streaming its 228 x 128 fp32 slab of W (114 KB) once.
 constexpr int kLSplits = 16;
-constexpr int kLK = Geo::XK / kLSplits;        // 228
-constexpr int kLStages = 3;
-constexpr int kLStageK = kLK / kLStages;       // 76
-constexpr int kLThreads = 256;
-static_assert(kLK * kLSplits == Geo::XK && kLStageK * kLStages == kLK && kLStageK % 4 == 0, "LSTM split tiling");
-static_assert(Geo::FLAT % 4 == 0 && (Geo::FLAT + Geo::EMB) % 4 == 0 && kLK % 4 == 0, "float4 gather");
-
-constexpr size_t lstm_smem_bytes(int R) { return (size_t)kLK * kLN * 4 + (size_t)R * kLK * 4 + 8 * kLStages; }
-
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(umma::smem_u32(bar)), "r"(bytes) : "memory");
-}
-
-template <int R>
-__global__ void __launch_bounds__(kLThreads, 1) policy_lstm_fwd_kernel(
-    const float* __restrict__ a3, const float* __restrict__ table, const int32_t* __restrict__ pa,
-    const float* __restrict__ h0, const float* __restrict__ w, float* __restrict__ zpart, int n) {
-  kernel_prologue();
-  extern __shared__ __align__(128) uint8_t smem[];
-  float* sw = reinterpret_cast<float*>(smem);     // [kLK][kLN]
-  float* sx = sw + kLK * kLN;                      // [R][kLK]
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sx + R * kLK);
-  const int tid = threadIdx.x;
-  const int n0 = blockIdx.x * kLN, split = blockIdx.y, k0 = split * kLK;
-  if (tid == 0) {
-    for (int s = 0; s < kLStages; ++s) umma::mbar_init(&bar[s], 1);
-    umma::fence_barrier_init();
-  }
-  __syncthreads();
-  if (tid < 32) {
-    for (int s = 0; s < kLStages; ++s) {
-      if (tid == 0) mbar_arrive_expect_tx(&bar[s], kLStageK * kLN * 4);
-      __syncwarp();
-      for (int k = s * kLStageK + tid; k < (s + 1) * kLStageK; k += 32)
-        umma::bulk_g2s(sw + k * kLN, w + (size_t)(k0 + k) * Geo::G4 + n0, kLN * 4, &bar[s]);
-    }
-  }
-  // x = [a3 | table[pa] | h0] over this CTA's K range (every float4 lies in one of the three parts); rows >= n are zero
-  constexpr int K4 = kLK / 4;
-  for (int i = tid; i < R * K4; i += kLThreads) {
-    const int r = i / K4, q = i - r * K4, k = k0 + 4 * q;
-    float4 v = zero4();
-    if (r < n) {
-      if (k < Geo::FLAT) v = ldg4(a3 + (size_t)r * Geo::FLAT + k);
-      else if (k < Geo::FLAT + Geo::EMB) v = ldg4(table + (size_t)__ldg(pa + r) * Geo::EMB + (k - Geo::FLAT));
-      else v = ldg4(h0 + (size_t)r * Geo::L + (k - Geo::FLAT - Geo::EMB));
-    }
-    reinterpret_cast<float4*>(sx + r * kLK)[q] = v;
-  }
-  __syncthreads();
-  constexpr int RT = R / 4;
-  const int c = tid & 63, r0 = (tid >> 6) * RT;
-  float acc0[RT], acc1[RT];
-#pragma unroll
-  for (int r = 0; r < RT; ++r) acc0[r] = acc1[r] = 0.f;
-  for (int s = 0; s < kLStages; ++s) {
-    umma::mbar_wait(&bar[s], 0);
-#pragma unroll 2
-    for (int k = s * kLStageK; k < (s + 1) * kLStageK; k += 4) {
-      float w0[4], w1[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        w0[j] = sw[(k + j) * kLN + c];
-        w1[j] = sw[(k + j) * kLN + c + 64];
-      }
-#pragma unroll
-      for (int r = 0; r < RT; ++r) {
-        const float4 x = *reinterpret_cast<const float4*>(sx + (r0 + r) * kLK + k);
-        acc0[r] = fmaf(x.x, w0[0], acc0[r]);
-        acc1[r] = fmaf(x.x, w1[0], acc1[r]);
-        acc0[r] = fmaf(x.y, w0[1], acc0[r]);
-        acc1[r] = fmaf(x.y, w1[1], acc1[r]);
-        acc0[r] = fmaf(x.z, w0[2], acc0[r]);
-        acc1[r] = fmaf(x.z, w1[2], acc1[r]);
-        acc0[r] = fmaf(x.w, w0[3], acc0[r]);
-        acc1[r] = fmaf(x.w, w1[3], acc1[r]);
-      }
-    }
-  }
-  float* out = zpart + (size_t)split * n * Geo::G4 + n0;
-#pragma unroll
-  for (int r = 0; r < RT; ++r) {
-    if (r0 + r < n) {
-      out[(size_t)(r0 + r) * Geo::G4 + c] = acc0[r];
-      out[(size_t)(r0 + r) * Geo::G4 + c + 64] = acc1[r];
-    }
-  }
-}
 
 // ---- policy_head_fused ------------------------------------------------------------------------------------------
 // One CTA per kHR rows, 256 threads.  With 8 rows per CTA the 0.54 MB of actor-head weights is read from L2 once per 8
@@ -295,23 +203,8 @@ InLayout in_layout(int n) {
   return l;
 }
 
-template <int R>
-int launch_policy_lstm(cudaStream_t s, const float* a3, const float* table, const int32_t* pa, const float* h0,
-                       const float* w, float* zpart, int n) {
-  DRL_CUDA_CHECK((launch_k(policy_lstm_fwd_kernel<R>, dim3(Geo::G4 / kLN, kLSplits), kLThreads, lstm_smem_bytes(R), s,
-                           a3, table, pa, h0, w, zpart, n)));
-  return DRL_OK;
-}
-
 int set_policy_kernel_attributes() {
-  DRL_CUDA_CHECK(cudaFuncSetAttribute(policy_lstm_fwd_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)lstm_smem_bytes(8)));
-  DRL_CUDA_CHECK(cudaFuncSetAttribute(policy_lstm_fwd_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)lstm_smem_bytes(16)));
-  DRL_CUDA_CHECK(cudaFuncSetAttribute(policy_lstm_fwd_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)lstm_smem_bytes(32)));
-  DRL_CUDA_CHECK(cudaFuncSetAttribute(policy_lstm_fwd_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)lstm_smem_bytes(64)));
+  DRL_TRY((set_policy_lstm_attributes<Geo::L, kLSplits>()));
   DRL_CUDA_CHECK(cudaFuncSetAttribute(policy_head_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)kHeadSmem));
   return DRL_OK;
@@ -372,11 +265,7 @@ int enqueue_act(drl_policy* h, int n) {
   const int32_t* pa = reinterpret_cast<const int32_t*>(h->d_in + l.pa);
   const float* h0 = reinterpret_cast<const float*>(h->d_in + l.h0);
   DRL_TRY(conv_forward16(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3));
-  const float* w = P + pl.lstm_w;
-  if (n <= 8) DRL_TRY(launch_policy_lstm<8>(s, h->a3, h->table, pa, h0, w, h->zpart, n));
-  else if (n <= 16) DRL_TRY(launch_policy_lstm<16>(s, h->a3, h->table, pa, h0, w, h->zpart, n));
-  else if (n <= 32) DRL_TRY(launch_policy_lstm<32>(s, h->a3, h->table, pa, h0, w, h->zpart, n));
-  else DRL_TRY(launch_policy_lstm<64>(s, h->a3, h->table, pa, h0, w, h->zpart, n));
+  DRL_TRY((launch_policy_lstm<Geo::L, kLSplits>(s, h->a3, h->table, pa, h0, P + pl.lstm_w, h->zpart, n)));
   HeadArgs a;
   a.zpart = h->zpart;
   a.lstm_b = P + pl.lstm_b;

@@ -17,30 +17,9 @@
 
 #include "adam_learner.cuh"
 #include "layer_defs.cuh"
+#include "r2d2_defs.cuh"
 
 namespace drl {
-
-constexpr int kR2L = 64;                 // lstm_size (config.json:93): the recurrence kernels keep W_h (L x 4L) on chip
-constexpr int kR2G = 4 * kR2L;           // 256 gate columns
-constexpr int kR2H = 128;                // dense width between the LSTM and the two output streams (model/r2d2_lstm.py:50)
-constexpr int kR2Cat = Geo::FLAT + Geo::EMB;   // 3392 rows of the LSTM kernel that multiply the step input
-
-struct R2Layout : FlatLayout {
-  int A, C;
-  int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b, emb1_w, emb1_b, emb2_w, emb2_b;
-  int64_t lstm_w, lstm_b, q1_w, q1_b, value_w, value_b, mean_w, mean_b;
-  void init(int num_action, int channels) {
-    A = num_action; C = channels;
-    const int64_t sizes[] = {
-        8 * 8 * (int64_t)C * 32, 32, 4 * 4 * 32 * 64, 64, 3 * 3 * 64 * 64, 64,
-        (int64_t)A * 256, 256, 256 * 256, 256,
-        (int64_t)(kR2Cat + kR2L) * kR2G, kR2G,
-        (int64_t)kR2L * kR2H, kR2H, (int64_t)kR2H * A, A, kR2H, 1};
-    int64_t* const named[] = {&conv1_w, &conv1_b, &conv2_w, &conv2_b, &conv3_w, &conv3_b, &emb1_w, &emb1_b, &emb2_w,
-                              &emb2_b, &lstm_w, &lstm_b, &q1_w, &q1_b, &value_w, &value_b, &mean_w, &mean_b};
-    set(sizes, named);
-  }
-};
 
 struct R2Acts {            // activations of one scope, time-major rows m = t*B + b
   float *a1, *a2, *a3, *e1, *table;
@@ -68,8 +47,7 @@ struct R2In {              // one staged minibatch, caller's batch-major layout
   const float* weight;     // [B]
 };
 
-// conv1 over single-channel frames (config.json:91 model_input [84, 84, 1]); the 4-channel instantiations are layer_defs'
-using Conv1A1 = ConvFwdA<uint8_t, 84, 84, 1, 20, 20, 8, 4, true>;
+// conv1 weight gradient over single-channel frames (Conv1A1: r2d2_defs.cuh)
 using Conv1WA1 = ConvWgradA<uint8_t, 84, 84, 1, 20, 20, 8, 4, true>;
 
 // [x | h_in]^T for the LSTM kernel gradient: feature index i < 3392 -> [a3 | emb] (as LstmAT), else h_in (device, time-major)
@@ -401,6 +379,48 @@ __global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
 
 constexpr size_t kR2FwdSmem = 0, kR2BwdSmem = 0;     // the recurrence kernels only use small static shared arrays
 
+int r2_conv_forward(cudaStream_t s, const R2Layout& pl, const float* P, const uint8_t* img_conv2,
+                    const uint8_t* img_conv3, const uint8_t* frames, int B, int S, float* a1, float* a2, float* a3,
+                    int mode, bool tgt, cudaEvent_t images_ready, int* launches) {
+  const int M = B * S;
+  const RowMap map{B, S};
+  int n = 0;
+  if (pl.C == 1) {
+    Conv1A1 al{frames, map};
+    PlainB bl{P + pl.conv1_w, 32, 0};
+    EpConv1 ep{a1, 32, P + pl.conv1_b};
+    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 64, 1, 64, 0);
+  } else {
+    Conv1A al{frames, map};
+    PlainB bl{P + pl.conv1_w, 32, 0};
+    EpConv1 ep{a1, 32, P + pl.conv1_b};
+    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
+  }
+  if (images_ready) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, images_ready, 0));
+  {
+    Conv2A al{a1, map};
+    PlainB bl{P + pl.conv2_w, 64, 0};
+    PretiledB<PlainB> blp{img_conv2, 512 / 32};
+    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
+    GEMM_W(tgt ? "target_conv2_fwd" : "conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
+  }
+  {
+    Conv3A al{a2, map};
+    PlainB bl{P + pl.conv3_w, 64, 0};
+    PretiledB<PlainB> blp{img_conv3, 576 / 32};
+    EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
+    GEMM_W(tgt ? "target_conv3_fwd" : "conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
+  }
+  *launches += n;
+  return DRL_OK;
+}
+
+int r2_conv_images(cudaStream_t s, const R2Layout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3) {
+  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, img_conv2)));
+  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, img_conv3)));
+  return DRL_OK;
+}
+
 // Forward of one scope over B sequences of S steps (rows m = t*B + b).  c_last (optional): un-masked c_t (act path).
 static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, const WeightImages& wi, const R2In& in,
                       const R2Acts& act, float* c_last, int B, int S, int mode, bool retile_fwd, bool retile_bwd, bool tgt,
@@ -428,32 +448,8 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
     n += 2;
   }
   s = st.main;
-  if (pl.C == 1) {
-    Conv1A1 al{in.frames, map};
-    PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
-    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 64, 1, 64, 0);
-  } else {
-    Conv1A al{in.frames, map};
-    PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
-    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
-  }
-  if (st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
-  {
-    Conv2A al{act.a1, map};
-    PlainB bl{P + pl.conv2_w, 64, 0};
-    PretiledB<PlainB> blp{wi.img[1], 512 / 32};
-    EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv2_fwd" : "conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
-  }
-  {
-    Conv3A al{act.a2, map};
-    PlainB bl{P + pl.conv3_w, 64, 0};
-    PretiledB<PlainB> blp{wi.img[2], 576 / 32};
-    EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv3_fwd" : "conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
-  }
+  DRL_TRY(r2_conv_forward(s, pl, P, wi.img[1], wi.img[2], in.frames, B, S, act.a1, act.a2, act.a3, mode, tgt,
+                          st.par ? st.ev[7] : nullptr, &n));
   DRL_TRY(join_from_side(st, 1));
   // input half of the LSTM contraction for all S steps at once: [M, 3392] x W[:3392, :4L] (split-K partial sums)
   const SplitPlan sp = plan_r2_x(M, mode);
@@ -847,6 +843,22 @@ int drl_r2d2_stage(drl_r2d2* h, int32_t slot, const uint8_t* state, const int32_
   s.has_data = true;
   return DRL_OK;
 }
+
+}  // extern "C"
+
+int drl::r2d2_params_snapshot(drl_r2d2* h, int device, int num_action, int channels, cudaStream_t dst_stream,
+                              float* dst, cudaEvent_t ev_ready, cudaEvent_t ev_copied) {
+  DRL_TRY(check_handle(h, kName));
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  if (h->A != num_action || h->C != channels) {
+    set_error("sync: the learner has num_action %d and %d channels, the policy %d and %d", h->A, h->C, num_action,
+              channels);
+    return DRL_ERR_INVALID;
+  }
+  return adam_params_snapshot(h, kName, device, dst_stream, dst, ev_ready, ev_copied);
+}
+
+extern "C" {
 
 int drl_r2d2_step_async(drl_r2d2* h, int32_t slot) { return adam_step_async(h, kName, slot); }
 int drl_r2d2_forward_backward(drl_r2d2* h, int32_t slot) { return adam_forward_backward(h, kName, slot); }

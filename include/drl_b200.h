@@ -229,6 +229,47 @@ int drl_policy_act(drl_policy* h, int32_t n, const uint8_t* state, const int32_t
 int drl_policy_last_act_ms(drl_policy* h, float* ms);
 
 /* ------------------------------------------------------------------------------------------
+ * R2D2 policy engine (new): the actor side of train_r2d2.py:167-251 (the actor loop itself is
+ * distributed_reinforcement_learning_b200/actor.py: R2D2VectorActor).  A forward-only handle that serves
+ * Agent.get_action (agent/r2d2.py:171-191) for up to 64 environments per call, on its own stream next to a training
+ * R2D2 learner, and takes the learner's main-scope parameters device to device.  The explore decision and the random
+ * action are drawn on the host (numpy's global stream, as the reference); the argmax and the selection run on the GPU.
+ * It holds no target scope, optimizer state, gradients or backward buffers.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_r2d2_policy drl_r2d2_policy;
+
+typedef struct drl_r2d2_policy_config {
+  int32_t max_batch;                 /* 1..64 rows (environments) per drl_r2d2_policy_act call        */
+  int32_t height, width, channels;   /* 84,84,1 or 84,84,4 (as drl_r2d2_create)                        */
+  int32_t num_action;                /* A, 2..32                                                      */
+  int32_t lstm_size;                 /* 64 -- only this size is supported (as the learner)            */
+  int32_t device;                    /* CUDA device ordinal                                           */
+  int32_t use_cuda_graph;            /* 1: one CUDA graph per row count n (input copy + kernels)      */
+} drl_r2d2_policy_config;
+
+int drl_r2d2_policy_create(const drl_r2d2_policy_config* cfg, drl_r2d2_policy** out);
+int drl_r2d2_policy_destroy(drl_r2d2_policy* h);
+/* The R2D2 learner's main-scope inventory and flat TF order (drl_r2d2_param_count / drl_r2d2_get_params(.., 0, ..)). */
+int drl_r2d2_policy_param_count(const drl_r2d2_policy* h, int64_t* n);
+int drl_r2d2_policy_set_params(drl_r2d2_policy* h, const float* host_flat, int64_t n);
+int drl_r2d2_policy_get_params(drl_r2d2_policy* h, float* host_flat, int64_t n);
+/* parameter_sync without a host round trip: the learner's main parameters after all work enqueued on it so far (a step
+ * in flight included), copied device to device on the policy's stream; the learner's next update waits for the copy.
+ * The learner must be on the same device and have the same num_action and channels (DRL_ERR_INVALID otherwise).
+ * Returns without waiting for the copy. */
+int drl_r2d2_policy_sync_from_learner(drl_r2d2_policy* h, struct drl_r2d2* learner);
+/* Agent.get_action (agent/r2d2.py:171-191) for n <= max_batch environments.  state u8 [n,H,W,C]; previous_action i32
+ * [n] in [0, A); h_in, c_in f32 [n,64]; explore_action i32 [n] or NULL -> q f32 [n,A] (value - mean of the main scope),
+ * action i32 [n], q_action f32 [n] (= q[action]), h_out, c_out f32 [n,64].  Per row, explore_action -1 (or NULL) is the
+ * greedy action, the first maximum of q (np.argmax); a value in [0, A) is taken as the action; anything else is
+ * DRL_ERR_INVALID.  Synchronous (the outputs are in the caller's memory on return); any output pointer may be NULL. */
+int drl_r2d2_policy_act(drl_r2d2_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action,
+                        const float* h_in, const float* c_in, const int32_t* explore_action, int32_t* action, float* q,
+                        float* q_action, float* h_out, float* c_out);
+/* Device time of the most recent drl_r2d2_policy_act (input copy + kernels; CUDA events on the policy's stream), ms. */
+int drl_r2d2_policy_last_act_ms(drl_r2d2_policy* h, float* ms);
+
+/* ------------------------------------------------------------------------------------------
  * Stand-alone V-trace (optimizer/vtrace.py), host-pointer convenience forms + device forms.
  * ------------------------------------------------------------------------------------------ */
 /* vtrace.from_importance_weights (optimizer/vtrace.py:71-103): time-major [T,B] float32 inputs,
