@@ -89,6 +89,11 @@ class R2d2PolicyConfig(C.Structure):
                 ("use_cuda_graph", C.c_int32)]
 
 
+class ApexPolicyConfig(C.Structure):
+    _fields_ = [("max_batch", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32),
+                ("num_action", C.c_int32), ("algo", C.c_int32), ("device", C.c_int32), ("use_cuda_graph", C.c_int32)]
+
+
 class RingBatch(C.Structure):
     _fields_ = [("state", C.c_void_p), ("reward", C.c_void_p), ("done", C.c_void_p),
                 ("behavior_policy", C.c_void_p), ("action", C.c_void_p), ("previous_action", C.c_void_p),
@@ -152,6 +157,15 @@ def _load():
         "drl_r2d2_policy_sync_from_learner": (C.c_int, [vp, vp]),
         "drl_r2d2_policy_act": (C.c_int, [vp, i32] + [vp] * 10),
         "drl_r2d2_policy_last_act_ms": (C.c_int, [vp, C.POINTER(f32)]),
+        "drl_apex_policy_create": (C.c_int, [C.POINTER(ApexPolicyConfig), C.POINTER(vp)]),
+        "drl_apex_policy_destroy": (C.c_int, [vp]),
+        "drl_apex_policy_param_count": (C.c_int, [vp, C.POINTER(i64)]),
+        "drl_apex_policy_set_params": (C.c_int, [vp, vp, i64]),
+        "drl_apex_policy_get_params": (C.c_int, [vp, vp, i64]),
+        "drl_apex_policy_sync_from_learner": (C.c_int, [vp, vp]),
+        "drl_apex_policy_act": (C.c_int, [vp, i32] + [vp] * 6),
+        "drl_a3c_policy_act": (C.c_int, [vp, i32] + [vp] * 6),
+        "drl_apex_policy_last_act_ms": (C.c_int, [vp, C.POINTER(f32)]),
         "drl_vtrace_from_importance_weights": (C.c_int, [vp] * 5 + [i32, i32, f32, vp, vp]),
         "drl_vtrace_from_importance_weights_dev": (C.c_int, [vp] * 5 + [i32, i32, f32, vp, vp, vp]),
         "drl_vtrace_from_softmax": (C.c_int, [vp] * 7 + [i32, i32, i32, f32, vp, vp]),

@@ -1,5 +1,7 @@
-"""Vector actors: the actor branches of ``train_impala.py:117-194`` (VectorActor, on one NativePolicy) and of
-``train_r2d2.py:167-251`` (R2D2VectorActor, on one NativeR2D2Policy) for N environments in lockstep.
+"""Vector actors: the actor branches of ``train_impala.py:117-194`` (VectorActor, on one NativePolicy), of
+``train_r2d2.py:167-251`` (R2D2VectorActor, on one NativeR2D2Policy), of ``train_apex.py:157-231`` (ApexVectorActor, on
+one NativeApexPolicy) and of ``train_a3c.py:112-183`` (A3CVectorActor, on one NativeA3CPolicy) for N environments in
+lockstep.
 
 VectorActor: each environment is its own actor task ``i`` (what ``FLAGS.task`` selects in the reference).  Per unroll:
 
@@ -180,4 +182,174 @@ class R2D2VectorActor:
                 task=i, unrolled_state=u["state"], unrolled_previous_action=u["previous_action"],
                 unrolled_action=u["action"], unrolled_reward=u["reward"], unrolled_done=u["done"],
                 unrolled_previous_h=u["initial_h"], unrolled_previous_c=u["initial_c"])
+        return finished
+
+
+class ApexVectorActor:
+    """The actor branch of ``train_apex.py:157-231`` for N environments in lockstep on one NativeApexPolicy; each
+    environment is its own actor task ``i``.  Per unroll (``trajectory`` steps):
+
+      - one ``learner.sync_policy(policy)`` (the learner-side ``apex.Agent``; device to device when it has a CUDA
+        learner);
+      - ``trajectory`` batched ``policy.act`` calls with each environment's epsilon: the explore draws of environments
+        0..n-1 from the global ``np.random`` stream, in that order; then, environment by environment, ``env.step`` with
+        ``action % available_action[i]`` (the buffer stores the raw action), the append to its ``LocalBuffer(1e4)``
+        and, once the buffer holds more than 3 ``trajectory`` transitions, a ``sample(trajectory)`` (a
+        ``np.random.permutation`` draw) pushed to ``queue.append_to_queue(task=i, ...)`` -- every step from then on;
+      - a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True; the score keeps the raw
+        reward; ``lives`` follows ``info['ale.lives']`` after every step;
+      - at an episode's end epsilon becomes 1 / (0.05 episode + 1), and the environment, the previous action and
+        lives (5) are reset.  ``episode_step`` is reset, the summed ``q[action]`` behind the logged ratio is not (the
+        reference's behaviour, SURVEY.md App. D).
+    At n = 1 this is the reference actor's loop, including the order of its ``np.random`` draws.
+    """
+
+    def __init__(self, policy, envs, queue, trajectory, available_action, learner=None, buffer_capacity=int(1e4)):
+        self.policy, self.envs, self.queue, self.learner = policy, list(envs), queue, learner
+        self.trajectory = int(trajectory)
+        self.available_action = [int(a) for a in available_action]
+        n = len(self.envs)
+        if not 1 <= n <= policy.max_batch:
+            raise ValueError("%d environments, the policy serves 1..%d per call" % (n, policy.max_batch))
+        if len(self.available_action) != n:
+            raise ValueError("available_action has %d entries for %d environments" % (len(self.available_action), n))
+        self.buffers = [buffer_queue.LocalBuffer(capacity=buffer_capacity) for _ in range(n)]
+        self.states = [env.reset() for env in self.envs]
+        self.previous_action = np.zeros(n, np.int32)
+        self.lives = [START_LIVES] * n
+        self.episode = [0] * n
+        self.epsilon = [1.0] * n
+        self.score = [0.0] * n
+        self.episode_step = [0] * n
+        self.total_max_prob = [0.0] * n
+
+    def run_unroll(self):
+        """One unroll of `trajectory` steps for every environment.  Returns the episodes that finished during it:
+        dicts of task, episode, score, epsilon, episode_step and total_max_prob (the logged ratio: the running sum of
+        q[action] over episode_step), the values train_apex.py:215-220 logs."""
+        if self.learner is not None:
+            self.learner.sync_policy(self.policy)
+        finished = []
+        T = self.trajectory
+        for _ in range(T):
+            out = self.policy.act(np.stack(self.states), self.previous_action, epsilon=np.array(self.epsilon))
+            action, q_action = out["action"], out["q_action"]
+            next_pa = action.astype(np.int32)
+            for i, env in enumerate(self.envs):
+                a = int(action[i])
+                self.episode_step[i] += 1
+                self.total_max_prob[i] += float(q_action[i])
+                next_state, reward, done, info = env.step(a % self.available_action[i])
+                self.score[i] += reward
+                if self.lives[i] != info["ale.lives"]:
+                    r, d = -1, True
+                else:
+                    r, d = reward, False
+                buf = self.buffers[i]
+                buf.append(state=self.states[i], done=d, reward=r, next_state=next_state,
+                           previous_action=int(self.previous_action[i]), action=a)
+                self.states[i] = next_state
+                self.lives[i] = info["ale.lives"]
+                if len(buf) > 3 * T:
+                    u = buf.sample(T)
+                    self.queue.append_to_queue(
+                        task=i, unrolled_state=u["state"], unrolled_next_state=u["next_state"],
+                        unrolled_previous_action=u["previous_action"], unrolled_action=u["action"],
+                        unrolled_reward=u["reward"], unrolled_done=u["done"])
+                if done:
+                    finished.append(dict(task=i, episode=self.episode[i], score=self.score[i],
+                                         epsilon=self.epsilon[i], episode_step=self.episode_step[i],
+                                         total_max_prob=self.total_max_prob[i] / self.episode_step[i]))
+                    self.episode_step[i] = 0
+                    self.episode[i] += 1
+                    self.score[i] = 0
+                    self.lives[i] = START_LIVES
+                    self.epsilon[i] = 1 / (self.episode[i] * 0.05 + 1)
+                    self.states[i] = env.reset()
+                    next_pa[i] = 0
+            self.previous_action = next_pa
+        return finished
+
+
+class A3CVectorActor:
+    """The actor branch of ``train_a3c.py:112-183`` for N environments in lockstep on one NativeA3CPolicy; each
+    environment is its own actor task ``i``.  Per unroll (``trajectory`` steps):
+
+      - every environment's ``UnrolledA3CTrajectory.initialize()``, then one ``learner.sync_policy(policy)`` (the
+        learner-side ``a3c.Agent``; device to device when it has a CUDA learner);
+      - ``trajectory`` batched ``policy.act`` calls: ``np.random.random_sample(n)`` from the global stream (row i's
+        draw is the one the reference's ``np.random.choice(A, p=policy)`` reads), the actions picked on the GPU; then,
+        environment by environment, ``env.step`` with ``action % available_action[i]`` (the trajectory stores the raw
+        action);
+      - a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True; the score keeps the raw
+        reward; ``lives`` follows ``info['ale.lives']`` after every step;
+      - at an episode's end the environment, the previous action and lives (5) are reset, and so are the score,
+        ``episode_step`` and the summed ``policy[action]`` behind the logged "prob";
+      - every environment's trajectory goes to ``queue.append_to_queue(task=i, ...)``.
+    At n = 1 this is the reference actor's loop, including the order of its ``np.random`` draws.
+    """
+
+    def __init__(self, policy, envs, queue, trajectory, available_action, learner=None):
+        self.policy, self.envs, self.queue, self.learner = policy, list(envs), queue, learner
+        self.trajectory = int(trajectory)
+        self.available_action = [int(a) for a in available_action]
+        n = len(self.envs)
+        if not 1 <= n <= policy.max_batch:
+            raise ValueError("%d environments, the policy serves 1..%d per call" % (n, policy.max_batch))
+        if len(self.available_action) != n:
+            raise ValueError("available_action has %d entries for %d environments" % (len(self.available_action), n))
+        self.trajs = [utils.UnrolledA3CTrajectory() for _ in range(n)]
+        self.states = [env.reset() for env in self.envs]
+        self.previous_action = np.zeros(n, np.int32)
+        self.lives = [START_LIVES] * n
+        self.episode = [0] * n
+        self.score = [0.0] * n
+        self.episode_step = [0] * n
+        self.total_max_prob = [0.0] * n
+
+    def run_unroll(self):
+        """One unroll of `trajectory` steps for every environment, pushed to the queue.  Returns the episodes that
+        finished during it: dicts of task, episode, prob (the mean policy[action]), score and episode_step, the values
+        train_a3c.py:162-165 logs."""
+        for t in self.trajs:
+            t.initialize()
+        if self.learner is not None:
+            self.learner.sync_policy(self.policy)
+        finished = []
+        for _ in range(self.trajectory):
+            out = self.policy.act(np.stack(self.states), self.previous_action)
+            action, max_prob = out["action"], out["max_prob"]
+            next_pa = action.astype(np.int32)
+            for i, env in enumerate(self.envs):
+                a = int(action[i])
+                self.episode_step[i] += 1
+                self.total_max_prob[i] += float(max_prob[i])
+                next_state, reward, done, info = env.step(a % self.available_action[i])
+                self.score[i] += reward
+                if self.lives[i] != info["ale.lives"]:
+                    r, d = -1, True
+                else:
+                    r, d = reward, False
+                self.trajs[i].append(state=self.states[i], next_state=next_state,
+                                     previous_action=int(self.previous_action[i]), action=a, reward=r, done=d)
+                self.states[i] = next_state
+                self.lives[i] = info["ale.lives"]
+                if done:
+                    finished.append(dict(task=i, episode=self.episode[i],
+                                         prob=self.total_max_prob[i] / self.episode_step[i], score=self.score[i],
+                                         episode_step=self.episode_step[i]))
+                    self.episode[i] += 1
+                    self.score[i] = 0
+                    self.episode_step[i] = 0
+                    self.total_max_prob[i] = 0
+                    self.states[i] = env.reset()
+                    next_pa[i] = 0
+                    self.lives[i] = START_LIVES
+            self.previous_action = next_pa
+        for i, t in enumerate(self.trajs):
+            u = t.extract()
+            self.queue.append_to_queue(
+                task=i, unrolled_state=u["state"], unrolled_next_state=u["next_state"],
+                unrolled_previous_action=u["previous_action"], unrolled_action=u["action"],
+                unrolled_reward=u["reward"], unrolled_done=u["done"])
         return finished

@@ -6,8 +6,10 @@ learner branch of ``train_a3c.py`` runs on it unchanged), with the TF1 graph rep
   Agent.set_session            agent/a3c.py:105-107
   Agent.get_policy_and_action  agent/a3c.py:109-119 -> (action, policy, max_prob)
   Agent.parameter_sync         agent/a3c.py:121-122
+  Agent.sync_policy            parameter_sync into a NativeA3CPolicy (actor.py: A3CVectorActor)
 """
 import os
+import threading
 
 import numpy as np
 
@@ -40,6 +42,7 @@ class Agent:
         self._engine = None
         self._slot = 0
         self._last = {}
+        self._lock = threading.RLock()   # actor threads sync from / act on this agent while the learner thread trains
         _AGENTS[model_name] = self
 
     def _ensure_init(self):
@@ -117,6 +120,30 @@ class Agent:
         if self._engine is not None:
             self._engine.set_params(self._params)
 
+    def sync_policy(self, policy):
+        """parameter_sync into a NativeA3CPolicy (the actor side of A3CVectorActor): device to device from this
+        agent's learner when it has one, otherwise from the host copy of the parameters."""
+        with self._lock:
+            if self._engine is not None:
+                policy.sync_from(self._engine)
+            else:
+                self._ensure_init()
+                policy.set_params(self._params)
+
     learning_rate = property(lambda self: self._last.get("learning_rate"))
     grad_norm = property(lambda self: self._last.get("grad_norm"))
     num_env_frames = property(lambda self: self._last.get("step", (self._opt or {}).get("step", 0)))
+
+
+def _locked(fn):
+    def wrapper(self, *a, **k):
+        with self._lock:
+            return fn(self, *a, **k)
+    wrapper.__name__, wrapper.__doc__ = fn.__name__, fn.__doc__
+    return wrapper
+
+
+# actor threads call these on a shared agent while the learner thread trains (in-process launch mode); a sync from an
+# actor thread never meets the learner thread's engine rebuild in train
+for _n in ('train', 'set_session', 'get_policy_and_action', 'parameter_sync'):
+    setattr(Agent, _n, _locked(getattr(Agent, _n)))

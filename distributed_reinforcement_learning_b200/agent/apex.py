@@ -10,6 +10,7 @@ values -- so the learner branch of ``train_apex.py:82-155`` runs on it unchanged
   Agent.get_td_error          agent/apex.py:116-133
   Agent.distributed_train     agent/apex.py:135-154 -> (loss, td_error)
   Agent.train                 agent/apex.py:156-168
+  Agent.sync_policy           parameter_sync into a NativeApexPolicy (actor.py: ApexVectorActor)
 """
 import os
 import threading
@@ -115,6 +116,17 @@ class Agent:
             if self._engine is not None:
                 self._engine.set_params(self._main, MAIN)
                 self._engine.set_params(self._target, TARGET)
+
+    def sync_policy(self, policy):
+        """parameter_sync into a NativeApexPolicy (the actor side of ApexVectorActor): device to device from this
+        agent's learner when it has one, otherwise from the host copy.  The actor only evaluates the main network, so
+        only the main scope is copied."""
+        with self._lock:
+            if self._engine is not None:
+                policy.sync_from(self._engine)
+            else:
+                self._ensure_init()
+                policy.set_params(self._main)
 
     def set_session(self, sess):
         self.sess = sess

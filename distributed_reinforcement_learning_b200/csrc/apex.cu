@@ -13,31 +13,10 @@
 #include <vector>
 
 #include "adam_learner.cuh"
+#include "apex_defs.cuh"
 #include "layer_defs.cuh"
 
 namespace drl {
-
-// Offsets (in floats) inside the padded flat vectors of ONE network (FlatLayout, kernels.h)
-struct ApexLayout : FlatLayout {
-  int A;
-  int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b;
-  int64_t emb1_w, emb1_b, emb2_w, emb2_b;
-  int64_t value1_w, value1_b, value2_w, value2_b, value3_w, value3_b;
-  int64_t mean1_w, mean1_b, mean2_w, mean2_b, mean3_w, mean3_b;
-  void init(int num_action) {
-    A = num_action;
-    const int64_t CAT = Geo::FLAT + Geo::EMB;
-    const int64_t sizes[] = {
-        8 * 8 * 4 * 32, 32, 4 * 4 * 32 * 64, 64, 3 * 3 * 64 * 64, 64,
-        (int64_t)A * 256, 256, 256 * 256, 256,
-        CAT * 256, 256, 256 * 256, 256, 256 * (int64_t)A, A,
-        CAT * 256, 256, 256 * 256, 256, 256, 1};
-    int64_t* const named[] = {&conv1_w, &conv1_b, &conv2_w, &conv2_b, &conv3_w, &conv3_b, &emb1_w, &emb1_b,
-                              &emb2_w, &emb2_b, &value1_w, &value1_b, &value2_w, &value2_b, &value3_w, &value3_b,
-                              &mean1_w, &mean1_b, &mean2_w, &mean2_b, &mean3_w, &mean3_b};
-    set(sizes, named);
-  }
-};
 
 struct ApexActs {          // forward activations of one network over up to `cap` rows (caller row order)
   float* a1;               // [M,20,20,32]
@@ -60,9 +39,6 @@ struct ApexBwd {           // backward workspace, Mb = B rows
   float *da3, *du, *dpre2, *dpre1, *da2, *da1;
   float *wg_part, *wg_part2, *dcol;
 };
-
-constexpr int kHeadN = 2 * Geo::HID;             // 512 columns: [value hidden | mean hidden]
-constexpr int kCat = Geo::FLAT + Geo::EMB;       // 3392
 
 static SplitPlan plan_head1(int M) { return plan_split(kCat, cdiv(M, CfgMid::BM) * (kHeadN / CfgMid::BN), 16, 1); }
 
@@ -219,6 +195,43 @@ __global__ void __launch_bounds__(256) a3c_loss_kernel(A3cArgs a) {
   }
 }
 
+// conv1 (model/apex_value.py:5), conv2 (:6), conv3 -> flatten HWC (:7-9)
+int apex_conv_forward(cudaStream_t s, const ApexLayout& pl, const float* P, const uint8_t* img_conv2,
+                      const uint8_t* img_conv3, const uint8_t* frames, int M, float* a1, float* a2, float* a3, int mode,
+                      bool tgt, cudaEvent_t images_ready, int* launches) {
+  const RowMap map{M, 1};          // rows are already in caller order: src(m) == m
+  int n = 0;
+  {
+    Conv1A al{frames, map};
+    PlainB bl{P + pl.conv1_w, 32, 0};
+    EpConv1 ep{a1, 32, P + pl.conv1_b};
+    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
+  }
+  if (images_ready) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, images_ready, 0));
+  {
+    Conv2A al{a1, map};
+    PlainB bl{P + pl.conv2_w, 64, 0};
+    PretiledB<PlainB> blp{img_conv2, 512 / 32};
+    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
+    GEMM_W(tgt ? "target_conv2_fwd" : "conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
+  }
+  {
+    Conv3A al{a2, map};
+    PlainB bl{P + pl.conv3_w, 64, 0};
+    PretiledB<PlainB> blp{img_conv3, 576 / 32};
+    EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
+    GEMM_W(tgt ? "target_conv3_fwd" : "conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
+  }
+  *launches += n;
+  return DRL_OK;
+}
+
+int apex_conv_images(cudaStream_t s, const ApexLayout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3) {
+  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, img_conv2)));
+  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, img_conv3)));
+  return DRL_OK;
+}
+
 // ------------------------------------------------------------------------------------------
 // Forward of the dueling network (model/apex_value.py:22-41) over M rows.  `tgt` only selects the profile names.
 // Weight images (tensor-core modes): img[1]/img[2] conv2/conv3 forward, img[5]/img[6] the dCol operands of backward.
@@ -227,7 +240,6 @@ __global__ void __launch_bounds__(256) a3c_loss_kernel(A3cArgs a) {
 static int apex_forward(const Streams& st, const ApexLayout& pl, const float* P, const WeightImages& wi,
                         const uint8_t* frames, const int32_t* pa, const ApexActs& act, int M, int mode,
                         bool retile_fwd, bool retile_bwd, bool tgt, int* launches) {
-  const RowMap map{M, 1};          // rows are already in caller order: src(m) == m
   int n = 0;
   cudaStream_t s = st.main;
   const cudaStream_t side = st.par ? st.side : st.main;
@@ -249,27 +261,8 @@ static int apex_forward(const Streams& st, const ApexLayout& pl, const float* P,
     n += 2;
   }
   s = st.main;
-  {  // conv1: u8 frames -> a1 (model/apex_value.py:5)
-    Conv1A al{frames, map};
-    PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
-    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
-  }
-  if (st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
-  {  // conv2 (:6)
-    Conv2A al{act.a1, map};
-    PlainB bl{P + pl.conv2_w, 64, 0};
-    PretiledB<PlainB> blp{wi.img[1], 512 / 32};
-    EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv2_fwd" : "conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
-  }
-  {  // conv3 -> flatten HWC (:7-9)
-    Conv3A al{act.a2, map};
-    PlainB bl{P + pl.conv3_w, 64, 0};
-    PretiledB<PlainB> blp{wi.img[2], 576 / 32};
-    EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv3_fwd" : "conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
-  }
+  DRL_TRY(apex_conv_forward(s, pl, P, wi.img[1], wi.img[2], frames, M, act.a1, act.a2, act.a3, mode, tgt,
+                            st.par ? st.ev[7] : nullptr, &n));
   DRL_TRY(join_from_side(st, 1));
   // first layers of both streams: [M, 3392] x [3392, 256 | 256], split-K partial sums, then bias + ReLU (:17-19,28-37)
   const SplitPlan sp = plan_head1(M);
@@ -896,3 +889,15 @@ int drl_a3c_stream(drl_a3c* h, void** stream) { return drl_apex_stream(h, stream
 int drl_a3c_launches_per_step(const drl_a3c* h, int32_t* n) { return drl_apex_launches_per_step(h, n); }
 
 }  // extern "C"
+
+int drl::apex_params_snapshot(drl_apex* h, int device, int algo, int num_action, cudaStream_t dst_stream, float* dst,
+                              cudaEvent_t ev_ready, cudaEvent_t ev_copied) {
+  DRL_TRY(check_handle(h, kName));
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  if (h->algo != algo || h->A != num_action) {
+    set_error("sync: the learner is %s with num_action %d, the policy %s with %d", h->algo ? "A3C" : "Ape-X", h->A,
+              algo ? "A3C" : "Ape-X", num_action);
+    return DRL_ERR_INVALID;
+  }
+  return adam_params_snapshot(h, kName, device, dst_stream, dst, ev_ready, ev_copied);
+}

@@ -1,0 +1,49 @@
+// apex_defs.cuh -- definitions shared by the Ape-X / A3C learner (apex.cu) and the Ape-X / A3C policy engine
+// (apex_policy.cu): the dueling network's flat parameter layout, its head sizes and the learner's conv forward.
+#pragma once
+#include "kernels.h"
+
+namespace drl {
+
+// Offsets (in floats) inside the padded flat vectors of ONE network (FlatLayout, kernels.h).  A3C uses the same layout:
+// its actor stream sits in the value* slots and its critic stream in the mean* slots (model/actor_critic.py:27-38).
+struct ApexLayout : FlatLayout {
+  int A;
+  int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b;
+  int64_t emb1_w, emb1_b, emb2_w, emb2_b;
+  int64_t value1_w, value1_b, value2_w, value2_b, value3_w, value3_b;
+  int64_t mean1_w, mean1_b, mean2_w, mean2_b, mean3_w, mean3_b;
+  void init(int num_action) {
+    A = num_action;
+    const int64_t CAT = Geo::FLAT + Geo::EMB;
+    const int64_t sizes[] = {
+        8 * 8 * 4 * 32, 32, 4 * 4 * 32 * 64, 64, 3 * 3 * 64 * 64, 64,
+        (int64_t)A * 256, 256, 256 * 256, 256,
+        CAT * 256, 256, 256 * 256, 256, 256 * (int64_t)A, A,
+        CAT * 256, 256, 256 * 256, 256, 256, 1};
+    int64_t* const named[] = {&conv1_w, &conv1_b, &conv2_w, &conv2_b, &conv3_w, &conv3_b, &emb1_w, &emb1_b,
+                              &emb2_w, &emb2_b, &value1_w, &value1_b, &value2_w, &value2_b, &value3_w, &value3_b,
+                              &mean1_w, &mean1_b, &mean2_w, &mean2_b, &mean3_w, &mean3_b};
+    set(sizes, named);
+  }
+};
+
+constexpr int kHeadN = 2 * Geo::HID;             // 512 columns: [value hidden | mean hidden]
+constexpr int kCat = Geo::FLAT + Geo::EMB;       // 3392
+
+// conv1 / conv2 / conv3 forward of one network over M rows (caller row order) on stream s, with the learner's kernels
+// and configurations for math mode `mode` (1: FP32 FFMA; 2: wgmma 3xTF32 with the conv2 / conv3 weight images of
+// apex_conv_images).  When images_ready is not null, conv2 waits for it (the images and the embedding are built on
+// another stream).  `tgt` only names the launches for the per-kernel profile; adds the launches to *launches.
+int apex_conv_forward(cudaStream_t s, const ApexLayout& pl, const float* P, const uint8_t* img_conv2,
+                      const uint8_t* img_conv3, const uint8_t* frames, int M, float* a1, float* a2, float* a3, int mode,
+                      bool tgt, cudaEvent_t images_ready, int* launches);
+// the conv2 / conv3 forward weight images of math mode 2 (WeightImages slots 1 and 2 sizes)
+int apex_conv_images(cudaStream_t s, const ApexLayout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3);
+
+// drl_apex_policy_sync_from_learner: adam_params_snapshot of the main network of an Ape-X (algo 0) or A3C (algo 1)
+// learner with num_action actions (DRL_ERR_INVALID for another algo or num_action)
+int apex_params_snapshot(drl_apex* h, int device, int algo, int num_action, cudaStream_t dst_stream, float* dst,
+                         cudaEvent_t ev_ready, cudaEvent_t ev_copied);
+
+}  // namespace drl

@@ -19,6 +19,7 @@
 #include <nvtx3/nvToolsExt.h>
 
 #include "kernels.h"
+#include "policy_head.cuh"
 #include "policy_lstm.cuh"
 
 namespace drl {
@@ -42,7 +43,6 @@ constexpr int kLSplits = 16;
 // 16 float4 weight loads in flight; the four K partials are added in fixed order (0 + 1) + 2 + 3.  The output layer and
 // the softmax: warp r = row r, lane a = logit a (K in four interleaved chains added in fixed order); the softmax is that
 // of heads_out_forward_kernel (max, expf(l - max), warp_sum, divide).
-constexpr int kHR = 8;
 constexpr int kHThreads = 256;
 constexpr int kMaxA = 32;
 // shared memory (floats): h1 / hid2 [kHR][256], hid1 [kHR][256], K partials [4][kHR][256], W3 [256][A <= 32]
@@ -61,45 +61,6 @@ struct HeadArgs {
   int32_t* action;         // [n]
   int n, A;
 };
-
-// out[r][u] = relu(sum_k in[r][k] W[k][u] + b[u]) for the kHR rows of the CTA (W [256][256] row-major)
-__device__ __forceinline__ void dense256_relu(const float* __restrict__ in, const float* __restrict__ W,
-                                              const float* __restrict__ b, float* part, float* out, int tid) {
-  const int q = tid & 63, g = tid >> 6;
-  float acc[kHR][4];
-#pragma unroll
-  for (int r = 0; r < kHR; ++r) acc[r][0] = acc[r][1] = acc[r][2] = acc[r][3] = 0.f;
-#pragma unroll 1
-  for (int kk = 0; kk < 64; kk += 16) {
-    float4 wv[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) wv[j] = ldg4(W + (size_t)(g * 64 + kk + j) * 256 + 4 * q);
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int k = g * 64 + kk + j;
-#pragma unroll
-      for (int r = 0; r < kHR; ++r) {
-        const float x = in[r * 256 + k];
-        acc[r][0] = fmaf(x, wv[j].x, acc[r][0]);
-        acc[r][1] = fmaf(x, wv[j].y, acc[r][1]);
-        acc[r][2] = fmaf(x, wv[j].z, acc[r][2]);
-        acc[r][3] = fmaf(x, wv[j].w, acc[r][3]);
-      }
-    }
-  }
-#pragma unroll
-  for (int r = 0; r < kHR; ++r)
-    reinterpret_cast<float4*>(part + (g * kHR + r) * 256)[q] = make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
-  __syncthreads();
-  const float bias = __ldg(b + tid);
-#pragma unroll
-  for (int r = 0; r < kHR; ++r) {
-    const float* p = part + r * 256 + tid;
-    const float v = ((p[0] + p[kHR * 256]) + p[2 * kHR * 256]) + p[3 * kHR * 256];
-    out[r * 256 + tid] = fmaxf(v + bias, 0.f);
-  }
-  __syncthreads();
-}
 
 __global__ void __launch_bounds__(kHThreads, 1) policy_head_fused_kernel(const HeadArgs a) {
   kernel_prologue();
@@ -167,23 +128,11 @@ __global__ void __launch_bounds__(kHThreads, 1) policy_head_fused_kernel(const H
   const float sum = warp_sum(e);
   const float p = e / sum;
   if (lane < A) a.policy[(size_t)m * A + lane] = p;
-  // sampling: cdf = cumsum(float64(policy)) / cdf[A-1] in index order; action = #(cdf <= u), clamped to A - 1 -- the
-  // searchsorted(cdf, u, side='right') of numpy's RandomState.choice(A, p=policy)
+  // sampling: numpy's RandomState.choice(A, p=policy) for the row's uniform draw (policy_head.cuh)
   float* sp = part + warp * 32;      // the K partials are dead after the second dense layer
   sp[lane] = p;
   __syncwarp();
-  if (lane == 0) {
-    double total = 0.0;
-    for (int i = 0; i < A; ++i) total += (double)sp[i];
-    const double u = a.uniform[m];
-    double run = 0.0;
-    int cnt = 0;
-    for (int i = 0; i < A; ++i) {
-      run += (double)sp[i];
-      cnt += (run / total <= u) ? 1 : 0;
-    }
-    a.action[m] = cnt < A - 1 ? cnt : A - 1;
-  }
+  if (lane == 0) a.action[m] = sample_choice(sp, A, a.uniform, m);
 }
 
 // ---- handle -----------------------------------------------------------------------------------------------------

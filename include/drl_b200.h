@@ -270,6 +270,57 @@ int drl_r2d2_policy_act(drl_r2d2_policy* h, int32_t n, const uint8_t* state, con
 int drl_r2d2_policy_last_act_ms(drl_r2d2_policy* h, float* ms);
 
 /* ------------------------------------------------------------------------------------------
+ * Ape-X / A3C policy engine (new): the actor side of train_apex.py:157-231 and train_a3c.py:112-183 (the actor loops
+ * themselves are distributed_reinforcement_learning_b200/actor.py: ApexVectorActor, A3CVectorActor).  A forward-only
+ * handle that serves the family's get_policy_and_action (agent/apex.py:88-102, agent/a3c.py:109-119) for up to 64
+ * environments per call, on its own stream next to a training learner, and takes the learner's parameters device to
+ * device.  The two families share the network body and the learner handle (drl_a3c is drl_apex with algo 1), so one
+ * engine serves both; only the action rule differs:
+ *   algo 0 (Ape-X)  q = value - "mean"; the first maximum of q, or the row's explore action (epsilon drawn on the host)
+ *   algo 1 (A3C)    policy = softmax(actor); numpy's RandomState.choice(A, p=policy) for the row's host uniform draw
+ * It holds no target scope, optimizer state, gradients or backward buffers.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_apex_policy drl_apex_policy;
+typedef struct drl_apex_policy drl_a3c_policy;
+
+typedef struct drl_apex_policy_config {
+  int32_t max_batch;                 /* 1..64 rows (environments) per act call                        */
+  int32_t height, width, channels;   /* 84,84,4 only (as drl_apex_create / drl_a3c_create)            */
+  int32_t num_action;                /* A, 2..32                                                      */
+  int32_t algo;                      /* 0 = Ape-X (drl_apex_policy_act), 1 = A3C (drl_a3c_policy_act)  */
+  int32_t device;                    /* CUDA device ordinal                                           */
+  int32_t use_cuda_graph;            /* 1: one CUDA graph per row count n (input copy + kernels)      */
+} drl_apex_policy_config;
+
+int drl_apex_policy_create(const drl_apex_policy_config* cfg, drl_apex_policy** out);
+int drl_apex_policy_destroy(drl_apex_policy* h);
+/* The learner's one-network inventory and flat TF order (drl_apex_get_params(.., DRL_APEX_MAIN, ..) for Ape-X,
+ * drl_a3c_get_params for A3C). */
+int drl_apex_policy_param_count(const drl_apex_policy* h, int64_t* n);
+int drl_apex_policy_set_params(drl_apex_policy* h, const float* host_flat, int64_t n);
+int drl_apex_policy_get_params(drl_apex_policy* h, float* host_flat, int64_t n);
+/* parameter_sync without a host round trip: the learner's main parameters after all work enqueued on it so far (a step
+ * in flight included), copied device to device on the policy's stream; the learner's next update waits for the copy.
+ * Takes a drl_apex* or a drl_a3c* (the same type).  The learner must be of the policy's algo, on the same device and
+ * have the same num_action (DRL_ERR_INVALID otherwise).  Returns without waiting for the copy. */
+int drl_apex_policy_sync_from_learner(drl_apex_policy* h, struct drl_apex* learner);
+/* Ape-X get_policy_and_action (agent/apex.py:88-102) for n <= max_batch environments (algo 0 only).  state u8
+ * [n,84,84,4]; previous_action i32 [n] in [0, A); explore_action i32 [n] or NULL -> q f32 [n,A] (value - mean),
+ * action i32 [n], q_action f32 [n] (= q[action]).  Per row, explore_action -1 (or NULL) is the greedy action, the first
+ * maximum of q (np.argmax); a value in [0, A) is taken as the action.  Synchronous; any output pointer may be NULL. */
+int drl_apex_policy_act(drl_apex_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action,
+                        const int32_t* explore_action, int32_t* action, float* q, float* q_action);
+/* A3C get_policy_and_action (agent/a3c.py:109-119) for n <= max_batch environments (algo 1 only).  state u8
+ * [n,84,84,4]; previous_action i32 [n] in [0, A); uniform f64 [n] in [0, 1) -> policy f32 [n,A] (softmax of the actor
+ * stream), action i32 [n] = min(searchsorted(cumsum(float64(policy)) / cdf[A-1], uniform, side='right'), A-1) -- what
+ * numpy's RandomState.choice(A, p=policy) picks for that draw -- and prob_action f32 [n] (= policy[action]).
+ * Synchronous; any output pointer may be NULL. */
+int drl_a3c_policy_act(drl_a3c_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action,
+                       const double* uniform, int32_t* action, float* policy, float* prob_action);
+/* Device time of the most recent act call (input copy + kernels; CUDA events on the policy's stream), ms. */
+int drl_apex_policy_last_act_ms(drl_apex_policy* h, float* ms);
+
+/* ------------------------------------------------------------------------------------------
  * Stand-alone V-trace (optimizer/vtrace.py), host-pointer convenience forms + device forms.
  * ------------------------------------------------------------------------------------------ */
 /* vtrace.from_importance_weights (optimizer/vtrace.py:71-103): time-major [T,B] float32 inputs,
