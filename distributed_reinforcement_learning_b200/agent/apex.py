@@ -11,13 +11,19 @@ values -- so the learner branch of ``train_apex.py:82-155`` runs on it unchanged
   Agent.distributed_train     agent/apex.py:135-154 -> (loss, td_error)
   Agent.train                 agent/apex.py:156-168
   Agent.sync_policy           parameter_sync into a NativeApexPolicy (actor.py: ApexVectorActor)
+  Agent.device_memory         a DeviceMemory: the replay memory of train_apex.py:87 on the GPU (apex_replay.py)
+  Agent.train_from_memory     Memory.sample + np.stack + distributed_train + Memory.update (train_apex.py:118-154)
+                              as one device-resident step -> (loss, td_error)
 """
 import os
+import random
 import threading
 
 import numpy as np
 
+from .. import dp
 from ..apex_learner import MAIN, TARGET, NativeApexLearner
+from ..apex_replay import NativeApexReplay
 from ..model import apex_value
 
 _AGENTS = {}
@@ -203,6 +209,33 @@ class Agent:
         self._last = out
         return out["loss"], td
 
+    def device_memory(self, capacity):
+        """A prioritized replay memory of ``capacity`` transitions on this agent's GPU (buffer_queue.Memory's
+        arithmetic); fill it with DeviceMemory.add, train from it with train_from_memory."""
+        return DeviceMemory(self, capacity)
+
+    def train_from_memory(self, memory, batch_size, u01=None):
+        """One iteration of the learner loop's training half (train_apex.py:118-154) against a DeviceMemory:
+        replay_buffer.sample(batch_size), the minibatch stack, distributed_train and the priority update, all on the GPU.
+        ``u01`` ([batch_size] in [0, 1)) are the strata's uniforms; by default ``random.random()`` draws them exactly as
+        Memory.sample does, so a host loop and a device loop seeded alike sample the same strata.  -> (loss, td_error)."""
+        if dp.distributed():
+            raise RuntimeError("train_from_memory: a DeviceMemory is local to one GPU; data-parallel training "
+                               "(torch.distributed world > 1) uses Memory and distributed_train")
+        if u01 is None:
+            u01 = [random.random() for _ in range(batch_size)]
+        if self._engine is not None and self._engine.B != batch_size:
+            self._pull_state()
+            self._engine.close()
+            self._engine = None
+        eng = self._get_engine(batch_size)
+        slot = self._slot
+        self._slot = (self._slot + 1) % eng.num_slots
+        memory.replay.step_async(eng, slot, u01)
+        out, td = eng.wait()
+        self._last = out
+        return out["loss"], td
+
     def distributed_train(self, state, next_state, previous_action, action, reward, done, is_weight):
         """agent/apex.py:135-154 -> (loss, td_error)."""
         return self._train(state, next_state, previous_action, action, reward, done, is_weight)
@@ -217,6 +250,50 @@ class Agent:
     num_env_frames = property(lambda self: self._last.get("step", (self._opt or {}).get("step", 0)))
 
 
+class DeviceMemory:
+    """The replay memory of train_apex.py:87 on the agent's GPU, for the device loop:
+
+        memory = learner.device_memory(capacity)
+        memory.add(state, next_state, previous_action, action, reward, done)   # get_td_error + the Memory.add loop
+        loss, td_error = learner.train_from_memory(memory, batch_size)         # sample .. distributed_train .. update
+
+    It outlives a rebuild of the agent's learner (another batch size): the agent passes its current learner to each
+    call.  ``replay`` is the NativeApexReplay; ``n_entries``, ``beta``, ``total()`` and ``last_sample()`` read its state."""
+
+    def __init__(self, agent, capacity):
+        self.agent = agent
+        self.capacity = int(capacity)
+        self.replay = NativeApexReplay(self.capacity, device=agent.device, input_shape=tuple(agent.input_shape))
+
+    def add(self, state, next_state, previous_action, action, reward, done):
+        """learner.get_td_error(...) followed by replay_buffer.add(td_error[i], ...) for each transition in order
+        (train_apex.py:99-116); the priorities are the learner's |td|, computed and applied on the device.  Transitions
+        beyond the learner's batch go through in chunks of it, as get_td_error does."""
+        a = self.agent
+        st = a._u8(np.stack(state))
+        ns = a._u8(np.stack(next_state))
+        pa, ac = np.asarray(previous_action), np.asarray(action)
+        rw, dn = np.asarray(reward), np.asarray(done)
+        with a._lock:
+            eng = a._engine if a._engine is not None else a._get_engine(st.shape[0])
+            for lo in range(0, st.shape[0], eng.B):
+                hi = min(lo + eng.B, st.shape[0])
+                self.replay.add(eng, st[lo:hi], ns[lo:hi], pa[lo:hi], ac[lo:hi], rw[lo:hi], dn[lo:hi])
+
+    n_entries = property(lambda self: self.replay.n_entries)
+    beta = property(lambda self: self.replay.beta)
+
+    def total(self):
+        return self.replay.total()
+
+    def last_sample(self):
+        """(tree_index, priority, is_weight) of the most recent training step's draws."""
+        return self.replay.last_sample()
+
+    def close(self):
+        self.replay.close()
+
+
 def _locked(fn):
     def wrapper(self, *a, **k):
         with self._lock:
@@ -226,6 +303,7 @@ def _locked(fn):
 
 
 # actor threads call these on a shared agent while the learner thread trains (in-process launch mode)
-for _n in ('save_weights', 'load_weights', 'set_session', 'target_to_main', 'get_policy_and_action', 'get_td_error', '_train'):
+for _n in ('save_weights', 'load_weights', 'set_session', 'target_to_main', 'get_policy_and_action', 'get_td_error', '_train',
+           'train_from_memory'):
     if hasattr(Agent, _n):
         setattr(Agent, _n, _locked(getattr(Agent, _n)))

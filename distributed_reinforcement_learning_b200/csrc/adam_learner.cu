@@ -260,7 +260,9 @@ int wait_staged(AdamLearner* h, int slot) {
   return DRL_OK;
 }
 
-int run_step(AdamLearner* h, int slot) {
+}  // namespace
+
+int adam_run_step(AdamLearner* h, int slot) {
   DRL_TRY(wait_staged(h, slot));
   if (h->use_cuda_graph) DRL_TRY(refresh_target_images(h));
   DRL_CUDA_CHECK(cudaEventRecord(h->ev_start, h->compute));
@@ -289,8 +291,6 @@ int run_step(AdamLearner* h, int slot) {
   h->pending = true;
   return DRL_OK;
 }
-
-}  // namespace
 
 int check_handle(const AdamLearner* h, const char* family) {
   if (!h) { set_error("null %s handle", family); return DRL_ERR_INVALID; }
@@ -417,7 +417,7 @@ int adam_step_async(AdamLearner* h, const char* family, int slot) {
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   DRL_TRY(check_slot(h, slot));
   DRL_TRY(set_device(h));
-  return run_step(h, slot);
+  return adam_run_step(h, slot);
 }
 
 // data parallel: the step in two halves around the caller's all-reduce of the bucket (eager launches)

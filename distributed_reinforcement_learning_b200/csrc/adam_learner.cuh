@@ -89,6 +89,10 @@ int adam_main_to_target(AdamLearner* h, const char* family);
 int adam_params_snapshot(AdamLearner* h, const char* family, int device, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);
 int adam_step_async(AdamLearner* h, const char* family, int slot);
+// the body of adam_step_async (the caller holds the lock and has set the device): waits for the slot's `staged` event,
+// enqueues forward + loss + backward + update (graph or eager) on the compute stream, records `consumed`, ev_stop and
+// ev_done, marks the step pending
+int adam_run_step(AdamLearner* h, int slot);
 int adam_forward_backward(AdamLearner* h, const char* family, int slot);
 int adam_grad_bucket(AdamLearner* h, const char* family, void** dev_ptr, int64_t* count);
 int adam_apply(AdamLearner* h, const char* family, float grad_scale);

@@ -18,28 +18,6 @@
 
 namespace drl {
 
-struct ApexActs {          // forward activations of one network over up to `cap` rows (caller row order)
-  float* a1;               // [M,20,20,32]
-  float* a2;               // [M,9,9,64]
-  float* a3;               // [M,3136]
-  float* e1;               // [A,256]
-  float* table;            // [A,256]
-  float* zpart;            // [splits][M,512] split-K partial sums of the two first head layers
-  float* hid1;             // [2][M,256]  value / mean stream hidden 1
-  float* hid2;             // [2][M,256]
-  float* vstream;          // [M,A]  value stream output
-  float* scratch_sm;       // [M,A]  (softmax of the value stream: by-product of the shared output kernel, unused)
-  float* mstream;          // [M]    "mean" stream output
-  int cap;
-};
-
-struct ApexBwd {           // backward workspace, Mb = B rows
-  float *dq, *dmean;       // [Mb,32] each (columns >= A / >= 1 stay zero)
-  float *dhid2, *dhid1;    // [2][Mb,256]
-  float *da3, *du, *dpre2, *dpre1, *da2, *da1;
-  float *wg_part, *wg_part2, *dcol;
-};
-
 static SplitPlan plan_head1(int M) { return plan_split(kCat, cdiv(M, CfgMid::BM) * (kHeadN / CfgMid::BN), 16, 1); }
 
 // hid1[z][m][j] = relu(sum_s zpart[s][m][z*256 + j] + b1[z][j])   (first layers of both streams, model/apex_value.py:17-19)
@@ -418,33 +396,9 @@ static int apex_backward(const Streams& st, const ApexLayout& pl, const float* P
   return DRL_OK;
 }
 
-struct ApexIn {                // views of one staging slot
-  uint8_t* frames;             // [2B][84,84,4]: state rows, then next_state rows
-  int32_t* pa2;                // [2B]: previous_action, then action (the embedding input of the rows s')
-  float* reward;               // [B]
-  uint8_t* done;               // [B]
-  float* weight;               // [B]
-};
-
 }  // namespace drl
 
 using namespace drl;
-
-struct drl_apex : AdamLearner {
-  drl_apex_config cfg{};
-  int A = 0;
-  ApexLayout pl{};
-  ApexActs act{}, tact{};
-  ApexBwd bwd{};
-  float *main_q = nullptr, *next_main_q = nullptr, *target_q = nullptr, *target_value = nullptr, *sav = nullptr,
-        *td_dev = nullptr;
-  // A3C runs on the same body (drl_a3c_*): no target scope, the loss kernel above, three loss scalars
-  int algo = 0;                // 0 = Ape-X DQN, 1 = A3C
-  float a3c_baseline_coef = 0.f, a3c_entropy_coef = 0.f;
-  int a3c_clip = 0;
-  float* adv = nullptr;        // [B] advantage tap
-  std::vector<ApexIn> in;      // per slot
-};
 
 namespace {
 
@@ -469,8 +423,9 @@ int alloc_acts(drl_apex* h, ApexActs& a, int cap) {
   return DRL_OK;
 }
 
-// forward passes + TD kernel over n transitions held by `sl`; train = also head gradients and the loss
-int enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* td_host, int* launches) {
+}  // namespace
+
+int drl::enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* td_host, int* launches) {
   const Streams st = h->streams(), tst = h->target_streams();
   if (h->algo == 1) {      // A3C: one scope; rows [0, n) = network(s, prev_a), rows [n, 2n) = network(s', a)
     DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, sl.frames, sl.pa2, h->act, 2 * n, h->mode, h->main_images_stale,
@@ -517,6 +472,8 @@ int enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* 
   if (launches) *launches += 1;
   return DRL_OK;
 }
+
+namespace {
 
 int fwd_bwd(AdamLearner* core, int slot, int* launches) {
   drl_apex* h = static_cast<drl_apex*>(core);

@@ -1,6 +1,10 @@
-// apex_defs.cuh -- definitions shared by the Ape-X / A3C learner (apex.cu) and the Ape-X / A3C policy engine
-// (apex_policy.cu): the dueling network's flat parameter layout, its head sizes and the learner's conv forward.
+// apex_defs.cuh -- definitions shared by the Ape-X / A3C learner (apex.cu), the Ape-X / A3C policy engine
+// (apex_policy.cu) and the Ape-X device replay memory (apex_replay.cu): the dueling network's flat parameter layout, its
+// head sizes, the learner's conv forward, the learner handle and its forward + TD path.
 #pragma once
+#include <vector>
+
+#include "adam_learner.cuh"
 #include "kernels.h"
 
 namespace drl {
@@ -45,5 +49,61 @@ int apex_conv_images(cudaStream_t s, const ApexLayout& pl, const float* P, uint8
 // learner with num_action actions (DRL_ERR_INVALID for another algo or num_action)
 int apex_params_snapshot(drl_apex* h, int device, int algo, int num_action, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);
+
+struct ApexActs {          // forward activations of one network over up to `cap` rows (caller row order)
+  float* a1;               // [M,20,20,32]
+  float* a2;               // [M,9,9,64]
+  float* a3;               // [M,3136]
+  float* e1;               // [A,256]
+  float* table;            // [A,256]
+  float* zpart;            // [splits][M,512] split-K partial sums of the two first head layers
+  float* hid1;             // [2][M,256]  value / mean stream hidden 1
+  float* hid2;             // [2][M,256]
+  float* vstream;          // [M,A]  value stream output
+  float* scratch_sm;       // [M,A]  (softmax of the value stream: by-product of the shared output kernel, unused)
+  float* mstream;          // [M]    "mean" stream output
+  int cap;
+};
+
+struct ApexBwd {           // backward workspace, Mb = B rows
+  float *dq, *dmean;       // [Mb,32] each (columns >= A / >= 1 stay zero)
+  float *dhid2, *dhid1;    // [2][Mb,256]
+  float *da3, *du, *dpre2, *dpre1, *da2, *da1;
+  float *wg_part, *wg_part2, *dcol;
+};
+
+struct ApexIn {                // views of one staging slot
+  uint8_t* frames;             // [2B][84,84,4]: state rows, then next_state rows
+  int32_t* pa2;                // [2B]: previous_action, then action (the embedding input of the rows s')
+  float* reward;               // [B]
+  uint8_t* done;               // [B]
+  float* weight;               // [B]
+};
+
+}  // namespace drl
+
+// the Ape-X / A3C learner handle (apex.cu); the device replay memory (apex_replay.cu) drives its step
+struct drl_apex : drl::AdamLearner {
+  drl_apex_config cfg{};
+  int A = 0;
+  drl::ApexLayout pl{};
+  drl::ApexActs act{}, tact{};
+  drl::ApexBwd bwd{};
+  float *main_q = nullptr, *next_main_q = nullptr, *target_q = nullptr, *target_value = nullptr, *sav = nullptr,
+        *td_dev = nullptr;
+  // A3C runs on the same body (drl_a3c_*): no target scope, the A3C loss kernel of apex.cu, three loss scalars
+  int algo = 0;                // 0 = Ape-X DQN, 1 = A3C
+  float a3c_baseline_coef = 0.f, a3c_entropy_coef = 0.f;
+  int a3c_clip = 0;
+  float* adv = nullptr;        // [B] advantage tap
+  std::vector<drl::ApexIn> in;      // per slot
+};
+
+namespace drl {
+
+// forward passes + TD kernel over n transitions held by `sl` on the compute stream (the target forward on its own stream
+// pair when the step runs parallel); train = also the head gradients and the loss.  Writes |target - q(s, a)| to td_dev
+// and, when td_host is not null, to td_host.  Adds the launches to *launches unless it is null.
+int enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* td_host, int* launches);
 
 }  // namespace drl

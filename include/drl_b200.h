@@ -519,6 +519,44 @@ int drl_per_size(const drl_per* p, int64_t* n_entries);  /* SumTree.n_entries */
 int drl_per_beta(const drl_per* p, double* beta);
 
 /* ------------------------------------------------------------------------------------------
+ * Ape-X prioritized replay memory on the device (DESIGN.md section 10): buffer_queue.Memory with the transitions in HBM
+ * (state, next_state u8 [capacity,84,84,4]; previous_action, action i32; reward f32; done u8; zero-initialised), the
+ * float64 sum tree on the device, and the learner loop of train_apex.py:82-155 -- ingest, sample, minibatch gather,
+ * step, priority update -- as kernels on the learner's compute stream.  Same constants and arithmetic as drl_per_*
+ * (e = 0.001, a = 0.6, beta 0.4 -> 1 by +0.001 per sample); the uniforms of random.uniform(a, b) come from the caller.
+ * The memory outlives any learner: every call that uses one takes a drl_apex* (Ape-X, not A3C, on the memory's
+ * device) and orders itself after the memory's previous work on whichever stream that ran.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_apex_replay drl_apex_replay;
+/* capacity in [2, 2^31]: 56 KB of device memory per transition (5.6 GB at the reference's 1e5). */
+int drl_apex_replay_create(int32_t device, int64_t capacity, drl_apex_replay** out);
+int drl_apex_replay_destroy(drl_apex_replay* r);
+/* Memory.add for n transitions in order at the write cursor (wrapping).  error == NULL: the priorities are the
+ * learner's |td| of these transitions (agent/apex.py:116-133), computed on the device and never copied to the host;
+ * then 1 <= n <= the learner's batch.  Otherwise error [n] are the caller's and learner may be NULL.  Does not wait
+ * for the learner's compute stream. */
+int drl_apex_replay_add(drl_apex_replay* r, drl_apex* learner, int32_t n, const uint8_t* state,
+                        const uint8_t* next_state, const int32_t* previous_action, const int32_t* action,
+                        const float* reward, const uint8_t* done, const double* error);
+/* Memory.sample(B) with the caller's uniforms u01 [B] (B = the learner's batch) -> gather into staging slot `slot` ->
+ * the learner's step on that slot -> Memory.update of the sampled leaves with the step's |td|.  Asynchronous:
+ * drl_apex_wait returns the loss and the priorities once the update has run.  DRL_ERR_STATE on an empty memory. */
+int drl_apex_replay_step_async(drl_apex_replay* r, drl_apex* learner, int32_t slot, const double* u01);
+/* The device kernels without a learner (tests, callers with their own loop); synchronous.  sample is Memory.sample
+ * (drl_per_sample's outputs, advances beta); update is Memory.update of n leaves in order. */
+int drl_apex_replay_sample(drl_apex_replay* r, int32_t n, const double* u01, int64_t* tree_index,
+                           int64_t* data_index, double* priority, double* is_weight);
+int drl_apex_replay_update(drl_apex_replay* r, int32_t n, const int64_t* tree_index, const double* error);
+/* The draws of the most recent sample (or step): tree_index, priority, is_weight [n]; any pointer may be NULL. */
+int drl_apex_replay_last_sample(drl_apex_replay* r, int64_t* tree_index, double* priority, double* is_weight);
+/* Rows [data_index, data_index + n) of the storage; any pointer may be NULL. */
+int drl_apex_replay_read(drl_apex_replay* r, int64_t data_index, int32_t n, uint8_t* state, uint8_t* next_state,
+                         int32_t* previous_action, int32_t* action, float* reward, uint8_t* done);
+int drl_apex_replay_total(drl_apex_replay* r, double* total);      /* SumTree.total */
+int drl_apex_replay_size(drl_apex_replay* r, int64_t* n_entries);  /* SumTree.n_entries */
+int drl_apex_replay_beta(drl_apex_replay* r, double* beta);
+
+/* ------------------------------------------------------------------------------------------
  * R2D2 learner (SURVEY.md section 8(f) row 3, BASELINE.json config 5): replaces r2d2.Agent's learner graph
  * (agent/r2d2.py:13-95) over model/r2d2_lstm.py:28-116 (conv stack + action embedding + ONE LSTMCell, unrolled seq_len
  * steps per scope from a stored (h, c) with the carried state multiplied by (1 - done) after every step; dense 128;
