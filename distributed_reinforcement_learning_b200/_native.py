@@ -266,6 +266,17 @@ def _load():
         "drl_apex_replay_total": (C.c_int, [vp, C.POINTER(C.c_double)]),
         "drl_apex_replay_size": (C.c_int, [vp, C.POINTER(i64)]),
         "drl_apex_replay_beta": (C.c_int, [vp, C.POINTER(C.c_double)]),
+        "drl_r2d2_replay_create": (C.c_int, [i32, i64, i32, i32, i32, C.POINTER(vp)]),
+        "drl_r2d2_replay_destroy": (C.c_int, [vp]),
+        "drl_r2d2_replay_add": (C.c_int, [vp, vp, i32] + [vp] * 8),
+        "drl_r2d2_replay_step_async": (C.c_int, [vp, vp, i32, vp]),
+        "drl_r2d2_replay_sample": (C.c_int, [vp, i32] + [vp] * 5),
+        "drl_r2d2_replay_update": (C.c_int, [vp, i32, vp, vp]),
+        "drl_r2d2_replay_last_sample": (C.c_int, [vp, vp, vp, vp]),
+        "drl_r2d2_replay_read": (C.c_int, [vp, i64, i32] + [vp] * 7),
+        "drl_r2d2_replay_total": (C.c_int, [vp, C.POINTER(C.c_double)]),
+        "drl_r2d2_replay_size": (C.c_int, [vp, C.POINTER(i64)]),
+        "drl_r2d2_replay_beta": (C.c_int, [vp, C.POINTER(C.c_double)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)

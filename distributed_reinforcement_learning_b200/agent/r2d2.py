@@ -7,15 +7,21 @@ the learner branch of ``train_r2d2.py:87-165`` runs on it unchanged, with the TF
   Agent.parameter_sync agent/r2d2.py:161-162 ; Agent.main_to_target :164-165 ; Agent.set_session :167-169
   Agent.get_action     agent/r2d2.py:171-191 -> (action, q_value[action], h', c')
   Agent.sync_policy    (new) parameter_sync into a NativeR2D2Policy (r2d2_policy.py), device to device from the learner
+  Agent.device_memory  (new) a DeviceMemory: the replay memory of train_r2d2.py:92-93 on the GPU (r2d2_replay.py)
+  Agent.train_from_memory (new) Memory.sample + the minibatch lists + train + Memory.update (train_r2d2.py:122-162)
+                       as one device-resident step -> (loss, td_error)
   Agent.main_q_value_test / target_q_value_test   agent/r2d2.py:193-217
 """
 import os
+import random
 import threading
 
 import numpy as np
 
+from .. import dp
 from ..model import r2d2_lstm
 from ..r2d2_learner import MAIN, TARGET, NativeR2D2Learner
+from ..r2d2_replay import NativeR2D2Replay
 
 _AGENTS = {}
 
@@ -106,6 +112,33 @@ class Agent:
         self._last = out
         return out["loss"], td
 
+    def device_memory(self, capacity):
+        """A prioritized replay memory of ``capacity`` sequences on this agent's GPU (buffer_queue.Memory's
+        arithmetic); fill it with DeviceMemory.add, train from it with train_from_memory."""
+        return DeviceMemory(self, capacity)
+
+    def train_from_memory(self, memory, batch_size, u01=None):
+        """One iteration of the learner loop's training half (train_r2d2.py:122-162) against a DeviceMemory:
+        per_replay_buffer.sample(batch_size), the minibatch lists, train and the priority update, all on the GPU.
+        ``u01`` ([batch_size] in [0, 1)) are the strata's uniforms; by default ``random.random()`` draws them exactly as
+        Memory.sample does, so a host loop and a device loop seeded alike sample the same strata.  -> (loss, td_error)."""
+        if dp.distributed():
+            raise RuntimeError("train_from_memory: a DeviceMemory is local to one GPU; data-parallel training "
+                               "(torch.distributed world > 1) uses Memory and train")
+        if u01 is None:
+            u01 = [random.random() for _ in range(batch_size)]
+        if self._engine is not None and self._engine.B != batch_size:
+            self._pull_state()
+            self._engine.close()
+            self._engine = None
+        eng = self._get_engine(batch_size)
+        slot = self._slot
+        self._slot = (self._slot + 1) % eng.num_slots
+        memory.replay.step_async(eng, slot, u01)
+        out, td = eng.wait()
+        self._last = out
+        return out["loss"], td
+
     def _snapshot_params(self):
         with self._lock:
             self._ensure_init()
@@ -178,6 +211,59 @@ class Agent:
     grad_norm = property(lambda self: self._last.get("grad_norm"))
 
 
+class DeviceMemory:
+    """The replay memory of train_r2d2.py:92-93 on the agent's GPU, for the device loop:
+
+        memory = learner.device_memory(capacity)
+        q = r2d2_queue.sample_batch()
+        memory.add(q.state, q.previous_action, q.action, q.previous_h, q.previous_c, q.reward, q.done)
+        loss, td_error = learner.train_from_memory(memory, batch_size)  # sample .. train .. update
+
+    It outlives a rebuild of the agent's learner (another batch size): the agent passes its current learner to each
+    call.  ``replay`` is the NativeR2D2Replay; ``n_entries``, ``beta``, ``total()`` and ``last_sample()`` read its state."""
+
+    def __init__(self, agent, capacity):
+        self.agent = agent
+        self.capacity = int(capacity)
+        self.replay = NativeR2D2Replay(self.capacity, seq_len=agent.seq_len, num_action=agent.num_action,
+                                       input_shape=tuple(agent.input_shape), device=agent.device)
+
+    @staticmethod
+    def _step0(x):
+        """h / c as stored by the actors ([n, S, L]) or already at step 0 ([n, L]) -> [n, L] float32."""
+        x = np.asarray(x, np.float32)
+        return x[:, 0] if x.ndim == 3 else x
+
+    def add(self, state, previous_action, action, h, c, reward, done):
+        """learner.get_td_error(...) followed by per_replay_buffer.add(td_error, ...) for each sequence of one
+        R2D2FIFOQueue.sample_batch() in order (train_r2d2.py:101-120); the priorities are the learner's |td|, computed
+        for the whole batch at once and applied on the device.  Sequences beyond the learner's batch go through in
+        chunks of it."""
+        a = self.agent
+        st = a._u8(state)
+        pa, ac = np.asarray(previous_action), np.asarray(action)
+        h0, c0 = self._step0(h), self._step0(c)
+        rw, dn = np.asarray(reward), np.asarray(done)
+        with a._lock:
+            eng = a._engine if a._engine is not None else a._get_engine(st.shape[0])
+            for lo in range(0, st.shape[0], eng.B):
+                hi = min(lo + eng.B, st.shape[0])
+                self.replay.add(eng, st[lo:hi], pa[lo:hi], ac[lo:hi], h0[lo:hi], c0[lo:hi], rw[lo:hi], dn[lo:hi])
+
+    n_entries = property(lambda self: self.replay.n_entries)
+    beta = property(lambda self: self.replay.beta)
+
+    def total(self):
+        return self.replay.total()
+
+    def last_sample(self):
+        """(tree_index, priority, is_weight) of the most recent training step's draws."""
+        return self.replay.last_sample()
+
+    def close(self):
+        self.replay.close()
+
+
 def _locked(fn):
     def wrapper(self, *a, **k):
         with self._lock:
@@ -187,6 +273,7 @@ def _locked(fn):
 
 
 # actor threads call these on a shared agent while the learner thread trains (in-process launch mode)
-for _n in ('save_weights', 'load_weights', 'set_session', 'main_to_target', 'get_action', 'get_td_error', 'train', 'main_q_value_test', 'target_q_value_test'):
+for _n in ('save_weights', 'load_weights', 'set_session', 'main_to_target', 'get_action', 'get_td_error', 'train', 'main_q_value_test', 'target_q_value_test',
+           'train_from_memory'):
     if hasattr(Agent, _n):
         setattr(Agent, _n, _locked(getattr(Agent, _n)))

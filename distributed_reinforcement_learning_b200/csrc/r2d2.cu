@@ -21,32 +21,6 @@
 
 namespace drl {
 
-struct R2Acts {            // activations of one scope, time-major rows m = t*B + b
-  float *a1, *a2, *a3, *e1, *table;
-  float* zpart;            // [splits][M, 4L]: [a3 | emb] W_x partial sums
-  float* zx;               // [M, 4L]: their sum (the recurrence reads one value per gate and step)
-  float* gates;            // [M, 4L] sigmoid(i), tanh(j), sigmoid(f + 1), sigmoid(o)
-  float *tc, *hout;        // [M, L] tanh(c_t), h_t (the cell output, BEFORE the done mask)
-  float *hin, *cin;        // [M, L] the (masked) state that entered step t
-  float* q1;               // [M, 128]
-  float* q;                // [M, A]
-};
-struct R2Bwd {
-  float *dq, *dmean;       // [M, 32]
-  float *dq1, *dhout, *dz; // [M,128], [M,L], [M,4L]
-  float *da3, *du, *dpre2, *dpre1, *da2, *da1, *wg_part, *wg_part2, *dcol;
-};
-struct R2In {              // one staged minibatch, caller's batch-major layout
-  const uint8_t* frames;   // [B, S, 84, 84, C]
-  const int32_t* pa;       // [B, S]
-  const int32_t* action;   // [B, S]
-  const float* h0;         // [B, L]
-  const float* c0;         // [B, L]
-  const float* reward;     // [B, S]
-  const uint8_t* done;     // [B, S]
-  const float* weight;     // [B]
-};
-
 // conv1 weight gradient over single-channel frames (Conv1A1: r2d2_defs.cuh)
 using Conv1WA1 = ConvWgradA<uint8_t, 84, 84, 1, 20, 20, 8, 4, true>;
 
@@ -621,45 +595,8 @@ static int r2_backward(const Streams& st, const R2Layout& pl, const float* P, co
 
 using namespace drl;
 
-struct drl_r2d2 : AdamLearner {
-  drl_r2d2_config cfg{};
-  int S = 0, A = 0, C = 1, Nt = 0;
-  size_t frame = 0;
-  R2Layout pl{};
-  R2Acts act{}, tact{};
-  R2Bwd bwd{};
-  float *sav = nullptr, *target_value = nullptr, *td_dev = nullptr, *c_last = nullptr;
-  std::vector<R2In> in;                 // per slot
-};
-
-namespace {
-
-constexpr const char* kName = "r2d2";
-
-int alloc_acts(drl_r2d2* h, R2Acts& a) {
-  const size_t M = (size_t)h->B * h->S, A = h->A;
-  DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
-  DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
-  DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
-  DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
-  DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
-  size_t zmax = 0;
-  for (int mode = 1; mode <= 2; ++mode)
-    for (int m = 1; m <= (int)M; ++m) zmax = std::max(zmax, (size_t)plan_r2_x(m, mode).splits * m * kR2G);
-  DRL_TRY(dev_alloc(h, &a.zpart, zmax));
-  DRL_TRY(dev_alloc(h, &a.zx, M * kR2G));
-  DRL_TRY(dev_alloc(h, &a.gates, M * kR2G));
-  DRL_TRY(dev_alloc(h, &a.tc, M * kR2L));
-  DRL_TRY(dev_alloc(h, &a.hout, M * kR2L));
-  DRL_TRY(dev_alloc(h, &a.hin, M * kR2L));
-  DRL_TRY(dev_alloc(h, &a.cin, M * kR2L));
-  DRL_TRY(dev_alloc(h, &a.q1, M * kR2H));
-  DRL_TRY(dev_alloc(h, &a.q, M * A));
-  return DRL_OK;
-}
-
-// both unrolls + TD kernel over nb sequences held by `in`
-int enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, float* td_host, int* launches) {
+// both unrolls + TD kernel over nb sequences held by `in` (r2d2_defs.cuh)
+int drl::enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, float* td_host, int* launches) {
   const Streams st = h->streams(), tst = h->target_streams();
   // the two unrolls are independent (and each recurrence kernel only occupies nb SMs): the target scope runs on its
   // own stream pair beside the main scope and joins before the TD kernel
@@ -685,6 +622,32 @@ int enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, float* t
   prof_mark(h->compute, "td_target_loss");
   DRL_CUDA_CHECK((launch_k(r2d2_td_kernel, 1, 256, 0, h->compute, a)));
   if (launches) *launches += 1;
+  return DRL_OK;
+}
+
+namespace {
+
+constexpr const char* kName = "r2d2";
+
+int alloc_acts(drl_r2d2* h, R2Acts& a) {
+  const size_t M = (size_t)h->B * h->S, A = h->A;
+  DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
+  DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
+  DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
+  DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
+  DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
+  size_t zmax = 0;
+  for (int mode = 1; mode <= 2; ++mode)
+    for (int m = 1; m <= (int)M; ++m) zmax = std::max(zmax, (size_t)plan_r2_x(m, mode).splits * m * kR2G);
+  DRL_TRY(dev_alloc(h, &a.zpart, zmax));
+  DRL_TRY(dev_alloc(h, &a.zx, M * kR2G));
+  DRL_TRY(dev_alloc(h, &a.gates, M * kR2G));
+  DRL_TRY(dev_alloc(h, &a.tc, M * kR2L));
+  DRL_TRY(dev_alloc(h, &a.hout, M * kR2L));
+  DRL_TRY(dev_alloc(h, &a.hin, M * kR2L));
+  DRL_TRY(dev_alloc(h, &a.cin, M * kR2L));
+  DRL_TRY(dev_alloc(h, &a.q1, M * kR2H));
+  DRL_TRY(dev_alloc(h, &a.q, M * A));
   return DRL_OK;
 }
 

@@ -1,6 +1,10 @@
-// r2d2_defs.cuh -- definitions shared by the R2D2 learner (r2d2.cu) and the R2D2 policy engine (r2d2_policy.cu): the
-// network's sizes, its flat parameter layout, the single-channel conv1 loader and the learner's conv forward.
+// r2d2_defs.cuh -- definitions shared by the R2D2 learner (r2d2.cu), the R2D2 policy engine (r2d2_policy.cu) and the
+// R2D2 device replay memory (r2d2_replay.cu): the network's sizes, its flat parameter layout, the single-channel conv1
+// loader, the learner's conv forward, the learner handle and its forward + TD path.
 #pragma once
+#include <vector>
+
+#include "adam_learner.cuh"
 #include "kernels.h"
 #include "loaders.cuh"
 
@@ -45,5 +49,53 @@ int r2_conv_images(cudaStream_t s, const R2Layout& pl, const float* P, uint8_t* 
 // `channels` input channels (DRL_ERR_INVALID otherwise)
 int r2d2_params_snapshot(drl_r2d2* h, int device, int num_action, int channels, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);
+
+struct R2Acts {            // activations of one scope, time-major rows m = t*B + b
+  float *a1, *a2, *a3, *e1, *table;
+  float* zpart;            // [splits][M, 4L]: [a3 | emb] W_x partial sums
+  float* zx;               // [M, 4L]: their sum (the recurrence reads one value per gate and step)
+  float* gates;            // [M, 4L] sigmoid(i), tanh(j), sigmoid(f + 1), sigmoid(o)
+  float *tc, *hout;        // [M, L] tanh(c_t), h_t (the cell output, BEFORE the done mask)
+  float *hin, *cin;        // [M, L] the (masked) state that entered step t
+  float* q1;               // [M, 128]
+  float* q;                // [M, A]
+};
+struct R2Bwd {
+  float *dq, *dmean;       // [M, 32]
+  float *dq1, *dhout, *dz; // [M,128], [M,L], [M,4L]
+  float *da3, *du, *dpre2, *dpre1, *da2, *da1, *wg_part, *wg_part2, *dcol;
+};
+struct R2In {              // one staged minibatch, caller's batch-major layout
+  const uint8_t* frames;   // [B, S, 84, 84, C]
+  const int32_t* pa;       // [B, S]
+  const int32_t* action;   // [B, S]
+  const float* h0;         // [B, L]
+  const float* c0;         // [B, L]
+  const float* reward;     // [B, S]
+  const uint8_t* done;     // [B, S]
+  const float* weight;     // [B]
+};
+
+}  // namespace drl
+
+// the R2D2 learner handle (r2d2.cu); the device replay memory (r2d2_replay.cu) drives its step
+struct drl_r2d2 : drl::AdamLearner {
+  drl_r2d2_config cfg{};
+  int S = 0, A = 0, C = 1, Nt = 0;
+  size_t frame = 0;
+  drl::R2Layout pl{};
+  drl::R2Acts act{}, tact{};
+  drl::R2Bwd bwd{};
+  float *sav = nullptr, *target_value = nullptr, *td_dev = nullptr, *c_last = nullptr;
+  std::vector<drl::R2In> in;            // per slot
+};
+
+namespace drl {
+
+// both unrolls (main and target scope) + TD kernel over the nb sequences held by `in` on the compute stream (the target
+// unroll on its own stream pair when the step runs parallel); train = also the head gradients and the loss.  Writes
+// |mean_t(target - q)| per sequence to td_dev and, when td_host is not null, to td_host.  Adds the launches to
+// *launches unless it is null.
+int enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, float* td_host, int* launches);
 
 }  // namespace drl

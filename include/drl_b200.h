@@ -640,6 +640,47 @@ int drl_r2d2_stream(drl_r2d2* h, void** stream);
 int drl_r2d2_launches_per_step(const drl_r2d2* h, int32_t* n);
 
 /* ------------------------------------------------------------------------------------------
+ * R2D2 prioritized sequence replay memory on the device (DESIGN.md section 11): buffer_queue.Memory with one
+ * stored-state sequence per record in HBM (state u8 [S,84,84,C]; previous_action, action i32 [S]; reward f32 [S]; done
+ * u8 [S]; h0, c0 f32 [64], step 0 of the stored states, the only step the learner reads; zero-initialised), the float64
+ * sum tree on the device, and the learner loop of train_r2d2.py:87-165 -- ingest, sample, minibatch gather, step,
+ * priority update -- as kernels on the learner's compute stream.  The sum tree, its constants and arithmetic and the
+ * sample / update / last_sample / total / size / beta calls behave as drl_apex_replay_*'s.  The memory outlives any
+ * learner: every call that uses one takes a drl_r2d2* on the memory's device with the memory's seq_len, channels and
+ * num_action, and orders itself after the memory's previous work on whichever stream that ran.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_r2d2_replay drl_r2d2_replay;
+/* capacity in [2, 2^31], seq_len >= 2, channels 1 or 4, num_action in [2, 32].  Device memory per sequence:
+ * S * (7,056 C + 13) + 512 bytes: 106,547 B at S = 15, C = 1 (10.7 GB at the reference's capacity 1e5), 424,067 B at
+ * C = 4 (42.4 GB). */
+int drl_r2d2_replay_create(int32_t device, int64_t capacity, int32_t seq_len, int32_t channels, int32_t num_action,
+                           drl_r2d2_replay** out);
+int drl_r2d2_replay_destroy(drl_r2d2_replay* r);
+/* Memory.add for n sequences in order at the write cursor (wrapping); the arguments are drl_r2d2_td_error's (h0, c0
+ * [n, 64]).  error == NULL: the priorities are the learner's |td| of these sequences (agent/r2d2.py:97-130, all n in
+ * one pass), computed on the device and never copied to the host; then 1 <= n <= the learner's batch.  Otherwise
+ * error [n] are the caller's and learner may be NULL.  Every previous_action and action must be in [0, num_action).
+ * Does not wait for the learner's compute stream. */
+int drl_r2d2_replay_add(drl_r2d2_replay* r, drl_r2d2* learner, int32_t n, const uint8_t* state,
+                        const int32_t* previous_action, const int32_t* action, const float* h0, const float* c0,
+                        const float* reward, const uint8_t* done, const double* error);
+/* Memory.sample(B) with the caller's uniforms u01 [B] (B = the learner's batch) -> gather into staging slot `slot` ->
+ * the learner's step on that slot -> Memory.update of the sampled leaves with the step's |td|.  Asynchronous:
+ * drl_r2d2_wait returns the loss and the priorities once the update has run.  DRL_ERR_STATE on an empty memory. */
+int drl_r2d2_replay_step_async(drl_r2d2_replay* r, drl_r2d2* learner, int32_t slot, const double* u01);
+/* As drl_apex_replay_sample / _update / _last_sample. */
+int drl_r2d2_replay_sample(drl_r2d2_replay* r, int32_t n, const double* u01, int64_t* tree_index,
+                           int64_t* data_index, double* priority, double* is_weight);
+int drl_r2d2_replay_update(drl_r2d2_replay* r, int32_t n, const int64_t* tree_index, const double* error);
+int drl_r2d2_replay_last_sample(drl_r2d2_replay* r, int64_t* tree_index, double* priority, double* is_weight);
+/* Rows [data_index, data_index + n) of the storage (h0, c0 [n, 64]); any pointer may be NULL. */
+int drl_r2d2_replay_read(drl_r2d2_replay* r, int64_t data_index, int32_t n, uint8_t* state, int32_t* previous_action,
+                         int32_t* action, float* h0, float* c0, float* reward, uint8_t* done);
+int drl_r2d2_replay_total(drl_r2d2_replay* r, double* total);      /* SumTree.total */
+int drl_r2d2_replay_size(drl_r2d2_replay* r, int64_t* n_entries);  /* SumTree.n_entries */
+int drl_r2d2_replay_beta(drl_r2d2_replay* r, double* beta);
+
+/* ------------------------------------------------------------------------------------------
  * A3C learner: replaces a3c.Agent's learner graph (agent/a3c.py:11-78) over model/actor_critic.py:3-56 (the same body
  * as the Ape-X network: attention_CNN || action embedding -> concat 3392 -> actor [256,256,A + softmax] and critic
  * [256,256,1]) and optimizer/a2c.py:3-26, with TF1 Adam + polynomial decay + global-norm clipping.  network(s, prev_a)
