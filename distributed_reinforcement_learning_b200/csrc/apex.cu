@@ -173,43 +173,6 @@ __global__ void __launch_bounds__(256) a3c_loss_kernel(A3cArgs a) {
   }
 }
 
-// conv1 (model/apex_value.py:5), conv2 (:6), conv3 -> flatten HWC (:7-9)
-int apex_conv_forward(cudaStream_t s, const ApexLayout& pl, const float* P, const uint8_t* img_conv2,
-                      const uint8_t* img_conv3, const uint8_t* frames, int M, float* a1, float* a2, float* a3, int mode,
-                      bool tgt, cudaEvent_t images_ready, int* launches) {
-  const RowMap map{M, 1};          // rows are already in caller order: src(m) == m
-  int n = 0;
-  {
-    Conv1A al{frames, map};
-    PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{a1, 32, P + pl.conv1_b};
-    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
-  }
-  if (images_ready) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, images_ready, 0));
-  {
-    Conv2A al{a1, map};
-    PlainB bl{P + pl.conv2_w, 64, 0};
-    PretiledB<PlainB> blp{img_conv2, 512 / 32};
-    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv2_fwd" : "conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
-  }
-  {
-    Conv3A al{a2, map};
-    PlainB bl{P + pl.conv3_w, 64, 0};
-    PretiledB<PlainB> blp{img_conv3, 576 / 32};
-    EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv3_fwd" : "conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
-  }
-  *launches += n;
-  return DRL_OK;
-}
-
-int apex_conv_images(cudaStream_t s, const ApexLayout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3) {
-  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, img_conv2)));
-  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, img_conv3)));
-  return DRL_OK;
-}
-
 // ------------------------------------------------------------------------------------------
 // Forward of the dueling network (model/apex_value.py:22-41) over M rows.  `tgt` only selects the profile names.
 // Weight images (tensor-core modes): img[1]/img[2] conv2/conv3 forward, img[5]/img[6] the dCol operands of backward.
@@ -225,8 +188,7 @@ static int apex_forward(const Streams& st, const ApexLayout& pl, const float* P,
   s = side;
   if (retile_fwd && mode >= 2) {
     prof_mark(s, tgt ? "target_weight_retile" : "weight_retile");
-    DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, wi.img[1])));
-    DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, wi.img[2])));
+    DRL_TRY(conv_images_tf32(s, pl, P, wi.img[1], wi.img[2]));
     n += 2;
   }
   if (st.par) DRL_CUDA_CHECK(cudaEventRecord(st.ev[7], side));
@@ -239,8 +201,9 @@ static int apex_forward(const Streams& st, const ApexLayout& pl, const float* P,
     n += 2;
   }
   s = st.main;
-  DRL_TRY(apex_conv_forward(s, pl, P, wi.img[1], wi.img[2], frames, M, act.a1, act.a2, act.a3, mode, tgt,
-                            st.par ? st.ev[7] : nullptr, &n));
+  // conv1 (model/apex_value.py:5), conv2 (:6), conv3 -> flatten HWC (:7-9), rows in the caller's order
+  DRL_TRY(conv_forward_tf32<Geo::IC>(s, pl, P, wi.img[1], wi.img[2], frames, M, 1, act.a1, act.a2, act.a3, mode, tgt,
+                                      st.par ? st.ev[7] : nullptr, &n));
   DRL_TRY(join_from_side(st, 1));
   // first layers of both streams: [M, 3392] x [3392, 256 | 256], split-K partial sums, then bias + ReLU (:17-19,28-37)
   const SplitPlan sp = plan_head1(M);

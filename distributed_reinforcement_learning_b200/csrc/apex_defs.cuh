@@ -1,6 +1,6 @@
 // apex_defs.cuh -- definitions shared by the Ape-X / A3C learner (apex.cu), the Ape-X / A3C policy engine
 // (apex_policy.cu) and the Ape-X device replay memory (apex_replay.cu): the dueling network's flat parameter layout, its
-// head sizes, the learner's conv forward, the learner handle and its forward + TD path.
+// head sizes, the learner handle and its forward + TD path.
 #pragma once
 #include <vector>
 
@@ -11,10 +11,7 @@ namespace drl {
 
 // Offsets (in floats) inside the padded flat vectors of ONE network (FlatLayout, kernels.h).  A3C uses the same layout:
 // its actor stream sits in the value* slots and its critic stream in the mean* slots (model/actor_critic.py:27-38).
-struct ApexLayout : FlatLayout {
-  int A;
-  int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b;
-  int64_t emb1_w, emb1_b, emb2_w, emb2_b;
+struct ApexLayout : TrunkLayout {
   int64_t value1_w, value1_b, value2_w, value2_b, value3_w, value3_b;
   int64_t mean1_w, mean1_b, mean2_w, mean2_b, mean3_w, mean3_b;
   void init(int num_action) {
@@ -34,16 +31,6 @@ struct ApexLayout : FlatLayout {
 
 constexpr int kHeadN = 2 * Geo::HID;             // 512 columns: [value hidden | mean hidden]
 constexpr int kCat = Geo::FLAT + Geo::EMB;       // 3392
-
-// conv1 / conv2 / conv3 forward of one network over M rows (caller row order) on stream s, with the learner's kernels
-// and configurations for math mode `mode` (1: FP32 FFMA; 2: wgmma 3xTF32 with the conv2 / conv3 weight images of
-// apex_conv_images).  When images_ready is not null, conv2 waits for it (the images and the embedding are built on
-// another stream).  `tgt` only names the launches for the per-kernel profile; adds the launches to *launches.
-int apex_conv_forward(cudaStream_t s, const ApexLayout& pl, const float* P, const uint8_t* img_conv2,
-                      const uint8_t* img_conv3, const uint8_t* frames, int M, float* a1, float* a2, float* a3, int mode,
-                      bool tgt, cudaEvent_t images_ready, int* launches);
-// the conv2 / conv3 forward weight images of math mode 2 (WeightImages slots 1 and 2 sizes)
-int apex_conv_images(cudaStream_t s, const ApexLayout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3);
 
 // drl_apex_policy_sync_from_learner: adam_params_snapshot of the main network of an Ape-X (algo 0) or A3C (algo 1)
 // learner with num_action actions (DRL_ERR_INVALID for another algo or num_action)

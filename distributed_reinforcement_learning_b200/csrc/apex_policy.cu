@@ -9,7 +9,7 @@
 //                                         stream is never evaluated (the reference actor fetches only the policy).
 //
 // One call = one H2D of the staged inputs + 5 kernels on the engine's own stream:
-//   conv1 / conv2 / conv3   the Ape-X learner's math-mode-2 kernels and configurations (apex.cu: apex_conv_forward)
+//   conv1 / conv2 / conv3   the Ape-X learner's math-mode-2 kernels and configurations (layer_defs.cuh: conv_forward_tf32)
 //   skinny_splitk_fwd       z = [a3 | table[pa]] [W1_value | W1_mean] (Ape-X, N = 512) or [a3 | table[pa]] W1_actor
 //                           (A3C, N = 256) as a skinny split-K FP32-FFMA GEMM (K = 3392, policy_lstm.cuh)
 //   apex_policy_head        split-K sum + bias + ReLU, the 256 x 256 layer(s), the output layer(s) and the action rule;
@@ -18,27 +18,17 @@
 // Both new kernels sum in a fixed order without atomics: eager and graph replays, and repeated calls, are bitwise equal.
 #include <string.h>
 
-#include <mutex>
-#include <string>
-#include <vector>
-
-#include <nvtx3/nvToolsExt.h>
-
 #include "apex_defs.cuh"
+#include "policy_core.cuh"
 #include "policy_head.cuh"
 #include "policy_lstm.cuh"
 
 namespace drl {
 namespace {
 
-struct ApexPolicyNvtx {
-  explicit ApexPolicyNvtx(const char* name) { nvtxRangePushA(name); }
-  ~ApexPolicyNvtx() { nvtxRangePop(); }
-};
-
+constexpr const char* kName = "apex policy";
 constexpr int kMaxApexPolicyRows = 64;
 constexpr int kApexMaxA = 32;
-constexpr int kApexConvMode = 2;   // the learner's default math mode (wgmma 3xTF32 convolutions on weight images)
 
 // ---- skinny_splitk_fwd (policy_lstm.cuh) ------------------------------------------------------------------------
 // K = 3392 = 2^6 * 53.  grid (N / 128 column chunks) x (kApexSplits K splits): Ape-X 4 x 53 = 212 CTAs, A3C 2 x 53 =
@@ -213,57 +203,24 @@ int set_apex_policy_kernel_attributes() {
 
 using namespace drl;
 
-struct drl_apex_policy {
-  drl_apex_policy_config cfg{};
-  int A = 0;
+struct drl_apex_policy : PolicyCore {
   ApexLayout pl{};
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev_ready = nullptr, ev_copied = nullptr;   // learner -> policy and policy -> learner edges of a sync
-  cudaEvent_t ev_start = nullptr, ev_stop = nullptr;     // device time of the last act
-  bool timed = false;
-  float* params = nullptr;       // padded one-network vector (learner layout)
-  uint8_t* img_conv2 = nullptr;  // conv2 / conv3 forward weight images (math mode 2)
-  uint8_t* img_conv3 = nullptr;
-  float* e1 = nullptr;           // [A,256] relu(emb1), scratch of emb_forward
-  float* table = nullptr;        // [A,256] action-embedding table (depends on the parameters only)
-  float *a1 = nullptr, *a2 = nullptr, *a3 = nullptr;
-  float* zpart = nullptr;        // [kApexSplits][max_batch][N]
-  uint8_t* d_in = nullptr;       // device input block (apex_in_layout)
-  uint8_t* h_in = nullptr;       // pinned staging of the same block
-  uint8_t* h_out = nullptr;      // mapped pinned outputs: q / policy [max_batch][A] | action | q[action] / policy[action]
-  uint8_t* d_out = nullptr;      // its device alias
+  int algo = 0;   // 0 = Ape-X, 1 = A3C
+  // mapped outputs: q / policy [max_batch][A] | action | q[action] / policy[action]
   size_t off_act = 0, off_sel = 0;
-  std::vector<cudaGraphExec_t> graphs;   // per row count n
-  std::vector<void*> allocs;
-  std::recursive_mutex mu;
 };
-#define DRL_APEX_POLICY_LOCK(h) std::lock_guard<std::recursive_mutex> _drl_apex_policy_lock((h)->mu)
 
 namespace {
 
-int check_apex_policy(const drl_apex_policy* h) {
-  if (!h) { set_error("null apex policy handle"); return DRL_ERR_INVALID; }
-  return DRL_OK;
-}
-
-// embedding table and conv weight images of the current parameters, on the policy's stream
-int refresh_derived(drl_apex_policy* h) {
-  const ApexLayout& pl = h->pl;
-  const float* P = h->params;
-  DRL_TRY(emb_forward(h->stream, P + pl.emb1_w, P + pl.emb1_b, P + pl.emb2_w, P + pl.emb2_b, h->e1, h->table, h->A));
-  return apex_conv_images(h->stream, pl, P, h->img_conv2, h->img_conv3);
-}
-
-int enqueue_act(drl_apex_policy* h, int n) {
+int enqueue_act(PolicyCore* c, int n) {
+  drl_apex_policy* h = static_cast<drl_apex_policy*>(c);
   const ApexInLayout l = apex_in_layout(n);
   const ApexLayout& pl = h->pl;
   const float* P = h->params;
   cudaStream_t s = h->stream;
   DRL_CUDA_CHECK(cudaMemcpyAsync(h->d_in, h->h_in, l.total, cudaMemcpyHostToDevice, s));
   const int32_t* pa = reinterpret_cast<const int32_t*>(h->d_in + l.pa);
-  int launches = 0;
-  DRL_TRY(apex_conv_forward(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3,
-                            kApexConvMode, false, nullptr, &launches));
+  DRL_TRY(policy_conv_forward_tf32(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3));
   ApexHeadArgs a;
   a.zpart = h->zpart;
   a.b1v = P + pl.value1_b; a.b1m = P + pl.mean1_b;
@@ -279,7 +236,7 @@ int enqueue_act(drl_apex_policy* h, int n) {
   a.n = n;
   a.A = h->A;
   const int grid = cdiv(n, kHR);
-  if (h->cfg.algo == 0) {
+  if (h->algo == 0) {
     DRL_TRY(launch_head1<0>(s, h->a3, h->table, pa, P + pl.value1_w, P + pl.mean1_w, h->zpart, n));
     DRL_CUDA_CHECK((launch_k(apex_policy_head_kernel<0>, grid, kApexHeadThreads, apex_head_smem<0>(), s, a)));
   } else {
@@ -291,43 +248,22 @@ int enqueue_act(drl_apex_policy* h, int n) {
 
 // checks common to both act entry points; on success the caller stages `sel` and calls run_act
 int check_act(drl_apex_policy* h, int algo, int32_t n, const uint8_t* state, const int32_t* previous_action) {
-  if (h->cfg.algo != algo) {
-    set_error("act: this policy is %s, use %s", h->cfg.algo ? "A3C" : "Ape-X",
-              h->cfg.algo ? "drl_a3c_policy_act" : "drl_apex_policy_act");
+  if (h->algo != algo) {
+    set_error("act: this policy is %s, use %s", h->algo ? "A3C" : "Ape-X",
+              h->algo ? "drl_a3c_policy_act" : "drl_apex_policy_act");
     return DRL_ERR_INVALID;
   }
-  if (n < 1 || n > h->cfg.max_batch) { set_error("act: n must be in [1, %d] (got %d)", h->cfg.max_batch, n); return DRL_ERR_INVALID; }
-  if (!state || !previous_action) { set_error("act: null input pointer"); return DRL_ERR_INVALID; }
-  for (int i = 0; i < n; ++i) {
-    if (previous_action[i] < 0 || previous_action[i] >= h->A) {
-      set_error("act: previous_action[%d] = %d is outside [0, %d)", i, previous_action[i], h->A);
-      return DRL_ERR_INVALID;
-    }
-  }
-  return DRL_OK;
+  DRL_TRY(policy_check_n(h, n, state && previous_action));
+  return policy_check_actions(h, n, previous_action, nullptr);
 }
 
 // stages frames and previous actions (the row selectors are already staged), runs the call, copies the outputs out
 int run_act(drl_apex_policy* h, int n, const uint8_t* state, const int32_t* previous_action, int32_t* action,
             float* out, float* out_action) {
-  DRL_CUDA_CHECK(cudaSetDevice(h->cfg.device));
   const ApexInLayout l = apex_in_layout(n);
   memcpy(h->h_in + l.frames, state, (size_t)n * Geo::FRAME);
   memcpy(h->h_in + l.pa, previous_action, (size_t)n * 4);
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_start, h->stream));
-  if (h->cfg.use_cuda_graph) {
-    if (!h->graphs[n]) {
-      // one eager pass first: the launchers set their kernel attributes outside capture
-      DRL_TRY(enqueue_act(h, n));
-      DRL_TRY(capture_graph(h->stream, [&] { return enqueue_act(h, n); }, &h->graphs[n]));
-    }
-    DRL_CUDA_CHECK(cudaGraphLaunch(h->graphs[n], h->stream));
-  } else {
-    DRL_TRY(enqueue_act(h, n));
-  }
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->stream));
-  DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
-  h->timed = true;
+  DRL_TRY(policy_run_act(h, n));
   if (out) memcpy(out, h->h_out, (size_t)n * h->A * 4);
   if (action) memcpy(action, h->h_out + h->off_act, (size_t)n * 4);
   if (out_action) memcpy(out_action, h->h_out + h->off_sel, (size_t)n * 4);
@@ -352,148 +288,61 @@ int drl_apex_policy_create(const drl_apex_policy_config* cfg, drl_apex_policy** 
   }
   if (cfg->num_action < 2 || cfg->num_action > kApexMaxA) { set_error("num_action must be in [2,32]"); return DRL_ERR_INVALID; }
   if (cfg->algo != 0 && cfg->algo != 1) { set_error("algo must be 0 (Ape-X) or 1 (A3C) (got %d)", cfg->algo); return DRL_ERR_INVALID; }
-  if (drl_device_count() <= cfg->device || cfg->device < 0) {
-    set_error("CUDA device %d not available (no CPU fallback)", cfg->device);
-    return DRL_ERR_CUDA;
-  }
-  ApexPolicyNvtx nv("drl:apex_policy_create");
+  DRL_TRY(policy_check_device(cfg->device));
+  NvtxRange nv("drl:apex_policy_create");
   drl_apex_policy* h = new drl_apex_policy();
-  h->cfg = *cfg;
+  h->device = cfg->device;
+  h->max_batch = cfg->max_batch;
   h->A = cfg->num_action;
+  h->use_cuda_graph = cfg->use_cuda_graph != 0;
+  h->algo = cfg->algo;
   h->pl.init(h->A);
-  const int MB = cfg->max_batch;
-  int rc = [&]() -> int {
-    DRL_CUDA_CHECK(cudaSetDevice(cfg->device));
-    DRL_TRY(set_apex_policy_kernel_attributes());
-    DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_ready, cudaEventDisableTiming));
-    DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_copied, cudaEventDisableTiming));
-    DRL_CUDA_CHECK(cudaEventCreate(&h->ev_start));
-    DRL_CUDA_CHECK(cudaEventCreate(&h->ev_stop));
-    DRL_TRY(dev_alloc(h, &h->params, (size_t)h->pl.padded_total));
-    size_t wb[WeightImages::kCount];
-    weight_image_sizes(wb);
-    DRL_TRY(dev_alloc(h, &h->img_conv2, wb[1]));
-    DRL_TRY(dev_alloc(h, &h->img_conv3, wb[2]));
-    DRL_TRY(dev_alloc(h, &h->e1, (size_t)h->A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &h->table, (size_t)h->A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &h->a1, (size_t)MB * 400 * 32));
-    DRL_TRY(dev_alloc(h, &h->a2, (size_t)MB * 81 * 64));
-    DRL_TRY(dev_alloc(h, &h->a3, (size_t)MB * Geo::FLAT));
-    DRL_TRY(dev_alloc(h, &h->zpart, (size_t)kApexSplits * MB * (cfg->algo == 0 ? ApexAlgo<0>::N : ApexAlgo<1>::N)));
-    const size_t in_bytes = apex_in_layout(MB).total;
-    DRL_TRY(dev_alloc(h, &h->d_in, in_bytes));
-    DRL_CUDA_CHECK(cudaHostAlloc((void**)&h->h_in, in_bytes, cudaHostAllocDefault));
-    memset(h->h_in, 0, in_bytes);
-    h->off_act = align_up((size_t)MB * kApexMaxA * 4, 256);
-    h->off_sel = h->off_act + align_up((size_t)MB * 4, 256);
-    const size_t out_bytes = h->off_sel + align_up((size_t)MB * 4, 256);
-    DRL_CUDA_CHECK(cudaHostAlloc((void**)&h->h_out, out_bytes, cudaHostAllocMapped));
-    memset(h->h_out, 0, out_bytes);
-    DRL_CUDA_CHECK(cudaHostGetDevicePointer((void**)&h->d_out, h->h_out, 0));
-    h->graphs.assign(MB + 1, nullptr);
-    DRL_TRY(refresh_derived(h));   // zero parameters until set_params / sync
-    DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
-    return DRL_OK;
-  }();
-  if (rc != DRL_OK) {
-    std::string keep = get_error();
-    drl_apex_policy_destroy(h);
-    set_error("%s", keep.c_str());
-    return rc;
-  }
+  h->layout = &h->pl;
+  h->enqueue_act = enqueue_act;
+  h->conv_images = policy_conv_images_tf32;
+  const size_t MB = cfg->max_batch;
+  h->off_act = align_up(MB * kApexMaxA * 4, 256);
+  h->off_sel = h->off_act + align_up(MB * 4, 256);
+  const size_t out_bytes = h->off_sel + align_up(MB * 4, 256);
+  const size_t N = cfg->algo == 0 ? ApexAlgo<0>::N : ApexAlgo<1>::N;
+  const int rc = policy_core_init(h, set_apex_policy_kernel_attributes, kApexSplits * MB * N, apex_in_layout(MB).total,
+                                  out_bytes);
+  if (rc != DRL_OK) { delete h; return rc; }
   *out = h;
   return DRL_OK;
 }
 
-int drl_apex_policy_destroy(drl_apex_policy* h) {
-  if (!h) return DRL_OK;
-  cudaSetDevice(h->cfg.device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  for (auto g : h->graphs) if (g) cudaGraphExecDestroy(g);
-  for (void* p : h->allocs) cudaFree(p);
-  if (h->h_in) cudaFreeHost(h->h_in);
-  if (h->h_out) cudaFreeHost(h->h_out);
-  for (cudaEvent_t e : {h->ev_ready, h->ev_copied, h->ev_start, h->ev_stop}) if (e) cudaEventDestroy(e);
-  if (h->stream) cudaStreamDestroy(h->stream);
-  cudaGetLastError();
-  delete h;
-  return DRL_OK;
-}
-
-int drl_apex_policy_param_count(const drl_apex_policy* h, int64_t* n) {
-  DRL_TRY(check_apex_policy(h));
-  if (!n) { set_error("null argument"); return DRL_ERR_INVALID; }
-  *n = h->pl.packed_total;
-  return DRL_OK;
-}
-
+int drl_apex_policy_destroy(drl_apex_policy* h) { return policy_destroy(h); }
+int drl_apex_policy_param_count(const drl_apex_policy* h, int64_t* n) { return policy_param_count(h, kName, n); }
 int drl_apex_policy_set_params(drl_apex_policy* h, const float* host_flat, int64_t n) {
-  DRL_TRY(check_apex_policy(h));
-  DRL_APEX_POLICY_LOCK(h);
-  if (!host_flat || n != h->pl.packed_total) {
-    set_error("set_params: expected %lld floats, got %lld", (long long)h->pl.packed_total, (long long)n);
-    return DRL_ERR_INVALID;
-  }
-  ApexPolicyNvtx nv("drl:apex_policy_set_params");
-  DRL_CUDA_CHECK(cudaSetDevice(h->cfg.device));
-  std::vector<float> flat((size_t)h->pl.padded_total);
-  DRL_TRY(upload_flat(h->stream, flat.data(), h->pl, h->params, host_flat, 0.0f));
-  DRL_TRY(refresh_derived(h));
-  DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
-  return DRL_OK;
+  return policy_set_params(h, kName, host_flat, n);
 }
-
 int drl_apex_policy_get_params(drl_apex_policy* h, float* host_flat, int64_t n) {
-  DRL_TRY(check_apex_policy(h));
-  DRL_APEX_POLICY_LOCK(h);
-  if (!host_flat || n != h->pl.packed_total) {
-    set_error("get_params: expected %lld floats, got %lld", (long long)h->pl.packed_total, (long long)n);
-    return DRL_ERR_INVALID;
-  }
-  ApexPolicyNvtx nv("drl:apex_policy_get_params");
-  DRL_CUDA_CHECK(cudaSetDevice(h->cfg.device));
-  std::vector<float> flat((size_t)h->pl.padded_total);
-  return download_flat(h->stream, flat.data(), h->pl, h->params, host_flat);
+  return policy_get_params(h, kName, host_flat, n);
 }
-
 int drl_apex_policy_sync_from_learner(drl_apex_policy* h, drl_apex* learner) {
-  DRL_TRY(check_apex_policy(h));
-  DRL_APEX_POLICY_LOCK(h);
-  if (!learner) { set_error("null learner handle"); return DRL_ERR_INVALID; }
-  ApexPolicyNvtx nv("drl:apex_policy_sync");
-  DRL_CUDA_CHECK(cudaSetDevice(h->cfg.device));
-  DRL_TRY(apex_params_snapshot(learner, h->cfg.device, h->cfg.algo, h->A, h->stream, h->params, h->ev_ready,
-                               h->ev_copied));
-  DRL_CUDA_CHECK(cudaSetDevice(h->cfg.device));
-  return refresh_derived(h);
+  return policy_sync(h, kName, learner, [&] {
+    return apex_params_snapshot(learner, h->device, h->algo, h->A, h->stream, h->params, h->ev_ready, h->ev_copied);
+  });
 }
+int drl_apex_policy_last_act_ms(drl_apex_policy* h, float* ms) { return policy_last_act_ms(h, kName, ms); }
 
 int drl_apex_policy_act(drl_apex_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action,
                         const int32_t* explore_action, int32_t* action, float* q, float* q_action) {
-  DRL_TRY(check_apex_policy(h));
-  DRL_APEX_POLICY_LOCK(h);
+  DRL_TRY(policy_check(h, kName));
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
   DRL_TRY(check_act(h, 0, n, state, previous_action));
-  if (explore_action) {
-    for (int i = 0; i < n; ++i) {
-      if (explore_action[i] < -1 || explore_action[i] >= h->A) {
-        set_error("act: explore_action[%d] = %d is outside [-1, %d)", i, explore_action[i], h->A);
-        return DRL_ERR_INVALID;
-      }
-    }
-  }
-  ApexPolicyNvtx nv("drl:apex_policy_act");
+  DRL_TRY(policy_check_actions(h, n, nullptr, explore_action));
+  NvtxRange nv("drl:apex_policy_act");
   // the previous call has completed (this entry point is synchronous): the staging block is free
-  uint8_t* sel = h->h_in + apex_in_layout(n).sel;
-  if (explore_action) memcpy(sel, explore_action, (size_t)n * 4);
-  else memset(sel, 0xff, (size_t)n * 4);      // -1: greedy
+  policy_stage_explore(h->h_in + apex_in_layout(n).sel, explore_action, n);
   return run_act(h, n, state, previous_action, action, q, q_action);
 }
 
 int drl_a3c_policy_act(drl_a3c_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action,
                        const double* uniform, int32_t* action, float* policy, float* prob_action) {
-  DRL_TRY(check_apex_policy(h));
-  DRL_APEX_POLICY_LOCK(h);
+  DRL_TRY(policy_check(h, kName));
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
   DRL_TRY(check_act(h, 1, n, state, previous_action));
   if (!uniform) { set_error("act: null input pointer (uniform: one draw in [0, 1) per row)"); return DRL_ERR_INVALID; }
   for (int i = 0; i < n; ++i) {
@@ -502,19 +351,9 @@ int drl_a3c_policy_act(drl_a3c_policy* h, int32_t n, const uint8_t* state, const
       return DRL_ERR_INVALID;
     }
   }
-  ApexPolicyNvtx nv("drl:a3c_policy_act");
+  NvtxRange nv("drl:a3c_policy_act");
   memcpy(h->h_in + apex_in_layout(n).sel, uniform, (size_t)n * 8);
   return run_act(h, n, state, previous_action, action, policy, prob_action);
-}
-
-int drl_apex_policy_last_act_ms(drl_apex_policy* h, float* ms) {
-  DRL_TRY(check_apex_policy(h));
-  DRL_APEX_POLICY_LOCK(h);
-  if (!ms) { set_error("null argument"); return DRL_ERR_INVALID; }
-  if (!h->timed) { set_error("last_act_ms: no act call has run yet"); return DRL_ERR_STATE; }
-  DRL_CUDA_CHECK(cudaSetDevice(h->cfg.device));
-  DRL_CUDA_CHECK(cudaEventElapsedTime(ms, h->ev_start, h->ev_stop));
-  return DRL_OK;
 }
 
 }  // extern "C"

@@ -1,9 +1,18 @@
 // kernels.h -- internal interface between the learner orchestration (learner.cu; adam_learner.cu with apex.cu and
 // r2d2.cu) and the kernel launchers (layers.cu, elementwise.cu, vtrace.cu, optimizer.cu).  Not part of the C-ABI.
 #pragma once
+#include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: no link dependency, a no-op unless a profiler injects itself
+
 #include "common.cuh"
 
 namespace drl {
+
+// an NVTX range over a host-side phase (the learners' step phases, the policy engines' calls); SURVEY.md section 5:
+// the reference has no tracing at all
+struct NvtxRange {
+  explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
+  ~NvtxRange() { nvtxRangePop(); }
+};
 
 // Offsets (in floats) of each tensor inside the padded flat parameter / gradient / slot vectors of one network.
 // Order = TF1 variable-creation order (SURVEY.md App. A.6); every bias directly follows its
@@ -26,10 +35,16 @@ struct FlatLayout {
   void set(int n, const int64_t* sizes, int64_t* const* named);
 };
 
-struct ParamLayout : FlatLayout {   // IMPALA network
+// The tensors every network here starts with, in this order: the attention_CNN (conv1, conv2, conv3) and the action
+// embedding (emb1, emb2).  The IMPALA, Ape-X / A3C and R2D2 layouts derive from it.
+struct TrunkLayout : FlatLayout {
   int A;
+  int C = Geo::IC;   // input channels (R2D2: 1 or 4)
   int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b;
   int64_t emb1_w, emb1_b, emb2_w, emb2_b;
+};
+
+struct ParamLayout : TrunkLayout {   // IMPALA network
   int64_t lstm_w, lstm_b;
   int64_t actor1_w, actor1_b, actor2_w, actor2_b, actor3_w, actor3_b;
   int64_t critic1_w, critic1_b, critic2_w, critic2_b, critic3_w, critic3_b;
@@ -187,11 +202,18 @@ size_t wgrad_partial_floats(int B, int T);
 size_t lstm_image_bytes(int which, int M, int Mb);
 int forward_launch_count();
 int backward_launch_count();
-// the policy engine's convolutions (policy.cu): the math-mode-5 conv1 / conv2 / conv3 forward of net_forward over n
-// single frames on one stream, and the build of its conv2 / conv3 weight images (WeightImages slots 1 and 2 sizes)
+// the IMPALA policy engine's convolutions (policy.cu): the math-mode-5 conv1 / conv2 / conv3 forward of net_forward over
+// n single frames on one stream, and the build of its conv2 / conv3 weight images (WeightImages slots 1 and 2 sizes)
 int conv_images16(cudaStream_t s, const ParamLayout& pl, const float* params, uint8_t* img_conv2, uint8_t* img_conv3);
 int conv_forward16(cudaStream_t s, const ParamLayout& pl, const float* params, const uint8_t* img_conv2,
                    const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3);
+// the Ape-X / A3C and R2D2 policy engines' convolutions (apex_policy.cu, r2d2_policy.cu; defined in r2d2.cu, whose
+// learner instantiates both channel counts): the math-mode-2 conv_forward_tf32 of layer_defs.cuh over n single frames
+// of pl.C channels, and conv_images_tf32
+int policy_conv_forward_tf32(cudaStream_t s, const TrunkLayout& pl, const float* params, const uint8_t* img_conv2,
+                             const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3);
+int policy_conv_images_tf32(cudaStream_t s, const TrunkLayout& pl, const float* params, uint8_t* img_conv2,
+                            uint8_t* img_conv3);
 
 // ---- learner.cu: parameter snapshot for the policy engine (drl_policy_sync_from_learner) ---------------------------
 // Under the learner's lock: records ev_ready on the learner's compute stream (after everything enqueued so far, a step

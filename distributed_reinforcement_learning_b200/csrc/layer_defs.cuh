@@ -153,6 +153,53 @@ static SplitPlan plan_conv3_wgrad(int Mb, int mode) {
   return mode >= 2 ? plan_split(Mb * 49, 5, 32, 2) : plan_split(Mb * 49, cdiv(576, CfgBig::BM), 16, 2);
 }
 
+// The conv1 / conv2 / conv3 forward of the Ape-X / A3C and R2D2 networks over B sequences of S frames of C channels
+// (rows m = t*B + b; S = 1: the caller's row order) on stream s, with the learner's kernels and configurations for math
+// mode `mode` (1: FP32 FFMA; 2: wgmma 3xTF32 with the conv2 / conv3 weight images of conv_images_tf32).  When
+// images_ready is not null, conv2 waits for it (the images are built on another stream).  `tgt` only names the launches
+// for the per-kernel profile; adds the launches to *launches.  Defined here so that each learner (apex.cu, r2d2.cu)
+// instantiates the kernels it launches; the policy engines reach it through policy_conv_forward_tf32 (r2d2.cu).
+template <int C>
+int conv_forward_tf32(cudaStream_t s, const TrunkLayout& pl, const float* P, const uint8_t* img_conv2,
+                      const uint8_t* img_conv3, const uint8_t* frames, int B, int S, float* a1, float* a2, float* a3,
+                      int mode, bool tgt, cudaEvent_t images_ready, int* launches) {
+  const int M = B * S;
+  const RowMap map{B, S};
+  int n = 0;
+  {
+    ConvFwdA<uint8_t, 84, 84, C, 20, 20, 8, 4, true> al{frames, map};
+    PlainB bl{P + pl.conv1_w, 32, 0};
+    EpConv1 ep{a1, 32, P + pl.conv1_b};
+    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 64 * C, 1, 64 * C, 0);
+  }
+  if (images_ready) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, images_ready, 0));
+  {
+    Conv2A al{a1, map};
+    PlainB bl{P + pl.conv2_w, 64, 0};
+    PretiledB<PlainB> blp{img_conv2, 512 / 32};
+    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
+    GEMM_W(tgt ? "target_conv2_fwd" : "conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
+  }
+  {
+    Conv3A al{a2, map};
+    PlainB bl{P + pl.conv3_w, 64, 0};
+    PretiledB<PlainB> blp{img_conv3, 576 / 32};
+    EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
+    GEMM_W(tgt ? "target_conv3_fwd" : "conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
+  }
+  *launches += n;
+  return DRL_OK;
+}
+
+// the conv2 / conv3 forward weight images of math mode 2 (WeightImages slots 1 and 2 sizes); a template like
+// conv_forward_tf32, so that only the translation units that call it instantiate its kernel
+template <class Layout>
+int conv_images_tf32(cudaStream_t s, const Layout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3) {
+  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, img_conv2)));
+  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, img_conv3)));
+  return DRL_OK;
+}
+
 // Fork/join helpers: kernels that are off the critical path (the action-embedding table in the forward, every
 // weight gradient except conv1's in the backward) run on the side stream so they fill SMs the critical
 // dgrad chain leaves idle.  Inside CUDA-graph capture the event record/wait pairs become graph edges.

@@ -10,19 +10,13 @@
 #include <string>
 #include <vector>
 
-#include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: no link dependency, a no-op unless a profiler injects itself
-
 #include "kernels.h"
 
 namespace drl {
 
-// NVTX ranges (SURVEY.md section 5: the reference has no tracing at all) around the host-side phases of a step:
-// stage (H2D enqueue), forward, vtrace_losses, backward, exchange, update.  Inside a CUDA-graph replay the phases are
-// one cudaGraphLaunch, so the ranges mark the capture / eager enqueue and the replay as a whole ("step(graph)").
-struct NvtxRange {
-  explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
-  ~NvtxRange() { nvtxRangePop(); }
-};
+// NVTX ranges (NvtxRange, kernels.h) around the host-side phases of a step: stage (H2D enqueue), forward,
+// vtrace_losses, backward, exchange, update.  Inside a CUDA-graph replay the phases are one cudaGraphLaunch, so the
+// ranges mark the capture / eager enqueue and the replay as a whole ("step(graph)").
 
 static thread_local char g_err[1024] = {0};
 void set_error(const char* fmt, ...) {

@@ -21,7 +21,7 @@
 
 namespace drl {
 
-// conv1 weight gradient over single-channel frames (Conv1A1: r2d2_defs.cuh)
+// conv1 weight gradient over single-channel frames
 using Conv1WA1 = ConvWgradA<uint8_t, 84, 84, 1, 20, 20, 8, 4, true>;
 
 // [x | h_in]^T for the LSTM kernel gradient: feature index i < 3392 -> [a3 | emb] (as LstmAT), else h_in (device, time-major)
@@ -353,46 +353,18 @@ __global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
 
 constexpr size_t kR2FwdSmem = 0, kR2BwdSmem = 0;     // the recurrence kernels only use small static shared arrays
 
-int r2_conv_forward(cudaStream_t s, const R2Layout& pl, const float* P, const uint8_t* img_conv2,
-                    const uint8_t* img_conv3, const uint8_t* frames, int B, int S, float* a1, float* a2, float* a3,
-                    int mode, bool tgt, cudaEvent_t images_ready, int* launches) {
-  const int M = B * S;
-  const RowMap map{B, S};
-  int n = 0;
-  if (pl.C == 1) {
-    Conv1A1 al{frames, map};
-    PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{a1, 32, P + pl.conv1_b};
-    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 64, 1, 64, 0);
-  } else {
-    Conv1A al{frames, map};
-    PlainB bl{P + pl.conv1_w, 32, 0};
-    EpConv1 ep{a1, 32, P + pl.conv1_b};
-    GEMM(tgt ? "target_conv1_fwd" : "conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
-  }
-  if (images_ready) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, images_ready, 0));
-  {
-    Conv2A al{a1, map};
-    PlainB bl{P + pl.conv2_w, 64, 0};
-    PretiledB<PlainB> blp{img_conv2, 512 / 32};
-    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv2_fwd" : "conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
-  }
-  {
-    Conv3A al{a2, map};
-    PlainB bl{P + pl.conv3_w, 64, 0};
-    PretiledB<PlainB> blp{img_conv3, 576 / 32};
-    EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    GEMM_W(tgt ? "target_conv3_fwd" : "conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
-  }
-  *launches += n;
-  return DRL_OK;
+int policy_conv_forward_tf32(cudaStream_t s, const TrunkLayout& pl, const float* P, const uint8_t* img_conv2,
+                             const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3) {
+  int launches = 0;
+  return pl.C == 1 ? conv_forward_tf32<1>(s, pl, P, img_conv2, img_conv3, frames, n, 1, a1, a2, a3, 2, false, nullptr,
+                                          &launches)
+                   : conv_forward_tf32<4>(s, pl, P, img_conv2, img_conv3, frames, n, 1, a1, a2, a3, 2, false, nullptr,
+                                          &launches);
 }
 
-int r2_conv_images(cudaStream_t s, const R2Layout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3) {
-  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, img_conv2)));
-  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, img_conv3)));
-  return DRL_OK;
+int policy_conv_images_tf32(cudaStream_t s, const TrunkLayout& pl, const float* P, uint8_t* img_conv2,
+                            uint8_t* img_conv3) {
+  return conv_images_tf32(s, pl, P, img_conv2, img_conv3);
 }
 
 // Forward of one scope over B sequences of S steps (rows m = t*B + b).  c_last (optional): un-masked c_t (act path).
@@ -408,8 +380,7 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
   s = side;
   if (retile_fwd && mode >= 2) {
     prof_mark(s, tgt ? "target_weight_retile" : "weight_retile");
-    DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, wi.img[1])));
-    DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, wi.img[2])));
+    DRL_TRY(conv_images_tf32(s, pl, P, wi.img[1], wi.img[2]));
     n += 2;
   }
   if (st.par) DRL_CUDA_CHECK(cudaEventRecord(st.ev[7], side));
@@ -422,8 +393,11 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
     n += 2;
   }
   s = st.main;
-  DRL_TRY(r2_conv_forward(s, pl, P, wi.img[1], wi.img[2], in.frames, B, S, act.a1, act.a2, act.a3, mode, tgt,
-                          st.par ? st.ev[7] : nullptr, &n));
+  const cudaEvent_t images_ready = st.par ? st.ev[7] : nullptr;
+  DRL_TRY(pl.C == 1 ? conv_forward_tf32<1>(s, pl, P, wi.img[1], wi.img[2], in.frames, B, S, act.a1, act.a2, act.a3,
+                                           mode, tgt, images_ready, &n)
+                    : conv_forward_tf32<4>(s, pl, P, wi.img[1], wi.img[2], in.frames, B, S, act.a1, act.a2, act.a3,
+                                           mode, tgt, images_ready, &n));
   DRL_TRY(join_from_side(st, 1));
   // input half of the LSTM contraction for all S steps at once: [M, 3392] x W[:3392, :4L] (split-K partial sums)
   const SplitPlan sp = plan_r2_x(M, mode);

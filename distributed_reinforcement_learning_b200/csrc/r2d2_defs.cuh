@@ -1,12 +1,11 @@
 // r2d2_defs.cuh -- definitions shared by the R2D2 learner (r2d2.cu), the R2D2 policy engine (r2d2_policy.cu) and the
-// R2D2 device replay memory (r2d2_replay.cu): the network's sizes, its flat parameter layout, the single-channel conv1
-// loader, the learner's conv forward, the learner handle and its forward + TD path.
+// R2D2 device replay memory (r2d2_replay.cu): the network's sizes, its flat parameter layout, the learner handle and its
+// forward + TD path.
 #pragma once
 #include <vector>
 
 #include "adam_learner.cuh"
 #include "kernels.h"
-#include "loaders.cuh"
 
 namespace drl {
 
@@ -15,9 +14,7 @@ constexpr int kR2G = 4 * kR2L;           // 256 gate columns
 constexpr int kR2H = 128;                // dense width between the LSTM and the two output streams (model/r2d2_lstm.py:50)
 constexpr int kR2Cat = Geo::FLAT + Geo::EMB;   // 3392 rows of the LSTM kernel that multiply the step input
 
-struct R2Layout : FlatLayout {
-  int A, C;
-  int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b, emb1_w, emb1_b, emb2_w, emb2_b;
+struct R2Layout : TrunkLayout {
   int64_t lstm_w, lstm_b, q1_w, q1_b, value_w, value_b, mean_w, mean_b;
   void init(int num_action, int channels) {
     A = num_action; C = channels;
@@ -31,19 +28,6 @@ struct R2Layout : FlatLayout {
     set(sizes, named);
   }
 };
-
-// conv1 over single-channel frames (config.json:91 model_input [84, 84, 1]); the 4-channel instantiations are layer_defs'
-using Conv1A1 = ConvFwdA<uint8_t, 84, 84, 1, 20, 20, 8, 4, true>;
-
-// conv1 / conv2 / conv3 forward of one scope over B sequences of S frames (rows m = t*B + b) on stream s, with the
-// learner's kernels and configurations for math mode `mode` (1: FP32 FFMA; 2: wgmma 3xTF32 with the conv2 / conv3
-// weight images of r2_conv_images).  When images_ready is not null, conv2 waits for it (the images are built on another
-// stream).  `tgt` only names the launches for the per-kernel profile; adds the launches to *launches.
-int r2_conv_forward(cudaStream_t s, const R2Layout& pl, const float* P, const uint8_t* img_conv2,
-                    const uint8_t* img_conv3, const uint8_t* frames, int B, int S, float* a1, float* a2, float* a3,
-                    int mode, bool tgt, cudaEvent_t images_ready, int* launches);
-// the conv2 / conv3 forward weight images of math mode 2 (WeightImages slots 1 and 2 sizes)
-int r2_conv_images(cudaStream_t s, const R2Layout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3);
 
 // drl_r2d2_policy_sync_from_learner: adam_params_snapshot of an R2D2 learner whose network has num_action actions and
 // `channels` input channels (DRL_ERR_INVALID otherwise)
