@@ -178,6 +178,16 @@ def _load():
         "drl_ring_pop_batch": (C.c_int, [vp, C.POINTER(RingBatch), i32]),
         "drl_ring_release": (C.c_int, [vp, i32]),
         "drl_ring_size": (C.c_int, [vp]),
+        "drl_traj_queue_create": (C.c_int, [i32] * 9 + [C.POINTER(vp)]),
+        "drl_traj_queue_destroy": (C.c_int, [vp]),
+        "drl_traj_queue_size": (C.c_int, [vp]),
+        "drl_traj_queue_read": (C.c_int, [vp, i32] + [vp] * 8),
+        "drl_policy_recorder_create": (C.c_int, [vp, vp, i32, C.POINTER(vp)]),
+        "drl_policy_recorder_destroy": (C.c_int, [vp]),
+        "drl_policy_recorder_act": (C.c_int, [vp] + [vp] * 9),
+        "drl_policy_recorder_commit": (C.c_int, [vp, vp, vp, i32]),
+        "drl_policy_recorder_reset": (C.c_int, [vp]),
+        "drl_learner_stage_from_queue": (C.c_int, [vp, i32, vp, i32]),
         "drl_apex_create": (C.c_int, [C.POINTER(ApexConfig), C.POINTER(vp)]),
         "drl_apex_destroy": (C.c_int, [vp]),
         "drl_apex_param_count": (C.c_int, [vp, C.POINTER(i64)]),

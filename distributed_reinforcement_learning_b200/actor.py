@@ -13,7 +13,10 @@ VectorActor: each environment is its own actor task ``i`` (what ``FLAGS.task`` s
     (SURVEY.md App. D);
   - a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True; the score keeps the raw reward;
   - at an episode's end the environment is reset, and previous action, h and c go back to 0;
-  - every environment's ``utils.UnrolledTrajectory`` goes to ``queue.append_to_queue(task=i, ...)``.
+  - every environment's ``utils.UnrolledTrajectory`` goes to ``queue.append_to_queue(task=i, ...)``; with a
+    ``DeviceFIFOQueue`` the acts go through a recorder of the policy instead (``NativePolicy.recorder``), which keeps
+    the trajectories on the GPU, and the unroll ends with one ``commit`` of the rewards and done flags of all N
+    environments, in environment order.
 """
 import numpy as np
 
@@ -43,6 +46,26 @@ class VectorActor:
         self.score = [0.0] * n
         self.episode_step = [0] * n
         self.total_max_prob = [0.0] * n
+        self.recorder = None
+        if isinstance(queue, buffer_queue.DeviceFIFOQueue):
+            self._check_device_queue(queue)
+            self.recorder = policy.recorder(queue, n)
+
+    def _check_device_queue(self, queue):
+        p = self.policy
+        if queue.trajectory != self.trajectory:
+            raise ValueError("queue records trajectories of %d steps, the actor unrolls %d"
+                             % (queue.trajectory, self.trajectory))
+        if queue.output_size != p.A:
+            raise ValueError("queue has num_action %d, the policy %d" % (queue.output_size, p.A))
+        if queue.lstm_size != p.L or tuple(queue.input_shape) != tuple(p.input_shape):
+            raise ValueError("queue stores %s frames and lstm %d, the policy takes %s and %d"
+                             % (tuple(queue.input_shape), queue.lstm_size, tuple(p.input_shape), p.L))
+        if queue.device != p.device:
+            raise ValueError("queue is on device %d, the policy on device %d" % (queue.device, p.device))
+        n = len(self.envs)
+        if n > queue.max_rows:
+            raise ValueError("%d environments per commit, the queue takes at most %d at once" % (n, queue.max_rows))
 
     def run_unroll(self):
         """One unroll of `trajectory` steps for every environment, pushed to the queue.  Returns the episodes that
@@ -51,12 +74,20 @@ class VectorActor:
         if self.learner is not None:
             self.learner.sync_policy(self.policy)
         n = len(self.envs)
-        trajs = [utils.UnrolledTrajectory() for _ in range(n)]
-        for t in trajs:
-            t.initialize()
+        rec = self.recorder
+        if rec is None:
+            trajs = [utils.UnrolledTrajectory() for _ in range(n)]
+            for t in trajs:
+                t.initialize()
+            act = self.policy.act
+        else:
+            rec.reset()   # an unroll that raised half-way left its steps behind: start this one at step 0
+            rewards = np.zeros((n, self.trajectory), np.float32)
+            dones = np.zeros((n, self.trajectory), np.bool_)
+            act = rec.act
         finished = []
-        for _ in range(self.trajectory):
-            out = self.policy.act(np.stack(self.states), self.previous_action, self.h, self.c)
+        for step in range(self.trajectory):
+            out = act(np.stack(self.states), self.previous_action, self.h, self.c)
             action, policy, max_prob = out["action"], out["policy"], out["max_prob"]
             # fresh copies: rows already stored in a trajectory, and the arrays act returned, are never written again
             next_pa, next_h, next_c = action.astype(np.int32), out["h"].copy(), out["c"].copy()
@@ -70,9 +101,12 @@ class VectorActor:
                     r, d = -1.0, True
                 else:
                     r, d = reward, False
-                trajs[i].append(state=self.states[i], next_state=next_state, reward=r, done=d, action=a,
-                                behavior_policy=policy[i], previous_action=int(self.previous_action[i]),
-                                initial_h=self.h[i], initial_c=self.c[i])
+                if rec is None:
+                    trajs[i].append(state=self.states[i], next_state=next_state, reward=r, done=d, action=a,
+                                    behavior_policy=policy[i], previous_action=int(self.previous_action[i]),
+                                    initial_h=self.h[i], initial_c=self.c[i])
+                else:   # the rest of the step is on the device already
+                    rewards[i, step], dones[i, step] = r, d
                 self.states[i] = next_state
                 self.lives[i] = info["ale.lives"]
                 if done:
@@ -87,6 +121,9 @@ class VectorActor:
                     next_h[i] = 0.0
                     next_c[i] = 0.0
             self.previous_action, self.h, self.c = next_pa, next_h, next_c
+        if rec is not None:
+            rec.commit(rewards, dones)
+            return finished
         for i, t in enumerate(trajs):
             u = t.extract()
             self.queue.append_to_queue(

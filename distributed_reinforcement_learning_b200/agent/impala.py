@@ -5,6 +5,7 @@ unchanged -- with the TF1 graph + ``tf.Session`` replaced by the CUDA learner be
   Agent.__init__            agent/impala.py:11-103   (graph construction -> records the config)
   Agent.set_session         agent/impala.py:114-116  (also initialises all variables, like the reference)
   Agent.train               agent/impala.py:132-148  -> stage + one fused device step
+  Agent.train_from_queue    (new) the same step on a batch of a DeviceFIFOQueue, staged device to device
   Agent.get_policy_and_action  agent/impala.py:118-130
   Agent.parameter_sync      agent/impala.py:111-112  (learner -> this agent's variables)
   Agent.sync_policy         (new) parameter_sync into a NativePolicy (policy.py), device to device from the learner
@@ -188,6 +189,31 @@ class Agent:
             slot = self._slot
             self._slot = (self._slot + 1) % eng.num_slots
             eng.stage(slot, state, reward, action, done, behavior_policy, previous_action, initial_h, initial_c)
+            out = eng.step(slot)
+            self._last = out
+            return out["pi_loss"], out["baseline_loss"], out["entropy"], out["learning_rate"]
+
+    def train_from_queue(self, queue, timeout_ms=-1):
+        """``train`` on the oldest batch of a ``DeviceFIFOQueue`` (the actors' recorders fill it on the GPU): the
+        batch is staged device to device, then the same step runs.  Blocks until the queue holds a batch
+        (``timeout_ms`` >= 0 raises ``TimeoutError_`` with nothing changed).  -> (pi_loss, value_loss, entropy,
+        learning_rate), as ``train``.  One learner thread calls it; do not interleave it with ``train`` from another
+        thread (with two staging slots, a ``train`` that runs while this call waits for a batch can reuse its slot)."""
+        with self._lock:
+            if NativeLearner._distributed():
+                raise RuntimeError("train_from_queue is single-replica: the queue lives on one device")
+            eng = self._get_engine(queue.batch_size)
+            slot = self._slot
+            self._slot = (slot + 1) % eng.num_slots    # taken now, so a train() meanwhile picks the other slot
+        # wait for the batch without the agent's lock: actor threads sync their policies from this agent meanwhile
+        try:
+            eng.stage_from_queue(slot, queue, timeout_ms)
+        except Exception:
+            with self._lock:
+                if self._slot == (slot + 1) % eng.num_slots:
+                    self._slot = slot                  # nothing was staged: the slot is not used up
+            raise
+        with self._lock:
             out = eng.step(slot)
             self._last = out
             return out["pi_loss"], out["baseline_loss"], out["entropy"], out["learning_rate"]

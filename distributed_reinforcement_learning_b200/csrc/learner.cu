@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "kernels.h"
+#include "traj_queue.cuh"
 
 namespace drl {
 
@@ -666,6 +667,52 @@ int drl_learner_stage(drl_learner* h, int32_t slot, const uint8_t* state, const 
   DRL_CUDA_CHECK(cudaEventRecord(s.staged, h->copy));
   s.has_data = true;
   return DRL_OK;
+}
+
+int drl_learner_stage_from_queue(drl_learner* h, int32_t slot, drl_traj_queue* q, int32_t timeout_ms) {
+  DRL_TRY(check_handle(h));
+  if (!q) { set_error("null trajectory queue handle"); return DRL_ERR_INVALID; }
+  {
+    DRL_LOCK(h);
+    if (slot < 0 || slot >= (int)h->slots.size()) { set_error("slot %d out of range", slot); return DRL_ERR_INVALID; }
+    if (q->device != h->cfg.device) {
+      set_error("stage_from_queue: the queue is on device %d, the learner on device %d", q->device, h->cfg.device);
+      return DRL_ERR_INVALID;
+    }
+    if (q->batch != h->B || q->T != h->T || q->A != h->A) {
+      set_error("stage_from_queue: the queue has batch %d, trajectory %d, num_action %d; the learner %d, %d, %d",
+                q->batch, q->T, q->A, h->B, h->T, h->A);
+      return DRL_ERR_INVALID;
+    }
+    if (q->H != Geo::IH || q->W != Geo::IW || q->C != Geo::IC || q->L != Geo::L) {
+      set_error("stage_from_queue: the queue stores %dx%dx%d frames and lstm %d, the learner takes %dx%dx%d and %d",
+                q->H, q->W, q->C, q->L, Geo::IH, Geo::IW, Geo::IC, Geo::L);
+      return DRL_ERR_INVALID;
+    }
+  }
+  // wait for a full batch without the learner's lock: actor threads sync their engines from this learner meanwhile
+  int qs = 0;
+  std::vector<cudaEvent_t> ev_commit;
+  DRL_TRY(traj_queue_pop(q, timeout_ms, &qs, &ev_commit));
+  DRL_LOCK(h);
+  NvtxRange nvtx_r("drl:stage_from_queue");
+  Slot& s = h->slots[slot];
+  const int rc = [&]() -> int {
+    DRL_TRY(set_device(h));
+    // do not overwrite a slot the compute stream is still reading; do not read rows whose commit copies are pending
+    DRL_CUDA_CHECK(cudaStreamWaitEvent(h->copy, s.consumed, 0));
+    for (cudaEvent_t e : ev_commit) DRL_CUDA_CHECK(cudaStreamWaitEvent(h->copy, e, 0));
+    const void* dst[kTrajFields] = {s.in.frames, s.in.reward, s.in.done, s.in.mu, s.in.action, s.in.pa, s.in.h0, s.in.c0};
+    for (int f = 0; f < kTrajFields; ++f)
+      DRL_CUDA_CHECK(cudaMemcpyAsync(const_cast<void*>(dst[f]), q->field(qs, f), (size_t)q->batch * q->sz[f],
+                                     cudaMemcpyDeviceToDevice, h->copy));
+    DRL_CUDA_CHECK(cudaEventRecord(s.staged, h->copy));
+    s.has_data = true;
+    return DRL_OK;
+  }();
+  // the queue slot goes back to the producers either way (their copies into it wait for its release event)
+  const int rc_release = traj_queue_release(q, qs, h->copy);
+  return rc != DRL_OK ? rc : rc_release;
 }
 
 int drl_learner_forward_backward(drl_learner* h, int32_t slot) {

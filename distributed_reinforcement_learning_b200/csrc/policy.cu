@@ -10,11 +10,18 @@
 //   policy_head_fused       split-K sum + bias + gates (c1, h1), actor dense 256 / 256 / A, softmax, sampling; writes
 //                           policy, h1, c1 and action straight into mapped pinned memory (no D2H node)
 // Both new kernels sum in a fixed order without atomics: eager and graph replays, and repeated calls, are bitwise equal.
+//
+// A recorder (drl_policy_recorder_*, DESIGN.md section 12) binds the engine to a device trajectory queue
+// (traj_queue.cuh).  Its act is the engine's act with policy_head_record in place of policy_head_fused (the same head
+// that also writes policy and action into the recorder's staging) plus policy_record_step (frames, previous action,
+// h0, c0 of the device input block into the staging); the step t reaches both through a device word staged per call,
+// so one graph per recorder replays every step.
 #include <string.h>
 
 #include "policy_core.cuh"
 #include "policy_head.cuh"
 #include "policy_lstm.cuh"
+#include "traj_queue.cuh"
 
 namespace drl {
 namespace {
@@ -50,6 +57,14 @@ struct HeadArgs {
   float* c1;               // [n][256]
   int32_t* action;         // [n]
   int n, A;
+};
+
+// what the recording head writes besides HeadArgs' outputs: policy and action of step *t of rows 0..n-1
+struct HeadRecord {
+  const int32_t* t;        // device word, staged per call
+  float* mu;               // [n][T][A]
+  int32_t* action;         // [n][T]
+  int T;
 };
 
 __global__ void __launch_bounds__(kHThreads, 1) policy_head_fused_kernel(const HeadArgs a) {
@@ -125,6 +140,118 @@ __global__ void __launch_bounds__(kHThreads, 1) policy_head_fused_kernel(const H
   if (lane == 0) a.action[m] = sample_choice(sp, A, a.uniform, m);
 }
 
+// The recording head: policy_head_fused_kernel, plus each row's policy and sampled action written into a recorder's
+// staging at step *rec.t.  A separate copy rather than a template flag or a shared device function: both of those
+// changed the code nvcc generates for policy_head_fused_kernel itself, which the plain act path keeps as it was.
+__global__ void __launch_bounds__(kHThreads, 1) policy_head_record_kernel(const HeadArgs a, const HeadRecord rec) {
+  kernel_prologue();
+  extern __shared__ __align__(16) float hs[];
+  float* sh = hs;                    // h1, later hid2
+  float* shid = sh + kHR * 256;      // hid1
+  float* part = shid + kHR * 256;
+  float* sw3 = part + 4 * kHR * 256;
+  const int tid = threadIdx.x, row0 = blockIdx.x * kHR;
+  const int nr = min(kHR, a.n - row0), A = a.A;
+  // the output layer's weights first: their loads overlap the gate math
+  for (int i = tid; i < Geo::HID * A / 4; i += kHThreads)
+    reinterpret_cast<float4*>(sw3)[i] = ldg4(a.w3 + 4 * i);
+  // LSTM cell (TF1 LSTMCell, gate order i, j, f, o, forget bias 1.0): the split partials in fixed order + bias
+  {
+    const int u = tid;
+    float bz[4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) bz[g] = __ldg(a.lstm_b + g * Geo::L + u);
+    for (int r = 0; r < kHR; ++r) {
+      float hv = 0.f;
+      if (r < nr) {
+        const int m = row0 + r;
+        float z[4];
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          float acc = 0.f;
+#pragma unroll
+          for (int s = 0; s < kLSplits; ++s) acc += a.zpart[((size_t)s * a.n + m) * Geo::G4 + g * Geo::L + u];
+          z[g] = acc + bz[g];
+        }
+        const float si = sigmoidf_acc(z[0]);
+        const float tj = tanhf(z[1]);
+        const float sf = sigmoidf_acc(z[2] + 1.0f);
+        const float so = sigmoidf_acc(z[3]);
+        const float cv = sf * a.c0[(size_t)m * Geo::L + u] + si * tj;
+        hv = so * tanhf(cv);
+        a.c1[(size_t)m * Geo::L + u] = cv;
+        a.h1[(size_t)m * Geo::L + u] = hv;
+      }
+      sh[r * 256 + u] = hv;
+    }
+  }
+  __syncthreads();
+  dense256_relu(sh, a.w1, a.b1, part, shid, tid);    // hid1
+  dense256_relu(shid, a.w2, a.b2, part, sh, tid);    // hid2 (over h1, no longer needed)
+  const int warp = tid >> 5, lane = tid & 31;
+  if (warp >= nr) return;
+  const int m = row0 + warp;
+  const float* x = sh + warp * 256;
+  float logit = -INFINITY;
+  if (lane < A) {
+    float c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f;
+#pragma unroll 4
+    for (int k = 0; k < Geo::HID; k += 4) {
+      c0 = fmaf(x[k], sw3[k * A + lane], c0);
+      c1 = fmaf(x[k + 1], sw3[(k + 1) * A + lane], c1);
+      c2 = fmaf(x[k + 2], sw3[(k + 2) * A + lane], c2);
+      c3 = fmaf(x[k + 3], sw3[(k + 3) * A + lane], c3);
+    }
+    logit = ((c0 + c1) + (c2 + c3)) + __ldg(a.b3 + lane);
+  }
+  const float mx = warp_max(logit);
+  const float e = (lane < A) ? expf(logit - mx) : 0.f;
+  const float sum = warp_sum(e);
+  const float p = e / sum;
+  if (lane < A) a.policy[(size_t)m * A + lane] = p;
+  // sampling: numpy's RandomState.choice(A, p=policy) for the row's uniform draw (policy_head.cuh)
+  float* sp = part + warp * 32;      // the K partials are dead after the second dense layer
+  sp[lane] = p;
+  __syncwarp();
+  const size_t rec_row = (size_t)m * rec.T + *rec.t;
+  if (lane < A) rec.mu[rec_row * A + lane] = p;
+  if (lane == 0) a.action[m] = rec.action[rec_row] = sample_choice(sp, A, a.uniform, m);
+}
+
+// ---- policy_record_step -----------------------------------------------------------------------------------------
+// One CTA per row: the frame, previous action, h0 and c0 the act read from the device input block, into step *t of
+// the row's trajectory in the recorder's staging.  16-byte copies (frame 28,224 B, h0 / c0 1 KB each).
+struct RecordArgs {
+  const uint8_t* frames;   // device input block: [n][FRAME]
+  const int32_t* pa;       // [n]
+  const float* h0;         // [n][256]
+  const float* c0;         // [n][256]
+  const int32_t* t;        // device word, staged per call
+  uint8_t* rec_frames;     // staging [n][T][FRAME]
+  int32_t* rec_pa;         // [n][T]
+  float* rec_h0;           // [n][T][256]
+  float* rec_c0;           // [n][T][256]
+  int T;
+};
+constexpr int kRecThreads = 256;
+
+__global__ void __launch_bounds__(kRecThreads) policy_record_step_kernel(const RecordArgs a) {
+  kernel_prologue();
+  const int row = blockIdx.x, tid = threadIdx.x;
+  const size_t dst = (size_t)row * a.T + *a.t;
+  const uint4* f = reinterpret_cast<const uint4*>(a.frames + (size_t)row * Geo::FRAME);
+  uint4* fd = reinterpret_cast<uint4*>(a.rec_frames + dst * Geo::FRAME);
+  for (int i = tid; i < Geo::FRAME / 16; i += kRecThreads) fd[i] = f[i];
+  if (tid < Geo::L / 4) {
+    reinterpret_cast<float4*>(a.rec_h0 + dst * Geo::L)[tid] = reinterpret_cast<const float4*>(a.h0 + (size_t)row * Geo::L)[tid];
+  } else if (tid < Geo::L / 2) {
+    const int i = tid - Geo::L / 4;
+    reinterpret_cast<float4*>(a.rec_c0 + dst * Geo::L)[i] = reinterpret_cast<const float4*>(a.c0 + (size_t)row * Geo::L)[i];
+  } else if (tid == Geo::L / 2) {
+    a.rec_pa[dst] = a.pa[row];
+  }
+}
+
 // ---- handle -----------------------------------------------------------------------------------------------------
 // device input block of one call with n rows, one contiguous H2D: [frames | previous_action | h0 | c0 | uniform]
 struct InLayout {
@@ -146,6 +273,8 @@ int set_policy_kernel_attributes() {
   DRL_TRY((set_policy_lstm_attributes<Geo::L, kLSplits>()));
   DRL_CUDA_CHECK(cudaFuncSetAttribute(policy_head_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)kHeadSmem));
+  DRL_CUDA_CHECK(cudaFuncSetAttribute(policy_head_record_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)kHeadSmem));
   return DRL_OK;
 }
 
@@ -160,10 +289,25 @@ struct drl_policy : PolicyCore {
   size_t off_h = 0, off_c = 0, off_act = 0;
 };
 
+struct drl_policy_recorder {
+  drl_policy* engine = nullptr;
+  drl_traj_queue* q = nullptr;
+  int n = 0, T = 0;
+  int t = 0;                          // steps recorded since the last commit
+  uint8_t* staging = nullptr;         // [n] trajectories, field-major in the queue's field order
+  size_t off[kTrajFields] = {};
+  int32_t* d_t = nullptr;             // the step, read by the recording kernels
+  int32_t* h_t = nullptr;             // its pinned staging
+  uint8_t* h_rd = nullptr;            // pinned reward [n][T] f32 | done [n][T] u8 of a commit
+  cudaGraphExec_t graph = nullptr;
+  std::vector<void*> allocs;
+  uint8_t* field(int f) { return staging + off[f]; }
+};
+
 namespace {
 
-int enqueue_act(PolicyCore* c, int n) {
-  drl_policy* h = static_cast<drl_policy*>(c);
+// the engine's act of n rows; with a recorder, the recording head and policy_record_step as well
+int enqueue_act_impl(drl_policy* h, int n, drl_policy_recorder* rec) {
   const InLayout l = in_layout(n);
   const ParamLayout& pl = h->pl;
   const float* P = h->params;
@@ -187,8 +331,70 @@ int enqueue_act(PolicyCore* c, int n) {
   a.action = reinterpret_cast<int32_t*>(h->d_out + h->off_act);
   a.n = n;
   a.A = h->A;
-  DRL_CUDA_CHECK((launch_k(policy_head_fused_kernel, cdiv(n, kHR), kHThreads, kHeadSmem, s, a)));
+  if (!rec) {
+    DRL_CUDA_CHECK((launch_k(policy_head_fused_kernel, cdiv(n, kHR), kHThreads, kHeadSmem, s, a)));
+    return DRL_OK;
+  }
+  HeadRecord hr;
+  hr.t = rec->d_t;
+  hr.mu = reinterpret_cast<float*>(rec->field(kTrajMu));
+  hr.action = reinterpret_cast<int32_t*>(rec->field(kTrajAction));
+  hr.T = rec->T;
+  DRL_CUDA_CHECK((launch_k(policy_head_record_kernel, cdiv(n, kHR), kHThreads, kHeadSmem, s, a, hr)));
+  RecordArgs r;
+  r.frames = h->d_in + l.frames;
+  r.pa = pa;
+  r.h0 = h0;
+  r.c0 = a.c0;
+  r.t = rec->d_t;
+  r.rec_frames = rec->field(kTrajState);
+  r.rec_pa = reinterpret_cast<int32_t*>(rec->field(kTrajPa));
+  r.rec_h0 = reinterpret_cast<float*>(rec->field(kTrajH));
+  r.rec_c0 = reinterpret_cast<float*>(rec->field(kTrajC));
+  r.T = rec->T;
+  DRL_CUDA_CHECK((launch_k(policy_record_step_kernel, n, kRecThreads, 0, s, r)));
   return DRL_OK;
+}
+
+int enqueue_act(PolicyCore* c, int n) { return enqueue_act_impl(static_cast<drl_policy*>(c), n, nullptr); }
+
+// the recorder's act: the step word, then the recording act of its n rows
+int enqueue_record(drl_policy_recorder* r) {
+  DRL_CUDA_CHECK(cudaMemcpyAsync(r->d_t, r->h_t, sizeof(int32_t), cudaMemcpyHostToDevice, r->engine->stream));
+  return enqueue_act_impl(r->engine, r->n, r);
+}
+
+// act's argument checks and the staging of its inputs into h_in (the caller holds the engine's lock)
+int stage_act(drl_policy* h, int n, const uint8_t* state, const int32_t* previous_action, const float* h_in,
+              const float* c_in, const double* uniform, const int32_t* action) {
+  DRL_TRY(policy_check_n(h, n, state && previous_action && h_in && c_in));
+  if (action && !uniform) { set_error("act: `action` needs `uniform` (one draw in [0, 1) per row)"); return DRL_ERR_INVALID; }
+  DRL_TRY(policy_check_actions(h, n, previous_action, nullptr));
+  // the previous call has completed (this entry point is synchronous): the staging block is free
+  const InLayout l = in_layout(n);
+  memcpy(h->h_in + l.frames, state, (size_t)n * Geo::FRAME);
+  memcpy(h->h_in + l.pa, previous_action, (size_t)n * 4);
+  memcpy(h->h_in + l.h0, h_in, (size_t)n * Geo::L * 4);
+  memcpy(h->h_in + l.c0, c_in, (size_t)n * Geo::L * 4);
+  if (uniform) memcpy(h->h_in + l.u, uniform, (size_t)n * 8);
+  else memset(h->h_in + l.u, 0, (size_t)n * 8);
+  return DRL_OK;
+}
+
+void copy_act_outputs(const drl_policy* h, int n, int32_t* action, float* policy, float* h_out, float* c_out) {
+  if (policy) memcpy(policy, h->h_out, (size_t)n * h->A * 4);
+  if (h_out) memcpy(h_out, h->h_out + h->off_h, (size_t)n * Geo::L * 4);
+  if (c_out) memcpy(c_out, h->h_out + h->off_c, (size_t)n * Geo::L * 4);
+  if (action) memcpy(action, h->h_out + h->off_act, (size_t)n * 4);
+}
+
+void recorder_release(drl_policy_recorder* r) {
+  if (r->engine && r->engine->stream) cudaStreamSynchronize(r->engine->stream);
+  if (r->graph) cudaGraphExecDestroy(r->graph);
+  for (void* p : r->allocs) cudaFree(p);
+  if (r->h_t) cudaFreeHost(r->h_t);
+  if (r->h_rd) cudaFreeHost(r->h_rd);
+  cudaGetLastError();
 }
 
 }  // namespace
@@ -254,23 +460,165 @@ int drl_policy_act(drl_policy* h, int32_t n, const uint8_t* state, const int32_t
                    float* c_out) {
   DRL_TRY(policy_check(h, kName));
   std::lock_guard<std::recursive_mutex> lk(h->mu);
-  DRL_TRY(policy_check_n(h, n, state && previous_action && h_in && c_in));
-  if (action && !uniform) { set_error("act: `action` needs `uniform` (one draw in [0, 1) per row)"); return DRL_ERR_INVALID; }
-  DRL_TRY(policy_check_actions(h, n, previous_action, nullptr));
+  DRL_TRY(stage_act(h, n, state, previous_action, h_in, c_in, uniform, action));
   NvtxRange nv("drl:policy_act");
-  // the previous call has completed (this entry point is synchronous): the staging block is free
-  const InLayout l = in_layout(n);
-  memcpy(h->h_in + l.frames, state, (size_t)n * Geo::FRAME);
-  memcpy(h->h_in + l.pa, previous_action, (size_t)n * 4);
-  memcpy(h->h_in + l.h0, h_in, (size_t)n * Geo::L * 4);
-  memcpy(h->h_in + l.c0, c_in, (size_t)n * Geo::L * 4);
-  if (uniform) memcpy(h->h_in + l.u, uniform, (size_t)n * 8);
-  else memset(h->h_in + l.u, 0, (size_t)n * 8);
   DRL_TRY(policy_run_act(h, n));
-  if (policy) memcpy(policy, h->h_out, (size_t)n * h->A * 4);
-  if (h_out) memcpy(h_out, h->h_out + h->off_h, (size_t)n * Geo::L * 4);
-  if (c_out) memcpy(c_out, h->h_out + h->off_c, (size_t)n * Geo::L * 4);
-  if (action) memcpy(action, h->h_out + h->off_act, (size_t)n * 4);
+  copy_act_outputs(h, n, action, policy, h_out, c_out);
+  return DRL_OK;
+}
+
+// ---- recorder ---------------------------------------------------------------------------------------------------
+int drl_policy_recorder_create(drl_policy* h, drl_traj_queue* q, int32_t n, drl_policy_recorder** out) {
+  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
+  *out = nullptr;
+  if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
+  DRL_TRY(policy_check(h, kName));
+  if (!q) { set_error("null trajectory queue handle"); return DRL_ERR_INVALID; }
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  if (n < 1 || n > h->max_batch) {
+    set_error("recorder: n must be in [1, %d] (the engine's max_batch; got %d)", h->max_batch, n);
+    return DRL_ERR_INVALID;
+  }
+  if (q->device != h->device) {
+    set_error("recorder: the queue is on device %d, the policy on device %d", q->device, h->device);
+    return DRL_ERR_INVALID;
+  }
+  if (q->A != h->A) { set_error("recorder: the queue has num_action %d, the policy %d", q->A, h->A); return DRL_ERR_INVALID; }
+  if (q->H != Geo::IH || q->W != Geo::IW || q->C != Geo::IC || q->L != Geo::L) {
+    set_error("recorder: the queue stores %dx%dx%d frames and lstm %d, the policy takes %dx%dx%d and %d", q->H, q->W,
+              q->C, q->L, Geo::IH, Geo::IW, Geo::IC, Geo::L);
+    return DRL_ERR_INVALID;
+  }
+  if (n > traj_queue_max_rows(q)) {
+    set_error("recorder: %d rows per commit can never fit in the queue (at most %d)", n, traj_queue_max_rows(q));
+    return DRL_ERR_INVALID;
+  }
+  NvtxRange nv("drl:policy_recorder_create");
+  drl_policy_recorder* r = new drl_policy_recorder();
+  r->engine = h;
+  r->q = q;
+  r->n = n;
+  r->T = q->T;
+  const int rc = [&]() -> int {
+    DRL_CUDA_CHECK(cudaSetDevice(h->device));
+    size_t off = 0;
+    for (int f = 0; f < kTrajFields; ++f) {
+      r->off[f] = off;
+      off = align_up(off + (size_t)n * q->sz[f], 256);
+    }
+    DRL_TRY(dev_alloc(r, &r->staging, off));
+    DRL_TRY(dev_alloc(r, &r->d_t, 1));
+    DRL_CUDA_CHECK(cudaHostAlloc((void**)&r->h_t, sizeof(int32_t), cudaHostAllocDefault));
+    *r->h_t = 0;
+    DRL_CUDA_CHECK(cudaHostAlloc((void**)&r->h_rd, (size_t)n * r->T * 5, cudaHostAllocDefault));
+    return DRL_OK;
+  }();
+  if (rc != DRL_OK) {
+    const std::string keep = get_error();
+    recorder_release(r);
+    delete r;
+    set_error("%s", keep.c_str());
+    return rc;
+  }
+  *out = r;
+  return DRL_OK;
+}
+
+int drl_policy_recorder_destroy(drl_policy_recorder* r) {
+  if (!r) return DRL_OK;
+  {
+    std::lock_guard<std::recursive_mutex> lk(r->engine->mu);
+    cudaSetDevice(r->engine->device);
+    recorder_release(r);
+  }
+  delete r;
+  return DRL_OK;
+}
+
+int drl_policy_recorder_act(drl_policy_recorder* r, const uint8_t* state, const int32_t* previous_action,
+                            const float* h_in, const float* c_in, const double* uniform, int32_t* action,
+                            float* policy, float* h_out, float* c_out) {
+  if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
+  drl_policy* h = r->engine;
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  if (r->t >= r->T) {
+    set_error("recorder act: all %d steps of the unroll are recorded (commit them first)", r->T);
+    return DRL_ERR_STATE;
+  }
+  if (!uniform) { set_error("recorder act: `uniform` is required (the recorded actions are the sampled ones)"); return DRL_ERR_INVALID; }
+  DRL_TRY(stage_act(h, r->n, state, previous_action, h_in, c_in, uniform, action));
+  NvtxRange nv("drl:policy_recorder_act");
+  *r->h_t = r->t;
+  DRL_CUDA_CHECK(cudaSetDevice(h->device));
+  DRL_CUDA_CHECK(cudaEventRecord(h->ev_start, h->stream));
+  if (h->use_cuda_graph) {
+    if (!r->graph) {
+      DRL_TRY(enqueue_record(r));   // eager pass first: attributes and tensor maps outside capture (idempotent)
+      DRL_TRY(capture_graph(h->stream, [&] { return enqueue_record(r); }, &r->graph));
+    }
+    DRL_CUDA_CHECK(cudaGraphLaunch(r->graph, h->stream));
+  } else {
+    DRL_TRY(enqueue_record(r));
+  }
+  DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->stream));
+  DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
+  h->timed = true;
+  copy_act_outputs(h, r->n, action, policy, h_out, c_out);
+  r->t++;
+  return DRL_OK;
+}
+
+int drl_policy_recorder_commit(drl_policy_recorder* r, const float* reward, const uint8_t* done, int32_t timeout_ms) {
+  if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
+  if (!reward || !done) { set_error("recorder commit: null argument"); return DRL_ERR_INVALID; }
+  drl_policy* h = r->engine;
+  {
+    std::lock_guard<std::recursive_mutex> lk(h->mu);
+    if (r->t != r->T) {
+      set_error("recorder commit: %d of %d steps recorded (commit follows step T-1)", r->t, r->T);
+      return DRL_ERR_STATE;
+    }
+  }
+  // reserve without the engine's lock: a learner thread may sync this engine while the commit waits for space
+  std::vector<TrajSegment> segs;
+  DRL_TRY(traj_queue_reserve(r->q, r->n, timeout_ms, &segs));
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  NvtxRange nv("drl:policy_recorder_commit");
+  drl_traj_queue* q = r->q;
+  cudaStream_t s = h->stream;
+  const size_t nT = (size_t)r->n * r->T;
+  const int rc = [&]() -> int {
+    // h_rd is free: every act since the previous commit waited for the stream
+    memcpy(r->h_rd, reward, nT * 4);
+    memcpy(r->h_rd + nT * 4, done, nT);
+    DRL_CUDA_CHECK(cudaSetDevice(h->device));
+    DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(kTrajReward), r->h_rd, nT * 4, cudaMemcpyHostToDevice, s));
+    DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(kTrajDone), r->h_rd + nT * 4, nT, cudaMemcpyHostToDevice, s));
+    for (const TrajSegment& g : segs) {
+      DRL_CUDA_CHECK(cudaStreamWaitEvent(s, g.ev_release, 0));
+      for (int f = 0; f < kTrajFields; ++f)
+        DRL_CUDA_CHECK(cudaMemcpyAsync(q->field(g.slot, f) + (size_t)g.row0 * q->sz[f],
+                                       r->field(f) + (size_t)g.src0 * q->sz[f], (size_t)g.rows * q->sz[f],
+                                       cudaMemcpyDeviceToDevice, s));
+      DRL_CUDA_CHECK(cudaEventRecord(g.ev_commit, s));
+    }
+    return DRL_OK;
+  }();
+  if (rc != DRL_OK) {
+    // the reserved positions will never be filled: rather than leave every producer and the learner waiting behind
+    // them, the queue goes into its failed state (every later reserve / pop / read returns DRL_ERR_STATE)
+    traj_queue_fail(q, get_error());
+    return rc;
+  }
+  traj_queue_commit(q, segs);
+  r->t = 0;
+  return DRL_OK;
+}
+
+int drl_policy_recorder_reset(drl_policy_recorder* r) {
+  if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
+  std::lock_guard<std::recursive_mutex> lk(r->engine->mu);
+  r->t = 0;
   return DRL_OK;
 }
 

@@ -1,0 +1,250 @@
+// traj_queue.cu -- the device-resident IMPALA trajectory queue behind drl_traj_queue_* (include/drl_b200.h; layout
+// and ordering in traj_queue.cuh).  Producers are policy-engine recorders (policy.cu), the consumer is
+// drl_learner_stage_from_queue (learner.cu); no trajectory byte crosses PCIe except the reward and done of a commit.
+#include <string.h>
+
+#include <algorithm>
+#include <chrono>
+#include <string>
+
+#include "traj_queue.cuh"
+
+using namespace drl;
+
+namespace drl {
+
+namespace {
+
+size_t tq_align(size_t v) { return (v + 255) / 256 * 256; }
+
+// every slot the n positions from reserved_total fall in is free for them (held slots and slots still holding an
+// unpopped batch are not)
+bool has_space(const drl_traj_queue* q, int n) {
+  long long p = q->reserved_total;
+  const long long end = p + n;
+  while (p < end) {
+    const int slot = (int)((p / q->batch) % q->nslots), row0 = (int)(p % q->batch);
+    const drl_traj_queue::Slot& s = q->st[slot];
+    if (s.held || s.reserved != row0) return false;
+    p += q->batch - row0;
+  }
+  return true;
+}
+
+template <class Pred>
+bool wait_for(std::condition_variable& cv, std::unique_lock<std::mutex>& lk, int timeout_ms, Pred pred) {
+  if (timeout_ms < 0) {
+    cv.wait(lk, pred);
+    return true;
+  }
+  return cv.wait_for(lk, std::chrono::milliseconds(timeout_ms), pred);
+}
+
+// the caller holds q->mu
+int check_failed(const drl_traj_queue* q) {
+  if (!q->failed) return DRL_OK;
+  set_error("trajectory queue is in the failed state: a commit failed after reserving its positions (%s)",
+            q->failure.c_str());
+  return DRL_ERR_STATE;
+}
+
+}  // namespace
+
+void traj_queue_fail(drl_traj_queue* q, const char* why) {
+  {
+    std::lock_guard<std::mutex> lk(q->mu);
+    q->failed = true;
+    q->failure = why;
+  }
+  q->cv_space.notify_all();
+  q->cv_ready.notify_all();
+}
+
+int traj_queue_max_rows(const drl_traj_queue* q) { return (q->nslots - 1) * q->batch + 1; }
+
+int traj_queue_reserve(drl_traj_queue* q, int n, int timeout_ms, std::vector<TrajSegment>* segs) {
+  if (n < 1 || n > traj_queue_max_rows(q)) {
+    set_error("trajectory queue: %d rows per commit can never fit (at most %d in this queue: %d slots of %d)", n,
+              traj_queue_max_rows(q), q->nslots, q->batch);
+    return DRL_ERR_INVALID;
+  }
+  std::unique_lock<std::mutex> lk(q->mu);
+  if (!wait_for(q->cv_space, lk, timeout_ms, [&] { return q->failed || has_space(q, n); })) {
+    set_error("trajectory queue commit: timed out (queue full)");
+    return DRL_ERR_TIMEOUT;
+  }
+  DRL_TRY(check_failed(q));
+  segs->clear();
+  long long p = q->reserved_total;
+  int src = 0;
+  while (src < n) {
+    const int slot = (int)((p / q->batch) % q->nslots), row0 = (int)(p % q->batch);
+    const int rows = std::min(q->batch - row0, n - src);
+    drl_traj_queue::Slot& s = q->st[slot];
+    segs->push_back(TrajSegment{slot, row0, rows, src, s.ev_commit[s.n_commit], s.ev_release});
+    s.n_commit++;
+    s.reserved += rows;
+    p += rows;
+    src += rows;
+  }
+  q->reserved_total = p;
+  return DRL_OK;
+}
+
+void traj_queue_commit(drl_traj_queue* q, const std::vector<TrajSegment>& segs) {
+  std::lock_guard<std::mutex> lk(q->mu);
+  bool ready = false;
+  for (const TrajSegment& g : segs) {
+    drl_traj_queue::Slot& s = q->st[g.slot];
+    s.committed += g.rows;
+    q->committed_total += g.rows;
+    ready = ready || s.committed == q->batch;
+  }
+  if (ready) q->cv_ready.notify_all();
+}
+
+int traj_queue_pop(drl_traj_queue* q, int timeout_ms, int* slot, std::vector<cudaEvent_t>* ev_commit) {
+  std::unique_lock<std::mutex> lk(q->mu);
+  auto head = [&] { return (int)((q->popped_total / q->batch) % q->nslots); };
+  auto ready = [&] {
+    const drl_traj_queue::Slot& s = q->st[head()];
+    return !s.held && s.committed == q->batch;
+  };
+  if (!wait_for(q->cv_ready, lk, timeout_ms, [&] { return q->failed || ready(); })) {
+    set_error("trajectory queue stage: timed out (fewer than batch trajectories queued)");
+    return DRL_ERR_TIMEOUT;
+  }
+  DRL_TRY(check_failed(q));
+  *slot = head();
+  drl_traj_queue::Slot& s = q->st[*slot];
+  s.held = true;
+  ev_commit->assign(s.ev_commit.begin(), s.ev_commit.begin() + s.n_commit);
+  q->popped_total += q->batch;
+  return DRL_OK;
+}
+
+int traj_queue_release(drl_traj_queue* q, int slot, cudaStream_t s) {
+  const cudaError_t e = cudaEventRecord(q->st[slot].ev_release, s);
+  {
+    std::lock_guard<std::mutex> lk(q->mu);
+    drl_traj_queue::Slot& st = q->st[slot];
+    st.held = false;
+    st.reserved = 0;
+    st.committed = 0;
+    st.n_commit = 0;
+  }
+  q->cv_space.notify_all();
+  if (e != cudaSuccess) { set_error("trajectory queue release: %s", cudaGetErrorString(e)); return DRL_ERR_CUDA; }
+  return DRL_OK;
+}
+
+}  // namespace drl
+
+extern "C" {
+
+int drl_traj_queue_create(int32_t trajectory, int32_t height, int32_t width, int32_t channels, int32_t num_action,
+                          int32_t lstm_size, int32_t capacity, int32_t batch, int32_t device, drl_traj_queue** out) {
+  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
+  *out = nullptr;
+  if (trajectory < 1 || height < 1 || width < 1 || channels < 1 || num_action < 1 || lstm_size < 1 || batch < 1 ||
+      capacity < batch) {
+    set_error("trajectory queue: invalid dimensions (capacity must be >= batch)");
+    return DRL_ERR_INVALID;
+  }
+  if (drl_device_count() <= device || device < 0) {
+    set_error("CUDA device %d not available (no CPU fallback)", device);
+    return DRL_ERR_CUDA;
+  }
+  drl_traj_queue* q = new drl_traj_queue();
+  q->T = trajectory; q->H = height; q->W = width; q->C = channels; q->A = num_action; q->L = lstm_size;
+  q->batch = batch;
+  q->device = device;
+  q->nslots = (capacity + batch - 1) / batch + 1;
+  const size_t T = trajectory;
+  q->sz[kTrajState] = T * height * width * channels;
+  q->sz[kTrajReward] = T * 4;
+  q->sz[kTrajDone] = T;
+  q->sz[kTrajMu] = T * num_action * 4;
+  q->sz[kTrajAction] = T * 4;
+  q->sz[kTrajPa] = T * 4;
+  q->sz[kTrajH] = T * lstm_size * 4;
+  q->sz[kTrajC] = T * lstm_size * 4;
+  size_t off = 0;
+  for (int f = 0; f < kTrajFields; ++f) {
+    q->off[f] = off;
+    off = tq_align(off + (size_t)batch * q->sz[f]);
+  }
+  q->slot_bytes = off;
+  q->st.resize(q->nslots);
+  const int rc = [&]() -> int {
+    DRL_CUDA_CHECK(cudaSetDevice(device));
+    DRL_CUDA_CHECK(cudaMalloc((void**)&q->base, q->slot_bytes * q->nslots));
+    DRL_CUDA_CHECK(cudaMemset(q->base, 0, q->slot_bytes * q->nslots));
+    // a slot takes at most `batch` commits (each writes at least one row) before it is popped
+    for (auto& s : q->st) {
+      DRL_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_release, cudaEventDisableTiming));
+      s.ev_commit.assign(batch, nullptr);
+      for (auto& e : s.ev_commit) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    DRL_CUDA_CHECK(cudaDeviceSynchronize());
+    return DRL_OK;
+  }();
+  if (rc != DRL_OK) {
+    const std::string keep = get_error();
+    drl_traj_queue_destroy(q);
+    set_error("%s", keep.c_str());
+    return rc;
+  }
+  *out = q;
+  return DRL_OK;
+}
+
+int drl_traj_queue_destroy(drl_traj_queue* q) {
+  if (!q) return DRL_OK;
+  cudaSetDevice(q->device);
+  for (auto& s : q->st) {
+    if (s.ev_release) cudaEventSynchronize(s.ev_release);
+    for (cudaEvent_t e : s.ev_commit) if (e) { cudaEventSynchronize(e); cudaEventDestroy(e); }
+    if (s.ev_release) cudaEventDestroy(s.ev_release);
+  }
+  if (q->base) cudaFree(q->base);
+  cudaGetLastError();
+  delete q;
+  return DRL_OK;
+}
+
+int drl_traj_queue_size(drl_traj_queue* q) {
+  if (!q) return 0;
+  std::lock_guard<std::mutex> lk(q->mu);
+  return (int)(q->committed_total - q->popped_total);
+}
+
+int drl_traj_queue_read(drl_traj_queue* q, int32_t k, uint8_t* state, float* reward, uint8_t* done,
+                        float* behavior_policy, int32_t* action, int32_t* previous_action, float* previous_h,
+                        float* previous_c) {
+  if (!q) { set_error("null trajectory queue handle"); return DRL_ERR_INVALID; }
+  void* dst[kTrajFields] = {state, reward, done, behavior_policy, action, previous_action, previous_h, previous_c};
+  for (void* p : dst)
+    if (!p) { set_error("trajectory queue read: null output pointer"); return DRL_ERR_INVALID; }
+  std::lock_guard<std::mutex> lk(q->mu);
+  DRL_TRY(check_failed(q));
+  const long long size = q->committed_total - q->popped_total;
+  if (k < 0 || k >= size) {
+    set_error("trajectory queue read: k = %d is outside [0, %lld) (the queued trajectories)", k, size);
+    return DRL_ERR_INVALID;
+  }
+  const long long p = q->popped_total + k;
+  const int slot = (int)((p / q->batch) % q->nslots), row = (int)(p % q->batch);
+  const drl_traj_queue::Slot& s = q->st[slot];
+  if (s.committed != s.reserved) {
+    set_error("trajectory queue read: a commit into slot %d is still in progress", slot);
+    return DRL_ERR_STATE;
+  }
+  DRL_CUDA_CHECK(cudaSetDevice(q->device));
+  for (int i = 0; i < s.n_commit; ++i) DRL_CUDA_CHECK(cudaEventSynchronize(s.ev_commit[i]));
+  for (int f = 0; f < kTrajFields; ++f)
+    DRL_CUDA_CHECK(cudaMemcpy(dst[f], q->field(slot, f) + (size_t)row * q->sz[f], q->sz[f], cudaMemcpyDeviceToHost));
+  return DRL_OK;
+}
+
+}  // extern "C"

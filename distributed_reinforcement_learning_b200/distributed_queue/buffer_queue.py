@@ -1,5 +1,6 @@
 """H100-native stand-ins for ``distributed_queue/buffer_queue.py``: ``FIFOQueue`` (reference :418-512, the IMPALA
-trajectory queue) and ``SumTree`` / ``Memory`` (reference :326-416, the Ape-X prioritized replay memory).
+trajectory queue; ``DeviceFIFOQueue`` keeps it in GPU memory) and ``SumTree`` / ``Memory`` (reference :326-416, the
+Ape-X prioritized replay memory).
 
 The reference keeps a ``tf.FIFOQueue`` of 9-field trajectories on the learner's CPU and dequeues a
 batch with ``batch_size`` serial ``sess.run`` RPCs, after which the launcher ``np.stack``s eight
@@ -129,6 +130,71 @@ class FIFOQueue:
     def set_session(self, sess):
         """buffer_queue.py:511-512 (kept for call compatibility; there is no session)."""
         self.sess = sess
+
+
+class DeviceFIFOQueue:
+    """``FIFOQueue`` with its batch slots in GPU memory (``drl_traj_queue_*``, DESIGN.md section 12).
+
+    Producers are policy-engine recorders (``NativePolicy.recorder``): each act writes its step of every trajectory on
+    the device, and a commit moves whole trajectories into the queue with device-to-device copies; only reward and done
+    cross PCIe.  The consumer is ``impala.Agent.train_from_queue``, which stages the oldest batch into the learner
+    device to device.  Same constructor arguments as ``FIFOQueue`` plus ``device``; ``get_size`` counts committed and
+    not yet trained trajectories, as ``FIFOQueue.get_size`` does.  There is no host producer (``append_to_queue``) and
+    no host read of a batch (``sample_batch``); ``read(k)`` copies one queued trajectory out, for tests."""
+
+    def __init__(self, trajectory, input_shape, output_size,
+                 queue_size, batch_size, num_actors, lstm_size, device=0):
+        self.trajectory = int(trajectory)
+        self.input_shape = tuple(int(x) for x in input_shape)
+        if len(self.input_shape) != 3:
+            raise ValueError("input_shape: expected (height, width, channels), got %s" % (self.input_shape,))
+        self.output_size = int(output_size)
+        self.batch_size = int(batch_size)
+        self.lstm_size = int(lstm_size)
+        self.queue_size = int(queue_size)
+        self.num_actors = num_actors
+        self.device = int(device)
+        self.sess = None
+        # batch slots as the ring rounds them; one commit of n rows may span slots, so at most max_rows fit at once
+        nslots = -(-max(self.queue_size, self.batch_size) // self.batch_size) + 1
+        self.max_rows = (nslots - 1) * self.batch_size + 1
+        h, w, c = self.input_shape
+        self._q = C.c_void_p()
+        N.check(N.lib.drl_traj_queue_create(self.trajectory, h, w, c, self.output_size, self.lstm_size,
+                                            max(self.queue_size, self.batch_size), self.batch_size, self.device,
+                                            C.byref(self._q)))
+
+    def close(self):
+        if getattr(self, "_q", None) is not None and self._q.value:
+            N.lib.drl_traj_queue_destroy(self._q)
+            self._q = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def get_size(self):
+        """buffer_queue.py:507-509: trajectories committed and not yet popped by a learner."""
+        return int(N.lib.drl_traj_queue_size(self._q))
+
+    def set_session(self, sess):
+        """buffer_queue.py:511-512 (kept for call compatibility; there is no session)."""
+        self.sess = sess
+
+    def read(self, k):
+        """The k-th queued trajectory (0 = the next one a learner pops), copied to the host: a dict of state,
+        reward, done, behavior_policy, action, previous_action, previous_h, previous_c as ``append_to_queue`` takes
+        them."""
+        T, A, L = self.trajectory, self.output_size, self.lstm_size
+        out = dict(state=np.empty((T,) + self.input_shape, np.uint8), reward=np.empty(T, np.float32),
+                   done=np.empty(T, np.uint8), behavior_policy=np.empty((T, A), np.float32),
+                   action=np.empty(T, np.int32), previous_action=np.empty(T, np.int32),
+                   previous_h=np.empty((T, L), np.float32), previous_c=np.empty((T, L), np.float32))
+        N.check(N.lib.drl_traj_queue_read(self._q, int(k), *[N.ptr(a) for a in out.values()]))
+        out["done"] = out["done"].view(np.bool_)
+        return out
 
 
 class SumTree:

@@ -97,6 +97,12 @@ class NativeLearner:
         self._keep[slot] = arrs
         N.check(N.lib.drl_learner_stage(self._h, slot, *[N.ptr(a) for a in arrs]))
 
+    def stage_from_queue(self, slot, queue, timeout_ms=-1):
+        """Stage the oldest full batch of a ``DeviceFIFOQueue`` into ``slot`` device to device (blocks until one is
+        queued; ``timeout_ms`` >= 0 raises ``TimeoutError_`` with the queue and the slot untouched)."""
+        N.check(N.lib.drl_learner_stage_from_queue(self._h, int(slot), queue._q, int(timeout_ms)))
+        self._keep[slot] = None      # no host arrays behind this slot's copies
+
     @staticmethod
     def _out(o):
         return dict(pi_loss=o.pi_loss, baseline_loss=o.baseline_loss, entropy=o.entropy,

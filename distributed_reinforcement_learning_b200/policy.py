@@ -4,7 +4,13 @@ One ``NativePolicy`` serves the actor loop of ``train_impala.py:132-194`` for up
 batched ``get_policy_and_action`` (agent/impala.py:118-130) with the action drawn on the GPU, on its own CUDA stream
 next to a training ``NativeLearner``, and ``parameter_sync`` (agent/impala.py:111-112) device to device from that
 learner.  It owns no optimizer state, gradients or backward buffers.
+
+``NativePolicy.recorder(queue, n)`` binds the engine to a ``DeviceFIFOQueue``: the recorder's ``act`` is the engine's
+act that also writes the step's frames, previous actions, h, c, policies and actions into device staging, and its
+``commit`` moves the n recorded trajectories into the queue without copying them through the host.
 """
+import ctypes as C
+
 import numpy as np
 
 from . import _native as N
@@ -26,12 +32,20 @@ class NativePolicy(PolicyHandle):
         from .learner import NativeLearner
         return NativeLearner
 
+    def close(self):
+        # recorders first: a recorder's handle refers to this engine (the garbage collector may finalize the two in
+        # either order, so the engine owns the recorders' handle boxes, not the recorders)
+        for r in getattr(self, "_recorder_handles", ()):
+            _destroy_recorder(r)
+        self._recorder_handles = []
+        super().close()
+
+    def recorder(self, queue, n):
+        """A ``PolicyRecorder`` of n rows (n <= max_batch) into ``queue`` (a ``DeviceFIFOQueue`` on this device)."""
+        return PolicyRecorder(self, queue, n)
+
     # ---- inference -------------------------------------------------------------------
-    def act(self, state, previous_action, h, c, uniform=None):
-        """Batched get_policy_and_action for n <= max_batch rows: state uint8 [n, 84, 84, 4], previous_action [n],
-        h, c float32 [n, 256].  ``uniform`` (float64 [n] in [0, 1)) are the draws of the GPU sampler; without it they
-        come from ``np.random.random_sample(n)``, the global stream the reference's ``np.random.choice`` reads.
-        Returns dict(action, policy, max_prob, h, c)."""
+    def _act_args(self, state, previous_action, h, c, uniform):
         n, st, pa = self._inputs(state, previous_action)
         hh = N.as_c(h, np.float32, (n, self.L), "h")
         cc = N.as_c(c, np.float32, (n, self.L), "c")
@@ -40,10 +54,78 @@ class NativePolicy(PolicyHandle):
         u = N.as_c(uniform, np.float64, (n,), "uniform")
         if not np.all((u >= 0.0) & (u < 1.0)):
             raise ValueError("uniform: draws must lie in [0, 1)")
-        action = np.empty(n, np.int32)
-        pol = np.empty((n, self.A), np.float32)
-        ho = np.empty((n, self.L), np.float32)
-        co = np.empty((n, self.L), np.float32)
-        N.check(N.lib.drl_policy_act(self._h, n, N.ptr(st), N.ptr(pa), N.ptr(hh), N.ptr(cc), N.ptr(u), N.ptr(action),
-                                     N.ptr(pol), N.ptr(ho), N.ptr(co)))
+        outs = (np.empty(n, np.int32), np.empty((n, self.A), np.float32), np.empty((n, self.L), np.float32),
+                np.empty((n, self.L), np.float32))
+        return n, (st, pa, hh, cc, u), outs
+
+    @staticmethod
+    def _act_result(outs):
+        action, pol, ho, co = outs
         return dict(action=action, policy=pol, max_prob=pol.max(-1), h=ho, c=co)
+
+    def act(self, state, previous_action, h, c, uniform=None):
+        """Batched get_policy_and_action for n <= max_batch rows: state uint8 [n, 84, 84, 4], previous_action [n],
+        h, c float32 [n, 256].  ``uniform`` (float64 [n] in [0, 1)) are the draws of the GPU sampler; without it they
+        come from ``np.random.random_sample(n)``, the global stream the reference's ``np.random.choice`` reads.
+        Returns dict(action, policy, max_prob, h, c)."""
+        n, ins, outs = self._act_args(state, previous_action, h, c, uniform)
+        N.check(N.lib.drl_policy_act(self._h, n, *[N.ptr(a) for a in ins + outs]))
+        return self._act_result(outs)
+
+
+def _destroy_recorder(handle):
+    if handle.value:
+        N.lib.drl_policy_recorder_destroy(handle)
+        handle.value = None
+
+
+class PolicyRecorder:
+    """Records n rows of a ``NativePolicy``'s acts as trajectories of ``queue.trajectory`` steps, on the device.
+
+    ``act`` has ``NativePolicy.act``'s signature and return value; call it for steps t = 0 .. T-1 with exactly n rows,
+    then ``commit(reward, done)`` with the [n, T] rewards and done flags the environments gave.  The commit moves the n
+    trajectories into the queue in row order (blocking while it is full; ``timeout_ms`` >= 0 raises
+    ``TimeoutError_`` with nothing changed) and starts the next unroll.  Each trajectory stores the frames, previous
+    actions, h and c the acts were given and the policies and actions they returned.  Closing the policy closes its
+    recorders; keep the queue open while a recorder is in use."""
+
+    def __init__(self, policy, queue, n):
+        from .distributed_queue.buffer_queue import DeviceFIFOQueue
+        if not isinstance(queue, DeviceFIFOQueue):
+            raise TypeError("recorder: queue must be a DeviceFIFOQueue, got %s" % type(queue).__name__)
+        n = int(n)
+        if not 1 <= n <= policy.max_batch:
+            raise ValueError("recorder: n = %d rows, the policy serves 1..%d" % (n, policy.max_batch))
+        self.policy, self.queue, self.n, self.T = policy, queue, n, queue.trajectory
+        self._r = C.c_void_p()
+        N.check(N.lib.drl_policy_recorder_create(policy._h, queue._q, n, C.byref(self._r)))
+        live = [r for r in getattr(policy, "_recorder_handles", ()) if r.value]
+        policy._recorder_handles = live + [self._r]
+
+    def close(self):
+        if getattr(self, "_r", None) is not None:
+            _destroy_recorder(self._r)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def act(self, state, previous_action, h, c, uniform=None):
+        """``NativePolicy.act`` of the recorder's n rows, recorded as the next step of the unroll."""
+        n, ins, outs = self.policy._act_args(state, previous_action, h, c, uniform)
+        if n != self.n:
+            raise ValueError("recorder act: %d rows, the recorder records %d" % (n, self.n))
+        N.check(N.lib.drl_policy_recorder_act(self._r, *[N.ptr(a) for a in ins + outs]))
+        return self.policy._act_result(outs)
+
+    def reset(self):
+        """Discard the steps recorded since the last commit (an unroll abandoned half-way); the next act is step 0."""
+        N.check(N.lib.drl_policy_recorder_reset(self._r))
+
+    def commit(self, reward, done, timeout_ms=-1):
+        """Moves the n recorded trajectories into the queue; reward float32 [n, T], done bool / uint8 [n, T]."""
+        rw = N.as_c(reward, np.float32, (self.n, self.T), "reward")
+        dn = N.as_c(N.as_u8(done), np.uint8, (self.n, self.T), "done")
+        N.check(N.lib.drl_policy_recorder_commit(self._r, N.ptr(rw), N.ptr(dn), int(timeout_ms)))

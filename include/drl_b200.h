@@ -108,6 +108,14 @@ int drl_learner_stage(drl_learner* h, int32_t slot,
                       const uint8_t* state, const float* reward, const int32_t* action,
                       const uint8_t* done, const float* behavior_policy,
                       const int32_t* previous_action, const float* initial_h, const float* initial_c);
+/* The device trajectory queue (drl_traj_queue_create, below). */
+typedef struct drl_traj_queue drl_traj_queue;
+/* drl_learner_stage from a device trajectory queue: pops the oldest full batch (blocking like drl_ring_pop_batch;
+ * a time-out is DRL_ERR_TIMEOUT and leaves the queue and the slot untouched), then on the copy stream waits for the
+ * slot's last reader and the batch's commits, copies the batch device to device and hands the queue slot back to the
+ * producers without a host wait.  The queue must have the learner's batch, trajectory, num_action, geometry and device
+ * (DRL_ERR_INVALID otherwise). */
+int drl_learner_stage_from_queue(drl_learner* h, int32_t slot, drl_traj_queue* queue, int32_t timeout_ms);
 
 /* sess.run([pi_loss, baseline_loss, entropy, learning_rate, train_op]) (agent/impala.py:144-146):
  * forward, V-trace, losses, backward, global-norm clip, RMSProp, step += 1 on slot `slot`;
@@ -227,6 +235,32 @@ int drl_policy_act(drl_policy* h, int32_t n, const uint8_t* state, const int32_t
                    float* c_out);
 /* Device time of the most recent drl_policy_act (input copy + kernels; CUDA events on the policy's stream), ms. */
 int drl_policy_last_act_ms(drl_policy* h, float* ms);
+
+/* Recorder: binds an engine to a device trajectory queue (drl_traj_queue_create below) for n <= max_batch rows, with
+ * device staging of n trajectories of the queue's T steps (39 MB at n = 64, T = 20).  Queue and engine must be on the
+ * same device, with the same num_action and the 84x84x4 / lstm 256 geometry, and n must fit the queue at once; all
+ * DRL_ERR_INVALID otherwise.  Without a device, DRL_ERR_CUDA.  Destroy the recorder before its engine and queue. */
+typedef struct drl_policy_recorder drl_policy_recorder;
+int drl_policy_recorder_create(drl_policy* h, drl_traj_queue* queue, int32_t n, drl_policy_recorder** out);
+int drl_policy_recorder_destroy(drl_policy_recorder* r);
+/* drl_policy_act of the recorder's n rows (same inputs, outputs and results; `uniform` is required) that also records
+ * step t of rows 0..n-1 on the device: the frame, previous action, h_in and c_in given, and the policy and action
+ * computed.  Steps are recorded in order t = 0..T-1; an act after step T-1 is DRL_ERR_STATE until the commit.  With
+ * use_cuda_graph one graph per recorder replays every step (the step reaches the kernels through the staged input).
+ * drl_policy_recorder_reset discards the steps recorded since the last commit (an unroll abandoned half-way, e.g. when
+ * an environment raised); the queue never saw them. */
+int drl_policy_recorder_act(drl_policy_recorder* r, const uint8_t* state, const int32_t* previous_action,
+                            const float* h_in, const float* c_in, const double* uniform, int32_t* action,
+                            float* policy, float* h_out, float* c_out);
+int drl_policy_recorder_reset(drl_policy_recorder* r);
+/* After step T-1 (DRL_ERR_STATE otherwise): reward f32 [n,T] and done u8 [n,T] complete the n trajectories, which are
+ * appended to the queue in row order at n consecutive positions.  Blocks while those positions are not free
+ * (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with nothing changed otherwise).  Only reward and done are copied from the
+ * host; the rest moves device to device on the engine's stream after the target slots' last readers, and the learner's
+ * staging waits for it.  Returns without waiting for the copies; the next unroll starts at t = 0.  If enqueueing the
+ * copies fails after the positions were reserved, the queue goes into a failed state instead of blocking forever: this
+ * commit returns the CUDA error, and every later commit, stage or read of the queue returns DRL_ERR_STATE. */
+int drl_policy_recorder_commit(drl_policy_recorder* r, const float* reward, const uint8_t* done, int32_t timeout_ms);
 
 /* ------------------------------------------------------------------------------------------
  * R2D2 policy engine (new): the actor side of train_r2d2.py:167-251 (the actor loop itself is
@@ -395,6 +429,26 @@ int drl_ring_pop_batch(drl_ring* r, drl_ring_batch* out, int32_t timeout_ms);
 int drl_ring_release(drl_ring* r, int32_t slot);
 /* FIFOQueue.get_size (buffer_queue.py:507-509): trajectories enqueued and not yet popped. */
 int drl_ring_size(drl_ring* r);
+
+/* ------------------------------------------------------------------------------------------
+ * Device trajectory queue (new): the ring's FIFO with its batch slots in GPU memory.  Producers are policy recorders
+ * (drl_policy_recorder_commit), the consumer is drl_learner_stage_from_queue; a batch never passes through the host.
+ * A slot holds `batch` trajectories field-major in the learner's batch-major staging layout, so staging a batch is
+ * eight device-to-device copies.  capacity is rounded up as the ring's, plus one slot (97 MB at T = 20, A = 18,
+ * capacity 128, batch 32).  Thread-safe: several recorders may commit while one learner stages.
+ * ------------------------------------------------------------------------------------------ */
+/* (drl_traj_queue is declared with the learner above.)  DRL_ERR_CUDA ("no CPU fallback") when `device` does not exist. */
+int drl_traj_queue_create(int32_t trajectory, int32_t height, int32_t width, int32_t channels, int32_t num_action,
+                          int32_t lstm_size, int32_t capacity, int32_t batch, int32_t device, drl_traj_queue** out);
+int drl_traj_queue_destroy(drl_traj_queue* q);
+/* trajectories committed and not yet popped by a learner (as drl_ring_size) */
+int drl_traj_queue_size(drl_traj_queue* q);
+/* Synchronous copy of the k-th queued trajectory (0 = the next to be popped) into host arrays laid out as
+ * drl_ring_push takes them; for tests.  DRL_ERR_INVALID for k outside [0, size), DRL_ERR_STATE while a commit into
+ * its slot is in progress. */
+int drl_traj_queue_read(drl_traj_queue* q, int32_t k, uint8_t* state, float* reward, uint8_t* done,
+                        float* behavior_policy, int32_t* action, int32_t* previous_action, float* previous_h,
+                        float* previous_c);
 
 /* ------------------------------------------------------------------------------------------
  * Ape-X DQN learner (SURVEY.md section 8(f) row 2, BASELINE.json config 4): replaces apex.Agent's learner graph
