@@ -188,6 +188,15 @@ def _load():
         "drl_policy_recorder_commit": (C.c_int, [vp, vp, vp, i32]),
         "drl_policy_recorder_reset": (C.c_int, [vp]),
         "drl_learner_stage_from_queue": (C.c_int, [vp, i32, vp, i32]),
+        "drl_r2d2_queue_create": (C.c_int, [i32] * 6 + [C.POINTER(vp)]),
+        "drl_r2d2_queue_destroy": (C.c_int, [vp]),
+        "drl_r2d2_queue_size": (C.c_int, [vp]),
+        "drl_r2d2_queue_read": (C.c_int, [vp, i32] + [vp] * 7),
+        "drl_r2d2_policy_recorder_create": (C.c_int, [vp, vp, i32, C.POINTER(vp)]),
+        "drl_r2d2_policy_recorder_destroy": (C.c_int, [vp]),
+        "drl_r2d2_policy_recorder_act": (C.c_int, [vp] + [vp] * 10),
+        "drl_r2d2_policy_recorder_commit": (C.c_int, [vp, vp, vp, i32]),
+        "drl_r2d2_policy_recorder_reset": (C.c_int, [vp]),
         "drl_apex_create": (C.c_int, [C.POINTER(ApexConfig), C.POINTER(vp)]),
         "drl_apex_destroy": (C.c_int, [vp]),
         "drl_apex_param_count": (C.c_int, [vp, C.POINTER(i64)]),
@@ -279,6 +288,7 @@ def _load():
         "drl_r2d2_replay_create": (C.c_int, [i32, i64, i32, i32, i32, C.POINTER(vp)]),
         "drl_r2d2_replay_destroy": (C.c_int, [vp]),
         "drl_r2d2_replay_add": (C.c_int, [vp, vp, i32] + [vp] * 8),
+        "drl_r2d2_replay_add_from_queue": (C.c_int, [vp, vp, vp, i32]),
         "drl_r2d2_replay_step_async": (C.c_int, [vp, vp, i32, vp]),
         "drl_r2d2_replay_sample": (C.c_int, [vp, i32] + [vp] * 5),
         "drl_r2d2_replay_update": (C.c_int, [vp, i32, vp, vp]),

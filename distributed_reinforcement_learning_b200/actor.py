@@ -149,7 +149,10 @@ class R2D2VectorActor:
       - at an episode's end epsilon becomes 1 / (0.01 episode + 1), and the environment, the previous action, h, c
         and lives are reset.  episode_step and the summed q of the logged average are never reset, as in the
         reference;
-      - every environment's trajectory goes to ``queue.append_to_queue(task=i, ...)``.
+      - every environment's trajectory goes to ``queue.append_to_queue(task=i, ...)``; with an
+        ``R2D2DeviceFIFOQueue`` the acts go through a recorder of the policy instead (``NativeR2D2Policy.recorder``),
+        which keeps the sequences on the GPU, and the unroll ends with one ``commit`` of the rewards and done flags of
+        all N environments, in environment order.
     At n = 1 this is the reference actor's loop, including the order of its ``np.random`` draws.
     """
 
@@ -171,19 +174,46 @@ class R2D2VectorActor:
         self.score = [0.0] * n
         self.episode_step = [0] * n
         self.episode_q_value = [0.0] * n
+        self.recorder = None
+        if isinstance(queue, buffer_queue.R2D2DeviceFIFOQueue):
+            self._check_device_queue(queue)
+            self.recorder = policy.recorder(queue, n)
+
+    def _check_device_queue(self, queue):
+        p = self.policy
+        if queue.seq_len != self.seq_len:
+            raise ValueError("queue records sequences of %d steps, the actor unrolls %d" % (queue.seq_len, self.seq_len))
+        if queue.output_size != p.A:
+            raise ValueError("queue has num_action %d, the policy %d" % (queue.output_size, p.A))
+        if queue.lstm_size != p.L or tuple(queue.input_shape) != tuple(p.input_shape):
+            raise ValueError("queue stores %s frames and lstm %d, the policy takes %s and %d"
+                             % (tuple(queue.input_shape), queue.lstm_size, tuple(p.input_shape), p.L))
+        if queue.device != p.device:
+            raise ValueError("queue is on device %d, the policy on device %d" % (queue.device, p.device))
+        n = len(self.envs)
+        if n > queue.max_rows:
+            raise ValueError("%d environments per commit, the queue takes at most %d at once" % (n, queue.max_rows))
 
     def run_unroll(self):
         """One unroll of `seq_len` steps for every environment, pushed to the queue.  Returns the episodes that
         finished during it: dicts of task, episode, score, epsilon, episode_step and avg_q_value, the values
         train_r2d2.py:227-230 logs."""
-        for b in self.buffers:
-            b.init()
+        n = len(self.envs)
+        rec = self.recorder
+        if rec is None:
+            for b in self.buffers:
+                b.init()
+            act = self.policy.act
+        else:
+            rec.reset()   # an unroll that raised half-way left its steps behind: start this one at step 0
+            rewards = np.zeros((n, self.seq_len), np.float32)
+            dones = np.zeros((n, self.seq_len), np.bool_)
+            act = rec.act
         if self.learner is not None:
             self.learner.sync_policy(self.policy)
         finished = []
-        for _ in range(self.seq_len):
-            out = self.policy.act(np.stack(self.states), self.previous_action, self.h, self.c,
-                                  epsilon=np.array(self.epsilon))
+        for step in range(self.seq_len):
+            out = act(np.stack(self.states), self.previous_action, self.h, self.c, epsilon=np.array(self.epsilon))
             action, q_action = out["action"], out["q_action"]
             # fresh copies: rows already stored in a trajectory, and the arrays act returned, are never written again
             next_pa, next_h, next_c = action.astype(np.int32), out["h"].copy(), out["c"].copy()
@@ -197,8 +227,11 @@ class R2D2VectorActor:
                     r, d = -1, True
                 else:
                     r, d = reward, False
-                self.buffers[i].append(state=self.states[i], previous_action=int(self.previous_action[i]), action=a,
-                                       reward=r, done=d, initial_h=self.h[i], initial_c=self.c[i])
+                if rec is None:
+                    self.buffers[i].append(state=self.states[i], previous_action=int(self.previous_action[i]),
+                                           action=a, reward=r, done=d, initial_h=self.h[i], initial_c=self.c[i])
+                else:   # the rest of the step is on the device already
+                    rewards[i, step], dones[i, step] = r, d
                 self.states[i] = next_state
                 if done:
                     finished.append(dict(task=i, episode=self.episode[i], score=self.score[i],
@@ -213,6 +246,9 @@ class R2D2VectorActor:
                     next_c[i] = 0.0
                     self.lives[i] = START_LIVES
             self.previous_action, self.h, self.c = next_pa, next_h, next_c
+        if rec is not None:
+            rec.commit(rewards, dones)
+            return finished
         for i, b in enumerate(self.buffers):
             u = b.extract()
             self.queue.append_to_queue(

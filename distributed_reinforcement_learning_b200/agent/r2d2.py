@@ -7,7 +7,8 @@ the learner branch of ``train_r2d2.py:87-165`` runs on it unchanged, with the TF
   Agent.parameter_sync agent/r2d2.py:161-162 ; Agent.main_to_target :164-165 ; Agent.set_session :167-169
   Agent.get_action     agent/r2d2.py:171-191 -> (action, q_value[action], h', c')
   Agent.sync_policy    (new) parameter_sync into a NativeR2D2Policy (r2d2_policy.py), device to device from the learner
-  Agent.device_memory  (new) a DeviceMemory: the replay memory of train_r2d2.py:92-93 on the GPU (r2d2_replay.py)
+  Agent.device_memory  (new) a DeviceMemory: the replay memory of train_r2d2.py:92-93 on the GPU (r2d2_replay.py);
+                       DeviceMemory.add_from_queue ingests a batch of an R2D2DeviceFIFOQueue without a host copy
   Agent.train_from_memory (new) Memory.sample + the minibatch lists + train + Memory.update (train_r2d2.py:122-162)
                        as one device-resident step -> (loss, td_error)
   Agent.main_q_value_test / target_q_value_test   agent/r2d2.py:193-217
@@ -219,6 +220,9 @@ class DeviceMemory:
         memory.add(q.state, q.previous_action, q.action, q.previous_h, q.previous_c, q.reward, q.done)
         loss, td_error = learner.train_from_memory(memory, batch_size)  # sample .. train .. update
 
+    or, with the actors' R2D2VectorActor recording into an R2D2DeviceFIFOQueue, ``memory.add_from_queue(queue)`` in
+    place of the sample_batch and the add.
+
     It outlives a rebuild of the agent's learner (another batch size): the agent passes its current learner to each
     call.  ``replay`` is the NativeR2D2Replay; ``n_entries``, ``beta``, ``total()`` and ``last_sample()`` read its state."""
 
@@ -249,6 +253,21 @@ class DeviceMemory:
             for lo in range(0, st.shape[0], eng.B):
                 hi = min(lo + eng.B, st.shape[0])
                 self.replay.add(eng, st[lo:hi], pa[lo:hi], ac[lo:hi], h0[lo:hi], c0[lo:hi], rw[lo:hi], dn[lo:hi])
+
+    def add_from_queue(self, queue, timeout_ms=-1):
+        """``add`` of the oldest ``queue.batch_size`` sequences of an R2D2DeviceFIFOQueue (train_r2d2.py:97-120
+        without a host copy): the learner's |td| of the batch and the store read the queue's GPU memory directly.
+        Blocks while fewer than a batch are queued; ``timeout_ms`` >= 0 raises ``TimeoutError_`` with nothing
+        changed.  One learner thread calls it, as it calls train_from_memory; actor threads may record into the
+        queue and sync their policies from the agent meanwhile."""
+        if dp.distributed():
+            raise RuntimeError("add_from_queue: a DeviceMemory is local to one GPU; data-parallel training "
+                               "(torch.distributed world > 1) uses Memory and train")
+        a = self.agent
+        with a._lock:
+            eng = a._engine if a._engine is not None else a._get_engine(queue.batch_size)
+        # the wait for a full batch runs without the agent's lock: actor threads take it in sync_policy meanwhile
+        self.replay.add_from_queue(eng, queue, timeout_ms)
 
     n_entries = property(lambda self: self.replay.n_entries)
     beta = property(lambda self: self.replay.beta)

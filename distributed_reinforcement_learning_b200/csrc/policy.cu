@@ -21,7 +21,7 @@
 #include "policy_core.cuh"
 #include "policy_head.cuh"
 #include "policy_lstm.cuh"
-#include "traj_queue.cuh"
+#include "queue_recorder.cuh"
 
 namespace drl {
 namespace {
@@ -289,19 +289,9 @@ struct drl_policy : PolicyCore {
   size_t off_h = 0, off_c = 0, off_act = 0;
 };
 
-struct drl_policy_recorder {
-  drl_policy* engine = nullptr;
-  drl_traj_queue* q = nullptr;
-  int n = 0, T = 0;
-  int t = 0;                          // steps recorded since the last commit
-  uint8_t* staging = nullptr;         // [n] trajectories, field-major in the queue's field order
-  size_t off[kTrajFields] = {};
-  int32_t* d_t = nullptr;             // the step, read by the recording kernels
-  int32_t* h_t = nullptr;             // its pinned staging
-  uint8_t* h_rd = nullptr;            // pinned reward [n][T] f32 | done [n][T] u8 of a commit
-  cudaGraphExec_t graph = nullptr;
-  std::vector<void*> allocs;
-  uint8_t* field(int f) { return staging + off[f]; }
+// the recorder's staging (RecorderCore) is in the queue's field order (TrajField)
+struct drl_policy_recorder : RecorderCore {
+  drl_policy* policy = nullptr;
 };
 
 namespace {
@@ -360,8 +350,8 @@ int enqueue_act(PolicyCore* c, int n) { return enqueue_act_impl(static_cast<drl_
 
 // the recorder's act: the step word, then the recording act of its n rows
 int enqueue_record(drl_policy_recorder* r) {
-  DRL_CUDA_CHECK(cudaMemcpyAsync(r->d_t, r->h_t, sizeof(int32_t), cudaMemcpyHostToDevice, r->engine->stream));
-  return enqueue_act_impl(r->engine, r->n, r);
+  DRL_CUDA_CHECK(cudaMemcpyAsync(r->d_t, r->h_t, sizeof(int32_t), cudaMemcpyHostToDevice, r->policy->stream));
+  return enqueue_act_impl(r->policy, r->n, r);
 }
 
 // act's argument checks and the staging of its inputs into h_in (the caller holds the engine's lock)
@@ -386,15 +376,6 @@ void copy_act_outputs(const drl_policy* h, int n, int32_t* action, float* policy
   if (h_out) memcpy(h_out, h->h_out + h->off_h, (size_t)n * Geo::L * 4);
   if (c_out) memcpy(c_out, h->h_out + h->off_c, (size_t)n * Geo::L * 4);
   if (action) memcpy(action, h->h_out + h->off_act, (size_t)n * 4);
-}
-
-void recorder_release(drl_policy_recorder* r) {
-  if (r->engine && r->engine->stream) cudaStreamSynchronize(r->engine->stream);
-  if (r->graph) cudaGraphExecDestroy(r->graph);
-  for (void* p : r->allocs) cudaFree(p);
-  if (r->h_t) cudaFreeHost(r->h_t);
-  if (r->h_rd) cudaFreeHost(r->h_rd);
-  cudaGetLastError();
 }
 
 }  // namespace
@@ -495,27 +476,16 @@ int drl_policy_recorder_create(drl_policy* h, drl_traj_queue* q, int32_t n, drl_
   }
   NvtxRange nv("drl:policy_recorder_create");
   drl_policy_recorder* r = new drl_policy_recorder();
-  r->engine = h;
+  r->engine = r->policy = h;
   r->q = q;
   r->n = n;
   r->T = q->T;
-  const int rc = [&]() -> int {
-    DRL_CUDA_CHECK(cudaSetDevice(h->device));
-    size_t off = 0;
-    for (int f = 0; f < kTrajFields; ++f) {
-      r->off[f] = off;
-      off = align_up(off + (size_t)n * q->sz[f], 256);
-    }
-    DRL_TRY(dev_alloc(r, &r->staging, off));
-    DRL_TRY(dev_alloc(r, &r->d_t, 1));
-    DRL_CUDA_CHECK(cudaHostAlloc((void**)&r->h_t, sizeof(int32_t), cudaHostAllocDefault));
-    *r->h_t = 0;
-    DRL_CUDA_CHECK(cudaHostAlloc((void**)&r->h_rd, (size_t)n * r->T * 5, cudaHostAllocDefault));
-    return DRL_OK;
-  }();
+  r->f_reward = kTrajReward;
+  r->f_done = kTrajDone;
+  const int rc = recorder_core_init(r);
   if (rc != DRL_OK) {
     const std::string keep = get_error();
-    recorder_release(r);
+    recorder_core_release(r);
     delete r;
     set_error("%s", keep.c_str());
     return rc;
@@ -524,102 +494,31 @@ int drl_policy_recorder_create(drl_policy* h, drl_traj_queue* q, int32_t n, drl_
   return DRL_OK;
 }
 
-int drl_policy_recorder_destroy(drl_policy_recorder* r) {
-  if (!r) return DRL_OK;
-  {
-    std::lock_guard<std::recursive_mutex> lk(r->engine->mu);
-    cudaSetDevice(r->engine->device);
-    recorder_release(r);
-  }
-  delete r;
-  return DRL_OK;
-}
+int drl_policy_recorder_destroy(drl_policy_recorder* r) { return recorder_destroy(r); }
 
 int drl_policy_recorder_act(drl_policy_recorder* r, const uint8_t* state, const int32_t* previous_action,
                             const float* h_in, const float* c_in, const double* uniform, int32_t* action,
                             float* policy, float* h_out, float* c_out) {
   if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
-  drl_policy* h = r->engine;
+  drl_policy* h = r->policy;
   std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (r->t >= r->T) {
-    set_error("recorder act: all %d steps of the unroll are recorded (commit them first)", r->T);
-    return DRL_ERR_STATE;
-  }
+  DRL_TRY(recorder_check_step(r));
   if (!uniform) { set_error("recorder act: `uniform` is required (the recorded actions are the sampled ones)"); return DRL_ERR_INVALID; }
   DRL_TRY(stage_act(h, r->n, state, previous_action, h_in, c_in, uniform, action));
   NvtxRange nv("drl:policy_recorder_act");
-  *r->h_t = r->t;
-  DRL_CUDA_CHECK(cudaSetDevice(h->device));
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_start, h->stream));
-  if (h->use_cuda_graph) {
-    if (!r->graph) {
-      DRL_TRY(enqueue_record(r));   // eager pass first: attributes and tensor maps outside capture (idempotent)
-      DRL_TRY(capture_graph(h->stream, [&] { return enqueue_record(r); }, &r->graph));
-    }
-    DRL_CUDA_CHECK(cudaGraphLaunch(r->graph, h->stream));
-  } else {
-    DRL_TRY(enqueue_record(r));
-  }
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->stream));
-  DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
-  h->timed = true;
+  DRL_TRY(recorder_run_act(r, [r] { return enqueue_record(r); }));
   copy_act_outputs(h, r->n, action, policy, h_out, c_out);
-  r->t++;
   return DRL_OK;
 }
 
 int drl_policy_recorder_commit(drl_policy_recorder* r, const float* reward, const uint8_t* done, int32_t timeout_ms) {
   if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
-  if (!reward || !done) { set_error("recorder commit: null argument"); return DRL_ERR_INVALID; }
-  drl_policy* h = r->engine;
-  {
-    std::lock_guard<std::recursive_mutex> lk(h->mu);
-    if (r->t != r->T) {
-      set_error("recorder commit: %d of %d steps recorded (commit follows step T-1)", r->t, r->T);
-      return DRL_ERR_STATE;
-    }
-  }
-  // reserve without the engine's lock: a learner thread may sync this engine while the commit waits for space
-  std::vector<TrajSegment> segs;
-  DRL_TRY(traj_queue_reserve(r->q, r->n, timeout_ms, &segs));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  NvtxRange nv("drl:policy_recorder_commit");
-  drl_traj_queue* q = r->q;
-  cudaStream_t s = h->stream;
-  const size_t nT = (size_t)r->n * r->T;
-  const int rc = [&]() -> int {
-    // h_rd is free: every act since the previous commit waited for the stream
-    memcpy(r->h_rd, reward, nT * 4);
-    memcpy(r->h_rd + nT * 4, done, nT);
-    DRL_CUDA_CHECK(cudaSetDevice(h->device));
-    DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(kTrajReward), r->h_rd, nT * 4, cudaMemcpyHostToDevice, s));
-    DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(kTrajDone), r->h_rd + nT * 4, nT, cudaMemcpyHostToDevice, s));
-    for (const TrajSegment& g : segs) {
-      DRL_CUDA_CHECK(cudaStreamWaitEvent(s, g.ev_release, 0));
-      for (int f = 0; f < kTrajFields; ++f)
-        DRL_CUDA_CHECK(cudaMemcpyAsync(q->field(g.slot, f) + (size_t)g.row0 * q->sz[f],
-                                       r->field(f) + (size_t)g.src0 * q->sz[f], (size_t)g.rows * q->sz[f],
-                                       cudaMemcpyDeviceToDevice, s));
-      DRL_CUDA_CHECK(cudaEventRecord(g.ev_commit, s));
-    }
-    return DRL_OK;
-  }();
-  if (rc != DRL_OK) {
-    // the reserved positions will never be filled: rather than leave every producer and the learner waiting behind
-    // them, the queue goes into its failed state (every later reserve / pop / read returns DRL_ERR_STATE)
-    traj_queue_fail(q, get_error());
-    return rc;
-  }
-  traj_queue_commit(q, segs);
-  r->t = 0;
-  return DRL_OK;
+  return recorder_commit(r, reward, done, timeout_ms);
 }
 
 int drl_policy_recorder_reset(drl_policy_recorder* r) {
   if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
-  std::lock_guard<std::recursive_mutex> lk(r->engine->mu);
-  r->t = 0;
-  return DRL_OK;
+  return recorder_reset(r);
 }
 
 }  // extern "C"

@@ -1,10 +1,12 @@
-// policy_core.cu -- the network-independent half of the batched policy engines (policy_core.cuh).
+// policy_core.cu -- the network-independent half of the batched policy engines (policy_core.cuh) and of their queue
+// recorders (queue_recorder.cuh).
 #include <string.h>
 
 #include <algorithm>
 #include <string>
 
 #include "policy_core.cuh"
+#include "queue_recorder.cuh"
 
 namespace drl {
 namespace {
@@ -192,6 +194,112 @@ int policy_last_act_ms(PolicyCore* h, const char* family, float* ms) {
   if (!h->timed) { set_error("last_act_ms: no act call has run yet"); return DRL_ERR_STATE; }
   DRL_CUDA_CHECK(cudaSetDevice(h->device));
   DRL_CUDA_CHECK(cudaEventElapsedTime(ms, h->ev_start, h->ev_stop));
+  return DRL_OK;
+}
+
+// ---- recorders ---------------------------------------------------------------------------------------------------
+int recorder_core_init(RecorderCore* r) {
+  DRL_CUDA_CHECK(cudaSetDevice(r->engine->device));
+  size_t off = 0;
+  for (int f = 0; f < r->q->nfields; ++f) {
+    r->off[f] = off;
+    off = align_up(off + (size_t)r->n * r->q->sz[f], 256);
+  }
+  DRL_TRY(dev_alloc(r, &r->staging, off));
+  DRL_TRY(dev_alloc(r, &r->d_t, 1));
+  DRL_CUDA_CHECK(cudaHostAlloc((void**)&r->h_t, sizeof(int32_t), cudaHostAllocDefault));
+  *r->h_t = 0;
+  DRL_CUDA_CHECK(cudaHostAlloc((void**)&r->h_rd, (size_t)r->n * r->T * 5, cudaHostAllocDefault));
+  return DRL_OK;
+}
+
+void recorder_core_release(RecorderCore* r) {
+  if (r->engine && r->engine->stream) cudaStreamSynchronize(r->engine->stream);
+  if (r->graph) cudaGraphExecDestroy(r->graph);
+  for (void* p : r->allocs) cudaFree(p);
+  if (r->h_t) cudaFreeHost(r->h_t);
+  if (r->h_rd) cudaFreeHost(r->h_rd);
+  cudaGetLastError();
+}
+
+int recorder_check_step(const RecorderCore* r) {
+  if (r->t >= r->T) {
+    set_error("recorder act: all %d steps of the unroll are recorded (commit them first)", r->T);
+    return DRL_ERR_STATE;
+  }
+  return DRL_OK;
+}
+
+int recorder_run_act(RecorderCore* r, const std::function<int()>& enqueue_step) {
+  PolicyCore* h = r->engine;
+  *r->h_t = r->t;
+  DRL_CUDA_CHECK(cudaSetDevice(h->device));
+  DRL_CUDA_CHECK(cudaEventRecord(h->ev_start, h->stream));
+  if (h->use_cuda_graph) {
+    if (!r->graph) {
+      DRL_TRY(enqueue_step());   // eager pass first: attributes and tensor maps outside capture (idempotent)
+      DRL_TRY(capture_graph(h->stream, enqueue_step, &r->graph));
+    }
+    DRL_CUDA_CHECK(cudaGraphLaunch(r->graph, h->stream));
+  } else {
+    DRL_TRY(enqueue_step());
+  }
+  DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->stream));
+  DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
+  h->timed = true;
+  r->t++;
+  return DRL_OK;
+}
+
+int recorder_commit(RecorderCore* r, const float* reward, const uint8_t* done, int timeout_ms) {
+  if (!reward || !done) { set_error("recorder commit: null argument"); return DRL_ERR_INVALID; }
+  PolicyCore* h = r->engine;
+  {
+    Lock lk(h->mu);
+    if (r->t != r->T) {
+      set_error("recorder commit: %d of %d steps recorded (commit follows step %s)", r->t, r->T, r->last_step);
+      return DRL_ERR_STATE;
+    }
+  }
+  // reserve without the engine's lock: a learner thread may sync this engine while the commit waits for space
+  std::vector<TrajSegment> segs;
+  DRL_TRY(traj_queue_reserve(r->q, r->n, timeout_ms, &segs));
+  Lock lk(h->mu);
+  NvtxRange nv(r->commit_range);
+  QueueCore* q = r->q;
+  cudaStream_t s = h->stream;
+  const size_t nT = (size_t)r->n * r->T;
+  const int rc = [&]() -> int {
+    // h_rd is free: every act since the previous commit waited for the stream
+    memcpy(r->h_rd, reward, nT * 4);
+    memcpy(r->h_rd + nT * 4, done, nT);
+    DRL_CUDA_CHECK(cudaSetDevice(h->device));
+    DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(r->f_reward), r->h_rd, nT * 4, cudaMemcpyHostToDevice, s));
+    DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(r->f_done), r->h_rd + nT * 4, nT, cudaMemcpyHostToDevice, s));
+    for (const TrajSegment& g : segs) {
+      DRL_CUDA_CHECK(cudaStreamWaitEvent(s, g.ev_release, 0));
+      for (int f = 0; f < q->nfields; ++f)
+        DRL_CUDA_CHECK(cudaMemcpyAsync(q->field(g.slot, f) + (size_t)g.row0 * q->sz[f],
+                                       r->field(f) + (size_t)g.src0 * q->sz[f], (size_t)g.rows * q->sz[f],
+                                       cudaMemcpyDeviceToDevice, s));
+      DRL_CUDA_CHECK(cudaEventRecord(g.ev_commit, s));
+    }
+    return DRL_OK;
+  }();
+  if (rc != DRL_OK) {
+    // the reserved positions will never be filled: rather than leave every producer and the consumer waiting behind
+    // them, the queue goes into its failed state (every later reserve / pop / read returns DRL_ERR_STATE)
+    traj_queue_fail(q, get_error());
+    return rc;
+  }
+  traj_queue_commit(q, segs);
+  r->t = 0;
+  return DRL_OK;
+}
+
+int recorder_reset(RecorderCore* r) {
+  Lock lk(r->engine->mu);
+  r->t = 0;
   return DRL_OK;
 }
 

@@ -17,6 +17,7 @@
 
 #include "r2d2_defs.cuh"
 #include "replay_core.cuh"
+#include "traj_queue.cuh"
 
 using namespace drl;
 
@@ -236,6 +237,65 @@ int drl_r2d2_replay_add(drl_r2d2_replay* r, drl_r2d2* learner, int32_t n, const 
                            (int)(r->frame / 16))));
   DRL_TRY(replay_launch_update(r, s, n, nullptr, r->cursor, error ? reinterpret_cast<const double*>(d + L.er) : nullptr,
                                error ? nullptr : learner->td_dev));
+  DRL_TRY(replay_end(r, s));
+  replay_advance(r, n);
+  return DRL_OK;
+}
+
+int drl_r2d2_replay_add_from_queue(drl_r2d2_replay* r, drl_r2d2* learner, drl_r2d2_queue* q, int32_t timeout_ms) {
+  DRL_TRY(check_replay(r));
+  if (!q) { set_error("null r2d2 queue handle"); return DRL_ERR_INVALID; }
+  {
+    std::lock_guard<std::recursive_mutex> lk(r->mu);
+    DRL_TRY(check_learner(r, learner));
+    std::lock_guard<std::recursive_mutex> llk(learner->mu);
+    if (q->device != r->device) {
+      set_error("r2d2 replay add_from_queue: the queue is on device %d, the memory on device %d", q->device, r->device);
+      return DRL_ERR_INVALID;
+    }
+    if (q->S != r->S || q->C != r->C || q->A != r->A) {
+      set_error("r2d2 replay add_from_queue: the queue has seq_len %d, %d channels and num_action %d, the memory %d, %d "
+                "and %d", q->S, q->C, q->A, r->S, r->C, r->A);
+      return DRL_ERR_INVALID;
+    }
+    if (q->batch > learner->B) {
+      set_error("r2d2 replay add_from_queue: the queue's batch %d exceeds the learner's batch %d", q->batch, learner->B);
+      return DRL_ERR_INVALID;
+    }
+  }
+  // wait for a full batch without either lock: actor threads sync their engines from this learner meanwhile
+  int qs = 0;
+  std::vector<cudaEvent_t> ev_commit;
+  DRL_TRY(traj_queue_pop(q, timeout_ms, &qs, &ev_commit));
+  std::lock_guard<std::recursive_mutex> lk(r->mu);
+  std::lock_guard<std::recursive_mutex> llk(learner->mu);
+  NvtxRange nv("drl:r2d2_replay_add_from_queue");
+  const int n = q->batch, S = r->S;
+  const cudaStream_t s = learner->compute;
+  // The slot is an R2In of n rows as it is: the learner and the store read it in place.  Unlike drl_r2d2_replay_add,
+  // nothing here checks the actions on the host: the queue's only producers are R2D2 recorders, whose acts check every
+  // previous action and explore action before recording it, so every recorded action and previous action is in [0, A)
+  // (the embedding gathers table + action * 256 without a bounds check).
+  const R2SeqRows rows{q->field(qs, kR2QFrames), reinterpret_cast<int32_t*>(q->field(qs, kR2QPa)),
+                       reinterpret_cast<int32_t*>(q->field(qs, kR2QAction)), reinterpret_cast<float*>(q->field(qs, kR2QH)),
+                       reinterpret_cast<float*>(q->field(qs, kR2QC)), reinterpret_cast<float*>(q->field(qs, kR2QReward)),
+                       q->field(qs, kR2QDone)};
+  const int rc = [&]() -> int {
+    DRL_CUDA_CHECK(cudaSetDevice(r->device));
+    DRL_TRY(replay_begin(r, s));
+    for (cudaEvent_t e : ev_commit) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, e, 0));
+    const R2In in{rows.frames, rows.pa, rows.action, rows.h0, rows.c0, rows.reward, rows.done, nullptr};
+    DRL_TRY(enqueue_forward_td(learner, in, n, false, nullptr, nullptr));
+    learner->last_n = n;
+    prof_mark(s, "replay_store_seq");
+    DRL_CUDA_CHECK((launch_k(replay_store_seq_kernel, dim3(n, S), 256, 0, s, rows, r->cursor, r->capacity, r->mem, S,
+                             (int)(r->frame / 16))));
+    return replay_launch_update(r, s, n, nullptr, r->cursor, nullptr, learner->td_dev);
+  }();
+  // the queue slot goes back to the producers either way (their copies into it wait for its release event)
+  const int rc_release = traj_queue_release(q, qs, s);
+  DRL_TRY(rc);
+  DRL_TRY(rc_release);
   DRL_TRY(replay_end(r, s));
   replay_advance(r, n);
   return DRL_OK;

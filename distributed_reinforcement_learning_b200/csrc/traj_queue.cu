@@ -1,6 +1,7 @@
-// traj_queue.cu -- the device-resident IMPALA trajectory queue behind drl_traj_queue_* (include/drl_b200.h; layout
-// and ordering in traj_queue.cuh).  Producers are policy-engine recorders (policy.cu), the consumer is
-// drl_learner_stage_from_queue (learner.cu); no trajectory byte crosses PCIe except the reward and done of a commit.
+// traj_queue.cu -- the device-resident queues behind drl_traj_queue_* (IMPALA trajectories) and drl_r2d2_queue_* (R2D2
+// sequences) (include/drl_b200.h; layout and ordering in traj_queue.cuh).  Producers are policy-engine recorders
+// (queue_recorder.cuh), the consumers are drl_learner_stage_from_queue (learner.cu) and drl_r2d2_replay_add_from_queue
+// (r2d2_replay.cu); no record byte crosses PCIe except the reward and done of a commit.
 #include <string.h>
 
 #include <algorithm>
@@ -19,12 +20,12 @@ size_t tq_align(size_t v) { return (v + 255) / 256 * 256; }
 
 // every slot the n positions from reserved_total fall in is free for them (held slots and slots still holding an
 // unpopped batch are not)
-bool has_space(const drl_traj_queue* q, int n) {
+bool has_space(const QueueCore* q, int n) {
   long long p = q->reserved_total;
   const long long end = p + n;
   while (p < end) {
     const int slot = (int)((p / q->batch) % q->nslots), row0 = (int)(p % q->batch);
-    const drl_traj_queue::Slot& s = q->st[slot];
+    const QueueCore::Slot& s = q->st[slot];
     if (s.held || s.reserved != row0) return false;
     p += q->batch - row0;
   }
@@ -41,16 +42,82 @@ bool wait_for(std::condition_variable& cv, std::unique_lock<std::mutex>& lk, int
 }
 
 // the caller holds q->mu
-int check_failed(const drl_traj_queue* q) {
+int check_failed(const QueueCore* q) {
   if (!q->failed) return DRL_OK;
-  set_error("trajectory queue is in the failed state: a commit failed after reserving its positions (%s)",
+  set_error("%s is in the failed state: a commit failed after reserving its positions (%s)", q->name,
             q->failure.c_str());
   return DRL_ERR_STATE;
 }
 
 }  // namespace
 
-void traj_queue_fail(drl_traj_queue* q, const char* why) {
+int queue_core_init(QueueCore* q, int nfields, const size_t* sz, int capacity, int batch, int device) {
+  q->nfields = nfields;
+  q->batch = batch;
+  q->device = device;
+  q->nslots = (capacity + batch - 1) / batch + 1;
+  size_t off = 0;
+  for (int f = 0; f < nfields; ++f) {
+    q->sz[f] = sz[f];
+    q->off[f] = off;
+    off = tq_align(off + (size_t)batch * sz[f]);
+  }
+  q->slot_bytes = off;
+  q->st.resize(q->nslots);
+  DRL_CUDA_CHECK(cudaSetDevice(device));
+  DRL_CUDA_CHECK(cudaMalloc((void**)&q->base, q->slot_bytes * q->nslots));
+  DRL_CUDA_CHECK(cudaMemset(q->base, 0, q->slot_bytes * q->nslots));
+  // a slot takes at most `batch` commits (each writes at least one row) before it is popped
+  for (auto& s : q->st) {
+    DRL_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_release, cudaEventDisableTiming));
+    s.ev_commit.assign(batch, nullptr);
+    for (auto& e : s.ev_commit) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  }
+  DRL_CUDA_CHECK(cudaDeviceSynchronize());
+  return DRL_OK;
+}
+
+void queue_core_release(QueueCore* q) {
+  cudaSetDevice(q->device);
+  for (auto& s : q->st) {
+    if (s.ev_release) cudaEventSynchronize(s.ev_release);
+    for (cudaEvent_t e : s.ev_commit) if (e) { cudaEventSynchronize(e); cudaEventDestroy(e); }
+    if (s.ev_release) cudaEventDestroy(s.ev_release);
+  }
+  if (q->base) cudaFree(q->base);
+  cudaGetLastError();
+}
+
+int queue_size(QueueCore* q) {
+  std::lock_guard<std::mutex> lk(q->mu);
+  return (int)(q->committed_total - q->popped_total);
+}
+
+int queue_read(QueueCore* q, int k, void* const* dst) {
+  for (int f = 0; f < q->nfields; ++f)
+    if (!dst[f]) { set_error("%s read: null output pointer", q->name); return DRL_ERR_INVALID; }
+  std::lock_guard<std::mutex> lk(q->mu);
+  DRL_TRY(check_failed(q));
+  const long long size = q->committed_total - q->popped_total;
+  if (k < 0 || k >= size) {
+    set_error("%s read: k = %d is outside [0, %lld) (the queued %s)", q->name, k, size, q->items);
+    return DRL_ERR_INVALID;
+  }
+  const long long p = q->popped_total + k;
+  const int slot = (int)((p / q->batch) % q->nslots), row = (int)(p % q->batch);
+  const QueueCore::Slot& s = q->st[slot];
+  if (s.committed != s.reserved) {
+    set_error("%s read: a commit into slot %d is still in progress", q->name, slot);
+    return DRL_ERR_STATE;
+  }
+  DRL_CUDA_CHECK(cudaSetDevice(q->device));
+  for (int i = 0; i < s.n_commit; ++i) DRL_CUDA_CHECK(cudaEventSynchronize(s.ev_commit[i]));
+  for (int f = 0; f < q->nfields; ++f)
+    DRL_CUDA_CHECK(cudaMemcpy(dst[f], q->field(slot, f) + (size_t)row * q->sz[f], q->sz[f], cudaMemcpyDeviceToHost));
+  return DRL_OK;
+}
+
+void traj_queue_fail(QueueCore* q, const char* why) {
   {
     std::lock_guard<std::mutex> lk(q->mu);
     q->failed = true;
@@ -60,17 +127,17 @@ void traj_queue_fail(drl_traj_queue* q, const char* why) {
   q->cv_ready.notify_all();
 }
 
-int traj_queue_max_rows(const drl_traj_queue* q) { return (q->nslots - 1) * q->batch + 1; }
+int traj_queue_max_rows(const QueueCore* q) { return (q->nslots - 1) * q->batch + 1; }
 
-int traj_queue_reserve(drl_traj_queue* q, int n, int timeout_ms, std::vector<TrajSegment>* segs) {
+int traj_queue_reserve(QueueCore* q, int n, int timeout_ms, std::vector<TrajSegment>* segs) {
   if (n < 1 || n > traj_queue_max_rows(q)) {
-    set_error("trajectory queue: %d rows per commit can never fit (at most %d in this queue: %d slots of %d)", n,
+    set_error("%s: %d rows per commit can never fit (at most %d in this queue: %d slots of %d)", q->name, n,
               traj_queue_max_rows(q), q->nslots, q->batch);
     return DRL_ERR_INVALID;
   }
   std::unique_lock<std::mutex> lk(q->mu);
   if (!wait_for(q->cv_space, lk, timeout_ms, [&] { return q->failed || has_space(q, n); })) {
-    set_error("trajectory queue commit: timed out (queue full)");
+    set_error("%s commit: timed out (queue full)", q->name);
     return DRL_ERR_TIMEOUT;
   }
   DRL_TRY(check_failed(q));
@@ -80,7 +147,7 @@ int traj_queue_reserve(drl_traj_queue* q, int n, int timeout_ms, std::vector<Tra
   while (src < n) {
     const int slot = (int)((p / q->batch) % q->nslots), row0 = (int)(p % q->batch);
     const int rows = std::min(q->batch - row0, n - src);
-    drl_traj_queue::Slot& s = q->st[slot];
+    QueueCore::Slot& s = q->st[slot];
     segs->push_back(TrajSegment{slot, row0, rows, src, s.ev_commit[s.n_commit], s.ev_release});
     s.n_commit++;
     s.reserved += rows;
@@ -91,11 +158,11 @@ int traj_queue_reserve(drl_traj_queue* q, int n, int timeout_ms, std::vector<Tra
   return DRL_OK;
 }
 
-void traj_queue_commit(drl_traj_queue* q, const std::vector<TrajSegment>& segs) {
+void traj_queue_commit(QueueCore* q, const std::vector<TrajSegment>& segs) {
   std::lock_guard<std::mutex> lk(q->mu);
   bool ready = false;
   for (const TrajSegment& g : segs) {
-    drl_traj_queue::Slot& s = q->st[g.slot];
+    QueueCore::Slot& s = q->st[g.slot];
     s.committed += g.rows;
     q->committed_total += g.rows;
     ready = ready || s.committed == q->batch;
@@ -103,42 +170,69 @@ void traj_queue_commit(drl_traj_queue* q, const std::vector<TrajSegment>& segs) 
   if (ready) q->cv_ready.notify_all();
 }
 
-int traj_queue_pop(drl_traj_queue* q, int timeout_ms, int* slot, std::vector<cudaEvent_t>* ev_commit) {
+int traj_queue_pop(QueueCore* q, int timeout_ms, int* slot, std::vector<cudaEvent_t>* ev_commit) {
   std::unique_lock<std::mutex> lk(q->mu);
   auto head = [&] { return (int)((q->popped_total / q->batch) % q->nslots); };
   auto ready = [&] {
-    const drl_traj_queue::Slot& s = q->st[head()];
+    const QueueCore::Slot& s = q->st[head()];
     return !s.held && s.committed == q->batch;
   };
   if (!wait_for(q->cv_ready, lk, timeout_ms, [&] { return q->failed || ready(); })) {
-    set_error("trajectory queue stage: timed out (fewer than batch trajectories queued)");
+    set_error("%s %s: timed out (fewer than batch %s queued)", q->name, q->pop_verb, q->items);
     return DRL_ERR_TIMEOUT;
   }
   DRL_TRY(check_failed(q));
   *slot = head();
-  drl_traj_queue::Slot& s = q->st[*slot];
+  QueueCore::Slot& s = q->st[*slot];
   s.held = true;
   ev_commit->assign(s.ev_commit.begin(), s.ev_commit.begin() + s.n_commit);
   q->popped_total += q->batch;
   return DRL_OK;
 }
 
-int traj_queue_release(drl_traj_queue* q, int slot, cudaStream_t s) {
+int traj_queue_release(QueueCore* q, int slot, cudaStream_t s) {
   const cudaError_t e = cudaEventRecord(q->st[slot].ev_release, s);
   {
     std::lock_guard<std::mutex> lk(q->mu);
-    drl_traj_queue::Slot& st = q->st[slot];
+    QueueCore::Slot& st = q->st[slot];
     st.held = false;
     st.reserved = 0;
     st.committed = 0;
     st.n_commit = 0;
   }
   q->cv_space.notify_all();
-  if (e != cudaSuccess) { set_error("trajectory queue release: %s", cudaGetErrorString(e)); return DRL_ERR_CUDA; }
+  if (e != cudaSuccess) { set_error("%s release: %s", q->name, cudaGetErrorString(e)); return DRL_ERR_CUDA; }
   return DRL_OK;
 }
 
 }  // namespace drl
+
+namespace {
+
+// create's tail shared by both families: the core's slots, or the handle released with the error message kept
+template <class Q>
+int finish_create(Q* q, int nfields, const size_t* sz, int capacity, int batch, int device, Q** out,
+                  int (*destroy)(Q*)) {
+  const int rc = queue_core_init(q, nfields, sz, capacity, batch, device);
+  if (rc != DRL_OK) {
+    const std::string keep = get_error();
+    destroy(q);
+    set_error("%s", keep.c_str());
+    return rc;
+  }
+  *out = q;
+  return DRL_OK;
+}
+
+int check_queue_device(int device) {
+  if (drl_device_count() <= device || device < 0) {
+    set_error("CUDA device %d not available (no CPU fallback)", device);
+    return DRL_ERR_CUDA;
+  }
+  return DRL_OK;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -151,100 +245,86 @@ int drl_traj_queue_create(int32_t trajectory, int32_t height, int32_t width, int
     set_error("trajectory queue: invalid dimensions (capacity must be >= batch)");
     return DRL_ERR_INVALID;
   }
-  if (drl_device_count() <= device || device < 0) {
-    set_error("CUDA device %d not available (no CPU fallback)", device);
-    return DRL_ERR_CUDA;
-  }
+  DRL_TRY(check_queue_device(device));
   drl_traj_queue* q = new drl_traj_queue();
+  q->name = "trajectory queue";
+  q->pop_verb = "stage";
+  q->items = "trajectories";
   q->T = trajectory; q->H = height; q->W = width; q->C = channels; q->A = num_action; q->L = lstm_size;
-  q->batch = batch;
-  q->device = device;
-  q->nslots = (capacity + batch - 1) / batch + 1;
   const size_t T = trajectory;
-  q->sz[kTrajState] = T * height * width * channels;
-  q->sz[kTrajReward] = T * 4;
-  q->sz[kTrajDone] = T;
-  q->sz[kTrajMu] = T * num_action * 4;
-  q->sz[kTrajAction] = T * 4;
-  q->sz[kTrajPa] = T * 4;
-  q->sz[kTrajH] = T * lstm_size * 4;
-  q->sz[kTrajC] = T * lstm_size * 4;
-  size_t off = 0;
-  for (int f = 0; f < kTrajFields; ++f) {
-    q->off[f] = off;
-    off = tq_align(off + (size_t)batch * q->sz[f]);
-  }
-  q->slot_bytes = off;
-  q->st.resize(q->nslots);
-  const int rc = [&]() -> int {
-    DRL_CUDA_CHECK(cudaSetDevice(device));
-    DRL_CUDA_CHECK(cudaMalloc((void**)&q->base, q->slot_bytes * q->nslots));
-    DRL_CUDA_CHECK(cudaMemset(q->base, 0, q->slot_bytes * q->nslots));
-    // a slot takes at most `batch` commits (each writes at least one row) before it is popped
-    for (auto& s : q->st) {
-      DRL_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_release, cudaEventDisableTiming));
-      s.ev_commit.assign(batch, nullptr);
-      for (auto& e : s.ev_commit) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
-    DRL_CUDA_CHECK(cudaDeviceSynchronize());
-    return DRL_OK;
-  }();
-  if (rc != DRL_OK) {
-    const std::string keep = get_error();
-    drl_traj_queue_destroy(q);
-    set_error("%s", keep.c_str());
-    return rc;
-  }
-  *out = q;
-  return DRL_OK;
+  size_t sz[kTrajFields];
+  sz[kTrajState] = T * height * width * channels;
+  sz[kTrajReward] = T * 4;
+  sz[kTrajDone] = T;
+  sz[kTrajMu] = T * num_action * 4;
+  sz[kTrajAction] = T * 4;
+  sz[kTrajPa] = T * 4;
+  sz[kTrajH] = T * lstm_size * 4;
+  sz[kTrajC] = T * lstm_size * 4;
+  return finish_create(q, kTrajFields, sz, capacity, batch, device, out, drl_traj_queue_destroy);
 }
 
 int drl_traj_queue_destroy(drl_traj_queue* q) {
   if (!q) return DRL_OK;
-  cudaSetDevice(q->device);
-  for (auto& s : q->st) {
-    if (s.ev_release) cudaEventSynchronize(s.ev_release);
-    for (cudaEvent_t e : s.ev_commit) if (e) { cudaEventSynchronize(e); cudaEventDestroy(e); }
-    if (s.ev_release) cudaEventDestroy(s.ev_release);
-  }
-  if (q->base) cudaFree(q->base);
-  cudaGetLastError();
+  queue_core_release(q);
   delete q;
   return DRL_OK;
 }
 
-int drl_traj_queue_size(drl_traj_queue* q) {
-  if (!q) return 0;
-  std::lock_guard<std::mutex> lk(q->mu);
-  return (int)(q->committed_total - q->popped_total);
-}
+int drl_traj_queue_size(drl_traj_queue* q) { return q ? queue_size(q) : 0; }
 
 int drl_traj_queue_read(drl_traj_queue* q, int32_t k, uint8_t* state, float* reward, uint8_t* done,
                         float* behavior_policy, int32_t* action, int32_t* previous_action, float* previous_h,
                         float* previous_c) {
   if (!q) { set_error("null trajectory queue handle"); return DRL_ERR_INVALID; }
-  void* dst[kTrajFields] = {state, reward, done, behavior_policy, action, previous_action, previous_h, previous_c};
-  for (void* p : dst)
-    if (!p) { set_error("trajectory queue read: null output pointer"); return DRL_ERR_INVALID; }
-  std::lock_guard<std::mutex> lk(q->mu);
-  DRL_TRY(check_failed(q));
-  const long long size = q->committed_total - q->popped_total;
-  if (k < 0 || k >= size) {
-    set_error("trajectory queue read: k = %d is outside [0, %lld) (the queued trajectories)", k, size);
+  void* const dst[kTrajFields] = {state, reward, done, behavior_policy, action, previous_action, previous_h, previous_c};
+  return queue_read(q, k, dst);
+}
+
+int drl_r2d2_queue_create(int32_t seq_len, int32_t channels, int32_t num_action, int32_t capacity, int32_t batch,
+                          int32_t device, drl_r2d2_queue** out) {
+  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
+  *out = nullptr;
+  if (seq_len < 2) { set_error("r2d2 queue: seq_len must be >= 2 (got %d)", seq_len); return DRL_ERR_INVALID; }
+  if (channels != 1 && channels != 4) { set_error("r2d2 queue: channels must be 1 or 4 (got %d)", channels); return DRL_ERR_INVALID; }
+  if (num_action < 2 || num_action > 32) { set_error("r2d2 queue: num_action must be in [2, 32] (got %d)", num_action); return DRL_ERR_INVALID; }
+  if (batch < 1 || capacity < batch) {
+    set_error("r2d2 queue: invalid dimensions (batch must be >= 1 and capacity >= batch; got %d, %d)", batch, capacity);
     return DRL_ERR_INVALID;
   }
-  const long long p = q->popped_total + k;
-  const int slot = (int)((p / q->batch) % q->nslots), row = (int)(p % q->batch);
-  const drl_traj_queue::Slot& s = q->st[slot];
-  if (s.committed != s.reserved) {
-    set_error("trajectory queue read: a commit into slot %d is still in progress", slot);
-    return DRL_ERR_STATE;
-  }
-  DRL_CUDA_CHECK(cudaSetDevice(q->device));
-  for (int i = 0; i < s.n_commit; ++i) DRL_CUDA_CHECK(cudaEventSynchronize(s.ev_commit[i]));
-  for (int f = 0; f < kTrajFields; ++f)
-    DRL_CUDA_CHECK(cudaMemcpy(dst[f], q->field(slot, f) + (size_t)row * q->sz[f], q->sz[f], cudaMemcpyDeviceToHost));
+  DRL_TRY(check_queue_device(device));
+  drl_r2d2_queue* q = new drl_r2d2_queue();
+  q->name = "r2d2 queue";
+  q->pop_verb = "add_from_queue";
+  q->items = "sequences";
+  q->S = seq_len; q->C = channels; q->A = num_action;
+  q->frame = (size_t)Geo::IH * Geo::IW * channels;
+  const size_t S = seq_len, L = 64;   // L: the R2D2 network's lstm_size (kR2L)
+  size_t sz[kR2QFields];
+  sz[kR2QFrames] = S * q->frame;
+  sz[kR2QPa] = S * 4;
+  sz[kR2QAction] = S * 4;
+  sz[kR2QH] = L * 4;
+  sz[kR2QC] = L * 4;
+  sz[kR2QReward] = S * 4;
+  sz[kR2QDone] = S;
+  return finish_create(q, kR2QFields, sz, capacity, batch, device, out, drl_r2d2_queue_destroy);
+}
+
+int drl_r2d2_queue_destroy(drl_r2d2_queue* q) {
+  if (!q) return DRL_OK;
+  queue_core_release(q);
+  delete q;
   return DRL_OK;
+}
+
+int drl_r2d2_queue_size(drl_r2d2_queue* q) { return q ? queue_size(q) : 0; }
+
+int drl_r2d2_queue_read(drl_r2d2_queue* q, int32_t k, uint8_t* state, int32_t* previous_action, int32_t* action,
+                        float* previous_h, float* previous_c, float* reward, uint8_t* done) {
+  if (!q) { set_error("null r2d2 queue handle"); return DRL_ERR_INVALID; }
+  void* const dst[kR2QFields] = {state, previous_action, action, previous_h, previous_c, reward, done};
+  return queue_read(q, k, dst);
 }
 
 }  // extern "C"

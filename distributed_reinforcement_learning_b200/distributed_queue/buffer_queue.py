@@ -1,6 +1,7 @@
 """H100-native stand-ins for ``distributed_queue/buffer_queue.py``: ``FIFOQueue`` (reference :418-512, the IMPALA
 trajectory queue; ``DeviceFIFOQueue`` keeps it in GPU memory) and ``SumTree`` / ``Memory`` (reference :326-416, the
-Ape-X prioritized replay memory).
+Ape-X prioritized replay memory), and the other launchers' record queues (``R2D2FIFOQueue``; ``R2D2DeviceFIFOQueue``
+keeps it in GPU memory).
 
 The reference keeps a ``tf.FIFOQueue`` of 9-field trajectories on the learner's CPU and dequeues a
 batch with ``batch_size`` serial ``sess.run`` RPCs, after which the launcher ``np.stack``s eight
@@ -384,6 +385,71 @@ class R2D2FIFOQueue(_QueueBase):
 
     def sample_batch(self, timeout=None):
         return self._q.get_many(self.batch_size, timeout)
+
+
+class R2D2DeviceFIFOQueue:
+    """``R2D2FIFOQueue`` with its batch slots in GPU memory (``drl_r2d2_queue_*``, DESIGN.md section 13).
+
+    Producers are R2D2 policy-engine recorders (``NativeR2D2Policy.recorder``): each act writes its step of every
+    sequence on the device, and a commit moves whole sequences into the queue with device-to-device copies; only reward
+    and done cross PCIe.  The consumer is ``r2d2.DeviceMemory.add_from_queue``, which ingests the oldest batch into the
+    device replay memory straight from the queue.  Same constructor arguments as ``R2D2FIFOQueue`` plus ``device``;
+    ``get_size`` counts committed and not yet ingested sequences.  A record keeps step 0 of the stored (h, c) only, as
+    the replay memory does.  There is no host producer (``append_to_queue``) and no host read of a batch
+    (``sample_batch``); ``read(k)`` copies one queued sequence out, for tests."""
+
+    def __init__(self, seq_len, input_shape, output_size, queue_size, batch_size, num_actors, lstm_size, device=0):
+        self.seq_len = int(seq_len)
+        self.input_shape = tuple(int(x) for x in input_shape)
+        if len(self.input_shape) != 3 or self.input_shape[:2] != (84, 84):
+            raise ValueError("input_shape: expected (84, 84, channels), got %s" % (self.input_shape,))
+        self.output_size = int(output_size)
+        self.batch_size = int(batch_size)
+        self.lstm_size = int(lstm_size)
+        if self.lstm_size != 64:
+            raise ValueError("lstm_size: only 64 is supported (the R2D2 network's), got %d" % self.lstm_size)
+        self.queue_size = int(queue_size)
+        self.num_actors = num_actors
+        self.device = int(device)
+        self.sess = None
+        # batch slots as the ring rounds them; one commit of n rows may span slots, so at most max_rows fit at once
+        nslots = -(-max(self.queue_size, self.batch_size) // self.batch_size) + 1
+        self.max_rows = (nslots - 1) * self.batch_size + 1
+        self._q = C.c_void_p()
+        N.check(N.lib.drl_r2d2_queue_create(self.seq_len, self.input_shape[2], self.output_size,
+                                            max(self.queue_size, self.batch_size), self.batch_size, self.device,
+                                            C.byref(self._q)))
+
+    def close(self):
+        if getattr(self, "_q", None) is not None and self._q.value:
+            N.lib.drl_r2d2_queue_destroy(self._q)
+            self._q = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def get_size(self):
+        """Sequences committed and not yet ingested."""
+        return int(N.lib.drl_r2d2_queue_size(self._q))
+
+    def set_session(self, sess):
+        """Kept for call compatibility; there is no session."""
+        self.sess = sess
+
+    def read(self, k):
+        """The k-th queued sequence (0 = the next one ingested), copied to the host: a dict of state, previous_action,
+        action, reward, done, previous_h, previous_c.  Unlike an ``R2D2FIFOQueue`` record, previous_h and previous_c
+        are step 0 only: [lstm_size], not [seq_len, lstm_size]."""
+        S, L = self.seq_len, self.lstm_size
+        out = dict(state=np.empty((S,) + self.input_shape, np.uint8), previous_action=np.empty(S, np.int32),
+                   action=np.empty(S, np.int32), previous_h=np.empty(L, np.float32),
+                   previous_c=np.empty(L, np.float32), reward=np.empty(S, np.float32), done=np.empty(S, np.uint8))
+        N.check(N.lib.drl_r2d2_queue_read(self._q, int(k), *[N.ptr(a) for a in out.values()]))
+        out["done"] = out["done"].view(np.bool_)
+        return {f: out[f] for f in R2D2FIFOQueue._FIELDS}
 
 
 class A3CFIFOQueue(_QueueBase):

@@ -9,12 +9,10 @@ learner.  It owns no optimizer state, gradients or backward buffers.
 act that also writes the step's frames, previous actions, h, c, policies and actions into device staging, and its
 ``commit`` moves the n recorded trajectories into the queue without copying them through the host.
 """
-import ctypes as C
-
 import numpy as np
 
 from . import _native as N
-from .policy_handle import MAX_BATCH, PolicyHandle  # noqa: F401  (MAX_BATCH: rows per call)
+from .policy_handle import MAX_BATCH, PolicyHandle, RecorderHandle  # noqa: F401  (MAX_BATCH: rows per call)
 
 
 class NativePolicy(PolicyHandle):
@@ -31,14 +29,6 @@ class NativePolicy(PolicyHandle):
     def _learner_type(self):
         from .learner import NativeLearner
         return NativeLearner
-
-    def close(self):
-        # recorders first: a recorder's handle refers to this engine (the garbage collector may finalize the two in
-        # either order, so the engine owns the recorders' handle boxes, not the recorders)
-        for r in getattr(self, "_recorder_handles", ()):
-            _destroy_recorder(r)
-        self._recorder_handles = []
-        super().close()
 
     def recorder(self, queue, n):
         """A ``PolicyRecorder`` of n rows (n <= max_batch) into ``queue`` (a ``DeviceFIFOQueue`` on this device)."""
@@ -73,13 +63,7 @@ class NativePolicy(PolicyHandle):
         return self._act_result(outs)
 
 
-def _destroy_recorder(handle):
-    if handle.value:
-        N.lib.drl_policy_recorder_destroy(handle)
-        handle.value = None
-
-
-class PolicyRecorder:
+class PolicyRecorder(RecorderHandle):
     """Records n rows of a ``NativePolicy``'s acts as trajectories of ``queue.trajectory`` steps, on the device.
 
     ``act`` has ``NativePolicy.act``'s signature and return value; call it for steps t = 0 .. T-1 with exactly n rows,
@@ -91,41 +75,11 @@ class PolicyRecorder:
 
     def __init__(self, policy, queue, n):
         from .distributed_queue.buffer_queue import DeviceFIFOQueue
-        if not isinstance(queue, DeviceFIFOQueue):
-            raise TypeError("recorder: queue must be a DeviceFIFOQueue, got %s" % type(queue).__name__)
-        n = int(n)
-        if not 1 <= n <= policy.max_batch:
-            raise ValueError("recorder: n = %d rows, the policy serves 1..%d" % (n, policy.max_batch))
-        self.policy, self.queue, self.n, self.T = policy, queue, n, queue.trajectory
-        self._r = C.c_void_p()
-        N.check(N.lib.drl_policy_recorder_create(policy._h, queue._q, n, C.byref(self._r)))
-        live = [r for r in getattr(policy, "_recorder_handles", ()) if r.value]
-        policy._recorder_handles = live + [self._r]
-
-    def close(self):
-        if getattr(self, "_r", None) is not None:
-            _destroy_recorder(self._r)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._bind(policy, queue, DeviceFIFOQueue, n, getattr(queue, "trajectory", 0))
 
     def act(self, state, previous_action, h, c, uniform=None):
         """``NativePolicy.act`` of the recorder's n rows, recorded as the next step of the unroll."""
         n, ins, outs = self.policy._act_args(state, previous_action, h, c, uniform)
-        if n != self.n:
-            raise ValueError("recorder act: %d rows, the recorder records %d" % (n, self.n))
+        self._check_rows(n)
         N.check(N.lib.drl_policy_recorder_act(self._r, *[N.ptr(a) for a in ins + outs]))
         return self.policy._act_result(outs)
-
-    def reset(self):
-        """Discard the steps recorded since the last commit (an unroll abandoned half-way); the next act is step 0."""
-        N.check(N.lib.drl_policy_recorder_reset(self._r))
-
-    def commit(self, reward, done, timeout_ms=-1):
-        """Moves the n recorded trajectories into the queue; reward float32 [n, T], done bool / uint8 [n, T]."""
-        rw = N.as_c(reward, np.float32, (self.n, self.T), "reward")
-        dn = N.as_c(N.as_u8(done), np.uint8, (self.n, self.T), "done")
-        N.check(N.lib.drl_policy_recorder_commit(self._r, N.ptr(rw), N.ptr(dn), int(timeout_ms)))

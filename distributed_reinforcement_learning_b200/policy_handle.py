@@ -1,6 +1,6 @@
 """The part of the IMPALA, R2D2 and Ape-X / A3C policy-engine wrappers that is the same for all three: each drives one
 ``drl_<prefix>_*`` policy handle of the C-ABI (include/drl_b200.h), and these entry points differ only in that
-prefix."""
+prefix.  ``RecorderHandle`` is the same for the recorders of the IMPALA and R2D2 engines (``drl_<prefix>_recorder_*``)."""
 import ctypes as C
 
 import numpy as np
@@ -37,6 +37,11 @@ class PolicyHandle:
 
     # ---- lifetime ----------------------------------------------------------------
     def close(self):
+        # recorders first: a recorder's handle refers to this engine (the garbage collector may finalize the two in
+        # either order, so the engine owns the recorders' handle boxes, not the recorders)
+        for r in getattr(self, "_recorder_handles", ()):
+            _destroy_recorder(self.prefix, r)
+        self._recorder_handles = []
         if getattr(self, "_h", None) is not None and self._h.value:
             self._fn("destroy")(self._h)
             self._h = C.c_void_p()
@@ -113,3 +118,54 @@ class PolicyHandle:
         if ex.min() < -1 or ex.max() >= self.A:
             raise ValueError("explore_action: values must lie in [-1, %d)" % self.A)
         return ex
+
+
+def _destroy_recorder(prefix, handle):
+    if handle.value:
+        getattr(N.lib, "drl_%s_recorder_destroy" % prefix)(handle)
+        handle.value = None
+
+
+class RecorderHandle:
+    """A ``drl_<prefix>_recorder_*`` handle that binds one policy engine to one device queue for n rows.  The family's
+    class binds it (``_bind``) and implements ``act``."""
+
+    def _bind(self, policy, queue, queue_type, n, T):
+        """queue must be a ``queue_type``; T: its steps per record."""
+        if not isinstance(queue, queue_type):
+            raise TypeError("recorder: queue must be a %s, got %s" % (queue_type.__name__, type(queue).__name__))
+        n = int(n)
+        if not 1 <= n <= policy.max_batch:
+            raise ValueError("recorder: n = %d rows, the policy serves 1..%d" % (n, policy.max_batch))
+        self.policy, self.queue, self.n, self.T = policy, queue, n, int(T)
+        self._r = C.c_void_p()
+        N.check(policy._fn("recorder_create")(policy._h, queue._q, n, C.byref(self._r)))
+        live = [r for r in getattr(policy, "_recorder_handles", ()) if r.value]
+        policy._recorder_handles = live + [self._r]
+
+    def _rfn(self, name):
+        return self.policy._fn("recorder_" + name)
+
+    def close(self):
+        if getattr(self, "_r", None) is not None:
+            _destroy_recorder(self.policy.prefix, self._r)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _check_rows(self, n):
+        if n != self.n:
+            raise ValueError("recorder act: %d rows, the recorder records %d" % (n, self.n))
+
+    def reset(self):
+        """Discard the steps recorded since the last commit (an unroll abandoned half-way); the next act is step 0."""
+        N.check(self._rfn("reset")(self._r))
+
+    def commit(self, reward, done, timeout_ms=-1):
+        """Moves the n recorded records into the queue; reward float32 [n, T], done bool / uint8 [n, T]."""
+        rw = N.as_c(reward, np.float32, (self.n, self.T), "reward")
+        dn = N.as_c(N.as_u8(done), np.uint8, (self.n, self.T), "done")
+        N.check(self._rfn("commit")(self._r, N.ptr(rw), N.ptr(dn), int(timeout_ms)))

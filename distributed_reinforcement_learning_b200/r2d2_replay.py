@@ -76,6 +76,15 @@ class NativeR2D2Replay:
         N.check(N.lib.drl_r2d2_replay_add(self._h, learner._h if learner is not None else None, n,
                                           *[N.ptr(a) for a in arrs], N.ptr(err) if err is not None else None))
 
+    def add_from_queue(self, learner, queue, timeout_ms=-1):
+        """``add`` of the oldest full batch of an ``R2D2DeviceFIFOQueue`` with ``learner``'s |td| as the priorities,
+        read straight from the queue's GPU memory (queue.batch_size <= learner.B).  Blocks while fewer than a batch
+        of sequences are queued; ``timeout_ms`` >= 0 raises ``TimeoutError_`` with nothing changed."""
+        from .distributed_queue.buffer_queue import R2D2DeviceFIFOQueue
+        if not isinstance(queue, R2D2DeviceFIFOQueue):
+            raise TypeError("add_from_queue: queue must be an R2D2DeviceFIFOQueue, got %s" % type(queue).__name__)
+        N.check(N.lib.drl_r2d2_replay_add_from_queue(self._h, learner._h, queue._q, int(timeout_ms)))
+
     def step_async(self, learner, slot, u01):
         """Sample learner.B draws with the uniforms ``u01`` -> gather into ``slot`` -> learner step -> priority update.
         ``learner.wait()`` returns (scalars, td_error) afterwards."""

@@ -304,6 +304,52 @@ int drl_r2d2_policy_act(drl_r2d2_policy* h, int32_t n, const uint8_t* state, con
 int drl_r2d2_policy_last_act_ms(drl_r2d2_policy* h, float* ms);
 
 /* ------------------------------------------------------------------------------------------
+ * Device R2D2 sequence queue (new): R2D2FIFOQueue with its batch slots in GPU memory.  Producers are R2D2 policy
+ * recorders (drl_r2d2_policy_recorder_commit), the consumer is drl_r2d2_replay_add_from_queue; a sequence never passes
+ * through the host except its reward and done.  A record is one stored-state sequence in the replay memory's row layout:
+ * state u8 [S,84,84,C], previous_action i32 [S], action i32 [S], h0 f32 [64], c0 f32 [64], reward f32 [S], done u8 [S]
+ * (106,547 B at S = 15, C = 1).  Like the replay memory, it keeps only step 0 of the stored (h, c), the only step the
+ * learner reads.  A slot holds `batch` sequences field-major, each field batch-major, so a slot is a learner minibatch
+ * as it is.  capacity is rounded up as the ring's, plus one slot (9 slots, 15.3 MB at S = 15, C = 1, capacity 128,
+ * batch 16).  Thread-safe: several recorders may commit while one learner thread ingests.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_r2d2_queue drl_r2d2_queue;
+/* seq_len >= 2, channels 1 or 4, num_action in [2, 32] (DRL_ERR_INVALID otherwise, checked first), 1 <= batch <=
+ * capacity; DRL_ERR_CUDA ("no CPU fallback") when `device` does not exist. */
+int drl_r2d2_queue_create(int32_t seq_len, int32_t channels, int32_t num_action, int32_t capacity, int32_t batch,
+                          int32_t device, drl_r2d2_queue** out);
+int drl_r2d2_queue_destroy(drl_r2d2_queue* q);
+/* sequences committed and not yet popped */
+int drl_r2d2_queue_size(drl_r2d2_queue* q);
+/* Synchronous copy of the k-th queued sequence (0 = the next to be popped) into host arrays; for tests.  previous_h
+ * and previous_c are step 0 only, f32 [64] (an R2D2FIFOQueue record holds [S, 64]).  DRL_ERR_INVALID for k outside
+ * [0, size), DRL_ERR_STATE while a commit into its slot is in progress. */
+int drl_r2d2_queue_read(drl_r2d2_queue* q, int32_t k, uint8_t* state, int32_t* previous_action, int32_t* action,
+                        float* previous_h, float* previous_c, float* reward, uint8_t* done);
+
+/* R2D2 recorder: binds an R2D2 engine to a device R2D2 queue for n <= max_batch rows, with device staging of n
+ * sequences (4.3 MB at n = 40, S = 15, C = 1).  Queue and engine must be on the same device with the same num_action
+ * and channels, and n must fit the queue at once; all DRL_ERR_INVALID otherwise.  Without a device, DRL_ERR_CUDA.
+ * Destroy the recorder before its engine and queue. */
+typedef struct drl_r2d2_policy_recorder drl_r2d2_policy_recorder;
+int drl_r2d2_policy_recorder_create(drl_r2d2_policy* h, drl_r2d2_queue* queue, int32_t n,
+                                    drl_r2d2_policy_recorder** out);
+int drl_r2d2_policy_recorder_destroy(drl_r2d2_policy_recorder* r);
+/* drl_r2d2_policy_act of the recorder's n rows (same inputs, checks, outputs and results) that also records step t of
+ * rows 0..n-1 on the device: the frame and previous action given, the action chosen, and at t = 0 h_in and c_in.
+ * Steps are recorded in order t = 0..S-1; an act after step S-1 is DRL_ERR_STATE until the commit.  With use_cuda_graph
+ * one graph per recorder replays every step.  drl_r2d2_policy_recorder_reset discards the steps recorded since the
+ * last commit. */
+int drl_r2d2_policy_recorder_act(drl_r2d2_policy_recorder* r, const uint8_t* state, const int32_t* previous_action,
+                                 const float* h_in, const float* c_in, const int32_t* explore_action, int32_t* action,
+                                 float* q, float* q_action, float* h_out, float* c_out);
+int drl_r2d2_policy_recorder_reset(drl_r2d2_policy_recorder* r);
+/* After step S-1 (DRL_ERR_STATE otherwise): reward f32 [n,S] and done u8 [n,S] complete the n sequences, which are
+ * appended to the queue in row order; otherwise as drl_policy_recorder_commit. */
+int drl_r2d2_policy_recorder_commit(drl_r2d2_policy_recorder* r, const float* reward, const uint8_t* done,
+                                    int32_t timeout_ms);
+
+/* ------------------------------------------------------------------------------------------
  * Ape-X / A3C policy engine (new): the actor side of train_apex.py:157-231 and train_a3c.py:112-183 (the actor loops
  * themselves are distributed_reinforcement_learning_b200/actor.py: ApexVectorActor, A3CVectorActor).  A forward-only
  * handle that serves the family's get_policy_and_action (agent/apex.py:88-102, agent/a3c.py:109-119) for up to 64
@@ -721,6 +767,13 @@ int drl_r2d2_replay_add(drl_r2d2_replay* r, drl_r2d2* learner, int32_t n, const 
 /* Memory.sample(B) with the caller's uniforms u01 [B] (B = the learner's batch) -> gather into staging slot `slot` ->
  * the learner's step on that slot -> Memory.update of the sampled leaves with the step's |td|.  Asynchronous:
  * drl_r2d2_wait returns the loss and the priorities once the update has run.  DRL_ERR_STATE on an empty memory. */
+/* drl_r2d2_replay_add of the oldest full batch of a device R2D2 queue (train_r2d2.py:97-120 without a host copy): pops it
+ * without holding the memory's or the learner's lock, blocking while fewer than batch sequences are queued
+ * (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with nothing changed otherwise), then, on the learner's compute stream, the
+ * learner's |td| of the batch read from the queue slot, the store and the priority update; the slot goes back to the
+ * producers after them, also when enqueueing fails.  The queue's seq_len, channels, num_action and device must be the
+ * memory's and its batch at most the learner's (DRL_ERR_INVALID).  Does not wait for the learner's compute stream. */
+int drl_r2d2_replay_add_from_queue(drl_r2d2_replay* r, drl_r2d2* learner, drl_r2d2_queue* queue, int32_t timeout_ms);
 int drl_r2d2_replay_step_async(drl_r2d2_replay* r, drl_r2d2* learner, int32_t slot, const double* u01);
 /* As drl_apex_replay_sample / _update / _last_sample. */
 int drl_r2d2_replay_sample(drl_r2d2_replay* r, int32_t n, const double* u01, int64_t* tree_index,
