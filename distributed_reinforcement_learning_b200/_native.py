@@ -285,6 +285,17 @@ def _load():
         "drl_apex_replay_total": (C.c_int, [vp, C.POINTER(C.c_double)]),
         "drl_apex_replay_size": (C.c_int, [vp, C.POINTER(i64)]),
         "drl_apex_replay_beta": (C.c_int, [vp, C.POINTER(C.c_double)]),
+        "drl_apex_replay_add_from_queue": (C.c_int, [vp, vp, vp, i32]),
+        "drl_apex_queue_create": (C.c_int, [i32] * 4 + [C.POINTER(vp)]),
+        "drl_apex_queue_destroy": (C.c_int, [vp]),
+        "drl_apex_queue_size": (C.c_int, [vp]),
+        "drl_apex_queue_read": (C.c_int, [vp, i32] + [vp] * 6),
+        "drl_apex_actor_buffer_create": (C.c_int, [i32] * 4 + [C.POINTER(vp)]),
+        "drl_apex_actor_buffer_destroy": (C.c_int, [vp]),
+        "drl_apex_actor_buffer_append": (C.c_int, [vp, i32] + [vp] * 6),
+        "drl_apex_actor_buffer_push": (C.c_int, [vp, vp, i32, vp, i32]),
+        "drl_apex_actor_buffer_size": (C.c_int, [vp, C.POINTER(i64)]),
+        "drl_apex_actor_buffer_read": (C.c_int, [vp, i32, i64] + [vp] * 6),
         "drl_r2d2_replay_create": (C.c_int, [i32, i64, i32, i32, i32, C.POINTER(vp)]),
         "drl_r2d2_replay_destroy": (C.c_int, [vp]),
         "drl_r2d2_replay_add": (C.c_int, [vp, vp, i32] + [vp] * 8),

@@ -268,7 +268,11 @@ class ApexVectorActor:
         0..n-1 from the global ``np.random`` stream, in that order; then, environment by environment, ``env.step`` with
         ``action % available_action[i]`` (the buffer stores the raw action), the append to its ``LocalBuffer(1e4)``
         and, once the buffer holds more than 3 ``trajectory`` transitions, a ``sample(trajectory)`` (a
-        ``np.random.permutation`` draw) pushed to ``queue.append_to_queue(task=i, ...)`` -- every step from then on;
+        ``np.random.permutation`` draw) pushed to ``queue.append_to_queue(task=i, ...)`` -- every step from then on.
+        With an ``ApexDeviceFIFOQueue`` the buffers are one ``DeviceLocalBuffers`` on the GPU instead: the
+        environment loop makes the same draws at the same points, and after it one ``append`` of all n rows and one
+        ``push`` per draw, in environment order, fill the queue on the device with the same records (only the moment
+        a full queue blocks moves to after the environment loop);
       - a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True; the score keeps the raw
         reward; ``lives`` follows ``info['ale.lives']`` after every step;
       - at an episode's end epsilon becomes 1 / (0.05 episode + 1), and the environment, the previous action and
@@ -286,7 +290,13 @@ class ApexVectorActor:
             raise ValueError("%d environments, the policy serves 1..%d per call" % (n, policy.max_batch))
         if len(self.available_action) != n:
             raise ValueError("available_action has %d entries for %d environments" % (len(self.available_action), n))
-        self.buffers = [buffer_queue.LocalBuffer(capacity=buffer_capacity) for _ in range(n)]
+        self.device_buffers = None
+        if isinstance(queue, buffer_queue.ApexDeviceFIFOQueue):
+            self._check_device_queue(queue)
+            self.buffers = None
+            self.device_buffers = buffer_queue.DeviceLocalBuffers(n, buffer_capacity, policy.A, policy.device)
+        else:
+            self.buffers = [buffer_queue.LocalBuffer(capacity=buffer_capacity) for _ in range(n)]
         self.states = [env.reset() for env in self.envs]
         self.previous_action = np.zeros(n, np.int32)
         self.lives = [START_LIVES] * n
@@ -296,6 +306,16 @@ class ApexVectorActor:
         self.episode_step = [0] * n
         self.total_max_prob = [0.0] * n
 
+    def _check_device_queue(self, queue):
+        p = self.policy
+        if queue.trajectory != self.trajectory:
+            raise ValueError("queue records samples of %d transitions, the actor samples %d"
+                             % (queue.trajectory, self.trajectory))
+        if queue.output_size != p.A:
+            raise ValueError("queue has num_action %d, the policy %d" % (queue.output_size, p.A))
+        if queue.device != p.device:
+            raise ValueError("queue is on device %d, the policy on device %d" % (queue.device, p.device))
+
     def run_unroll(self):
         """One unroll of `trajectory` steps for every environment.  Returns the episodes that finished during it:
         dicts of task, episode, score, epsilon, episode_step and total_max_prob (the logged ratio: the running sum of
@@ -304,10 +324,18 @@ class ApexVectorActor:
             self.learner.sync_policy(self.policy)
         finished = []
         T = self.trajectory
+        db = self.device_buffers
+        n = len(self.envs)
         for _ in range(T):
             out = self.policy.act(np.stack(self.states), self.previous_action, epsilon=np.array(self.epsilon))
             action, q_action = out["action"], out["q_action"]
             next_pa = action.astype(np.int32)
+            if db is not None:
+                # every buffer's length after this step's append, and the rows of that append
+                length = min(len(db) + 1, db.capacity)
+                rows = dict(state=list(self.states), next_state=[None] * n, reward=np.zeros(n, np.float32),
+                            done=np.zeros(n, np.bool_))
+                draws = []
             for i, env in enumerate(self.envs):
                 a = int(action[i])
                 self.episode_step[i] += 1
@@ -318,12 +346,18 @@ class ApexVectorActor:
                     r, d = -1, True
                 else:
                     r, d = reward, False
-                buf = self.buffers[i]
-                buf.append(state=self.states[i], done=d, reward=r, next_state=next_state,
-                           previous_action=int(self.previous_action[i]), action=a)
+                if db is None:
+                    buf = self.buffers[i]
+                    buf.append(state=self.states[i], done=d, reward=r, next_state=next_state,
+                               previous_action=int(self.previous_action[i]), action=a)
+                else:
+                    rows["next_state"][i], rows["reward"][i], rows["done"][i] = next_state, r, d
                 self.states[i] = next_state
                 self.lives[i] = info["ale.lives"]
-                if len(buf) > 3 * T:
+                if db is not None:
+                    if length > 3 * T:   # LocalBuffer.sample's draw, at the same point of the stream
+                        draws.append((i, np.random.permutation(length)[:T]))
+                elif len(buf) > 3 * T:
                     u = buf.sample(T)
                     self.queue.append_to_queue(
                         task=i, unrolled_state=u["state"], unrolled_next_state=u["next_state"],
@@ -340,6 +374,11 @@ class ApexVectorActor:
                     self.epsilon[i] = 1 / (self.episode[i] * 0.05 + 1)
                     self.states[i] = env.reset()
                     next_pa[i] = 0
+            if db is not None:
+                db.append(np.stack(rows["state"]), np.stack(rows["next_state"]), self.previous_action, action,
+                          rows["reward"], rows["done"])
+                for i, order in draws:   # a full queue blocks here, after the environment loop
+                    db.push(self.queue, i, order)
             self.previous_action = next_pa
         return finished
 

@@ -11,7 +11,8 @@ values -- so the learner branch of ``train_apex.py:82-155`` runs on it unchanged
   Agent.distributed_train     agent/apex.py:135-154 -> (loss, td_error)
   Agent.train                 agent/apex.py:156-168
   Agent.sync_policy           parameter_sync into a NativeApexPolicy (actor.py: ApexVectorActor)
-  Agent.device_memory         a DeviceMemory: the replay memory of train_apex.py:87 on the GPU (apex_replay.py)
+  Agent.device_memory         a DeviceMemory: the replay memory of train_apex.py:87 on the GPU (apex_replay.py);
+                              DeviceMemory.add_from_queue ingests a record of an ApexDeviceFIFOQueue without a host copy
   Agent.train_from_memory     Memory.sample + np.stack + distributed_train + Memory.update (train_apex.py:118-154)
                               as one device-resident step -> (loss, td_error)
 """
@@ -257,6 +258,9 @@ class DeviceMemory:
         memory.add(state, next_state, previous_action, action, reward, done)   # get_td_error + the Memory.add loop
         loss, td_error = learner.train_from_memory(memory, batch_size)         # sample .. distributed_train .. update
 
+    or, with the actors' ApexVectorActor pushing into an ApexDeviceFIFOQueue, ``memory.add_from_queue(queue)`` in place
+    of the sample_batch(1) and the add.
+
     It outlives a rebuild of the agent's learner (another batch size): the agent passes its current learner to each
     call.  ``replay`` is the NativeApexReplay; ``n_entries``, ``beta``, ``total()`` and ``last_sample()`` read its state."""
 
@@ -279,6 +283,21 @@ class DeviceMemory:
             for lo in range(0, st.shape[0], eng.B):
                 hi = min(lo + eng.B, st.shape[0])
                 self.replay.add(eng, st[lo:hi], ns[lo:hi], pa[lo:hi], ac[lo:hi], rw[lo:hi], dn[lo:hi])
+
+    def add_from_queue(self, queue, timeout_ms=-1):
+        """``add`` of the oldest record of an ApexDeviceFIFOQueue (train_apex.py:94-116 without a host copy): the
+        learner's |td| of its ``trajectory`` transitions and the store read the queue's GPU memory directly
+        (trajectory <= the learner's batch).  Blocks while the queue is empty; ``timeout_ms`` >= 0 raises
+        ``TimeoutError_`` with nothing changed.  One learner thread calls it, as it calls train_from_memory; actor
+        threads may push into the queue and sync their policies from the agent meanwhile."""
+        if dp.distributed():
+            raise RuntimeError("add_from_queue: a DeviceMemory is local to one GPU; data-parallel training "
+                               "(torch.distributed world > 1) uses Memory and distributed_train")
+        a = self.agent
+        with a._lock:
+            eng = a._engine if a._engine is not None else a._get_engine(queue.trajectory)
+        # the wait for a record runs without the agent's lock: actor threads take it in sync_policy meanwhile
+        self.replay.add_from_queue(eng, queue, timeout_ms)
 
     n_entries = property(lambda self: self.replay.n_entries)
     beta = property(lambda self: self.replay.beta)

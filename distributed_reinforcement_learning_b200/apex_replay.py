@@ -70,6 +70,15 @@ class NativeApexReplay:
         N.check(N.lib.drl_apex_replay_add(self._h, learner._h if learner is not None else None, n,
                                           *[N.ptr(a) for a in arrs], N.ptr(err) if err is not None else None))
 
+    def add_from_queue(self, learner, queue, timeout_ms=-1):
+        """``add`` of the oldest record of an ``ApexDeviceFIFOQueue`` with ``learner``'s |td| as the priorities, read
+        straight from the queue's GPU memory (queue.trajectory <= learner.B).  Blocks while the queue is empty;
+        ``timeout_ms`` >= 0 raises ``TimeoutError_`` with nothing changed."""
+        from .distributed_queue.buffer_queue import ApexDeviceFIFOQueue
+        if not isinstance(queue, ApexDeviceFIFOQueue):
+            raise TypeError("add_from_queue: queue must be an ApexDeviceFIFOQueue, got %s" % type(queue).__name__)
+        N.check(N.lib.drl_apex_replay_add_from_queue(self._h, learner._h, queue._q, int(timeout_ms)))
+
     def step_async(self, learner, slot, u01):
         """Sample learner.B draws with the uniforms ``u01`` -> gather into ``slot`` -> learner step -> priority update.
         ``learner.wait()`` returns (scalars, td_error) afterwards."""

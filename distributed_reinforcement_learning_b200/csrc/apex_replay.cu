@@ -15,6 +15,7 @@
 
 #include "apex_defs.cuh"
 #include "replay_core.cuh"
+#include "traj_queue.cuh"
 
 using namespace drl;
 
@@ -206,6 +207,66 @@ int drl_apex_replay_add(drl_apex_replay* r, drl_apex* learner, int32_t n, const 
                            r->next_state, r->previous_action, r->action, r->reward, r->done)));
   DRL_TRY(replay_launch_update(r, s, n, nullptr, r->cursor, error ? reinterpret_cast<const double*>(d + L.er) : nullptr,
                                error ? nullptr : learner->td_dev));
+  DRL_TRY(replay_end(r, s));
+  replay_advance(r, n);
+  return DRL_OK;
+}
+
+int drl_apex_replay_add_from_queue(drl_apex_replay* r, drl_apex* learner, drl_apex_queue* q, int32_t timeout_ms) {
+  DRL_TRY(check_replay(r));
+  if (!q) { set_error("null apex queue handle"); return DRL_ERR_INVALID; }
+  {
+    std::lock_guard<std::recursive_mutex> lk(r->mu);
+    DRL_TRY(check_learner(r, learner));
+    std::lock_guard<std::recursive_mutex> llk(learner->mu);
+    if (q->device != r->device) {
+      set_error("apex replay add_from_queue: the queue is on device %d, the memory on device %d", q->device, r->device);
+      return DRL_ERR_INVALID;
+    }
+    if (q->A != learner->A) {
+      set_error("apex replay add_from_queue: the queue has num_action %d, the learner %d", q->A, learner->A);
+      return DRL_ERR_INVALID;
+    }
+    // drl_apex_replay_add chunks a longer record; the slot is read in place and cannot be
+    if (q->T > learner->B) {
+      set_error("apex replay add_from_queue: the queue's trajectory %d exceeds the learner's batch %d", q->T, learner->B);
+      return DRL_ERR_INVALID;
+    }
+    if (q->T > r->capacity) {
+      set_error("apex replay add_from_queue: the queue's trajectory %d exceeds the memory's capacity %lld", q->T,
+                (long long)r->capacity);
+      return DRL_ERR_INVALID;
+    }
+  }
+  // wait for a record without either lock: actor threads sync their engines from this learner meanwhile
+  int qs = 0;
+  std::vector<cudaEvent_t> ev_commit;
+  DRL_TRY(traj_queue_pop(q, timeout_ms, &qs, &ev_commit));
+  std::lock_guard<std::recursive_mutex> lk(r->mu);
+  std::lock_guard<std::recursive_mutex> llk(learner->mu);
+  NvtxRange nv("drl:apex_replay_add_from_queue");
+  const int n = q->T;
+  const cudaStream_t s = learner->compute;
+  // The slot is an ApexIn of n = T rows as it is: the learner and the store read it in place.  Its weight is null, which
+  // the TD kernel reads as 1, the value drl_apex_replay_add stages.  Nothing here checks the actions on the host: the
+  // queue's only producers are actor buffers, whose appends check every previous action and action.
+  const ApexIn in{q->field(qs, kApexQFrames), reinterpret_cast<int32_t*>(q->field(qs, kApexQPa2)),
+                  reinterpret_cast<float*>(q->field(qs, kApexQReward)), q->field(qs, kApexQDone), nullptr};
+  const int rc = [&]() -> int {
+    DRL_CUDA_CHECK(cudaSetDevice(r->device));
+    DRL_TRY(replay_begin(r, s));
+    for (cudaEvent_t e : ev_commit) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, e, 0));
+    DRL_TRY(enqueue_forward_td(learner, in, n, false, nullptr, nullptr));
+    learner->last_n = n;
+    prof_mark(s, "replay_store");
+    DRL_CUDA_CHECK((launch_k(apex_replay_store_kernel, dim3(n, 2), 256, 0, s, in, n, r->cursor, r->capacity, r->state,
+                             r->next_state, r->previous_action, r->action, r->reward, r->done)));
+    return replay_launch_update(r, s, n, nullptr, r->cursor, nullptr, learner->td_dev);
+  }();
+  // the queue slot goes back to the producers either way (their gathers into it wait for its release event)
+  const int rc_release = traj_queue_release(q, qs, s);
+  DRL_TRY(rc);
+  DRL_TRY(rc_release);
   DRL_TRY(replay_end(r, s));
   replay_advance(r, n);
   return DRL_OK;

@@ -1,7 +1,9 @@
-// traj_queue.cu -- the device-resident queues behind drl_traj_queue_* (IMPALA trajectories) and drl_r2d2_queue_* (R2D2
-// sequences) (include/drl_b200.h; layout and ordering in traj_queue.cuh).  Producers are policy-engine recorders
-// (queue_recorder.cuh), the consumers are drl_learner_stage_from_queue (learner.cu) and drl_r2d2_replay_add_from_queue
-// (r2d2_replay.cu); no record byte crosses PCIe except the reward and done of a commit.
+// traj_queue.cu -- the device-resident queues behind drl_traj_queue_* (IMPALA trajectories), drl_r2d2_queue_* (R2D2
+// sequences) and drl_apex_queue_* (Ape-X local-buffer samples) (include/drl_b200.h; layout and ordering in
+// traj_queue.cuh).  Producers are policy-engine recorders (queue_recorder.cuh) and Ape-X actor buffers
+// (apex_actor_buffer.cu), the consumers are drl_learner_stage_from_queue (learner.cu), drl_r2d2_replay_add_from_queue
+// (r2d2_replay.cu) and drl_apex_replay_add_from_queue (apex_replay.cu); no record byte crosses PCIe on its way into or
+// out of a queue except the reward and done of a recorder's commit.
 #include <string.h>
 
 #include <algorithm>
@@ -325,6 +327,58 @@ int drl_r2d2_queue_read(drl_r2d2_queue* q, int32_t k, uint8_t* state, int32_t* p
   if (!q) { set_error("null r2d2 queue handle"); return DRL_ERR_INVALID; }
   void* const dst[kR2QFields] = {state, previous_action, action, previous_h, previous_c, reward, done};
   return queue_read(q, k, dst);
+}
+
+int drl_apex_queue_create(int32_t trajectory, int32_t num_action, int32_t capacity, int32_t device,
+                          drl_apex_queue** out) {
+  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
+  *out = nullptr;
+  if (trajectory < 1 || trajectory > kApexQueueMaxT) {
+    set_error("apex queue: trajectory must be in [1, %d] (got %d)", kApexQueueMaxT, trajectory);
+    return DRL_ERR_INVALID;
+  }
+  if (num_action < 2 || num_action > 32) { set_error("apex queue: num_action must be in [2, 32] (got %d)", num_action); return DRL_ERR_INVALID; }
+  if (capacity < 1) { set_error("apex queue: capacity must be >= 1 (got %d)", capacity); return DRL_ERR_INVALID; }
+  DRL_TRY(check_queue_device(device));
+  drl_apex_queue* q = new drl_apex_queue();
+  q->name = "apex queue";
+  q->pop_verb = "add_from_queue";
+  q->items = "records";
+  q->T = trajectory; q->A = num_action;
+  const size_t T = trajectory;
+  size_t sz[kApexQFields];
+  sz[kApexQFrames] = 2 * T * Geo::FRAME;
+  sz[kApexQPa2] = 2 * T * 4;
+  sz[kApexQReward] = T * 4;
+  sz[kApexQDone] = T;
+  // one record per slot: a slot is an ApexIn of n = T rows
+  return finish_create(q, kApexQFields, sz, capacity, 1, device, out, drl_apex_queue_destroy);
+}
+
+int drl_apex_queue_destroy(drl_apex_queue* q) {
+  if (!q) return DRL_OK;
+  queue_core_release(q);
+  delete q;
+  return DRL_OK;
+}
+
+int drl_apex_queue_size(drl_apex_queue* q) { return q ? queue_size(q) : 0; }
+
+int drl_apex_queue_read(drl_apex_queue* q, int32_t k, uint8_t* state, uint8_t* next_state, int32_t* previous_action,
+                        int32_t* action, float* reward, uint8_t* done) {
+  if (!q) { set_error("null apex queue handle"); return DRL_ERR_INVALID; }
+  if (!state || !next_state || !previous_action || !action) { set_error("apex queue read: null output pointer"); return DRL_ERR_INVALID; }
+  // the slot's frames and pa2 fields hold both halves; queue_read copies them into one block each, split below
+  const size_t T = q->T;
+  std::vector<uint8_t> frames(2 * T * Geo::FRAME);
+  std::vector<int32_t> pa2(2 * T);
+  void* const dst[kApexQFields] = {frames.data(), pa2.data(), reward, done};
+  DRL_TRY(queue_read(q, k, dst));
+  memcpy(state, frames.data(), T * Geo::FRAME);
+  memcpy(next_state, frames.data() + T * Geo::FRAME, T * Geo::FRAME);
+  memcpy(previous_action, pa2.data(), T * 4);
+  memcpy(action, pa2.data() + T, T * 4);
+  return DRL_OK;
 }
 
 }  // extern "C"

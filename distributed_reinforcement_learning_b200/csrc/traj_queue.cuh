@@ -1,12 +1,14 @@
-// traj_queue.cuh -- the device-resident queues (DESIGN.md sections 12 and 13): the FIFO core they share, the IMPALA
-// trajectory queue (drl_traj_queue) and the R2D2 sequence queue (drl_r2d2_queue), all in traj_queue.cu.  The
-// producers are policy-engine recorders (queue_recorder.cuh); the consumers are drl_learner_stage_from_queue
-// (learner.cu) and drl_r2d2_replay_add_from_queue (r2d2_replay.cu).
+// traj_queue.cuh -- the device-resident queues (DESIGN.md sections 12, 13 and 14): the FIFO core they share, the
+// IMPALA trajectory queue (drl_traj_queue), the R2D2 sequence queue (drl_r2d2_queue) and the Ape-X transition queue
+// (drl_apex_queue), all in traj_queue.cu.  The producers are policy-engine recorders (queue_recorder.cuh) and the Ape-X
+// actor buffers (apex_actor_buffer.cu); the consumers are drl_learner_stage_from_queue (learner.cu),
+// drl_r2d2_replay_add_from_queue (r2d2_replay.cu) and drl_apex_replay_add_from_queue (apex_replay.cu).
 //
 // The FIFO of drl_ring (ring.cu) with its batch slots in HBM instead of pinned host memory.  A slot holds `batch` records
 // field-major, each field batch-major (`sz[f]` bytes per record), in the consumer's layout: the learner staging slot's
-// (kernels.h: Inputs) for IMPALA, R2SeqRows / R2In (r2d2_replay.cu, r2d2_defs.cuh) for R2D2.  Queue position P (0, 1, 2,
-// ... in reservation order) is row P % batch of slot (P / batch) % nslots.
+// (kernels.h: Inputs) for IMPALA, R2SeqRows / R2In (r2d2_replay.cu, r2d2_defs.cuh) for R2D2, ApexIn (apex_defs.cuh) of
+// n = T rows for Ape-X (batch 1).  Queue position P (0, 1, 2, ... in reservation order) is row P % batch of slot
+// (P / batch) % nslots.
 //
 // Ordering across streams, all through events the queue owns:
 //   commit  (engine stream)     waits for ev_release of every slot it writes, copies, records one ev_commit per slot
@@ -26,6 +28,11 @@ namespace drl {
 enum TrajField { kTrajState = 0, kTrajReward, kTrajDone, kTrajMu, kTrajAction, kTrajPa, kTrajH, kTrajC, kTrajFields };
 // field order of an R2D2 slot (and of its recorders' staging): R2SeqRows'
 enum R2QueueField { kR2QFrames = 0, kR2QPa, kR2QAction, kR2QH, kR2QC, kR2QReward, kR2QDone, kR2QFields };
+// field order of an Ape-X slot: ApexIn's (frames [2T]: state rows, then next_state rows; pa2 [2T]: previous_action, then
+// action; reward [T]; done [T])
+enum ApexQueueField { kApexQFrames = 0, kApexQPa2, kApexQReward, kApexQDone, kApexQFields };
+// the largest T of an Ape-X queue: a push passes its T ring rows to the gather kernel by value
+constexpr int kApexQueueMaxT = 512;
 constexpr int kQueueMaxFields = 8;
 
 // the rows [row0, row0 + rows) of `slot` that one commit writes, from its staging rows [src0, src0 + rows)
@@ -73,6 +80,10 @@ struct drl_traj_queue : drl::QueueCore {
 struct drl_r2d2_queue : drl::QueueCore {
   int S = 0, C = 1, A = 0;
   size_t frame = 0;                   // bytes of one 84x84xC frame
+};
+
+struct drl_apex_queue : drl::QueueCore {
+  int T = 0, A = 0;                   // transitions per record, num_action
 };
 
 namespace drl {

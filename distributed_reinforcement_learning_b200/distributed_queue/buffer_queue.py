@@ -1,7 +1,8 @@
 """H100-native stand-ins for ``distributed_queue/buffer_queue.py``: ``FIFOQueue`` (reference :418-512, the IMPALA
 trajectory queue; ``DeviceFIFOQueue`` keeps it in GPU memory) and ``SumTree`` / ``Memory`` (reference :326-416, the
 Ape-X prioritized replay memory), and the other launchers' record queues (``R2D2FIFOQueue``; ``R2D2DeviceFIFOQueue``
-keeps it in GPU memory).
+keeps it in GPU memory; ``ApexFIFOQueue``; ``ApexDeviceFIFOQueue`` keeps it in GPU memory, filled from the Ape-X actor's
+``DeviceLocalBuffers``).
 
 The reference keeps a ``tf.FIFOQueue`` of 9-field trajectories on the learner's CPU and dequeues a
 batch with ``batch_size`` serial ``sess.run`` RPCs, after which the launcher ``np.stack``s eight
@@ -366,6 +367,63 @@ class ApexFIFOQueue(_QueueBase):
         return self._q.get_many(batch_size, timeout)
 
 
+class ApexDeviceFIFOQueue:
+    """``ApexFIFOQueue`` with its records in GPU memory (``drl_apex_queue_*``, DESIGN.md section 14).
+
+    Producers are ``DeviceLocalBuffers.push`` calls (``ApexVectorActor`` with this queue): each gathers one
+    local-buffer sample of ``trajectory`` transitions on the device into a slot.  The consumer is
+    ``apex.DeviceMemory.add_from_queue``, which ingests the oldest record into the device replay memory straight from
+    the slot.  Same constructor arguments as ``ApexFIFOQueue`` plus ``device``; ``get_size`` counts pushed and not yet
+    ingested records.  The queue holds ``queue_size + 1`` records, one more than an ``ApexFIFOQueue``: its capacity is
+    rounded as the other device queues round theirs.  There is no host producer (``append_to_queue``) and no host read
+    of a batch (``sample_batch``); ``read(k)`` copies one queued record out, for tests."""
+
+    def __init__(self, trajectory, input_shape, output_size, queue_size, batch_size, num_actors, device=0):
+        self.trajectory = int(trajectory)
+        self.input_shape = tuple(int(x) for x in input_shape)
+        if self.input_shape != (84, 84, 4):
+            raise ValueError("input_shape: expected (84, 84, 4), got %s" % (self.input_shape,))
+        self.output_size = int(output_size)
+        self.batch_size = int(batch_size)
+        self.queue_size = int(queue_size)
+        self.num_actors = num_actors
+        self.device = int(device)
+        self.sess = None
+        self._q = C.c_void_p()
+        N.check(N.lib.drl_apex_queue_create(self.trajectory, self.output_size, self.queue_size, self.device,
+                                            C.byref(self._q)))
+
+    def close(self):
+        if getattr(self, "_q", None) is not None and self._q.value:
+            N.lib.drl_apex_queue_destroy(self._q)
+            self._q = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def get_size(self):
+        """Records pushed and not yet ingested."""
+        return int(N.lib.drl_apex_queue_size(self._q))
+
+    def set_session(self, sess):
+        """Kept for call compatibility; there is no session."""
+        self.sess = sess
+
+    def read(self, k):
+        """The k-th queued record (0 = the next one ingested), copied to the host: a dict of state, next_state,
+        previous_action, action, reward, done as ``append_to_queue`` takes them."""
+        T = self.trajectory
+        out = dict(state=np.empty((T,) + self.input_shape, np.uint8),
+                   next_state=np.empty((T,) + self.input_shape, np.uint8), previous_action=np.empty(T, np.int32),
+                   action=np.empty(T, np.int32), reward=np.empty(T, np.float32), done=np.empty(T, np.uint8))
+        N.check(N.lib.drl_apex_queue_read(self._q, int(k), *[N.ptr(a) for a in out.values()]))
+        out["done"] = out["done"].view(np.bool_)
+        return out
+
+
 class R2D2FIFOQueue(_QueueBase):
     """buffer_queue.py:69-160: records of one stored-state sequence."""
     _FIELDS = ('state', 'previous_action', 'action', 'reward', 'done', 'previous_h', 'previous_c')
@@ -501,6 +559,75 @@ class LocalBuffer(_FieldDeques):
     def sample(self, batch_size):
         order = np.random.permutation(len(self))[:batch_size]
         return {f: [getattr(self, f)[i] for i in order] for f in self._FIELDS}
+
+
+class DeviceLocalBuffers:
+    """The ``LocalBuffer(capacity)`` of each of n environments in GPU memory (``drl_apex_actor_buffer_*``, DESIGN.md
+    section 14), for environments that append in lockstep: one length describes every buffer.  56,461 bytes of device
+    memory per transition and environment (11.3 GB at 20 environments x 1e4).
+
+      append(state, next_state, previous_action, action, reward, done)  LocalBuffer.append of all n environments
+      push(queue, env, order)     LocalBuffer.sample with the draws ``order`` given, then append_to_queue into an
+                                  ApexDeviceFIFOQueue, on the device
+      len(b), read(env, j)        the deque length; deque index j of environment env (for tests)
+    """
+
+    def __init__(self, n, capacity, num_action, device=0):
+        self.n, self.capacity, self.num_action, self.device = int(n), int(capacity), int(num_action), int(device)
+        self._b = C.c_void_p()
+        N.check(N.lib.drl_apex_actor_buffer_create(self.n, self.capacity, self.num_action, self.device,
+                                                   C.byref(self._b)))
+
+    def close(self):
+        if getattr(self, "_b", None) is not None and self._b.value:
+            N.lib.drl_apex_actor_buffer_destroy(self._b)
+            self._b = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __len__(self):
+        v = C.c_int64()
+        N.check(N.lib.drl_apex_actor_buffer_size(self._b, C.byref(v)))
+        return int(v.value)
+
+    def append(self, state, next_state, previous_action, action, reward, done):
+        """Row i of every argument is environment i's transition: state / next_state uint8 [n, 84, 84, 4],
+        previous_action / action [n] in [0, num_action), reward [n], done [n]."""
+        n = self.n
+        arrs = (N.as_c(state, np.uint8, (n, 84, 84, 4), "state"),
+                N.as_c(next_state, np.uint8, (n, 84, 84, 4), "next_state"),
+                N.as_c(previous_action, np.int32, (n,), "previous_action"),
+                N.as_c(action, np.int32, (n,), "action"),
+                N.as_c(reward, np.float32, (n,), "reward"),
+                N.as_c(N.as_u8(done), np.uint8, (n,), "done"))
+        for name, a in (("previous_action", arrs[2]), ("action", arrs[3])):
+            if ((a < 0) | (a >= self.num_action)).any():
+                raise ValueError("%s: values must lie in [0, %d)" % (name, self.num_action))
+        N.check(N.lib.drl_apex_actor_buffer_append(self._b, n, *[N.ptr(a) for a in arrs]))
+
+    def push(self, queue, env, order, timeout_ms=-1):
+        """Environment ``env``'s transitions at the deque indices ``order`` ([queue.trajectory] in [0, len)) as one
+        record of ``queue``.  Blocks while the queue is full; ``timeout_ms`` >= 0 raises ``TimeoutError_`` with nothing
+        changed."""
+        if not isinstance(queue, ApexDeviceFIFOQueue):
+            raise TypeError("push: queue must be an ApexDeviceFIFOQueue, got %s" % type(queue).__name__)
+        o = N.as_c(order, np.int32, (queue.trajectory,), "order")
+        if ((o < 0) | (o >= self.capacity)).any():   # the native call checks them against the length
+            raise ValueError("order: deque indices must lie in [0, %d)" % self.capacity)
+        N.check(N.lib.drl_apex_actor_buffer_push(self._b, queue._q, int(env), N.ptr(o), int(timeout_ms)))
+
+    def read(self, env, j):
+        """Deque index j of environment env as a dict of state, next_state, previous_action, action, reward, done."""
+        out = dict(state=np.empty((84, 84, 4), np.uint8), next_state=np.empty((84, 84, 4), np.uint8),
+                   previous_action=np.empty(1, np.int32), action=np.empty(1, np.int32),
+                   reward=np.empty(1, np.float32), done=np.empty(1, np.uint8))
+        N.check(N.lib.drl_apex_actor_buffer_read(self._b, int(env), int(j), *[N.ptr(a) for a in out.values()]))
+        return dict(state=out["state"], next_state=out["next_state"], previous_action=int(out["previous_action"][0]),
+                    action=int(out["action"][0]), reward=float(out["reward"][0]), done=bool(out["done"][0]))
 
 
 class R2D2TrajectoryBuffer(_FieldDeques):

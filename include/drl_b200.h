@@ -657,6 +657,66 @@ int drl_apex_replay_size(drl_apex_replay* r, int64_t* n_entries);  /* SumTree.n_
 int drl_apex_replay_beta(drl_apex_replay* r, double* beta);
 
 /* ------------------------------------------------------------------------------------------
+ * Device Ape-X transition queue (new, DESIGN.md section 14): ApexFIFOQueue with its records in GPU memory.  Producers
+ * are Ape-X actor buffers (drl_apex_actor_buffer_push, below), the consumer is drl_apex_replay_add_from_queue; a record
+ * never passes through the host.  A record is one local-buffer sample of T transitions, and a slot holds one record in
+ * the learner's ApexIn order: frames u8 [2T,84,84,4] (the state rows, then the next_state rows), previous_action then
+ * action i32 [2T], reward f32 [T], done u8 [T] (1,807,104 B at T = 32).  capacity is rounded as the other device
+ * queues round it: capacity + 1 slots (59.6 MB at T = 32, capacity 32), so the queue holds one record more than an
+ * ApexFIFOQueue of the same queue_size.  Thread-safe: several buffers may push while one learner thread ingests.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_apex_queue drl_apex_queue;
+/* trajectory in [1, 512], num_action in [2, 32], capacity >= 1 (DRL_ERR_INVALID otherwise, checked first);
+ * DRL_ERR_CUDA ("no CPU fallback") when `device` does not exist. */
+int drl_apex_queue_create(int32_t trajectory, int32_t num_action, int32_t capacity, int32_t device,
+                          drl_apex_queue** out);
+int drl_apex_queue_destroy(drl_apex_queue* q);
+/* records pushed and not yet popped */
+int drl_apex_queue_size(drl_apex_queue* q);
+/* Synchronous copy of the k-th queued record (0 = the next to be popped) into host arrays: state, next_state u8
+ * [T,84,84,4], previous_action, action i32 [T], reward f32 [T], done u8 [T]; for tests.  DRL_ERR_INVALID for k outside
+ * [0, size), DRL_ERR_STATE while a push into its slot is in progress. */
+int drl_apex_queue_read(drl_apex_queue* q, int32_t k, uint8_t* state, uint8_t* next_state, int32_t* previous_action,
+                        int32_t* action, float* reward, uint8_t* done);
+
+/* Ape-X actor buffers (new, DESIGN.md section 14): the n LocalBuffer(capacity)s of one vector actor in GPU memory,
+ * n * capacity rows in the replay memory's field layout, 56,461 B per row (11.3 GB at 20 environments x 1e4, 36 GB at
+ * 64).  All n environments append in lockstep, so one length describes every buffer; deque index j of environment e is
+ * the transition collections.deque(maxlen=capacity) would hold at index j.  Work runs on the buffer's own stream.
+ * Thread-safe, but one actor thread is expected to own a buffer. */
+typedef struct drl_apex_actor_buffer drl_apex_actor_buffer;
+/* n >= 1, capacity >= 2, num_action in [2, 32] (DRL_ERR_INVALID, checked first); DRL_ERR_CUDA without the device. */
+int drl_apex_actor_buffer_create(int32_t n, int32_t capacity, int32_t num_action, int32_t device,
+                                 drl_apex_actor_buffer** out);
+int drl_apex_actor_buffer_destroy(drl_apex_actor_buffer* b);
+/* LocalBuffer.append for all n environments at once (n must be the buffer's): state, next_state u8 [n,84,84,4];
+ * previous_action, action i32 [n] in [0, num_action) (DRL_ERR_INVALID otherwise, nothing changed); reward f32 [n]; done
+ * u8 [n].  All of next_state crosses PCIe; a row's state only when it differs from the same environment's previous
+ * next_state (otherwise the device copies that row).  One H2D from a pinned block, then one kernel. */
+int drl_apex_actor_buffer_append(drl_apex_actor_buffer* b, int32_t n, const uint8_t* state, const uint8_t* next_state,
+                                 const int32_t* previous_action, const int32_t* action, const float* reward,
+                                 const uint8_t* done);
+/* LocalBuffer.sample(T) of environment `env` with the draws given, then ApexFIFOQueue.append_to_queue: order i32 [T]
+ * (T = the queue's) are deque indices in [0, size), checked on the host.  Reserves one queue position without holding
+ * the buffer's lock, blocking while the queue is full (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with nothing changed
+ * otherwise), then gathers the rows into the slot on the device.  The queue's num_action and device must be the
+ * buffer's (DRL_ERR_INVALID).  A failure after the reservation puts the queue into its failed state. */
+int drl_apex_actor_buffer_push(drl_apex_actor_buffer* b, drl_apex_queue* queue, int32_t env, const int32_t* order,
+                               int32_t timeout_ms);
+/* the deque length (the same for every environment) */
+int drl_apex_actor_buffer_size(drl_apex_actor_buffer* b, int64_t* len);
+/* Synchronous copy of deque index j of environment env (one transition, the append's fields); for tests. */
+int drl_apex_actor_buffer_read(drl_apex_actor_buffer* b, int32_t env, int64_t j, uint8_t* state, uint8_t* next_state,
+                               int32_t* previous_action, int32_t* action, float* reward, uint8_t* done);
+/* drl_apex_replay_add of the oldest record of a device Ape-X queue (train_apex.py:94-116 without a host copy): pops it
+ * without holding the memory's or the learner's lock, blocking while the queue is empty (timeout_ms < 0: forever;
+ * DRL_ERR_TIMEOUT with nothing changed otherwise), then, on the learner's compute stream, the learner's |td| of the T
+ * transitions read from the queue slot, the store and the priority update; the slot goes back to the producers after
+ * them, also when enqueueing fails.  The learner must be an Ape-X (not A3C) handle on the memory's device with the
+ * queue's num_action and device, and T at most its batch (DRL_ERR_INVALID).  Does not wait for the compute stream. */
+int drl_apex_replay_add_from_queue(drl_apex_replay* r, drl_apex* learner, drl_apex_queue* queue, int32_t timeout_ms);
+
+/* ------------------------------------------------------------------------------------------
  * R2D2 learner (SURVEY.md section 8(f) row 3, BASELINE.json config 5): replaces r2d2.Agent's learner graph
  * (agent/r2d2.py:13-95) over model/r2d2_lstm.py:28-116 (conv stack + action embedding + ONE LSTMCell, unrolled seq_len
  * steps per scope from a stored (h, c) with the carried state multiplied by (1 - done) after every step; dense 128;
