@@ -55,6 +55,33 @@ size_t wgrad_partial_floats(int B, int T) {
   return std::max(mx, (size_t)16 * 32 * 256);   // also the scratch of emb_backward (kEmbChunks * A * 256)
 }
 
+}  // namespace drl
+
+// The launch plan net_backward / net_forward use at B x T in math mode `mode`, read by the per-kernel tests to assert which
+// edges a case reaches (tests/layer_parity.py launch_facts): out[0..2] = split-K count of the conv1 / conv2 / conv3 weight
+// gradients, out[3] / out[4] = frames per CTA of the persistent conv1 forward / weight-gradient kernels (math mode 5; 0
+// otherwise), out[5] = the M tile of the 16-bit split core (rows per CTA of every GEMM16 launch).
+extern "C" int drl_debug_launch_plan(int32_t B, int32_t T, int32_t mode, int32_t* out) {
+  using namespace drl;
+  if (!out || B < 1 || T < 3) { set_error("launch_plan: need out, B >= 1, T >= 3"); return DRL_ERR_INVALID; }
+  const int M = B * T, Mb = B * (T - 2);
+  if (mode == 5) {
+    const int sms = device_sm_count();
+    out[0] = std::min(Mb, sms);                                 // launch_conv1_wgrad_tma: one partial slab per CTA
+    out[3] = cdiv(M, std::min(M, sms));
+    out[4] = cdiv(Mb, std::min(Mb, sms));
+  } else {
+    out[0] = plan_conv1_wgrad(Mb, mode).splits;
+    out[3] = out[4] = 0;
+  }
+  out[1] = plan_conv2_wgrad(Mb, mode).splits;
+  out[2] = plan_conv3_wgrad(Mb, mode).splits;
+  out[5] = X64L8x2::BM;
+  return DRL_OK;
+}
+
+namespace drl {
+
 size_t lstm_image_bytes(int which, int M, int Mb) {
   (void)M;
   return which == 1 ? operand_image16_bytes<128>(Geo::XK, Mb)     // x^T  (A of lstm_wgrad)

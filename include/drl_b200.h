@@ -186,6 +186,10 @@ int drl_learner_profile_step(drl_learner* h, int32_t slot, char* names, int64_t 
  * C: `splits` slabs of [(M+1), N] floats (split-K partials; row M = column sums of B for N-major B). */
 int drl_debug_gemm(int32_t core, int32_t bn, int32_t a_kmajor, int32_t b_kmajor, int32_t M, int32_t N,
                    int32_t K, int32_t splits, const float* A, const float* B, float* C);
+/* Test aid: the IMPALA step's launch plan at B x T in math mode `mode` (needs the current device for its SM count):
+ * out[0..2] = split-K count of the conv1 / conv2 / conv3 weight gradients, out[3] / out[4] = frames per CTA of the
+ * persistent conv1 forward / weight-gradient kernels (math mode 5, else 0), out[5] = M tile of the 16-bit split core. */
+int drl_debug_launch_plan(int32_t B, int32_t T, int32_t mode, int32_t* out);
 /* Test aid: arm (dev_buf: device buffer of >= 8001 uint64, word 0 = entry count, zeroed by the caller) or disarm
  * (NULL) the kernel start-time trace: CTA 0 of every kernel of the step appends {globaltimer ns, grid size << 32 |
  * block size}.  Gives the true timeline of a CUDA-graph replay across both streams (tools/timeline.py). */

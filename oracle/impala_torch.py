@@ -270,6 +270,44 @@ def compute_entropy_loss(softmax):
     return -torch.sum(torch.sum(-softmax * torch.log(softmax), dim=1))
 
 
+def loss_inputs(reward, action, done, behavior_policy, dtype):
+    """The fed tensors the losses read (agent/impala.py:134-142): r, a, d, mu."""
+    return dict(r=torch.from_numpy(np.asarray(reward, dtype=np.float32)).to(dtype),
+                a=torch.from_numpy(np.asarray(action).astype(np.int64)),
+                d=torch.from_numpy(np.asarray(done).astype(bool)),
+                mu=torch.from_numpy(np.asarray(behavior_policy, dtype=np.float32)).to(dtype))
+
+
+def loss_terms(cfg, t, fp, fv, mp, mv, lp, lv):
+    """agent/impala.py:45-93 from the first / middle / last policy [B, T-2, A] and value [B, T-2] windows and the
+    prepared batch ``t`` (keys r, a, d, mu of ``loss_inputs``): V-trace targets, advantages and the three losses."""
+    c = cfg
+    if c["reward_clipping"] == "abs_one":                                # agent/impala.py:45-49
+        cr = torch.clamp(t["r"], -1.0, 1.0)
+    elif c["reward_clipping"] == "soft_asymmetric":
+        sq = torch.tanh(t["r"] / 5.0)
+        cr = torch.where(t["r"] < 0, 0.3 * sq, sq) * 5.0
+    else:
+        raise ValueError(c["reward_clipping"])
+    discounts = (~t["d"]).to(fv.dtype) * c["discount_factor"]            # :51
+    fa, ma, _ = split_data(t["a"])
+    fr, mr, _ = split_data(cr)
+    fd, md, _ = split_data(discounts)
+    fb, mb, _ = split_data(t["mu"])
+    A = c["num_action"]
+    vs, clipped_rho = from_softmax(fb, fp, fa, fd, fr, fv, mv, A)          # :68-71
+    vs_plus_1, _ = from_softmax(mb, mp, ma, md, mr, mv, lv, A)             # :73-76
+    pg_adv = (clipped_rho * (fr + fd * vs_plus_1 - fv)).detach()          # :78-80
+    pi_loss = compute_policy_gradient_loss(fp, fa, pg_adv, A)             # :82-86
+    baseline_loss = compute_baseline_loss(vs, fv)                         # :87-89
+    entropy = compute_entropy_loss(fp)                                    # :90-91
+    total = pi_loss + baseline_loss * c["baseline_loss_coef"] + entropy * c["entropy_coef"]   # :93
+    return dict(vs=vs, clipped_rho=clipped_rho, vs_plus_1=vs_plus_1, pg_advantage=pg_adv,
+                pi_loss=pi_loss, baseline_loss=baseline_loss, entropy=entropy, total_loss=total,
+                first_policy=fp, first_value=fv, middle_policy=mp, middle_value=mv,
+                last_policy=lp, last_value=lv)
+
+
 # --------------------------------------------------------------------------------------
 # Learner (agent/impala.py)
 # --------------------------------------------------------------------------------------
@@ -317,11 +355,8 @@ class Learner:
         # agent/impala.py:133 -- float64 divide on the host, then the feed casts to float32.
         x = (np.stack(state).astype(np.float64) / 255).astype(np.float32)
         return dict(
+            loss_inputs(reward, action, done, behavior_policy, dt),
             x=torch.from_numpy(x).to(dt),
-            r=torch.from_numpy(np.asarray(reward, dtype=np.float32)).to(dt),
-            a=torch.from_numpy(np.asarray(action).astype(np.int64)),
-            d=torch.from_numpy(np.asarray(done).astype(bool)),
-            mu=torch.from_numpy(np.asarray(behavior_policy, dtype=np.float32)).to(dt),
             pa=torch.from_numpy(np.asarray(previous_action).astype(np.int64)),
             h0=torch.from_numpy(np.asarray(initial_h, dtype=np.float32)).to(dt),
             c0=torch.from_numpy(np.asarray(initial_c, dtype=np.float32)).to(dt))
@@ -346,33 +381,9 @@ class Learner:
 
     # ---- graph (agent/impala.py:45-93) -------------------------------------------
     def losses(self, state, reward, action, done, behavior_policy, previous_action, initial_h, initial_c):
-        c = self.cfg
         t = self._prep(state, reward, action, done, behavior_policy, previous_action, initial_h, initial_c)
-        if c["reward_clipping"] == "abs_one":                            # agent/impala.py:45-49
-            cr = torch.clamp(t["r"], -1.0, 1.0)
-        elif c["reward_clipping"] == "soft_asymmetric":
-            sq = torch.tanh(t["r"] / 5.0)
-            cr = torch.where(t["r"] < 0, 0.3 * sq, sq) * 5.0
-        else:
-            raise ValueError(c["reward_clipping"])
-        discounts = (~t["d"]).to(self.dtype) * c["discount_factor"]       # :51
-        (fp, fv, mp, mv, lp, lv), taps = self._unrolled(t)
-        fa, ma, _ = split_data(t["a"])
-        fr, mr, _ = split_data(cr)
-        fd, md, _ = split_data(discounts)
-        fb, mb, _ = split_data(t["mu"])
-        A = c["num_action"]
-        vs, clipped_rho = from_softmax(fb, fp, fa, fd, fr, fv, mv, A)      # :68-71
-        vs_plus_1, _ = from_softmax(mb, mp, ma, md, mr, mv, lv, A)         # :73-76
-        pg_adv = (clipped_rho * (fr + fd * vs_plus_1 - fv)).detach()      # :78-80
-        pi_loss = compute_policy_gradient_loss(fp, fa, pg_adv, A)         # :82-86
-        baseline_loss = compute_baseline_loss(vs, fv)                     # :87-89
-        entropy = compute_entropy_loss(fp)                                # :90-91
-        total = pi_loss + baseline_loss * c["baseline_loss_coef"] + entropy * c["entropy_coef"]   # :93
-        return dict(vs=vs, clipped_rho=clipped_rho, vs_plus_1=vs_plus_1, pg_advantage=pg_adv,
-                    pi_loss=pi_loss, baseline_loss=baseline_loss, entropy=entropy, total_loss=total,
-                    first_policy=fp, first_value=fv, middle_policy=mp, middle_value=mv,
-                    last_policy=lp, last_value=lv, taps=taps)
+        windows, taps = self._unrolled(t)
+        return dict(loss_terms(self.cfg, t, *windows), taps=taps)
 
     def gradients(self, *batch, **kbatch):
         out = self.losses(*batch, **kbatch)
