@@ -112,8 +112,10 @@ struct Umma16Tile {
 // TAPSUM: every K tile of 64 starts a fresh accumulator, which is added in fp32 to a running sum in K-tile order once its
 // MMAs are complete (two register sets).  For the conv data gradients, whose K tiles are filter taps, this rounds and
 // sums exactly as a per-tap GEMM followed by a fixed-order tap sum would.
+// PREG (MINB = 2 only): the CTA's registers are split by role with setmaxnreg -- each producer thread keeps PREG, the two
+// consumer warpgroups take the rest (CREG each).  0: every thread keeps the count it was launched with.
 template <int BN_, int STAGES_, int MINB_ = 1, int PW_ = 4, int LW_ = 0, class AF_ = umma16::BF16, class BF_ = umma16::BF16,
-          int PFD_ = 0, bool TAPSUM_ = false>
+          int PFD_ = 0, bool TAPSUM_ = false, int PREG_ = 0>
 struct Umma16Cfg {
   static constexpr int PFD = PFD_;   // register prefetch ring depth in 32-wide K sub-tiles (0: 4 / 3 / 2 by operand kind)
   static constexpr int BM = 128, BN = BN_, BK = 64, SUBK = 32, STAGES = STAGES_, MINB = MINB_;
@@ -123,8 +125,20 @@ struct Umma16Cfg {
   static constexpr int NT = NPROD + wg::kConsumerThreads + 32 * LW;   // producers + two consumer warpgroups [+ loader]
   static_assert(PW == 4 || PW == 8, "4 or 8 producer warps");
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN must be a power of two in [32,256]");
-  static_assert((TAPSUM ? BN : BN / 2) + 40 <= 65536 / (NT * MINB),
-                "accumulator does not fit the register budget: fewer threads or CTAs");
+  // register budgets per thread: at launch (allocated in units of 8), then per role
+  static constexpr int PREG = PREG_;
+  static constexpr int REGS = 65536 / (NT * MINB);
+  static constexpr int CREG = PREG ? ((REGS & ~7) * NT - PREG * NPROD) / wg::kConsumerThreads & ~7 : REGS;
+  // setmaxnreg acts on whole warpgroups: the lone loader warp would be a partial one (the producers issue the bulk copy)
+  static_assert(PREG == 0 || (MINB == 2 && LW == 0), "per-role registers: two CTAs per SM, no loader warp");
+  static_assert(PREG % 8 == 0 && (PREG == 0 || (PREG >= 24 && PREG <= REGS)) && CREG <= 256,
+                "setmaxnreg takes multiples of 8 in [24, 256]; the producers give registers away");
+  // a consumer needs ~16 registers beside its accumulators; with one count for every role, the producers' state counts too
+  static_assert((TAPSUM ? BN : BN / 2) + (PREG ? 16 : 40) <= CREG,
+                "accumulator does not fit the consumers' register budget: fewer threads or CTAs");
+  // registers of the producers' prefetch ring: with one count for every role it shares the CTA with the accumulators and
+  // is capped at ~96; a producer with its own budget keeps ~24 registers for its rows and addresses
+  static constexpr int PF_REGS = PREG ? PREG - 24 : 96;
   using AF = AF_;   // 16-bit format of the A operand (uint8 operands are always fp16: exact)
   using BF = BF_;
 };
@@ -222,6 +236,7 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
 
   if (warp < Cfg::PW) {
     // ================= PRODUCERS =================
+    if constexpr (Cfg::PREG > 0) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PREG));
     // per-unit state: up to two Row handles (MN-major units span two 4-element loader groups), element offset inside
     // the sub-tile along K, and the byte offset of the unit's 16-byte chunk inside the plane for sub-tile 0
     typename AL::Row arow[UA][AR];
@@ -367,10 +382,11 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
       if (tid == 0) TR(2000 + g);
     };
 
-    // register prefetch ring, in sub-tiles; the accumulators live in registers of the same CTA, so it is capped at ~96
+    // register prefetch ring, in sub-tiles, within Cfg::PF_REGS registers
     constexpr int RPS = 4 * UA * AR + (BPT ? 0 : 8 * UB);      // registers one gathered sub-tile occupies
     constexpr int PF0 = Cfg::PFD > 0 ? Cfg::PFD : (A16 ? 4 : (BPT ? 3 : 2));
-    constexpr int PF = (PF0 * RPS <= 96) ? PF0 : (96 / RPS >= 1 ? 96 / RPS : 1);
+    constexpr int PFR = Cfg::PF_REGS;
+    constexpr int PF = (PF0 * RPS <= PFR) ? PF0 : (PFR / RPS >= 1 ? PFR / RPS : 1);
     const int nsub = 2 * ntiles;
     ARaw ra[PF][UA][AR];
     float4 rb[PF][UB][2];
@@ -435,6 +451,7 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
     }
   } else {
     // ================= CONSUMERS (warps PW .. PW+7: warpgroup cw = rows 64 cw .. 64 cw + 63) =================
+    if constexpr (Cfg::PREG > 0) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::CREG));
     const int ct = tid - NPROD, cw = ct >> 7, cwarp = (ct >> 5) & 3;
     // A rows of this warpgroup: K-major +64 rows of 128 bytes; MN-major the second 64-element atom of every k-group
     const uint32_t a_off = AK ? (uint32_t)(cw * 64 * 128) : (uint32_t)(cw * 1024);

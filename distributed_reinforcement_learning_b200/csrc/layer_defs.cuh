@@ -34,8 +34,8 @@ using Conv2DBm = ConvDgradBMerged<32, 64, 2, 4, 4>;     // math mode 5: the four
 using Conv2DEm = EpConvDxMerged<20, 20, 32, 2, 10, 10>;
 
 // Every tensor-core configuration has two consumer warpgroups (256 threads) whose wgmma accumulators hold BN / 2 fp32
-// registers per thread, next to the producer warps, in one CTA per SM: BN = 256 (128 accumulator registers) leaves
-// room for 4 producer warps and no loader warp within the 65,536 registers of an H100 SM.
+// registers per thread, next to the producer warps, in one CTA per SM unless MINB says otherwise: BN = 256 (128
+// accumulator registers) leaves room for 4 producer warps and no loader warp within the 65,536 registers of an H100 SM.
 using U32 = UmmaCfg<32, 2, 1>;   // 24 KB / stage (A exact: conv1 only)
 using U64 = UmmaCfg<64, 2, 1>;   // 48 KB / stage
 using U128 = UmmaCfg<128, 3, 1, 8>;   // 64 KB / stage, 8 producer warps
@@ -50,8 +50,11 @@ using U256L = U256;                    // (no loader warp: the same configuratio
 // and saturates at 65504 -- conv1 (conv1_tma.cuh) uses it because one operand is EXACT in it (the uint8 frames) and the
 // other is an O(0.1) weight.
 using Fmt16 = umma16::BF16;     // every GEMM whose operands are fp32 activations / gradients / weights
-using X64L8x2 = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16>;     // conv2 / conv3 fwd: 48 KB per K = 64 stage, 8 producer warps
-                                                             // (the gathers are latency-bound)
+// Two CTAs per SM (MINB = 2, 106 KB of shared memory each): one CTA's pipeline fill and epilogue overlap the other's main
+// loop.  512 threads x 64 registers, split by role: 8 producer warps (the gathers are latency-bound) keep PREG registers and
+// issue the weight image's bulk copy themselves, the consumer warpgroups take the rest.
+using X64L2 = Umma16Cfg<64, 2, 2, 8, 0, Fmt16, Fmt16, 0, false, 56>;  // conv2 / conv3 fwd: 48 KB per K = 64 stage; producers
+                                                                     // 56 (a prefetch ring of 2 sub-tiles), consumers 72
 using X64W8x2 = Umma16Cfg<64, 2, 1, 8, 0, Fmt16, Fmt16>;     // conv2 / conv3 weight gradients (both operands gathered)
 using XH = Umma16Cfg<64, 4, 1, 8, 0, Fmt16, Fmt16>;          // head layers (K = 256 = all four stages in flight)
 // bulk-fed LSTM weight gradient (gemm_bulk16.cuh): both operands are pre-tiled images, no producer warps
@@ -59,10 +62,13 @@ using BK256 = Bulk16Cfg<256, 2>;       // 96 KB per stage (A 32 KB + B 64 KB), 2
 using X256L = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm fwd: 96 KB per stage
 using X128D = Umma16Cfg<128, 3, 1, 8, 1, Fmt16, Fmt16>;      // lstm data gradient: 64 KB per stage
 // conv data gradients (pre-tiled B, one K tile of 64 co per filter tap): per-tap partial sums added in tap order, the
-// rounding of the dCol GEMM + col2im of math modes 2 and 3.  The second register set costs conv2 (BN = 128) its loader warp
-// and half its producer warps (384 threads: 170 registers each).
+// rounding of the dCol GEMM + col2im of math modes 2 and 3.
 using X64T = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16, 0, true>;    // conv3: K = 9 taps x 64 co, N = 64 ci
-using X128T = Umma16Cfg<128, 3, 1, 4, 0, Fmt16, Fmt16, 0, true>;  // conv2: K = 4 taps x 64 co, N = 4 parity classes x 32 ci
+// conv2: K = 4 taps x 64 co, N = 4 parity classes x 32 ci, as two N tiles of (py, px = 0..1) x 32 ci, two CTAs per SM as
+// X64L2 (each N tile gathers the dY taps itself: ~59 MB more L2 reads at B = 32, T = 20).  The second register set (64
+// per consumer thread) leaves the producers 48 registers: no register prefetch beyond the sub-tile in flight.  (conv3's
+// data gradient measured slower this way, 0.070 -> 0.072 ms on an H100 SXM at 700 W, and keeps X64T.)
+using X64T2 = Umma16Cfg<64, 2, 2, 8, 0, Fmt16, Fmt16, 0, true, 48>;
 
 // math mode 3 (experimental): the persistent, fully warp-specialised variant of each tensor-core configuration
 template <class U> struct PersistOf;

@@ -76,7 +76,35 @@ extern "C" int drl_debug_launch_plan(int32_t B, int32_t T, int32_t mode, int32_t
   }
   out[1] = plan_conv2_wgrad(Mb, mode).splits;
   out[2] = plan_conv3_wgrad(Mb, mode).splits;
-  out[5] = X64L8x2::BM;
+  out[5] = X64L2::BM;
+  return DRL_OK;
+}
+
+namespace drl {
+template <class Cfg, class AL, class BL, class EP>
+static int umma16_resident_ctas(int32_t* out) {
+  using SM = Umma16Smem<Cfg, AL, BL>;
+  auto kern = gemm_umma16_kernel<Cfg, AL, BL, EP>;
+  int n = 0;
+  DRL_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::BYTES));
+  DRL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, Cfg::NT, SM::BYTES));
+  *out = n;
+  return DRL_OK;
+}
+}  // namespace drl
+
+// The CTAs per SM that the two-CTA-per-SM kernels of math mode 5 actually get (occupancy at the block size and dynamic
+// shared memory they launch with): out[0] / out[1] = conv2 / conv3 forward, out[2] = conv2 data gradient.
+// A register or shared-memory change that drops one of them to one CTA per SM changes no result, only the step time.
+extern "C" int drl_debug_gemm16_residency(int32_t* out) {
+  using namespace drl;
+  if (!out) { set_error("gemm16_residency: need out"); return DRL_ERR_INVALID; }
+  if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
+  using FwdB = PretiledB<PlainB>;
+  using FwdE = EpBiasAct<true, true>;
+  DRL_TRY((umma16_resident_ctas<X64L2, Conv2A, FwdB, FwdE>(out + 0)));
+  DRL_TRY((umma16_resident_ctas<X64L2, Conv3A, FwdB, FwdE>(out + 1)));
+  DRL_TRY((umma16_resident_ctas<X64T2, Conv2DA, PretiledB<Conv2DBm>, Conv2DEm>(out + 2)));
   return DRL_OK;
 }
 
@@ -95,7 +123,7 @@ void weight_image_sizes(size_t (&b)[WeightImages::kCount]) {
   b[3] = weight_image_bytes<256>(Geo::G4, Geo::XK);
   b[4] = weight_image_bytes<128>(Geo::FLAT + Geo::EMB, Geo::G4);
   b[5] = weight_image_bytes<256>(576, 64);   // the dCol operands of math modes 2 and 3; larger than the 16-bit dgrad images
-  b[6] = weight_image_bytes<256>(512, 64);   // of math mode 5 (weight_image16_bytes<64>(64, 576), <128>(128, 256))
+  b[6] = weight_image_bytes<256>(512, 64);   // of math mode 5 (weight_image16_bytes<64>(64, 576), <64>(128, 256))
 }
 
 // Refresh the weight images (4 launches on the side stream + 1 for the two conv-forward images; ~60 MB written).
@@ -105,7 +133,7 @@ void weight_image_sizes(size_t (&b)[WeightImages::kCount]) {
 // Images 5 / 6 are the B operands of the conv3 / conv2 data gradients (gather form: B(k = (tap, co), n = ci)).
 static int retile_dgrad16(cudaStream_t s, const ParamLayout& pl, const float* P, const WeightImages& wi) {
   DRL_TRY((launch_retile_b16<64, Fmt16>(s, Conv3DB{P + pl.conv3_w}, 64, 576, wi.img[5])));
-  DRL_TRY((launch_retile_b16<128, Fmt16>(s, Conv2DBm{{P + pl.conv2_w}}, 128, 256, wi.img[6])));
+  DRL_TRY((launch_retile_b16<64, Fmt16>(s, Conv2DBm{{P + pl.conv2_w}}, 128, 256, wi.img[6])));
   return DRL_OK;
 }
 
@@ -194,7 +222,7 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     PlainB bl{P + pl.conv2_w, 64, 0};
     PretiledB<PlainB> blp{wi.img[1], m16 ? 512 / 64 : 512 / 32};
     EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    if (m16) GEMM16("conv2_fwd", X64L8x2, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
+    if (m16) GEMM16("conv2_fwd", X64L2, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
     else GEMM_W("conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
   }
   if (c3_event) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[4], 0));
@@ -204,7 +232,7 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     PlainB bl{P + pl.conv3_w, 64, 0};
     PretiledB<PlainB> blp{wi.img[2], m16 ? 576 / 64 : 576 / 32};
     EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    if (m16) GEMM16("conv3_fwd", X64L8x2, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
+    if (m16) GEMM16("conv3_fwd", X64L2, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
     else GEMM_W("conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
   }
   if (late_images) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[1], 0));
@@ -272,13 +300,13 @@ int conv_forward16(cudaStream_t s, const ParamLayout& pl, const float* P, const 
     Conv2A al{a1, map};
     PretiledB<PlainB> blp{img_conv2, 512 / 64};
     EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    DRL_TRY((launch_gemm_umma16<X64L8x2>(s, al, blp, ep, n * 81, 64, 512, 1, 512, 0)));
+    DRL_TRY((launch_gemm_umma16<X64L2>(s, al, blp, ep, n * 81, 64, 512, 1, 512, 0)));
   }
   {
     Conv3A al{a2, map};
     PretiledB<PlainB> blp{img_conv3, 576 / 64};
     EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    DRL_TRY((launch_gemm_umma16<X64L8x2>(s, al, blp, ep, n * 49, 64, 576, 1, 576, 0)));
+    DRL_TRY((launch_gemm_umma16<X64L2>(s, al, blp, ep, n * 49, 64, 576, 1, 576, 0)));
   }
   return DRL_OK;
 }
@@ -469,12 +497,12 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
   s = st.main;
   if (m16) {
     // merged-phase gather form: row = the 2 x 2 block of input pixels (2i + py, 2j + px); all four parity classes read
-    // the same dY taps (i - a, j - b), so K = (a, b, co) = 256 and N = (py, px, ci) = 128; ReLU mask of a1 in the epilogue;
-    // per-tap partial sums added in (a, b) order, as in col2im_conv2
+    // the same dY taps (i - a, j - b), so K = (a, b, co) = 256 and N = (py, px, ci) = 128, in two N tiles (py = 0, 1);
+    // ReLU mask of a1 in the epilogue; per-tap partial sums added in (a, b) order, as in col2im_conv2
     Conv2DA al{bw.da2};
     PretiledB<Conv2DBm> blp{wi.img[6], 256 / 64};
     Conv2DEm ep{{bw.da1, act.a1}};
-    GEMM16("conv2_dgrad", X128T, al, blp, ep, Mb * 100, 128, 256, 1, 256, 0);
+    GEMM16("conv2_dgrad", X64T2, al, blp, ep, Mb * 100, 128, 256, 1, 256, 0);
   } else if (mode >= 2) {
     PlainA al{bw.da2, 64, 0};
     PlainBT bl{P + pl.conv2_w, 64, 0};               // B(k = co, n = (ky,kx,ci)) = W[n*64 + co]

@@ -190,6 +190,10 @@ int drl_debug_gemm(int32_t core, int32_t bn, int32_t a_kmajor, int32_t b_kmajor,
  * out[0..2] = split-K count of the conv1 / conv2 / conv3 weight gradients, out[3] / out[4] = frames per CTA of the
  * persistent conv1 forward / weight-gradient kernels (math mode 5, else 0), out[5] = M tile of the 16-bit split core. */
 int drl_debug_launch_plan(int32_t B, int32_t T, int32_t mode, int32_t* out);
+/* Test aid: CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor at the launch's block size and dynamic shared
+ * memory) of the math-mode-5 kernels sized for two per SM: out[0] / out[1] = conv2 / conv3 forward, out[2] = conv2
+ * data gradient. */
+int drl_debug_gemm16_residency(int32_t* out);
 /* Test aid: arm (dev_buf: device buffer of >= 8001 uint64, word 0 = entry count, zeroed by the caller) or disarm
  * (NULL) the kernel start-time trace: CTA 0 of every kernel of the step appends {globaltimer ns, grid size << 32 |
  * block size}.  Gives the true timeline of a CUDA-graph replay across both streams (tools/timeline.py). */
