@@ -298,6 +298,16 @@ def _load():
         "drl_apex_actor_buffer_push": (C.c_int, [vp, vp, i32, vp, i32]),
         "drl_apex_actor_buffer_size": (C.c_int, [vp, C.POINTER(i64)]),
         "drl_apex_actor_buffer_read": (C.c_int, [vp, i32, i64] + [vp] * 6),
+        "drl_a3c_queue_create": (C.c_int, [i32] * 4 + [C.POINTER(vp)]),
+        "drl_a3c_queue_destroy": (C.c_int, [vp]),
+        "drl_a3c_queue_size": (C.c_int, [vp]),
+        "drl_a3c_queue_read": (C.c_int, [vp, i32] + [vp] * 6),
+        "drl_a3c_policy_recorder_create": (C.c_int, [vp, vp, i32, C.POINTER(vp)]),
+        "drl_a3c_policy_recorder_destroy": (C.c_int, [vp]),
+        "drl_a3c_policy_recorder_act": (C.c_int, [vp] + [vp] * 7),
+        "drl_a3c_policy_recorder_commit": (C.c_int, [vp, vp, vp, vp, i32]),
+        "drl_a3c_policy_recorder_reset": (C.c_int, [vp]),
+        "drl_a3c_stage_from_queue": (C.c_int, [vp, i32, vp, i32]),
         "drl_r2d2_replay_create": (C.c_int, [i32, i64, i32, i32, i32, C.POINTER(vp)]),
         "drl_r2d2_replay_destroy": (C.c_int, [vp]),
         "drl_r2d2_replay_add": (C.c_int, [vp, vp, i32] + [vp] * 8),

@@ -46,6 +46,15 @@ class NativeA3CLearner(AdamLearnerHandle):
         self._keep[slot] = arrs
         N.check(N.lib.drl_a3c_stage(self._h, slot, *[N.ptr(a) for a in arrs]))
 
+    def stage_from_queue(self, slot, queue, timeout_ms=-1):
+        """Stage the oldest record of an ``A3CDeviceFIFOQueue`` into ``slot`` device to device (blocks until one is
+        queued; ``timeout_ms`` >= 0 raises ``TimeoutError_`` with the queue and the slot untouched)."""
+        from .distributed_queue.buffer_queue import A3CDeviceFIFOQueue
+        if not isinstance(queue, A3CDeviceFIFOQueue):
+            raise TypeError("stage_from_queue: queue must be an A3CDeviceFIFOQueue, got %s" % type(queue).__name__)
+        N.check(N.lib.drl_a3c_stage_from_queue(self._h, int(slot), queue._q, int(timeout_ms)))
+        self._keep[slot] = None      # no host arrays behind this slot's copies
+
     def wait(self):
         o = N.A3cOut()
         N.check(N.lib.drl_a3c_wait(self._h, C.byref(o)))

@@ -397,7 +397,10 @@ class A3CVectorActor:
         reward; ``lives`` follows ``info['ale.lives']`` after every step;
       - at an episode's end the environment, the previous action and lives (5) are reset, and so are the score,
         ``episode_step`` and the summed ``policy[action]`` behind the logged "prob";
-      - every environment's trajectory goes to ``queue.append_to_queue(task=i, ...)``.
+      - every environment's trajectory goes to ``queue.append_to_queue(task=i, ...)``; with an
+        ``A3CDeviceFIFOQueue`` the acts go through a recorder of the policy instead (``NativeA3CPolicy.recorder``),
+        which keeps the unrolls on the GPU, and the unroll ends with one ``commit`` of the rewards, done flags and
+        final next_state frames of all N environments, in environment order.  No host trajectory is kept.
     At n = 1 this is the reference actor's loop, including the order of its ``np.random`` draws.
     """
 
@@ -418,18 +421,48 @@ class A3CVectorActor:
         self.score = [0.0] * n
         self.episode_step = [0] * n
         self.total_max_prob = [0.0] * n
+        self.recorder = None
+        if isinstance(queue, buffer_queue.A3CDeviceFIFOQueue):
+            self._check_device_queue(queue)
+            self.trajs = None
+            self.recorder = policy.recorder(queue, n)
+
+    def _check_device_queue(self, queue):
+        p = self.policy
+        if queue.trajectory != self.trajectory:
+            raise ValueError("queue records unrolls of %d steps, the actor unrolls %d" % (queue.trajectory,
+                                                                                        self.trajectory))
+        if queue.output_size != p.A:
+            raise ValueError("queue has num_action %d, the policy %d" % (queue.output_size, p.A))
+        if queue.device != p.device:
+            raise ValueError("queue is on device %d, the policy on device %d" % (queue.device, p.device))
+        n = len(self.envs)
+        if n > queue.max_rows:
+            raise ValueError("%d environments per commit, the queue takes at most %d at once" % (n, queue.max_rows))
 
     def run_unroll(self):
         """One unroll of `trajectory` steps for every environment, pushed to the queue.  Returns the episodes that
         finished during it: dicts of task, episode, prob (the mean policy[action]), score and episode_step, the values
         train_a3c.py:162-165 logs."""
-        for t in self.trajs:
-            t.initialize()
+        n = len(self.envs)
+        rec = self.recorder
+        if rec is None:
+            for t in self.trajs:
+                t.initialize()
+        else:
+            rec.reset()   # an unroll that raised half-way left its steps behind: start this one at step 0
+            rewards = np.zeros((n, self.trajectory), np.float32)
+            dones = np.zeros((n, self.trajectory), np.bool_)
+            next_states = None   # env.step's frames of the previous step
         if self.learner is not None:
             self.learner.sync_policy(self.policy)
         finished = []
-        for _ in range(self.trajectory):
-            out = self.policy.act(np.stack(self.states), self.previous_action)
+        for step in range(self.trajectory):
+            if rec is None:
+                out = self.policy.act(np.stack(self.states), self.previous_action)
+            else:
+                out = rec.act(np.stack(self.states), self.previous_action, previous_next_state=next_states)
+                next_states = [None] * n
             action, max_prob = out["action"], out["max_prob"]
             next_pa = action.astype(np.int32)
             for i, env in enumerate(self.envs):
@@ -442,8 +475,12 @@ class A3CVectorActor:
                     r, d = -1, True
                 else:
                     r, d = reward, False
-                self.trajs[i].append(state=self.states[i], next_state=next_state,
-                                     previous_action=int(self.previous_action[i]), action=a, reward=r, done=d)
+                if rec is None:
+                    self.trajs[i].append(state=self.states[i], next_state=next_state,
+                                         previous_action=int(self.previous_action[i]), action=a, reward=r, done=d)
+                else:   # state, the actions and (from the next act on) next_state are on the device already
+                    rewards[i, step], dones[i, step] = r, d
+                    next_states[i] = next_state
                 self.states[i] = next_state
                 self.lives[i] = info["ale.lives"]
                 if done:
@@ -458,6 +495,9 @@ class A3CVectorActor:
                     next_pa[i] = 0
                     self.lives[i] = START_LIVES
             self.previous_action = next_pa
+        if rec is not None:
+            rec.commit(rewards, dones, np.stack(next_states))
+            return finished
         for i, t in enumerate(self.trajs):
             u = t.extract()
             self.queue.append_to_queue(

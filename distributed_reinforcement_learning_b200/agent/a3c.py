@@ -3,6 +3,7 @@ learner branch of ``train_a3c.py`` runs on it unchanged), with the TF1 graph rep
 
   Agent.__init__               agent/a3c.py:11-83
   Agent.train                  agent/a3c.py:85-103 -> (pi_loss, value_loss, entropy, learning_rate)
+  Agent.train_from_queue       train on the oldest record of an A3CDeviceFIFOQueue, staged device to device
   Agent.set_session            agent/a3c.py:105-107
   Agent.get_policy_and_action  agent/a3c.py:109-119 -> (action, policy, max_prob)
   Agent.parameter_sync         agent/a3c.py:121-122
@@ -13,6 +14,7 @@ import threading
 
 import numpy as np
 
+from .. import dp
 from ..a3c_learner import NativeA3CLearner
 from ..model import actor_critic
 
@@ -90,6 +92,35 @@ class Agent:
         out = eng.step(slot)
         self._last = out
         return out["pi_loss"], out["baseline_loss"], out["entropy"], out["learning_rate"]
+
+    def train_from_queue(self, queue, timeout_ms=-1):
+        """``train`` on the oldest record of an ``A3CDeviceFIFOQueue`` (the actors' recorders fill it on the GPU): the
+        record is staged device to device, then the same step runs.  Blocks until the queue holds a record
+        (``timeout_ms`` >= 0 raises ``TimeoutError_`` with nothing changed).  -> (pi_loss, value_loss, entropy,
+        learning_rate), as ``train``.  One learner thread calls it; do not interleave it with ``train`` from another
+        thread."""
+        with self._lock:
+            if dp.distributed():
+                raise RuntimeError("train_from_queue is single-replica: the queue lives on one device")
+            if self._engine is not None and self._engine.B != queue.trajectory:
+                self._pull_state()
+                self._engine.close()
+                self._engine = None
+            eng = self._get_engine(queue.trajectory)
+            slot = self._slot
+            self._slot = (slot + 1) % eng.num_slots    # taken now, so a train() meanwhile picks the other slot
+        # wait for the record without the agent's lock: actor threads sync their policies from this agent meanwhile
+        try:
+            eng.stage_from_queue(slot, queue, timeout_ms)
+        except Exception:
+            with self._lock:
+                if self._slot == (slot + 1) % eng.num_slots:
+                    self._slot = slot                  # nothing was staged: the slot is not used up
+            raise
+        with self._lock:
+            out = eng.step(slot)
+            self._last = out
+            return out["pi_loss"], out["baseline_loss"], out["entropy"], out["learning_rate"]
 
     def set_session(self, sess):
         self.sess = sess

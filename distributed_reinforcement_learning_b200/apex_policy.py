@@ -12,7 +12,7 @@ backward buffers.
 import numpy as np
 
 from . import _native as N
-from .policy_handle import MAX_BATCH, PolicyHandle  # noqa: F401  (MAX_BATCH: rows per call)
+from .policy_handle import MAX_BATCH, PolicyHandle, RecorderHandle  # noqa: F401  (MAX_BATCH: rows per call)
 
 APEX, A3C = 0, 1
 
@@ -62,11 +62,12 @@ class NativeA3CPolicy(_ApexPolicyBase):
         from .a3c_learner import NativeA3CLearner
         return NativeA3CLearner
 
-    def act(self, state, previous_action, uniform=None):
-        """Batched get_policy_and_action for n <= max_batch rows: state uint8 [n, 84, 84, 4], previous_action [n].
-        Row i's action is what ``np.random.choice(A, p=policy[i])`` picks for the uniform draw ``uniform[i]`` in
-        [0, 1); by default the draws are ``np.random.random_sample(n)``, the stream that choice reads.
-        Returns dict(action, policy, max_prob) with max_prob = policy[action] (the reference's name for it)."""
+    def recorder(self, queue, n):
+        """An ``A3CPolicyRecorder`` of n rows (n <= max_batch) into ``queue`` (an ``A3CDeviceFIFOQueue`` on this
+        device)."""
+        return A3CPolicyRecorder(self, queue, n)
+
+    def _act_args(self, state, previous_action, uniform):
         n, st, pa = self._inputs(state, previous_action)
         if uniform is None:
             uniform = np.random.random_sample(n)
@@ -76,9 +77,54 @@ class NativeA3CPolicy(_ApexPolicyBase):
         u = N.as_c(u, np.float64, (n,), "uniform")
         if not ((u >= 0.0) & (u < 1.0)).all():
             raise ValueError("uniform: values must lie in [0, 1)")
-        action = np.empty(n, np.int32)
-        policy = np.empty((n, self.A), np.float32)
-        prob = np.empty(n, np.float32)
+        outs = (np.empty(n, np.int32), np.empty((n, self.A), np.float32), np.empty(n, np.float32))
+        return n, st, pa, u, outs
+
+    def act(self, state, previous_action, uniform=None):
+        """Batched get_policy_and_action for n <= max_batch rows: state uint8 [n, 84, 84, 4], previous_action [n].
+        Row i's action is what ``np.random.choice(A, p=policy[i])`` picks for the uniform draw ``uniform[i]`` in
+        [0, 1); by default the draws are ``np.random.random_sample(n)``, the stream that choice reads.
+        Returns dict(action, policy, max_prob) with max_prob = policy[action] (the reference's name for it)."""
+        n, st, pa, u, (action, policy, prob) = self._act_args(state, previous_action, uniform)
         N.check(N.lib.drl_a3c_policy_act(self._h, n, N.ptr(st), N.ptr(pa), N.ptr(u), N.ptr(action), N.ptr(policy),
                                          N.ptr(prob)))
         return dict(action=action, policy=policy, max_prob=prob)
+
+
+class A3CPolicyRecorder(RecorderHandle):
+    """Records n rows of a ``NativeA3CPolicy``'s acts as unrolls of ``queue.trajectory`` steps, on the device.
+
+    ``act`` is ``NativeA3CPolicy.act`` plus ``previous_next_state``: the [n] frames ``env.step`` returned at the
+    previous step (ignored at step 0).  Call it for steps t = 0 .. T-1 with exactly n rows, then ``commit(reward, done,
+    next_state)`` with the [n, T] rewards and done flags and the [n] frames of step T-1.  The commit moves the n unrolls
+    into the queue in row order (blocking while it is full; ``timeout_ms`` >= 0 raises ``TimeoutError_`` with nothing
+    changed) and starts the next unroll.  Each unroll stores the frames and previous actions the acts were given, the
+    actions they chose, and as next_state row t the frame of step t + 1 (or, after an episode reset, the
+    ``previous_next_state`` given; or, at T-1, the commit's).  Closing the policy closes its recorders; keep the queue
+    open while a recorder is in use."""
+    prefix = "a3c_policy"
+
+    def __init__(self, policy, queue, n):
+        from .distributed_queue.buffer_queue import A3CDeviceFIFOQueue
+        self._bind(policy, queue, A3CDeviceFIFOQueue, n, getattr(queue, "trajectory", 0))
+
+    def _frames(self, frames, name):
+        return N.as_c(frames, np.uint8, (self.n,) + self.policy.input_shape, name)
+
+    def act(self, state, previous_action, uniform=None, previous_next_state=None):
+        """``NativeA3CPolicy.act`` of the recorder's n rows, recorded as the next step of the unroll."""
+        n, st, pa, u, (action, policy, prob) = self.policy._act_args(state, previous_action, uniform)
+        self._check_rows(n)
+        pn = None if previous_next_state is None else self._frames(previous_next_state, "previous_next_state")
+        N.check(self._rfn("act")(self._r, N.ptr(st), N.ptr(pa), N.ptr(u),
+                                                  N.ptr(pn) if pn is not None else None, N.ptr(action),
+                                                  N.ptr(policy), N.ptr(prob)))
+        return dict(action=action, policy=policy, max_prob=prob)
+
+    def commit(self, reward, done, next_state, timeout_ms=-1):
+        """Moves the n recorded unrolls into the queue; reward float32 [n, T], done bool / uint8 [n, T], next_state
+        uint8 [n, 84, 84, 4] (the frames of step T-1)."""
+        rw = N.as_c(reward, np.float32, (self.n, self.T), "reward")
+        dn = N.as_c(N.as_u8(done), np.uint8, (self.n, self.T), "done")
+        ns = self._frames(next_state, "next_state")
+        N.check(self._rfn("commit")(self._r, N.ptr(rw), N.ptr(dn), N.ptr(ns), int(timeout_ms)))

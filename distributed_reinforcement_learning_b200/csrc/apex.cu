@@ -15,6 +15,7 @@
 #include "adam_learner.cuh"
 #include "apex_defs.cuh"
 #include "layer_defs.cuh"
+#include "traj_queue.cuh"
 
 namespace drl {
 
@@ -750,6 +751,50 @@ int drl_a3c_get_grads(drl_a3c* h, float* host_flat, int64_t n) { return drl_apex
 int drl_a3c_stage(drl_a3c* h, int32_t slot, const uint8_t* state, const uint8_t* next_state, const int32_t* previous_action,
                   const int32_t* action, const float* reward, const uint8_t* done) {
   return drl_apex_stage(h, slot, state, next_state, previous_action, action, reward, done, nullptr);
+}
+int drl_a3c_stage_from_queue(drl_a3c* h, int32_t slot, drl_a3c_queue* q, int32_t timeout_ms) {
+  DRL_TRY(check_handle(h, kName));
+  if (!q) { set_error("null a3c queue handle"); return DRL_ERR_INVALID; }
+  {
+    std::lock_guard<std::recursive_mutex> lk(h->mu);
+    if (h->algo != 1) { set_error("stage_from_queue: not an A3C handle"); return DRL_ERR_INVALID; }
+    DRL_TRY(check_slot(h, slot));
+    if (q->device != h->device) {
+      set_error("stage_from_queue: the queue is on device %d, the learner on device %d", q->device, h->device);
+      return DRL_ERR_INVALID;
+    }
+    if (q->T != h->B || q->A != h->A) {
+      set_error("stage_from_queue: the queue has trajectory %d, num_action %d; the learner batch %d, num_action %d",
+                q->T, q->A, h->B, h->A);
+      return DRL_ERR_INVALID;
+    }
+  }
+  // wait for a record without the learner's lock: actor threads sync their engines from this learner meanwhile
+  int qs = 0;
+  std::vector<cudaEvent_t> ev_commit;
+  DRL_TRY(traj_queue_pop(q, timeout_ms, &qs, &ev_commit));
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  NvtxRange nv("drl:a3c_stage_from_queue");
+  AdamSlot& s = h->slots[slot];
+  const ApexIn& in = h->in[slot];
+  const int rc = [&]() -> int {
+    DRL_CUDA_CHECK(cudaSetDevice(h->device));
+    // do not overwrite a slot the compute stream is still reading; do not read a record whose commit copies are pending
+    DRL_CUDA_CHECK(cudaStreamWaitEvent(h->copy, s.consumed, 0));
+    for (cudaEvent_t e : ev_commit) DRL_CUDA_CHECK(cudaStreamWaitEvent(h->copy, e, 0));
+    // the queue slot is an ApexIn of B = T rows: field by field, the same bytes drl_a3c_stage uploads
+    void* const dst[kApexQFields] = {in.frames, in.pa2, in.reward, in.done};
+    for (int f = 0; f < kApexQFields; ++f)
+      DRL_CUDA_CHECK(cudaMemcpyAsync(dst[f], q->field(qs, f), q->sz[f], cudaMemcpyDeviceToDevice, h->copy));
+    // unit weights, as stage_into stages them: a captured graph never depends on which entry point fed the slot
+    DRL_CUDA_CHECK(cudaMemcpyAsync(in.weight, h->h_ones, (size_t)h->B * 4, cudaMemcpyHostToDevice, h->copy));
+    DRL_CUDA_CHECK(cudaEventRecord(s.staged, h->copy));
+    s.has_data = true;
+    return DRL_OK;
+  }();
+  // the queue slot goes back to the producers either way (their copies into it wait for its release event)
+  const int rc_release = traj_queue_release(q, qs, h->copy);
+  return rc != DRL_OK ? rc : rc_release;
 }
 int drl_a3c_step_async(drl_a3c* h, int32_t slot) {
   DRL_TRY(check_handle(h, kName));

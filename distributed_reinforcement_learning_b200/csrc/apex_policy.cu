@@ -16,12 +16,16 @@
 //                           writes q / policy, action and q[action] / policy[action] straight into mapped pinned
 //                           memory (no D2H node)
 // Both new kernels sum in a fixed order without atomics: eager and graph replays, and repeated calls, are bitwise equal.
+//
+// The A3C recorder (drl_a3c_policy_recorder_*, DESIGN.md section 15) runs this act unchanged and then one more kernel,
+// a3c_record_step, that writes the step into its staging of n unrolls in the device A3C queue's record layout.
 #include <string.h>
 
 #include "apex_defs.cuh"
 #include "policy_core.cuh"
 #include "policy_head.cuh"
 #include "policy_lstm.cuh"
+#include "queue_recorder.cuh"
 
 namespace drl {
 namespace {
@@ -172,6 +176,49 @@ __global__ void __launch_bounds__(kApexHeadThreads, 1) apex_policy_head_kernel(c
   }
 }
 
+// ---- a3c_record_step --------------------------------------------------------------------------------------------
+// Step t of the A3C recorder's n unrolls, one CTA per row, 16-byte copies, after the act's head in stream order.  Row i
+// of the staging (the queue's record layout, ApexQueueField) gets: state row t <- the act's frame; pa2[t] <- its
+// previous action; pa2[T + t] <- the action the head sampled (read from the engine's mapped outputs); and for t >= 1
+// next_state row t-1 <- the same frame, or the host's reset frame when the host flagged the row (its previous
+// next_state differed from this state: an episode reset).  The step and the flags are read from mapped host memory at
+// run time, so one captured graph replays every step; a flagged row's frame crosses PCIe only then.
+constexpr int kA3CRecThreads = 256;
+
+struct A3CRecordArgs {
+  const uint8_t* frames;       // the act's input frames [n] (engine input block)
+  const int32_t* pa;           // [n]
+  const int32_t* action;       // [n] the head's actions (mapped)
+  const int32_t* ctl;          // mapped: [0] the step t, [1 + i] nonzero when row i's next_state of step t-1 is reset[i]
+  const uint8_t* reset;        // mapped [n] frames
+  uint8_t* rec_frames;         // staging [n][2T] frames
+  int32_t* rec_pa2;            // staging [n][2T]
+  int T;
+};
+
+__global__ void __launch_bounds__(kA3CRecThreads) a3c_record_step_kernel(const A3CRecordArgs a) {
+  kernel_prologue();
+  constexpr int kF16 = Geo::FRAME / 16;
+  const int row = blockIdx.x, tid = threadIdx.x, t = a.ctl[0];
+  const bool from_reset = t > 0 && a.ctl[1 + row] != 0;
+  const uint4* f = reinterpret_cast<const uint4*>(a.frames) + (size_t)row * kF16;
+  const uint4* fr = reinterpret_cast<const uint4*>(a.reset) + (size_t)row * kF16;
+  uint4* st = reinterpret_cast<uint4*>(a.rec_frames) + ((size_t)row * 2 * a.T + t) * kF16;
+  uint4* nx = reinterpret_cast<uint4*>(a.rec_frames) + ((size_t)row * 2 * a.T + a.T + t - 1) * kF16;
+  const bool next_is_frame = t > 0 && !from_reset;
+  for (int i = tid; i < kF16; i += kA3CRecThreads) {
+    const uint4 v = f[i];
+    st[i] = v;
+    if (next_is_frame) nx[i] = v;
+  }
+  if (from_reset)
+    for (int i = tid; i < kF16; i += kA3CRecThreads) nx[i] = fr[i];
+  if (tid == 0) {
+    a.rec_pa2[(size_t)row * 2 * a.T + t] = a.pa[row];
+    a.rec_pa2[(size_t)row * 2 * a.T + a.T + t] = a.action[row];
+  }
+}
+
 // ---- handle -----------------------------------------------------------------------------------------------------
 // device input block of one call with n rows, one contiguous H2D: [frames | previous_action | explore (i32) or uniform
 // (f64)]
@@ -208,6 +255,18 @@ struct drl_apex_policy : PolicyCore {
   int algo = 0;   // 0 = Ape-X, 1 = A3C
   // mapped outputs: q / policy [max_batch][A] | action | q[action] / policy[action]
   size_t off_act = 0, off_sel = 0;
+};
+
+// the recorder's staging (RecorderCore) is in the A3C queue's field order (ApexQueueField)
+struct drl_a3c_policy_recorder : RecorderCore {
+  drl_apex_policy* policy = nullptr;
+  // mapped pinned block: control words [1 + n] i32 (a3c_record_step_kernel's ctl) | n frames, the reset frames of an
+  // act and the final next_state frames of a commit
+  uint8_t* h_blk = nullptr;
+  uint8_t* d_blk = nullptr;
+  size_t off_frames = 0;
+  int32_t* ctl() { return reinterpret_cast<int32_t*>(h_blk); }
+  uint8_t* frames() { return h_blk + off_frames; }
 };
 
 namespace {
@@ -257,16 +316,58 @@ int check_act(drl_apex_policy* h, int algo, int32_t n, const uint8_t* state, con
   return policy_check_actions(h, n, previous_action, nullptr);
 }
 
-// stages frames and previous actions (the row selectors are already staged), runs the call, copies the outputs out
-int run_act(drl_apex_policy* h, int n, const uint8_t* state, const int32_t* previous_action, int32_t* action,
-            float* out, float* out_action) {
+// stages frames and previous actions (the row selectors are already staged)
+void stage_rows(drl_apex_policy* h, int n, const uint8_t* state, const int32_t* previous_action) {
   const ApexInLayout l = apex_in_layout(n);
   memcpy(h->h_in + l.frames, state, (size_t)n * Geo::FRAME);
   memcpy(h->h_in + l.pa, previous_action, (size_t)n * 4);
-  DRL_TRY(policy_run_act(h, n));
+}
+
+void copy_outputs(const drl_apex_policy* h, int n, int32_t* action, float* out, float* out_action) {
   if (out) memcpy(out, h->h_out, (size_t)n * h->A * 4);
   if (action) memcpy(action, h->h_out + h->off_act, (size_t)n * 4);
   if (out_action) memcpy(out_action, h->h_out + h->off_sel, (size_t)n * 4);
+}
+
+// stages frames and previous actions (the row selectors are already staged), runs the call, copies the outputs out
+int run_act(drl_apex_policy* h, int n, const uint8_t* state, const int32_t* previous_action, int32_t* action,
+            float* out, float* out_action) {
+  stage_rows(h, n, state, previous_action);
+  DRL_TRY(policy_run_act(h, n));
+  copy_outputs(h, n, action, out, out_action);
+  return DRL_OK;
+}
+
+// drl_a3c_policy_act's checks of its inputs and the staging of its uniforms (the caller holds the engine's lock)
+int check_stage_a3c(drl_apex_policy* h, int n, const uint8_t* state, const int32_t* previous_action,
+                    const double* uniform) {
+  DRL_TRY(check_act(h, 1, n, state, previous_action));
+  if (!uniform) { set_error("act: null input pointer (uniform: one draw in [0, 1) per row)"); return DRL_ERR_INVALID; }
+  for (int i = 0; i < n; ++i) {
+    if (!(uniform[i] >= 0.0 && uniform[i] < 1.0)) {
+      set_error("act: uniform[%d] = %g is outside [0, 1)", i, uniform[i]);
+      return DRL_ERR_INVALID;
+    }
+  }
+  memcpy(h->h_in + apex_in_layout(n).sel, uniform, (size_t)n * 8);
+  return DRL_OK;
+}
+
+// the recorder's step: the plain act of its n rows, then a3c_record_step
+int enqueue_a3c_record(drl_a3c_policy_recorder* r) {
+  drl_apex_policy* h = r->policy;
+  DRL_TRY(enqueue_act(h, r->n));
+  const ApexInLayout l = apex_in_layout(r->n);
+  A3CRecordArgs a;
+  a.frames = h->d_in + l.frames;
+  a.pa = reinterpret_cast<const int32_t*>(h->d_in + l.pa);
+  a.action = reinterpret_cast<const int32_t*>(h->d_out + h->off_act);
+  a.ctl = reinterpret_cast<const int32_t*>(r->d_blk);
+  a.reset = r->d_blk + r->off_frames;
+  a.rec_frames = r->field(kApexQFrames);
+  a.rec_pa2 = reinterpret_cast<int32_t*>(r->field(kApexQPa2));
+  a.T = r->T;
+  DRL_CUDA_CHECK((launch_k(a3c_record_step_kernel, r->n, kA3CRecThreads, 0, h->stream, a)));
   return DRL_OK;
 }
 
@@ -343,17 +444,119 @@ int drl_a3c_policy_act(drl_a3c_policy* h, int32_t n, const uint8_t* state, const
                        const double* uniform, int32_t* action, float* policy, float* prob_action) {
   DRL_TRY(policy_check(h, kName));
   std::lock_guard<std::recursive_mutex> lk(h->mu);
-  DRL_TRY(check_act(h, 1, n, state, previous_action));
-  if (!uniform) { set_error("act: null input pointer (uniform: one draw in [0, 1) per row)"); return DRL_ERR_INVALID; }
-  for (int i = 0; i < n; ++i) {
-    if (!(uniform[i] >= 0.0 && uniform[i] < 1.0)) {
-      set_error("act: uniform[%d] = %g is outside [0, 1)", i, uniform[i]);
-      return DRL_ERR_INVALID;
-    }
-  }
+  DRL_TRY(check_stage_a3c(h, n, state, previous_action, uniform));
   NvtxRange nv("drl:a3c_policy_act");
-  memcpy(h->h_in + apex_in_layout(n).sel, uniform, (size_t)n * 8);
   return run_act(h, n, state, previous_action, action, policy, prob_action);
+}
+
+// ---- A3C recorder -----------------------------------------------------------------------------------------------
+int drl_a3c_policy_recorder_destroy(drl_a3c_policy_recorder* r) {
+  if (!r) return DRL_OK;
+  {
+    std::lock_guard<std::recursive_mutex> lk(r->engine->mu);
+    cudaSetDevice(r->engine->device);
+    recorder_core_release(r);   // waits for the engine's stream: nothing reads h_blk any more
+    if (r->h_blk) cudaFreeHost(r->h_blk);
+  }
+  delete r;
+  return DRL_OK;
+}
+
+int drl_a3c_policy_recorder_create(drl_a3c_policy* h, drl_a3c_queue* q, int32_t n, drl_a3c_policy_recorder** out) {
+  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
+  *out = nullptr;
+  if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
+  DRL_TRY(policy_check(h, kName));
+  if (!q) { set_error("null a3c queue handle"); return DRL_ERR_INVALID; }
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  if (h->algo != 1) { set_error("recorder: this policy is Ape-X; an A3C recorder needs an A3C engine (algo 1)"); return DRL_ERR_INVALID; }
+  if (n < 1 || n > h->max_batch) {
+    set_error("recorder: n must be in [1, %d] (the engine's max_batch; got %d)", h->max_batch, n);
+    return DRL_ERR_INVALID;
+  }
+  if (q->device != h->device) {
+    set_error("recorder: the queue is on device %d, the policy on device %d", q->device, h->device);
+    return DRL_ERR_INVALID;
+  }
+  if (q->A != h->A) { set_error("recorder: the queue has num_action %d, the policy %d", q->A, h->A); return DRL_ERR_INVALID; }
+  if (n > traj_queue_max_rows(q)) {
+    set_error("recorder: %d rows per commit can never fit in the queue (at most %d)", n, traj_queue_max_rows(q));
+    return DRL_ERR_INVALID;
+  }
+  NvtxRange nv("drl:a3c_policy_recorder_create");
+  drl_a3c_policy_recorder* r = new drl_a3c_policy_recorder();
+  r->engine = r->policy = h;
+  r->q = q;
+  r->n = n;
+  r->T = q->T;
+  r->f_reward = kApexQReward;
+  r->f_done = kApexQDone;
+  r->commit_range = "drl:a3c_policy_recorder_commit";
+  const int rc = [&]() -> int {
+    DRL_TRY(recorder_core_init(r));
+    r->off_frames = align_up((size_t)(1 + n) * 4, 256);
+    const size_t bytes = r->off_frames + (size_t)n * Geo::FRAME;
+    DRL_CUDA_CHECK(cudaHostAlloc((void**)&r->h_blk, bytes, cudaHostAllocMapped));
+    memset(r->h_blk, 0, bytes);
+    DRL_CUDA_CHECK(cudaHostGetDevicePointer((void**)&r->d_blk, r->h_blk, 0));
+    return DRL_OK;
+  }();
+  if (rc != DRL_OK) {
+    const std::string keep = get_error();
+    drl_a3c_policy_recorder_destroy(r);
+    set_error("%s", keep.c_str());
+    return rc;
+  }
+  *out = r;
+  return DRL_OK;
+}
+
+int drl_a3c_policy_recorder_act(drl_a3c_policy_recorder* r, const uint8_t* state, const int32_t* previous_action,
+                                const double* uniform, const uint8_t* previous_next_state, int32_t* action,
+                                float* policy, float* prob_action) {
+  if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
+  drl_apex_policy* h = r->policy;
+  std::lock_guard<std::recursive_mutex> lk(h->mu);
+  DRL_TRY(recorder_check_step(r));
+  DRL_TRY(check_stage_a3c(h, r->n, state, previous_action, uniform));
+  if (r->t > 0 && !previous_next_state) {
+    set_error("recorder act: null previous_next_state (step %d needs the next_state of step %d)", r->t, r->t - 1);
+    return DRL_ERR_INVALID;
+  }
+  NvtxRange nv("drl:a3c_policy_recorder_act");
+  // the previous act waited for the stream: the mapped block is free.  A row's next_state of step t-1 is this act's
+  // frame unless the environment was reset in between; only then does the host frame go up.
+  int32_t* ctl = r->ctl();
+  ctl[0] = r->t;
+  for (int i = 0; r->t > 0 && i < r->n; ++i) {
+    const uint8_t* prev = previous_next_state + (size_t)i * Geo::FRAME;
+    ctl[1 + i] = memcmp(prev, state + (size_t)i * Geo::FRAME, Geo::FRAME) != 0;
+    if (ctl[1 + i]) memcpy(r->frames() + (size_t)i * Geo::FRAME, prev, Geo::FRAME);
+  }
+  stage_rows(h, r->n, state, previous_action);
+  DRL_TRY(recorder_run_act(r, [r] { return enqueue_a3c_record(r); }));
+  copy_outputs(h, r->n, action, policy, prob_action);
+  return DRL_OK;
+}
+
+int drl_a3c_policy_recorder_commit(drl_a3c_policy_recorder* r, const float* reward, const uint8_t* done,
+                                   const uint8_t* next_state, int32_t timeout_ms) {
+  if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
+  if (!next_state) { set_error("recorder commit: null argument"); return DRL_ERR_INVALID; }
+  // next_state row T-1 of each unroll: the frames env.step returned at step T-1, which no later act sees.  One strided
+  // H2D writes row i's frame at its record's last next_state row.
+  return recorder_commit(r, reward, done, timeout_ms, [r, next_state]() -> int {
+    const size_t F = Geo::FRAME, T = r->T;
+    memcpy(r->frames(), next_state, (size_t)r->n * F);   // every act since the last commit waited for the stream
+    DRL_CUDA_CHECK(cudaMemcpy2DAsync(r->field(kApexQFrames) + (2 * T - 1) * F, 2 * T * F, r->frames(), F, F, r->n,
+                                     cudaMemcpyHostToDevice, r->policy->stream));
+    return DRL_OK;
+  });
+}
+
+int drl_a3c_policy_recorder_reset(drl_a3c_policy_recorder* r) {
+  if (!r) { set_error("null recorder handle"); return DRL_ERR_INVALID; }
+  return recorder_reset(r);
 }
 
 }  // extern "C"

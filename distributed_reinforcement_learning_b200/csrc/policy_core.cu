@@ -251,7 +251,8 @@ int recorder_run_act(RecorderCore* r, const std::function<int()>& enqueue_step) 
   return DRL_OK;
 }
 
-int recorder_commit(RecorderCore* r, const float* reward, const uint8_t* done, int timeout_ms) {
+int recorder_commit(RecorderCore* r, const float* reward, const uint8_t* done, int timeout_ms,
+                    const std::function<int()>& before_copies) {
   if (!reward || !done) { set_error("recorder commit: null argument"); return DRL_ERR_INVALID; }
   PolicyCore* h = r->engine;
   {
@@ -276,6 +277,7 @@ int recorder_commit(RecorderCore* r, const float* reward, const uint8_t* done, i
     DRL_CUDA_CHECK(cudaSetDevice(h->device));
     DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(r->f_reward), r->h_rd, nT * 4, cudaMemcpyHostToDevice, s));
     DRL_CUDA_CHECK(cudaMemcpyAsync(r->field(r->f_done), r->h_rd + nT * 4, nT, cudaMemcpyHostToDevice, s));
+    if (before_copies) DRL_TRY(before_copies());
     for (const TrajSegment& g : segs) {
       DRL_CUDA_CHECK(cudaStreamWaitEvent(s, g.ev_release, 0));
       for (int f = 0; f < q->nfields; ++f)

@@ -3,7 +3,8 @@
 // device staging of n records in the queue's field order, the step word the recording kernels read, the graph that
 // replays every step, the recording act's driver and the commit.  The IMPALA recorder (policy.cu: drl_policy_recorder)
 // and the R2D2 recorder (r2d2_policy.cu: drl_r2d2_policy_recorder) derive from RecorderCore; each adds its kernels and
-// its enqueue of one recorded step.
+// its enqueue of one recorded step.  The A3C recorder (apex_policy.cu: drl_a3c_policy_recorder) does the same, and
+// passes its commit a hook that uploads the final next_state frames.
 #pragma once
 #include <functional>
 #include <vector>
@@ -60,8 +61,11 @@ int recorder_run_act(RecorderCore* r, const std::function<int()>& enqueue_step);
 // The commit of n complete records (after step T-1; DRL_ERR_STATE otherwise): reserves n queue positions without the
 // engine's lock, then, on the engine's stream, uploads reward and done into the staging, waits for each target slot's
 // release event, copies every field of each segment device to device and records the segment's commit event.  A
-// failure after the reservation puts the queue into its failed state (traj_queue_fail).
-int recorder_commit(RecorderCore* r, const float* reward, const uint8_t* done, int timeout_ms);
+// failure after the reservation puts the queue into its failed state (traj_queue_fail).  `before_copies`, when given,
+// runs under the engine's lock after the reward / done upload and before the copies (its work goes on the engine's
+// stream); its failure counts as a failure after the reservation.
+int recorder_commit(RecorderCore* r, const float* reward, const uint8_t* done, int timeout_ms,
+                    const std::function<int()>& before_copies = nullptr);
 int recorder_reset(RecorderCore* r);
 
 }  // namespace drl

@@ -1,9 +1,10 @@
 // traj_queue.cu -- the device-resident queues behind drl_traj_queue_* (IMPALA trajectories), drl_r2d2_queue_* (R2D2
-// sequences) and drl_apex_queue_* (Ape-X local-buffer samples) (include/drl_b200.h; layout and ordering in
-// traj_queue.cuh).  Producers are policy-engine recorders (queue_recorder.cuh) and Ape-X actor buffers
-// (apex_actor_buffer.cu), the consumers are drl_learner_stage_from_queue (learner.cu), drl_r2d2_replay_add_from_queue
-// (r2d2_replay.cu) and drl_apex_replay_add_from_queue (apex_replay.cu); no record byte crosses PCIe on its way into or
-// out of a queue except the reward and done of a recorder's commit.
+// sequences), drl_apex_queue_* (Ape-X local-buffer samples) and drl_a3c_queue_* (A3C unrolls) (include/drl_b200.h;
+// layout and ordering in traj_queue.cuh).  Producers are policy-engine recorders (queue_recorder.cuh) and Ape-X actor
+// buffers (apex_actor_buffer.cu), the consumers are drl_learner_stage_from_queue (learner.cu),
+// drl_r2d2_replay_add_from_queue (r2d2_replay.cu), drl_apex_replay_add_from_queue (apex_replay.cu) and
+// drl_a3c_stage_from_queue (apex.cu); no record byte crosses PCIe on its way into or out of a queue except what a
+// recorder's commit uploads (reward and done; for A3C also the final next_state frames).
 #include <string.h>
 
 #include <algorithm>
@@ -234,6 +235,52 @@ int check_queue_device(int device) {
   return DRL_OK;
 }
 
+// drl_apex_queue_create / drl_a3c_queue_create: one record of T transitions (or steps) in ApexIn order, one record per
+// slot.  `family` prefixes the error messages ("apex queue", "a3c queue").
+template <class Q>
+int create_apex_layout_queue(const char* family, int trajectory, int num_action, int capacity, int device, Q** out,
+                             int (*destroy)(Q*)) {
+  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
+  *out = nullptr;
+  if (trajectory < 1 || trajectory > kApexQueueMaxT) {
+    set_error("%s: trajectory must be in [1, %d] (got %d)", family, kApexQueueMaxT, trajectory);
+    return DRL_ERR_INVALID;
+  }
+  if (num_action < 2 || num_action > 32) { set_error("%s: num_action must be in [2, 32] (got %d)", family, num_action); return DRL_ERR_INVALID; }
+  if (capacity < 1) { set_error("%s: capacity must be >= 1 (got %d)", family, capacity); return DRL_ERR_INVALID; }
+  DRL_TRY(check_queue_device(device));
+  Q* q = new Q();
+  q->name = family;
+  q->pop_verb = "add_from_queue";
+  q->items = "records";
+  q->T = trajectory; q->A = num_action;
+  const size_t T = trajectory;
+  size_t sz[kApexQFields];
+  sz[kApexQFrames] = 2 * T * Geo::FRAME;
+  sz[kApexQPa2] = 2 * T * 4;
+  sz[kApexQReward] = T * 4;
+  sz[kApexQDone] = T;
+  // one record per slot: a slot is an ApexIn of n = T rows
+  return finish_create(q, kApexQFields, sz, capacity, 1, device, out, destroy);
+}
+
+// drl_apex_queue_read / drl_a3c_queue_read
+int read_apex_layout_queue(QueueCore* q, int T, int k, uint8_t* state, uint8_t* next_state, int32_t* previous_action,
+                           int32_t* action, float* reward, uint8_t* done) {
+  if (!state || !next_state || !previous_action || !action) { set_error("%s read: null output pointer", q->name); return DRL_ERR_INVALID; }
+  // the slot's frames and pa2 fields hold both halves; queue_read copies them into one block each, split below
+  const size_t t = T;
+  std::vector<uint8_t> frames(2 * t * Geo::FRAME);
+  std::vector<int32_t> pa2(2 * t);
+  void* const dst[kApexQFields] = {frames.data(), pa2.data(), reward, done};
+  DRL_TRY(queue_read(q, k, dst));
+  memcpy(state, frames.data(), t * Geo::FRAME);
+  memcpy(next_state, frames.data() + t * Geo::FRAME, t * Geo::FRAME);
+  memcpy(previous_action, pa2.data(), t * 4);
+  memcpy(action, pa2.data() + t, t * 4);
+  return DRL_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -331,28 +378,7 @@ int drl_r2d2_queue_read(drl_r2d2_queue* q, int32_t k, uint8_t* state, int32_t* p
 
 int drl_apex_queue_create(int32_t trajectory, int32_t num_action, int32_t capacity, int32_t device,
                           drl_apex_queue** out) {
-  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
-  *out = nullptr;
-  if (trajectory < 1 || trajectory > kApexQueueMaxT) {
-    set_error("apex queue: trajectory must be in [1, %d] (got %d)", kApexQueueMaxT, trajectory);
-    return DRL_ERR_INVALID;
-  }
-  if (num_action < 2 || num_action > 32) { set_error("apex queue: num_action must be in [2, 32] (got %d)", num_action); return DRL_ERR_INVALID; }
-  if (capacity < 1) { set_error("apex queue: capacity must be >= 1 (got %d)", capacity); return DRL_ERR_INVALID; }
-  DRL_TRY(check_queue_device(device));
-  drl_apex_queue* q = new drl_apex_queue();
-  q->name = "apex queue";
-  q->pop_verb = "add_from_queue";
-  q->items = "records";
-  q->T = trajectory; q->A = num_action;
-  const size_t T = trajectory;
-  size_t sz[kApexQFields];
-  sz[kApexQFrames] = 2 * T * Geo::FRAME;
-  sz[kApexQPa2] = 2 * T * 4;
-  sz[kApexQReward] = T * 4;
-  sz[kApexQDone] = T;
-  // one record per slot: a slot is an ApexIn of n = T rows
-  return finish_create(q, kApexQFields, sz, capacity, 1, device, out, drl_apex_queue_destroy);
+  return create_apex_layout_queue("apex queue", trajectory, num_action, capacity, device, out, drl_apex_queue_destroy);
 }
 
 int drl_apex_queue_destroy(drl_apex_queue* q) {
@@ -367,18 +393,27 @@ int drl_apex_queue_size(drl_apex_queue* q) { return q ? queue_size(q) : 0; }
 int drl_apex_queue_read(drl_apex_queue* q, int32_t k, uint8_t* state, uint8_t* next_state, int32_t* previous_action,
                         int32_t* action, float* reward, uint8_t* done) {
   if (!q) { set_error("null apex queue handle"); return DRL_ERR_INVALID; }
-  if (!state || !next_state || !previous_action || !action) { set_error("apex queue read: null output pointer"); return DRL_ERR_INVALID; }
-  // the slot's frames and pa2 fields hold both halves; queue_read copies them into one block each, split below
-  const size_t T = q->T;
-  std::vector<uint8_t> frames(2 * T * Geo::FRAME);
-  std::vector<int32_t> pa2(2 * T);
-  void* const dst[kApexQFields] = {frames.data(), pa2.data(), reward, done};
-  DRL_TRY(queue_read(q, k, dst));
-  memcpy(state, frames.data(), T * Geo::FRAME);
-  memcpy(next_state, frames.data() + T * Geo::FRAME, T * Geo::FRAME);
-  memcpy(previous_action, pa2.data(), T * 4);
-  memcpy(action, pa2.data() + T, T * 4);
+  return read_apex_layout_queue(q, q->T, k, state, next_state, previous_action, action, reward, done);
+}
+
+int drl_a3c_queue_create(int32_t trajectory, int32_t num_action, int32_t capacity, int32_t device,
+                         drl_a3c_queue** out) {
+  return create_apex_layout_queue("a3c queue", trajectory, num_action, capacity, device, out, drl_a3c_queue_destroy);
+}
+
+int drl_a3c_queue_destroy(drl_a3c_queue* q) {
+  if (!q) return DRL_OK;
+  queue_core_release(q);
+  delete q;
   return DRL_OK;
+}
+
+int drl_a3c_queue_size(drl_a3c_queue* q) { return q ? queue_size(q) : 0; }
+
+int drl_a3c_queue_read(drl_a3c_queue* q, int32_t k, uint8_t* state, uint8_t* next_state, int32_t* previous_action,
+                       int32_t* action, float* reward, uint8_t* done) {
+  if (!q) { set_error("null a3c queue handle"); return DRL_ERR_INVALID; }
+  return read_apex_layout_queue(q, q->T, k, state, next_state, previous_action, action, reward, done);
 }
 
 }  // extern "C"

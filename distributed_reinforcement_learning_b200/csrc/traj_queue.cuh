@@ -1,13 +1,14 @@
-// traj_queue.cuh -- the device-resident queues (DESIGN.md sections 12, 13 and 14): the FIFO core they share, the
-// IMPALA trajectory queue (drl_traj_queue), the R2D2 sequence queue (drl_r2d2_queue) and the Ape-X transition queue
-// (drl_apex_queue), all in traj_queue.cu.  The producers are policy-engine recorders (queue_recorder.cuh) and the Ape-X
-// actor buffers (apex_actor_buffer.cu); the consumers are drl_learner_stage_from_queue (learner.cu),
-// drl_r2d2_replay_add_from_queue (r2d2_replay.cu) and drl_apex_replay_add_from_queue (apex_replay.cu).
+// traj_queue.cuh -- the device-resident queues (DESIGN.md sections 12 to 15): the FIFO core they share, the IMPALA
+// trajectory queue (drl_traj_queue), the R2D2 sequence queue (drl_r2d2_queue), the Ape-X transition queue
+// (drl_apex_queue) and the A3C trajectory queue (drl_a3c_queue), all in traj_queue.cu.  The producers are policy-engine
+// recorders (queue_recorder.cuh) and the Ape-X actor buffers (apex_actor_buffer.cu); the consumers are
+// drl_learner_stage_from_queue (learner.cu), drl_r2d2_replay_add_from_queue (r2d2_replay.cu),
+// drl_apex_replay_add_from_queue (apex_replay.cu) and drl_a3c_stage_from_queue (apex.cu).
 //
 // The FIFO of drl_ring (ring.cu) with its batch slots in HBM instead of pinned host memory.  A slot holds `batch` records
 // field-major, each field batch-major (`sz[f]` bytes per record), in the consumer's layout: the learner staging slot's
 // (kernels.h: Inputs) for IMPALA, R2SeqRows / R2In (r2d2_replay.cu, r2d2_defs.cuh) for R2D2, ApexIn (apex_defs.cuh) of
-// n = T rows for Ape-X (batch 1).  Queue position P (0, 1, 2, ... in reservation order) is row P % batch of slot
+// n = T rows for Ape-X and A3C (batch 1).  Queue position P (0, 1, 2, ... in reservation order) is row P % batch of slot
 // (P / batch) % nslots.
 //
 // Ordering across streams, all through events the queue owns:
@@ -28,7 +29,7 @@ namespace drl {
 enum TrajField { kTrajState = 0, kTrajReward, kTrajDone, kTrajMu, kTrajAction, kTrajPa, kTrajH, kTrajC, kTrajFields };
 // field order of an R2D2 slot (and of its recorders' staging): R2SeqRows'
 enum R2QueueField { kR2QFrames = 0, kR2QPa, kR2QAction, kR2QH, kR2QC, kR2QReward, kR2QDone, kR2QFields };
-// field order of an Ape-X slot: ApexIn's (frames [2T]: state rows, then next_state rows; pa2 [2T]: previous_action, then
+// field order of an Ape-X or A3C slot: ApexIn's (frames [2T]: state rows, then next_state rows; pa2 [2T]: previous_action, then
 // action; reward [T]; done [T])
 enum ApexQueueField { kApexQFrames = 0, kApexQPa2, kApexQReward, kApexQDone, kApexQFields };
 // the largest T of an Ape-X queue: a push passes its T ring rows to the gather kernel by value
@@ -84,6 +85,12 @@ struct drl_r2d2_queue : drl::QueueCore {
 
 struct drl_apex_queue : drl::QueueCore {
   int T = 0, A = 0;                   // transitions per record, num_action
+};
+
+// the same record as drl_apex_queue (one actor unroll of T steps), a distinct type so that neither handle is accepted
+// where the other is expected
+struct drl_a3c_queue : drl::QueueCore {
+  int T = 0, A = 0;                   // steps per record, num_action
 };
 
 namespace drl {

@@ -2,7 +2,7 @@
 trajectory queue; ``DeviceFIFOQueue`` keeps it in GPU memory) and ``SumTree`` / ``Memory`` (reference :326-416, the
 Ape-X prioritized replay memory), and the other launchers' record queues (``R2D2FIFOQueue``; ``R2D2DeviceFIFOQueue``
 keeps it in GPU memory; ``ApexFIFOQueue``; ``ApexDeviceFIFOQueue`` keeps it in GPU memory, filled from the Ape-X actor's
-``DeviceLocalBuffers``).
+``DeviceLocalBuffers``; ``A3CFIFOQueue``; ``A3CDeviceFIFOQueue`` keeps it in GPU memory).
 
 The reference keeps a ``tf.FIFOQueue`` of 9-field trajectories on the learner's CPU and dequeues a
 batch with ``batch_size`` serial ``sess.run`` RPCs, after which the launcher ``np.stack``s eight
@@ -527,6 +527,65 @@ class A3CFIFOQueue(_QueueBase):
 
     def sample_batch(self, timeout=None):
         return self._q.get_many(1, timeout)
+
+
+class A3CDeviceFIFOQueue:
+    """``A3CFIFOQueue`` with its records in GPU memory (``drl_a3c_queue_*``, DESIGN.md section 15).
+
+    Producers are A3C policy-engine recorders (``NativeA3CPolicy.recorder``): each act writes its step of every unroll
+    on the device, and a commit moves whole unrolls into the queue with device-to-device copies; only reward, done, the
+    final next_state frames and the frames of episode resets cross PCIe.  The consumer is ``a3c.Agent.train_from_queue``,
+    which stages the oldest record into the learner device to device.  Same constructor arguments as ``A3CFIFOQueue``
+    plus ``queue_size`` and ``device``.  An ``A3CFIFOQueue`` holds one record; one recorder commit places all n of its
+    unrolls at once, so this queue holds ``queue_size + 1`` records (``queue_size`` defaults to ``num_actors``; the
+    rounding is the other device queues').  ``get_size`` counts committed and not yet staged records.  There is no host
+    producer (``append_to_queue``) and no host read of a batch (``sample_batch``); ``read(k)`` copies one queued record
+    out, for tests."""
+
+    def __init__(self, trajectory_size, input_shape, output_size, num_actors, queue_size=None, device=0):
+        self.trajectory = int(trajectory_size)
+        self.input_shape = tuple(int(x) for x in input_shape)
+        if self.input_shape != (84, 84, 4):
+            raise ValueError("input_shape: expected (84, 84, 4), got %s" % (self.input_shape,))
+        self.output_size = int(output_size)
+        self.num_actors = num_actors
+        self.queue_size = int(num_actors if queue_size is None else queue_size)
+        self.max_rows = self.queue_size + 1      # records one commit can place at once
+        self.device = int(device)
+        self.sess = None
+        self._q = C.c_void_p()
+        N.check(N.lib.drl_a3c_queue_create(self.trajectory, self.output_size, self.queue_size, self.device,
+                                           C.byref(self._q)))
+
+    def close(self):
+        if getattr(self, "_q", None) is not None and self._q.value:
+            N.lib.drl_a3c_queue_destroy(self._q)
+            self._q = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def get_size(self):
+        """Records committed and not yet staged."""
+        return int(N.lib.drl_a3c_queue_size(self._q))
+
+    def set_session(self, sess):
+        """Kept for call compatibility; there is no session."""
+        self.sess = sess
+
+    def read(self, k):
+        """The k-th queued record (0 = the next one staged), copied to the host: a dict of state, next_state,
+        previous_action, action, reward, done as ``append_to_queue`` takes them."""
+        T = self.trajectory
+        out = dict(state=np.empty((T,) + self.input_shape, np.uint8),
+                   next_state=np.empty((T,) + self.input_shape, np.uint8), previous_action=np.empty(T, np.int32),
+                   action=np.empty(T, np.int32), reward=np.empty(T, np.float32), done=np.empty(T, np.uint8))
+        N.check(N.lib.drl_a3c_queue_read(self._q, int(k), *[N.ptr(a) for a in out.values()]))
+        out["done"] = out["done"].view(np.bool_)
+        return out
 
 
 class _FieldDeques:

@@ -1,6 +1,7 @@
 """The part of the IMPALA, R2D2 and Ape-X / A3C policy-engine wrappers that is the same for all three: each drives one
 ``drl_<prefix>_*`` policy handle of the C-ABI (include/drl_b200.h), and these entry points differ only in that
-prefix.  ``RecorderHandle`` is the same for the recorders of the IMPALA and R2D2 engines (``drl_<prefix>_recorder_*``)."""
+prefix.  ``RecorderHandle`` is the same for the recorders of the IMPALA, R2D2 and A3C engines
+(``drl_<prefix>_recorder_*``)."""
 import ctypes as C
 
 import numpy as np
@@ -39,8 +40,8 @@ class PolicyHandle:
     def close(self):
         # recorders first: a recorder's handle refers to this engine (the garbage collector may finalize the two in
         # either order, so the engine owns the recorders' handle boxes, not the recorders)
-        for r in getattr(self, "_recorder_handles", ()):
-            _destroy_recorder(self.prefix, r)
+        for prefix, r in getattr(self, "_recorder_handles", ()):
+            _destroy_recorder(prefix, r)
         self._recorder_handles = []
         if getattr(self, "_h", None) is not None and self._h.value:
             self._fn("destroy")(self._h)
@@ -129,6 +130,10 @@ def _destroy_recorder(prefix, handle):
 class RecorderHandle:
     """A ``drl_<prefix>_recorder_*`` handle that binds one policy engine to one device queue for n rows.  The family's
     class binds it (``_bind``) and implements ``act``."""
+    prefix = None      # the C-ABI prefix of the recorder's entry points; None: the policy's
+
+    def _prefix(self):
+        return self.prefix or self.policy.prefix
 
     def _bind(self, policy, queue, queue_type, n, T):
         """queue must be a ``queue_type``; T: its steps per record."""
@@ -139,16 +144,16 @@ class RecorderHandle:
             raise ValueError("recorder: n = %d rows, the policy serves 1..%d" % (n, policy.max_batch))
         self.policy, self.queue, self.n, self.T = policy, queue, n, int(T)
         self._r = C.c_void_p()
-        N.check(policy._fn("recorder_create")(policy._h, queue._q, n, C.byref(self._r)))
-        live = [r for r in getattr(policy, "_recorder_handles", ()) if r.value]
-        policy._recorder_handles = live + [self._r]
+        N.check(self._rfn("create")(policy._h, queue._q, n, C.byref(self._r)))
+        live = [(p, r) for p, r in getattr(policy, "_recorder_handles", ()) if r.value]
+        policy._recorder_handles = live + [(self._prefix(), self._r)]
 
     def _rfn(self, name):
-        return self.policy._fn("recorder_" + name)
+        return getattr(N.lib, "drl_%s_recorder_%s" % (self._prefix(), name))
 
     def close(self):
         if getattr(self, "_r", None) is not None:
-            _destroy_recorder(self.policy.prefix, self._r)
+            _destroy_recorder(self._prefix(), self._r)
 
     def __del__(self):
         try:

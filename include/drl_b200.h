@@ -409,6 +409,53 @@ int drl_a3c_policy_act(drl_a3c_policy* h, int32_t n, const uint8_t* state, const
 int drl_apex_policy_last_act_ms(drl_apex_policy* h, float* ms);
 
 /* ------------------------------------------------------------------------------------------
+ * Device A3C trajectory queue (new, DESIGN.md section 15): A3CFIFOQueue with its records in GPU memory.  Producers are
+ * A3C policy recorders (drl_a3c_policy_recorder_commit, below), the consumer is drl_a3c_stage_from_queue; a record never
+ * passes through the host.  A record is one actor unroll of T steps in the A3C learner's staging order (the Ape-X
+ * queue's): frames u8 [2T,84,84,4] (the state rows, then the next_state rows), previous_action then action i32 [2T],
+ * reward f32 [T], done u8 [T] (1,807,104 B at T = 32).  One record per slot.  An A3CFIFOQueue holds one record; this
+ * queue takes a capacity (one recorder commit of n unrolls needs n free records at once), rounded as the other device
+ * queues round theirs: it holds capacity + 1 records.  Thread-safe: several recorders may commit while one learner
+ * thread stages.  A distinct type from drl_apex_queue, with the same record.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct drl_a3c_queue drl_a3c_queue;
+/* trajectory in [1, 512], num_action in [2, 32], capacity >= 1 (DRL_ERR_INVALID otherwise, checked first);
+ * DRL_ERR_CUDA ("no CPU fallback") when `device` does not exist. */
+int drl_a3c_queue_create(int32_t trajectory, int32_t num_action, int32_t capacity, int32_t device, drl_a3c_queue** out);
+int drl_a3c_queue_destroy(drl_a3c_queue* q);
+/* records committed and not yet staged */
+int drl_a3c_queue_size(drl_a3c_queue* q);
+/* Synchronous copy of the k-th queued record (0 = the next to be staged) into host arrays: state, next_state u8
+ * [T,84,84,4], previous_action, action i32 [T], reward f32 [T], done u8 [T]; for tests.  DRL_ERR_INVALID for k outside
+ * [0, size), DRL_ERR_STATE while a commit into its slot is in progress. */
+int drl_a3c_queue_read(drl_a3c_queue* q, int32_t k, uint8_t* state, uint8_t* next_state, int32_t* previous_action,
+                       int32_t* action, float* reward, uint8_t* done);
+
+/* A3C recorder: binds an A3C engine (algo 1) to a device A3C queue for n <= max_batch rows, with device staging of n
+ * unrolls (36.1 MB at n = 20, T = 32).  An Ape-X engine, another device, another num_action, or an n that cannot fit
+ * the queue at once are DRL_ERR_INVALID.  Without a device, DRL_ERR_CUDA.  Destroy the recorder before its engine and
+ * queue. */
+typedef struct drl_a3c_policy_recorder drl_a3c_policy_recorder;
+int drl_a3c_policy_recorder_create(drl_a3c_policy* h, drl_a3c_queue* queue, int32_t n, drl_a3c_policy_recorder** out);
+int drl_a3c_policy_recorder_destroy(drl_a3c_policy_recorder* r);
+/* drl_a3c_policy_act of the recorder's n rows (same inputs, checks, outputs and results) that also records step t of
+ * rows 0..n-1 on the device: state row t (the frame given), previous_action[t], action[t] (the action sampled) and, for
+ * t >= 1, next_state row t-1.  previous_next_state u8 [n,84,84,4] is what env.step returned at step t-1 (ignored, and
+ * may be NULL, at t = 0).  A row whose previous_next_state equals its state (byte compare on the host) gets the device
+ * copy of its frame; otherwise (an episode reset) its previous_next_state crosses PCIe.  Steps are recorded in order
+ * t = 0..T-1; an act after step T-1 is DRL_ERR_STATE until the commit.  With use_cuda_graph one graph per recorder
+ * replays every step.  drl_a3c_policy_recorder_reset discards the steps recorded since the last commit. */
+int drl_a3c_policy_recorder_act(drl_a3c_policy_recorder* r, const uint8_t* state, const int32_t* previous_action,
+                                const double* uniform, const uint8_t* previous_next_state, int32_t* action,
+                                float* policy, float* prob_action);
+int drl_a3c_policy_recorder_reset(drl_a3c_policy_recorder* r);
+/* After step T-1 (DRL_ERR_STATE otherwise): reward f32 [n,T], done u8 [n,T] and next_state u8 [n,84,84,4] (the step
+ * T-1 results) complete the n unrolls, which are appended to the queue in row order; the n frames are uploaded with
+ * reward and done and land in next_state row T-1.  Otherwise as drl_policy_recorder_commit. */
+int drl_a3c_policy_recorder_commit(drl_a3c_policy_recorder* r, const float* reward, const uint8_t* done,
+                                   const uint8_t* next_state, int32_t timeout_ms);
+
+/* ------------------------------------------------------------------------------------------
  * Stand-alone V-trace (optimizer/vtrace.py), host-pointer convenience forms + device forms.
  * ------------------------------------------------------------------------------------------ */
 /* vtrace.from_importance_weights (optimizer/vtrace.py:71-103): time-major [T,B] float32 inputs,
@@ -909,6 +956,13 @@ int drl_a3c_stage(drl_a3c* h, int32_t slot, const uint8_t* state, const uint8_t*
                   const int32_t* previous_action, const int32_t* action, const float* reward, const uint8_t* done);
 /* sess.run([pi_loss, baseline_loss, entropy, learning_rate, train_op]) (agent/a3c.py:89-103). */
 int drl_a3c_step(drl_a3c* h, int32_t slot, drl_a3c_out* out);
+/* drl_a3c_stage of the oldest record of a device A3C queue (train_a3c.py's learner loop without a host copy): pops it
+ * without holding the learner's lock, blocking while the queue is empty (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with
+ * nothing changed otherwise), then, on the copy stream after the slot's last reader and the record's commit, copies it
+ * device to device into `slot` (weights 1, as drl_a3c_stage) and records the slot's staged event; the queue slot goes
+ * back to the producers after the copies, also when enqueueing fails.  The learner must be an A3C handle on the queue's
+ * device with batch = the queue's trajectory and the queue's num_action (DRL_ERR_INVALID). */
+int drl_a3c_stage_from_queue(drl_a3c* h, int32_t slot, drl_a3c_queue* queue, int32_t timeout_ms);
 int drl_a3c_step_async(drl_a3c* h, int32_t slot);
 int drl_a3c_wait(drl_a3c* h, drl_a3c_out* out);
 /* (new) Data-parallel halves (all three A2C losses are batch means: grad_scale = 1 / world_size). */
