@@ -141,6 +141,7 @@ def _load():
         "drl_debug_trace": (C.c_int, [vp]),
         "drl_debug_launch_plan": (C.c_int, [i32, i32, i32, vp]),
         "drl_debug_gemm16_residency": (C.c_int, [vp]),
+        "drl_debug_gemm16_local_bytes": (C.c_int, [vp]),
         "drl_learner_last_step_ms": (C.c_int, [vp, C.POINTER(f32)]),
         "drl_learner_launches_per_step": (C.c_int, [vp, C.POINTER(i32)]),
         "drl_policy_create": (C.c_int, [C.POINTER(PolicyConfig), C.POINTER(vp)]),

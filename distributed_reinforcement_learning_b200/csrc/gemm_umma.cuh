@@ -250,7 +250,9 @@ __device__ __forceinline__ void wg_epilogue(const EP& ep, const float (&acc)[BN 
                                             int row0, int n0, int M, int N) {
   constexpr int W = FOLD ? BN / 2 : BN;
   const int r = lane >> 2, q = lane & 3;
-#pragma unroll 1
+  // fully unrolled: a runtime index into acc would put the accumulator in local memory, and ptxas then serialises
+  // every wgmma of the main loop (warning C7514), which cost the 16-bit GEMMs about a quarter of their time on H100
+#pragma unroll
   for (int cb = 0; cb < W / 32; ++cb) {
 #pragma unroll
     for (int c = 0; c < 4; ++c) {

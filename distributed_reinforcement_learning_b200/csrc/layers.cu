@@ -108,6 +108,21 @@ extern "C" int drl_debug_gemm16_residency(int32_t* out) {
   return DRL_OK;
 }
 
+// Local memory per thread of three math-mode-5 GEMMs of the IMPALA step: out[0] = lstm_fwd, out[1] = lstm_dgrad,
+// out[2] = lstm_wgrad.  An accumulator that lands in local memory makes ptxas serialise every wgmma of the main loop:
+// the results stay the same, only the kernels get slower.
+extern "C" int drl_debug_gemm16_local_bytes(int32_t* out) {
+  using namespace drl;
+  if (!out) { set_error("gemm16_local_bytes: need out"); return DRL_ERR_INVALID; }
+  if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
+  cudaFuncAttributes fa[3];
+  DRL_CUDA_CHECK(cudaFuncGetAttributes(&fa[0], gemm_umma16_kernel<X256L, LstmA, PretiledB<PlainB>, EpRaw<false>>));
+  DRL_CUDA_CHECK(cudaFuncGetAttributes(&fa[1], gemm_umma16_kernel<X128D, PlainA, PretiledB<PlainBT>, EpLstmDx>));
+  DRL_CUDA_CHECK(cudaFuncGetAttributes(&fa[2], gemm_bulk16_kernel<BK256, EpRaw<false>>));
+  for (int i = 0; i < 3; ++i) out[i] = (int32_t)fa[i].localSizeBytes;
+  return DRL_OK;
+}
+
 namespace drl {
 
 size_t lstm_image_bytes(int which, int M, int Mb) {

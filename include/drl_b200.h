@@ -194,6 +194,10 @@ int drl_debug_launch_plan(int32_t B, int32_t T, int32_t mode, int32_t* out);
  * memory) of the math-mode-5 kernels sized for two per SM: out[0] / out[1] = conv2 / conv3 forward, out[2] = conv2
  * data gradient. */
 int drl_debug_gemm16_residency(int32_t* out);
+/* Test aid: local memory per thread (bytes) of three math-mode-5 GEMMs of the IMPALA step: out[0] = LSTM forward,
+ * out[1] = LSTM data gradient, out[2] = LSTM weight gradient.  A nonzero count means a wgmma accumulator left the
+ * registers, which serialises the kernel's MMAs. */
+int drl_debug_gemm16_local_bytes(int32_t* out);
 /* Test aid: arm (dev_buf: device buffer of >= 8001 uint64, word 0 = entry count, zeroed by the caller) or disarm
  * (NULL) the kernel start-time trace: CTA 0 of every kernel of the step appends {globaltimer ns, grid size << 32 |
  * block size}.  Gives the true timeline of a CUDA-graph replay across both streams (tools/timeline.py). */
