@@ -4,6 +4,7 @@
 #include "adam_learner.cuh"
 #include "gemm_umma.cuh"
 #include "loaders.cuh"
+#include "trunk_images.cuh"
 
 namespace drl {
 
@@ -235,8 +236,7 @@ int check_which(int which) {
 // copy / set_params.  Refreshed outside of the graph so that the captured step never contains them.
 int refresh_target_images(AdamLearner* h) {
   if (h->target_images_stale && h->mode >= 2) {
-    DRL_TRY((launch_retile_b<64>(h->compute, PlainB{h->target + h->conv2_w, 64, 0}, 64, 512, h->twi.img[1])));
-    DRL_TRY((launch_retile_b<64>(h->compute, PlainB{h->target + h->conv3_w, 64, 0}, 64, 576, h->twi.img[2])));
+    DRL_TRY(conv_images_tf32(h->compute, *h->layout, h->target, h->twi.img[1], h->twi.img[2]));
   }
   h->target_images_stale = false;
   return DRL_OK;

@@ -28,8 +28,7 @@ struct AdamLearner {
   // set by the family before adam_learner_init
   int device = 0, num_slots = 2, B = 0, mode = 2;
   bool use_cuda_graph = false;
-  const FlatLayout* layout = nullptr;      // the family's layout (one network)
-  int64_t conv2_w = 0, conv3_w = 0;        // its offsets of the tensors behind the target weight images
+  const TrunkLayout* layout = nullptr;     // the family's layout (one network)
   FwdBwd fwd_bwd = nullptr;
 
   cudaStream_t compute = nullptr, copy = nullptr, side = nullptr;

@@ -197,8 +197,7 @@ static int apex_forward(const Streams& st, const ApexLayout& pl, const float* P,
          emb_forward(s, P + pl.emb1_w, P + pl.emb1_b, P + pl.emb2_w, P + pl.emb2_b, act.e1, act.table, pl.A), 1);
   if (retile_bwd && mode >= 2) {
     prof_mark(s, "weight_retile_bwd");
-    DRL_TRY((launch_retile_b<256>(s, PlainBT{P + pl.conv3_w, 64, 0}, 576, 64, wi.img[5])));
-    DRL_TRY((launch_retile_b<256>(s, PlainBT{P + pl.conv2_w, 64, 0}, 512, 64, wi.img[6])));
+    DRL_TRY(conv_dcol_images_tf32(s, pl, P, wi.img[5], wi.img[6]));
     n += 2;
   }
   s = st.main;
@@ -294,67 +293,7 @@ static int apex_backward(const Streams& st, const ApexLayout& pl, const float* P
   KERNEL("emb_bwd",
          emb_backward(s, bw.du, pa, act.e1, act.table, P + pl.emb2_w, bw.dpre2, bw.dpre1, G + pl.emb1_w,
                       G + pl.emb1_b, G + pl.emb2_w, G + pl.emb2_b, bw.wg_part, Mb, M, 1, A), 4);
-  {
-    const SplitPlan sp = plan_conv3_wgrad(Mb, mode);
-    const size_t slab = 577 * 64;
-    Conv3WA al{act.a2, map};
-    PlainB bl{bw.da3, 64, 0};
-    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 576, 64};
-    GEMM("conv3_wgrad", CfgBig, U64, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv3_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv3_w, slab), 1);
-  }
-  s = st.main;
-  if (mode >= 2) {
-    PlainA al{bw.da3, 64, 0};
-    EpRaw<false> ep{bw.dcol, 576, 0, 1.0f, 0, 576};
-    prof_mark(s, "conv3_dgrad");
-    PretiledB<PlainBT> blp{wi.img[5], 2};
-    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 49, 576, 64, 1, 64, 0)));
-    prof_mark(s, "conv3_col2im");
-    DRL_TRY(col2im_conv3(s, bw.dcol, act.a2, bw.da2, Mb));
-    n += 2;
-  } else {
-    Conv3DA al{bw.da3};
-    Conv3DB bl{P + pl.conv3_w};
-    Conv3DE ep{bw.da2, act.a2};
-    GEMM_FFMA("conv3_dgrad", CfgBig, al, bl, ep, Mb * 81, 64, 576, 1, 576, 0);
-  }
-  DRL_TRY(fork_to_side(st, 5));
-  s = side;
-  {
-    const SplitPlan sp = plan_conv2_wgrad(Mb, mode);
-    const size_t slab = 513 * 64;
-    Conv2WA al{act.a1, map};
-    PlainB bl{bw.da2, 64, 0};
-    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 512, 64};
-    GEMM("conv2_wgrad", CfgBig, U64, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv2_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv2_w, slab), 1);
-  }
-  s = st.main;
-  if (mode >= 2) {
-    PlainA al{bw.da2, 64, 0};
-    EpRaw<false> ep{bw.dcol, 512, 0, 1.0f, 0, 512};
-    prof_mark(s, "conv2_dgrad");
-    PretiledB<PlainBT> blp{wi.img[6], 2};
-    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 81, 512, 64, 1, 64, 0)));
-    prof_mark(s, "conv2_col2im");
-    DRL_TRY(col2im_conv2(s, bw.dcol, act.a1, bw.da1, Mb));
-    n += 2;
-  } else {
-    Conv2DA al{bw.da2};
-    Conv2DB bl{P + pl.conv2_w};
-    Conv2DE ep{bw.da1, act.a1};
-    GEMM_FFMA("conv2_dgrad", CfgN32, al, bl, ep, Mb * 100, 32, 256, 4, 256, 0);
-  }
-  {
-    const SplitPlan sp = plan_conv1_wgrad(Mb, mode);
-    const size_t slab = 257 * 32;
-    Conv1WA al{frames, map};
-    PlainB bl{bw.da1, 32, 0};
-    EpRaw<true> ep{bw.wg_part2, 32, slab, 1.0f / 255.0f, 256, 32};
-    GEMM("conv1_wgrad", CfgWg1, U32, al, bl, ep, 256, 32, Mb * 400, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, sp.splits, G + pl.conv1_w, slab), 1);
-  }
+  DRL_TRY(conv_backward_tf32<Geo::IC>(st, pl, P, wi, G, frames, map, Mb, act, bw, mode, &n));
   DRL_TRY(join_from_side(st, 6));
   if (launches) *launches += n;
   return DRL_OK;
@@ -371,11 +310,7 @@ constexpr const char* kName = "apex";
 int alloc_acts(drl_apex* h, ApexActs& a, int cap) {
   const size_t M = cap, A = h->A;
   a.cap = cap;
-  DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
-  DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
-  DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
-  DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
-  DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
+  DRL_TRY(alloc_trunk_acts(h, a, M, A));
   size_t zmax = 0;
   for (int m = 1; m <= cap; ++m) zmax = std::max(zmax, (size_t)plan_head1(m).splits * m * kHeadN);
   DRL_TRY(dev_alloc(h, &a.zpart, zmax));
@@ -501,7 +436,6 @@ int drl_apex_create(const drl_apex_config* cfg, drl_apex** out) {
   h->B = cfg->batch; h->A = cfg->num_action;
   h->pl.init(h->A);
   h->layout = &h->pl;
-  h->conv2_w = h->pl.conv2_w; h->conv3_w = h->pl.conv3_w;
   h->fwd_bwd = fwd_bwd;
   AdamState& o = h->opt;
   o.start_lr = cfg->start_learning_rate; o.end_lr = cfg->end_learning_rate; o.learning_frame = cfg->learning_frame;
@@ -526,16 +460,7 @@ int drl_apex_create(const drl_apex_config* cfg, drl_apex** out) {
     DRL_TRY(dev_alloc(h, &b.dmean, B * 32));
     DRL_TRY(dev_alloc(h, &b.dhid2, 2 * B * Geo::HID));
     DRL_TRY(dev_alloc(h, &b.dhid1, 2 * B * Geo::HID));
-    DRL_TRY(dev_alloc(h, &b.da3, B * Geo::FLAT));
-    DRL_TRY(dev_alloc(h, &b.du, B * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.dpre2, A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.dpre1, A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.da2, B * 81 * 64));
-    DRL_TRY(dev_alloc(h, &b.da1, B * 400 * 32));
-    const size_t wg = wgrad_partial_floats(h->B, 3);     // Mb = B * (3 - 2)
-    DRL_TRY(dev_alloc(h, &b.wg_part, wg));
-    DRL_TRY(dev_alloc(h, &b.wg_part2, wg));
-    DRL_TRY(dev_alloc(h, &b.dcol, B * 81 * 512));
+    DRL_TRY(alloc_trunk_bwd(h, b, B, A, Geo::IC, true));
     DRL_TRY(dev_alloc(h, &h->main_q, B * A));
     DRL_TRY(dev_alloc(h, &h->next_main_q, B * A));
     DRL_TRY(dev_alloc(h, &h->target_q, B * A));

@@ -37,12 +37,7 @@ constexpr int kCat = Geo::FLAT + Geo::EMB;       // 3392
 int apex_params_snapshot(drl_apex* h, int device, int algo, int num_action, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);
 
-struct ApexActs {          // forward activations of one network over up to `cap` rows (caller row order)
-  float* a1;               // [M,20,20,32]
-  float* a2;               // [M,9,9,64]
-  float* a3;               // [M,3136]
-  float* e1;               // [A,256]
-  float* table;            // [A,256]
+struct ApexActs : TrunkActs {   // forward activations of one network over up to `cap` rows (caller row order)
   float* zpart;            // [splits][M,512] split-K partial sums of the two first head layers
   float* hid1;             // [2][M,256]  value / mean stream hidden 1
   float* hid2;             // [2][M,256]
@@ -52,11 +47,9 @@ struct ApexActs {          // forward activations of one network over up to `cap
   int cap;
 };
 
-struct ApexBwd {           // backward workspace, Mb = B rows
+struct ApexBwd : TrunkBwd {     // backward workspace, Mb = B rows
   float *dq, *dmean;       // [Mb,32] each (columns >= A / >= 1 stay zero)
   float *dhid2, *dhid1;    // [2][Mb,256]
-  float *da3, *du, *dpre2, *dpre1, *da2, *da1;
-  float *wg_part, *wg_part2, *dcol;
 };
 
 struct ApexIn {                // views of one staging slot

@@ -97,12 +97,55 @@ struct Inputs {          // one device staging slot, caller's batch-major layout
   const float* c0;       // [B,T,256]
 };
 
-struct Acts {            // forward activations, time-major rows m = t*B + b, M = B*T rows
+// The trunk's forward activations over M rows and its backward workspace over Mb rows (the rows that receive gradient),
+// the bases of every learner's activation and workspace structs.
+struct TrunkActs {
   float* a1;             // [M,20,20,32]
   float* a2;             // [M,9,9,64]
   float* a3;             // [M,3136]
   float* e1;             // [A,256]  relu(emb1)
   float* table;          // [A,256]  action-embedding table
+};
+struct TrunkBwd {
+  float* da3;            // [Mb,3136]
+  float* du;             // [Mb,256]
+  float* dpre2;          // [A,256]
+  float* dpre1;          // [A,256]
+  float* da2;            // [Mb,9,9,64]
+  float* da1;            // [Mb,20,20,32]
+  float* wg_part;        // split-K partial slabs for the conv3/conv2 weight gradients (side stream) + emb scratch
+  float* wg_part2;       // split-K partial slabs for the conv1 weight gradient (main stream)
+  float* dcol = nullptr; // [Mb*81, 512] (conv2) / [Mb*49, 576] (conv3): per-output-pixel tap gradients before col2im
+                         // (math modes 2 and 3; math mode 5 computes the conv data gradients without it)
+};
+// floats of wg_part / wg_part2 for Mb rows of C-channel frames: the largest split-K slab set of the conv weight gradients
+// in any math mode, at least the scratch of emb_backward
+size_t trunk_partial_floats(int Mb, int C);
+template <class H>
+int alloc_trunk_acts(H* h, TrunkActs& a, size_t M, size_t A) {
+  DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
+  DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
+  DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
+  DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
+  DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
+  return DRL_OK;
+}
+template <class H>
+int alloc_trunk_bwd(H* h, TrunkBwd& b, size_t Mb, size_t A, int C, bool dcol) {
+  DRL_TRY(dev_alloc(h, &b.da3, Mb * Geo::FLAT));
+  DRL_TRY(dev_alloc(h, &b.du, Mb * Geo::EMB));
+  DRL_TRY(dev_alloc(h, &b.dpre2, A * Geo::EMB));
+  DRL_TRY(dev_alloc(h, &b.dpre1, A * Geo::EMB));
+  DRL_TRY(dev_alloc(h, &b.da2, Mb * 81 * 64));
+  DRL_TRY(dev_alloc(h, &b.da1, Mb * 400 * 32));
+  const size_t wg = trunk_partial_floats((int)Mb, C);
+  DRL_TRY(dev_alloc(h, &b.wg_part, wg));
+  DRL_TRY(dev_alloc(h, &b.wg_part2, wg));
+  if (dcol) DRL_TRY(dev_alloc(h, &b.dcol, Mb * 81 * 512));
+  return DRL_OK;
+}
+
+struct Acts : TrunkActs { // forward activations, time-major rows m = t*B + b, M = B*T rows
   float* zpart;          // [SPLITS][M,1024] LSTM pre-activation partial sums
   float* gates;          // [M,4,256] sigmoid(i), tanh(j), sigmoid(f+1), sigmoid(o)
   float* c1;             // [M,256]
@@ -117,7 +160,7 @@ struct Acts {            // forward activations, time-major rows m = t*B + b, M 
   uint8_t* img_xt = nullptr;   // x^T : rows = features (3648) x K = Mb rows -- A operand of lstm_wgrad
 };
 
-struct Bwd {             // backward workspace, Mb = B*(T-2) rows
+struct Bwd : TrunkBwd {  // backward workspace, Mb = B*(T-2) rows
   float* dlogits;        // [Mb,32] (columns >= A stay zero)
   float* dv;             // [Mb,32] (column 0 = dL/dV, others stay zero)
   float* dhid2;          // [2][Mb,256]
@@ -125,17 +168,7 @@ struct Bwd {             // backward workspace, Mb = B*(T-2) rows
   float* dh_part;        // [2][Mb,256] actor and critic contributions to dL/dh1
   float* dz;             // [Mb,1024]
   uint8_t* img_dzt = nullptr;  // dz^T : rows n (1024) x K = Mb rows  -- B operand of the bulk-fed lstm_wgrad (see Acts::img_xt)
-  float* da3;            // [Mb,3136]
-  float* du;             // [Mb,256]
-  float* dpre2;          // [A,256]
-  float* dpre1;          // [A,256]
-  float* da2;            // [Mb,9,9,64]
-  float* da1;            // [Mb,20,20,32]
-  float* wg_part;        // split-K partial slabs for the conv3/conv2 weight gradients (side stream) + emb scratch
-  float* wg_part2;       // split-K partial slabs for the conv1 weight gradient (main stream)
-  float* dcol = nullptr; // [Mb*81, 512] (conv2) / [Mb*49, 576] (conv3): per-output-pixel tap gradients before col2im
-                         // (math modes 2 and 3; math mode 5 computes the conv data gradients without it)
-  size_t wg_part_floats;
+  size_t wg_part_floats; // floats of wg_part / wg_part2 (checked by the conv1 weight gradient of math mode 5)
   float* emb_scratch = nullptr;   // own scratch of emb_backward (16 * 32 * 256 floats): lets it run on the second side lane
                                   // beside the conv weight gradients; nullptr: it borrows wg_part on `side`
 };
@@ -197,7 +230,6 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* params, c
                 const Acts& act, int B, int T, int mode, bool retile);
 int net_backward(const Streams& st, const ParamLayout& pl, const float* params, const WeightImages& wi, float* grads,
                  const Inputs& in, const Acts& act, const Bwd& bwd, int B, int T, int mode);
-size_t wgrad_partial_floats(int B, int T);
 // bytes of the operand images of the bulk-fed lstm_wgrad: which = 1 x^T (K = Mb), 3 dz^T (K = Mb)
 size_t lstm_image_bytes(int which, int M, int Mb);
 int forward_launch_count();

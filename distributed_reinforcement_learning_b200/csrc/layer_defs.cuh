@@ -1,6 +1,7 @@
-// layer_defs.cuh -- loader / tile-configuration instantiations, launch macros and split-K plans shared by the
-// IMPALA actor-critic (layers.cu) and the Ape-X dueling network (apex.cu): both run the same attention_CNN
-// (model/impala_actor_critic.py:5-10 == model/apex_value.py:4-9) through the same gather-GEMM kernels.
+// layer_defs.cuh -- loader / tile-configuration instantiations, launch macros, split-K plans and the conv trunk's
+// forward and backward shared by the IMPALA actor-critic (layers.cu), the Ape-X / A3C network (apex.cu) and the R2D2
+// network (r2d2.cu): all run the same attention_CNN (model/impala_actor_critic.py:5-10 == model/apex_value.py:4-9)
+// through the same gather-GEMM kernels.
 #pragma once
 #include <algorithm>
 
@@ -12,6 +13,7 @@
 #include "gemm_umma_persist.cuh"
 #include "kernels.h"
 #include "loaders.cuh"
+#include "trunk_images.cuh"
 
 namespace drl {
 
@@ -150,6 +152,11 @@ static SplitPlan plan_split(int K, int tiles_mn, int bk, int waves) {
 static SplitPlan plan_conv1_wgrad(int Mb, int mode) {
   return mode >= 2 ? plan_split(Mb * 400, 2, 32, 2) : plan_split(Mb * 400, cdiv(256, CfgWg1::BM), 16, 2);
 }
+// conv1 weight gradient with single-channel frames (R2D2) is a [64 x 32] output with K = Mb*400: half of a 128-row MMA
+// tile would be padding and the producers, not the tensor pipe, set the pace on the 128-row tensor-core core.  A 64 x 32
+// FFMA tile with the reduction split over ~4 CTAs per SM fits the shape in both math modes.
+using CfgWgC1 = TileCfg<64, 32, 16, 4, 4>;
+static SplitPlan plan_conv1_wgrad_c1(int Mb) { return plan_split(Mb * 400, 1, 16, 4); }
 static SplitPlan plan_conv2_wgrad(int Mb, int mode) {
   if (mode == 5) return plan_split(Mb * 81, 4, 64, 2);
   return mode >= 2 ? plan_split(Mb * 81, 4, 32, 2) : plan_split(Mb * 81, cdiv(512, CfgBig::BM), 16, 2);
@@ -159,12 +166,12 @@ static SplitPlan plan_conv3_wgrad(int Mb, int mode) {
   return mode >= 2 ? plan_split(Mb * 49, 5, 32, 2) : plan_split(Mb * 49, cdiv(576, CfgBig::BM), 16, 2);
 }
 
-// The conv1 / conv2 / conv3 forward of the Ape-X / A3C and R2D2 networks over B sequences of S frames of C channels
-// (rows m = t*B + b; S = 1: the caller's row order) on stream s, with the learner's kernels and configurations for math
-// mode `mode` (1: FP32 FFMA; 2: wgmma 3xTF32 with the conv2 / conv3 weight images of conv_images_tf32).  When
-// images_ready is not null, conv2 waits for it (the images are built on another stream).  `tgt` only names the launches
-// for the per-kernel profile; adds the launches to *launches.  Defined here so that each learner (apex.cu, r2d2.cu)
-// instantiates the kernels it launches; the policy engines reach it through policy_conv_forward_tf32 (r2d2.cu).
+// The conv1 / conv2 / conv3 forward of every network's trunk over B sequences of S frames of C channels (rows m = t*B + b;
+// S = 1: the caller's row order) on stream s, with the learner's kernels and configurations for math mode `mode` (1: FP32
+// FFMA; 2 and 3: wgmma 3xTF32 with the conv2 / conv3 weight images of conv_images_tf32).  When images_ready is not null,
+// conv2 waits for it (the images are built on another stream).  `tgt` only names the launches for the per-kernel
+// profile; adds the launches to *launches.  Defined here so that each learner (layers.cu, apex.cu, r2d2.cu) instantiates
+// the kernels it launches; the Ape-X / A3C and R2D2 policy engines reach it through policy_conv_forward_tf32 (r2d2.cu).
 template <int C>
 int conv_forward_tf32(cudaStream_t s, const TrunkLayout& pl, const float* P, const uint8_t* img_conv2,
                       const uint8_t* img_conv3, const uint8_t* frames, int B, int S, float* a1, float* a2, float* a3,
@@ -197,15 +204,6 @@ int conv_forward_tf32(cudaStream_t s, const TrunkLayout& pl, const float* P, con
   return DRL_OK;
 }
 
-// the conv2 / conv3 forward weight images of math mode 2 (WeightImages slots 1 and 2 sizes); a template like
-// conv_forward_tf32, so that only the translation units that call it instantiate its kernel
-template <class Layout>
-int conv_images_tf32(cudaStream_t s, const Layout& pl, const float* P, uint8_t* img_conv2, uint8_t* img_conv3) {
-  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, img_conv2)));
-  DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, img_conv3)));
-  return DRL_OK;
-}
-
 // Fork/join helpers: kernels that are off the critical path (the action-embedding table in the forward, every
 // weight gradient except conv1's in the backward) run on the side stream so they fill SMs the critical
 // dgrad chain leaves idle.  Inside CUDA-graph capture the event record/wait pairs become graph edges.
@@ -232,6 +230,91 @@ static inline int join_from_side(const Streams& st, int i) {
   if (!st.par) return DRL_OK;
   DRL_CUDA_CHECK(cudaEventRecord(st.ev[i], st.side));
   DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[i], 0));
+  return DRL_OK;
+}
+
+// The conv trunk backward in math modes 1 to 3 over Mb rows (row order `map`, the forward's), from "da3 ready on main,
+// side forked at ev[4]" to the conv1 weight-gradient reduce: the conv3 / conv2 weight gradients on the side stream, the
+// data gradients on main (modes 2 and 3: the dCol GEMM with the img[5] / img[6] images of conv_dcol_images_tf32, then
+// col2im; mode 1: the FFMA gather), then conv1's weight gradient on main.  The caller joins side back at ev[6].  Adds
+// the launches to *launches; a template like conv_forward_tf32.
+template <int C>
+int conv_backward_tf32(const Streams& st, const TrunkLayout& pl, const float* P, const WeightImages& wi, float* G,
+                       const uint8_t* frames, RowMap map, int Mb, const TrunkActs& act, const TrunkBwd& bw, int mode,
+                       int* launches) {
+  cudaStream_t s = st.par ? st.side : st.main;
+  int n = 0;
+  {
+    const SplitPlan sp = plan_conv3_wgrad(Mb, mode);
+    const size_t slab = 577 * 64;
+    Conv3WA al{act.a2, map};
+    PlainB bl{bw.da3, 64, 0};
+    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 576, 64};
+    GEMM("conv3_wgrad", CfgBig, U64, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
+    KERNEL("conv3_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv3_w, slab), 1);
+  }
+  s = st.main;
+  if (mode >= 2) {
+    // "dCol" form: one plain GEMM with K = 64 output channels (instead of gathering every dY value 9 times
+    // through the producers), then a gather of <= 9 taps per input pixel with the ReLU mask.  K = 64 (two K tiles) and
+    // 128 x 256 outputs per tile: epilogue-dominated, so the persistent kernel whose dedicated epilogue warps wins here
+    // while the producers gather the next tile.
+    PlainA al{bw.da3, 64, 0};
+    EpRaw<false> ep{bw.dcol, 576, 0, 1.0f, 0, 576};
+    prof_mark(s, "conv3_dgrad");
+    PretiledB<PlainBT> blp{wi.img[5], 2};   // B(k = co, n = (ky,kx,ci)) = W[n*64 + co]
+    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 49, 576, 64, 1, 64, 0)));
+    prof_mark(s, "conv3_col2im");
+    DRL_TRY(col2im_conv3(s, bw.dcol, act.a2, bw.da2, Mb));
+    n += 2;
+  } else {
+    Conv3DA al{bw.da3};
+    Conv3DB bl{P + pl.conv3_w};
+    Conv3DE ep{bw.da2, act.a2};
+    GEMM_FFMA("conv3_dgrad", CfgBig, al, bl, ep, Mb * 81, 64, 576, 1, 576, 0);
+  }
+  DRL_TRY(fork_to_side(st, 5));
+  s = st.par ? st.side : st.main;
+  {
+    const SplitPlan sp = plan_conv2_wgrad(Mb, mode);
+    const size_t slab = 513 * 64;
+    Conv2WA al{act.a1, map};
+    PlainB bl{bw.da2, 64, 0};
+    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 512, 64};
+    GEMM("conv2_wgrad", CfgBig, U64, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
+    KERNEL("conv2_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv2_w, slab), 1);
+  }
+  s = st.main;
+  if (mode >= 2) {
+    PlainA al{bw.da2, 64, 0};
+    EpRaw<false> ep{bw.dcol, 512, 0, 1.0f, 0, 512};
+    prof_mark(s, "conv2_dgrad");                      // persistent kernel: 0.079 vs 0.091 ms
+    PretiledB<PlainBT> blp{wi.img[6], 2};
+    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 81, 512, 64, 1, 64, 0)));
+    prof_mark(s, "conv2_col2im");
+    DRL_TRY(col2im_conv2(s, bw.dcol, act.a1, bw.da1, Mb));
+    n += 2;
+  } else {
+    Conv2DA al{bw.da2};
+    Conv2DB bl{P + pl.conv2_w};
+    Conv2DE ep{bw.da1, act.a1};
+    GEMM_FFMA("conv2_dgrad", CfgN32, al, bl, ep, Mb * 100, 32, 256, 4, 256, 0);
+  }
+  // conv1 (input is data: weight gradient only), own partial buffer: runs beside the side stream
+  ConvWgradA<uint8_t, 84, 84, C, 20, 20, 8, 4, true> al{frames, map};
+  PlainB bl{bw.da1, 32, 0};
+  const size_t slab = (64 * C + 1) * 32;
+  EpRaw<true> ep{bw.wg_part2, 32, slab, 1.0f / 255.0f, 64 * C, 32};
+  if constexpr (C == 1) {
+    const SplitPlan sp = plan_conv1_wgrad_c1(Mb);
+    GEMM_FFMA("conv1_wgrad", CfgWgC1, al, bl, ep, 64, 32, Mb * 400, sp.splits, sp.kchunk, sp.kchunk);
+    KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, sp.splits, G + pl.conv1_w, slab), 1);
+  } else {
+    const SplitPlan sp = plan_conv1_wgrad(Mb, mode);
+    GEMM("conv1_wgrad", CfgWg1, U32, al, bl, ep, 256, 32, Mb * 400, sp.splits, sp.kchunk, sp.kchunk);
+    KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, sp.splits, G + pl.conv1_w, slab), 1);
+  }
+  *launches += n;
   return DRL_OK;
 }
 

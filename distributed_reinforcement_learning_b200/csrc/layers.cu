@@ -44,14 +44,14 @@ int forward_launch_count() { return g_fwd_launches; }
 int backward_launch_count() { return g_bwd_launches; }
 
 
-size_t wgrad_partial_floats(int B, int T) {
-  const int Mb = B * (T - 2);
+size_t trunk_partial_floats(int Mb, int C) {
   size_t mx = 0;
   for (int mode : {1, 2, 3, 5}) {
     mx = std::max(mx, (size_t)plan_conv1_wgrad(Mb, mode).splits * 257 * 32);
     mx = std::max(mx, (size_t)plan_conv2_wgrad(Mb, mode).splits * 513 * 64);
     mx = std::max(mx, (size_t)plan_conv3_wgrad(Mb, mode).splits * 577 * 64);
   }
+  if (C == 1) mx = std::max(mx, (size_t)plan_conv1_wgrad_c1(Mb).splits * 65 * 32);
   return std::max(mx, (size_t)16 * 32 * 256);   // also the scratch of emb_backward (kEmbChunks * A * 256)
 }
 
@@ -163,9 +163,7 @@ int net_retile(cudaStream_t, cudaStream_t s_rest, const ParamLayout& pl, const f
   prof_mark(s_rest, "weight_retile");
   DRL_TRY((launch_retile_b<256>(s_rest, PlainB{P + pl.lstm_w, Geo::G4, 0}, Geo::G4, Geo::XK, wi.img[3])));
   DRL_TRY((launch_retile_b<128>(s_rest, PlainBT{P + pl.lstm_w, Geo::G4, 0}, Geo::FLAT + Geo::EMB, Geo::G4, wi.img[4])));
-  DRL_TRY((launch_retile_b<256>(s_rest, PlainBT{P + pl.conv3_w, 64, 0}, 576, 64, wi.img[5])));
-  DRL_TRY((launch_retile_b<256>(s_rest, PlainBT{P + pl.conv2_w, 64, 0}, 512, 64, wi.img[6])));
-  return DRL_OK;
+  return conv_dcol_images_tf32(s_rest, pl, P, wi.img[5], wi.img[6]);
 }
 
 int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const WeightImages& wi, const Inputs& in,
@@ -193,8 +191,7 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     n += 2;
   } else if (retile && mode >= 2) {
     prof_mark(s, "weight_retile");
-    DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv2_w, 64, 0}, 64, 512, wi.img[1])));
-    DRL_TRY((launch_retile_b<64>(s, PlainB{P + pl.conv3_w, 64, 0}, 64, 576, wi.img[2])));
+    DRL_TRY(conv_images_tf32(s, pl, P, wi.img[1], wi.img[2]));
     n += 2;
     if (st.par) DRL_CUDA_CHECK(cudaEventRecord(st.ev[7], side));
   }
@@ -217,38 +214,30 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
     }
     n += 4;
   }
-  // conv1: u8 frames -> a1 [M,20,20,32]   (attention_CNN, model/impala_actor_critic.py:6)
-  {
-    EpConv1 ep{act.a1, 32, P + pl.conv1_b};
-    if (m16) {
-      prof_mark(s, "conv1_fwd");
-      DRL_TRY(launch_conv1_fwd_tma(s, in.frames, M, map, P + pl.conv1_w, ep));
-      ++n;
-    } else {
-      Conv1A al{in.frames, map};
-      PlainB bl{P + pl.conv1_w, 32, 0};
-      GEMM("conv1_fwd", CfgN32, U32, al, bl, ep, M * 400, 32, 256, 1, 256, 0);
+  // attention_CNN (model/impala_actor_critic.py:6-10): u8 frames -> a1 [M,20,20,32] -> a2 [M,9,9,64] -> a3 [M,7,7,64]
+  // = flatten HWC [M,3136]; conv2 waits for its weight image, conv3 for its own in math mode 5
+  if (m16) {
+    prof_mark(s, "conv1_fwd");
+    DRL_TRY(launch_conv1_fwd_tma(s, in.frames, M, map, P + pl.conv1_w, EpConv1{act.a1, 32, P + pl.conv1_b}));
+    ++n;
+    if (retile && st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
+    {
+      Conv2A al{act.a1, map};
+      PretiledB<PlainB> blp{wi.img[1], 512 / 64};
+      EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
+      GEMM16("conv2_fwd", X64L2, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
     }
-  }
-  if (retile && mode >= 2 && st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
-  // conv2 -> a2 [M,9,9,64]   (:7)
-  {
-    Conv2A al{act.a1, map};
-    PlainB bl{P + pl.conv2_w, 64, 0};
-    PretiledB<PlainB> blp{wi.img[1], m16 ? 512 / 64 : 512 / 32};
-    EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
-    if (m16) GEMM16("conv2_fwd", X64L2, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
-    else GEMM_W("conv2_fwd", CfgBig, U64L, al, bl, blp, ep, M * 81, 64, 512, 1, 512, 0);
-  }
-  if (c3_event) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[4], 0));
-  // conv3 -> a3 [M,7,7,64] = flatten HWC [M,3136]   (:8-10)
-  {
-    Conv3A al{act.a2, map};
-    PlainB bl{P + pl.conv3_w, 64, 0};
-    PretiledB<PlainB> blp{wi.img[2], m16 ? 576 / 64 : 576 / 32};
-    EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
-    if (m16) GEMM16("conv3_fwd", X64L2, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
-    else GEMM_W("conv3_fwd", CfgBig, U64L, al, bl, blp, ep, M * 49, 64, 576, 1, 576, 0);
+    if (c3_event) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[4], 0));
+    {
+      Conv3A al{act.a2, map};
+      PretiledB<PlainB> blp{wi.img[2], 576 / 64};
+      EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
+      GEMM16("conv3_fwd", X64L2, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
+    }
+  } else {
+    const cudaEvent_t images_ready = retile && mode >= 2 && st.par ? st.ev[7] : nullptr;
+    DRL_TRY(conv_forward_tf32<Geo::IC>(s, pl, P, wi.img[1], wi.img[2], in.frames, B, T, act.a1, act.a2, act.a3, mode,
+                                        false, images_ready, &n));
   }
   if (late_images) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[1], 0));
   else DRL_TRY(join_from_side(st, 1));
@@ -323,6 +312,66 @@ int conv_forward16(cudaStream_t s, const ParamLayout& pl, const float* P, const 
     EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
     DRL_TRY((launch_gemm_umma16<X64L2>(s, al, blp, ep, n * 49, 64, 576, 1, 576, 0)));
   }
+  return DRL_OK;
+}
+
+// The conv trunk backward of math mode 5, the same steps, streams and events as conv_backward_tf32 (layer_defs.cuh) on
+// the 16-bit split core: weight gradients from two gathered operands, data gradients in gather form, the frame-resident
+// TMA kernel for conv1's weight gradient.
+static int conv_backward16(const Streams& st, const ParamLayout& pl, const WeightImages& wi, float* G,
+                           const uint8_t* frames, int B, int T, const Acts& act, const Bwd& bw, int* launches) {
+  const int mode = 5, M = B * T, Mb = B * (T - 2);
+  const RowMap map{B, T};
+  cudaStream_t s = st.par ? st.side : st.main;
+  int n = 0;
+  {
+    const SplitPlan sp = plan_conv3_wgrad(Mb, mode);
+    const size_t slab = 577 * 64;
+    Conv3WA al{act.a2, map};
+    PlainB bl{bw.da3, 64, 0};
+    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 576, 64};
+    GEMM16("conv3_wgrad", X64W8x2, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
+    KERNEL("conv3_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv3_w, slab), 1);
+  }
+  s = st.main;
+  {
+    // gather form: rows = input pixels, K = 9 taps x 64 output channels (taps outside the output are zero), ReLU mask of
+    // a2 in the epilogue; each tap's partial sum is rounded to fp32 and the taps are added in (ky, kx) order, as
+    // col2im_conv3 adds the dCol of math modes 2 and 3: the same da2, bit for bit
+    Conv3DA al{bw.da3};
+    PretiledB<Conv3DB> blp{wi.img[5], 576 / 64};
+    Conv3DE ep{bw.da2, act.a2};
+    GEMM16("conv3_dgrad", X64T, al, blp, ep, Mb * 81, 64, 576, 1, 576, 0);
+  }
+  DRL_TRY(fork_to_side(st, 5));
+  s = st.par ? st.side : st.main;
+  {
+    const SplitPlan sp = plan_conv2_wgrad(Mb, mode);
+    const size_t slab = 513 * 64;
+    Conv2WA al{act.a1, map};
+    PlainB bl{bw.da2, 64, 0};
+    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 512, 64};
+    GEMM16("conv2_wgrad", X64W8x2, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
+    KERNEL("conv2_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv2_w, slab), 1);
+  }
+  s = st.main;
+  {
+    // merged-phase gather form: row = the 2 x 2 block of input pixels (2i + py, 2j + px); all four parity classes read
+    // the same dY taps (i - a, j - b), so K = (a, b, co) = 256 and N = (py, px, ci) = 128, in two N tiles (py = 0, 1);
+    // ReLU mask of a1 in the epilogue; per-tap partial sums added in (a, b) order, as in col2im_conv2
+    Conv2DA al{bw.da2};
+    PretiledB<Conv2DBm> blp{wi.img[6], 256 / 64};
+    Conv2DEm ep{{bw.da1, act.a1}};
+    GEMM16("conv2_dgrad", X64T2, al, blp, ep, Mb * 100, 128, 256, 1, 256, 0);
+  }
+  // conv1 (input is data: weight gradient only): one partial slab per CTA, then the fixed-order reduce
+  const size_t slab = 257 * 32;
+  int splits = 0;
+  prof_mark(s, "conv1_wgrad");
+  DRL_TRY(launch_conv1_wgrad_tma(s, frames, M, Mb, map, bw.da1, bw.wg_part2, bw.wg_part_floats, &splits));
+  ++n;
+  KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, splits, G + pl.conv1_w, slab), 1);
+  *launches += n;
   return DRL_OK;
 }
 
@@ -456,102 +505,9 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     KERNEL("emb_bwd",
            emb_backward(s, bw.du, in.pa, act.e1, act.table, P + pl.emb2_w, bw.dpre2, bw.dpre1, G + pl.emb1_w,
                         G + pl.emb1_b, G + pl.emb2_w, G + pl.emb2_b, bw.wg_part, Mb, B, T, A), 4);
-  // ---- conv3 -------------------------------------------------------------------------------
-  {
-    const SplitPlan sp = plan_conv3_wgrad(Mb, mode);
-    const size_t slab = 577 * 64;
-    Conv3WA al{act.a2, map};
-    PlainB bl{bw.da3, 64, 0};
-    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 576, 64};
-    if (m16) GEMM16("conv3_wgrad", X64W8x2, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
-    else GEMM("conv3_wgrad", CfgBig, U64, al, bl, ep, 576, 64, Mb * 49, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv3_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv3_w, slab), 1);
-  }
-  s = st.main;
-  if (m16) {
-    // gather form: rows = input pixels, K = 9 taps x 64 output channels (taps outside the output are zero), ReLU mask of
-    // a2 in the epilogue; each tap's partial sum is rounded to fp32 and the taps are added in (ky, kx) order, as
-    // col2im_conv3 adds the dCol of math modes 2 and 3: the same da2, bit for bit
-    Conv3DA al{bw.da3};
-    PretiledB<Conv3DB> blp{wi.img[5], 576 / 64};
-    Conv3DE ep{bw.da2, act.a2};
-    GEMM16("conv3_dgrad", X64T, al, blp, ep, Mb * 81, 64, 576, 1, 576, 0);
-  } else if (mode >= 2) {
-    // "dCol" form: one plain GEMM with K = 64 output channels (instead of gathering every dY value 9 times
-    // through the producers), then a gather of <= 9 taps per input pixel with the ReLU mask.
-    PlainA al{bw.da3, 64, 0};
-    PlainBT bl{P + pl.conv3_w, 64, 0};               // B(k = co, n = (ky,kx,ci)) = W[n*64 + co]
-    EpRaw<false> ep{bw.dcol, 576, 0, 1.0f, 0, 576};
-    // K = 64 (two K tiles) and 128 x 256 outputs per tile: epilogue-dominated, so the persistent kernel whose
-    // dedicated epilogue warps wins here while the producers gather the next tile.
-    prof_mark(s, "conv3_dgrad");
-    PretiledB<PlainBT> blp{wi.img[5], 2};
-    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 49, 576, 64, 1, 64, 0)));
-    prof_mark(s, "conv3_col2im");
-    DRL_TRY(col2im_conv3(s, bw.dcol, act.a2, bw.da2, Mb));
-    n += 2;
-  } else {
-    Conv3DA al{bw.da3};
-    Conv3DB bl{P + pl.conv3_w};
-    Conv3DE ep{bw.da2, act.a2};
-    GEMM_FFMA("conv3_dgrad", CfgBig, al, bl, ep, Mb * 81, 64, 576, 1, 576, 0);
-  }
-  // ---- conv2 -------------------------------------------------------------------------------
-  DRL_TRY(fork_to_side(st, 5));
-  s = side;
-  {
-    const SplitPlan sp = plan_conv2_wgrad(Mb, mode);
-    const size_t slab = 513 * 64;
-    Conv2WA al{act.a1, map};
-    PlainB bl{bw.da2, 64, 0};
-    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 512, 64};
-    if (m16) GEMM16("conv2_wgrad", X64W8x2, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
-    else GEMM("conv2_wgrad", CfgBig, U64, al, bl, ep, 512, 64, Mb * 81, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv2_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv2_w, slab), 1);
-  }
-  s = st.main;
-  if (m16) {
-    // merged-phase gather form: row = the 2 x 2 block of input pixels (2i + py, 2j + px); all four parity classes read
-    // the same dY taps (i - a, j - b), so K = (a, b, co) = 256 and N = (py, px, ci) = 128, in two N tiles (py = 0, 1);
-    // ReLU mask of a1 in the epilogue; per-tap partial sums added in (a, b) order, as in col2im_conv2
-    Conv2DA al{bw.da2};
-    PretiledB<Conv2DBm> blp{wi.img[6], 256 / 64};
-    Conv2DEm ep{{bw.da1, act.a1}};
-    GEMM16("conv2_dgrad", X64T2, al, blp, ep, Mb * 100, 128, 256, 1, 256, 0);
-  } else if (mode >= 2) {
-    PlainA al{bw.da2, 64, 0};
-    PlainBT bl{P + pl.conv2_w, 64, 0};               // B(k = co, n = (ky,kx,ci)) = W[n*64 + co]
-    EpRaw<false> ep{bw.dcol, 512, 0, 1.0f, 0, 512};
-    prof_mark(s, "conv2_dgrad");                      // persistent kernel: 0.079 vs 0.091 ms
-    PretiledB<PlainBT> blp{wi.img[6], 2};
-    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, Mb * 81, 512, 64, 1, 64, 0)));
-    prof_mark(s, "conv2_col2im");
-    DRL_TRY(col2im_conv2(s, bw.dcol, act.a1, bw.da1, Mb));
-    n += 2;
-  } else {
-    Conv2DA al{bw.da2};
-    Conv2DB bl{P + pl.conv2_w};
-    Conv2DE ep{bw.da1, act.a1};
-    GEMM_FFMA("conv2_dgrad", CfgN32, al, bl, ep, Mb * 100, 32, 256, 4, 256, 0);
-  }
-  // ---- conv1 (input is data: weight gradient only) -----------------------------------------
-  if (m16) {
-    // frame-resident TMA kernel (conv1_tma.cuh): one partial slab per CTA, then the fixed-order reduce
-    const size_t slab = 257 * 32;
-    int splits = 0;
-    prof_mark(s, "conv1_wgrad");
-    DRL_TRY(launch_conv1_wgrad_tma(s, in.frames, M, Mb, map, bw.da1, bw.wg_part2, bw.wg_part_floats, &splits));
-    ++n;
-    KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, splits, G + pl.conv1_w, slab), 1);
-  } else {
-    const SplitPlan sp = plan_conv1_wgrad(Mb, mode);
-    const size_t slab = 257 * 32;
-    Conv1WA al{in.frames, map};
-    PlainB bl{bw.da1, 32, 0};
-    EpRaw<true> ep{bw.wg_part2, 32, slab, 1.0f / 255.0f, 256, 32};   // own partial buffer: runs beside the side stream
-    GEMM("conv1_wgrad", CfgWg1, U32, al, bl, ep, 256, 32, Mb * 400, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, sp.splits, G + pl.conv1_w, slab), 1);
-  }
+  // ---- conv trunk --------------------------------------------------------------------------
+  if (m16) DRL_TRY(conv_backward16(st, pl, wi, G, in.frames, B, T, act, bw, &n));
+  else DRL_TRY(conv_backward_tf32<Geo::IC>(st, pl, P, wi, G, in.frames, map, Mb, act, bw, mode, &n));
   if (lane2) DRL_TRY(join_side2_into(st, 2, st.main));
   DRL_TRY(join_from_side(st, 6));
   g_bwd_launches = n;

@@ -432,11 +432,7 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
       DRL_CUDA_CHECK(cudaMemcpy(h->ms, ones.data(), NP * sizeof(float), cudaMemcpyHostToDevice));
     }
     Acts& a = h->act;
-    DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
-    DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
-    DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
-    DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
+    DRL_TRY(alloc_trunk_acts(h, a, M, A));
     DRL_TRY(dev_alloc(h, &a.zpart, (size_t)kLstmSplits * M * Geo::G4));
     DRL_TRY(dev_alloc(h, &a.gates, M * Geo::G4));
     DRL_TRY(dev_alloc(h, &a.c1, M * Geo::L));
@@ -458,17 +454,9 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     DRL_TRY(dev_alloc(h, &b.dhid1, 2 * Mb * Geo::HID));
     DRL_TRY(dev_alloc(h, &b.dh_part, 2 * Mb * Geo::L));
     DRL_TRY(dev_alloc(h, &b.dz, Mb * Geo::G4));
-    DRL_TRY(dev_alloc(h, &b.da3, Mb * Geo::FLAT));
-    DRL_TRY(dev_alloc(h, &b.du, Mb * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.dpre2, A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.dpre1, A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.da2, Mb * 81 * 64));
-    DRL_TRY(dev_alloc(h, &b.da1, Mb * 400 * 32));
-    b.wg_part_floats = wgrad_partial_floats(h->B, h->T);
-    DRL_TRY(dev_alloc(h, &b.wg_part, b.wg_part_floats));
-    DRL_TRY(dev_alloc(h, &b.wg_part2, b.wg_part_floats));
+    DRL_TRY(alloc_trunk_bwd(h, b, Mb, A, Geo::IC, h->mode != 5));
+    b.wg_part_floats = trunk_partial_floats((int)Mb, Geo::IC);
     DRL_TRY(dev_alloc(h, &b.emb_scratch, (size_t)16 * 32 * 256));
-    if (h->mode != 5) DRL_TRY(dev_alloc(h, &b.dcol, Mb * 81 * 512));
     {
       size_t wb[WeightImages::kCount];
       weight_image_sizes(wb);

@@ -21,9 +21,6 @@
 
 namespace drl {
 
-// conv1 weight gradient over single-channel frames
-using Conv1WA1 = ConvWgradA<uint8_t, 84, 84, 1, 20, 20, 8, 4, true>;
-
 // [x | h_in]^T for the LSTM kernel gradient: feature index i < 3392 -> [a3 | emb] (as LstmAT), else h_in (device, time-major)
 struct R2XhAT {
   static constexpr bool kContigK = false;
@@ -60,11 +57,6 @@ struct R2XA {
 static SplitPlan plan_r2_x(int M, int mode) {
   return mode >= 2 ? plan_split(kR2Cat, cdiv(M, 128), 32, 1) : plan_split(kR2Cat, cdiv(M, CfgMid::BM) * (kR2G / CfgMid::BN), 16, 1);
 }
-// conv1 weight gradient with single-channel frames is a [64 x 32] output with K = M*400: half of a 128-row MMA tile
-// would be padding and the producers, not the tensor pipe, set the pace on the 128-row tensor-core
-// core).  A 64 x 32 FFMA tile with the reduction split over ~4 CTAs per SM fits the shape in both math modes.
-using CfgWgC1 = TileCfg<64, 32, 16, 4, 4>;
-static SplitPlan plan_r2_conv1_wgrad(int M, int) { return plan_split(M * 400, 1, 16, 4); }
 
 // ------------------------------------------------------------------------------------------
 // LSTM recurrence, forward (model/r2d2_lstm.py:12-21 inside the unroll :67-84; TF 1.14 LSTMCell):
@@ -388,8 +380,7 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
          emb_forward(s, P + pl.emb1_w, P + pl.emb1_b, P + pl.emb2_w, P + pl.emb2_b, act.e1, act.table, pl.A), 1);
   if (retile_bwd && mode >= 2) {
     prof_mark(s, "weight_retile_bwd");
-    DRL_TRY((launch_retile_b<256>(s, PlainBT{P + pl.conv3_w, 64, 0}, 576, 64, wi.img[5])));
-    DRL_TRY((launch_retile_b<256>(s, PlainBT{P + pl.conv2_w, 64, 0}, 512, 64, wi.img[6])));
+    DRL_TRY(conv_dcol_images_tf32(s, pl, P, wi.img[5], wi.img[6]));
     n += 2;
   }
   s = st.main;
@@ -491,75 +482,8 @@ static int r2_backward(const Streams& st, const R2Layout& pl, const float* P, co
   KERNEL("emb_bwd",
          emb_backward(s, bw.du, in.pa, act.e1, act.table, P + pl.emb2_w, bw.dpre2, bw.dpre1, G + pl.emb1_w,
                       G + pl.emb1_b, G + pl.emb2_w, G + pl.emb2_b, bw.wg_part, M, B, S, A), 4);
-  {
-    const SplitPlan sp = plan_conv3_wgrad(M, mode);
-    const size_t slab = 577 * 64;
-    Conv3WA al{act.a2, map};
-    PlainB bl{bw.da3, 64, 0};
-    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 576, 64};
-    GEMM("conv3_wgrad", CfgBig, U64, al, bl, ep, 576, 64, M * 49, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv3_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv3_w, slab), 1);
-  }
-  s = st.main;
-  if (mode >= 2) {
-    PlainA al{bw.da3, 64, 0};
-    EpRaw<false> ep{bw.dcol, 576, 0, 1.0f, 0, 576};
-    prof_mark(s, "conv3_dgrad");
-    PretiledB<PlainBT> blp{wi.img[5], 2};
-    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, M * 49, 576, 64, 1, 64, 0)));
-    prof_mark(s, "conv3_col2im");
-    DRL_TRY(col2im_conv3(s, bw.dcol, act.a2, bw.da2, M));
-    n += 2;
-  } else {
-    Conv3DA al{bw.da3};
-    Conv3DB bl{P + pl.conv3_w};
-    Conv3DE ep{bw.da2, act.a2};
-    GEMM_FFMA("conv3_dgrad", CfgBig, al, bl, ep, M * 81, 64, 576, 1, 576, 0);
-  }
-  DRL_TRY(fork_to_side(st, 5));
-  s = side;
-  {
-    const SplitPlan sp = plan_conv2_wgrad(M, mode);
-    const size_t slab = 513 * 64;
-    Conv2WA al{act.a1, map};
-    PlainB bl{bw.da2, 64, 0};
-    EpRaw<true> ep{bw.wg_part, 64, slab, 1.0f, 512, 64};
-    GEMM("conv2_wgrad", CfgBig, U64, al, bl, ep, 512, 64, M * 81, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv2_wgrad_reduce", splitk_reduce(s, bw.wg_part, slab, sp.splits, G + pl.conv2_w, slab), 1);
-  }
-  s = st.main;
-  if (mode >= 2) {
-    PlainA al{bw.da2, 64, 0};
-    EpRaw<false> ep{bw.dcol, 512, 0, 1.0f, 0, 512};
-    prof_mark(s, "conv2_dgrad");
-    PretiledB<PlainBT> blp{wi.img[6], 2};
-    DRL_TRY((launch_gemm_umma_persist<PersistOf<U256>::type>(s, al, blp, ep, M * 81, 512, 64, 1, 64, 0)));
-    prof_mark(s, "conv2_col2im");
-    DRL_TRY(col2im_conv2(s, bw.dcol, act.a1, bw.da1, M));
-    n += 2;
-  } else {
-    Conv2DA al{bw.da2};
-    Conv2DB bl{P + pl.conv2_w};
-    Conv2DE ep{bw.da1, act.a1};
-    GEMM_FFMA("conv2_dgrad", CfgN32, al, bl, ep, M * 100, 32, 256, 4, 256, 0);
-  }
-  if (pl.C == 1) {
-    const SplitPlan sp = plan_r2_conv1_wgrad(M, mode);
-    const size_t slab = 65 * 32;
-    Conv1WA1 al{in.frames, map};
-    PlainB bl{bw.da1, 32, 0};
-    EpRaw<true> ep{bw.wg_part2, 32, slab, 1.0f / 255.0f, 64, 32};
-    GEMM_FFMA("conv1_wgrad", CfgWgC1, al, bl, ep, 64, 32, M * 400, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, sp.splits, G + pl.conv1_w, slab), 1);
-  } else {
-    const SplitPlan sp = plan_conv1_wgrad(M, mode);
-    const size_t slab = 257 * 32;
-    Conv1WA al{in.frames, map};
-    PlainB bl{bw.da1, 32, 0};
-    EpRaw<true> ep{bw.wg_part2, 32, slab, 1.0f / 255.0f, 256, 32};
-    GEMM("conv1_wgrad", CfgWg1, U32, al, bl, ep, 256, 32, M * 400, sp.splits, sp.kchunk, sp.kchunk);
-    KERNEL("conv1_wgrad_reduce", splitk_reduce(s, bw.wg_part2, slab, sp.splits, G + pl.conv1_w, slab), 1);
-  }
+  DRL_TRY(pl.C == 1 ? conv_backward_tf32<1>(st, pl, P, wi, G, in.frames, map, M, act, bw, mode, &n)
+                    : conv_backward_tf32<4>(st, pl, P, wi, G, in.frames, map, M, act, bw, mode, &n));
   DRL_TRY(join_from_side(st, 6));
   if (launches) *launches += n;
   return DRL_OK;
@@ -605,11 +529,7 @@ constexpr const char* kName = "r2d2";
 
 int alloc_acts(drl_r2d2* h, R2Acts& a) {
   const size_t M = (size_t)h->B * h->S, A = h->A;
-  DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
-  DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
-  DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
-  DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
-  DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
+  DRL_TRY(alloc_trunk_acts(h, a, M, A));
   size_t zmax = 0;
   for (int mode = 1; mode <= 2; ++mode)
     for (int m = 1; m <= (int)M; ++m) zmax = std::max(zmax, (size_t)plan_r2_x(m, mode).splits * m * kR2G);
@@ -682,7 +602,6 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
   h->frame = (size_t)Geo::IH * Geo::IW * h->C;
   h->pl.init(h->A, h->C);
   h->layout = &h->pl;
-  h->conv2_w = h->pl.conv2_w; h->conv3_w = h->pl.conv3_w;
   h->fwd_bwd = fwd_bwd;
   AdamState& o = h->opt;
   o.start_lr = cfg->learning_rate; o.end_lr = cfg->learning_rate; o.learning_frame = 1.0;   // constant (agent/r2d2.py:91)
@@ -712,17 +631,7 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
     DRL_TRY(dev_alloc(h, &b.dq1, M * kR2H));
     DRL_TRY(dev_alloc(h, &b.dhout, M * kR2L));
     DRL_TRY(dev_alloc(h, &b.dz, M * kR2G));
-    DRL_TRY(dev_alloc(h, &b.da3, M * Geo::FLAT));
-    DRL_TRY(dev_alloc(h, &b.du, M * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.dpre2, A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.dpre1, A * Geo::EMB));
-    DRL_TRY(dev_alloc(h, &b.da2, M * 81 * 64));
-    DRL_TRY(dev_alloc(h, &b.da1, M * 400 * 32));
-    size_t wg = wgrad_partial_floats((int)M, 3);                       // rows with gradient = M * (3 - 2)
-    for (int mode = 1; mode <= 2; ++mode) wg = std::max(wg, (size_t)plan_r2_conv1_wgrad((int)M, mode).splits * 65 * 32);
-    DRL_TRY(dev_alloc(h, &b.wg_part, wg));
-    DRL_TRY(dev_alloc(h, &b.wg_part2, wg));
-    DRL_TRY(dev_alloc(h, &b.dcol, M * 81 * 512));
+    DRL_TRY(alloc_trunk_bwd(h, b, M, A, h->C, true));
     const size_t Nt = h->Nt;
     DRL_TRY(dev_alloc(h, &h->sav, B * Nt));
     DRL_TRY(dev_alloc(h, &h->target_value, B * Nt));

@@ -34,8 +34,7 @@ struct R2Layout : TrunkLayout {
 int r2d2_params_snapshot(drl_r2d2* h, int device, int num_action, int channels, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);
 
-struct R2Acts {            // activations of one scope, time-major rows m = t*B + b
-  float *a1, *a2, *a3, *e1, *table;
+struct R2Acts : TrunkActs {   // activations of one scope, time-major rows m = t*B + b
   float* zpart;            // [splits][M, 4L]: [a3 | emb] W_x partial sums
   float* zx;               // [M, 4L]: their sum (the recurrence reads one value per gate and step)
   float* gates;            // [M, 4L] sigmoid(i), tanh(j), sigmoid(f + 1), sigmoid(o)
@@ -44,10 +43,9 @@ struct R2Acts {            // activations of one scope, time-major rows m = t*B 
   float* q1;               // [M, 128]
   float* q;                // [M, A]
 };
-struct R2Bwd {
+struct R2Bwd : TrunkBwd {     // backward workspace, all M rows
   float *dq, *dmean;       // [M, 32]
   float *dq1, *dhout, *dz; // [M,128], [M,L], [M,4L]
-  float *da3, *du, *dpre2, *dpre1, *da2, *da1, *wg_part, *wg_part2, *dcol;
 };
 struct R2In {              // one staged minibatch, caller's batch-major layout
   const uint8_t* frames;   // [B, S, 84, 84, C]
