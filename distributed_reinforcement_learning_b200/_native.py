@@ -191,6 +191,10 @@ def _load():
         "drl_policy_recorder_commit": (C.c_int, [vp, vp, vp, i32]),
         "drl_policy_recorder_reset": (C.c_int, [vp]),
         "drl_learner_stage_from_queue": (C.c_int, [vp, i32, vp, i32]),
+        "drl_policy_server_exchange_bytes": (C.c_int, [i32, C.POINTER(i64)]),
+        "drl_policy_server_create": (C.c_int, [vp, vp, i32, vp, i64, C.POINTER(vp)]),
+        "drl_policy_server_destroy": (C.c_int, [vp]),
+        "drl_policy_server_serve": (C.c_int, [vp, i32, vp, i32]),
         "drl_r2d2_queue_create": (C.c_int, [i32] * 6 + [C.POINTER(vp)]),
         "drl_r2d2_queue_destroy": (C.c_int, [vp]),
         "drl_r2d2_queue_size": (C.c_int, [vp]),

@@ -9,10 +9,11 @@ VectorActor: each environment is its own actor task ``i`` (what ``FLAGS.task`` s
     when it has a CUDA learner);
   - ``trajectory`` batched ``policy.act`` calls: one forward over all N environments, the actions drawn on the GPU
     from the same global ``np.random`` stream the reference's ``np.random.choice`` reads;
-  - every environment steps with ``action % available_action[i]``; the trajectory stores the action unmodified
-    (SURVEY.md App. D);
-  - a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True; the score keeps the raw reward;
-  - at an episode's end the environment is reset, and previous action, h and c go back to 0;
+  - every environment steps under ``utils.impala_env_step`` (the rule the worker processes of
+    ``actor_server.EnvWorkerPool`` follow too): ``action % available_action[i]``, the trajectory stores the action
+    unmodified (SURVEY.md App. D); a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True,
+    the score keeps the raw reward; at an episode's end the environment is reset, and previous action, h and c go
+    back to 0;
   - every environment's ``utils.UnrolledTrajectory`` goes to ``queue.append_to_queue(task=i, ...)``; with a
     ``DeviceFIFOQueue`` the acts go through a recorder of the policy instead (``NativePolicy.recorder``), which keeps
     the trajectories on the GPU, and the unroll ends with one ``commit`` of the rewards and done flags of all N
@@ -22,8 +23,7 @@ import numpy as np
 
 from . import utils
 from .distributed_queue import buffer_queue
-
-START_LIVES = 5   # the reference actor's life counter starts (and restarts after every episode) at 5
+from .utils import START_LIVES
 
 
 class VectorActor:
@@ -93,30 +93,17 @@ class VectorActor:
             next_pa, next_h, next_c = action.astype(np.int32), out["h"].copy(), out["c"].copy()
             for i, env in enumerate(self.envs):
                 a = int(action[i])
-                self.episode_step[i] += 1
-                self.total_max_prob[i] += float(max_prob[i])
-                next_state, reward, done, info = env.step(a % self.available_action[i])
-                self.score[i] += reward
-                if self.lives[i] != info["ale.lives"]:
-                    r, d = -1.0, True
-                else:
-                    r, d = reward, False
+                next_state, r, d, state, episode = utils.impala_env_step(env, a, self.available_action[i], self, i,
+                                                                         max_prob[i])
                 if rec is None:
                     trajs[i].append(state=self.states[i], next_state=next_state, reward=r, done=d, action=a,
                                     behavior_policy=policy[i], previous_action=int(self.previous_action[i]),
                                     initial_h=self.h[i], initial_c=self.c[i])
                 else:   # the rest of the step is on the device already
                     rewards[i, step], dones[i, step] = r, d
-                self.states[i] = next_state
-                self.lives[i] = info["ale.lives"]
-                if done:
-                    finished.append(dict(task=i, episode=self.episode[i], score=self.score[i],
-                                         episode_step=self.episode_step[i],
-                                         prob=self.total_max_prob[i] / self.episode_step[i]))
-                    self.episode[i] += 1
-                    self.score[i], self.episode_step[i], self.total_max_prob[i] = 0.0, 0, 0.0
-                    self.states[i] = env.reset()
-                    self.lives[i] = START_LIVES
+                self.states[i] = state
+                if episode is not None:
+                    finished.append(episode)
                     next_pa[i] = 0
                     next_h[i] = 0.0
                     next_c[i] = 0.0

@@ -1,0 +1,369 @@
+"""IMPALA environments in worker processes, served by one batched policy engine beside the learner.
+
+The reference runs every actor in its own process (``train_impala.py``); ``VectorActor`` steps all its environments
+one after another in one thread.  Here the environments step in parallel in CPU-only worker processes
+(``EnvWorkerPool``), and one ``PolicyServer`` in the learner's process acts for all of them through one
+``NativePolicy`` (``drl_policy_server_*``, include/drl_b200.h), with every environment's h, c, previous action and
+unfinished trajectory kept on the GPU.  Completed trajectories go into a ``DeviceFIFOQueue`` that
+``impala.Agent.train_from_queue`` trains from.
+
+Workers and server share one exchange block (``multiprocessing.shared_memory``): a report record per environment
+(the frame to act on, the uniform draw of the action, the reward and done of the previous step, a reset flag) and a
+reply record per environment (action, max probability), laid out as ``DRL_SERVER_*`` in include/drl_b200.h.  The
+server registers the block with CUDA; its kernels read the reports and write the replies directly.  A worker writes
+its environments' reports, then signals on its pipe; the server answers on the same pipe once the replies are written.
+
+This module imports neither torch nor the native library at module level: the spawned workers import it.
+"""
+import collections
+import ctypes as C
+import multiprocessing as mp
+import multiprocessing.connection
+import pickle
+import sys
+import threading
+import traceback
+from multiprocessing import shared_memory
+
+import numpy as np
+
+from . import utils
+
+# the exchange block's records (include/drl_b200.h: DRL_SERVER_*)
+FRAME_SHAPE = (84, 84, 4)
+REPORT_FRAME, REPORT_UNIFORM, REPORT_REWARD, REPORT_DONE, REPORT_RESET, REPORT_BYTES = 0, 28224, 28240, 28256, 28272, 28288
+REPLY_ACTION, REPLY_MAX_PROB, REPLY_BYTES = 0, 16, 32
+PAGE = 4096
+MAX_ENVS = 256
+
+
+def exchange_bytes(num_envs):
+    """Size of the exchange block of num_envs environments: the reports, then the replies, rounded up to a page."""
+    n = num_envs * (REPORT_BYTES + REPLY_BYTES)
+    return -(-n // PAGE) * PAGE
+
+
+def exchange_views(buf, num_envs):
+    """numpy views of the records in the exchange block `buf` (a writable buffer of exchange_bytes(num_envs))."""
+    E = num_envs
+
+    def field(offset, dtype, shape=(), strides=()):
+        return np.ndarray((E,) + shape, dtype, buffer=buf, offset=offset, strides=(stride,) + strides)
+
+    stride = REPORT_BYTES
+    v = dict(frame=field(REPORT_FRAME, np.uint8, FRAME_SHAPE, (FRAME_SHAPE[1] * FRAME_SHAPE[2], FRAME_SHAPE[2], 1)),
+             uniform=field(REPORT_UNIFORM, np.float64), reward=field(REPORT_REWARD, np.float32),
+             done=field(REPORT_DONE, np.uint8), reset=field(REPORT_RESET, np.uint8))
+    stride = REPLY_BYTES
+    base = E * REPORT_BYTES
+    v.update(action=field(base + REPLY_ACTION, np.int32), max_prob=field(base + REPLY_MAX_PROB, np.float32))
+    return v
+
+
+class _Stats:
+    """The per-environment episode bookkeeping utils.impala_env_step updates."""
+
+    def __init__(self, k):
+        self.lives = [utils.START_LIVES] * k
+        self.episode = [0] * k
+        self.score = [0.0] * k
+        self.episode_step = [0] * k
+        self.total_max_prob = [0.0] * k
+
+
+def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, seeds):
+    """A worker process: k environments, each task env_ids[j] with its own RandomState(seeds[j]) for the uniform
+    draws of its actions."""
+    shm = shared_memory.SharedMemory(name=shm_name)
+    v = exchange_views(shm.buf, num_envs)
+    task = env_ids[0]
+    try:
+        envs = []
+        for j, fn in enumerate(env_fns):
+            task = env_ids[j]
+            envs.append(fn())
+        rngs = [np.random.RandomState(s) for s in seeds]
+        stats = _Stats(len(envs))
+        for j, e in enumerate(env_ids):
+            task = e
+            v["frame"][e] = envs[j].reset()
+            v["uniform"][e] = rngs[j].random_sample()
+            v["reward"][e], v["done"][e], v["reset"][e] = 0.0, 0, 1
+        info = dict(torch="torch" in sys.modules,
+                    native="distributed_reinforcement_learning_b200._native" in sys.modules)
+        conn.send(("ready", [], info))
+        while conn.recv() == "go":
+            finished = []
+            for j, e in enumerate(env_ids):
+                task = e
+                _, r, d, state, episode = utils.impala_env_step(envs[j], int(v["action"][e]), available_action[j],
+                                                                stats, j, v["max_prob"][e], task=e)
+                v["frame"][e] = state
+                v["reward"][e], v["done"][e], v["reset"][e] = r, d, episode is not None
+                v["uniform"][e] = rngs[j].random_sample()
+                if episode is not None:
+                    finished.append(episode)
+            conn.send(("ready", finished, None))
+    except BaseException:
+        try:
+            conn.send(("error", task, traceback.format_exc()))
+        except Exception:
+            pass
+    finally:
+        del v
+        shm.close()
+        conn.close()
+
+
+class EnvWorkerPool:
+    """``len(env_fns)`` environments (1..256) in spawned worker processes of ``envs_per_worker`` environments each.
+
+    Environment i is task i: ``env_fns[i]()`` builds it in its worker, it steps under ``utils.impala_env_step`` with
+    ``available_action[i]``, and the uniform draws of its actions come from ``np.random.RandomState(seeds[i])``, so
+    they do not depend on batching or on how environments are grouped into workers.  The env factories must be
+    picklable (ValueError otherwise).  The workers import neither torch nor CUDA.
+
+    ``close()`` (also on leaving a ``with`` block) first closes every ``PolicyServer`` still bound to the pool (each
+    has the exchange block registered with CUDA), then stops every worker, terminating the ones that do not exit in
+    time, and frees the exchange block."""
+
+    def __init__(self, env_fns, available_action, envs_per_worker, seeds, start_timeout=300.0, join_timeout=10.0):
+        env_fns, seeds = list(env_fns), [int(s) for s in seeds]
+        available_action = [int(a) for a in available_action]
+        n, k = len(env_fns), int(envs_per_worker)
+        if not 1 <= n <= MAX_ENVS:
+            raise ValueError("%d environments, a pool serves 1..%d" % (n, MAX_ENVS))
+        if len(available_action) != n or len(seeds) != n:
+            raise ValueError("available_action and seeds need one entry per environment (%d)" % n)
+        if k < 1:
+            raise ValueError("envs_per_worker must be >= 1 (got %d)" % k)
+        for i, fn in enumerate(env_fns):
+            try:
+                pickle.dumps(fn)
+            except Exception as e:
+                raise ValueError("env_fns[%d] cannot be pickled for a spawned worker: %s" % (i, e)) from None
+        self.num_envs, self.envs_per_worker = n, k
+        self.join_timeout = join_timeout
+        self.exchange_bytes = exchange_bytes(n)
+        self._workers = []
+        self._pending = set()
+        self._servers = []
+        self._shm = shared_memory.SharedMemory(create=True, size=self.exchange_bytes)
+        self.views = exchange_views(self._shm.buf, n)
+        self._anchor = C.c_char.from_buffer(self._shm.buf)
+        self.address = C.addressof(self._anchor)
+        self.worker_info = []
+        try:
+            ctx = mp.get_context("spawn")
+            for w in range(0, n, k):
+                ids = list(range(w, min(n, w + k)))
+                parent, child = ctx.Pipe()
+                p = ctx.Process(target=_worker_main, name="env-worker-%d" % (w // k),
+                                args=(child, self._shm.name, n, ids, env_fns[w:w + k], available_action[w:w + k],
+                                      seeds[w:w + k]), daemon=True)
+                p.start()
+                child.close()
+                self._workers.append(dict(process=p, conn=parent, env_ids=ids))
+            while len(self.worker_info) < len(self._workers):
+                if not self._collect(start_timeout):
+                    raise RuntimeError("environment workers did not start within %.0f s" % start_timeout)
+        except BaseException:
+            self.close()
+            raise
+
+    @property
+    def num_workers(self):
+        return len(self._workers)
+
+    def env_ids(self, w):
+        return self._workers[w]["env_ids"]
+
+    def _collect(self, timeout, finished=None):
+        """Receives the reports of the workers that have one ready, waiting up to `timeout` s (None: forever) for the
+        first; -> whether any arrived."""
+        waiting = {id(x["conn"]): w for w, x in enumerate(self._workers) if w not in self._pending}
+        conns = [self._workers[w]["conn"] for w in waiting.values()]
+        ready = mp.connection.wait(conns, timeout) if conns else []
+        for c in ready:
+            w = waiting[id(c)]
+            ids = self._workers[w]["env_ids"]
+            try:
+                kind, a, b = c.recv()
+            except (EOFError, OSError):
+                raise RuntimeError("environment worker %d (tasks %s) exited without a report (exit code %s)"
+                                   % (w, ids, self._workers[w]["process"].exitcode)) from None
+            if kind == "error":
+                raise RuntimeError("environment task %d raised in worker %d:\n%s" % (a, w, b))
+            if b is not None:
+                self.worker_info.append(b)
+            if finished is not None:
+                finished.extend(a)
+            self._pending.add(w)
+        return bool(ready)
+
+    def wait_ready(self, timeout=None):
+        """Waits up to `timeout` s (None: forever) until at least one worker has reported, and takes every report
+        that is ready.  -> (the workers whose reports await a reply, in worker order; the episodes they finished)."""
+        finished = []
+        if not self._pending:
+            self._collect(timeout, finished)
+        self._collect(0, finished)
+        return sorted(self._pending), finished
+
+    def reply(self, workers):
+        """Tells these workers that their reply records are written."""
+        for w in workers:
+            self._pending.discard(w)
+            self._workers[w]["conn"].send("go")
+
+    def _bind(self, server):
+        """Called by a PolicyServer that registered the exchange block: close() closes it before freeing the block."""
+        if getattr(self, "_shm", None) is None:
+            raise ValueError("the pool is closed")
+        self._servers.append(server)
+
+    def _unbind(self, server):
+        self._servers = [s for s in self._servers if s is not server]
+
+    def close(self):
+        for server in list(getattr(self, "_servers", ())):
+            server.close()
+        for x in self._workers:
+            try:
+                x["conn"].send("stop")
+            except Exception:
+                pass
+        for x in self._workers:
+            p = x["process"]
+            p.join(self.join_timeout)
+            if p.is_alive():
+                p.terminate()
+                p.join(self.join_timeout)
+            if p.is_alive():
+                p.kill()
+                p.join()
+            x["conn"].close()
+        self._workers, self._pending = [], set()
+        if getattr(self, "_shm", None) is not None:
+            self.views = None
+            self._anchor = None
+            self._shm.close()
+            self._shm.unlink()
+            self._shm = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class PolicyServer:
+    """Serves the environments of an ``EnvWorkerPool`` from one ``NativePolicy`` into one ``DeviceFIFOQueue``.
+
+    ``serve_once`` waits for at least one worker's reports, takes every report that is ready and serves them in
+    chunks of ``policy.max_batch`` environments (no batching knob: batches grow with load), then answers the workers.
+    Before a serve it syncs the policy from ``learner`` (an ``impala.Agent``) whenever the learner has trained since
+    the last sync, so parameters can change inside an unroll; each trajectory records the policy that acted, which is
+    what V-trace corrects for.  While the queue is full a serve blocks: that is the workers' backpressure.
+    ``batch_sizes`` counts the served batches by size.  Single-replica, like ``train_from_queue``.  Closing the pool
+    closes its server first, so the exchange block is never freed while CUDA has it registered."""
+
+    def __init__(self, policy, queue, pool, learner=None):
+        from . import _native as N
+        from .distributed_queue.buffer_queue import DeviceFIFOQueue
+        from .learner import NativeLearner
+        if not isinstance(queue, DeviceFIFOQueue):
+            raise TypeError("PolicyServer: queue must be a DeviceFIFOQueue, got %s" % type(queue).__name__)
+        if NativeLearner._distributed():
+            raise RuntimeError("PolicyServer is single-replica: the queue lives on one device")
+        self._N = N
+        self.policy, self.queue, self.pool, self.learner = policy, queue, pool, learner
+        self.batch_sizes = collections.Counter()
+        self.syncs = 0
+        self._synced_step = None
+        self._todo, self._workers, self._finished = [], [], []
+        self._lock = threading.Lock()   # a serve and close() never overlap
+        self._s = C.c_void_p()
+        bind = getattr(pool, "_bind", None)
+        if bind is not None:
+            bind(self)
+        try:
+            N.check(N.lib.drl_policy_server_create(policy._h, queue._q, pool.num_envs, C.c_void_p(pool.address),
+                                                   pool.exchange_bytes, C.byref(self._s)))
+        except BaseException:
+            self.close()
+            raise
+
+    def close(self):
+        """Destroys the server (unregistering the exchange block); waits for a serve in progress."""
+        with self._lock:
+            if self._s.value:
+                self._N.lib.drl_policy_server_destroy(self._s)
+                self._s = C.c_void_p()
+        unbind = getattr(getattr(self, "pool", None), "_unbind", None)
+        if unbind is not None:
+            unbind(self)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _sync(self):
+        if self.learner is None:
+            return
+        step = self.learner.num_env_frames
+        if step != self._synced_step:
+            self.learner.sync_policy(self.policy)
+            self._synced_step = step
+            self.syncs += 1
+
+    def serve(self, env_ids, timeout_ms=-1):
+        """One ``drl_policy_server_serve`` of these environments (at most max_batch, distinct)."""
+        ids = np.ascontiguousarray(env_ids, np.int32)
+        N = self._N
+        with self._lock:
+            if not self._s.value:
+                raise ValueError("the policy server is closed")
+            N.check(N.lib.drl_policy_server_serve(self._s, int(ids.size), N.ptr(ids), int(timeout_ms)))
+        self.batch_sizes[int(ids.size)] += 1
+
+    def serve_once(self, wait=None, timeout_ms=-1):
+        """Serves every report that is ready, waiting up to `wait` s (None: forever) for the first.  A serve blocked
+        by a full queue for `timeout_ms` (>= 0) raises ``TimeoutError_``; the reports not yet served then wait for the
+        next call.  -> the episodes that finished, as dicts of task, episode, score, episode_step and prob (the values
+        train_impala.py:170-172 logs)."""
+        if not self._todo:
+            self._workers, finished = self.pool.wait_ready(wait)
+            self._finished += finished
+            self._todo = [e for w in self._workers for e in self.pool.env_ids(w)]
+        if self._todo:
+            self._sync()
+        mb = self.policy.max_batch
+        while self._todo:
+            self.serve(self._todo[:mb], timeout_ms)
+            self._todo = self._todo[mb:]
+        self.pool.reply(self._workers)
+        self._workers = []
+        out, self._finished = self._finished, []
+        return out
+
+    def run(self, stop, on_episodes=None):
+        """serve_once until the threading.Event `stop` is set; `on_episodes` (if given) receives each non-empty list
+        of finished episodes."""
+        N = self._N
+        while not stop.is_set():
+            try:
+                episodes = self.serve_once(wait=0.05, timeout_ms=100)
+            except N.TimeoutError_:
+                continue
+            if episodes and on_episodes is not None:
+                on_episodes(episodes)

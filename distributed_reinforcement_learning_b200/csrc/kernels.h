@@ -247,6 +247,29 @@ int policy_conv_forward_tf32(cudaStream_t s, const TrunkLayout& pl, const float*
 int policy_conv_images_tf32(cudaStream_t s, const TrunkLayout& pl, const float* params, uint8_t* img_conv2,
                             uint8_t* img_conv3);
 
+// ---- policy.cu: the IMPALA policy engine's act on device-resident inputs (policy_server.cu) ------------------------
+struct PolicyCore;
+PolicyCore* policy_core_of(drl_policy* h);
+// the rows of an n-row act inside the engine's device input block
+struct PolicyInRows {
+  uint8_t* frames;   // [n][84*84*4]
+  int32_t* pa;       // [n]
+  float* h0;         // [n][256]
+  float* c0;         // [n][256]
+  double* uniform;   // [n]
+};
+// where the act's head writes: policy [n][A], h1 / c1 [n][256], action [n]
+struct PolicyOutRows {
+  float* policy;
+  float* h1;
+  float* c1;
+  int32_t* action;
+};
+PolicyInRows policy_input_rows(drl_policy* h, int n);
+// the engine's act kernels of n rows (drl_policy_act without the upload of its input block) on the engine's stream,
+// reading the rows of policy_input_rows(h, n) and writing `out`; the caller holds the engine's lock
+int policy_enqueue_forward(drl_policy* h, int n, const PolicyOutRows& out);
+
 // ---- learner.cu: parameter snapshot for the policy engine (drl_policy_sync_from_learner) ---------------------------
 // Under the learner's lock: records ev_ready on the learner's compute stream (after everything enqueued so far, a step
 // in flight included), makes `dst_stream` wait for it, copies the padded parameter vector device to device into `dst`

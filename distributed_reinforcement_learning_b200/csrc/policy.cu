@@ -296,13 +296,20 @@ struct drl_policy_recorder : RecorderCore {
 
 namespace {
 
-// the engine's act of n rows; with a recorder, the recording head and policy_record_step as well
-int enqueue_act_impl(drl_policy* h, int n, drl_policy_recorder* rec) {
+// the engine's mapped outputs of an n-row act
+PolicyOutRows mapped_outputs(drl_policy* h) {
+  return PolicyOutRows{reinterpret_cast<float*>(h->d_out), reinterpret_cast<float*>(h->d_out + h->off_h),
+                       reinterpret_cast<float*>(h->d_out + h->off_c),
+                       reinterpret_cast<int32_t*>(h->d_out + h->off_act)};
+}
+
+// the kernels of the engine's act of n rows on the device input block d_in, writing `out`; with a recorder, the
+// recording head and policy_record_step as well
+int enqueue_forward(drl_policy* h, int n, const PolicyOutRows& out, drl_policy_recorder* rec) {
   const InLayout l = in_layout(n);
   const ParamLayout& pl = h->pl;
   const float* P = h->params;
   cudaStream_t s = h->stream;
-  DRL_CUDA_CHECK(cudaMemcpyAsync(h->d_in, h->h_in, l.total, cudaMemcpyHostToDevice, s));
   const int32_t* pa = reinterpret_cast<const int32_t*>(h->d_in + l.pa);
   const float* h0 = reinterpret_cast<const float*>(h->d_in + l.h0);
   DRL_TRY(conv_forward16(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3));
@@ -315,10 +322,10 @@ int enqueue_act_impl(drl_policy* h, int n, drl_policy_recorder* rec) {
   a.w1 = P + pl.actor1_w; a.b1 = P + pl.actor1_b;
   a.w2 = P + pl.actor2_w; a.b2 = P + pl.actor2_b;
   a.w3 = P + pl.actor3_w; a.b3 = P + pl.actor3_b;
-  a.policy = reinterpret_cast<float*>(h->d_out);
-  a.h1 = reinterpret_cast<float*>(h->d_out + h->off_h);
-  a.c1 = reinterpret_cast<float*>(h->d_out + h->off_c);
-  a.action = reinterpret_cast<int32_t*>(h->d_out + h->off_act);
+  a.policy = out.policy;
+  a.h1 = out.h1;
+  a.c1 = out.c1;
+  a.action = out.action;
   a.n = n;
   a.A = h->A;
   if (!rec) {
@@ -344,6 +351,12 @@ int enqueue_act_impl(drl_policy* h, int n, drl_policy_recorder* rec) {
   r.T = rec->T;
   DRL_CUDA_CHECK((launch_k(policy_record_step_kernel, n, kRecThreads, 0, s, r)));
   return DRL_OK;
+}
+
+// the engine's act of n rows: the upload of the staged input block, then its kernels
+int enqueue_act_impl(drl_policy* h, int n, drl_policy_recorder* rec) {
+  DRL_CUDA_CHECK(cudaMemcpyAsync(h->d_in, h->h_in, in_layout(n).total, cudaMemcpyHostToDevice, h->stream));
+  return enqueue_forward(h, n, mapped_outputs(h), rec);
 }
 
 int enqueue_act(PolicyCore* c, int n) { return enqueue_act_impl(static_cast<drl_policy*>(c), n, nullptr); }
@@ -379,6 +392,23 @@ void copy_act_outputs(const drl_policy* h, int n, int32_t* action, float* policy
 }
 
 }  // namespace
+
+namespace drl {
+
+PolicyCore* policy_core_of(drl_policy* h) { return h; }
+
+PolicyInRows policy_input_rows(drl_policy* h, int n) {
+  const InLayout l = in_layout(n);
+  return PolicyInRows{h->d_in + l.frames, reinterpret_cast<int32_t*>(h->d_in + l.pa),
+                      reinterpret_cast<float*>(h->d_in + l.h0), reinterpret_cast<float*>(h->d_in + l.c0),
+                      reinterpret_cast<double*>(h->d_in + l.u)};
+}
+
+int policy_enqueue_forward(drl_policy* h, int n, const PolicyOutRows& out) {
+  return enqueue_forward(h, n, out, nullptr);
+}
+
+}  // namespace drl
 
 extern "C" {
 

@@ -5,8 +5,45 @@
 
   UnrolledTrajectory utils.py:80-119  (the actor-side accumulator whose ``extract()`` feeds ``FIFOQueue.append_to_queue``,
                                        train_impala.py:117,165-189: closes the actor -> ring -> learner loop)
+  impala_env_step    (new) the IMPALA actor's rule for one environment step, shared by actor.VectorActor and the
+                     worker processes of actor_server.EnvWorkerPool
 """
 import collections
+
+START_LIVES = 5   # the reference actor's life counter starts (and restarts after every episode) at 5
+
+
+def impala_env_step(env, action, available_action, stats, i, max_prob, task=None):
+    """One step of environment i under the IMPALA actor's rules (train_impala.py:150-175).  ``stats`` holds the
+    per-environment lists ``lives``, ``episode``, ``score``, ``episode_step`` and ``total_max_prob``; ``max_prob`` is
+    the largest probability of the policy the action was drawn from.
+
+      - the environment steps with ``action % available_action`` (the trajectory stores the action unmodified);
+      - a lost life (``info['ale.lives']`` changed) is stored as reward -1 and done=True; the score keeps the raw reward;
+      - at an episode's end the environment is reset and the caller sets previous action, h and c back to 0.
+
+    Returns (next_state, reward, done, state, finished): env.step's frame, the reward and done flag the trajectory
+    stores, the frame the next action is for (a fresh episode's first frame after an episode end), and the finished
+    episode's dict of task (``task``, default i), episode, score, episode_step and prob (mean max probability) -- the
+    values train_impala.py:170-172 logs -- or None."""
+    stats.episode_step[i] += 1
+    stats.total_max_prob[i] += float(max_prob)
+    next_state, reward, done, info = env.step(action % available_action)
+    stats.score[i] += reward
+    if stats.lives[i] != info["ale.lives"]:
+        r, d = -1.0, True
+    else:
+        r, d = reward, False
+    stats.lives[i] = info["ale.lives"]
+    state, finished = next_state, None
+    if done:
+        finished = dict(task=i if task is None else task, episode=stats.episode[i], score=stats.score[i],
+                        episode_step=stats.episode_step[i], prob=stats.total_max_prob[i] / stats.episode_step[i])
+        stats.episode[i] += 1
+        stats.score[i], stats.episode_step[i], stats.total_max_prob[i] = 0.0, 0, 0.0
+        state = env.reset()
+        stats.lives[i] = START_LIVES
+    return next_state, r, d, state, finished
 
 
 def check_properties(data):

@@ -274,6 +274,49 @@ int drl_policy_recorder_reset(drl_policy_recorder* r);
  * commit returns the CUDA error, and every later commit, stage or read of the queue returns DRL_ERR_STATE. */
 int drl_policy_recorder_commit(drl_policy_recorder* r, const float* reward, const uint8_t* done, int32_t timeout_ms);
 
+/* Policy server: one engine serving num_envs environments (1..256) that step in other processes, with each
+ * environment's recurrent state and unfinished trajectory on the GPU.  The server binds one engine, one device
+ * trajectory queue (drl_traj_queue_create below) and an exchange block the caller allocates in memory it shares with
+ * the processes that step the environments.  It keeps a device state table (per environment: h and c f32 [256], the
+ * previous action, and t, the step of the current unroll the next act records) and a device staging of one trajectory
+ * per environment in the queue's field order.
+ *
+ * Exchange block (page-aligned, at least drl_policy_server_exchange_bytes(num_envs) bytes): num_envs report records,
+ * then num_envs reply records, every field 16-byte aligned.  Before environment e is served, its report holds the
+ * frame the next action is for, the uniform draw the action is sampled with (as drl_policy_act's `uniform`), the
+ * reward and done flag the environment gave for its previous action, and `reset` = 1 when the episode restarted (the
+ * previous action, h and c taken as 0) or it is the environment's first act.  After the serve its reply holds the
+ * action and the largest probability of its policy. */
+#define DRL_SERVER_REPORT_FRAME 0          /* u8 [84,84,4]  */
+#define DRL_SERVER_REPORT_UNIFORM 28224    /* f64, in [0, 1) */
+#define DRL_SERVER_REPORT_REWARD 28240     /* f32            */
+#define DRL_SERVER_REPORT_DONE 28256       /* u8             */
+#define DRL_SERVER_REPORT_RESET 28272      /* u8             */
+#define DRL_SERVER_REPORT_BYTES 28288
+#define DRL_SERVER_REPLY_ACTION 0          /* i32            */
+#define DRL_SERVER_REPLY_MAX_PROB 16       /* f32            */
+#define DRL_SERVER_REPLY_BYTES 32
+typedef struct drl_policy_server drl_policy_server;
+/* num_envs * (REPORT_BYTES + REPLY_BYTES) rounded up to 4096; DRL_ERR_INVALID for num_envs outside [1, 256] */
+int drl_policy_server_exchange_bytes(int32_t num_envs, int64_t* bytes);
+/* Registers the exchange block with CUDA (mapped, portable) until destroy.  Queue and engine must be on the same device
+ * with the same num_action and the 84x84x4 / lstm 256 geometry, the queue must take min(num_envs, max_batch)
+ * trajectories at once, and the block must be page-aligned and large enough; all DRL_ERR_INVALID otherwise.  Without
+ * a device, DRL_ERR_CUDA.  Destroy the server before its engine and queue; after that the block may be registered
+ * again. */
+int drl_policy_server_create(drl_policy* h, drl_traj_queue* queue, int32_t num_envs, void* exchange,
+                             int64_t exchange_bytes, drl_policy_server** out);
+int drl_policy_server_destroy(drl_policy_server* s);
+/* Serves the n <= max_batch distinct environments env_ids (any subset of [0, num_envs), any order; DRL_ERR_INVALID
+ * otherwise) from their reports, in one act of the engine on its stream: the reward and done of each one's previous
+ * step land in its staged trajectory, every trajectory whose step T-1 that completes is appended to the queue (in
+ * env_ids order), then the act records step t of each environment and writes its reply.  No host thread copies frame
+ * bytes: the kernels read the reports from the registered block.  Blocks while the queue has no room for the completed
+ * trajectories (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with nothing changed otherwise).  Synchronous: the replies
+ * are written on return.  With use_cuda_graph one graph per n replays the kernels.  A failure after the queue
+ * positions were reserved puts the queue into its failed state, as drl_policy_recorder_commit. */
+int drl_policy_server_serve(drl_policy_server* s, int32_t n, const int32_t* env_ids, int32_t timeout_ms);
+
 /* ------------------------------------------------------------------------------------------
  * R2D2 policy engine (new): the actor side of train_r2d2.py:167-251 (the actor loop itself is
  * distributed_reinforcement_learning_b200/actor.py: R2D2VectorActor).  A forward-only handle that serves

@@ -1,9 +1,12 @@
 """One tiny learner step per math mode for compute-sanitizer (memcheck / racecheck / synccheck of the mbarrier + wgmma
-pipelines), and with --peer under torchrun the 2-GPU fused exchange (flag protocol over NVLink peer memory).
+pipelines), with --peer under torchrun the 2-GPU fused exchange (flag protocol over NVLink peer memory), and with
+--serve one eager serve loop of the IMPALA policy server (drl_policy_server_*: gather, per-row commit, act, scatter)
+over a registered exchange block the script fills itself, without worker processes.
 
     compute-sanitizer --tool memcheck  python tools/sanitize_step.py --modes 2 3
     compute-sanitizer --tool racecheck python tools/sanitize_step.py --modes 2
     torchrun --nproc-per-node 2 ... tools/sanitize_step.py --peer      (run each rank under compute-sanitizer)
+    DRL_B200_CUDA_GRAPH=0 compute-sanitizer --tool memcheck python tools/sanitize_step.py --serve
 """
 import argparse
 import os
@@ -15,6 +18,58 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
+def serve_loop(envs=6, max_batch=4, trajectory=3, unrolls=3):
+    """Serves `envs` environments for `unrolls` unrolls in random subsets of at most max_batch, with reset flags now
+    and then, and checks the committed trajectories' frames against the reports."""
+    import ctypes as C
+    import mmap
+    from distributed_reinforcement_learning_b200.actor_server import PolicyServer, exchange_bytes, exchange_views
+    from distributed_reinforcement_learning_b200.distributed_queue.buffer_queue import DeviceFIFOQueue
+    from distributed_reinforcement_learning_b200.model import impala_actor_critic as model
+    from distributed_reinforcement_learning_b200.policy import NativePolicy
+
+    class Block:   # the exchange block of a pool, without workers
+        def __init__(self):
+            self.num_envs, self.exchange_bytes = envs, exchange_bytes(envs)
+            self.mem = mmap.mmap(-1, self.exchange_bytes)
+            self.anchor = C.c_char.from_buffer(self.mem)
+            self.address = C.addressof(self.anchor)
+            self.views = exchange_views(self.mem, envs)
+
+    graph = os.environ.get("DRL_B200_CUDA_GRAPH", "1") != "0"
+    rng = np.random.RandomState(0)
+    pol = NativePolicy(max_batch, num_action=18, use_cuda_graph=graph)
+    pol.set_params(model.init_params(seed=0))
+    q = DeviceFIFOQueue(trajectory, (84, 84, 4), 18, envs * unrolls, envs, 1, 256)
+    blk = Block()
+    v = blk.views
+    server = PolicyServer(pol, q, blk)
+    frames = {e: [] for e in range(envs)}
+    for step in range(unrolls * trajectory + 1):
+        for e in range(envs):
+            v["frame"][e] = rng.randint(0, 256, (84, 84, 4))
+            v["uniform"][e] = rng.random_sample()
+            v["reward"][e], v["done"][e], v["reset"][e] = rng.randint(3), rng.rand() < 0.2, step == 0 or rng.rand() < 0.1
+            frames[e].append(v["frame"][e].copy())
+        ids = rng.permutation(envs).astype(np.int32)
+        k = 0
+        while k < envs:
+            c = rng.randint(1, max_batch + 1)
+            server.serve(ids[k:k + c])
+            k += c
+        assert ((v["action"][:envs] >= 0) & (v["action"][:envs] < 18)).all()
+    assert q.get_size() == envs * unrolls
+    want = {np.stack(frames[e][u * trajectory:(u + 1) * trajectory]).tobytes()
+            for e in range(envs) for u in range(unrolls)}
+    got = {q.read(j)["state"].tobytes() for j in range(envs * unrolls)}
+    assert got == want
+    server.close()
+    q.close()
+    pol.close()
+    print("serve loop (cuda graph %s): %d serves of %d environments, %d trajectories committed ok"
+          % (graph, unrolls * trajectory + 1, envs, envs * unrolls), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--modes", type=int, nargs="*", default=[2])
@@ -22,7 +77,11 @@ def main():
     ap.add_argument("--trajectory", type=int, default=3)
     ap.add_argument("--peer", action="store_true")
     ap.add_argument("--steps", type=int, default=2)
+    ap.add_argument("--serve", action="store_true", help="the policy server's serve loop instead of learner steps")
     a = ap.parse_args()
+    if a.serve:
+        serve_loop()
+        return
     from distributed_reinforcement_learning_b200.learner import NativeLearner
     from distributed_reinforcement_learning_b200.model import impala_actor_critic as model
     from oracle import synthetic
