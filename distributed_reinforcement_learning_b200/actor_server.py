@@ -277,11 +277,11 @@ class PolicyServer:
 
     def __init__(self, policy, queue, pool, learner=None):
         from . import _native as N
+        from . import dp
         from .distributed_queue.buffer_queue import DeviceFIFOQueue
-        from .learner import NativeLearner
         if not isinstance(queue, DeviceFIFOQueue):
             raise TypeError("PolicyServer: queue must be a DeviceFIFOQueue, got %s" % type(queue).__name__)
-        if NativeLearner._distributed():
+        if dp.distributed():
             raise RuntimeError("PolicyServer is single-replica: the queue lives on one device")
         self._N = N
         self.policy, self.queue, self.pool, self.learner = policy, queue, pool, learner

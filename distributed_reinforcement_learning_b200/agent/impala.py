@@ -24,6 +24,7 @@ import threading
 
 import numpy as np
 
+from .. import dp
 from ..learner import NativeLearner
 from ..model import impala_actor_critic
 
@@ -200,7 +201,7 @@ class Agent:
         learning_rate), as ``train``.  One learner thread calls it; do not interleave it with ``train`` from another
         thread (with two staging slots, a ``train`` that runs while this call waits for a batch can reuse its slot)."""
         with self._lock:
-            if NativeLearner._distributed():
+            if dp.distributed():
                 raise RuntimeError("train_from_queue is single-replica: the queue lives on one device")
             eng = self._get_engine(queue.batch_size)
             slot = self._slot

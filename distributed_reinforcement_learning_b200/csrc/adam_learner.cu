@@ -1,4 +1,4 @@
-// adam_learner.cu -- TF1 Adam and the learner-handle core of the Ape-X / A3C and the R2D2 handles (adam_learner.cuh).
+// adam_learner.cu -- TF1 Adam and the Adam layer of the Ape-X / A3C and the R2D2 handles (adam_learner.cuh).
 #include <string.h>
 
 #include "adam_learner.cuh"
@@ -103,16 +103,8 @@ int adam_step(cudaStream_t s, const AdamState& o) {
   return DRL_OK;
 }
 
-// ---- handle core ----------------------------------------------------------------------------
 
-Streams AdamLearner::streams() const {
-  Streams st;
-  st.main = compute;
-  st.side = side;
-  for (int i = 0; i < 8; ++i) st.ev[i] = fj[i];
-  st.par = par;
-  return st;
-}
+// ---- Adam layer -----------------------------------------------------------------------------
 
 Streams AdamLearner::target_streams() const {
   Streams st;
@@ -123,48 +115,49 @@ Streams AdamLearner::target_streams() const {
   return st;
 }
 
+namespace {
+
+int update(LearnerCore* core, int out_row, float grad_scale, bool, bool) {
+  AdamLearner* h = static_cast<AdamLearner*>(core);
+  AdamState o = h->opt;
+  o.out = h->d_out + 8 * out_row;
+  o.grad_scale = grad_scale;
+  prof_mark(h->compute, "optimizer(norm+adam)");
+  DRL_TRY(adam_step(h->compute, o));
+  prof_mark(h->compute, "end");
+  return DRL_OK;
+}
+
+}  // namespace
+
 int adam_learner_init(AdamLearner* h, size_t slot_bytes, size_t ones) {
-  DRL_CUDA_CHECK(cudaSetDevice(h->device));
-  DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->compute, cudaStreamNonBlocking));
-  DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->copy, cudaStreamNonBlocking));
-  DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
-  for (int i = 0; i < 8; ++i) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->fj[i], cudaEventDisableTiming));
+  h->scratch_slots = 1;
+  h->update = update;
+  DRL_TRY(learner_core_init(h, slot_bytes));
   DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->tmain, cudaStreamNonBlocking));
   DRL_CUDA_CHECK(cudaStreamCreateWithFlags(&h->tside, cudaStreamNonBlocking));
   for (int i = 0; i < 8; ++i) DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->tfj[i], cudaEventDisableTiming));
   DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_tfork, cudaEventDisableTiming));
   DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_tjoin, cudaEventDisableTiming));
-  DRL_CUDA_CHECK(cudaEventCreate(&h->ev_start));
-  DRL_CUDA_CHECK(cudaEventCreate(&h->ev_stop));
-  DRL_CUDA_CHECK(cudaEventCreateWithFlags(&h->ev_done, cudaEventDisableTiming));
   const size_t B = h->B, NP = h->layout->padded_total;
-  DRL_TRY(dev_alloc(h, &h->params, NP));
   DRL_TRY(dev_alloc(h, &h->target, NP));
   DRL_TRY(dev_alloc(h, &h->adam_m, NP));
   DRL_TRY(dev_alloc(h, &h->adam_v, NP));
-  DRL_TRY(dev_alloc(h, &h->grads, NP + 4));
-  h->loss = h->grads + NP;
   {
     size_t wb[WeightImages::kCount];
     weight_image_sizes(wb);
     for (int i : {1, 2, 5, 6}) DRL_TRY(dev_alloc(h, &h->wi.img[i], wb[i]));
     for (int i : {1, 2}) DRL_TRY(dev_alloc(h, &h->twi.img[i], wb[i]));
   }
-  DRL_TRY(dev_alloc(h, &h->d_step, 1));
-  DRL_TRY(dev_alloc(h, &h->d_lr, 1));
   DRL_TRY(dev_alloc(h, &h->d_alpha, 1));
   DRL_TRY(dev_alloc(h, &h->d_b1p, 1));
   DRL_TRY(dev_alloc(h, &h->d_b2p, 1));
   DRL_CUDA_CHECK(cudaMemcpy(h->d_b1p, &kBeta1, 4, cudaMemcpyHostToDevice));
   DRL_CUDA_CHECK(cudaMemcpy(h->d_b2p, &kBeta2, 4, cudaMemcpyHostToDevice));
   const size_t ns = h->num_slots;
-  DRL_CUDA_CHECK(cudaHostAlloc((void**)&h->h_out, ns * 8 * sizeof(float), cudaHostAllocMapped));
-  DRL_CUDA_CHECK(cudaHostGetDevicePointer((void**)&h->d_out, h->h_out, 0));
-  memset(h->h_out, 0, ns * 8 * sizeof(float));
   DRL_CUDA_CHECK(cudaHostAlloc((void**)&h->h_td, ns * B * sizeof(float), cudaHostAllocMapped));
   DRL_CUDA_CHECK(cudaHostGetDevicePointer((void**)&h->d_td, h->h_td, 0));
   memset(h->h_td, 0, ns * B * sizeof(float));
-  DRL_CUDA_CHECK(cudaHostAlloc((void**)&h->h_flat, NP * sizeof(float), cudaHostAllocDefault));
   DRL_CUDA_CHECK(cudaHostAlloc((void**)&h->h_ones, ones * sizeof(float), cudaHostAllocDefault));
   for (size_t i = 0; i < ones; ++i) h->h_ones[i] = 1.0f;
   AdamState& o = h->opt;
@@ -174,169 +167,63 @@ int adam_learner_init(AdamLearner* h, size_t slot_bytes, size_t ones) {
   o.step = h->d_step; o.lr_cur = h->d_lr; o.alpha = h->d_alpha; o.b1p = h->d_b1p; o.b2p = h->d_b2p;
   o.out = h->d_out; o.loss = h->loss;
   o.grad_scale = 1.0f;
-  h->slots.resize(ns + 1);
-  h->graph_step.assign(ns, nullptr);
-  for (AdamSlot& s : h->slots) {
-    DRL_TRY(dev_alloc(h, &s.base, slot_bytes));
-    DRL_CUDA_CHECK(cudaEventCreateWithFlags(&s.staged, cudaEventDisableTiming));
-    DRL_CUDA_CHECK(cudaEventCreateWithFlags(&s.consumed, cudaEventDisableTiming));
-  }
   return DRL_OK;
 }
 
 void adam_learner_release(AdamLearner* h) {
-  cudaSetDevice(h->device);
-  cudaDeviceSynchronize();
-  for (auto g : h->graph_step) if (g) cudaGraphExecDestroy(g);
-  for (AdamSlot& s : h->slots) {
-    if (s.staged) cudaEventDestroy(s.staged);
-    if (s.consumed) cudaEventDestroy(s.consumed);
-  }
-  for (void* p : h->allocs) cudaFree(p);
-  if (h->h_out) cudaFreeHost(h->h_out);
+  learner_core_release(h);
   if (h->h_td) cudaFreeHost(h->h_td);
-  if (h->h_flat) cudaFreeHost(h->h_flat);
   if (h->h_ones) cudaFreeHost(h->h_ones);
-  if (h->ev_start) cudaEventDestroy(h->ev_start);
-  if (h->ev_stop) cudaEventDestroy(h->ev_stop);
-  if (h->ev_done) cudaEventDestroy(h->ev_done);
-  for (int i = 0; i < 8; ++i) if (h->fj[i]) cudaEventDestroy(h->fj[i]);
   for (int i = 0; i < 8; ++i) if (h->tfj[i]) cudaEventDestroy(h->tfj[i]);
   if (h->ev_tfork) cudaEventDestroy(h->ev_tfork);
   if (h->ev_tjoin) cudaEventDestroy(h->ev_tjoin);
   if (h->tmain) cudaStreamDestroy(h->tmain);
   if (h->tside) cudaStreamDestroy(h->tside);
-  if (h->side) cudaStreamDestroy(h->side);
-  if (h->compute) cudaStreamDestroy(h->compute);
-  if (h->copy) cudaStreamDestroy(h->copy);
   cudaGetLastError();
 }
 
 namespace {
-
-int set_device(const AdamLearner* h) {
-  DRL_CUDA_CHECK(cudaSetDevice(h->device));
-  return DRL_OK;
-}
-
-int upload(AdamLearner* h, float* dev_padded, const float* host_packed) {
-  DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
-  return upload_flat(h->compute, h->h_flat, *h->layout, dev_padded, host_packed, 0.0f);
-}
-int download(AdamLearner* h, const float* dev_padded, float* host_packed) {
-  return download_flat(h->compute, h->h_flat, *h->layout, dev_padded, host_packed);
-}
 
 int check_which(int which) {
   if (which != 0 && which != 1) { set_error("which must be 0 (main) or 1 (target)"); return DRL_ERR_INVALID; }
   return DRL_OK;
 }
 
-// the main images follow the parameters, which change every step; the target images only change with the target
-// copy / set_params.  Refreshed outside of the graph so that the captured step never contains them.
-int refresh_target_images(AdamLearner* h) {
-  if (h->target_images_stale && h->mode >= 2) {
-    DRL_TRY(conv_images_tf32(h->compute, *h->layout, h->target, h->twi.img[1], h->twi.img[2]));
-  }
+// The main images follow the parameters, which change every step; the target images only change with the target
+// copy / set_params.  An eager forward rebuilds stale target images itself.  A captured step never contains that
+// rebuild (the first step's eager pass, which runs before the capture, does it), so under use_cuda_graph the images are
+// rebuilt here, outside of any graph, as soon as the target parameters change.
+int target_changed(AdamLearner* h) {
+  h->target_images_stale = true;
+  if (!h->use_cuda_graph) return DRL_OK;
+  if (h->mode >= 2) DRL_TRY(conv_images_tf32(h->compute, *h->layout, h->target, h->twi.img[1], h->twi.img[2]));
   h->target_images_stale = false;
-  return DRL_OK;
-}
-
-int enqueue_step(AdamLearner* h, int slot, int* launches) {
-  DRL_TRY(h->fwd_bwd(h, slot, launches));
-  AdamState o = h->opt;
-  o.out = h->d_out + 8 * slot;
-  prof_mark(h->compute, "optimizer(norm+adam)");
-  DRL_TRY(adam_step(h->compute, o));
-  prof_mark(h->compute, "end");
-  if (launches) *launches += 2;
-  return DRL_OK;
-}
-
-int wait_staged(AdamLearner* h, int slot) {
-  const AdamSlot& sl = h->slots[slot];
-  if (!sl.has_data) { set_error("slot %d has not been staged", slot); return DRL_ERR_STATE; }
-  DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, sl.staged, 0));
   return DRL_OK;
 }
 
 }  // namespace
 
-int adam_run_step(AdamLearner* h, int slot) {
-  DRL_TRY(wait_staged(h, slot));
-  if (h->use_cuda_graph) DRL_TRY(refresh_target_images(h));
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_start, h->compute));
-  h->main_images_stale = true;
-  int cnt = 0;
-  if (h->use_cuda_graph) {
-    if (!h->graph_step[slot]) {
-      // eager pass of forward + loss + backward first (sets the per-kernel attributes outside of capture; it does not
-      // change any state the captured pass depends on: parameters and optimizer state are only touched by the update)
-      DRL_TRY(h->fwd_bwd(h, slot, nullptr));
-      h->main_images_stale = true;
-      DRL_TRY(capture_graph(h->compute, [&] { return enqueue_step(h, slot, &cnt); }, &h->graph_step[slot]));
-      h->launches = cnt;
-    }
-    DRL_CUDA_CHECK(cudaGraphLaunch(h->graph_step[slot], h->compute));
-  } else {
-    DRL_TRY(enqueue_step(h, slot, &cnt));
-    h->launches = cnt;
-  }
-  h->main_images_stale = true;      // the update changed the main parameters
-  h->last_n = h->B;
-  h->last_slot = slot;
-  DRL_CUDA_CHECK(cudaEventRecord(h->slots[slot].consumed, h->compute));
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->compute));
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_done, h->compute));
-  h->pending = true;
-  return DRL_OK;
-}
-
-int check_handle(const AdamLearner* h, const char* family) {
-  if (!h) { set_error("null %s handle", family); return DRL_ERR_INVALID; }
-  return DRL_OK;
-}
-
-int check_slot(const AdamLearner* h, int slot) {
-  if (slot < 0 || slot >= h->num_slots) { set_error("slot %d out of range", slot); return DRL_ERR_INVALID; }
-  return DRL_OK;
-}
-
-int64_t step_of(const float* row) {
-  uint32_t lo, hi;
-  memcpy(&lo, &row[6], 4);
-  memcpy(&hi, &row[7], 4);
-  return (int64_t)(((uint64_t)hi << 32) | lo);
-}
-
-int adam_param_count(const AdamLearner* h, const char* family, int64_t* n) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (!n) { set_error("null argument"); return DRL_ERR_INVALID; }
-  *n = h->layout->packed_total;
-  return DRL_OK;
-}
-
 int adam_set_params(AdamLearner* h, const char* family, int which, const float* host_flat, int64_t n) {
   DRL_TRY(check_handle(h, family));
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   DRL_TRY(check_which(which));
+  if (which == 0) return learner_set_params(h, family, host_flat, n);
   const int64_t np = h->layout->packed_total;
   if (!host_flat || n != np) { set_error("set_params: expected %lld floats, got %lld", (long long)np, (long long)n); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  DRL_TRY(upload(h, which == 0 ? h->params : h->target, host_flat));
-  if (which == 0) h->main_images_stale = true; else h->target_images_stale = true;
-  return DRL_OK;
+  DRL_TRY(learner_upload(h, h->target, host_flat, 0.0f));
+  return target_changed(h);
 }
 
 int adam_get_params(AdamLearner* h, const char* family, int which, float* host_flat, int64_t n) {
   DRL_TRY(check_handle(h, family));
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   DRL_TRY(check_which(which));
+  if (which == 0) return learner_get_params(h, family, host_flat, n);
   const int64_t np = h->layout->packed_total;
   if (!host_flat || n != np) { set_error("get_params: expected %lld floats", (long long)np); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  return download(h, which == 0 ? h->params : h->target, host_flat);
+  return learner_download(h, h->target, host_flat);
 }
 
 int adam_set_opt_state(AdamLearner* h, const char* family, const float* host_m, const float* host_v, int64_t n,
@@ -346,8 +233,8 @@ int adam_set_opt_state(AdamLearner* h, const char* family, const float* host_m, 
   const int64_t np = h->layout->packed_total;
   if (!host_m || !host_v || n != np) { set_error("set_opt_state: expected %lld floats", (long long)np); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  DRL_TRY(upload(h, h->adam_m, host_m));
-  DRL_TRY(upload(h, h->adam_v, host_v));
+  DRL_TRY(learner_upload(h, h->adam_m, host_m, 0.0f));
+  DRL_TRY(learner_upload(h, h->adam_v, host_v, 0.0f));
   long long st = step;
   DRL_CUDA_CHECK(cudaMemcpy(h->d_step, &st, sizeof(st), cudaMemcpyHostToDevice));
   DRL_CUDA_CHECK(cudaMemcpy(h->d_b1p, &beta1_power, 4, cudaMemcpyHostToDevice));
@@ -362,8 +249,8 @@ int adam_get_opt_state(AdamLearner* h, const char* family, float* host_m, float*
   const int64_t np = h->layout->packed_total;
   if (n != np) { set_error("get_opt_state: expected %lld floats", (long long)np); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  if (host_m) DRL_TRY(download(h, h->adam_m, host_m));
-  if (host_v) DRL_TRY(download(h, h->adam_v, host_v));
+  if (host_m) DRL_TRY(learner_download(h, h->adam_m, host_m));
+  if (host_v) DRL_TRY(learner_download(h, h->adam_v, host_v));
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   if (step) {
     long long st = 0;
@@ -375,164 +262,21 @@ int adam_get_opt_state(AdamLearner* h, const char* family, float* host_m, float*
   return DRL_OK;
 }
 
-int adam_get_grads(AdamLearner* h, const char* family, float* host_flat, int64_t n) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  const int64_t np = h->layout->packed_total;
-  if (!host_flat || n != np) { set_error("get_grads: expected %lld floats", (long long)np); return DRL_ERR_INVALID; }
-  DRL_TRY(set_device(h));
-  return download(h, h->grads, host_flat);
-}
-
 int adam_main_to_target(AdamLearner* h, const char* family) {
   DRL_TRY(check_handle(h, family));
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   DRL_TRY(set_device(h));
   DRL_CUDA_CHECK(cudaMemcpyAsync(h->target, h->params, h->layout->padded_total * sizeof(float), cudaMemcpyDeviceToDevice,
                                  h->compute));
-  h->target_images_stale = true;
-  return DRL_OK;
-}
-
-int adam_params_snapshot(AdamLearner* h, const char* family, int device, cudaStream_t dst_stream, float* dst,
-                         cudaEvent_t ev_ready, cudaEvent_t ev_copied) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (h->device != device) {
-    set_error("sync: the learner is on device %d, the policy on device %d (no cross-device sync)", h->device, device);
-    return DRL_ERR_INVALID;
-  }
-  DRL_TRY(set_device(h));
-  DRL_CUDA_CHECK(cudaEventRecord(ev_ready, h->compute));
-  DRL_CUDA_CHECK(cudaStreamWaitEvent(dst_stream, ev_ready, 0));
-  DRL_CUDA_CHECK(cudaMemcpyAsync(dst, h->params, (size_t)h->layout->padded_total * sizeof(float),
-                                 cudaMemcpyDeviceToDevice, dst_stream));
-  DRL_CUDA_CHECK(cudaEventRecord(ev_copied, dst_stream));
-  DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, ev_copied, 0));
-  return DRL_OK;
-}
-
-int adam_step_async(AdamLearner* h, const char* family, int slot) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  DRL_TRY(check_slot(h, slot));
-  DRL_TRY(set_device(h));
-  return adam_run_step(h, slot);
-}
-
-// data parallel: the step in two halves around the caller's all-reduce of the bucket (eager launches)
-int adam_forward_backward(AdamLearner* h, const char* family, int slot) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  DRL_TRY(check_slot(h, slot));
-  DRL_TRY(set_device(h));
-  DRL_TRY(wait_staged(h, slot));
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_start, h->compute));
-  h->main_images_stale = true;
-  int cnt = 0;
-  DRL_TRY(h->fwd_bwd(h, slot, &cnt));
-  h->launches = cnt + 2;
-  h->last_n = h->B;
-  h->last_slot = slot;
-  DRL_CUDA_CHECK(cudaEventRecord(h->slots[slot].consumed, h->compute));
-  return DRL_OK;
-}
-
-int adam_grad_bucket(AdamLearner* h, const char* family, void** dev_ptr, int64_t* count) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (dev_ptr) *dev_ptr = h->grads;
-  if (count) *count = h->layout->padded_total + 4;
-  return DRL_OK;
-}
-
-int adam_apply(AdamLearner* h, const char* family, float grad_scale) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (!(grad_scale > 0.f)) { set_error("apply: grad_scale must be > 0"); return DRL_ERR_INVALID; }
-  DRL_TRY(set_device(h));
-  AdamState o = h->opt;
-  o.out = h->d_out + 8 * h->last_slot;
-  o.grad_scale = grad_scale;
-  DRL_TRY(adam_step(h->compute, o));
-  h->main_images_stale = true;
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->compute));
-  DRL_CUDA_CHECK(cudaEventRecord(h->ev_done, h->compute));
-  h->pending = true;
-  return DRL_OK;
+  return target_changed(h);
 }
 
 int adam_wait(AdamLearner* h, const char* family, const float** row, float* td_error) {
   DRL_TRY(check_handle(h, family));
   std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (!h->pending) { set_error("wait: no step in flight"); return DRL_ERR_STATE; }
-  DRL_TRY(set_device(h));
-  h->pending = false;
-  DRL_CUDA_CHECK(cudaEventSynchronize(h->ev_done));
-  *row = h->h_out + 8 * h->last_slot;
+  DRL_TRY(learner_wait(h, family, row));
   if (td_error) memcpy(td_error, h->h_td + (size_t)h->last_slot * h->B, (size_t)h->B * sizeof(float));
   return DRL_OK;
-}
-
-int adam_profile_step(AdamLearner* h, const char* family, int slot, char* names, int64_t names_len, float* ms,
-                      int32_t max_kernels, int32_t* count) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  DRL_TRY(check_slot(h, slot));
-  if (!names || !ms || !count) { set_error("null argument"); return DRL_ERR_INVALID; }
-  DRL_TRY(set_device(h));
-  DRL_TRY(wait_staged(h, slot));
-  DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
-  prof_begin();
-  const bool par_saved = h->par;
-  h->par = false;
-  h->main_images_stale = true;
-  int rc = enqueue_step(h, slot, nullptr);
-  h->par = par_saved;
-  h->main_images_stale = true;
-  h->last_n = h->B;
-  DRL_TRY(prof_end(h->compute, rc, names, names_len, ms, max_kernels, count));
-  h->pending = false;
-  return DRL_OK;
-}
-
-int adam_last_step_ms(AdamLearner* h, const char* family, float* ms) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (!ms) { set_error("null argument"); return DRL_ERR_INVALID; }
-  DRL_TRY(set_device(h));
-  DRL_CUDA_CHECK(cudaEventSynchronize(h->ev_stop));
-  DRL_CUDA_CHECK(cudaEventElapsedTime(ms, h->ev_start, h->ev_stop));
-  return DRL_OK;
-}
-
-int adam_stream(AdamLearner* h, const char* family, void** stream) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (!stream) { set_error("null argument"); return DRL_ERR_INVALID; }
-  *stream = h->compute;
-  return DRL_OK;
-}
-
-int adam_launches_per_step(const AdamLearner* h, const char* family, int32_t* n) {
-  DRL_TRY(check_handle(h, family));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  if (!n) { set_error("null argument"); return DRL_ERR_INVALID; }
-  *n = h->launches;     // valid after the first step
-  return DRL_OK;
-}
-
-int read_named_buffer(AdamLearner* h, const NamedBuffer* tab, int ntab, const char* name, float* host_dst, int64_t n) {
-  for (int i = 0; i < ntab; ++i) {
-    const NamedBuffer& e = tab[i];
-    if (strcmp(e.name, name) != 0) continue;
-    if ((size_t)n != e.count) { set_error("read_buffer(%s): expected %zu floats, got %lld", name, e.count, (long long)n); return DRL_ERR_INVALID; }
-    DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
-    DRL_CUDA_CHECK(cudaMemcpy(host_dst, e.p, e.count * sizeof(float), cudaMemcpyDeviceToHost));
-    return DRL_OK;
-  }
-  set_error("read_buffer: unknown buffer '%s'", name);
-  return DRL_ERR_INVALID;
 }
 
 }  // namespace drl

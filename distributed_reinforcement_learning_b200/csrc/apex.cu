@@ -327,9 +327,9 @@ int alloc_acts(drl_apex* h, ApexActs& a, int cap) {
 int drl::enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, float* td_host, int* launches) {
   const Streams st = h->streams(), tst = h->target_streams();
   if (h->algo == 1) {      // A3C: one scope; rows [0, n) = network(s, prev_a), rows [n, 2n) = network(s', a)
-    DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, sl.frames, sl.pa2, h->act, 2 * n, h->mode, h->main_images_stale,
-                         h->main_images_stale, false, launches));
-    h->main_images_stale = false;
+    DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, sl.frames, sl.pa2, h->act, 2 * n, h->mode, h->images_stale,
+                         h->images_stale, false, launches));
+    h->images_stale = false;
     A3cArgs a{};
     a.policy = h->act.scratch_sm; a.value = h->act.mstream;
     a.action = sl.pa2 + n; a.reward = sl.reward; a.done = sl.done;
@@ -352,9 +352,9 @@ int drl::enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, fl
   h->target_images_stale = false;
   if (h->par) DRL_CUDA_CHECK(cudaEventRecord(h->ev_tjoin, h->tmain));
   // rows [0, n) = s with previous_action, rows [n, 2n) = s' with action: one main-network forward covers both
-  DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, sl.frames, sl.pa2, h->act, 2 * n, h->mode, h->main_images_stale,
-                       h->main_images_stale, false, launches));
-  h->main_images_stale = false;
+  DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, sl.frames, sl.pa2, h->act, 2 * n, h->mode, h->images_stale,
+                       h->images_stale, false, launches));
+  h->images_stale = false;
   if (h->par) DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, h->ev_tjoin, 0));
   TdArgs a{};
   a.vstream = h->act.vstream; a.mstream = h->act.mstream;
@@ -374,7 +374,7 @@ int drl::enqueue_forward_td(drl_apex* h, const ApexIn& sl, int n, bool train, fl
 
 namespace {
 
-int fwd_bwd(AdamLearner* core, int slot, int* launches) {
+int fwd_bwd(LearnerCore* core, int slot, int* launches) {
   drl_apex* h = static_cast<drl_apex*>(core);
   const ApexIn& sl = h->in[slot];
   const int B = h->B;
@@ -406,9 +406,9 @@ int forward_main(drl_apex* h, int n, const uint8_t* state, const int32_t* previo
   const ApexIn& s = h->in[h->num_slots];
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   DRL_TRY(stage_into(h, s, h->compute, n, n, state, nullptr, previous_action, nullptr, nullptr, nullptr, nullptr));
-  DRL_TRY(apex_forward(h->streams(), h->pl, h->params, h->wi, s.frames, s.pa2, h->act, n, h->mode, h->main_images_stale,
-                       h->main_images_stale, false, nullptr));
-  h->main_images_stale = false;
+  DRL_TRY(apex_forward(h->streams(), h->pl, h->params, h->wi, s.frames, s.pa2, h->act, n, h->mode, h->images_stale,
+                       h->images_stale, false, nullptr));
+  h->images_stale = false;
   return DRL_OK;
 }
 
@@ -449,7 +449,7 @@ int drl_apex_create(const drl_apex_config* cfg, drl_apex** out) {
     const size_t o_dn = off; off = align_up(off + B, 256);
     const size_t o_wt = off; off = align_up(off + B * 4, 256);
     DRL_TRY(adam_learner_init(h, off, B));
-    for (const AdamSlot& s : h->slots)
+    for (const LearnerSlot& s : h->slots)
       h->in.push_back(ApexIn{s.base + o_fr, reinterpret_cast<int32_t*>(s.base + o_pa),
                              reinterpret_cast<float*>(s.base + o_rw), s.base + o_dn,
                              reinterpret_cast<float*>(s.base + o_wt)});
@@ -488,7 +488,7 @@ int drl_apex_destroy(drl_apex* h) {
   return DRL_OK;
 }
 
-int drl_apex_param_count(const drl_apex* h, int64_t* n) { return adam_param_count(h, kName, n); }
+int drl_apex_param_count(const drl_apex* h, int64_t* n) { return learner_param_count(h, kName, n); }
 int drl_apex_set_params(drl_apex* h, int32_t which, const float* host_flat, int64_t n) {
   return adam_set_params(h, kName, which, host_flat, n);
 }
@@ -503,7 +503,7 @@ int drl_apex_get_opt_state(drl_apex* h, float* host_m, float* host_v, int64_t n,
                            float* beta2_power) {
   return adam_get_opt_state(h, kName, host_m, host_v, n, step, beta1_power, beta2_power);
 }
-int drl_apex_get_grads(drl_apex* h, float* host_flat, int64_t n) { return adam_get_grads(h, kName, host_flat, n); }
+int drl_apex_get_grads(drl_apex* h, float* host_flat, int64_t n) { return learner_get_grads(h, kName, h->grads, host_flat, n); }
 int drl_apex_target_to_main(drl_apex* h) { return adam_main_to_target(h, kName); }   // target <- main (sic)
 
 int drl_apex_stage(drl_apex* h, int32_t slot, const uint8_t* state, const uint8_t* next_state,
@@ -514,7 +514,7 @@ int drl_apex_stage(drl_apex* h, int32_t slot, const uint8_t* state, const uint8_
   DRL_TRY(check_slot(h, slot));
   if (!state || !next_state || !previous_action || !action || !reward || !done) { set_error("stage: null input pointer"); return DRL_ERR_INVALID; }
   DRL_CUDA_CHECK(cudaSetDevice(h->device));
-  AdamSlot& s = h->slots[slot];
+  LearnerSlot& s = h->slots[slot];
   DRL_CUDA_CHECK(cudaStreamWaitEvent(h->copy, s.consumed, 0));
   DRL_TRY(stage_into(h, h->in[slot], h->copy, h->B, h->B, state, next_state, previous_action, action, reward, done,
                      is_weight));
@@ -523,10 +523,10 @@ int drl_apex_stage(drl_apex* h, int32_t slot, const uint8_t* state, const uint8_
   return DRL_OK;
 }
 
-int drl_apex_step_async(drl_apex* h, int32_t slot) { return adam_step_async(h, kName, slot); }
-int drl_apex_forward_backward(drl_apex* h, int32_t slot) { return adam_forward_backward(h, kName, slot); }
-int drl_apex_grad_bucket(drl_apex* h, void** dev_ptr, int64_t* count) { return adam_grad_bucket(h, kName, dev_ptr, count); }
-int drl_apex_apply(drl_apex* h, float grad_scale) { return adam_apply(h, kName, grad_scale); }
+int drl_apex_step_async(drl_apex* h, int32_t slot) { return learner_step_async(h, kName, slot); }
+int drl_apex_forward_backward(drl_apex* h, int32_t slot) { return learner_forward_backward(h, kName, slot); }
+int drl_apex_grad_bucket(drl_apex* h, void** dev_ptr, int64_t* count) { return learner_grad_bucket(h, kName, dev_ptr, count); }
+int drl_apex_apply(drl_apex* h, float grad_scale) { return learner_apply(h, kName, grad_scale); }
 
 int drl_apex_wait(drl_apex* h, drl_apex_out* out, float* td_error) {
   DRL_TRY(check_handle(h, kName));
@@ -560,9 +560,9 @@ int drl_apex_td_error(drl_apex* h, int32_t n, const uint8_t* state, const uint8_
   // rows [0, n) = s, rows [n, 2n) = s' (packed, so that one main-network forward covers both)
   DRL_TRY(stage_into(h, s, h->compute, n, n, state, next_state, previous_action, action, reward, done, nullptr));
   const Streams st = h->streams();
-  DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, s.frames, s.pa2, h->act, 2 * n, h->mode, h->main_images_stale,
-                       h->main_images_stale, false, nullptr));
-  h->main_images_stale = false;
+  DRL_TRY(apex_forward(st, h->pl, h->params, h->wi, s.frames, s.pa2, h->act, 2 * n, h->mode, h->images_stale,
+                       h->images_stale, false, nullptr));
+  h->images_stale = false;
   DRL_TRY(apex_forward(st, h->pl, h->target, h->twi, s.frames + (size_t)n * Geo::FRAME, s.pa2 + n, h->tact, n, h->mode,
                        h->target_images_stale, false, true, nullptr));
   h->target_images_stale = false;
@@ -632,11 +632,11 @@ int drl_apex_read_buffer(drl_apex* h, const char* name, float* host_dst, int64_t
 
 int drl_apex_profile_step(drl_apex* h, int32_t slot, char* names, int64_t names_len, float* ms, int32_t max_kernels,
                           int32_t* count) {
-  return adam_profile_step(h, kName, slot, names, names_len, ms, max_kernels, count);
+  return learner_profile_step(h, kName, slot, names, names_len, ms, max_kernels, count);
 }
-int drl_apex_last_step_ms(drl_apex* h, float* ms) { return adam_last_step_ms(h, kName, ms); }
-int drl_apex_stream(drl_apex* h, void** stream) { return adam_stream(h, kName, stream); }
-int drl_apex_launches_per_step(const drl_apex* h, int32_t* n) { return adam_launches_per_step(h, kName, n); }
+int drl_apex_last_step_ms(drl_apex* h, float* ms) { return learner_last_step_ms(h, kName, ms); }
+int drl_apex_stream(drl_apex* h, void** stream) { return learner_stream(h, kName, stream); }
+int drl_apex_launches_per_step(const drl_apex* h, int32_t* n) { return learner_launches_per_step(h, kName, n); }
 
 // ---- A3C learner: the same handle type with algo = 1 (include/drl_b200.h) ---------------------------------------
 int drl_a3c_create(const drl_a3c_config* cfg, drl_a3c** out) {
@@ -700,7 +700,7 @@ int drl_a3c_stage_from_queue(drl_a3c* h, int32_t slot, drl_a3c_queue* q, int32_t
   DRL_TRY(traj_queue_pop(q, timeout_ms, &qs, &ev_commit));
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   NvtxRange nv("drl:a3c_stage_from_queue");
-  AdamSlot& s = h->slots[slot];
+  LearnerSlot& s = h->slots[slot];
   const ApexIn& in = h->in[slot];
   const int rc = [&]() -> int {
     DRL_CUDA_CHECK(cudaSetDevice(h->device));
@@ -789,5 +789,5 @@ int drl::apex_params_snapshot(drl_apex* h, int device, int algo, int num_action,
               algo ? "A3C" : "Ape-X", num_action);
     return DRL_ERR_INVALID;
   }
-  return adam_params_snapshot(h, kName, device, dst_stream, dst, ev_ready, ev_copied);
+  return learner_params_snapshot(h, kName, device, dst_stream, dst, ev_ready, ev_copied);
 }

@@ -32,7 +32,7 @@ struct ApexLayout : TrunkLayout {
 constexpr int kHeadN = 2 * Geo::HID;             // 512 columns: [value hidden | mean hidden]
 constexpr int kCat = Geo::FLAT + Geo::EMB;       // 3392
 
-// drl_apex_policy_sync_from_learner: adam_params_snapshot of the main network of an Ape-X (algo 0) or A3C (algo 1)
+// drl_apex_policy_sync_from_learner: learner_params_snapshot of the main network of an Ape-X (algo 0) or A3C (algo 1)
 // learner with num_action actions (DRL_ERR_INVALID for another algo or num_action)
 int apex_params_snapshot(drl_apex* h, int device, int algo, int num_action, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);

@@ -61,7 +61,7 @@ __device__ __forceinline__ void kernel_prologue() {
   }
 }
 typedef void (*TraceSetter)(unsigned long long*);
-int register_trace_setter(TraceSetter f);            // learner.cu
+int register_trace_setter(TraceSetter f);            // learner_core.cu
 static void trace_set_tu(unsigned long long* p) { cudaMemcpyToSymbol(g_trace_tu, &p, sizeof(p)); }
 static const int g_trace_registered = register_trace_setter(&trace_set_tu);
 

@@ -1,4 +1,4 @@
-// kernels.h -- internal interface between the learner orchestration (learner.cu; adam_learner.cu with apex.cu and
+// kernels.h -- internal interface between the learner orchestration (learner_core.cu with learner.cu; adam_learner.cu with apex.cu and
 // r2d2.cu) and the kernel launchers (layers.cu, elementwise.cu, vtrace.cu, optimizer.cu).  Not part of the C-ABI.
 #pragma once
 #include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: no link dependency, a no-op unless a profiler injects itself
@@ -190,7 +190,7 @@ constexpr int kLstmSplits = 8;   // slabs allocated for the LSTM split-K partial
 #define DRL_DEFAULT_MATH_MODE_IMPALA 5   // IMPALA handle: wgmma with 16-bit split operands (gemm_umma16.cuh)
 #endif
 
-// Per-kernel device timing (learner.cu): when a profile run is active, prof_mark records a CUDA event
+// Per-kernel device timing (learner_core.cu): when a profile run is active, prof_mark records a CUDA event
 // on the launching stream before each named launch; otherwise it is a no-op.
 void prof_mark(cudaStream_t s, const char* name);
 // profile run bracket (shared by the IMPALA and the Ape-X learner): prof_begin arms prof_mark; prof_end synchronises
@@ -271,13 +271,10 @@ PolicyInRows policy_input_rows(drl_policy* h, int n);
 int policy_enqueue_forward(drl_policy* h, int n, const PolicyOutRows& out);
 
 // ---- learner.cu: parameter snapshot for the policy engine (drl_policy_sync_from_learner) ---------------------------
-// Under the learner's lock: records ev_ready on the learner's compute stream (after everything enqueued so far, a step
-// in flight included), makes `dst_stream` wait for it, copies the padded parameter vector device to device into `dst`
-// on `dst_stream`, records ev_copied there and makes the compute stream wait for it, so that the learner's next update
-// cannot overwrite the parameters while they are read.  DRL_ERR_INVALID for a learner on another device or with another
-// num_action, DRL_ERR_STATE for a learner in the failed state.
-int learner_params_snapshot(drl_learner* h, int device, int num_action, cudaStream_t dst_stream, float* dst,
-                            cudaEvent_t ev_ready, cudaEvent_t ev_copied);
+// learner_params_snapshot (learner_core.cuh) of an IMPALA learner whose network has num_action actions:
+// DRL_ERR_INVALID for a learner with another num_action, DRL_ERR_STATE for a learner in the failed state.
+int impala_params_snapshot(drl_learner* h, int device, int num_action, cudaStream_t dst_stream, float* dst,
+                           cudaEvent_t ev_ready, cudaEvent_t ev_copied);
 
 // ---- elementwise.cu -----------------------------------------------------------------------
 int emb_forward(cudaStream_t s, const float* w1, const float* b1, const float* w2, const float* b2, float* e1,

@@ -461,7 +461,7 @@ int drl_policy_get_params(drl_policy* h, float* host_flat, int64_t n) {
 }
 int drl_policy_sync_from_learner(drl_policy* h, drl_learner* learner) {
   return policy_sync(h, kName, learner, [&] {
-    return learner_params_snapshot(learner, h->device, h->A, h->stream, h->params, h->ev_ready, h->ev_copied);
+    return impala_params_snapshot(learner, h->device, h->A, h->stream, h->params, h->ev_ready, h->ev_copied);
   });
 }
 int drl_policy_last_act_ms(drl_policy* h, float* ms) { return policy_last_act_ms(h, kName, ms); }

@@ -88,7 +88,7 @@ int policy_check(const PolicyCore* h, const char* family);
 int policy_param_count(const PolicyCore* h, const char* family, int64_t* n);
 int policy_set_params(PolicyCore* h, const char* family, const float* host_flat, int64_t n);
 int policy_get_params(PolicyCore* h, const char* family, float* host_flat, int64_t n);
-// parameter_sync: `snapshot` is the family's learner snapshot (learner_params_snapshot, r2d2_params_snapshot or
+// parameter_sync: `snapshot` is the family's learner snapshot (impala_params_snapshot, r2d2_params_snapshot or
 // apex_params_snapshot) of `learner` into params on the engine's stream, ordered by ev_ready / ev_copied
 int policy_sync(PolicyCore* h, const char* family, const void* learner, const std::function<int()>& snapshot);
 int policy_last_act_ms(PolicyCore* h, const char* family, float* ms);

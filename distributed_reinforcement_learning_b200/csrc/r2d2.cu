@@ -506,9 +506,9 @@ int drl::enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, flo
                      true, launches));
   h->target_images_stale = false;
   if (h->par) DRL_CUDA_CHECK(cudaEventRecord(h->ev_tjoin, h->tmain));
-  DRL_TRY(r2_forward(st, h->pl, h->params, h->wi, in, h->act, nullptr, nb, h->S, h->mode, h->main_images_stale,
-                     h->main_images_stale, false, launches));
-  h->main_images_stale = false;
+  DRL_TRY(r2_forward(st, h->pl, h->params, h->wi, in, h->act, nullptr, nb, h->S, h->mode, h->images_stale,
+                     h->images_stale, false, launches));
+  h->images_stale = false;
   if (h->par) DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, h->ev_tjoin, 0));
   R2TdArgs a{};
   a.mq = h->act.q; a.tq = h->tact.q;
@@ -545,7 +545,7 @@ int alloc_acts(drl_r2d2* h, R2Acts& a) {
   return DRL_OK;
 }
 
-int fwd_bwd(AdamLearner* core, int slot, int* launches) {
+int fwd_bwd(LearnerCore* core, int slot, int* launches) {
   drl_r2d2* h = static_cast<drl_r2d2*>(core);
   const R2In& in = h->in[slot];
   DRL_TRY(enqueue_forward_td(h, in, h->B, true, h->d_td + (size_t)slot * h->B, launches));
@@ -618,7 +618,7 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
     const size_t o_dn = off; off = align_up(off + M, 256);
     const size_t o_wt = off; off = align_up(off + M * 4, 256);
     DRL_TRY(adam_learner_init(h, off, M));
-    for (const AdamSlot& s : h->slots)
+    for (const LearnerSlot& s : h->slots)
       h->in.push_back(R2In{s.base + o_fr, reinterpret_cast<int32_t*>(s.base + o_pa),
                            reinterpret_cast<int32_t*>(s.base + o_ac), reinterpret_cast<float*>(s.base + o_h),
                            reinterpret_cast<float*>(s.base + o_c), reinterpret_cast<float*>(s.base + o_rw),
@@ -657,7 +657,7 @@ int drl_r2d2_destroy(drl_r2d2* h) {
   return DRL_OK;
 }
 
-int drl_r2d2_param_count(const drl_r2d2* h, int64_t* n) { return adam_param_count(h, kName, n); }
+int drl_r2d2_param_count(const drl_r2d2* h, int64_t* n) { return learner_param_count(h, kName, n); }
 int drl_r2d2_set_params(drl_r2d2* h, int32_t which, const float* host_flat, int64_t n) {
   return adam_set_params(h, kName, which, host_flat, n);
 }
@@ -672,7 +672,7 @@ int drl_r2d2_get_opt_state(drl_r2d2* h, float* host_m, float* host_v, int64_t n,
                            float* beta2_power) {
   return adam_get_opt_state(h, kName, host_m, host_v, n, step, beta1_power, beta2_power);
 }
-int drl_r2d2_get_grads(drl_r2d2* h, float* host_flat, int64_t n) { return adam_get_grads(h, kName, host_flat, n); }
+int drl_r2d2_get_grads(drl_r2d2* h, float* host_flat, int64_t n) { return learner_get_grads(h, kName, h->grads, host_flat, n); }
 int drl_r2d2_main_to_target(drl_r2d2* h) { return adam_main_to_target(h, kName); }
 
 int drl_r2d2_stage(drl_r2d2* h, int32_t slot, const uint8_t* state, const int32_t* previous_action, const int32_t* action,
@@ -682,7 +682,7 @@ int drl_r2d2_stage(drl_r2d2* h, int32_t slot, const uint8_t* state, const int32_
   DRL_TRY(check_slot(h, slot));
   if (!state || !previous_action || !action || !h0 || !c0 || !reward || !done) { set_error("stage: null input pointer"); return DRL_ERR_INVALID; }
   DRL_CUDA_CHECK(cudaSetDevice(h->device));
-  AdamSlot& s = h->slots[slot];
+  LearnerSlot& s = h->slots[slot];
   DRL_CUDA_CHECK(cudaStreamWaitEvent(h->copy, s.consumed, 0));
   DRL_TRY(stage_into(h, h->in[slot], h->copy, h->B, h->S, state, previous_action, action, h0, c0, reward, done, weight));
   DRL_CUDA_CHECK(cudaEventRecord(s.staged, h->copy));
@@ -701,15 +701,15 @@ int drl::r2d2_params_snapshot(drl_r2d2* h, int device, int num_action, int chann
               channels);
     return DRL_ERR_INVALID;
   }
-  return adam_params_snapshot(h, kName, device, dst_stream, dst, ev_ready, ev_copied);
+  return learner_params_snapshot(h, kName, device, dst_stream, dst, ev_ready, ev_copied);
 }
 
 extern "C" {
 
-int drl_r2d2_step_async(drl_r2d2* h, int32_t slot) { return adam_step_async(h, kName, slot); }
-int drl_r2d2_forward_backward(drl_r2d2* h, int32_t slot) { return adam_forward_backward(h, kName, slot); }
-int drl_r2d2_grad_bucket(drl_r2d2* h, void** dev_ptr, int64_t* count) { return adam_grad_bucket(h, kName, dev_ptr, count); }
-int drl_r2d2_apply(drl_r2d2* h, float grad_scale) { return adam_apply(h, kName, grad_scale); }
+int drl_r2d2_step_async(drl_r2d2* h, int32_t slot) { return learner_step_async(h, kName, slot); }
+int drl_r2d2_forward_backward(drl_r2d2* h, int32_t slot) { return learner_forward_backward(h, kName, slot); }
+int drl_r2d2_grad_bucket(drl_r2d2* h, void** dev_ptr, int64_t* count) { return learner_grad_bucket(h, kName, dev_ptr, count); }
+int drl_r2d2_apply(drl_r2d2* h, float grad_scale) { return learner_apply(h, kName, grad_scale); }
 
 int drl_r2d2_wait(drl_r2d2* h, drl_r2d2_out* out, float* td_error) {
   DRL_TRY(check_handle(h, kName));
@@ -757,9 +757,9 @@ int drl_r2d2_act(drl_r2d2* h, int32_t n, const uint8_t* state, const int32_t* pr
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   DRL_TRY(stage_into(h, in, h->compute, n, 1, state, previous_action, nullptr, h_in, c_in, nullptr, nullptr, nullptr));
   in.done = nullptr;                                     // a single step: nothing is carried
-  DRL_TRY(r2_forward(h->streams(), h->pl, h->params, h->wi, in, h->act, h->c_last, n, 1, h->mode, h->main_images_stale,
-                     h->main_images_stale, false, nullptr));
-  h->main_images_stale = false;
+  DRL_TRY(r2_forward(h->streams(), h->pl, h->params, h->wi, in, h->act, h->c_last, n, 1, h->mode, h->images_stale,
+                     h->images_stale, false, nullptr));
+  h->images_stale = false;
   if (q_value) DRL_CUDA_CHECK(cudaMemcpyAsync(q_value, h->act.q, (size_t)n * h->A * 4, cudaMemcpyDeviceToHost, h->compute));
   if (h_out) DRL_CUDA_CHECK(cudaMemcpyAsync(h_out, h->act.hout, (size_t)n * kR2L * 4, cudaMemcpyDeviceToHost, h->compute));
   if (c_out) DRL_CUDA_CHECK(cudaMemcpyAsync(c_out, h->c_last, (size_t)n * kR2L * 4, cudaMemcpyDeviceToHost, h->compute));
@@ -809,10 +809,10 @@ int drl_r2d2_read_buffer(drl_r2d2* h, const char* name, float* host_dst, int64_t
 
 int drl_r2d2_profile_step(drl_r2d2* h, int32_t slot, char* names, int64_t names_len, float* ms, int32_t max_kernels,
                           int32_t* count) {
-  return adam_profile_step(h, kName, slot, names, names_len, ms, max_kernels, count);
+  return learner_profile_step(h, kName, slot, names, names_len, ms, max_kernels, count);
 }
-int drl_r2d2_last_step_ms(drl_r2d2* h, float* ms) { return adam_last_step_ms(h, kName, ms); }
-int drl_r2d2_stream(drl_r2d2* h, void** stream) { return adam_stream(h, kName, stream); }
-int drl_r2d2_launches_per_step(const drl_r2d2* h, int32_t* n) { return adam_launches_per_step(h, kName, n); }
+int drl_r2d2_last_step_ms(drl_r2d2* h, float* ms) { return learner_last_step_ms(h, kName, ms); }
+int drl_r2d2_stream(drl_r2d2* h, void** stream) { return learner_stream(h, kName, stream); }
+int drl_r2d2_launches_per_step(const drl_r2d2* h, int32_t* n) { return learner_launches_per_step(h, kName, n); }
 
 }  // extern "C"

@@ -29,7 +29,7 @@ struct R2Layout : TrunkLayout {
   }
 };
 
-// drl_r2d2_policy_sync_from_learner: adam_params_snapshot of an R2D2 learner whose network has num_action actions and
+// drl_r2d2_policy_sync_from_learner: learner_params_snapshot of an R2D2 learner whose network has num_action actions and
 // `channels` input channels (DRL_ERR_INVALID otherwise)
 int r2d2_params_snapshot(drl_r2d2* h, int device, int num_action, int channels, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);

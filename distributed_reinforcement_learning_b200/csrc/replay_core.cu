@@ -295,7 +295,7 @@ int replay_step(ReplayCore* r, AdamLearner* learner, int slot, const double* u01
   DRL_TRY(replay_acquire(ub, (size_t)B * 8));
   memcpy(ub.h, u01, (size_t)B * 8);
   const cudaStream_t s = learner->compute;
-  AdamSlot& sl = learner->slots[slot];
+  LearnerSlot& sl = learner->slots[slot];
   DRL_TRY(replay_begin(r, s));
   if (sl.has_data) DRL_CUDA_CHECK(cudaStreamWaitEvent(s, sl.staged, 0));   // an earlier drl_*_stage of the slot
   DRL_TRY(replay_launch_sample(r, s, B, reinterpret_cast<const double*>(ub.d), weight32));
@@ -303,10 +303,10 @@ int replay_step(ReplayCore* r, AdamLearner* learner, int slot, const double* u01
   DRL_TRY(gather(s));
   DRL_CUDA_CHECK(cudaEventRecord(sl.staged, s));
   sl.has_data = true;
-  DRL_TRY(adam_run_step(learner, slot));
+  DRL_TRY(learner_run_step(learner, slot));
   // Memory.update of the sampled leaves with the step's |td|, before drl_*_wait returns
   DRL_TRY(replay_launch_update(r, s, B, r->d_tree_index, 0, nullptr, td_dev));
-  DRL_CUDA_CHECK(cudaEventRecord(learner->ev_done, s));
+  DRL_CUDA_CHECK(cudaEventRecord(learner->ev_done[learner->last_row], s));
   return replay_end(r, s);
 }
 

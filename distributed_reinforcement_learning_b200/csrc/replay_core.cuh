@@ -89,8 +89,8 @@ void replay_advance(ReplayCore* r, int n);
 // The training half of one learner-loop iteration on the learner's compute stream (the caller holds both locks and has
 // checked the learner and the slot): Memory.sample(B) with the uniforms u01 [B], the importance weights as float32 into
 // `weight32` (the slot's weight view), gather(stream) of the sampled rows r->d_data_index [B] into the slot (after an
-// earlier drl_*_stage of the slot), the learner's step (adam_run_step), and Memory.update of the sampled leaves with
-// the step's |td| (td_dev), before the learner's ev_done.  DRL_ERR_STATE on an empty memory.
+// earlier drl_*_stage of the slot), the learner's step (learner_run_step), and Memory.update of the sampled leaves with
+// the step's |td| (td_dev), before the done event of the learner's result row.  DRL_ERR_STATE on an empty memory.
 int replay_step(ReplayCore* r, AdamLearner* learner, int slot, const double* u01, float* weight32, const float* td_dev,
                 const std::function<int(cudaStream_t)>& gather);
 

@@ -13,11 +13,15 @@ import ctypes as C
 import numpy as np
 
 from . import _native as N
+from . import dp
+from .learner_handle import LearnerHandle
 
 H, W, CH, LSTM = 84, 84, 4, 256
 
 
-class NativeLearner:
+class NativeLearner(LearnerHandle):
+    family = "learner"
+
     def __init__(self, batch, trajectory=20, num_action=18, lstm_hidden_size=256, input_shape=(84, 84, 4),
                  discount_factor=0.99, start_learning_rate=0.0006, end_learning_rate=0.0,
                  learning_frame=1000000000, baseline_loss_coef=1.0, entropy_coef=0.05,
@@ -33,29 +37,9 @@ class NativeLearner:
                               end_learning_rate, float(learning_frame), baseline_loss_coef, entropy_coef,
                               gradient_clip_norm, N.REWARD_CLIPPING[reward_clipping], self.device, int(num_slots),
                               int(bool(use_cuda_graph)), int(math_mode))
-        self._h = C.c_void_p()
-        N.check(N.lib.drl_learner_create(C.byref(cfg), C.byref(self._h)))
-        n = C.c_int64()
-        N.check(N.lib.drl_learner_param_count(self._h, C.byref(n)))
-        self.param_count = int(n.value)
-        self.num_slots = int(num_slots)
-        self._keep = [None] * self.num_slots     # host arrays referenced by in-flight H2D copies
-        self._bucket = None
-        self._ext_stream = None
+        self._create(cfg, self.device, num_slots)
         self._peer = False
         self._no_collective = False          # diagnostic only (bench.py --collective none)
-
-    # ---- lifetime ----------------------------------------------------------------
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h.value:
-            N.lib.drl_learner_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # ---- parameters / optimizer state ---------------------------------------------
     def set_params(self, flat):
@@ -76,11 +60,6 @@ class NativeLearner:
         st = C.c_int64()
         N.check(N.lib.drl_learner_get_opt_state(self._h, N.ptr(a), a.size, C.byref(st)))
         return a, int(st.value)
-
-    def get_grads(self):
-        a = np.empty(self.param_count, np.float32)
-        N.check(N.lib.drl_learner_get_grads(self._h, N.ptr(a), a.size))
-        return a
 
     # ---- data path -----------------------------------------------------------------
     def stage(self, slot, state, reward, action, done, behavior_policy, previous_action, initial_h, initial_c):
@@ -110,7 +89,7 @@ class NativeLearner:
 
     def step(self, slot=0):
         """sess.run([... train_op]) of agent/impala.py:144-146 on a staged slot."""
-        if self._distributed() and not self._peer:
+        if dp.distributed() and not self._peer:
             self.step_async(slot)
             return self.wait()
         o = N.StepOut()
@@ -120,10 +99,10 @@ class NativeLearner:
     def step_async(self, slot=0):
         if self._peer or self._no_collective:   # peer: the exchange is part of the step's CUDA graph (csrc/peer.cu)
             N.check(N.lib.drl_learner_step_async(self._h, slot))
-        elif self._distributed():
+        elif dp.distributed():
             N.check(N.lib.drl_learner_forward_backward(self._h, slot))
-            self._allreduce_bucket()
-            N.check(N.lib.drl_learner_apply(self._h))
+            self._dp.all_reduce()
+            N.check(N.lib.drl_learner_apply(self._h))     # no grad_scale: the losses are batch sums
         else:
             N.check(N.lib.drl_learner_step_async(self._h, slot))
 
@@ -155,11 +134,6 @@ class NativeLearner:
         N.check(N.lib.drl_learner_taps(self._h, *[N.ptr(a) for a in out]))
         return dict(vs=out[0], clipped_rho=out[1], vs_plus_1=out[2], pg_advantage=out[3])
 
-    def read_buffer(self, name, count):
-        a = np.empty(int(count), np.float32)
-        N.check(N.lib.drl_learner_read_buffer(self._h, name.encode(), N.ptr(a), a.size))
-        return a
-
     def act(self, state, previous_action, h, c):
         """n single-step forwards (agent/impala.py:118-130 without the sampling)."""
         st = N.as_c(state, np.uint8)
@@ -175,40 +149,7 @@ class NativeLearner:
                                       N.ptr(ho), N.ptr(co)))
         return pol, ho, co
 
-    def profile_step(self, slot=0, max_kernels=128):
-        """One real step with a CUDA event before every launch -> [(kernel name, device ms)]."""
-        names = C.create_string_buffer(8192)
-        ms = np.zeros(max_kernels, np.float32)
-        cnt = C.c_int32()
-        N.check(N.lib.drl_learner_profile_step(self._h, slot, names, len(names), N.ptr(ms), max_kernels,
-                                               C.byref(cnt)))
-        nm = names.value.decode().split("\n") if cnt.value else []
-        return list(zip(nm, [float(x) for x in ms[:cnt.value]]))
-
-    def last_step_ms(self):
-        ms = C.c_float()
-        N.check(N.lib.drl_learner_last_step_ms(self._h, C.byref(ms)))
-        return float(ms.value)
-
-    def launches_per_step(self):
-        n = C.c_int32()
-        N.check(N.lib.drl_learner_launches_per_step(self._h, C.byref(n)))
-        return int(n.value)
-
-    def stream_ptr(self):
-        s = C.c_void_p()
-        N.check(N.lib.drl_learner_stream(self._h, C.byref(s)))
-        return int(s.value or 0)
-
     # ---- data parallel ---------------------------------------------------------------
-    @staticmethod
-    def _distributed():
-        try:
-            import torch.distributed as dist
-        except Exception:      # pragma: no cover
-            return False
-        return dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
-
     def enable_peer_exchange(self, group=None):
         """Replace the NCCL all-reduce of the gradient bucket by the fused exchange over NVLink peer memory
         (csrc/peer.cu): the ranks of ONE node swap CUDA-IPC handles here (a 128-byte all_gather), after which
@@ -216,7 +157,7 @@ class NativeLearner:
         Returns True when every rank could map every peer; otherwise all ranks stay on the NCCL path (False)."""
         import torch
         import torch.distributed as dist
-        if not self._distributed():
+        if not dp.distributed():
             raise RuntimeError("enable_peer_exchange needs an initialised process group with world_size > 1")
         rank, world = dist.get_rank(group), dist.get_world_size(group)
         dev = torch.device("cuda", self.device)
@@ -240,17 +181,7 @@ class NativeLearner:
 
     def bucket_tensor(self):
         """torch view (no copy) of the device gradient bucket [padded grads | 3 loss sums | pad]."""
-        if self._bucket is None:
-            import torch
-            p, n = C.c_void_p(), C.c_int64()
-            N.check(N.lib.drl_learner_grad_bucket(self._h, C.byref(p), C.byref(n)))
-
-            class _View:
-                __cuda_array_interface__ = {"shape": (int(n.value),), "typestr": "<f4",
-                                            "data": (int(p.value), False), "version": 2}
-            self._bucket = torch.as_tensor(_View(), device="cuda:%d" % self.device)
-            self._ext_stream = torch.cuda.ExternalStream(self.stream_ptr(), device="cuda:%d" % self.device)
-        return self._bucket
+        return self._dp._tensor()
 
     def reduced_tensor(self):
         """torch view (no copy) of the bucket the update reads (the peer exchange's ``reduced`` buffer, else the
@@ -263,13 +194,6 @@ class NativeLearner:
             __cuda_array_interface__ = {"shape": (int(n.value),), "typestr": "<f4",
                                         "data": (int(p.value), False), "version": 2}
         return torch.as_tensor(_View(), device="cuda:%d" % self.device)
-
-    def _allreduce_bucket(self):
-        import torch
-        import torch.distributed as dist
-        t = self.bucket_tensor()
-        with torch.cuda.stream(self._ext_stream):       # ordered after backward, before apply
-            dist.all_reduce(t, op=dist.ReduceOp.SUM)
 
 
 def shard_range(rank, world_size, batch_total):

@@ -1,7 +1,7 @@
-"""The Ape-X, A3C and R2D2 handles share one core (csrc/adam_learner.cuh).  What it promises, for every family at small
-shapes: the CUDA-graph and the eager step compute the same bits, the data-parallel halves (forward_backward +
-apply(1.0)) compute what one step computes, parameter and optimizer state round-trip bitwise, and each misuse of the
-C-ABI fails with the same error code."""
+"""The IMPALA, Ape-X, A3C and R2D2 handles share one core (csrc/learner_core.cuh).  What it promises, for every family at
+small shapes: the CUDA-graph and the eager step compute the same bits, the data-parallel halves (forward_backward +
+apply, graph or eager) compute what one step computes, parameter and optimizer state round-trip bitwise, and each
+misuse of the C-ABI fails with the same error code."""
 import ctypes as C
 
 import numpy as np
@@ -9,11 +9,14 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
-FAMILIES = ["apex", "a3c", "r2d2"]
+FAMILIES = ["learner", "apex", "a3c", "r2d2"]
 A = 4
 
 
 def _learner(family, use_cuda_graph):
+    if family == "learner":
+        from distributed_reinforcement_learning_b200.learner import NativeLearner
+        return NativeLearner(batch=2, trajectory=5, num_action=A, use_cuda_graph=use_cuda_graph)
     if family == "apex":
         from distributed_reinforcement_learning_b200.apex_learner import NativeApexLearner
         return NativeApexLearner(batch=4, num_action=A, use_cuda_graph=use_cuda_graph)
@@ -26,7 +29,7 @@ def _learner(family, use_cuda_graph):
 
 def _init(eng, seed=0):
     rng = np.random.default_rng(seed)
-    if eng.family == "a3c":
+    if eng.family in ("learner", "a3c"):
         eng.set_params(rng.standard_normal(eng.param_count).astype(np.float32) * 0.05)
         return
     for which in (0, 1):
@@ -36,6 +39,13 @@ def _init(eng, seed=0):
 def _batch(eng, seed):
     rng = np.random.default_rng(seed)
     B = eng.B
+    if eng.family == "learner":
+        T = eng.T
+        mu = rng.random((B, T, A)).astype(np.float32) + 0.1
+        return (rng.integers(0, 256, (B, T) + eng.input_shape, dtype=np.uint8), rng.standard_normal((B, T)),
+                rng.integers(0, A, (B, T)), rng.random((B, T)) < 0.2, mu / mu.sum(-1, keepdims=True),
+                rng.integers(0, A, (B, T)), rng.standard_normal((B, T, eng.L)).astype(np.float32) * 0.1,
+                rng.standard_normal((B, T, eng.L)).astype(np.float32) * 0.1)
     if eng.family == "r2d2":
         S = eng.S
         return (rng.integers(0, 256, (B, S) + eng.input_shape, dtype=np.uint8), rng.integers(0, A, (B, S)),
@@ -60,9 +70,12 @@ def _scalars(out):
 
 
 def _state(eng):
-    s = dict(grads=eng.get_grads(), **{"opt_" + k: v for k, v in eng.get_opt_state().items()})
+    opt = eng.get_opt_state()
+    if eng.family == "learner":
+        opt = dict(ms=opt[0], step=opt[1])
+    s = dict(grads=eng.get_grads(), **{"opt_" + k: v for k, v in opt.items()})
     s["taps"] = eng.taps()
-    if eng.family == "a3c":
+    if eng.family in ("learner", "a3c"):
         s["params"] = eng.get_params()
     else:
         s["params"], s["target"] = eng.get_params(0), eng.get_params(1)
@@ -114,20 +127,30 @@ def test_graph_and_eager_steps_match_bitwise(native, family):
     _assert_same(s1, s2)
 
 
+def _apply(native, eng):
+    if eng.family == "learner":       # no grad_scale: the IMPALA losses are batch sums
+        native.check(eng._fn("apply")(eng._h))
+    else:
+        native.check(eng._fn("apply")(eng._h, C.c_float(1.0)))
+
+
+@pytest.mark.parametrize("use_cuda_graph", [False, True])
 @pytest.mark.parametrize("family", FAMILIES)
-def test_forward_backward_then_apply_matches_step(native, family):
-    ref = _learner(family, False)
-    eng = _learner(family, False)
+def test_forward_backward_then_apply_matches_step(native, family, use_cuda_graph):
+    ref = _learner(family, use_cuda_graph)
+    eng = _learner(family, use_cuda_graph)
     try:
         for e in (ref, eng):
             _init(e)
-            e.stage(0, *_batch(e, 3))
-        want = _scalars(ref.step(0))
-        native.check(eng._fn("forward_backward")(eng._h, 0))
-        native.check(eng._fn("apply")(eng._h, C.c_float(1.0)))
-        got = _scalars(eng.wait())
-        _assert_same(want, got)
-        _assert_same(_state(ref), _state(eng))
+        for i in range(3):            # a graph replays from the second call on
+            for e in (ref, eng):
+                e.stage(i % 2, *_batch(e, 3 + i))
+            want = _scalars(ref.step(i % 2))
+            native.check(eng._fn("forward_backward")(eng._h, i % 2))
+            _apply(native, eng)
+            got = _scalars(eng.wait())
+            _assert_same(want, got, "step%d" % i)
+            _assert_same(_state(ref), _state(eng), "step%d" % i)
     finally:
         ref.close()
         eng.close()
@@ -138,11 +161,17 @@ def test_params_and_opt_state_round_trip(native, family):
     eng = _learner(family, False)
     rng = np.random.default_rng(1)
     try:
-        whiches = [()] if family == "a3c" else [(0,), (1,)]
+        whiches = [()] if family in ("learner", "a3c") else [(0,), (1,)]
         for which in whiches:
             p = rng.standard_normal(eng.param_count).astype(np.float32)
             eng.set_params(p, *which)
             assert eng.get_params(*which).tobytes() == p.tobytes()
+        if family == "learner":       # RMSProp: the ms slots and global_step
+            ms = rng.random(eng.param_count).astype(np.float32)
+            eng.set_opt_state(ms, 12345678901)
+            got, step = eng.get_opt_state()
+            assert got.tobytes() == ms.tobytes() and step == 12345678901
+            return
         m = rng.standard_normal(eng.param_count).astype(np.float32)
         v = rng.random(eng.param_count).astype(np.float32)
         eng.set_opt_state(m, v, 12345678901, 0.25, 0.5)
@@ -162,7 +191,8 @@ def test_misuse_fails_with_the_same_code(native, family):
         return rc
 
     assert code(fn("step_async")(None, 0)) == native.DRL_ERR_INVALID
-    assert "null %s handle" % ("r2d2" if family == "r2d2" else "apex") in native.lib.drl_last_error().decode()
+    name = family if family in ("learner", "r2d2") else "apex"
+    assert "null %s handle" % name in native.lib.drl_last_error().decode()
     eng = _learner(family, False)
     try:
         h, n = eng._h, eng.param_count
@@ -175,14 +205,19 @@ def test_misuse_fails_with_the_same_code(native, family):
             eng.wait()                                                                    # nothing in flight
         assert ei.value.code == native.DRL_ERR_STATE
         assert code(fn("get_grads")(h, native.ptr(buf), n + 1)) == native.DRL_ERR_INVALID  # wrong length
-        assert code(fn("get_opt_state")(h, None, None, n - 1, None, None, None)) == native.DRL_ERR_INVALID
-        if family == "a3c":
+        if family == "learner":
+            assert code(fn("get_opt_state")(h, None, n - 1, None)) == native.DRL_ERR_INVALID
+            assert code(fn("wait_slot")(h, eng.num_slots, None)) == native.DRL_ERR_INVALID
+        else:
+            assert code(fn("get_opt_state")(h, None, None, n - 1, None, None, None)) == native.DRL_ERR_INVALID
+        if family in ("learner", "a3c"):
             assert code(fn("set_params")(h, native.ptr(buf), n + 1)) == native.DRL_ERR_INVALID
         else:
             assert code(fn("set_params")(h, 0, native.ptr(buf), n + 1)) == native.DRL_ERR_INVALID
             assert code(fn("get_params")(h, 2, native.ptr(buf), n)) == native.DRL_ERR_INVALID   # bad which
-        assert code(fn("apply")(h, C.c_float(0.0))) == native.DRL_ERR_INVALID              # grad_scale <= 0
-        assert code(fn("apply")(h, C.c_float(-1.0))) == native.DRL_ERR_INVALID
+        if family != "learner":
+            assert code(fn("apply")(h, C.c_float(0.0))) == native.DRL_ERR_INVALID          # grad_scale <= 0
+            assert code(fn("apply")(h, C.c_float(-1.0))) == native.DRL_ERR_INVALID
         if family == "apex":
             assert code(native.lib.drl_a3c_step_async(h, 0)) == native.DRL_ERR_INVALID
             assert "not an A3C handle" in native.lib.drl_last_error().decode()
