@@ -204,6 +204,9 @@ def _load():
         "drl_r2d2_policy_recorder_act": (C.c_int, [vp] + [vp] * 10),
         "drl_r2d2_policy_recorder_commit": (C.c_int, [vp, vp, vp, i32]),
         "drl_r2d2_policy_recorder_reset": (C.c_int, [vp]),
+        "drl_r2d2_policy_server_create": (C.c_int, [vp, vp, i32, vp, i64, C.POINTER(vp)]),
+        "drl_r2d2_policy_server_destroy": (C.c_int, [vp]),
+        "drl_r2d2_policy_server_serve": (C.c_int, [vp, i32, vp, i32]),
         "drl_apex_create": (C.c_int, [C.POINTER(ApexConfig), C.POINTER(vp)]),
         "drl_apex_destroy": (C.c_int, [vp]),
         "drl_apex_param_count": (C.c_int, [vp, C.POINTER(i64)]),

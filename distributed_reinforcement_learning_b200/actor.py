@@ -128,8 +128,9 @@ class R2D2VectorActor:
       - every environment's ``R2D2TrajectoryBuffer.init()``, then one ``learner.sync_policy(policy)`` (the
         learner-side ``r2d2.Agent``; device to device when it has a CUDA learner);
       - ``seq_len`` batched ``policy.act`` calls with each environment's epsilon: the explore draws of environments
-        0..n-1 from the global ``np.random`` stream, in that order, then ``env.step(action)`` for 0..n-1 with the raw
-        action (the R2D2 actor applies no ``% available_action``);
+        0..n-1 from the global ``np.random`` stream, in that order, then every environment steps under
+        ``utils.r2d2_env_step`` (the rule the worker processes of ``actor_server.R2D2EnvWorkerPool`` follow too), in
+        order 0..n-1, with the raw action (the R2D2 actor applies no ``% available_action``);
       - ``lives`` is only ever set back to 5 by an episode reset, never after a life loss, so every step after the
         first life loss of an episode is stored as reward -1 and done=True (the reference's behaviour, SURVEY.md
         App. D); the score keeps the raw reward;
@@ -206,32 +207,18 @@ class R2D2VectorActor:
             next_pa, next_h, next_c = action.astype(np.int32), out["h"].copy(), out["c"].copy()
             for i, env in enumerate(self.envs):
                 a = int(action[i])
-                self.episode_q_value[i] += float(q_action[i])
-                self.episode_step[i] += 1
-                next_state, reward, done, info = env.step(a)
-                self.score[i] += reward
-                if self.lives[i] != info["ale.lives"]:
-                    r, d = -1, True
-                else:
-                    r, d = reward, False
+                _, r, d, state, episode = utils.r2d2_env_step(env, a, self, i, q_action[i])
                 if rec is None:
                     self.buffers[i].append(state=self.states[i], previous_action=int(self.previous_action[i]),
                                            action=a, reward=r, done=d, initial_h=self.h[i], initial_c=self.c[i])
                 else:   # the rest of the step is on the device already
                     rewards[i, step], dones[i, step] = r, d
-                self.states[i] = next_state
-                if done:
-                    finished.append(dict(task=i, episode=self.episode[i], score=self.score[i],
-                                         epsilon=self.epsilon[i], episode_step=self.episode_step[i],
-                                         avg_q_value=self.episode_q_value[i] / self.episode_step[i]))
-                    self.episode[i] += 1
-                    self.score[i] = 0
-                    self.epsilon[i] = 1.0 / (0.01 * self.episode[i] + 1)
-                    self.states[i] = env.reset()
+                self.states[i] = state
+                if episode is not None:
+                    finished.append(episode)
                     next_pa[i] = 0
                     next_h[i] = 0.0
                     next_c[i] = 0.0
-                    self.lives[i] = START_LIVES
             self.previous_action, self.h, self.c = next_pa, next_h, next_c
         if rec is not None:
             rec.commit(rewards, dones)

@@ -13,6 +13,12 @@ reply record per environment (action, max probability), laid out as ``DRL_SERVER
 server registers the block with CUDA; its kernels read the reports and write the replies directly.  A worker writes
 its environments' reports, then signals on its pipe; the server answers on the same pipe once the replies are written.
 
+R2D2 has the same pair: ``R2D2EnvWorkerPool`` steps R2D2 environments under ``utils.r2d2_env_step`` and draws each
+environment's explore decision from its own stream, and ``R2D2PolicyServer`` acts for them through one
+``NativeR2D2Policy`` (``drl_r2d2_policy_server_*``) into an ``R2D2DeviceFIFOQueue`` that
+``r2d2.DeviceMemory.add_from_queue`` ingests.  Its records (``DRL_R2D2_SERVER_*``) have the IMPALA records' sizes; the
+report carries an explore action instead of a uniform draw, and the reply q_action instead of a max probability.
+
 This module imports neither torch nor the native library at module level: the spawned workers import it.
 """
 import collections
@@ -60,6 +66,38 @@ def exchange_views(buf, num_envs):
     return v
 
 
+# the R2D2 server's records (include/drl_b200.h: DRL_R2D2_SERVER_*): the IMPALA records' sizes and stride
+R2D2_REPORT_FRAME, R2D2_REPORT_EXPLORE, R2D2_REPORT_REWARD, R2D2_REPORT_DONE, R2D2_REPORT_RESET, R2D2_REPORT_BYTES = (
+    0, 28224, 28240, 28256, 28272, 28288)
+R2D2_REPLY_ACTION, R2D2_REPLY_Q_ACTION, R2D2_REPLY_BYTES = 0, 16, 32
+
+
+def r2d2_exchange_views(buf, num_envs, channels=1):
+    """numpy views of the R2D2 records in the exchange block `buf` (a writable buffer of exchange_bytes(num_envs));
+    frames are 84x84x`channels`."""
+    E, shape = num_envs, (84, 84, int(channels))
+
+    def field(offset, dtype, shape=(), strides=()):
+        return np.ndarray((E,) + shape, dtype, buffer=buf, offset=offset, strides=(stride,) + strides)
+
+    stride = R2D2_REPORT_BYTES
+    v = dict(frame=field(R2D2_REPORT_FRAME, np.uint8, shape, (shape[1] * shape[2], shape[2], 1)),
+             explore=field(R2D2_REPORT_EXPLORE, np.int32), reward=field(R2D2_REPORT_REWARD, np.float32),
+             done=field(R2D2_REPORT_DONE, np.uint8), reset=field(R2D2_REPORT_RESET, np.uint8))
+    stride = R2D2_REPLY_BYTES
+    base = E * R2D2_REPORT_BYTES
+    v.update(action=field(base + R2D2_REPLY_ACTION, np.int32), q_action=field(base + R2D2_REPLY_Q_ACTION, np.float32))
+    return v
+
+
+def explore_action(rng, epsilon, num_action):
+    """The epsilon-greedy draw of policy_handle.explore_actions for one environment, from its own RandomState `rng`:
+    ``rng.rand() > epsilon`` keeps the greedy action (-1), otherwise ``rng.choice(num_action)`` is the action."""
+    if rng.rand() > epsilon:
+        return -1
+    return int(rng.choice(num_action))
+
+
 class _Stats:
     """The per-environment episode bookkeeping utils.impala_env_step updates."""
 
@@ -71,24 +109,32 @@ class _Stats:
         self.total_max_prob = [0.0] * k
 
 
-def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, seeds):
-    """A worker process: k environments, each task env_ids[j] with its own RandomState(seeds[j]) for the uniform
-    draws of its actions."""
-    shm = shared_memory.SharedMemory(name=shm_name)
-    v = exchange_views(shm.buf, num_envs)
+class _R2D2Stats:
+    """The per-environment episode bookkeeping utils.r2d2_env_step updates."""
+
+    def __init__(self, k):
+        self.lives = [utils.START_LIVES] * k
+        self.episode = [0] * k
+        self.epsilon = [1.0] * k
+        self.score = [0.0] * k
+        self.episode_step = [0] * k
+        self.episode_q_value = [0.0] * k
+
+
+def _worker_loop(conn, shm, v, env_ids, env_fns, first_report, step):
+    """The loop of every worker process: build the environments, write each one's first report (first_report(j, e,
+    env)), signal ready, then per "go" step each environment (step(j, e, env) -> a finished episode or None) and signal
+    ready with the finished episodes.  A failure is sent as ("error", task, traceback)."""
     task = env_ids[0]
     try:
         envs = []
         for j, fn in enumerate(env_fns):
             task = env_ids[j]
             envs.append(fn())
-        rngs = [np.random.RandomState(s) for s in seeds]
-        stats = _Stats(len(envs))
+        start = first_report(envs)
         for j, e in enumerate(env_ids):
             task = e
-            v["frame"][e] = envs[j].reset()
-            v["uniform"][e] = rngs[j].random_sample()
-            v["reward"][e], v["done"][e], v["reset"][e] = 0.0, 0, 1
+            start(j, e, envs[j])
         info = dict(torch="torch" in sys.modules,
                     native="distributed_reinforcement_learning_b200._native" in sys.modules)
         conn.send(("ready", [], info))
@@ -96,11 +142,7 @@ def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, s
             finished = []
             for j, e in enumerate(env_ids):
                 task = e
-                _, r, d, state, episode = utils.impala_env_step(envs[j], int(v["action"][e]), available_action[j],
-                                                                stats, j, v["max_prob"][e], task=e)
-                v["frame"][e] = state
-                v["reward"][e], v["done"][e], v["reset"][e] = r, d, episode is not None
-                v["uniform"][e] = rngs[j].random_sample()
+                episode = step(j, e, envs[j])
                 if episode is not None:
                     finished.append(episode)
             conn.send(("ready", finished, None))
@@ -113,6 +155,63 @@ def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, s
         del v
         shm.close()
         conn.close()
+
+
+def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, seeds):
+    """An IMPALA worker process: k environments, each task env_ids[j] with its own RandomState(seeds[j]) for the uniform
+    draws of its actions."""
+    shm = shared_memory.SharedMemory(name=shm_name)
+    v = exchange_views(shm.buf, num_envs)
+    rngs, stats = [], None
+
+    def first_report(envs):
+        nonlocal stats
+        rngs.extend(np.random.RandomState(s) for s in seeds)
+        stats = _Stats(len(envs))
+
+        def start(j, e, env):
+            v["frame"][e] = env.reset()
+            v["uniform"][e] = rngs[j].random_sample()
+            v["reward"][e], v["done"][e], v["reset"][e] = 0.0, 0, 1
+        return start
+
+    def step(j, e, env):
+        _, r, d, state, episode = utils.impala_env_step(env, int(v["action"][e]), available_action[j], stats, j,
+                                                        v["max_prob"][e], task=e)
+        v["frame"][e] = state
+        v["reward"][e], v["done"][e], v["reset"][e] = r, d, episode is not None
+        v["uniform"][e] = rngs[j].random_sample()
+        return episode
+
+    _worker_loop(conn, shm, v, env_ids, env_fns, first_report, step)
+
+
+def _r2d2_worker_main(conn, shm_name, num_envs, env_ids, env_fns, num_action, channels, seeds):
+    """An R2D2 worker process: k environments, each task env_ids[j] with its own RandomState(seeds[j]) for its explore
+    decisions and random actions (explore_action)."""
+    shm = shared_memory.SharedMemory(name=shm_name)
+    v = r2d2_exchange_views(shm.buf, num_envs, channels)
+    rngs, stats = [], None
+
+    def first_report(envs):
+        nonlocal stats
+        rngs.extend(np.random.RandomState(s) for s in seeds)
+        stats = _R2D2Stats(len(envs))
+
+        def start(j, e, env):
+            v["frame"][e] = env.reset()
+            v["explore"][e] = explore_action(rngs[j], stats.epsilon[j], num_action)
+            v["reward"][e], v["done"][e], v["reset"][e] = 0.0, 0, 1
+        return start
+
+    def step(j, e, env):
+        _, r, d, state, episode = utils.r2d2_env_step(env, int(v["action"][e]), stats, j, v["q_action"][e], task=e)
+        v["frame"][e] = state
+        v["reward"][e], v["done"][e], v["reset"][e] = r, d, episode is not None
+        v["explore"][e] = explore_action(rngs[j], stats.epsilon[j], num_action)
+        return episode
+
+    _worker_loop(conn, shm, v, env_ids, env_fns, first_report, step)
 
 
 class EnvWorkerPool:
@@ -130,11 +229,23 @@ class EnvWorkerPool:
     def __init__(self, env_fns, available_action, envs_per_worker, seeds, start_timeout=300.0, join_timeout=10.0):
         env_fns, seeds = list(env_fns), [int(s) for s in seeds]
         available_action = [int(a) for a in available_action]
-        n, k = len(env_fns), int(envs_per_worker)
+        self._check(env_fns, envs_per_worker)
+        if len(available_action) != len(env_fns) or len(seeds) != len(env_fns):
+            raise ValueError("available_action and seeds need one entry per environment (%d)" % len(env_fns))
+        self._start(env_fns, envs_per_worker, seeds, exchange_views, _worker_main,
+                    lambda lo, hi: (available_action[lo:hi],), start_timeout, join_timeout)
+
+    @staticmethod
+    def _check(env_fns, envs_per_worker):
+        n = len(env_fns)
         if not 1 <= n <= MAX_ENVS:
             raise ValueError("%d environments, a pool serves 1..%d" % (n, MAX_ENVS))
-        if len(available_action) != n or len(seeds) != n:
-            raise ValueError("available_action and seeds need one entry per environment (%d)" % n)
+
+    def _start(self, env_fns, envs_per_worker, seeds, views, target, worker_args, start_timeout, join_timeout):
+        """Checks envs_per_worker and the factories, makes the exchange block (views(buf, n): its numpy views) and
+        spawns one `target` process per envs_per_worker environments, with the arguments (pipe, block name, n, env ids,
+        env factories, *worker_args(lo, hi), seeds) of environments lo..hi-1; waits for every worker's first report."""
+        n, k = len(env_fns), int(envs_per_worker)
         if k < 1:
             raise ValueError("envs_per_worker must be >= 1 (got %d)" % k)
         for i, fn in enumerate(env_fns):
@@ -149,7 +260,7 @@ class EnvWorkerPool:
         self._pending = set()
         self._servers = []
         self._shm = shared_memory.SharedMemory(create=True, size=self.exchange_bytes)
-        self.views = exchange_views(self._shm.buf, n)
+        self.views = views(self._shm.buf, n)
         self._anchor = C.c_char.from_buffer(self._shm.buf)
         self.address = C.addressof(self._anchor)
         self.worker_info = []
@@ -158,8 +269,8 @@ class EnvWorkerPool:
             for w in range(0, n, k):
                 ids = list(range(w, min(n, w + k)))
                 parent, child = ctx.Pipe()
-                p = ctx.Process(target=_worker_main, name="env-worker-%d" % (w // k),
-                                args=(child, self._shm.name, n, ids, env_fns[w:w + k], available_action[w:w + k],
+                p = ctx.Process(target=target, name="env-worker-%d" % (w // k),
+                                args=(child, self._shm.name, n, ids, env_fns[w:w + k], *worker_args(w, w + k),
                                       seeds[w:w + k]), daemon=True)
                 p.start()
                 child.close()
@@ -264,25 +375,45 @@ class EnvWorkerPool:
             pass
 
 
-class PolicyServer:
-    """Serves the environments of an ``EnvWorkerPool`` from one ``NativePolicy`` into one ``DeviceFIFOQueue``.
+class R2D2EnvWorkerPool(EnvWorkerPool):
+    """``len(env_fns)`` R2D2 environments (1..256) in spawned worker processes of ``envs_per_worker`` environments
+    each, for an ``R2D2PolicyServer``.
 
-    ``serve_once`` waits for at least one worker's reports, takes every report that is ready and serves them in
-    chunks of ``policy.max_batch`` environments (no batching knob: batches grow with load), then answers the workers.
-    Before a serve it syncs the policy from ``learner`` (an ``impala.Agent``) whenever the learner has trained since
-    the last sync, so parameters can change inside an unroll; each trajectory records the policy that acted, which is
-    what V-trace corrects for.  While the queue is full a serve blocks: that is the workers' backpressure.
-    ``batch_sizes`` counts the served batches by size.  Single-replica, like ``train_from_queue``.  Closing the pool
-    closes its server first, so the exchange block is never freed while CUDA has it registered."""
+    Environment i is task i: ``env_fns[i]()`` builds it in its worker (its frames are 84x84x``channels``), it steps
+    under ``utils.r2d2_env_step`` with the raw action, and its explore decisions and random actions in [0,
+    ``num_action``) come from ``np.random.RandomState(seeds[i])`` by the rule of ``policy_handle.explore_actions``
+    (``explore_action``), so they do not depend on batching or on how environments are grouped into workers.  The
+    reports and replies are the R2D2 records (``r2d2_exchange_views``); everything else -- the pipes, ``wait_ready``,
+    ``reply``, the failure reports and ``close()`` -- is ``EnvWorkerPool``'s."""
 
-    def __init__(self, policy, queue, pool, learner=None):
+    def __init__(self, env_fns, num_action, envs_per_worker, seeds, channels=1, start_timeout=300.0,
+                 join_timeout=10.0):
+        env_fns, seeds = list(env_fns), [int(s) for s in seeds]
+        num_action, channels = int(num_action), int(channels)
+        self._check(env_fns, envs_per_worker)
+        if len(seeds) != len(env_fns):
+            raise ValueError("seeds need one entry per environment (%d)" % len(env_fns))
+        if num_action < 2:
+            raise ValueError("num_action must be >= 2 (got %d)" % num_action)
+        if channels not in (1, 4):
+            raise ValueError("channels must be 1 or 4 (got %d)" % channels)
+        self.num_action, self.channels = num_action, channels
+        self._start(env_fns, envs_per_worker, seeds, lambda buf, n: r2d2_exchange_views(buf, n, channels),
+                    _r2d2_worker_main, lambda lo, hi: (num_action, channels), start_timeout, join_timeout)
+
+
+class _ServerBase:
+    """What PolicyServer and R2D2PolicyServer share: the binding to a pool, the serve lock, the C handle's lifetime,
+    the policy sync before a serve, and the serve loop.  A family sets `_prefix` (its ``drl_<prefix>_*`` entry
+    points) and `_what` (its name in messages) and implements ``_learner_step``."""
+    _prefix = None
+    _what = None
+
+    def _bind_and_create(self, policy, queue, pool, learner):
         from . import _native as N
         from . import dp
-        from .distributed_queue.buffer_queue import DeviceFIFOQueue
-        if not isinstance(queue, DeviceFIFOQueue):
-            raise TypeError("PolicyServer: queue must be a DeviceFIFOQueue, got %s" % type(queue).__name__)
         if dp.distributed():
-            raise RuntimeError("PolicyServer is single-replica: the queue lives on one device")
+            raise RuntimeError("%s is single-replica: the queue lives on one device" % type(self).__name__)
         self._N = N
         self.policy, self.queue, self.pool, self.learner = policy, queue, pool, learner
         self.batch_sizes = collections.Counter()
@@ -295,17 +426,20 @@ class PolicyServer:
         if bind is not None:
             bind(self)
         try:
-            N.check(N.lib.drl_policy_server_create(policy._h, queue._q, pool.num_envs, C.c_void_p(pool.address),
-                                                   pool.exchange_bytes, C.byref(self._s)))
+            N.check(self._fn("create")(policy._h, queue._q, pool.num_envs, C.c_void_p(pool.address),
+                                       pool.exchange_bytes, C.byref(self._s)))
         except BaseException:
             self.close()
             raise
+
+    def _fn(self, name):
+        return getattr(self._N.lib, "drl_%s_%s" % (self._prefix, name))
 
     def close(self):
         """Destroys the server (unregistering the exchange block); waits for a serve in progress."""
         with self._lock:
             if self._s.value:
-                self._N.lib.drl_policy_server_destroy(self._s)
+                self._fn("destroy")(self._s)
                 self._s = C.c_void_p()
         unbind = getattr(getattr(self, "pool", None), "_unbind", None)
         if unbind is not None:
@@ -317,30 +451,32 @@ class PolicyServer:
         except Exception:
             pass
 
+    def _learner_step(self):
+        raise NotImplementedError
+
     def _sync(self):
         if self.learner is None:
             return
-        step = self.learner.num_env_frames
+        step = self._learner_step()
         if step != self._synced_step:
             self.learner.sync_policy(self.policy)
             self._synced_step = step
             self.syncs += 1
 
     def serve(self, env_ids, timeout_ms=-1):
-        """One ``drl_policy_server_serve`` of these environments (at most max_batch, distinct)."""
+        """One ``drl_<prefix>_serve`` of these environments (at most max_batch, distinct)."""
         ids = np.ascontiguousarray(env_ids, np.int32)
         N = self._N
         with self._lock:
             if not self._s.value:
-                raise ValueError("the policy server is closed")
-            N.check(N.lib.drl_policy_server_serve(self._s, int(ids.size), N.ptr(ids), int(timeout_ms)))
+                raise ValueError("the %s is closed" % self._what)
+            N.check(self._fn("serve")(self._s, int(ids.size), N.ptr(ids), int(timeout_ms)))
         self.batch_sizes[int(ids.size)] += 1
 
     def serve_once(self, wait=None, timeout_ms=-1):
         """Serves every report that is ready, waiting up to `wait` s (None: forever) for the first.  A serve blocked
         by a full queue for `timeout_ms` (>= 0) raises ``TimeoutError_``; the reports not yet served then wait for the
-        next call.  -> the episodes that finished, as dicts of task, episode, score, episode_step and prob (the values
-        train_impala.py:170-172 logs)."""
+        next call.  -> the episodes that finished."""
         if not self._todo:
             self._workers, finished = self.pool.wait_ready(wait)
             self._finished += finished
@@ -367,3 +503,61 @@ class PolicyServer:
                 continue
             if episodes and on_episodes is not None:
                 on_episodes(episodes)
+
+
+class PolicyServer(_ServerBase):
+    """Serves the environments of an ``EnvWorkerPool`` from one ``NativePolicy`` into one ``DeviceFIFOQueue``.
+
+    ``serve_once`` waits for at least one worker's reports, takes every report that is ready and serves them in
+    chunks of ``policy.max_batch`` environments (no batching knob: batches grow with load), then answers the workers.
+    Before a serve it syncs the policy from ``learner`` (an ``impala.Agent``) whenever the learner has trained since
+    the last sync, so parameters can change inside an unroll; each trajectory records the policy that acted, which is
+    what V-trace corrects for.  While the queue is full a serve blocks: that is the workers' backpressure.
+    ``batch_sizes`` counts the served batches by size.  Single-replica, like ``train_from_queue``.  Closing the pool
+    closes its server first, so the exchange block is never freed while CUDA has it registered.  ``serve_once``
+    returns the finished episodes as dicts of task, episode, score, episode_step and prob (the values
+    train_impala.py:170-172 logs)."""
+    _prefix = "policy_server"
+    _what = "policy server"
+
+    def __init__(self, policy, queue, pool, learner=None):
+        from .distributed_queue.buffer_queue import DeviceFIFOQueue
+        if not isinstance(queue, DeviceFIFOQueue):
+            raise TypeError("PolicyServer: queue must be a DeviceFIFOQueue, got %s" % type(queue).__name__)
+        self._bind_and_create(policy, queue, pool, learner)
+
+    def _learner_step(self):
+        return self.learner.num_env_frames
+
+
+class R2D2PolicyServer(_ServerBase):
+    """Serves the environments of an ``R2D2EnvWorkerPool`` from one ``NativeR2D2Policy`` into one
+    ``R2D2DeviceFIFOQueue``, which ``r2d2.DeviceMemory.add_from_queue`` ingests.
+
+    ``serve``, ``serve_once``, ``run`` and ``close`` are ``PolicyServer``'s; the explore decisions come with the
+    reports.  Before a serve it syncs the policy from ``learner`` (an ``r2d2.Agent``) whenever the learner has trained
+    (``train_calls``) since the last sync.  The reference's actor runs ``parameter_sync`` once per sequence; here the
+    sync follows the learner, so one sequence may be recorded under several parameter versions.  R2D2 learns
+    off-policy from replay, and the stored (h, c) of a sequence's step 0 is burnt in again by the learner, so this
+    changes which parameters acted, not what the learner computes from a sequence.  While the queue is full a serve
+    blocks.  Single-replica, like the device replay memory.  Closing the pool closes its server first.  ``serve_once``
+    returns the finished episodes as dicts of task, episode, score, epsilon, episode_step and avg_q_value (the values
+    train_r2d2.py:227-230 logs)."""
+    _prefix = "r2d2_policy_server"
+    _what = "r2d2 policy server"
+
+    def __init__(self, policy, queue, pool, learner=None):
+        from .distributed_queue.buffer_queue import R2D2DeviceFIFOQueue
+        from .r2d2_policy import NativeR2D2Policy
+        if not isinstance(policy, NativeR2D2Policy):
+            raise TypeError("R2D2PolicyServer: policy must be a NativeR2D2Policy, got %s" % type(policy).__name__)
+        if not isinstance(queue, R2D2DeviceFIFOQueue):
+            raise TypeError("R2D2PolicyServer: queue must be an R2D2DeviceFIFOQueue, got %s" % type(queue).__name__)
+        channels = getattr(pool, "channels", None)
+        if channels is not None and channels != queue.input_shape[2]:
+            raise ValueError("R2D2PolicyServer: the pool's environments give 84x84x%d frames, the queue stores 84x84x%d"
+                             % (channels, queue.input_shape[2]))
+        self._bind_and_create(policy, queue, pool, learner)
+
+    def _learner_step(self):
+        return self.learner.train_calls

@@ -7,6 +7,8 @@ the learner branch of ``train_r2d2.py:87-165`` runs on it unchanged, with the TF
   Agent.parameter_sync agent/r2d2.py:161-162 ; Agent.main_to_target :164-165 ; Agent.set_session :167-169
   Agent.get_action     agent/r2d2.py:171-191 -> (action, q_value[action], h', c')
   Agent.sync_policy    (new) parameter_sync into a NativeR2D2Policy (r2d2_policy.py), device to device from the learner
+  Agent.train_calls    (new) read-only count of the training steps taken (train and train_from_memory); an
+                       actor_server.R2D2PolicyServer syncs its policy whenever it has changed
   Agent.device_memory  (new) a DeviceMemory: the replay memory of train_r2d2.py:92-93 on the GPU (r2d2_replay.py);
                        DeviceMemory.add_from_queue ingests a batch of an R2D2DeviceFIFOQueue without a host copy
   Agent.train_from_memory (new) Memory.sample + the minibatch lists + train + Memory.update (train_r2d2.py:122-162)
@@ -50,6 +52,7 @@ class Agent:
         self._engine = None
         self._slot = 0
         self._last = {}
+        self._train_calls = 0
         self._lock = threading.RLock()   # actor threads sync from / act on this agent while the learner thread trains
         _AGENTS[model_name] = self
 
@@ -111,6 +114,7 @@ class Agent:
                   np.stack(reward), np.stack(done), weight)
         out, td = eng.step(slot)
         self._last = out
+        self._train_calls += 1
         return out["loss"], td
 
     def device_memory(self, capacity):
@@ -138,6 +142,7 @@ class Agent:
         memory.replay.step_async(eng, slot, u01)
         out, td = eng.wait()
         self._last = out
+        self._train_calls += 1
         return out["loss"], td
 
     def _snapshot_params(self):
@@ -207,6 +212,11 @@ class Agent:
 
     def target_q_value_test(self, state, h, c, done, previous_action):
         return self._unroll_q("target_q", state, h, c, done, previous_action)
+
+    @property
+    def train_calls(self):
+        """Training steps taken so far: calls of train and train_from_memory that returned."""
+        return self._train_calls
 
     value_loss = property(lambda self: self._last.get("loss"))
     grad_norm = property(lambda self: self._last.get("grad_norm"))

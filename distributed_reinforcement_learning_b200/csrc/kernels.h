@@ -270,6 +270,31 @@ PolicyInRows policy_input_rows(drl_policy* h, int n);
 // reading the rows of policy_input_rows(h, n) and writing `out`; the caller holds the engine's lock
 int policy_enqueue_forward(drl_policy* h, int n, const PolicyOutRows& out);
 
+// ---- r2d2_policy.cu: the R2D2 policy engine's act on device-resident inputs (r2d2_policy_server.cu) ---------------
+PolicyCore* r2d2_policy_core_of(drl_r2d2_policy* h);
+int r2d2_policy_channels(const drl_r2d2_policy* h);   // C of the engine's 84x84xC frames
+// the rows of an n-row act inside the engine's device input block
+struct R2PolicyInRows {
+  uint8_t* frames;   // [n][84*84*C]
+  int32_t* pa;       // [n]
+  float* h0;         // [n][64]
+  float* c0;         // [n][64]
+  int32_t* explore;  // [n]: -1 greedy, otherwise the action (in [0, A): the head indexes q with it)
+};
+// where the act's head writes: q [n][A], h1 / c1 [n][64], action [n], q_action [n]
+struct R2PolicyOutRows {
+  float* q;
+  float* h1;
+  float* c1;
+  int32_t* action;
+  float* q_action;
+};
+R2PolicyInRows r2d2_policy_input_rows(drl_r2d2_policy* h, int n);
+// the engine's act kernels of n rows (drl_r2d2_policy_act without the upload of its input block: conv stack,
+// policy_lstm_fwd and r2d2_policy_head_kernel) on the engine's stream, reading the rows of r2d2_policy_input_rows(h, n)
+// and writing `out`; the caller holds the engine's lock
+int r2d2_policy_enqueue_forward(drl_r2d2_policy* h, int n, const R2PolicyOutRows& out);
+
 // ---- learner.cu: parameter snapshot for the policy engine (drl_policy_sync_from_learner) ---------------------------
 // learner_params_snapshot (learner_core.cuh) of an IMPALA learner whose network has num_action actions:
 // DRL_ERR_INVALID for a learner with another num_action, DRL_ERR_STATE for a learner in the failed state.

@@ -8,42 +8,22 @@
 //   server_gather_kernel       report -> the engine's device input rows (frame, uniform; h, c, previous action from
 //                              the table, or 0 on reset); the previous step's reward and done -> staging at t - 1
 //   queue_commit_rows_kernel   the staged trajectories that step T-1 completed -> their reserved queue positions
+//                              (server_core.cu)
 //   the engine's act kernels   (policy_enqueue_forward), outputs into device memory
 //   server_scatter_kernel      step t of each row into the staging; h, c, previous action, t into the table; action
 //                              and max probability into the row's reply record
 // The commit's waits on the target slots' release events precede these on the stream, its commit events follow them,
 // so one graph per n holds all four; a serve in which no row completes a trajectory replays a second graph of n
-// without the commit kernel.
-#include <string.h>
-#include <unistd.h>
-
-#include <algorithm>
-#include <mutex>
-#include <string>
-#include <vector>
-
-#include "policy_core.cuh"
-#include "traj_queue.cuh"
+// without the commit kernel.  The binding, the word block, the reservation and the graphs are the server core's
+// (server_core.cuh).
+#include "server_core.cuh"
 
 namespace drl {
 namespace {
 
-constexpr int kMaxEnvs = 256;
-constexpr int kThreads = 256;
-constexpr int kCommitSplit = 16;   // CTAs per committed trajectory (one trajectory is 0.6 MB at T = 20)
+constexpr int kThreads = kServerThreads;
 
 static_assert(DRL_SERVER_REPORT_FRAME == 0 && DRL_SERVER_REPORT_UNIFORM >= Geo::FRAME, "report layout");
-static_assert(DRL_SERVER_REPORT_BYTES % 16 == 0 && DRL_SERVER_REPLY_BYTES % 16 == 0, "16-byte records");
-
-// the device word block of one serve (int32): env ids [max_batch], completed-row count, then per completed row its
-// environment, target slot and row
-struct Words {
-  int max_batch;
-  size_t env() const { return 0; }
-  size_t m() const { return (size_t)max_batch; }
-  size_t commits() const { return (size_t)max_batch + 1; }
-  size_t count() const { return (size_t)max_batch + 1 + 3 * (size_t)max_batch; }
-};
 
 struct Table {
   float* h;          // [num_envs][256]
@@ -52,10 +32,9 @@ struct Table {
   int32_t* t;        // [num_envs]: the step the next act records, -1 before the first
 };
 
-// staging / queue field pointers, in TrajField order
+// staging field pointers, in TrajField order
 struct Fields {
   uint8_t* p[kTrajFields];
-  size_t sz[kTrajFields];
 };
 
 // ---- server_gather_kernel ---------------------------------------------------------------------------------------
@@ -105,39 +84,6 @@ __global__ void __launch_bounds__(kThreads) server_gather_kernel(const GatherArg
       const uint4 d = *reinterpret_cast<const uint4*>(rep + DRL_SERVER_REPORT_DONE);
       a.st_reward[prev] = __uint_as_float(r.x);
       a.st_done[prev] = (uint8_t)(d.x & 0xffu);
-    }
-  }
-}
-
-// ---- queue_commit_rows_kernel -----------------------------------------------------------------------------------
-// grid (n, kCommitSplit): CTA (j, k) copies part k of every field of completed row j (j < *m; the rest exit) from the
-// staging of its environment to its reserved queue position.  16-byte copies where the field allows.
-struct CommitArgs {
-  const int32_t* m;          // completed-row count
-  const int32_t* rows;       // [m][3]: environment, slot, row
-  Fields src;                // staging field bases (record e at + e * sz)
-  uint8_t* dst_base;         // queue slots
-  size_t dst_off[kTrajFields];
-  size_t slot_bytes;
-};
-
-__global__ void __launch_bounds__(kThreads) queue_commit_rows_kernel(const CommitArgs a) {
-  kernel_prologue();
-  const int j = blockIdx.x;
-  if (j >= *a.m) return;
-  const int e = a.rows[3 * j], slot = a.rows[3 * j + 1], qrow = a.rows[3 * j + 2];
-  const int nthreads = kThreads * kCommitSplit, gtid = blockIdx.y * kThreads + threadIdx.x;
-#pragma unroll 1
-  for (int f = 0; f < kTrajFields; ++f) {
-    const size_t sz = a.src.sz[f];
-    const uint8_t* s = a.src.p[f] + (size_t)e * sz;
-    uint8_t* d = a.dst_base + (size_t)slot * a.slot_bytes + a.dst_off[f] + (size_t)qrow * sz;
-    if (((reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(d) | sz) & 15) == 0) {
-      const uint4* s4 = reinterpret_cast<const uint4*>(s);
-      uint4* d4 = reinterpret_cast<uint4*>(d);
-      for (size_t i = gtid; i < sz / 16; i += nthreads) d4[i] = s4[i];
-    } else {
-      for (size_t i = gtid; i < sz; i += nthreads) d[i] = s[i];
     }
   }
 }
@@ -194,64 +140,41 @@ __global__ void __launch_bounds__(kThreads) server_scatter_kernel(const ScatterA
   if (tid == 0) a.tab.t[e] = (t + 1) % a.T;
 }
 
-int64_t exchange_bytes(int num_envs) {
-  return (int64_t)align_up((size_t)num_envs * (DRL_SERVER_REPORT_BYTES + DRL_SERVER_REPLY_BYTES), 4096);
-}
-
 }  // namespace
 }  // namespace drl
 
 using namespace drl;
 
-struct drl_policy_server {
+struct drl_policy_server : ServerCore {
   drl_policy* policy = nullptr;
-  PolicyCore* engine = nullptr;
-  drl_traj_queue* q = nullptr;
-  int num_envs = 0, T = 0;
-  std::mutex mu;                      // one serve at a time
-  uint8_t* host_block = nullptr;      // the caller's exchange block, registered while the server lives
-  uint8_t* d_block = nullptr;         // its device alias
   Table tab{};
-  Fields st{};                        // staging [num_envs] trajectories
   float* out_policy = nullptr;        // the act's outputs [max_batch][A] / [max_batch][256] / [max_batch]
   float *out_h = nullptr, *out_c = nullptr;
   int32_t* out_action = nullptr;
-  Words words{};
-  int32_t* d_words = nullptr;
-  int32_t* h_words = nullptr;         // pinned
-  std::vector<int> t;                 // host mirror of the table's t
-  std::vector<cudaGraphExec_t> graphs[2];   // per n: [0] without the commit kernel (no row completes), [1] with it
-  std::vector<void*> allocs;
 };
 
 namespace {
 
 // the serve of n rows; `commit`: with queue_commit_rows_kernel (some row completes a trajectory)
-int enqueue_serve(drl_policy_server* s, int n, bool commit) {
+int enqueue_serve(ServerCore* core, int n, bool commit) {
+  drl_policy_server* s = static_cast<drl_policy_server*>(core);
   PolicyCore* h = s->engine;
   cudaStream_t st = h->stream;
-  DRL_CUDA_CHECK(cudaMemcpyAsync(s->d_words, s->h_words, s->words.count() * 4, cudaMemcpyHostToDevice, st));
+  DRL_TRY(server_upload_words(s));
   const PolicyInRows in = policy_input_rows(s->policy, n);
   const int32_t* env = s->d_words + s->words.env();
+  Fields fields;
+  for (int f = 0; f < kTrajFields; ++f) fields.p[f] = s->st[f];
   GatherArgs g;
   g.reports = s->d_block;
   g.env = env;
   g.tab = s->tab;
   g.in = in;
-  g.st_reward = reinterpret_cast<float*>(s->st.p[kTrajReward]);
-  g.st_done = s->st.p[kTrajDone];
+  g.st_reward = reinterpret_cast<float*>(s->st[kTrajReward]);
+  g.st_done = s->st[kTrajDone];
   g.T = s->T;
   DRL_CUDA_CHECK((launch_k(server_gather_kernel, n, kThreads, 0, st, g)));
-  if (commit) {
-    CommitArgs c;
-    c.m = s->d_words + s->words.m();
-    c.rows = s->d_words + s->words.commits();
-    c.src = s->st;
-    c.dst_base = s->q->base;
-    for (int f = 0; f < kTrajFields; ++f) c.dst_off[f] = s->q->off[f];
-    c.slot_bytes = s->q->slot_bytes;
-    DRL_CUDA_CHECK((launch_k(queue_commit_rows_kernel, dim3(n, kCommitSplit), kThreads, 0, st, c)));
-  }
+  if (commit) DRL_TRY(server_enqueue_commit(s, n));
   const PolicyOutRows out{s->out_policy, s->out_h, s->out_c, s->out_action};
   DRL_TRY(policy_enqueue_forward(s->policy, n, out));
   ScatterArgs a;
@@ -259,7 +182,7 @@ int enqueue_serve(drl_policy_server* s, int n, bool commit) {
   a.in = in;
   a.out = out;
   a.tab = s->tab;
-  a.st = s->st;
+  a.st = fields;
   a.replies = s->d_block + (size_t)s->num_envs * DRL_SERVER_REPORT_BYTES;
   a.T = s->T;
   a.A = h->A;
@@ -267,45 +190,18 @@ int enqueue_serve(drl_policy_server* s, int n, bool commit) {
   return DRL_OK;
 }
 
-void release(drl_policy_server* s) {
-  if (s->engine) {
-    cudaSetDevice(s->engine->device);
-    if (s->engine->stream) cudaStreamSynchronize(s->engine->stream);
-  }
-  for (auto& v : s->graphs)
-    for (auto g : v) if (g) cudaGraphExecDestroy(g);
-  for (void* p : s->allocs) cudaFree(p);
-  if (s->h_words) cudaFreeHost(s->h_words);
-  if (s->host_block) cudaHostUnregister(s->host_block);
-  cudaGetLastError();
-}
-
 int server_init(drl_policy_server* s, void* exchange) {
+  DRL_TRY(server_core_init(s, exchange));
   PolicyCore* h = s->engine;
-  DRL_CUDA_CHECK(cudaSetDevice(h->device));
   const size_t E = s->num_envs, MB = h->max_batch;
   DRL_TRY(dev_alloc(s, &s->tab.h, E * Geo::L));
   DRL_TRY(dev_alloc(s, &s->tab.c, E * Geo::L));
   DRL_TRY(dev_alloc(s, &s->tab.pa, E));
   DRL_TRY(dev_alloc(s, &s->tab.t, E, 0xff));   // -1: no step yet
-  for (int f = 0; f < kTrajFields; ++f) {
-    s->st.sz[f] = s->q->sz[f];
-    DRL_TRY(dev_alloc(s, &s->st.p[f], E * s->q->sz[f]));
-  }
   DRL_TRY(dev_alloc(s, &s->out_policy, MB * h->A));
   DRL_TRY(dev_alloc(s, &s->out_h, MB * Geo::L));
   DRL_TRY(dev_alloc(s, &s->out_c, MB * Geo::L));
   DRL_TRY(dev_alloc(s, &s->out_action, MB));
-  s->words.max_batch = (int)MB;
-  DRL_TRY(dev_alloc(s, &s->d_words, s->words.count()));
-  DRL_CUDA_CHECK(cudaHostAlloc((void**)&s->h_words, s->words.count() * 4, cudaHostAllocDefault));
-  memset(s->h_words, 0, s->words.count() * 4);
-  DRL_CUDA_CHECK(cudaHostRegister(exchange, (size_t)exchange_bytes(s->num_envs),
-                                  cudaHostRegisterMapped | cudaHostRegisterPortable));
-  s->host_block = static_cast<uint8_t*>(exchange);
-  DRL_CUDA_CHECK(cudaHostGetDevicePointer((void**)&s->d_block, exchange, 0));
-  s->t.assign(E, -1);
-  for (auto& v : s->graphs) v.assign(MB + 1, nullptr);
   DRL_CUDA_CHECK(cudaDeviceSynchronize());
   return DRL_OK;
 }
@@ -314,16 +210,6 @@ int server_init(drl_policy_server* s, void* exchange) {
 
 extern "C" {
 
-int drl_policy_server_exchange_bytes(int32_t num_envs, int64_t* bytes) {
-  if (!bytes) { set_error("null argument"); return DRL_ERR_INVALID; }
-  if (num_envs < 1 || num_envs > kMaxEnvs) {
-    set_error("policy server: num_envs must be in [1, %d] (got %d)", kMaxEnvs, num_envs);
-    return DRL_ERR_INVALID;
-  }
-  *bytes = exchange_bytes(num_envs);
-  return DRL_OK;
-}
-
 int drl_policy_server_create(drl_policy* p, drl_traj_queue* q, int32_t num_envs, void* exchange,
                              int64_t exchange_size, drl_policy_server** out) {
   if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
@@ -331,18 +217,7 @@ int drl_policy_server_create(drl_policy* p, drl_traj_queue* q, int32_t num_envs,
   if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
   if (!p) { set_error("null policy handle"); return DRL_ERR_INVALID; }
   if (!q) { set_error("null trajectory queue handle"); return DRL_ERR_INVALID; }
-  int64_t need = 0;
-  DRL_TRY(drl_policy_server_exchange_bytes(num_envs, &need));
-  const long page = sysconf(_SC_PAGESIZE);
-  if (!exchange || reinterpret_cast<uintptr_t>(exchange) % (uintptr_t)page != 0) {
-    set_error("policy server: the exchange block must be page-aligned (%ld bytes)", page);
-    return DRL_ERR_INVALID;
-  }
-  if (exchange_size < need) {
-    set_error("policy server: the exchange block has %lld bytes, %d environments need %lld", (long long)exchange_size,
-              num_envs, (long long)need);
-    return DRL_ERR_INVALID;
-  }
+  DRL_TRY(server_check_block("policy server", num_envs, exchange, exchange_size));
   PolicyCore* h = policy_core_of(p);
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   if (q->device != h->device) {
@@ -355,23 +230,21 @@ int drl_policy_server_create(drl_policy* p, drl_traj_queue* q, int32_t num_envs,
               q->W, q->C, q->L, Geo::IH, Geo::IW, Geo::IC, Geo::L);
     return DRL_ERR_INVALID;
   }
-  const int most = std::min(num_envs, h->max_batch);
-  if (most > traj_queue_max_rows(q)) {
-    set_error("policy server: one serve may commit %d trajectories, the queue takes at most %d at once", most,
-              traj_queue_max_rows(q));
-    return DRL_ERR_INVALID;
-  }
   NvtxRange nv("drl:policy_server_create");
   drl_policy_server* s = new drl_policy_server();
+  s->name = "policy server";
+  s->serve_range = "drl:policy_server_serve";
   s->policy = p;
   s->engine = h;
   s->q = q;
   s->num_envs = num_envs;
   s->T = q->T;
-  const int rc = server_init(s, exchange);
+  s->enqueue_serve = enqueue_serve;
+  int rc = server_check_queue_rows(s, "trajectories");
+  if (rc == DRL_OK) rc = server_init(s, exchange);
   if (rc != DRL_OK) {
     const std::string keep = get_error();
-    release(s);
+    server_core_release(s);
     delete s;
     set_error("%s", keep.c_str());
     return rc;
@@ -380,87 +253,11 @@ int drl_policy_server_create(drl_policy* p, drl_traj_queue* q, int32_t num_envs,
   return DRL_OK;
 }
 
-int drl_policy_server_destroy(drl_policy_server* s) {
-  if (!s) return DRL_OK;
-  {
-    std::lock_guard<std::mutex> lk(s->mu);
-    std::lock_guard<std::recursive_mutex> lk2(s->engine->mu);
-    release(s);
-  }
-  delete s;
-  return DRL_OK;
-}
+int drl_policy_server_destroy(drl_policy_server* s) { return server_destroy(s); }
 
 int drl_policy_server_serve(drl_policy_server* s, int32_t n, const int32_t* env_ids, int32_t timeout_ms) {
   if (!s) { set_error("null policy server handle"); return DRL_ERR_INVALID; }
-  if (!env_ids) { set_error("policy server serve: null env_ids"); return DRL_ERR_INVALID; }
-  PolicyCore* h = s->engine;
-  if (n < 1 || n > h->max_batch) {
-    set_error("policy server serve: n must be in [1, %d] (the engine's max_batch; got %d)", h->max_batch, n);
-    return DRL_ERR_INVALID;
-  }
-  std::lock_guard<std::mutex> slk(s->mu);
-  std::vector<char> seen(s->num_envs, 0);
-  std::vector<int> done_rows;   // rows whose serve completes their staged trajectory
-  for (int r = 0; r < n; ++r) {
-    const int e = env_ids[r];
-    if (e < 0 || e >= s->num_envs) {
-      set_error("policy server serve: env_ids[%d] = %d is outside [0, %d)", r, e, s->num_envs);
-      return DRL_ERR_INVALID;
-    }
-    if (seen[e]) { set_error("policy server serve: environment %d is listed twice", e); return DRL_ERR_INVALID; }
-    seen[e] = 1;
-    if (s->t[e] == 0) done_rows.push_back(r);
-  }
-  const int m = (int)done_rows.size();
-  // reserve without the engine's lock: a learner thread may sync this engine while the serve waits for space
-  std::vector<TrajSegment> segs;
-  if (m > 0) DRL_TRY(traj_queue_reserve(s->q, m, timeout_ms, &segs));
-  std::lock_guard<std::recursive_mutex> lk(h->mu);
-  NvtxRange nv("drl:policy_server_serve");
-  int32_t* w = s->h_words;   // free: the previous serve waited for the stream
-  memcpy(w + s->words.env(), env_ids, (size_t)n * 4);
-  w[s->words.m()] = m;
-  int32_t* cw = w + s->words.commits();
-  for (const TrajSegment& g : segs)
-    for (int i = 0; i < g.rows; ++i) {
-      const int j = g.src0 + i;
-      cw[3 * j] = env_ids[done_rows[j]];
-      cw[3 * j + 1] = g.slot;
-      cw[3 * j + 2] = g.row0 + i;
-    }
-  cudaStream_t st = h->stream;
-  const int rc = [&]() -> int {
-    DRL_CUDA_CHECK(cudaSetDevice(h->device));
-    for (const TrajSegment& g : segs) DRL_CUDA_CHECK(cudaStreamWaitEvent(st, g.ev_release, 0));
-    const bool commit = m > 0;
-    if (h->use_cuda_graph) {
-      cudaGraphExec_t& graph = s->graphs[commit][n];
-      if (!graph) {
-        // this serve runs eagerly (the launchers set their attributes and tensor maps outside capture); the capture
-        // only records, so the state table advances once
-        DRL_TRY(enqueue_serve(s, n, commit));
-        DRL_TRY(capture_graph(st, [&] { return enqueue_serve(s, n, commit); }, &graph));
-      } else {
-        DRL_CUDA_CHECK(cudaGraphLaunch(graph, st));
-      }
-    } else {
-      DRL_TRY(enqueue_serve(s, n, commit));
-    }
-    for (const TrajSegment& g : segs) DRL_CUDA_CHECK(cudaEventRecord(g.ev_commit, st));
-    return DRL_OK;
-  }();
-  if (rc != DRL_OK) {
-    if (m > 0) traj_queue_fail(s->q, get_error());
-    return rc;
-  }
-  if (m > 0) traj_queue_commit(s->q, segs);
-  for (int r = 0; r < n; ++r) {
-    int& t = s->t[env_ids[r]];
-    t = (std::max(t, 0) + 1) % s->T;
-  }
-  DRL_CUDA_CHECK(cudaStreamSynchronize(st));
-  return DRL_OK;
+  return server_serve(s, n, env_ids, timeout_ms);
 }
 
 }  // extern "C"

@@ -11,6 +11,9 @@
 //                           first-maximum argmax and the explore override; writes q, h', c', action and q[action]
 //                           straight into mapped pinned memory (no D2H node)
 // Both new kernels sum in a fixed order without atomics: eager and graph replays, and repeated calls, are bitwise equal.
+// The act enqueues two halves: the H2D of its pinned input block, then the kernels on the device input block
+// (r2d2_policy_enqueue_forward), which the R2D2 policy server (r2d2_policy_server.cu) runs on input rows its own kernel
+// fills.
 //
 // A recorder (drl_r2d2_policy_recorder_*, DESIGN.md section 13) binds the engine to a device R2D2 sequence queue
 // (traj_queue.cuh, queue_recorder.cuh).  Its act is the engine's act with r2d2_policy_head_record in place of
@@ -282,13 +285,21 @@ struct drl_r2d2_policy_recorder : RecorderCore {
 
 namespace {
 
-// the engine's act of n rows; with a recorder, the recording head and r2d2_record_step as well
-int enqueue_act_impl(drl_r2d2_policy* h, int n, drl_r2d2_policy_recorder* rec) {
+// the engine's mapped outputs of an n-row act
+R2PolicyOutRows mapped_outputs(drl_r2d2_policy* h) {
+  return R2PolicyOutRows{reinterpret_cast<float*>(h->d_out), reinterpret_cast<float*>(h->d_out + h->off_h),
+                         reinterpret_cast<float*>(h->d_out + h->off_c),
+                         reinterpret_cast<int32_t*>(h->d_out + h->off_act),
+                         reinterpret_cast<float*>(h->d_out + h->off_qa)};
+}
+
+// the kernels of the engine's act of n rows on the device input block d_in, writing `out`; with a recorder, the
+// recording head and r2d2_record_step as well
+int enqueue_forward(drl_r2d2_policy* h, int n, const R2PolicyOutRows& out, drl_r2d2_policy_recorder* rec) {
   const R2InLayout l = r2_in_layout(n, h->frame);
   const R2Layout& pl = h->pl;
   const float* P = h->params;
   cudaStream_t s = h->stream;
-  DRL_CUDA_CHECK(cudaMemcpyAsync(h->d_in, h->h_in, l.total, cudaMemcpyHostToDevice, s));
   const int32_t* pa = reinterpret_cast<const int32_t*>(h->d_in + l.pa);
   const float* h0 = reinterpret_cast<const float*>(h->d_in + l.h0);
   DRL_TRY(policy_conv_forward_tf32(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3));
@@ -301,11 +312,11 @@ int enqueue_act_impl(drl_r2d2_policy* h, int n, drl_r2d2_policy_recorder* rec) {
   a.q1_w = P + pl.q1_w; a.q1_b = P + pl.q1_b;
   a.value_w = P + pl.value_w; a.value_b = P + pl.value_b;
   a.mean_w = P + pl.mean_w; a.mean_b = P + pl.mean_b;
-  a.q = reinterpret_cast<float*>(h->d_out);
-  a.h1 = reinterpret_cast<float*>(h->d_out + h->off_h);
-  a.c1 = reinterpret_cast<float*>(h->d_out + h->off_c);
-  a.action = reinterpret_cast<int32_t*>(h->d_out + h->off_act);
-  a.q_action = reinterpret_cast<float*>(h->d_out + h->off_qa);
+  a.q = out.q;
+  a.h1 = out.h1;
+  a.c1 = out.c1;
+  a.action = out.action;
+  a.q_action = out.q_action;
   a.n = n;
   a.A = h->A;
   if (!rec) {
@@ -331,6 +342,12 @@ int enqueue_act_impl(drl_r2d2_policy* h, int n, drl_r2d2_policy_recorder* rec) {
   r.frame16 = (int)(h->frame / 16);
   DRL_CUDA_CHECK((launch_k(r2d2_record_step_kernel, n, kR2RecThreads, 0, s, r)));
   return DRL_OK;
+}
+
+// the engine's act of n rows: the upload of the staged input block, then its kernels
+int enqueue_act_impl(drl_r2d2_policy* h, int n, drl_r2d2_policy_recorder* rec) {
+  DRL_CUDA_CHECK(cudaMemcpyAsync(h->d_in, h->h_in, r2_in_layout(n, h->frame).total, cudaMemcpyHostToDevice, h->stream));
+  return enqueue_forward(h, n, mapped_outputs(h), rec);
 }
 
 int enqueue_act(PolicyCore* c, int n) { return enqueue_act_impl(static_cast<drl_r2d2_policy*>(c), n, nullptr); }
@@ -366,6 +383,24 @@ void copy_act_outputs(const drl_r2d2_policy* h, int n, int32_t* action, float* q
 }
 
 }  // namespace
+
+namespace drl {
+
+PolicyCore* r2d2_policy_core_of(drl_r2d2_policy* h) { return h; }
+int r2d2_policy_channels(const drl_r2d2_policy* h) { return h->pl.C; }
+
+R2PolicyInRows r2d2_policy_input_rows(drl_r2d2_policy* h, int n) {
+  const R2InLayout l = r2_in_layout(n, h->frame);
+  return R2PolicyInRows{h->d_in + l.frames, reinterpret_cast<int32_t*>(h->d_in + l.pa),
+                        reinterpret_cast<float*>(h->d_in + l.h0), reinterpret_cast<float*>(h->d_in + l.c0),
+                        reinterpret_cast<int32_t*>(h->d_in + l.explore)};
+}
+
+int r2d2_policy_enqueue_forward(drl_r2d2_policy* h, int n, const R2PolicyOutRows& out) {
+  return enqueue_forward(h, n, out, nullptr);
+}
+
+}  // namespace drl
 
 extern "C" {
 

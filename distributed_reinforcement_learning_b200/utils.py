@@ -7,6 +7,8 @@
                                        train_impala.py:117,165-189: closes the actor -> ring -> learner loop)
   impala_env_step    (new) the IMPALA actor's rule for one environment step, shared by actor.VectorActor and the
                      worker processes of actor_server.EnvWorkerPool
+  r2d2_env_step      (new) the R2D2 actor's rule for one environment step, shared by actor.R2D2VectorActor and the
+                     worker processes of actor_server.R2D2EnvWorkerPool
 """
 import collections
 
@@ -41,6 +43,43 @@ def impala_env_step(env, action, available_action, stats, i, max_prob, task=None
                         episode_step=stats.episode_step[i], prob=stats.total_max_prob[i] / stats.episode_step[i])
         stats.episode[i] += 1
         stats.score[i], stats.episode_step[i], stats.total_max_prob[i] = 0.0, 0, 0.0
+        state = env.reset()
+        stats.lives[i] = START_LIVES
+    return next_state, r, d, state, finished
+
+
+def r2d2_env_step(env, action, stats, i, q_action, task=None):
+    """One step of environment i under the R2D2 actor's rules (train_r2d2.py:196-235).  ``stats`` holds the
+    per-environment lists ``lives``, ``episode``, ``epsilon``, ``score``, ``episode_step`` and ``episode_q_value``;
+    ``q_action`` is q[action] of the act that chose the action.
+
+      - the environment steps with the raw action (the R2D2 actor applies no ``% available_action``);
+      - ``lives`` is only set back to 5 at an episode's end, never after a life loss, so every step after the first
+        life loss of an episode is stored as reward -1 and done=True (the reference's behaviour); the score keeps the
+        raw reward;
+      - at an episode's end epsilon becomes 1 / (0.01 episode + 1), the environment is reset, and the caller sets the
+        previous action, h and c back to 0.  episode_step and the summed q of the logged average are never reset.
+
+    Returns (next_state, reward, done, state, finished): env.step's frame, the reward and done flag the sequence
+    stores, the frame the next action is for (a fresh episode's first frame after an episode end), and the finished
+    episode's dict of task (``task``, default i), episode, score, epsilon, episode_step and avg_q_value -- the values
+    train_r2d2.py:227-230 logs -- or None."""
+    stats.episode_q_value[i] += float(q_action)
+    stats.episode_step[i] += 1
+    next_state, reward, done, info = env.step(action)
+    stats.score[i] += reward
+    if stats.lives[i] != info["ale.lives"]:
+        r, d = -1, True
+    else:
+        r, d = reward, False
+    state, finished = next_state, None
+    if done:
+        finished = dict(task=i if task is None else task, episode=stats.episode[i], score=stats.score[i],
+                        epsilon=stats.epsilon[i], episode_step=stats.episode_step[i],
+                        avg_q_value=stats.episode_q_value[i] / stats.episode_step[i])
+        stats.episode[i] += 1
+        stats.score[i] = 0
+        stats.epsilon[i] = 1.0 / (0.01 * stats.episode[i] + 1)
         state = env.reset()
         stats.lives[i] = START_LIVES
     return next_state, r, d, state, finished

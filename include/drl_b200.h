@@ -404,6 +404,49 @@ int drl_r2d2_policy_recorder_reset(drl_r2d2_policy_recorder* r);
 int drl_r2d2_policy_recorder_commit(drl_r2d2_policy_recorder* r, const float* reward, const uint8_t* done,
                                     int32_t timeout_ms);
 
+/* R2D2 policy server: one R2D2 engine serving num_envs environments (1..256) that step in other processes, with each
+ * environment's recurrent state and unfinished sequence on the GPU (DESIGN.md section 17).  It binds one engine, one
+ * device R2D2 queue and an exchange block as the IMPALA policy server does, and keeps a device state table (per
+ * environment: h and c f32 [64], the previous action, and t, the step of the current sequence the next act records)
+ * and a device staging of one sequence per environment in the queue's field order (106,547 B per environment at
+ * S = 15, C = 1).
+ *
+ * Exchange block: the IMPALA server's record sizes and stride, so drl_policy_server_exchange_bytes sizes it; num_envs
+ * report records, then num_envs reply records, every field 16-byte aligned.  Before environment e is served, its report
+ * holds the frame the next action is for (84x84xC, the queue's C; the record keeps 84x84x4 bytes for it at either C),
+ * the explore action (-1: the greedy action; a value in [0, A): that action, as drl_r2d2_policy_act's explore_action),
+ * the reward and done flag the environment gave for its previous action, and `reset` = 1 when the episode restarted
+ * (the previous action, h and c taken as 0) or it is the environment's first act.  After the serve its reply holds the
+ * action and q_action (q of the main scope at the action). */
+#define DRL_R2D2_SERVER_REPORT_FRAME 0          /* u8 [84,84,C]  */
+#define DRL_R2D2_SERVER_REPORT_EXPLORE 28224    /* i32, in [-1, A) */
+#define DRL_R2D2_SERVER_REPORT_REWARD 28240     /* f32            */
+#define DRL_R2D2_SERVER_REPORT_DONE 28256       /* u8             */
+#define DRL_R2D2_SERVER_REPORT_RESET 28272      /* u8             */
+#define DRL_R2D2_SERVER_REPORT_BYTES 28288
+#define DRL_R2D2_SERVER_REPLY_ACTION 0          /* i32            */
+#define DRL_R2D2_SERVER_REPLY_Q_ACTION 16       /* f32            */
+#define DRL_R2D2_SERVER_REPLY_BYTES 32
+typedef struct drl_r2d2_policy_server drl_r2d2_policy_server;
+/* Registers the exchange block with CUDA (mapped, portable) until destroy.  Queue and engine must be on the same device
+ * with the same num_action and channels, the queue must take min(num_envs, max_batch) sequences at once, and the block
+ * must be page-aligned and large enough; all DRL_ERR_INVALID otherwise.  Without a device, DRL_ERR_CUDA.  Destroy the
+ * server before its engine and queue; after that the block may be registered again. */
+int drl_r2d2_policy_server_create(drl_r2d2_policy* h, drl_r2d2_queue* queue, int32_t num_envs, void* exchange,
+                                  int64_t exchange_bytes, drl_r2d2_policy_server** out);
+int drl_r2d2_policy_server_destroy(drl_r2d2_policy_server* s);
+/* Serves the n <= max_batch distinct environments env_ids (any subset of [0, num_envs), any order; DRL_ERR_INVALID
+ * otherwise) from their reports, in one act of the engine on its stream: the reward and done of each one's previous
+ * step land in its staged sequence, every sequence whose step S-1 that completes is appended to the queue (in env_ids
+ * order), then the act records step t of each environment (frame, previous action, action; at t = 0 h and c) and
+ * writes its reply.  The serve reads each explore action once from the block on the host; one outside [-1, A) is
+ * DRL_ERR_INVALID naming the environment, returned before anything is reserved or launched: the state table, the
+ * staging, the queue and every reply are as they were.  Blocks while the queue has no room for the completed sequences
+ * (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with nothing changed otherwise).  Synchronous: the replies are written on
+ * return.  With use_cuda_graph one graph per n replays the kernels.  A failure after the queue positions were reserved
+ * puts the queue into its failed state, as drl_policy_recorder_commit. */
+int drl_r2d2_policy_server_serve(drl_r2d2_policy_server* s, int32_t n, const int32_t* env_ids, int32_t timeout_ms);
+
 /* ------------------------------------------------------------------------------------------
  * Ape-X / A3C policy engine (new): the actor side of train_apex.py:157-231 and train_a3c.py:112-183 (the actor loops
  * themselves are distributed_reinforcement_learning_b200/actor.py: ApexVectorActor, A3CVectorActor).  A forward-only

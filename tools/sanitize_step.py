@@ -1,12 +1,14 @@
 """One tiny learner step per math mode for compute-sanitizer (memcheck / racecheck / synccheck of the mbarrier + wgmma
 pipelines), with --peer under torchrun the 2-GPU fused exchange (flag protocol over NVLink peer memory), and with
 --serve one eager serve loop of the IMPALA policy server (drl_policy_server_*: gather, per-row commit, act, scatter)
-over a registered exchange block the script fills itself, without worker processes.
+over a registered exchange block the script fills itself, without worker processes, and with --serve-r2d2 the same for
+the R2D2 policy server (drl_r2d2_policy_server_*).
 
     compute-sanitizer --tool memcheck  python tools/sanitize_step.py --modes 2 3
     compute-sanitizer --tool racecheck python tools/sanitize_step.py --modes 2
     torchrun --nproc-per-node 2 ... tools/sanitize_step.py --peer      (run each rank under compute-sanitizer)
     DRL_B200_CUDA_GRAPH=0 compute-sanitizer --tool memcheck python tools/sanitize_step.py --serve
+    DRL_B200_CUDA_GRAPH=0 compute-sanitizer --tool memcheck python tools/sanitize_step.py --serve-r2d2
 """
 import argparse
 import os
@@ -70,6 +72,67 @@ def serve_loop(envs=6, max_batch=4, trajectory=3, unrolls=3):
           % (graph, unrolls * trajectory + 1, envs, envs * unrolls), flush=True)
 
 
+def serve_r2d2_loop(envs=6, max_batch=4, seq_len=3, unrolls=3, channels=1, num_action=4):
+    """Serves `envs` R2D2 environments for `unrolls` sequences in random subsets of at most max_batch, with explore
+    actions and reset flags now and then, and checks the committed sequences' frames and actions against the reports
+    and replies."""
+    import ctypes as C
+    import mmap
+    from distributed_reinforcement_learning_b200.actor_server import (R2D2PolicyServer, exchange_bytes,
+                                                                      r2d2_exchange_views)
+    from distributed_reinforcement_learning_b200.distributed_queue.buffer_queue import R2D2DeviceFIFOQueue
+    from distributed_reinforcement_learning_b200.model import r2d2_lstm as model
+    from distributed_reinforcement_learning_b200.r2d2_policy import NativeR2D2Policy
+
+    class Block:   # the exchange block of a pool, without workers
+        def __init__(self):
+            self.num_envs, self.exchange_bytes = envs, exchange_bytes(envs)
+            self.mem = mmap.mmap(-1, self.exchange_bytes)
+            self.anchor = C.c_char.from_buffer(self.mem)
+            self.address = C.addressof(self.anchor)
+            self.views = r2d2_exchange_views(self.mem, envs, channels)
+
+    shape = (84, 84, channels)
+    graph = os.environ.get("DRL_B200_CUDA_GRAPH", "1") != "0"
+    rng = np.random.RandomState(0)
+    pol = NativeR2D2Policy(max_batch, num_action=num_action, input_shape=shape, use_cuda_graph=graph)
+    pol.set_params(model.init_params(0, num_action=num_action, lstm_size=64, input_shape=shape))
+    q = R2D2DeviceFIFOQueue(seq_len, shape, num_action, envs * unrolls, envs, 1, 64)
+    blk = Block()
+    v = blk.views
+    server = R2D2PolicyServer(pol, q, blk)
+    frames = {e: [] for e in range(envs)}
+    actions = {e: [] for e in range(envs)}
+    for step in range(unrolls * seq_len + 1):
+        for e in range(envs):
+            v["frame"][e] = rng.randint(0, 256, shape)
+            v["explore"][e] = rng.randint(0, num_action) if rng.rand() < 0.3 else -1
+            v["reward"][e], v["done"][e], v["reset"][e] = rng.randint(3), rng.rand() < 0.2, step == 0 or rng.rand() < 0.1
+            frames[e].append(v["frame"][e].copy())
+        ids = rng.permutation(envs).astype(np.int32)
+        k = 0
+        while k < envs:
+            c = rng.randint(1, max_batch + 1)
+            server.serve(ids[k:k + c])
+            k += c
+        assert ((v["action"][:envs] >= 0) & (v["action"][:envs] < num_action)).all()
+        explore = v["explore"][:envs]
+        assert (v["action"][:envs][explore >= 0] == explore[explore >= 0]).all()
+        for e in range(envs):
+            actions[e].append(int(v["action"][e]))
+    assert q.get_size() == envs * unrolls
+    want = {(np.stack(frames[e][u * seq_len:(u + 1) * seq_len]).tobytes(),
+             np.array(actions[e][u * seq_len:(u + 1) * seq_len], np.int32).tobytes())
+            for e in range(envs) for u in range(unrolls)}
+    got = {(r["state"].tobytes(), r["action"].tobytes()) for r in (q.read(j) for j in range(envs * unrolls))}
+    assert got == want
+    server.close()
+    q.close()
+    pol.close()
+    print("r2d2 serve loop (cuda graph %s): %d serves of %d environments, %d sequences committed ok"
+          % (graph, unrolls * seq_len + 1, envs, envs * unrolls), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--modes", type=int, nargs="*", default=[2])
@@ -78,9 +141,14 @@ def main():
     ap.add_argument("--peer", action="store_true")
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--serve", action="store_true", help="the policy server's serve loop instead of learner steps")
+    ap.add_argument("--serve-r2d2", action="store_true",
+                    help="the R2D2 policy server's serve loop instead of learner steps")
     a = ap.parse_args()
     if a.serve:
         serve_loop()
+        return
+    if a.serve_r2d2:
+        serve_r2d2_loop()
         return
     from distributed_reinforcement_learning_b200.learner import NativeLearner
     from distributed_reinforcement_learning_b200.model import impala_actor_critic as model
