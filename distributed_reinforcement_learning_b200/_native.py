@@ -315,6 +315,10 @@ def _load():
         "drl_a3c_policy_recorder_act": (C.c_int, [vp] + [vp] * 7),
         "drl_a3c_policy_recorder_commit": (C.c_int, [vp, vp, vp, vp, i32]),
         "drl_a3c_policy_recorder_reset": (C.c_int, [vp]),
+        "drl_a3c_policy_server_exchange_bytes": (C.c_int, [i32, C.POINTER(i64)]),
+        "drl_a3c_policy_server_create": (C.c_int, [vp, vp, i32, vp, i64, C.POINTER(vp)]),
+        "drl_a3c_policy_server_destroy": (C.c_int, [vp]),
+        "drl_a3c_policy_server_serve": (C.c_int, [vp, i32, vp, i32]),
         "drl_a3c_stage_from_queue": (C.c_int, [vp, i32, vp, i32]),
         "drl_r2d2_replay_create": (C.c_int, [i32, i64, i32, i32, i32, C.POINTER(vp)]),
         "drl_r2d2_replay_destroy": (C.c_int, [vp]),

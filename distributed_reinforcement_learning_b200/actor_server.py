@@ -19,6 +19,12 @@ environment's explore decision from its own stream, and ``R2D2PolicyServer`` act
 ``r2d2.DeviceMemory.add_from_queue`` ingests.  Its records (``DRL_R2D2_SERVER_*``) have the IMPALA records' sizes; the
 report carries an explore action instead of a uniform draw, and the reply q_action instead of a max probability.
 
+A3C has the pair ``A3CEnvWorkerPool`` / ``A3CPolicyServer``: the IMPALA step rule (``utils.impala_env_step``), one
+``NativeA3CPolicy`` (``drl_a3c_policy_server_*``) and an ``A3CDeviceFIFOQueue`` that ``a3c.Agent.train_from_queue``
+trains from.  An A3C record stores next_state, and after an episode end the frame to act on (the new episode's first)
+is not the previous step's next_state, so its report (``DRL_A3C_SERVER_*``) carries a second frame, written and read
+only then.
+
 This module imports neither torch nor the native library at module level: the spawned workers import it.
 """
 import collections
@@ -90,6 +96,39 @@ def r2d2_exchange_views(buf, num_envs, channels=1):
     return v
 
 
+# the A3C server's records (include/drl_b200.h: DRL_A3C_SERVER_*): two frames per report
+A3C_REPORT_FRAME, A3C_REPORT_NEXT_STATE, A3C_REPORT_UNIFORM, A3C_REPORT_REWARD, A3C_REPORT_DONE, A3C_REPORT_RESET = (
+    0, 28224, 56448, 56464, 56480, 56496)
+A3C_REPORT_BYTES = 56512
+A3C_REPLY_ACTION, A3C_REPLY_MAX_PROB, A3C_REPLY_BYTES = 0, 16, 32
+
+
+def a3c_exchange_bytes(num_envs):
+    """Size of the A3C exchange block of num_envs environments: the reports, then the replies, rounded up to a page."""
+    n = num_envs * (A3C_REPORT_BYTES + A3C_REPLY_BYTES)
+    return -(-n // PAGE) * PAGE
+
+
+def a3c_exchange_views(buf, num_envs):
+    """numpy views of the A3C records in the exchange block `buf` (a writable buffer of a3c_exchange_bytes(num_envs)):
+    frame, next_state, uniform, reward, done, reset, action and max_prob."""
+    E = num_envs
+
+    def field(offset, dtype, shape=(), strides=()):
+        return np.ndarray((E,) + shape, dtype, buffer=buf, offset=offset, strides=(stride,) + strides)
+
+    fs = (FRAME_SHAPE[1] * FRAME_SHAPE[2], FRAME_SHAPE[2], 1)
+    stride = A3C_REPORT_BYTES
+    v = dict(frame=field(A3C_REPORT_FRAME, np.uint8, FRAME_SHAPE, fs),
+             next_state=field(A3C_REPORT_NEXT_STATE, np.uint8, FRAME_SHAPE, fs),
+             uniform=field(A3C_REPORT_UNIFORM, np.float64), reward=field(A3C_REPORT_REWARD, np.float32),
+             done=field(A3C_REPORT_DONE, np.uint8), reset=field(A3C_REPORT_RESET, np.uint8))
+    stride = A3C_REPLY_BYTES
+    base = E * A3C_REPORT_BYTES
+    v.update(action=field(base + A3C_REPLY_ACTION, np.int32), max_prob=field(base + A3C_REPLY_MAX_PROB, np.float32))
+    return v
+
+
 def explore_action(rng, epsilon, num_action):
     """The epsilon-greedy draw of policy_handle.explore_actions for one environment, from its own RandomState `rng`:
     ``rng.rand() > epsilon`` keeps the greedy action (-1), otherwise ``rng.choice(num_action)`` is the action."""
@@ -157,11 +196,12 @@ def _worker_loop(conn, shm, v, env_ids, env_fns, first_report, step):
         conn.close()
 
 
-def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, seeds):
+def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, seeds, a3c=False):
     """An IMPALA worker process: k environments, each task env_ids[j] with its own RandomState(seeds[j]) for the uniform
-    draws of its actions."""
+    draws of its actions.  With `a3c` the records are the A3C server's, and after an episode end the worker also
+    writes env.step's frame into next_state."""
     shm = shared_memory.SharedMemory(name=shm_name)
-    v = exchange_views(shm.buf, num_envs)
+    v = (a3c_exchange_views if a3c else exchange_views)(shm.buf, num_envs)
     rngs, stats = [], None
 
     def first_report(envs):
@@ -176,14 +216,21 @@ def _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, s
         return start
 
     def step(j, e, env):
-        _, r, d, state, episode = utils.impala_env_step(env, int(v["action"][e]), available_action[j], stats, j,
-                                                        v["max_prob"][e], task=e)
+        next_state, r, d, state, episode = utils.impala_env_step(env, int(v["action"][e]), available_action[j], stats,
+                                                                 j, v["max_prob"][e], task=e)
+        if a3c and episode is not None:
+            v["next_state"][e] = next_state
         v["frame"][e] = state
         v["reward"][e], v["done"][e], v["reset"][e] = r, d, episode is not None
         v["uniform"][e] = rngs[j].random_sample()
         return episode
 
     _worker_loop(conn, shm, v, env_ids, env_fns, first_report, step)
+
+
+def _a3c_worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, seeds):
+    """An A3C worker process: the IMPALA worker on the A3C records."""
+    _worker_main(conn, shm_name, num_envs, env_ids, env_fns, available_action, seeds, a3c=True)
 
 
 def _r2d2_worker_main(conn, shm_name, num_envs, env_ids, env_fns, num_action, channels, seeds):
@@ -232,7 +279,7 @@ class EnvWorkerPool:
         self._check(env_fns, envs_per_worker)
         if len(available_action) != len(env_fns) or len(seeds) != len(env_fns):
             raise ValueError("available_action and seeds need one entry per environment (%d)" % len(env_fns))
-        self._start(env_fns, envs_per_worker, seeds, exchange_views, _worker_main,
+        self._start(env_fns, envs_per_worker, seeds, exchange_bytes, exchange_views, _worker_main,
                     lambda lo, hi: (available_action[lo:hi],), start_timeout, join_timeout)
 
     @staticmethod
@@ -241,10 +288,11 @@ class EnvWorkerPool:
         if not 1 <= n <= MAX_ENVS:
             raise ValueError("%d environments, a pool serves 1..%d" % (n, MAX_ENVS))
 
-    def _start(self, env_fns, envs_per_worker, seeds, views, target, worker_args, start_timeout, join_timeout):
-        """Checks envs_per_worker and the factories, makes the exchange block (views(buf, n): its numpy views) and
-        spawns one `target` process per envs_per_worker environments, with the arguments (pipe, block name, n, env ids,
-        env factories, *worker_args(lo, hi), seeds) of environments lo..hi-1; waits for every worker's first report."""
+    def _start(self, env_fns, envs_per_worker, seeds, size, views, target, worker_args, start_timeout, join_timeout):
+        """Checks envs_per_worker and the factories, makes the exchange block (size(n): its bytes; views(buf, n): its
+        numpy views) and spawns one `target` process per envs_per_worker environments, with the arguments (pipe, block
+        name, n, env ids, env factories, *worker_args(lo, hi), seeds) of environments lo..hi-1; waits for every
+        worker's first report."""
         n, k = len(env_fns), int(envs_per_worker)
         if k < 1:
             raise ValueError("envs_per_worker must be >= 1 (got %d)" % k)
@@ -255,7 +303,7 @@ class EnvWorkerPool:
                 raise ValueError("env_fns[%d] cannot be pickled for a spawned worker: %s" % (i, e)) from None
         self.num_envs, self.envs_per_worker = n, k
         self.join_timeout = join_timeout
-        self.exchange_bytes = exchange_bytes(n)
+        self.exchange_bytes = size(n)
         self._workers = []
         self._pending = set()
         self._servers = []
@@ -398,14 +446,38 @@ class R2D2EnvWorkerPool(EnvWorkerPool):
         if channels not in (1, 4):
             raise ValueError("channels must be 1 or 4 (got %d)" % channels)
         self.num_action, self.channels = num_action, channels
-        self._start(env_fns, envs_per_worker, seeds, lambda buf, n: r2d2_exchange_views(buf, n, channels),
-                    _r2d2_worker_main, lambda lo, hi: (num_action, channels), start_timeout, join_timeout)
+        self._start(env_fns, envs_per_worker, seeds, exchange_bytes,
+                    lambda buf, n: r2d2_exchange_views(buf, n, channels), _r2d2_worker_main,
+                    lambda lo, hi: (num_action, channels), start_timeout, join_timeout)
+
+
+class A3CEnvWorkerPool(EnvWorkerPool):
+    """``len(env_fns)`` A3C environments (1..256) in spawned worker processes of ``envs_per_worker`` environments each,
+    for an ``A3CPolicyServer``.
+
+    Environment i is task i: ``env_fns[i]()`` builds it in its worker, it steps under ``utils.impala_env_step`` with
+    ``available_action[i]`` -- the IMPALA rule is exactly the A3C actor's (train_a3c.py:150-178: the step with
+    ``action % available_action``, a lost life stored as reward -1 and done, the counters and the previous action reset
+    at an episode's end) -- and the uniform draws of its actions come from ``np.random.RandomState(seeds[i])``, drawn as
+    the IMPALA worker draws them, so they do not depend on batching or on how environments are grouped into workers.
+    The reports and replies are the A3C records (``a3c_exchange_views``); after an episode end the worker also writes
+    env.step's frame into next_state.  Everything else -- the pipes, ``wait_ready``, ``reply``, the failure reports and
+    ``close()`` -- is ``EnvWorkerPool``'s."""
+
+    def __init__(self, env_fns, available_action, envs_per_worker, seeds, start_timeout=300.0, join_timeout=10.0):
+        env_fns, seeds = list(env_fns), [int(s) for s in seeds]
+        available_action = [int(a) for a in available_action]
+        self._check(env_fns, envs_per_worker)
+        if len(available_action) != len(env_fns) or len(seeds) != len(env_fns):
+            raise ValueError("available_action and seeds need one entry per environment (%d)" % len(env_fns))
+        self._start(env_fns, envs_per_worker, seeds, a3c_exchange_bytes, a3c_exchange_views, _a3c_worker_main,
+                    lambda lo, hi: (available_action[lo:hi],), start_timeout, join_timeout)
 
 
 class _ServerBase:
-    """What PolicyServer and R2D2PolicyServer share: the binding to a pool, the serve lock, the C handle's lifetime,
-    the policy sync before a serve, and the serve loop.  A family sets `_prefix` (its ``drl_<prefix>_*`` entry
-    points) and `_what` (its name in messages) and implements ``_learner_step``."""
+    """What PolicyServer, R2D2PolicyServer and A3CPolicyServer share: the binding to a pool, the serve lock, the C
+    handle's lifetime, the policy sync before a serve, and the serve loop.  A family sets `_prefix` (its
+    ``drl_<prefix>_*`` entry points) and `_what` (its name in messages) and implements ``_learner_step``."""
     _prefix = None
     _what = None
 
@@ -561,3 +633,32 @@ class R2D2PolicyServer(_ServerBase):
 
     def _learner_step(self):
         return self.learner.train_calls
+
+
+class A3CPolicyServer(_ServerBase):
+    """Serves the environments of an ``A3CEnvWorkerPool`` from one ``NativeA3CPolicy`` into one
+    ``A3CDeviceFIFOQueue``, which ``a3c.Agent.train_from_queue`` trains from.
+
+    ``serve``, ``serve_once``, ``run`` and ``close`` are ``PolicyServer``'s; the uniform draws come with the reports.
+    Before a serve it syncs the policy from ``learner`` (an ``a3c.Agent``) whenever the learner has trained
+    (``num_env_frames``, its step counter) since the last sync.  The reference's actor runs ``parameter_sync`` once per
+    unroll, so each of its trajectories is recorded under one parameter version; here the sync follows the learner, so
+    one unroll may be recorded under several versions.  A3C has no off-policy correction; the lag is bounded by how far
+    acting runs ahead of training, which the queue's capacity limits as the reference's queue does.  While the queue is
+    full a serve blocks.  Single-replica, like ``train_from_queue``.  Closing the pool closes its server first.
+    ``serve_once`` returns the finished episodes as dicts of task, episode, prob, score and episode_step (the keys
+    ``A3CVectorActor.run_unroll`` returns)."""
+    _prefix = "a3c_policy_server"
+    _what = "a3c policy server"
+
+    def __init__(self, policy, queue, pool, learner=None):
+        from .apex_policy import NativeA3CPolicy
+        from .distributed_queue.buffer_queue import A3CDeviceFIFOQueue
+        if not isinstance(policy, NativeA3CPolicy):
+            raise TypeError("A3CPolicyServer: policy must be a NativeA3CPolicy, got %s" % type(policy).__name__)
+        if not isinstance(queue, A3CDeviceFIFOQueue):
+            raise TypeError("A3CPolicyServer: queue must be an A3CDeviceFIFOQueue, got %s" % type(queue).__name__)
+        self._bind_and_create(policy, queue, pool, learner)
+
+    def _learner_step(self):
+        return self.learner.num_env_frames

@@ -16,7 +16,7 @@ OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(CSRC, "libdrl_b200.so")
 SOURCES = ["learner_core.cu", "learner.cu", "layers.cu", "adam_learner.cu", "apex.cu", "r2d2.cu", "elementwise.cu", "vtrace.cu", "optimizer.cu", "ring.cu", "per.cu", "debug.cu",
            "peer.cu", "policy_core.cu", "policy.cu", "server_core.cu", "policy_server.cu", "r2d2_policy.cu",
-           "r2d2_policy_server.cu", "apex_policy.cu",
+           "r2d2_policy_server.cu", "apex_policy.cu", "a3c_policy_server.cu",
            "replay_core.cu", "apex_replay.cu", "r2d2_replay.cu", "traj_queue.cu", "apex_actor_buffer.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]

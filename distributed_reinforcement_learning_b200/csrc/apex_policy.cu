@@ -16,6 +16,9 @@
 //                           writes q / policy, action and q[action] / policy[action] straight into mapped pinned
 //                           memory (no D2H node)
 // Both new kernels sum in a fixed order without atomics: eager and graph replays, and repeated calls, are bitwise equal.
+// The act enqueues two halves: the H2D of its pinned input block, then the kernels on the device input block
+// (apex_policy_enqueue_forward), which the A3C policy server (a3c_policy_server.cu) runs on input rows its own kernel
+// fills.
 //
 // The A3C recorder (drl_a3c_policy_recorder_*, DESIGN.md section 15) runs this act unchanged and then one more kernel,
 // a3c_record_step, that writes the step into its staging of n unrolls in the device A3C queue's record layout.
@@ -271,13 +274,12 @@ struct drl_a3c_policy_recorder : RecorderCore {
 
 namespace {
 
-int enqueue_act(PolicyCore* c, int n) {
-  drl_apex_policy* h = static_cast<drl_apex_policy*>(c);
+// the kernels of the engine's act of n rows on the device input block d_in, writing `out`
+int enqueue_forward(drl_apex_policy* h, int n, const ApexPolicyOutRows& out) {
   const ApexInLayout l = apex_in_layout(n);
   const ApexLayout& pl = h->pl;
   const float* P = h->params;
   cudaStream_t s = h->stream;
-  DRL_CUDA_CHECK(cudaMemcpyAsync(h->d_in, h->h_in, l.total, cudaMemcpyHostToDevice, s));
   const int32_t* pa = reinterpret_cast<const int32_t*>(h->d_in + l.pa);
   DRL_TRY(policy_conv_forward_tf32(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3));
   ApexHeadArgs a;
@@ -289,9 +291,9 @@ int enqueue_act(PolicyCore* c, int n) {
   a.w3m = P + pl.mean3_w; a.b3m = P + pl.mean3_b;
   a.explore = reinterpret_cast<const int32_t*>(h->d_in + l.sel);
   a.uniform = reinterpret_cast<const double*>(h->d_in + l.sel);
-  a.out = reinterpret_cast<float*>(h->d_out);
-  a.action = reinterpret_cast<int32_t*>(h->d_out + h->off_act);
-  a.out_action = reinterpret_cast<float*>(h->d_out + h->off_sel);
+  a.out = out.out;
+  a.action = out.action;
+  a.out_action = out.out_action;
   a.n = n;
   a.A = h->A;
   const int grid = cdiv(n, kHR);
@@ -303,6 +305,15 @@ int enqueue_act(PolicyCore* c, int n) {
     DRL_CUDA_CHECK((launch_k(apex_policy_head_kernel<1>, grid, kApexHeadThreads, apex_head_smem<1>(), s, a)));
   }
   return DRL_OK;
+}
+
+// the engine's act of n rows: the upload of the staged input block, then its kernels into the mapped outputs
+int enqueue_act(PolicyCore* c, int n) {
+  drl_apex_policy* h = static_cast<drl_apex_policy*>(c);
+  DRL_CUDA_CHECK(cudaMemcpyAsync(h->d_in, h->h_in, apex_in_layout(n).total, cudaMemcpyHostToDevice, h->stream));
+  const ApexPolicyOutRows out{reinterpret_cast<float*>(h->d_out), reinterpret_cast<int32_t*>(h->d_out + h->off_act),
+                              reinterpret_cast<float*>(h->d_out + h->off_sel)};
+  return enqueue_forward(h, n, out);
 }
 
 // checks common to both act entry points; on success the caller stages `sel` and calls run_act
@@ -372,6 +383,23 @@ int enqueue_a3c_record(drl_a3c_policy_recorder* r) {
 }
 
 }  // namespace
+
+namespace drl {
+
+PolicyCore* apex_policy_core_of(drl_apex_policy* h) { return h; }
+int apex_policy_algo(const drl_apex_policy* h) { return h->algo; }
+
+ApexPolicyInRows apex_policy_input_rows(drl_apex_policy* h, int n) {
+  const ApexInLayout l = apex_in_layout(n);
+  return ApexPolicyInRows{h->d_in + l.frames, reinterpret_cast<int32_t*>(h->d_in + l.pa),
+                          reinterpret_cast<double*>(h->d_in + l.sel)};
+}
+
+int apex_policy_enqueue_forward(drl_apex_policy* h, int n, const ApexPolicyOutRows& out) {
+  return enqueue_forward(h, n, out);
+}
+
+}  // namespace drl
 
 extern "C" {
 

@@ -295,6 +295,27 @@ R2PolicyInRows r2d2_policy_input_rows(drl_r2d2_policy* h, int n);
 // and writing `out`; the caller holds the engine's lock
 int r2d2_policy_enqueue_forward(drl_r2d2_policy* h, int n, const R2PolicyOutRows& out);
 
+// ---- apex_policy.cu: the Ape-X / A3C policy engine's act on device-resident inputs (a3c_policy_server.cu) ---------
+PolicyCore* apex_policy_core_of(drl_apex_policy* h);
+int apex_policy_algo(const drl_apex_policy* h);   // 0 = Ape-X, 1 = A3C
+// the rows of an n-row act inside the engine's device input block
+struct ApexPolicyInRows {
+  uint8_t* frames;   // [n][84*84*4]
+  int32_t* pa;       // [n]
+  double* uniform;   // [n]: A3C's uniform draws (the Ape-X engine reads the same bytes as i32 explore actions)
+};
+// where the act's head writes: q or policy [n][A], action [n], q[action] or policy[action] [n]
+struct ApexPolicyOutRows {
+  float* out;
+  int32_t* action;
+  float* out_action;
+};
+ApexPolicyInRows apex_policy_input_rows(drl_apex_policy* h, int n);
+// the engine's act kernels of n rows (drl_apex_policy_act / drl_a3c_policy_act without the upload of the input block:
+// conv stack, skinny_splitk_fwd and apex_policy_head_kernel) on the engine's stream, reading the rows of
+// apex_policy_input_rows(h, n) and writing `out`; the caller holds the engine's lock
+int apex_policy_enqueue_forward(drl_apex_policy* h, int n, const ApexPolicyOutRows& out);
+
 // ---- learner.cu: parameter snapshot for the policy engine (drl_policy_sync_from_learner) ---------------------------
 // learner_params_snapshot (learner_core.cuh) of an IMPALA learner whose network has num_action actions:
 // DRL_ERR_INVALID for a learner with another num_action, DRL_ERR_STATE for a learner in the failed state.

@@ -217,7 +217,7 @@ int drl_policy_server_create(drl_policy* p, drl_traj_queue* q, int32_t num_envs,
   if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
   if (!p) { set_error("null policy handle"); return DRL_ERR_INVALID; }
   if (!q) { set_error("null trajectory queue handle"); return DRL_ERR_INVALID; }
-  DRL_TRY(server_check_block("policy server", num_envs, exchange, exchange_size));
+  DRL_TRY(server_check_block("policy server", num_envs, DRL_SERVER_REPORT_BYTES, exchange, exchange_size));
   PolicyCore* h = policy_core_of(p);
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   if (q->device != h->device) {
@@ -238,6 +238,7 @@ int drl_policy_server_create(drl_policy* p, drl_traj_queue* q, int32_t num_envs,
   s->engine = h;
   s->q = q;
   s->num_envs = num_envs;
+  s->report_bytes = DRL_SERVER_REPORT_BYTES;
   s->T = q->T;
   s->enqueue_serve = enqueue_serve;
   int rc = server_check_queue_rows(s, "trajectories");

@@ -267,7 +267,7 @@ int drl_r2d2_policy_server_create(drl_r2d2_policy* p, drl_r2d2_queue* q, int32_t
   if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
   if (!p) { set_error("null r2d2 policy handle"); return DRL_ERR_INVALID; }
   if (!q) { set_error("null r2d2 queue handle"); return DRL_ERR_INVALID; }
-  DRL_TRY(server_check_block(kName, num_envs, exchange, exchange_size));
+  DRL_TRY(server_check_block(kName, num_envs, DRL_SERVER_REPORT_BYTES, exchange, exchange_size));
   PolicyCore* h = r2d2_policy_core_of(p);
   std::lock_guard<std::recursive_mutex> lk(h->mu);
   if (q->device != h->device) {
@@ -288,6 +288,7 @@ int drl_r2d2_policy_server_create(drl_r2d2_policy* p, drl_r2d2_queue* q, int32_t
   s->engine = h;
   s->q = q;
   s->num_envs = num_envs;
+  s->report_bytes = DRL_SERVER_REPORT_BYTES;
   s->T = q->S;
   s->C = C;
   s->enqueue_serve = enqueue_serve;

@@ -55,16 +55,16 @@ __global__ void __launch_bounds__(kServerThreads) queue_commit_rows_kernel(const
 
 }  // namespace
 
-int64_t server_exchange_bytes(int num_envs) {
-  return (int64_t)align_up((size_t)num_envs * (DRL_SERVER_REPORT_BYTES + DRL_SERVER_REPLY_BYTES), 4096);
+int64_t server_exchange_bytes(int num_envs, int report_bytes) {
+  return (int64_t)align_up((size_t)num_envs * ((size_t)report_bytes + DRL_SERVER_REPLY_BYTES), 4096);
 }
 
-int server_check_block(const char* name, int num_envs, const void* exchange, int64_t exchange_size) {
+int server_check_block(const char* name, int num_envs, int report_bytes, const void* exchange, int64_t exchange_size) {
   if (num_envs < 1 || num_envs > kServerMaxEnvs) {
     set_error("%s: num_envs must be in [1, %d] (got %d)", name, kServerMaxEnvs, num_envs);
     return DRL_ERR_INVALID;
   }
-  const int64_t need = server_exchange_bytes(num_envs);
+  const int64_t need = server_exchange_bytes(num_envs, report_bytes);
   const long page = sysconf(_SC_PAGESIZE);
   if (!exchange || reinterpret_cast<uintptr_t>(exchange) % (uintptr_t)page != 0) {
     set_error("%s: the exchange block must be page-aligned (%ld bytes)", name, page);
@@ -98,7 +98,7 @@ int server_core_init(ServerCore* s, void* exchange) {
   DRL_TRY(dev_alloc(s, &s->d_words, s->words.count()));
   DRL_CUDA_CHECK(cudaHostAlloc((void**)&s->h_words, s->words.count() * 4, cudaHostAllocDefault));
   memset(s->h_words, 0, s->words.count() * 4);
-  DRL_CUDA_CHECK(cudaHostRegister(exchange, (size_t)server_exchange_bytes(s->num_envs),
+  DRL_CUDA_CHECK(cudaHostRegister(exchange, (size_t)server_exchange_bytes(s->num_envs, s->report_bytes),
                                   cudaHostRegisterMapped | cudaHostRegisterPortable));
   s->host_block = static_cast<uint8_t*>(exchange);
   DRL_CUDA_CHECK(cudaHostGetDevicePointer((void**)&s->d_block, exchange, 0));
@@ -233,7 +233,7 @@ int drl_policy_server_exchange_bytes(int32_t num_envs, int64_t* bytes) {
     set_error("policy server: num_envs must be in [1, %d] (got %d)", kServerMaxEnvs, num_envs);
     return DRL_ERR_INVALID;
   }
-  *bytes = server_exchange_bytes(num_envs);
+  *bytes = server_exchange_bytes(num_envs, DRL_SERVER_REPORT_BYTES);
   return DRL_OK;
 }
 

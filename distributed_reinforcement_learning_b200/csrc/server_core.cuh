@@ -6,8 +6,10 @@
 // drl_policy_server) and the R2D2 server (r2d2_policy_server.cu: drl_r2d2_policy_server) derive from ServerCore; each
 // adds its state table, its gather and scatter kernels and its enqueue of one serve.
 //
-// Both families use the same record sizes and stride in the exchange block (DRL_SERVER_REPORT_BYTES /
-// DRL_SERVER_REPLY_BYTES), so one drl_policy_server_exchange_bytes sizes the block of either.
+// The IMPALA and R2D2 families use the same record sizes and stride in the exchange block (DRL_SERVER_REPORT_BYTES /
+// DRL_SERVER_REPLY_BYTES), so one drl_policy_server_exchange_bytes sizes the block of either.  The A3C server
+// (a3c_policy_server.cu: drl_a3c_policy_server) reports two frames per environment, so each family sets its report
+// size (ServerCore::report_bytes); every family's reply record is DRL_SERVER_REPLY_BYTES.
 #pragma once
 #include <mutex>
 #include <vector>
@@ -49,6 +51,7 @@ struct ServerCore {
   EnqueueServe enqueue_serve = nullptr;
   StageRows stage_rows = nullptr;
   int extra_words = 0;
+  int report_bytes = 0;                     // stride of the report records; the replies follow num_envs of them
 
   std::mutex mu;                            // one serve at a time
   uint8_t* host_block = nullptr;            // the caller's exchange block, registered while the server lives
@@ -62,15 +65,16 @@ struct ServerCore {
   std::vector<void*> allocs;
 };
 
-// num_envs * (DRL_SERVER_REPORT_BYTES + DRL_SERVER_REPLY_BYTES) rounded up to a page
-int64_t server_exchange_bytes(int num_envs);
+// num_envs * (report_bytes + DRL_SERVER_REPLY_BYTES) rounded up to a page
+int64_t server_exchange_bytes(int num_envs, int report_bytes);
 // create's checks of the block, in this order: num_envs in [1, 256], a page-aligned block of at least
-// server_exchange_bytes(num_envs) bytes (DRL_ERR_INVALID, "<name>: ...")
-int server_check_block(const char* name, int num_envs, const void* exchange, int64_t exchange_size);
+// server_exchange_bytes(num_envs, report_bytes) bytes (DRL_ERR_INVALID, "<name>: ...")
+int server_check_block(const char* name, int num_envs, int report_bytes, const void* exchange, int64_t exchange_size);
 // "one serve may commit min(num_envs, max_batch) records, the queue takes at most ..." (DRL_ERR_INVALID)
 int server_check_queue_rows(const ServerCore* s, const char* records);
 // Allocates the staging (one record per environment in the queue's field order), the word block and the host mirror
-// of t, and registers the exchange block (mapped, portable) on the engine's device.  On failure the caller releases
+// of t, and registers the exchange block's server_exchange_bytes(num_envs, report_bytes) (mapped, portable) on the
+// engine's device.  On failure the caller releases
 // the server (server_core_release), keeping the error message.
 int server_core_init(ServerCore* s, void* exchange);
 // waits for the engine's stream, destroys the graphs, frees what server_core_init and dev_alloc made and unregisters

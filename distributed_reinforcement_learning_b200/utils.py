@@ -6,7 +6,8 @@
   UnrolledTrajectory utils.py:80-119  (the actor-side accumulator whose ``extract()`` feeds ``FIFOQueue.append_to_queue``,
                                        train_impala.py:117,165-189: closes the actor -> ring -> learner loop)
   impala_env_step    (new) the IMPALA actor's rule for one environment step, shared by actor.VectorActor and the
-                     worker processes of actor_server.EnvWorkerPool
+                     worker processes of actor_server.EnvWorkerPool; it is the A3C actor's rule too, and the workers of
+                     actor_server.A3CEnvWorkerPool step under it
   r2d2_env_step      (new) the R2D2 actor's rule for one environment step, shared by actor.R2D2VectorActor and the
                      worker processes of actor_server.R2D2EnvWorkerPool
 """

@@ -545,6 +545,50 @@ int drl_a3c_policy_recorder_reset(drl_a3c_policy_recorder* r);
 int drl_a3c_policy_recorder_commit(drl_a3c_policy_recorder* r, const float* reward, const uint8_t* done,
                                    const uint8_t* next_state, int32_t timeout_ms);
 
+/* A3C policy server: one A3C engine (algo 1) serving num_envs environments (1..256) that step in other processes, with
+ * each environment's unfinished unroll on the GPU (DESIGN.md section 18).  It binds one engine, one device A3C queue and
+ * an exchange block as the IMPALA policy server does, and keeps a device state table (per environment: the previous
+ * action and t, the step of the current unroll the next act records) and a device staging of one unroll per
+ * environment in the queue's record layout (1,806,752 B per environment at T = 32).
+ *
+ * Exchange block (page-aligned, at least drl_a3c_policy_server_exchange_bytes(num_envs) bytes): num_envs report
+ * records, then num_envs reply records, every field 16-byte aligned.  Before environment e is served, its report holds
+ * the frame the next action is for, the uniform draw the action is sampled with (as drl_a3c_policy_act's `uniform`),
+ * the reward and done flag the environment gave for its previous action, and `reset` = 1 when the episode restarted
+ * (the previous action taken as 0) or it is the environment's first act.  When `reset` follows a step, next_state holds
+ * the frame env.step returned for the previous action (the frame to act on is then the new episode's first frame); the
+ * server reads it only then.  After the serve its reply holds the action and max_prob = policy[action]. */
+#define DRL_A3C_SERVER_REPORT_FRAME 0          /* u8 [84,84,4]  */
+#define DRL_A3C_SERVER_REPORT_NEXT_STATE 28224 /* u8 [84,84,4]  */
+#define DRL_A3C_SERVER_REPORT_UNIFORM 56448    /* f64, in [0, 1) */
+#define DRL_A3C_SERVER_REPORT_REWARD 56464     /* f32            */
+#define DRL_A3C_SERVER_REPORT_DONE 56480       /* u8             */
+#define DRL_A3C_SERVER_REPORT_RESET 56496      /* u8             */
+#define DRL_A3C_SERVER_REPORT_BYTES 56512
+#define DRL_A3C_SERVER_REPLY_ACTION 0          /* i32            */
+#define DRL_A3C_SERVER_REPLY_MAX_PROB 16       /* f32            */
+#define DRL_A3C_SERVER_REPLY_BYTES 32
+typedef struct drl_a3c_policy_server drl_a3c_policy_server;
+/* num_envs * (REPORT_BYTES + REPLY_BYTES) rounded up to 4096; DRL_ERR_INVALID for num_envs outside [1, 256] */
+int drl_a3c_policy_server_exchange_bytes(int32_t num_envs, int64_t* bytes);
+/* Registers the exchange block with CUDA (mapped, portable) until destroy.  The engine must be an A3C engine (algo 1),
+ * queue and engine on the same device with the same num_action, the queue must take min(num_envs, max_batch) records at
+ * once, and the block must be page-aligned and large enough; all DRL_ERR_INVALID otherwise.  Without a device,
+ * DRL_ERR_CUDA.  Destroy the server before its engine and queue; after that the block may be registered again. */
+int drl_a3c_policy_server_create(drl_a3c_policy* h, drl_a3c_queue* queue, int32_t num_envs, void* exchange,
+                                 int64_t exchange_bytes, drl_a3c_policy_server** out);
+int drl_a3c_policy_server_destroy(drl_a3c_policy_server* s);
+/* Serves the n <= max_batch distinct environments env_ids (any subset of [0, num_envs), any order; DRL_ERR_INVALID
+ * otherwise) from their reports, in one act of the engine on its stream: the reward, done and next_state of each one's
+ * previous step land in its staged unroll, every unroll whose step T-1 that completes is appended to the queue (in
+ * env_ids order), then the act records step t of each environment (state, previous action, action) and writes its
+ * reply.  The uniform is read on the device only; the action is clamped to [0, A) whatever its value.  Blocks while
+ * the queue has no room for the completed unrolls (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with nothing changed
+ * otherwise).  Synchronous: the replies are written on return.  With use_cuda_graph one graph per n replays the
+ * kernels.  A failure after the queue positions were reserved puts the queue into its failed state, as
+ * drl_policy_recorder_commit. */
+int drl_a3c_policy_server_serve(drl_a3c_policy_server* s, int32_t n, const int32_t* env_ids, int32_t timeout_ms);
+
 /* ------------------------------------------------------------------------------------------
  * Stand-alone V-trace (optimizer/vtrace.py), host-pointer convenience forms + device forms.
  * ------------------------------------------------------------------------------------------ */

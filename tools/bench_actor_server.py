@@ -21,6 +21,14 @@ the main thread:
   server  R2D2EnvWorkerPool of P workers x k environments, R2D2PolicyServer.run in a thread
 S = 15, burn-in 7, 84x84x1 frames, A = 4, B = 16, lstm 64, a replay memory filled with 4 batches before the timed
 blocks, CUDA graphs on.
+
+With `--family a3c` the same comparison for A3C (`python tools/bench_actor_server.py --family a3c --steps 64`): both
+arms feed one A3CDeviceFIFOQueue, and one learner step is a3c.Agent.train_from_queue of one unroll, in the main thread:
+  vector  A3CVectorActor over n environments in the learner's thread (one unroll of T steps, then every learner step
+          the queue holds a record for)
+  server  A3CEnvWorkerPool of P workers x k environments, A3CPolicyServer.run in a thread
+T = 32, A = 4, a queue of 4n records, CUDA graphs on.  Environment frames/s and learner steps/s are reported as the
+median and the 10th-90th percentiles over blocks.
 """
 import argparse
 import json
@@ -48,6 +56,14 @@ R2_SHAPE = (84, 84, 1)
 R2_FRAME = 84 * 84 * 1
 R2_VECTOR_H2D = R2_FRAME + 4 + 4 * R2_L + 4 * R2_L + 4 + 5   # act row (frame, pa, h, c, explore) + reward, done at commit
 R2_SERVER_REPORT_READ = R2_FRAME + 3 * 16 + 4          # frame + 16-byte reads of reward, done, reset + the host's explore
+
+
+# the A3C family
+A3_T, A3_A = 32, 4
+A3_VECTOR_H2D = FRAME + 4 + 8 + 4 + 1 + FRAME / A3_T   # act row (frame, pa, uniform) + reward, done and 1/T of the final
+                                                       # next_state frame at commit (episode-reset frames not counted)
+A3_SERVER_REPORT_READ = FRAME + 4 * 16                # frame + 16-byte reads of uniform, reward, done, reset (the
+                                                       # next_state frame after an episode end not counted)
 
 
 class BusyEnv:
@@ -362,9 +378,127 @@ def run_r2d2(n, workers, step_us, blocks, steps, profile_steps, seed):
     return out
 
 
+def pstats(v):
+    return dict(median=float(np.median(v)), p10=float(np.percentile(v, 10)), p90=float(np.percentile(v, 90)))
+
+
+def make_a3c_agent(name, params):
+    from distributed_reinforcement_learning_b200.agent import a3c
+    ag = a3c.Agent(SHAPE, A3_A, 0.99, 1e-4, 0.0, 1e9, 0.5, 0.01, 40.0, "abs_one", name, name)
+    ag.use_cuda_graph = True
+    ag._ensure_init()
+    ag._params = params.copy()
+    ag._get_engine(A3_T)
+    return ag
+
+
+def a3c_queue(n):
+    from distributed_reinforcement_learning_b200.distributed_queue.buffer_queue import A3CDeviceFIFOQueue
+    return A3CDeviceFIFOQueue(A3_T, SHAPE, A3_A, n, queue_size=4 * n)
+
+
+class A3CVectorArm:
+    def __init__(self, n, step_us, params):
+        from distributed_reinforcement_learning_b200.actor import A3CVectorActor
+        from distributed_reinforcement_learning_b200.apex_policy import NativeA3CPolicy
+        self.agent = make_a3c_agent("bench_a3c_vector_%d" % step_us, params)
+        self.queue = a3c_queue(n)
+        self.policy = NativeA3CPolicy(64, num_action=A3_A, input_shape=SHAPE)
+        self.actor = A3CVectorActor(self.policy, [make_env(i, step_us) for i in range(n)], self.queue, A3_T,
+                                    [A3_A] * n, learner=self.agent)
+        self.n = n
+
+    def block(self, steps):
+        t0, frames, done = time.perf_counter(), 0, 0
+        while done < steps:
+            self.actor.run_unroll()
+            frames += self.n * A3_T
+            while self.queue.get_size() >= 1 and done < steps:
+                self.agent.train_from_queue(self.queue)
+                done += 1
+        dt = time.perf_counter() - t0
+        return frames / dt, steps / dt
+
+    def close(self):
+        self.policy.close()
+        self.queue.close()
+
+
+class A3CServerArm(ServerArm):
+    def __init__(self, n, workers, step_us, params):
+        import functools
+        from distributed_reinforcement_learning_b200.actor_server import A3CEnvWorkerPool, A3CPolicyServer
+        from distributed_reinforcement_learning_b200.apex_policy import NativeA3CPolicy
+        self.agent = make_a3c_agent("bench_a3c_server_%d" % step_us, params)
+        self.queue = a3c_queue(n)
+        self.policy = NativeA3CPolicy(64, num_action=A3_A, input_shape=SHAPE)
+        self.pool = A3CEnvWorkerPool([functools.partial(make_env, i, step_us) for i in range(n)], [A3_A] * n,
+                                     n // workers, seeds=range(n))
+        self.server = A3CPolicyServer(self.policy, self.queue, self.pool, learner=self.agent)
+        self.errors = []
+
+    def block(self, steps):
+        """`steps` learner steps with the server running; it runs only inside blocks, and the records it queued
+        before one are trained on first, untimed."""
+        while self.queue.get_size() >= 1:
+            self.agent.train_from_queue(self.queue)
+        stop = threading.Event()
+        th = threading.Thread(target=self._run, args=(stop,))
+        t0, f0 = time.perf_counter(), self.served()
+        th.start()
+        try:
+            for _ in range(steps):
+                self.agent.train_from_queue(self.queue, timeout_ms=300000)
+            dt = time.perf_counter() - t0
+            frames = self.served() - f0
+        finally:
+            stop.set()
+            th.join()
+        if self.errors:
+            raise self.errors[0]
+        return frames / dt, steps / dt
+
+
+def run_a3c(n, workers, step_us, blocks, steps, profile_steps, seed):
+    from distributed_reinforcement_learning_b200.model import actor_critic
+    params = actor_critic.init_params(seed, num_action=A3_A, input_shape=SHAPE)
+    arms = dict(vector=A3CVectorArm(n, step_us, params), server=A3CServerArm(n, workers, step_us, params))
+    res = {k: dict(frames=[], steps=[]) for k in arms}
+    try:
+        for arm in arms.values():     # warm-up: graphs of every batch size met so far, the learner's first steps
+            arm.block(2)
+        sizes0 = dict(arms["server"].server.batch_sizes)
+        for _ in range(blocks):
+            for kind, arm in arms.items():
+                f, s = arm.block(steps)
+                res[kind]["frames"].append(f)
+                res[kind]["steps"].append(s)
+        sizes = {k: v - sizes0.get(k, 0) for k, v in sorted(arms["server"].server.batch_sizes.items())}
+        names = ("a3c_server_gather_kernel", "queue_commit_rows_kernel", "a3c_server_scatter_kernel")
+        kernels = server_kernel_ms(arms["server"], profile_steps, names) if profile_steps else None
+    finally:
+        for arm in arms.values():
+            arm.close()
+    words = 4 * (64 + 1 + 3 * 64)
+    served = sum(k * v for k, v in sizes.items())
+    serves = sum(sizes.values())
+    out = dict(bench="actor_server_a3c", n=n, workers=workers, envs_per_worker=n // workers, step_us=step_us,
+               trajectory=A3_T, num_action=A3_A, blocks=blocks, learner_steps_per_block=steps)
+    for kind in arms:
+        out[kind] = dict(env_frames_per_s=pstats(res[kind]["frames"]),
+                         learner_steps_per_s=pstats(res[kind]["steps"]))
+    out["vector"]["h2d_bytes_per_env_step"] = A3_VECTOR_H2D
+    out["server"].update(batch_sizes={str(k): v for k, v in sizes.items() if v},
+                         mean_batch=served / serves if serves else None,
+                         h2d_bytes_per_env_step=A3_SERVER_REPORT_READ + (words * serves / served if served else 0),
+                         kernels=kernels)
+    out.update(gpu_info())
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--family", choices=("impala", "r2d2"), default="impala")
+    ap.add_argument("--family", choices=("impala", "r2d2", "a3c"), default="impala")
     ap.add_argument("--n", type=int, default=32, help="environments")
     ap.add_argument("--workers", type=int, default=8, help="worker processes P (n / P environments each)")
     ap.add_argument("--step-us", default="0,200,1000", help="host work per environment step, microseconds")
@@ -378,7 +512,7 @@ def main():
     from distributed_reinforcement_learning_b200 import _native as N
     if N.device_count() < 1:
         raise SystemExit("needs a CUDA device (no CPU fallback)")
-    bench = run_r2d2 if a.family == "r2d2" else run
+    bench = dict(impala=run, r2d2=run_r2d2, a3c=run_a3c)[a.family]
     for us in [int(x) for x in a.step_us.split(",")]:
         print(json.dumps(bench(a.n, a.workers, us, a.blocks, a.steps, a.profile_steps, a.seed)), flush=True)
 

@@ -1,14 +1,16 @@
 """One tiny learner step per math mode for compute-sanitizer (memcheck / racecheck / synccheck of the mbarrier + wgmma
 pipelines), with --peer under torchrun the 2-GPU fused exchange (flag protocol over NVLink peer memory), and with
 --serve one eager serve loop of the IMPALA policy server (drl_policy_server_*: gather, per-row commit, act, scatter)
-over a registered exchange block the script fills itself, without worker processes, and with --serve-r2d2 the same for
-the R2D2 policy server (drl_r2d2_policy_server_*).
+over a registered exchange block the script fills itself, without worker processes, and with --serve-r2d2 and
+--serve-a3c the same for the R2D2 policy server (drl_r2d2_policy_server_*) and the A3C policy server
+(drl_a3c_policy_server_*).
 
     compute-sanitizer --tool memcheck  python tools/sanitize_step.py --modes 2 3
     compute-sanitizer --tool racecheck python tools/sanitize_step.py --modes 2
     torchrun --nproc-per-node 2 ... tools/sanitize_step.py --peer      (run each rank under compute-sanitizer)
     DRL_B200_CUDA_GRAPH=0 compute-sanitizer --tool memcheck python tools/sanitize_step.py --serve
     DRL_B200_CUDA_GRAPH=0 compute-sanitizer --tool memcheck python tools/sanitize_step.py --serve-r2d2
+    DRL_B200_CUDA_GRAPH=0 compute-sanitizer --tool memcheck python tools/sanitize_step.py --serve-a3c
 """
 import argparse
 import os
@@ -133,6 +135,73 @@ def serve_r2d2_loop(envs=6, max_batch=4, seq_len=3, unrolls=3, channels=1, num_a
           % (graph, unrolls * seq_len + 1, envs, envs * unrolls), flush=True)
 
 
+def serve_a3c_loop(envs=6, max_batch=4, trajectory=3, unrolls=3, num_action=4):
+    """Serves `envs` A3C environments for `unrolls` unrolls in random subsets of at most max_batch, with reset flags
+    (and next_state frames) now and then, and checks the committed unrolls' state and next_state frames and actions
+    against the reports and replies."""
+    import ctypes as C
+    import mmap
+    from distributed_reinforcement_learning_b200.actor_server import (A3CPolicyServer, a3c_exchange_bytes,
+                                                                      a3c_exchange_views)
+    from distributed_reinforcement_learning_b200.apex_policy import NativeA3CPolicy
+    from distributed_reinforcement_learning_b200.distributed_queue.buffer_queue import A3CDeviceFIFOQueue
+    from distributed_reinforcement_learning_b200.model import actor_critic as model
+
+    class Block:   # the exchange block of a pool, without workers
+        def __init__(self):
+            self.num_envs, self.exchange_bytes = envs, a3c_exchange_bytes(envs)
+            self.mem = mmap.mmap(-1, self.exchange_bytes)
+            self.anchor = C.c_char.from_buffer(self.mem)
+            self.address = C.addressof(self.anchor)
+            self.views = a3c_exchange_views(self.mem, envs)
+
+    shape = (84, 84, 4)
+    graph = os.environ.get("DRL_B200_CUDA_GRAPH", "1") != "0"
+    rng = np.random.RandomState(0)
+    pol = NativeA3CPolicy(max_batch, num_action=num_action, input_shape=shape, use_cuda_graph=graph)
+    pol.set_params(model.init_params(0, num_action=num_action, input_shape=shape))
+    q = A3CDeviceFIFOQueue(trajectory, shape, num_action, envs, queue_size=envs * unrolls)
+    blk = Block()
+    v = blk.views
+    server = A3CPolicyServer(pol, q, blk)
+    frames = {e: [] for e in range(envs)}
+    nexts = {e: [] for e in range(envs)}
+    actions = {e: [] for e in range(envs)}
+    for step in range(unrolls * trajectory + 1):
+        for e in range(envs):
+            v["frame"][e] = rng.randint(0, 256, shape)
+            reset = step == 0 or rng.rand() < 0.2
+            if reset and step > 0:
+                v["next_state"][e] = rng.randint(0, 256, shape)
+            v["uniform"][e] = rng.random_sample()
+            v["reward"][e], v["done"][e], v["reset"][e] = rng.randint(3), rng.rand() < 0.2, reset
+            if step > 0:
+                nexts[e].append((v["next_state"][e] if reset else v["frame"][e]).copy())
+            frames[e].append(v["frame"][e].copy())
+        ids = rng.permutation(envs).astype(np.int32)
+        k = 0
+        while k < envs:
+            c = rng.randint(1, max_batch + 1)
+            server.serve(ids[k:k + c])
+            k += c
+        assert ((v["action"][:envs] >= 0) & (v["action"][:envs] < num_action)).all()
+        for e in range(envs):
+            actions[e].append(int(v["action"][e]))
+    assert q.get_size() == envs * unrolls
+    T = trajectory
+    want = {(np.stack(frames[e][u * T:(u + 1) * T]).tobytes(), np.stack(nexts[e][u * T:(u + 1) * T]).tobytes(),
+             np.array(actions[e][u * T:(u + 1) * T], np.int32).tobytes())
+            for e in range(envs) for u in range(unrolls)}
+    got = {(r["state"].tobytes(), r["next_state"].tobytes(), r["action"].tobytes())
+           for r in (q.read(j) for j in range(envs * unrolls))}
+    assert got == want
+    server.close()
+    q.close()
+    pol.close()
+    print("a3c serve loop (cuda graph %s): %d serves of %d environments, %d unrolls committed ok"
+          % (graph, unrolls * trajectory + 1, envs, envs * unrolls), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--modes", type=int, nargs="*", default=[2])
@@ -143,12 +212,17 @@ def main():
     ap.add_argument("--serve", action="store_true", help="the policy server's serve loop instead of learner steps")
     ap.add_argument("--serve-r2d2", action="store_true",
                     help="the R2D2 policy server's serve loop instead of learner steps")
+    ap.add_argument("--serve-a3c", action="store_true",
+                    help="the A3C policy server's serve loop instead of learner steps")
     a = ap.parse_args()
     if a.serve:
         serve_loop()
         return
     if a.serve_r2d2:
         serve_r2d2_loop()
+        return
+    if a.serve_a3c:
+        serve_a3c_loop()
         return
     from distributed_reinforcement_learning_b200.learner import NativeLearner
     from distributed_reinforcement_learning_b200.model import impala_actor_critic as model
