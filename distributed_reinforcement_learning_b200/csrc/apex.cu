@@ -626,8 +626,24 @@ int drl_apex_read_buffer(drl_apex* h, const char* name, float* host_dst, int64_t
       {"a1", h->act.a1, M * 400 * 32}, {"a2", h->act.a2, M * 81 * 64}, {"a3", h->act.a3, M * Geo::FLAT},
       {"emb", h->act.table, A * Geo::EMB}, {"e1", h->act.e1, A * Geo::EMB},
       {"hid1", h->act.hid1, 2 * M * Geo::HID}, {"hid2", h->act.hid2, 2 * M * Geo::HID},
+      {"vstream", h->act.vstream, M * A}, {"mstream", h->act.mstream, M}, {"policy", h->act.scratch_sm, M * A},
+      {"dq", h->bwd.dq, Mb * 32}, {"dmean", h->bwd.dmean, Mb * 32},
+      {"dhid2", h->bwd.dhid2, 2 * Mb * Geo::HID}, {"dhid1", h->bwd.dhid1, 2 * Mb * Geo::HID},
+      {"du", h->bwd.du, Mb * Geo::EMB},
       {"da3", h->bwd.da3, Mb * Geo::FLAT}, {"da2", h->bwd.da2, Mb * 81 * 64}, {"da1", h->bwd.da1, Mb * 400 * 32}};
   return read_named_buffer(h, tab, sizeof(tab) / sizeof(tab[0]), name, host_dst, n);
+}
+
+// The launch plan of an Ape-X / A3C step over B transitions in math mode `mode` (forward rows 2B, backward rows B), read
+// by the per-kernel tests to assert which edges a case reaches: out[0] = split-K count of heads_l1_fwd, out[1..3] =
+// split-K count of the conv1 / conv2 / conv3 weight gradients.
+int drl_debug_apex_launch_plan(int32_t B, int32_t mode, int32_t* out) {
+  if (!out || B < 1 || mode < 1 || mode > 2) { set_error("apex_launch_plan: need out, B >= 1, mode 1 or 2"); return DRL_ERR_INVALID; }
+  out[0] = plan_head1(2 * B).splits;
+  out[1] = plan_conv1_wgrad(B, mode).splits;
+  out[2] = plan_conv2_wgrad(B, mode).splits;
+  out[3] = plan_conv3_wgrad(B, mode).splits;
+  return DRL_OK;
 }
 
 int drl_apex_profile_step(drl_apex* h, int32_t slot, char* names, int64_t names_len, float* ms, int32_t max_kernels,

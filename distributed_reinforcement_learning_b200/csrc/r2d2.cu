@@ -803,8 +803,28 @@ int drl_r2d2_read_buffer(drl_r2d2* h, const char* name, float* host_dst, int64_t
       {"emb", h->act.table, A * Geo::EMB}, {"e1", h->act.e1, A * Geo::EMB}, {"q1", h->act.q1, M * kR2H},
       {"hout", h->act.hout, M * kR2L}, {"hin", h->act.hin, M * kR2L}, {"cin", h->act.cin, M * kR2L},
       {"gates", h->act.gates, M * kR2G}, {"dz", h->bwd.dz, M * kR2G}, {"dhout", h->bwd.dhout, M * kR2L},
-      {"da3", h->bwd.da3, M * Geo::FLAT}};
+      {"zx", h->act.zx, M * kR2G}, {"tc", h->act.tc, M * kR2L}, {"q", h->act.q, M * A},
+      {"dq", h->bwd.dq, M * 32}, {"dmean", h->bwd.dmean, M * 32}, {"dq1", h->bwd.dq1, M * kR2H},
+      {"du", h->bwd.du, M * Geo::EMB}, {"da3", h->bwd.da3, M * Geo::FLAT}, {"da2", h->bwd.da2, M * 81 * 64},
+      {"da1", h->bwd.da1, M * 400 * 32}};
   return read_named_buffer(h, tab, sizeof(tab) / sizeof(tab[0]), name, host_dst, n);
+}
+
+// The launch plan of an R2D2 step over B sequences of S steps of C-channel frames in math mode `mode` (M = B*S rows,
+// all of which receive gradient), read by the per-kernel tests to assert which edges a case reaches: out[0] = split-K
+// count of lstm_x_fwd, out[1..3] = split-K count of the conv1 / conv2 / conv3 weight gradients (conv1: the
+// single-channel plan when C == 1).
+int drl_debug_r2d2_launch_plan(int32_t B, int32_t S, int32_t C, int32_t mode, int32_t* out) {
+  if (!out || B < 1 || S < 1 || (C != 1 && C != 4) || mode < 1 || mode > 2) {
+    set_error("r2d2_launch_plan: need out, B >= 1, S >= 1, C 1 or 4, mode 1 or 2");
+    return DRL_ERR_INVALID;
+  }
+  const int M = B * S;
+  out[0] = plan_r2_x(M, mode).splits;
+  out[1] = C == 1 ? plan_conv1_wgrad_c1(M).splits : plan_conv1_wgrad(M, mode).splits;
+  out[2] = plan_conv2_wgrad(M, mode).splits;
+  out[3] = plan_conv3_wgrad(M, mode).splits;
+  return DRL_OK;
 }
 
 int drl_r2d2_profile_step(drl_r2d2* h, int32_t slot, char* names, int64_t names_len, float* ms, int32_t max_kernels,

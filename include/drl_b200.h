@@ -190,6 +190,14 @@ int drl_debug_gemm(int32_t core, int32_t bn, int32_t a_kmajor, int32_t b_kmajor,
  * out[0..2] = split-K count of the conv1 / conv2 / conv3 weight gradients, out[3] / out[4] = frames per CTA of the
  * persistent conv1 forward / weight-gradient kernels (math mode 5, else 0), out[5] = M tile of the 16-bit split core. */
 int drl_debug_launch_plan(int32_t B, int32_t T, int32_t mode, int32_t* out);
+/* Test aid: the launch plan of an Ape-X / A3C step over B transitions (forward rows 2B, backward rows B) in math mode 1
+ * or 2: out[0] = split-K count of the first head layer (heads_l1_fwd), out[1..3] = split-K count of the conv1 / conv2 /
+ * conv3 weight gradients. */
+int drl_debug_apex_launch_plan(int32_t B, int32_t mode, int32_t* out);
+/* Test aid: the launch plan of an R2D2 step over B sequences of S steps of C-channel frames (M = B*S rows) in math
+ * mode 1 or 2: out[0] = split-K count of the LSTM input contraction (lstm_x_fwd), out[1..3] = split-K count of the
+ * conv1 / conv2 / conv3 weight gradients (conv1: the single-channel plan when C == 1). */
+int drl_debug_r2d2_launch_plan(int32_t B, int32_t S, int32_t C, int32_t mode, int32_t* out);
 /* Test aid: CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor at the launch's block size and dynamic shared
  * memory) of the math-mode-5 kernels sized for two per SM: out[0] / out[1] = conv2 / conv3 forward, out[2] = conv2
  * data gradient. */

@@ -142,18 +142,12 @@ def gates_backward(dh, gates, c1, c0):
 def references(buf, p, batch, cfg, B, T, A):
     """{output name: float64 reference}, each computed from the GPU buffers its kernel read.
     ``p``: the parameters the step ran with (float64 torch tensors by name); ``batch``: the staged batch."""
-    M, Mb = B * T, B * (T - 2)
+    Mb = B * (T - 2)
     inp = device_inputs(batch)
     P = {k: v.detach().to(torch.float64) for k, v in p.items()}
-    ref = {}
+    ref = trunk_references(buf, P, inp["x"], inp["pa"], A, Mb)
     with torch.no_grad():
         # ---- forward -----------------------------------------------------------------------------------------
-        ref["a1"] = _np(torch.relu(it._conv2d_tf(_t(inp["x"]), P["conv1.w"], P["conv1.b"], 4)))
-        ref["a2"] = _np(torch.relu(it._conv2d_tf(_t(buf["a1"]), P["conv2.w"], P["conv2.b"], 2)))
-        ref["a3"] = _np(torch.relu(it._conv2d_tf(_t(buf["a2"]), P["conv3.w"], P["conv3.b"], 1))).reshape(M, FLAT)
-        acts = torch.arange(A)
-        ref["e1"] = _np(torch.relu(torch.nn.functional.one_hot(acts, A).to(torch.float64) @ P["emb1.w"] + P["emb1.b"]))
-        ref["emb"] = _np(torch.relu(_t(buf["e1"]) @ P["emb2.w"] + P["emb2.b"]))
         x = torch.cat([_t(buf["a3"]), _t(buf["emb"])[torch.from_numpy(inp["pa"])]], dim=1)
         h0, c0 = _t(inp["h0"]), _t(inp["c0"])
         z = torch.cat([x, h0], dim=1) @ P["lstm.w"] + P["lstm.b"]
@@ -195,11 +189,30 @@ def references(buf, p, batch, cfg, B, T, A):
     dx, ref["lstm.w"], ref["lstm.b"] = _dense(xb, W["lstm.w"], W["lstm.b"], buf["dz"])
     ref["da3"] = dx[:, :FLAT] * _mask(buf["a3"][:Mb])
     ref["du"] = dx[:, FLAT:FLAT + 256]
+    return ref
+
+
+def trunk_references(buf, P, x, pa, A, Mb):
+    """References of the conv trunk and the action embedding that the IMPALA, Ape-X / A3C and R2D2 learners share
+    (csrc/layer_defs.cuh): conv1-3 and the embedding forward from the GPU's own inputs to each layer, the embedding
+    weight gradients from the GPU's ``du`` at the GPU's e1 / table masks, the conv data and weight gradients from the
+    GPU's ``da3`` over the first ``Mb`` rows.  ``P``: float64 parameters by name; ``x``: the frames / 255 in device row
+    order ([M, 84, 84, C], any channel count C); ``pa``: the previous action of every device row."""
+    M = x.shape[0]
+    ref = {}
+    with torch.no_grad():
+        ref["a1"] = _np(torch.relu(it._conv2d_tf(_t(x), P["conv1.w"], P["conv1.b"], 4)))
+        ref["a2"] = _np(torch.relu(it._conv2d_tf(_t(buf["a1"]), P["conv2.w"], P["conv2.b"], 2)))
+        ref["a3"] = _np(torch.relu(it._conv2d_tf(_t(buf["a2"]), P["conv3.w"], P["conv3.b"], 1))).reshape(M, FLAT)
+        acts = torch.arange(A)
+        ref["e1"] = _np(torch.relu(torch.nn.functional.one_hot(acts, A).to(torch.float64) @ P["emb1.w"] + P["emb1.b"]))
+        ref["emb"] = _np(torch.relu(_t(buf["e1"]) @ P["emb2.w"] + P["emb2.b"]))
+    W = {k: _np(v) for k, v in P.items()}
     # ---- action embedding weight gradients (at the GPU's e1 / table masks) ---------------------------------------
     pe = {k: _t(W[k], True) for k in ("emb1.w", "emb1.b", "emb2.w", "emb2.b")}
     masks = {"e1": torch.from_numpy(buf["e1"] > 0), "emb": torch.from_numpy(buf["emb"] > 0)}
     with it.activation_pattern(masks):
-        rows = it.action_embedding(pe, torch.from_numpy(inp["pa"][:Mb]), A)
+        rows = it.action_embedding(pe, torch.from_numpy(np.asarray(pa)[:Mb]), A)
     grads = torch.autograd.grad(rows, list(pe.values()), _t(buf["du"]))
     ref.update({k: _np(g) for k, g in zip(pe, grads)})
     # ---- convolutions: data gradients from the GPU's upstream gradient, weight gradients ---------------------------
@@ -209,7 +222,7 @@ def references(buf, p, batch, cfg, B, T, A):
     ref["da2"] = dx * _mask(a2b)
     dx, ref["conv2.w"], ref["conv2.b"] = _conv_grads(a1b, W["conv2.w"], W["conv2.b"], 2, buf["da2"])
     ref["da1"] = dx * _mask(a1b)
-    _, ref["conv1.w"], ref["conv1.b"] = _conv_grads(inp["x"][:Mb], W["conv1.w"], W["conv1.b"], 4, buf["da1"])
+    _, ref["conv1.w"], ref["conv1.b"] = _conv_grads(x[:Mb], W["conv1.w"], W["conv1.b"], 4, buf["da1"])
     return ref
 
 
@@ -264,8 +277,9 @@ def _view2d(name, x):
     return x
 
 
-def errors(name, got, ref):
-    """(per-tensor error, worst block error, worst block label)."""
+def errors(name, got, ref, blocks_of=None):
+    """(per-tensor error, worst block error, worst block label); ``blocks_of``: the block function (default
+    ``blocks``)."""
     got = np.asarray(got, np.float64)
     ref = np.asarray(ref, np.float64)
     assert got.shape == ref.shape, (name, got.shape, ref.shape)
@@ -276,7 +290,7 @@ def errors(name, got, ref):
     tens = float(np.max(d)) / max(mx, 1e-30) if ref.size else 0.0
     g2, r2 = _view2d(name, d), _view2d(name, np.abs(ref))
     worst, label = 0.0, ""
-    for lab, idx in blocks(name, ref):
+    for lab, idx in (blocks_of or blocks)(name, ref):
         db, rb = g2[idx], r2[idx]
         if db.size == 0:
             continue
@@ -358,15 +372,17 @@ def bars(mode, B, T):
     return b
 
 
-def lstm_bounds(ref, c0, mode):
-    """Per-element bounds of the gates, c1 and h1 the LSTM kernels wrote, from the error model of lstm_fwd: a
-    pre-activation error of at most dz = bar * max|z| per element (K = 3648: the long-K bar of the core, relative to
-    max|z| like every GEMM bar here), carried through each nonlinearity by its derivative at the reference value
+def lstm_bounds(ref, c0, zbar):
+    """Per-element bounds of the gates, c1 and h1 the LSTM kernels wrote, from the error model of the contraction that
+    produced the pre-activation z: an error of at most dz = zbar * max|z| per element (IMPALA's lstm_fwd, K = 3648: the
+    long-K bar of its core; R2D2's recurrence: the K = 64 FFMA dot product; relative to max|z| like every GEMM bar
+    here), carried through each nonlinearity by its derivative at the reference value
     (sigmoid: s(1-s), tanh: 1-t^2; the second-order term |f''|/2 dz^2 <= dz^2), plus the float32 evaluation of the gate
     functions and of c1 = sf*c0 + si*tj, h1 = so*tanh(c1) (ELEM, relative to the magnitudes involved).  A saturated gate
     is held to ~ELEM: its derivative, and with it its share of the z error, vanishes."""
-    dz = (SPLIT16_LONGK if mode == 5 else TF32) * float(np.max(np.abs(ref["z"])))
+    dz = zbar * float(np.max(np.abs(ref["z"])))
     g = ref["gates"]
+    L = g.shape[1] // 4                 # the cell width (IMPALA 256, R2D2 64)
     si, tj, sf, so = g[:, :L], g[:, L:2 * L], g[:, 2 * L:3 * L], g[:, 3 * L:]
     deriv = np.concatenate([si * (1 - si), 1 - tj ** 2, sf * (1 - sf), so * (1 - so)], axis=1)
     eg = deriv * dz + dz ** 2 + ELEM
@@ -448,7 +464,7 @@ def run_case(mode, B, T, A, regime, seed=4242):
     inp = device_inputs(batch)
     got = gpu_outputs(buf, grads, A)
     bar = bars(mode, B, T)
-    per_element = dict(lstm_bounds(ref, inp["c0"], mode))
+    per_element = dict(lstm_bounds(ref, inp["c0"], SPLIT16_LONGK if mode == 5 else TF32))
     if mode == 5:
         per_element["a1"] = conv1_bound(inp["x"], p["conv1.w"], p["conv1.b"])
     rows = []

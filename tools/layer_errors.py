@@ -1,8 +1,11 @@
-"""Per-kernel error table of one IMPALA learner step: one JSON line per checked output with the kernel that wrote it, its
-per-tensor error, its worst block and the bar it is held to (tests/layer_parity.py; the same check as
-tests/test_gpu_layer_local.py).  A performance change can show with it which kernel's error moved.
+"""Per-kernel error table of one learner step: one JSON line per checked output with the kernel that wrote it, its
+per-tensor error, its worst block and the bar it is held to (tests/layer_parity.py for IMPALA, tests/adam_layer_parity.py
+for Ape-X, A3C and R2D2; the same checks as tests/test_gpu_layer_local.py and tests/test_gpu_adam_layer_local.py).  A
+performance change can show with it which kernel's error moved.
 
     python tools/layer_errors.py --mode 5 --B 32 --T 20 --A 18 --regime init [--regime trained ...]
+    python tools/layer_errors.py --family r2d2 --mode 2 --B 16 --T 80 --burn-in 40 --A 4 --C 1
+    python tools/layer_errors.py --family apex --mode 2 --B 32 --A 18 [--regime ties]
 """
 import argparse
 import json
@@ -13,24 +16,44 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
+import adam_layer_parity as alp  # noqa: E402
 import layer_parity as lp  # noqa: E402
+
+REGIMES = {"impala": lp.REGIMES, "apex": alp.APEX_REGIMES, "a3c": alp.A3C_REGIMES, "r2d2": alp.R2D2_REGIMES}
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--mode", type=int, default=5)
+    ap.add_argument("--family", choices=sorted(REGIMES), default="impala")
+    ap.add_argument("--mode", type=int, default=None, help="math mode (default: 5 for impala, 2 otherwise)")
     ap.add_argument("--B", type=int, default=32)
-    ap.add_argument("--T", type=int, default=20)
+    ap.add_argument("--T", type=int, default=20, help="trajectory (impala) or seq_len (r2d2)")
+    ap.add_argument("--burn-in", type=int, default=40, help="r2d2 only")
     ap.add_argument("--A", type=int, default=18)
-    ap.add_argument("--regime", action="append", choices=lp.REGIMES)
+    ap.add_argument("--C", type=int, default=1, help="r2d2 frame channels")
+    ap.add_argument("--regime", action="append")
     a = ap.parse_args()
+    mode = a.mode if a.mode is not None else (5 if a.family == "impala" else 2)
+    for r in a.regime or []:
+        if r not in REGIMES[a.family]:
+            ap.error("regime %r: %s has %s" % (r, a.family, ", ".join(REGIMES[a.family])))
     from distributed_reinforcement_learning_b200 import build
     build.build()
+    shape = dict(family=a.family, mode=mode, B=a.B, A=a.A)
+    if a.family in ("impala", "r2d2"):
+        shape["T"] = a.T
+    if a.family == "r2d2":
+        shape.update(burn_in=a.burn_in, C=a.C)
     for regime in a.regime or ["init"]:
-        rows, facts = lp.run_case(a.mode, a.B, a.T, a.A, regime)
+        if a.family == "impala":
+            rows, facts = lp.run_case(mode, a.B, a.T, a.A, regime)
+        elif a.family == "r2d2":
+            rows, facts = alp.run_r2d2_case(mode, a.B, a.T, a.burn_in, a.A, a.C, regime)
+        else:
+            rows, facts = alp.run_apex_case(a.family, mode, a.B, a.A, regime)
         for r in rows:
-            print(json.dumps(dict(mode=a.mode, B=a.B, T=a.T, A=a.A, regime=regime, **r)), flush=True)
-        print(json.dumps(dict(mode=a.mode, B=a.B, T=a.T, A=a.A, regime=regime, facts=facts)), flush=True)
+            print(json.dumps(dict(shape, regime=regime, **r)), flush=True)
+        print(json.dumps(dict(shape, regime=regime, facts=facts)), flush=True)
 
 
 if __name__ == "__main__":
