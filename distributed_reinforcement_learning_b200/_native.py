@@ -154,6 +154,8 @@ def _load():
         "drl_policy_sync_from_learner": (C.c_int, [vp, vp]),
         "drl_policy_act": (C.c_int, [vp, i32] + [vp] * 9),
         "drl_policy_last_act_ms": (C.c_int, [vp, C.POINTER(f32)]),
+        "drl_policy_read_buffer": (C.c_int, [vp, C.c_char_p, vp, i64]),
+        "drl_policy_buffer_dims": (C.c_int, [vp, vp]),
         "drl_r2d2_policy_create": (C.c_int, [C.POINTER(R2d2PolicyConfig), C.POINTER(vp)]),
         "drl_r2d2_policy_destroy": (C.c_int, [vp]),
         "drl_r2d2_policy_param_count": (C.c_int, [vp, C.POINTER(i64)]),
@@ -162,6 +164,8 @@ def _load():
         "drl_r2d2_policy_sync_from_learner": (C.c_int, [vp, vp]),
         "drl_r2d2_policy_act": (C.c_int, [vp, i32] + [vp] * 10),
         "drl_r2d2_policy_last_act_ms": (C.c_int, [vp, C.POINTER(f32)]),
+        "drl_r2d2_policy_read_buffer": (C.c_int, [vp, C.c_char_p, vp, i64]),
+        "drl_r2d2_policy_buffer_dims": (C.c_int, [vp, vp]),
         "drl_apex_policy_create": (C.c_int, [C.POINTER(ApexPolicyConfig), C.POINTER(vp)]),
         "drl_apex_policy_destroy": (C.c_int, [vp]),
         "drl_apex_policy_param_count": (C.c_int, [vp, C.POINTER(i64)]),
@@ -171,6 +175,8 @@ def _load():
         "drl_apex_policy_act": (C.c_int, [vp, i32] + [vp] * 6),
         "drl_a3c_policy_act": (C.c_int, [vp, i32] + [vp] * 6),
         "drl_apex_policy_last_act_ms": (C.c_int, [vp, C.POINTER(f32)]),
+        "drl_apex_policy_read_buffer": (C.c_int, [vp, C.c_char_p, vp, i64]),
+        "drl_apex_policy_buffer_dims": (C.c_int, [vp, vp]),
         "drl_vtrace_from_importance_weights": (C.c_int, [vp] * 5 + [i32, i32, f32, vp, vp]),
         "drl_vtrace_from_importance_weights_dev": (C.c_int, [vp] * 5 + [i32, i32, f32, vp, vp, vp]),
         "drl_vtrace_from_softmax": (C.c_int, [vp] * 7 + [i32, i32, i32, f32, vp, vp]),

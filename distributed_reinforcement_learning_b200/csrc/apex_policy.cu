@@ -434,6 +434,8 @@ int drl_apex_policy_create(const drl_apex_policy_config* cfg, drl_apex_policy** 
   h->off_sel = h->off_act + align_up(MB * 4, 256);
   const size_t out_bytes = h->off_sel + align_up(MB * 4, 256);
   const size_t N = cfg->algo == 0 ? ApexAlgo<0>::N : ApexAlgo<1>::N;
+  h->splits = kApexSplits;
+  h->zpart_cols = (int)N;
   const int rc = policy_core_init(h, set_apex_policy_kernel_attributes, kApexSplits * MB * N, apex_in_layout(MB).total,
                                   out_bytes);
   if (rc != DRL_OK) { delete h; return rc; }
@@ -455,6 +457,10 @@ int drl_apex_policy_sync_from_learner(drl_apex_policy* h, drl_apex* learner) {
   });
 }
 int drl_apex_policy_last_act_ms(drl_apex_policy* h, float* ms) { return policy_last_act_ms(h, kName, ms); }
+int drl_apex_policy_read_buffer(drl_apex_policy* h, const char* name, float* host_dst, int64_t n) {
+  return policy_read_buffer(h, kName, name, host_dst, n);
+}
+int drl_apex_policy_buffer_dims(drl_apex_policy* h, int32_t* out) { return policy_buffer_dims(h, kName, out); }
 
 int drl_apex_policy_act(drl_apex_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action,
                         const int32_t* explore_action, int32_t* action, float* q, float* q_action) {

@@ -433,6 +433,8 @@ int drl_policy_create(const drl_policy_config* cfg, drl_policy** out) {
   h->max_batch = cfg->max_batch;
   h->A = cfg->num_action;
   h->use_cuda_graph = cfg->use_cuda_graph != 0;
+  h->splits = kLSplits;
+  h->zpart_cols = Geo::G4;
   h->pl.init(h->A);
   h->layout = &h->pl;
   h->enqueue_act = enqueue_act;
@@ -465,6 +467,10 @@ int drl_policy_sync_from_learner(drl_policy* h, drl_learner* learner) {
   });
 }
 int drl_policy_last_act_ms(drl_policy* h, float* ms) { return policy_last_act_ms(h, kName, ms); }
+int drl_policy_read_buffer(drl_policy* h, const char* name, float* host_dst, int64_t n) {
+  return policy_read_buffer(h, kName, name, host_dst, n);
+}
+int drl_policy_buffer_dims(drl_policy* h, int32_t* out) { return policy_buffer_dims(h, kName, out); }
 
 int drl_policy_act(drl_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action, const float* h_in,
                    const float* c_in, const double* uniform, int32_t* action, float* policy, float* h_out,

@@ -105,6 +105,7 @@ int policy_run_act(PolicyCore* h, int n) {
   DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->stream));
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
   h->timed = true;
+  h->last_n = n;
   return DRL_OK;
 }
 
@@ -197,6 +198,38 @@ int policy_last_act_ms(PolicyCore* h, const char* family, float* ms) {
   return DRL_OK;
 }
 
+int policy_read_buffer(PolicyCore* h, const char* family, const char* name, float* host_dst, int64_t n) {
+  DRL_TRY(policy_check(h, family));
+  Lock lk(h->mu);
+  if (!name || !host_dst) { set_error("null argument"); return DRL_ERR_INVALID; }
+  if (h->last_n < 1) { set_error("read_buffer: no act call has run yet"); return DRL_ERR_STATE; }
+  const size_t m = h->last_n, A = h->A;
+  const struct { const char* name; const float* p; size_t count; } tab[] = {
+      {"a1", h->a1, m * 400 * 32}, {"a2", h->a2, m * 81 * 64}, {"a3", h->a3, m * Geo::FLAT},
+      {"e1", h->e1, A * Geo::EMB}, {"table", h->table, A * Geo::EMB},
+      {"zpart", h->zpart, (size_t)h->splits * m * h->zpart_cols}};
+  for (const auto& e : tab) {
+    if (strcmp(e.name, name) != 0) continue;
+    if ((size_t)n != e.count) { set_error("read_buffer(%s): expected %zu floats, got %lld", name, e.count, (long long)n); return DRL_ERR_INVALID; }
+    DRL_CUDA_CHECK(cudaSetDevice(h->device));
+    DRL_CUDA_CHECK(cudaMemcpyAsync(host_dst, e.p, e.count * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
+    return DRL_OK;
+  }
+  set_error("read_buffer: unknown buffer '%s'", name);
+  return DRL_ERR_INVALID;
+}
+
+int policy_buffer_dims(PolicyCore* h, const char* family, int32_t* out) {
+  DRL_TRY(policy_check(h, family));
+  Lock lk(h->mu);
+  if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
+  out[0] = h->last_n;
+  out[1] = h->splits;
+  out[2] = h->zpart_cols;
+  return DRL_OK;
+}
+
 // ---- recorders ---------------------------------------------------------------------------------------------------
 int recorder_core_init(RecorderCore* r) {
   DRL_CUDA_CHECK(cudaSetDevice(r->engine->device));
@@ -247,6 +280,7 @@ int recorder_run_act(RecorderCore* r, const std::function<int()>& enqueue_step) 
   DRL_CUDA_CHECK(cudaEventRecord(h->ev_stop, h->stream));
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->stream));
   h->timed = true;
+  h->last_n = r->n;
   r->t++;
   return DRL_OK;
 }

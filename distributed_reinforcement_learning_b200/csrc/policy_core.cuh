@@ -28,6 +28,7 @@ struct PolicyCore {
   std::recursive_mutex mu;
   // set by the family before policy_core_init
   int device = 0, max_batch = 0, A = 0;
+  int splits = 0, zpart_cols = 0;         // zpart is [splits][n][zpart_cols] for an act of n rows
   bool use_cuda_graph = false;
   const TrunkLayout* layout = nullptr;    // the family's layout (the learner's)
   EnqueueAct enqueue_act = nullptr;
@@ -37,6 +38,7 @@ struct PolicyCore {
   cudaEvent_t ev_ready = nullptr, ev_copied = nullptr;   // learner -> policy and policy -> learner edges of a sync
   cudaEvent_t ev_start = nullptr, ev_stop = nullptr;     // device time of the last act
   bool timed = false;
+  int last_n = 0;                // rows of the most recent act or recorder act (0: none yet), for policy_read_buffer
   float* params = nullptr;       // padded flat vector (learner layout)
   uint8_t* img_conv2 = nullptr;  // conv2 / conv3 forward weight images
   uint8_t* img_conv3 = nullptr;
@@ -92,5 +94,13 @@ int policy_get_params(PolicyCore* h, const char* family, float* host_flat, int64
 // apex_params_snapshot) of `learner` into params on the engine's stream, ordered by ev_ready / ev_copied
 int policy_sync(PolicyCore* h, const char* family, const void* learner, const std::function<int()>& snapshot);
 int policy_last_act_ms(PolicyCore* h, const char* family, float* ms);
+// Test aid: a copy of one buffer of the most recent act (policy_run_act or recorder_run_act, last_n rows) into host
+// memory, after the engine's stream: "a1" [n,20,20,32], "a2" [n,9,9,64], "a3" [n,3136], "e1" / "table" [A,256],
+// "zpart" [splits][n][zpart_cols].  n = element count (DRL_ERR_INVALID if it differs, or for an unknown name);
+// DRL_ERR_STATE before the first act.  A policy server's serve does not go through the act driver: it neither sets
+// last_n nor keeps these buffers as the last act left them.
+int policy_read_buffer(PolicyCore* h, const char* family, const char* name, float* host_dst, int64_t n);
+// out[0] = last_n (0 before the first act), out[1] = splits, out[2] = zpart_cols
+int policy_buffer_dims(PolicyCore* h, const char* family, int32_t* out);
 
 }  // namespace drl

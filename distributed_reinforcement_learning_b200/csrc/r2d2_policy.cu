@@ -424,6 +424,8 @@ int drl_r2d2_policy_create(const drl_r2d2_policy_config* cfg, drl_r2d2_policy** 
   h->max_batch = cfg->max_batch;
   h->A = cfg->num_action;
   h->use_cuda_graph = cfg->use_cuda_graph != 0;
+  h->splits = kR2Splits;
+  h->zpart_cols = kR2G;
   h->frame = (size_t)Geo::IH * Geo::IW * cfg->channels;
   h->pl.init(h->A, cfg->channels);
   h->layout = &h->pl;
@@ -456,6 +458,10 @@ int drl_r2d2_policy_sync_from_learner(drl_r2d2_policy* h, drl_r2d2* learner) {
   });
 }
 int drl_r2d2_policy_last_act_ms(drl_r2d2_policy* h, float* ms) { return policy_last_act_ms(h, kName, ms); }
+int drl_r2d2_policy_read_buffer(drl_r2d2_policy* h, const char* name, float* host_dst, int64_t n) {
+  return policy_read_buffer(h, kName, name, host_dst, n);
+}
+int drl_r2d2_policy_buffer_dims(drl_r2d2_policy* h, int32_t* out) { return policy_buffer_dims(h, kName, out); }
 
 int drl_r2d2_policy_act(drl_r2d2_policy* h, int32_t n, const uint8_t* state, const int32_t* previous_action,
                         const float* h_in, const float* c_in, const int32_t* explore_action, int32_t* action, float* q,

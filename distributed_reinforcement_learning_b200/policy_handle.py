@@ -83,6 +83,25 @@ class PolicyHandle:
         N.check(self._fn("last_act_ms")(self._h, C.byref(ms)))
         return float(ms.value)
 
+    # ---- test aids -------------------------------------------------------------------
+    def buffer_dims(self):
+        """(n, splits, N): the rows of the most recent act (0 before the first) and the split count and columns of its
+        "zpart" buffer."""
+        out = (C.c_int32 * 3)()
+        N.check(self._fn("buffer_dims")(self._h, out))
+        return int(out[0]), int(out[1]), int(out[2])
+
+    def read_buffer(self, name):
+        """A float32 copy of one buffer of the most recent act (n rows), in device layout: "a1" [n, 20, 20, 32], "a2"
+        [n, 9, 9, 64], "a3" [n, 3136], "e1" / "table" [A, 256], "zpart" [splits, n, N] (the first skinny GEMM's
+        partial sums per K split)."""
+        n, splits, cols = self.buffer_dims()
+        shape = {"a1": (n, 20, 20, 32), "a2": (n, 9, 9, 64), "a3": (n, 3136), "e1": (self.A, 256),
+                 "table": (self.A, 256), "zpart": (splits, n, cols)}.get(name, (0,))
+        a = np.empty(int(np.prod(shape)), np.float32)
+        N.check(self._fn("read_buffer")(self._h, name.encode(), N.ptr(a), a.size))
+        return a.reshape(shape)
+
     # ---- inputs ----------------------------------------------------------------------
     def _inputs(self, state, previous_action):
         """-> n, state uint8 [n] + input_shape, previous_action int32 [n] in [0, A), as C-contiguous arrays."""

@@ -255,6 +255,17 @@ int drl_policy_act(drl_policy* h, int32_t n, const uint8_t* state, const int32_t
                    float* c_out);
 /* Device time of the most recent drl_policy_act (input copy + kernels; CUDA events on the policy's stream), ms. */
 int drl_policy_last_act_ms(drl_policy* h, float* ms);
+/* Test aid: read of an internal buffer of the most recent act or recorder act (n rows) by name into host memory
+ * (float32, device layout), after the engine's stream: "a1" [n,20,20,32], "a2" [n,9,9,64], "a3" [n,3136] (the conv
+ * activations), "e1" [A,256] (relu of the first embedding layer), "table" [A,256] (the action-embedding table),
+ * "zpart" [splits][n][N] (the per-split partial sums of the first skinny GEMM; drl_policy_buffer_dims gives splits and
+ * N).  count = element count; a wrong count or an unknown name is DRL_ERR_INVALID, a read before the first act
+ * DRL_ERR_STATE.  A policy server's serve is not an act here: it leaves n as it was and overwrites the buffers.  The
+ * same holds for drl_r2d2_policy_read_buffer and drl_apex_policy_read_buffer. */
+int drl_policy_read_buffer(drl_policy* h, const char* name, float* host_dst, int64_t count);
+/* out[0] = n of the most recent act (0: none yet), out[1] = splits, out[2] = N of "zpart": IMPALA 16 and 1024, R2D2
+ * 48 and 256, Ape-X 53 and 512 (value stream, then mean stream), A3C 53 and 256. */
+int drl_policy_buffer_dims(drl_policy* h, int32_t* out);
 
 /* Recorder: binds an engine to a device trajectory queue (drl_traj_queue_create below) for n <= max_batch rows, with
  * device staging of n trajectories of the queue's T steps (39 MB at n = 64, T = 20).  Queue and engine must be on the
@@ -365,6 +376,9 @@ int drl_r2d2_policy_act(drl_r2d2_policy* h, int32_t n, const uint8_t* state, con
                         float* q_action, float* h_out, float* c_out);
 /* Device time of the most recent drl_r2d2_policy_act (input copy + kernels; CUDA events on the policy's stream), ms. */
 int drl_r2d2_policy_last_act_ms(drl_r2d2_policy* h, float* ms);
+/* Test aids: as drl_policy_read_buffer and drl_policy_buffer_dims. */
+int drl_r2d2_policy_read_buffer(drl_r2d2_policy* h, const char* name, float* host_dst, int64_t count);
+int drl_r2d2_policy_buffer_dims(drl_r2d2_policy* h, int32_t* out);
 
 /* ------------------------------------------------------------------------------------------
  * Device R2D2 sequence queue (new): R2D2FIFOQueue with its batch slots in GPU memory.  Producers are R2D2 policy
@@ -505,6 +519,9 @@ int drl_a3c_policy_act(drl_a3c_policy* h, int32_t n, const uint8_t* state, const
                        const double* uniform, int32_t* action, float* policy, float* prob_action);
 /* Device time of the most recent act call (input copy + kernels; CUDA events on the policy's stream), ms. */
 int drl_apex_policy_last_act_ms(drl_apex_policy* h, float* ms);
+/* Test aids: as drl_policy_read_buffer and drl_policy_buffer_dims (both algos). */
+int drl_apex_policy_read_buffer(drl_apex_policy* h, const char* name, float* host_dst, int64_t count);
+int drl_apex_policy_buffer_dims(drl_apex_policy* h, int32_t* out);
 
 /* ------------------------------------------------------------------------------------------
  * Device A3C trajectory queue (new, DESIGN.md section 15): A3CFIFOQueue with its records in GPU memory.  Producers are

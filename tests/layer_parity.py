@@ -192,12 +192,10 @@ def references(buf, p, batch, cfg, B, T, A):
     return ref
 
 
-def trunk_references(buf, P, x, pa, A, Mb):
-    """References of the conv trunk and the action embedding that the IMPALA, Ape-X / A3C and R2D2 learners share
-    (csrc/layer_defs.cuh): conv1-3 and the embedding forward from the GPU's own inputs to each layer, the embedding
-    weight gradients from the GPU's ``du`` at the GPU's e1 / table masks, the conv data and weight gradients from the
-    GPU's ``da3`` over the first ``Mb`` rows.  ``P``: float64 parameters by name; ``x``: the frames / 255 in device row
-    order ([M, 84, 84, C], any channel count C); ``pa``: the previous action of every device row."""
+def trunk_forward_references(buf, P, x, A, emb_key="emb"):
+    """The forward half of ``trunk_references`` (also the policy engines' trunk): conv1 from the frames ``x`` / 255,
+    conv2 / conv3 from the GPU's a1 / a2, the embedding's first layer from the parameters and its table from the GPU's
+    e1.  ``emb_key``: the name of the table (the learners' "emb", the policy engines' "table")."""
     M = x.shape[0]
     ref = {}
     with torch.no_grad():
@@ -206,7 +204,17 @@ def trunk_references(buf, P, x, pa, A, Mb):
         ref["a3"] = _np(torch.relu(it._conv2d_tf(_t(buf["a2"]), P["conv3.w"], P["conv3.b"], 1))).reshape(M, FLAT)
         acts = torch.arange(A)
         ref["e1"] = _np(torch.relu(torch.nn.functional.one_hot(acts, A).to(torch.float64) @ P["emb1.w"] + P["emb1.b"]))
-        ref["emb"] = _np(torch.relu(_t(buf["e1"]) @ P["emb2.w"] + P["emb2.b"]))
+        ref[emb_key] = _np(torch.relu(_t(buf["e1"]) @ P["emb2.w"] + P["emb2.b"]))
+    return ref
+
+
+def trunk_references(buf, P, x, pa, A, Mb):
+    """References of the conv trunk and the action embedding that the IMPALA, Ape-X / A3C and R2D2 learners share
+    (csrc/layer_defs.cuh): conv1-3 and the embedding forward from the GPU's own inputs to each layer, the embedding
+    weight gradients from the GPU's ``du`` at the GPU's e1 / table masks, the conv data and weight gradients from the
+    GPU's ``da3`` over the first ``Mb`` rows.  ``P``: float64 parameters by name; ``x``: the frames / 255 in device row
+    order ([M, 84, 84, C], any channel count C); ``pa``: the previous action of every device row."""
+    ref = trunk_forward_references(buf, P, x, A)
     W = {k: _np(v) for k, v in P.items()}
     # ---- action embedding weight gradients (at the GPU's e1 / table masks) ---------------------------------------
     pe = {k: _t(W[k], True) for k in ("emb1.w", "emb1.b", "emb2.w", "emb2.b")}
@@ -372,15 +380,17 @@ def bars(mode, B, T):
     return b
 
 
-def lstm_bounds(ref, c0, zbar):
+def lstm_bounds(ref, c0, zbar, dz=None):
     """Per-element bounds of the gates, c1 and h1 the LSTM kernels wrote, from the error model of the contraction that
     produced the pre-activation z: an error of at most dz = zbar * max|z| per element (IMPALA's lstm_fwd, K = 3648: the
     long-K bar of its core; R2D2's recurrence: the K = 64 FFMA dot product; relative to max|z| like every GEMM bar
-    here), carried through each nonlinearity by its derivative at the reference value
+    here) or, when given, the per-element bound ``dz`` (the policy engines' split sum, tests/policy_layer_parity.py),
+    carried through each nonlinearity by its derivative at the reference value
     (sigmoid: s(1-s), tanh: 1-t^2; the second-order term |f''|/2 dz^2 <= dz^2), plus the float32 evaluation of the gate
     functions and of c1 = sf*c0 + si*tj, h1 = so*tanh(c1) (ELEM, relative to the magnitudes involved).  A saturated gate
     is held to ~ELEM: its derivative, and with it its share of the z error, vanishes."""
-    dz = zbar * float(np.max(np.abs(ref["z"])))
+    if dz is None:
+        dz = zbar * float(np.max(np.abs(ref["z"])))
     g = ref["gates"]
     L = g.shape[1] // 4                 # the cell width (IMPALA 256, R2D2 64)
     si, tj, sf, so = g[:, :L], g[:, L:2 * L], g[:, 2 * L:3 * L], g[:, 3 * L:]
