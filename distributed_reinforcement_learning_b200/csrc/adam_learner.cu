@@ -11,8 +11,9 @@ namespace drl {
 // ------------------------------------------------------------------------------------------
 // Tail of the train op (agent/apex.py:70-75) with TF 1.14 semantics:
 //   lr    = polynomial_decay(start, global_step, decay_steps, end)      (float32, pre-increment step)
-//   g    <- g * clip * min(1/||g||, 1/clip)                              (clip_by_global_norm over the main variables;
-//                                                                         the target variables have gradient None)
+//   g    <- g * (clip * min(1/||g||, 1/clip) + (||g|| - ||g||))          (clip_by_global_norm over the main variables;
+//                                                                         the target variables have gradient None; a NaN
+//                                                                         or infinite norm makes every gradient NaN)
 //   alpha = lr * sqrt(1 - beta2_power) / (1 - beta1_power)               (ApplyAdam, float32)
 //   m    += (g - m)(1 - beta1) ; v += (g^2 - v)(1 - beta2) ; w -= m * alpha / (sqrt(v) + eps)
 //   beta powers *= beta ; global_step += 1
@@ -43,7 +44,7 @@ __global__ void __launch_bounds__(256) adam_prepare_kernel(AdamState o) {
       const float decay = (float)o.learning_frame;
       const float gs = fminf((float)step, decay);
       const float p = gs / decay;
-      const float lr = (o.start_lr - o.end_lr) * (1.0f - p) + o.end_lr;
+      const float lr = __fmul_rn(o.start_lr - o.end_lr, 1.0f - p) + o.end_lr;   // TF rounds the product: no FMA
       const float b1 = *o.b1p, b2 = *o.b2p;
       *o.lr_cur = lr;
       *o.alpha = lr * sqrtf(1.0f - b2) / (1.0f - b1);
@@ -68,7 +69,8 @@ __global__ void __launch_bounds__(256) adam_apply_kernel(AdamState o) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) s += red[i];
     const float norm = sqrtf(s) * o.grad_scale;
-    s_scale = ((o.clip_norm > 0.f) ? o.clip_norm * fminf(1.0f / norm, 1.0f / o.clip_norm) : 1.0f) * o.grad_scale;
+    s_scale = ((o.clip_norm > 0.f) ? o.clip_norm * fminf(1.0f / norm, 1.0f / o.clip_norm) + (norm - norm) : 1.0f) *
+              o.grad_scale;
     if (blockIdx.x == 0) {
       o.out[0] = o.loss[0] * o.grad_scale; o.out[1] = *o.lr_cur; o.out[2] = norm;
       o.out[3] = o.loss[1] * o.grad_scale; o.out[4] = o.loss[2] * o.grad_scale;          // A3C: baseline loss, entropy (zero for the DQN learners)

@@ -1,6 +1,7 @@
 // optimizer.cu -- the tail of the train op (agent/impala.py:95-100) with TF 1.14 semantics:
 //   lr    = polynomial_decay(start, global_step, decay_steps, end)  (power 1, evaluated in float32)
-//   g    <- g * clip * min(1/||g||_2, 1/clip)                        (tf.clip_by_global_norm over ALL params)
+//   g    <- g * (clip * min(1/||g||_2, 1/clip) + (||g|| - ||g||))   (tf.clip_by_global_norm over ALL params: a NaN or
+//                                                                      infinite norm makes every clipped gradient NaN)
 //   ms   <- ms + (1 - 0.99) (g^2 - ms)     (RMSProp slot initialised to ONES)
 //   w    <- w - lr * g / sqrt(ms + 0.1)     (epsilon INSIDE the sqrt, momentum 0, not centred; evaluated as
 //           lr * g * rsqrt(ms + 0.1) like TF's Eigen kernel -- rsqrt.approx is within 2 ulp and avoids the IEEE-division
@@ -33,12 +34,13 @@ __global__ void __launch_bounds__(256) sqnorm_partial_kernel(OptState o) {
     for (int i = 0; i < 8; ++i) s += red[i];
     o.norm_partials[blockIdx.x] = s;
     if (blockIdx.x == 0) {
-      // tf.train.polynomial_decay in float32 (agent/impala.py:96); uses the pre-increment step.
+      // tf.train.polynomial_decay in float32 (agent/impala.py:96); uses the pre-increment step.  TF rounds the product
+      // before it adds end_lr: __fmul_rn keeps the compiler from contracting the two into one FMA.
       const long long step = *o.step;
       const float decay = (float)o.learning_frame;
       const float gs = fminf((float)step, decay);
       const float p = gs / decay;
-      *o.lr_cur = (o.start_lr - o.end_lr) * (1.0f - p) + o.end_lr;
+      *o.lr_cur = __fmul_rn(o.start_lr - o.end_lr, 1.0f - p) + o.end_lr;
       *o.step = step + 1;                                                  // agent/impala.py:100
     }
   }
@@ -67,7 +69,8 @@ __global__ void __launch_bounds__(256) rmsprop_apply_kernel(OptState o) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) s += red[i];
     const float norm = sqrtf(s);
-    s_scale = o.clip_norm * fminf(1.0f / norm, 1.0f / o.clip_norm);        // tf.clip_by_global_norm
+    // tf.clip_by_global_norm: scale_for_finite + (norm - norm), so that a NaN or infinite norm gives a NaN scale
+    s_scale = o.clip_norm * fminf(1.0f / norm, 1.0f / o.clip_norm) + (norm - norm);
     if (blockIdx.x == 0) {
       const float pi = o.loss_sums[0], bl = o.loss_sums[1], en = o.loss_sums[2];
       o.out[0] = pi; o.out[1] = bl; o.out[2] = en; o.out[3] = *o.lr_cur; o.out[4] = norm;

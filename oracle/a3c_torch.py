@@ -149,9 +149,8 @@ class Learner:
         grads = torch.autograd.grad(out["total_loss"], [self.params[n] for n in names], allow_unused=True)
         g = OrderedDict((n, (gi if gi is not None else torch.zeros_like(self.params[n]))) for n, gi in zip(names, grads))
         lr = it.polynomial_decay_f32(c["start_learning_rate"], self.step, c["learning_frame"], c["end_learning_rate"])
-        gn = torch.sqrt(sum(torch.sum(v.double() ** 2) for v in g.values())).to(self.dtype)
-        clip = c["gradient_clip_norm"]
-        scale = clip * min(1.0 / float(gn), 1.0 / clip) if float(gn) > 0 else 1.0
+        gn = it.global_norm(g.values(), self.dtype)
+        scale = it.clip_scale(gn, c["gradient_clip_norm"])
         alpha = float(lr) * np.sqrt(1.0 - float(self.beta2_power)) / (1.0 - float(self.beta1_power))
         with torch.no_grad():
             for n, p in self.params.items():

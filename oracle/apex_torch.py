@@ -235,9 +235,8 @@ class Learner:
         lr = it.polynomial_decay_f32(c["start_learning_rate"], self.step, c["learning_frame"],
                                      c["end_learning_rate"])                                # :71
         # tf.clip_by_global_norm over the main variables (the target variables have gradient None and are skipped)
-        gn = torch.sqrt(sum(torch.sum(v.double() ** 2) for v in g.values())).to(self.dtype)
-        clip = c["gradient_clip_norm"]
-        scale = clip * min(1.0 / float(gn), 1.0 / clip) if float(gn) > 0 else 1.0
+        gn = it.global_norm(g.values(), self.dtype)
+        scale = it.clip_scale(gn, c["gradient_clip_norm"])
         # ApplyAdam (TF 1.14 training_ops): alpha = lr * sqrt(1 - beta2_power) / (1 - beta1_power);
         # m += (g - m)(1 - beta1); v += (g^2 - v)(1 - beta2); var -= m * alpha / (sqrt(v) + eps)
         b1p, b2p = float(self.beta1_power), float(self.beta2_power)

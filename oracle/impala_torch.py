@@ -325,6 +325,22 @@ def polynomial_decay_f32(start, step, decay_steps, end, power=1.0):
                       np.float32(np.power(np.float32(1.0) - p, np.float32(power))) + np.float32(end))
 
 
+def global_norm(grads, dtype):
+    """tf.global_norm of the gradient tensors ``grads``: the sum of squares is taken in float64 but overflows to inf
+    where a ``dtype`` sum would (TF sums in the variables' float32), so the norm is inf exactly when TF's is."""
+    ss = sum(torch.sum(v.double() ** 2) for v in grads)
+    return torch.sqrt(ss).to(dtype) if bool(torch.isfinite(ss.to(dtype))) else ss.to(dtype)
+
+
+def clip_scale(gn, clip):
+    """The factor tf.clip_by_global_norm (TF 1.14 clip_ops) multiplies every gradient by:
+    ``clip * min(1/norm, 1/clip) + (norm - norm)`` -- 1 for a zero norm, NaN for a NaN or infinite norm (TF's documented
+    error signal: every clipped gradient becomes NaN)."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        n = np.float64(gn)
+        return float(clip * np.minimum(1.0 / n, 1.0 / clip) + (n - n))
+
+
 class Learner:
     """agent/impala.py learner graph + Agent.train, on torch CPU.
 
@@ -406,10 +422,9 @@ class Learner:
                                 initial_h, initial_c)
         lr = polynomial_decay_f32(c["start_learning_rate"], self.step, c["learning_frame"],
                                   c["end_learning_rate"])                 # :96
-        # tf.clip_by_global_norm: scale = clip * min(1/norm, 1/clip)
-        gn = torch.sqrt(sum(torch.sum(v.double() ** 2) for v in g.values())).to(self.dtype)
-        clip = c["gradient_clip_norm"]
-        scale = clip * min(1.0 / float(gn), 1.0 / clip) if float(gn) > 0 else 1.0
+        # tf.clip_by_global_norm: scale = clip * min(1/norm, 1/clip) + (norm - norm)
+        gn = global_norm(g.values(), self.dtype)
+        scale = clip_scale(gn, c["gradient_clip_norm"])
         with torch.no_grad():
             for n, p in self.params.items():                              # RMSProp(decay .99, eps .1)
                 gc = g[n] * scale

@@ -17,7 +17,7 @@ Dockerfile:2):
   tf.scan                 sequential fold over axis 0 (``reverse`` honoured), ``back_prop=False`` => no gradient
   tf.train.RMSPropOptimizer  ms0 = 1, ms += (1-decay)(g^2 - ms), mom = momentum*mom + lr*g*rsqrt(ms+eps), var -= mom
   tf.train.AdamOptimizer  lr_t = lr*sqrt(1-b2^t)/(1-b1^t), var -= lr_t*m/(sqrt(v)+eps); beta powers updated after apply
-  tf.clip_by_global_norm  scale = clip*min(1/norm, 1/clip); None gradients ignored
+  tf.clip_by_global_norm  scale = clip*min(1/norm, 1/clip) + (norm - norm) (NaN for a non-finite norm); None gradients ignored
   tf.train.polynomial_decay  (lr-end)*(1-min(step,decay)/decay)^power + end
   variable_scope          default-name uniquification counters that are RESET for the sub-scopes when a scope is left
                           (``close_variable_subscopes``) -- this is what makes the reference's repeated
@@ -735,7 +735,8 @@ def clip_by_global_norm(t_list, clip_norm, use_norm=None, name=None):
     present = [(_f(t) if t is not None else None) for t in t_list]
     live = [t for t in present if t is not None]
     gnorm = Tensor(lambda ctx, *ts: torch.sqrt(sum(torch.sum(t * t) for t in ts)), live)
-    scale = Tensor(lambda ctx, n: clip_norm * torch.minimum(1.0 / n, torch.ones_like(n) / clip_norm), [gnorm])
+    # TF 1.14 clip_ops: scale_for_finite + (norm - norm), so a NaN or infinite norm makes every clipped gradient NaN
+    scale = Tensor(lambda ctx, n: clip_norm * torch.minimum(1.0 / n, torch.ones_like(n) / clip_norm) + (n - n), [gnorm])
     return [None if t is None else Tensor(lambda ctx, v, s: v * s, [t, scale]) for t in present], gnorm
 
 

@@ -45,7 +45,7 @@ def gpu_masks(eng, B, A):
 
 
 def adam_expected(p0, g, m0, v0, gn, clip, lr, b1p, b2p):
-    scale = clip * min(1.0 / gn, 1.0 / clip) if gn > 0 else 1.0
+    scale = it.clip_scale(gn, clip)
     gc = g * scale
     m = m0 + (gc - m0) * (1.0 - ax.BETA1)
     v = v0 + (gc * gc - v0) * (1.0 - ax.BETA2)

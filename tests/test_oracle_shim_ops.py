@@ -167,6 +167,25 @@ def test_clip_by_global_norm_and_polynomial_decay(tf):
         assert float(sess.run(lr)) == pytest.approx(float(exp), rel=1e-6)
 
 
+@pytest.mark.parametrize("bad", ["nan", "inf", "overflow", "zero"])
+def test_clip_by_global_norm_non_finite_and_zero_norms(tf, bad):
+    """TF 1.14 clip_ops: scale = clip * min(1/norm, 1/clip) + (norm - norm).  A NaN or infinite global norm (an element
+    NaN or infinite, or a sum of squares that overflows) makes every clipped tensor NaN; a zero norm leaves them as
+    they are."""
+    g1, g2 = np.zeros((3, 4)), np.linspace(-1.0, 1.0, 7) * (0.0 if bad == "zero" else 1.0)
+    if bad == "overflow":
+        g1[0, :2] = 1e155                           # each square is finite in float64, their sum is not
+    elif bad != "zero":
+        g1[1, 2] = float(bad)
+    clipped, norm = tf.clip_by_global_norm([tf.constant(g1), None, tf.constant(g2)], 40.0)
+    with np.errstate(all="ignore"):
+        c1, c2, n = tf.Session().run([clipped[0], clipped[2], norm])
+    if bad == "zero":
+        assert n == 0.0 and np.array_equal(c1, g1) and np.array_equal(c2, g2)
+    else:
+        assert not np.isfinite(n) and np.isnan(c1).all() and np.isnan(c2).all()
+
+
 def _quadratic(tf, w0):
     w = tf.get_variable("w", shape=list(w0.shape), initializer=tf.zeros_initializer())
     t = tf.placeholder(tf.float32, shape=list(w0.shape))
