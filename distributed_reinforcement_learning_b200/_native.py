@@ -284,6 +284,7 @@ def _load():
         "drl_r2d2_last_step_ms": (C.c_int, [vp, C.POINTER(f32)]),
         "drl_r2d2_stream": (C.c_int, [vp, C.POINTER(vp)]),
         "drl_r2d2_launches_per_step": (C.c_int, [vp, C.POINTER(i32)]),
+        "drl_r2d2_recurrence_clusters": (C.c_int, [vp] + [C.POINTER(i32)] * 3),
         "drl_per_create": (C.c_int, [i64, C.POINTER(vp)]),
         "drl_per_destroy": (C.c_int, [vp]),
         "drl_per_add": (C.c_int, [vp, C.c_double, C.POINTER(i64)]),
@@ -334,6 +335,7 @@ def _load():
         "drl_apex_policy_server_read": (C.c_int, [vp, i32, i64] + [vp] * 6),
         "drl_a3c_stage_from_queue": (C.c_int, [vp, i32, vp, i32]),
         "drl_r2d2_replay_create": (C.c_int, [i32, i64, i32, i32, i32, C.POINTER(vp)]),
+        "drl_r2d2_replay_create_lstm": (C.c_int, [i32, i64, i32, i32, i32, i32, C.POINTER(vp)]),
         "drl_r2d2_replay_destroy": (C.c_int, [vp]),
         "drl_r2d2_replay_add": (C.c_int, [vp, vp, i32] + [vp] * 8),
         "drl_r2d2_replay_add_from_queue": (C.c_int, [vp, vp, vp, i32]),

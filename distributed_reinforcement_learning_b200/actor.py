@@ -151,6 +151,9 @@ class R2D2VectorActor:
         if not 1 <= n <= policy.max_batch:
             raise ValueError("%d environments, the policy serves 1..%d per call" % (n, policy.max_batch))
         L = policy.L
+        if learner is not None and getattr(learner, "lstm_size", L) != L:
+            raise ValueError("the learner has lstm_size %d, the policy %d: the policy engine syncs from a learner of its "
+                             "own width" % (learner.lstm_size, L))
         self.buffers = [buffer_queue.R2D2TrajectoryBuffer(seq_len=self.seq_len) for _ in range(n)]
         self.states = [env.reset() for env in self.envs]
         self.previous_action = np.zeros(n, np.int32)

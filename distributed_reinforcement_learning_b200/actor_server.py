@@ -760,6 +760,9 @@ class R2D2PolicyServer(_ServerBase):
         if channels is not None and channels != queue.input_shape[2]:
             raise ValueError("R2D2PolicyServer: the pool's environments give 84x84x%d frames, the queue stores 84x84x%d"
                              % (channels, queue.input_shape[2]))
+        if learner is not None and getattr(learner, "lstm_size", policy.L) != policy.L:
+            raise ValueError("R2D2PolicyServer: the learner has lstm_size %d, the policy %d: the policy engine syncs "
+                             "from a learner of its own width" % (learner.lstm_size, policy.L))
         self._bind_and_create(policy, queue, pool, learner)
 
     def _learner_step(self):

@@ -14,6 +14,7 @@ the learner branch of ``train_r2d2.py:87-165`` runs on it unchanged, with the TF
   Agent.train_from_memory (new) Memory.sample + the minibatch lists + train + Memory.update (train_r2d2.py:122-162)
                        as one device-resident step -> (loss, td_error)
   Agent.main_q_value_test / target_q_value_test   agent/r2d2.py:193-217
+  Agent.save_weights / load_weights (new) both scopes and the Adam state in one .npz, as apex.Agent's
 """
 import os
 import random
@@ -188,6 +189,29 @@ class Agent:
         if self._engine is not None:
             self._push_state()
 
+    def save_weights(self, path):
+        self._ensure_init()
+        self._pull_state()
+        if not path.endswith(".npz"):
+            path = path + ".npz"
+        o = self._opt
+        np.savez(path, main=self._main, target=self._target, m=o["m"], v=o["v"], step=np.int64(o["step"]),
+                 beta1_power=np.float32(o["beta1_power"]), beta2_power=np.float32(o["beta2_power"]))
+
+    def load_weights(self, path):
+        if not path.endswith(".npz"):
+            path = path + ".npz"
+        z = np.load(path)
+        n = r2d2_lstm.param_count(**self._kw)
+        if z["main"].size != n:
+            raise ValueError("checkpoint has %d parameters per scope, this agent has %d (lstm_size %d)"
+                             % (z["main"].size, n, self.lstm_size))
+        self._main, self._target = z["main"].astype(np.float32), z["target"].astype(np.float32)
+        self._opt = dict(m=z["m"].astype(np.float32), v=z["v"].astype(np.float32), step=int(z["step"]),
+                         beta1_power=float(z["beta1_power"]), beta2_power=float(z["beta2_power"]))
+        if self._engine is not None:
+            self._push_state()
+
     def get_action(self, state, h, c, previous_action, epsilon):
         eng = self._engine if self._engine is not None else self._get_engine(1)
         q, h2, c2 = eng.act(self._u8(state)[None], np.asarray([previous_action], np.int32),
@@ -240,7 +264,8 @@ class DeviceMemory:
         self.agent = agent
         self.capacity = int(capacity)
         self.replay = NativeR2D2Replay(self.capacity, seq_len=agent.seq_len, num_action=agent.num_action,
-                                       input_shape=tuple(agent.input_shape), device=agent.device)
+                                       input_shape=tuple(agent.input_shape), device=agent.device,
+                                       lstm_size=agent.lstm_size)
 
     @staticmethod
     def _step0(x):

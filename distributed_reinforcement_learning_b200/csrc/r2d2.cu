@@ -10,13 +10,18 @@
 // persistent CTA per sequence keeps W_h in shared memory and walks the S steps (r2d2_lstm_fwd_kernel); BPTT is the
 // mirror image (r2d2_lstm_bwd_kernel, W_h^T in shared memory), after which every weight / data gradient is again one
 // batched GEMM over all M rows (all rows receive gradient: burn-in only slices the loss, agent/r2d2.py:64-68).
+// That holds at lstm_size 64; at 256 and 512, W_h (1 MB / 4 MB) is spread over a thread-block cluster instead
+// (r2d2_cluster.cuh), and the GEMMs take the width at run time.
 #include <string.h>
+
+#include <algorithm>
 
 #include <string>
 #include <vector>
 
 #include "adam_learner.cuh"
 #include "layer_defs.cuh"
+#include "r2d2_cluster.cuh"
 #include "r2d2_defs.cuh"
 
 namespace drl {
@@ -24,7 +29,7 @@ namespace drl {
 // [x | h_in]^T for the LSTM kernel gradient: feature index i < 3392 -> [a3 | emb] (as LstmAT), else h_in (device, time-major)
 struct R2XhAT {
   static constexpr bool kContigK = false;
-  const float* e; const float* table; const int* pa; const float* hin; RowMap map;
+  const float* e; const float* table; const int* pa; const float* hin; RowMap map; int L;
   struct Row { int i; };
   __device__ __forceinline__ Row row(int, int i) const { Row r; r.i = i; return r; }
   __device__ __forceinline__ float4 load(const Row& r, int m) const {
@@ -32,7 +37,7 @@ struct R2XhAT {
     const float* p;
     if (r.i < Geo::FLAT) p = e + (size_t)m * Geo::FLAT + r.i;
     else if (r.i < kR2Cat) p = table + (size_t)__ldg(pa + map.src(m)) * Geo::EMB + (r.i - Geo::FLAT);
-    else p = hin + (size_t)m * kR2L + (r.i - kR2Cat);
+    else p = hin + (size_t)m * L + (r.i - kR2Cat);
     return __ldg(reinterpret_cast<const float4*>(p));
   }
 };
@@ -54,8 +59,11 @@ struct R2XA {
   }
 };
 
-static SplitPlan plan_r2_x(int M, int mode) {
-  return mode >= 2 ? plan_split(kR2Cat, cdiv(M, 128), 32, 1) : plan_split(kR2Cat, cdiv(M, CfgMid::BM) * (kR2G / CfgMid::BN), 16, 1);
+// split-K plan of lstm_x_fwd ([M, 3392] x [3392, G = 4L]): about one wave over the M x N tiles (N: one 256-wide tensor-core
+// tile at L = 64, 4 or 8 at 256 / 512)
+static SplitPlan plan_r2_x(int M, int mode, int G) {
+  return mode >= 2 ? plan_split(kR2Cat, cdiv(M, 128) * cdiv(G, 256), 32, 1)
+                   : plan_split(kR2Cat, cdiv(M, CfgMid::BM) * (G / CfgMid::BN), 16, 1);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -359,10 +367,45 @@ int policy_conv_images_tf32(cudaStream_t s, const TrunkLayout& pl, const float* 
   return conv_images_tf32(s, pl, P, img_conv2, img_conv3);
 }
 
+// The recurrence at the handle's width: the one-CTA-per-sequence kernels at L = 64, a cluster kernel otherwise, with
+// as many clusters as there are R-sequence chunks, up to what the device places at once (drl_r2d2_create checks >= 1).
+template <int L>
+static cudaError_t lstm_fwd_cluster(cudaStream_t s, int max_clusters, const float* zx, const float* bias, const float* Wh,
+                                    const R2In& in, const R2Acts& act, float* c_last, int B, int S) {
+  using K = R2Clu<L>;
+  const int ncl = std::min(cdiv(B, K::R), max_clusters);
+  return launch_cluster_k(r2d2_lstm_fwd_cluster_kernel<L>, K::CL, ncl * K::CL, K::T, K::kFwdSmem, s, zx, bias, Wh, in.h0,
+                          in.c0, in.done, act.gates, act.tc, act.hout, act.hin, act.cin, c_last, B, S);
+}
+static cudaError_t lstm_fwd(cudaStream_t s, const drl_r2d2* h, const float* bias, const float* Wh, const R2In& in,
+                            const R2Acts& act, float* c_last, int B, int S) {
+  if (h->L == 256) return lstm_fwd_cluster<256>(s, h->clusters_fwd, act.zx, bias, Wh, in, act, c_last, B, S);
+  if (h->L == 512) return lstm_fwd_cluster<512>(s, h->clusters_fwd, act.zx, bias, Wh, in, act, c_last, B, S);
+  return launch_k(r2d2_lstm_fwd_kernel, B, kR2G, kR2FwdSmem, s, act.zx, 1, (size_t)0, bias, Wh, in.h0, in.c0, in.done,
+                  act.gates, act.tc, act.hout, act.hin, act.cin, c_last, B, S);
+}
+template <int L>
+static cudaError_t lstm_bwd_cluster(cudaStream_t s, int max_clusters, const R2Bwd& bw, const R2Acts& act, const float* Wh,
+                                    const uint8_t* done, int B, int S) {
+  using K = R2Clu<L>;
+  const int ncl = std::min(cdiv(B, K::R), max_clusters);
+  return launch_cluster_k(r2d2_lstm_bwd_cluster_kernel<L>, K::CL, ncl * K::CL, K::T, K::kBwdSmem, s, bw.dhout, act.gates,
+                          act.tc, act.cin, Wh, done, bw.dz, B, S);
+}
+static cudaError_t lstm_bwd(cudaStream_t s, const drl_r2d2* h, const R2Bwd& bw, const R2Acts& act, const float* Wh,
+                            const uint8_t* done, int B, int S) {
+  if (h->L == 256) return lstm_bwd_cluster<256>(s, h->clusters_bwd, bw, act, Wh, done, B, S);
+  if (h->L == 512) return lstm_bwd_cluster<512>(s, h->clusters_bwd, bw, act, Wh, done, B, S);
+  return launch_k(r2d2_lstm_bwd_kernel, B, kR2G, kR2BwdSmem, s, bw.dhout, act.gates, act.tc, act.cin, Wh, done, bw.dz, B,
+                  S);
+}
+
 // Forward of one scope over B sequences of S steps (rows m = t*B + b).  c_last (optional): un-masked c_t (act path).
-static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, const WeightImages& wi, const R2In& in,
+static int r2_forward(const drl_r2d2* h, const Streams& st, const float* P, const WeightImages& wi, const R2In& in,
                       const R2Acts& act, float* c_last, int B, int S, int mode, bool retile_fwd, bool retile_bwd, bool tgt,
                       int* launches) {
+  const R2Layout& pl = h->pl;
+  const int L = h->L, G = 4 * h->L;
   const int M = B * S;
   const RowMap map{B, S};
   int n = 0;
@@ -391,25 +434,23 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
                                            mode, tgt, images_ready, &n));
   DRL_TRY(join_from_side(st, 1));
   // input half of the LSTM contraction for all S steps at once: [M, 3392] x W[:3392, :4L] (split-K partial sums)
-  const SplitPlan sp = plan_r2_x(M, mode);
+  const SplitPlan sp = plan_r2_x(M, mode, G);
   {
     R2XA al{act.a3, act.table, in.pa, map};
-    PlainB bl{P + pl.lstm_w, kR2G, 0};
-    EpRaw<false> ep{act.zpart, kR2G, (size_t)M * kR2G, 1.0f, 0, kR2G};
-    GEMM(tgt ? "target_lstm_x_fwd" : "lstm_x_fwd", CfgMid, U256, al, bl, ep, M, kR2G, kR2Cat, sp.splits, sp.kchunk, sp.kchunk);
+    PlainB bl{P + pl.lstm_w, G, 0};
+    EpRaw<false> ep{act.zpart, G, (size_t)M * G, 1.0f, 0, G};
+    GEMM(tgt ? "target_lstm_x_fwd" : "lstm_x_fwd", CfgMid, U256, al, bl, ep, M, G, kR2Cat, sp.splits, sp.kchunk, sp.kchunk);
   }
   KERNEL(tgt ? "target_lstm_x_reduce" : "lstm_x_reduce",
-         splitk_reduce(s, act.zpart, (size_t)M * kR2G, sp.splits, act.zx, (size_t)M * kR2G), 1);
+         splitk_reduce(s, act.zpart, (size_t)M * G, sp.splits, act.zx, (size_t)M * G), 1);
   prof_mark(s, tgt ? "target_lstm_unroll_fwd" : "lstm_unroll_fwd");
-  DRL_CUDA_CHECK((launch_k(r2d2_lstm_fwd_kernel, B, kR2G, kR2FwdSmem, s, act.zx, 1, (size_t)0,
-                           P + pl.lstm_b, P + pl.lstm_w + (size_t)kR2Cat * kR2G, in.h0, in.c0, in.done, act.gates, act.tc,
-                           act.hout, act.hin, act.cin, c_last, B, S)));
+  DRL_CUDA_CHECK(lstm_fwd(s, h, P + pl.lstm_b, P + pl.lstm_w + (size_t)kR2Cat * G, in, act, c_last, B, S));
   ++n;
   {  // dense 128 ReLU (model/r2d2_lstm.py:50)
-    PlainA al{act.hout, kR2L, 0};
+    PlainA al{act.hout, L, 0};
     PlainB bl{P + pl.q1_w, kR2H, 0};
     EpBiasAct<true, true> ep{act.q1, kR2H, 0, P + pl.q1_b, 0, 1.0f};
-    GEMM_FFMA(tgt ? "target_q1_fwd" : "q1_fwd", CfgSmall, al, bl, ep, M, kR2H, kR2L, 1, kR2L, 0);
+    GEMM_FFMA(tgt ? "target_q1_fwd" : "q1_fwd", CfgSmall, al, bl, ep, M, kR2H, L, 1, L, 0);
   }
   prof_mark(s, tgt ? "target_q_out_fwd" : "q_out_fwd");
   DRL_CUDA_CHECK((launch_k(r2d2_out_kernel, cdiv(M, 4), 128, 0, s, act.q1, P + pl.value_w, P + pl.value_b, P + pl.mean_w,
@@ -419,8 +460,10 @@ static int r2_forward(const Streams& st, const R2Layout& pl, const float* P, con
   return DRL_OK;
 }
 
-static int r2_backward(const Streams& st, const R2Layout& pl, const float* P, const WeightImages& wi, float* G,
+static int r2_backward(const drl_r2d2* h, const Streams& st, const float* P, const WeightImages& wi, float* G,
                        const R2In& in, const R2Acts& act, const R2Bwd& bw, int B, int S, int mode, int* launches) {
+  const R2Layout& pl = h->pl;
+  const int L = h->L, NG = 4 * h->L;
   const int M = B * S;
   const RowMap map{B, S};
   cudaStream_t s = st.main;
@@ -446,36 +489,35 @@ static int r2_backward(const Streams& st, const R2Layout& pl, const float* P, co
     GEMM_FFMA("mean_wgrad", CfgSmall, al, bl, ep, kR2H, 32, M, 1, M, 0);
   }
   {  // d q1 kernel [L(+1), 128] = hout^T dq1
-    PlainAT al{act.hout, kR2L, 0};
+    PlainAT al{act.hout, L, 0};
     PlainB bl{bw.dq1, kR2H, 0};
-    EpRaw<true> ep{G + pl.q1_w, kR2H, 0, 1.0f, kR2L, kR2H};
-    GEMM_FFMA("q1_wgrad", CfgSmall, al, bl, ep, kR2L, kR2H, M, 1, M, 0);
+    EpRaw<true> ep{G + pl.q1_w, kR2H, 0, 1.0f, L, kR2H};
+    GEMM_FFMA("q1_wgrad", CfgSmall, al, bl, ep, L, kR2H, M, 1, M, 0);
   }
   s = st.main;
   {  // dhout = dq1 W1^T
     PlainA al{bw.dq1, kR2H, 0};
     PlainBT bl{P + pl.q1_w, kR2H, 0};
-    EpRaw<false> ep{bw.dhout, kR2L, 0, 1.0f, 0, kR2L};
-    GEMM_FFMA("q1_dgrad", CfgSmall, al, bl, ep, M, kR2L, kR2H, 1, kR2H, 0);
+    EpRaw<false> ep{bw.dhout, L, 0, 1.0f, 0, L};
+    GEMM_FFMA("q1_dgrad", CfgSmall, al, bl, ep, M, L, kR2H, 1, kR2H, 0);
   }
   prof_mark(s, "lstm_unroll_bwd");
-  DRL_CUDA_CHECK((launch_k(r2d2_lstm_bwd_kernel, B, kR2G, kR2BwdSmem, s, bw.dhout, act.gates, act.tc, act.cin,
-                           P + pl.lstm_w + (size_t)kR2Cat * kR2G, in.done, bw.dz, B, S)));
+  DRL_CUDA_CHECK(lstm_bwd(s, h, bw, act, P + pl.lstm_w + (size_t)kR2Cat * NG, in.done, B, S));
   ++n;
   DRL_TRY(fork_to_side(st, 3));
   s = side;
-  {  // d lstm kernel [3456(+1), 256] = [x | h_in]^T dz ; bias gradient = column sums of dz
-    R2XhAT al{act.a3, act.table, in.pa, act.hin, map};
-    PlainB bl{bw.dz, kR2G, 0};
-    EpRaw<true> ep{G + pl.lstm_w, kR2G, 0, 1.0f, kR2Cat + kR2L, kR2G};
-    GEMM("lstm_wgrad", CfgBig, U256, al, bl, ep, kR2Cat + kR2L, kR2G, M, 1, M, 0);
+  {  // d lstm kernel [3392 + L (+1), 4L] = [x | h_in]^T dz ; bias gradient = column sums of dz
+    R2XhAT al{act.a3, act.table, in.pa, act.hin, map, L};
+    PlainB bl{bw.dz, NG, 0};
+    EpRaw<true> ep{G + pl.lstm_w, NG, 0, 1.0f, kR2Cat + L, NG};
+    GEMM("lstm_wgrad", CfgBig, U256, al, bl, ep, kR2Cat + L, NG, M, 1, M, 0);
   }
   s = st.main;
   {  // d[a3 | emb] = dz W[:3392]^T
-    PlainA al{bw.dz, kR2G, 0};
-    PlainBT bl{P + pl.lstm_w, kR2G, 0};
+    PlainA al{bw.dz, NG, 0};
+    PlainBT bl{P + pl.lstm_w, NG, 0};
     EpLstmDx ep{bw.da3, act.a3, bw.du};
-    GEMM("lstm_dgrad", CfgMid, U128, al, bl, ep, M, kR2Cat, kR2G, 1, kR2G, 0);
+    GEMM("lstm_dgrad", CfgMid, U128, al, bl, ep, M, kR2Cat, NG, 1, NG, 0);
   }
   DRL_TRY(fork_to_side(st, 4));
   s = side;
@@ -502,11 +544,11 @@ int drl::enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, flo
     DRL_CUDA_CHECK(cudaEventRecord(h->ev_tfork, h->compute));
     DRL_CUDA_CHECK(cudaStreamWaitEvent(h->tmain, h->ev_tfork, 0));
   }
-  DRL_TRY(r2_forward(tst, h->pl, h->target, h->twi, in, h->tact, nullptr, nb, h->S, h->mode, h->target_images_stale, false,
+  DRL_TRY(r2_forward(h, tst, h->target, h->twi, in, h->tact, nullptr, nb, h->S, h->mode, h->target_images_stale, false,
                      true, launches));
   h->target_images_stale = false;
   if (h->par) DRL_CUDA_CHECK(cudaEventRecord(h->ev_tjoin, h->tmain));
-  DRL_TRY(r2_forward(st, h->pl, h->params, h->wi, in, h->act, nullptr, nb, h->S, h->mode, h->images_stale,
+  DRL_TRY(r2_forward(h, st, h->params, h->wi, in, h->act, nullptr, nb, h->S, h->mode, h->images_stale,
                      h->images_stale, false, launches));
   h->images_stale = false;
   if (h->par) DRL_CUDA_CHECK(cudaStreamWaitEvent(h->compute, h->ev_tjoin, 0));
@@ -528,18 +570,18 @@ namespace {
 constexpr const char* kName = "r2d2";
 
 int alloc_acts(drl_r2d2* h, R2Acts& a) {
-  const size_t M = (size_t)h->B * h->S, A = h->A;
+  const size_t M = (size_t)h->B * h->S, A = h->A, L = h->L, G = 4 * L;
   DRL_TRY(alloc_trunk_acts(h, a, M, A));
   size_t zmax = 0;
   for (int mode = 1; mode <= 2; ++mode)
-    for (int m = 1; m <= (int)M; ++m) zmax = std::max(zmax, (size_t)plan_r2_x(m, mode).splits * m * kR2G);
+    for (int m = 1; m <= (int)M; ++m) zmax = std::max(zmax, (size_t)plan_r2_x(m, mode, (int)G).splits * m * G);
   DRL_TRY(dev_alloc(h, &a.zpart, zmax));
-  DRL_TRY(dev_alloc(h, &a.zx, M * kR2G));
-  DRL_TRY(dev_alloc(h, &a.gates, M * kR2G));
-  DRL_TRY(dev_alloc(h, &a.tc, M * kR2L));
-  DRL_TRY(dev_alloc(h, &a.hout, M * kR2L));
-  DRL_TRY(dev_alloc(h, &a.hin, M * kR2L));
-  DRL_TRY(dev_alloc(h, &a.cin, M * kR2L));
+  DRL_TRY(dev_alloc(h, &a.zx, M * G));
+  DRL_TRY(dev_alloc(h, &a.gates, M * G));
+  DRL_TRY(dev_alloc(h, &a.tc, M * L));
+  DRL_TRY(dev_alloc(h, &a.hout, M * L));
+  DRL_TRY(dev_alloc(h, &a.hin, M * L));
+  DRL_TRY(dev_alloc(h, &a.cin, M * L));
   DRL_TRY(dev_alloc(h, &a.q1, M * kR2H));
   DRL_TRY(dev_alloc(h, &a.q, M * A));
   return DRL_OK;
@@ -549,7 +591,7 @@ int fwd_bwd(LearnerCore* core, int slot, int* launches) {
   drl_r2d2* h = static_cast<drl_r2d2*>(core);
   const R2In& in = h->in[slot];
   DRL_TRY(enqueue_forward_td(h, in, h->B, true, h->d_td + (size_t)slot * h->B, launches));
-  return r2_backward(h->streams(), h->pl, h->params, h->wi, h->grads, in, h->act, h->bwd, h->B, h->S, h->mode, launches);
+  return r2_backward(h, h->streams(), h->params, h->wi, h->grads, in, h->act, h->bwd, h->B, h->S, h->mode, launches);
 }
 
 // H2D of nb sequences into slot s on `stream` (fields that are null are skipped)
@@ -563,8 +605,8 @@ int stage_into(drl_r2d2* h, const R2In& s, cudaStream_t stream, int nb, int step
   DRL_CUDA_CHECK(cp(s.frames, state, n * h->frame));
   DRL_CUDA_CHECK(cp(s.pa, previous_action, n * 4));
   if (action) DRL_CUDA_CHECK(cp(s.action, action, n * 4));
-  DRL_CUDA_CHECK(cp(s.h0, h0, (size_t)nb * kR2L * 4));
-  DRL_CUDA_CHECK(cp(s.c0, c0, (size_t)nb * kR2L * 4));
+  DRL_CUDA_CHECK(cp(s.h0, h0, (size_t)nb * h->L * 4));
+  DRL_CUDA_CHECK(cp(s.c0, c0, (size_t)nb * h->L * 4));
   if (reward) DRL_CUDA_CHECK(cp(s.reward, reward, n * 4));
   if (done) DRL_CUDA_CHECK(cp(s.done, done, n));
   if (reward) DRL_CUDA_CHECK(cp(s.weight, weight ? weight : h->h_ones, (size_t)nb * 4));
@@ -582,7 +624,10 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
     set_error("only 84x84x1 (config.json:91) and 84x84x4 frames are supported (got %dx%dx%d)", cfg->height, cfg->width, cfg->channels);
     return DRL_ERR_INVALID;
   }
-  if (cfg->lstm_size != kR2L) { set_error("only lstm_size %d (config.json:93) is supported (got %d)", kR2L, cfg->lstm_size); return DRL_ERR_INVALID; }
+  if (cfg->lstm_size != kR2L && cfg->lstm_size != 256 && cfg->lstm_size != 512) {
+    set_error("lstm_size must be 64 (config.json:93), 256 or 512 (got %d)", cfg->lstm_size);
+    return DRL_ERR_INVALID;
+  }
   if (cfg->num_action < 2 || cfg->num_action > 32) { set_error("num_action must be in [2,32]"); return DRL_ERR_INVALID; }
   if (cfg->batch < 1) { set_error("batch must be >= 1"); return DRL_ERR_INVALID; }
   if (cfg->seq_len < 2 || cfg->burn_in < 0 || cfg->burn_in > cfg->seq_len - 2) {
@@ -597,27 +642,29 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
   h->num_slots = cfg->num_slots < 1 ? 2 : cfg->num_slots;
   h->use_cuda_graph = cfg->use_cuda_graph != 0;
   h->mode = (cfg->math_mode == 0) ? DRL_DEFAULT_MATH_MODE : cfg->math_mode;
-  h->B = cfg->batch; h->S = cfg->seq_len; h->A = cfg->num_action; h->C = cfg->channels;
+  h->B = cfg->batch; h->S = cfg->seq_len; h->A = cfg->num_action; h->C = cfg->channels; h->L = cfg->lstm_size;
   h->Nt = cfg->seq_len - cfg->burn_in - 1;
   h->frame = (size_t)Geo::IH * Geo::IW * h->C;
-  h->pl.init(h->A, h->C);
+  h->pl.init(h->A, h->C, h->L);
   h->layout = &h->pl;
   h->fwd_bwd = fwd_bwd;
   AdamState& o = h->opt;
   o.start_lr = cfg->learning_rate; o.end_lr = cfg->learning_rate; o.learning_frame = 1.0;   // constant (agent/r2d2.py:91)
   o.clip_norm = 0.0f;                                                                        // minimize(): no clipping
   int rc = [&]() -> int {
-    const size_t B = h->B, S = h->S, M = B * S, A = h->A;
+    const size_t B = h->B, S = h->S, M = B * S, A = h->A, L = h->L;
     size_t off = 0;
     const size_t o_fr = off; off = align_up(off + M * h->frame, 256);
     const size_t o_pa = off; off = align_up(off + M * 4, 256);
     const size_t o_ac = off; off = align_up(off + M * 4, 256);
-    const size_t o_h = off; off = align_up(off + M * kR2L * 4, 256);    // room for M rows: the act path stages n <= M states
-    const size_t o_c = off; off = align_up(off + M * kR2L * 4, 256);
+    const size_t o_h = off; off = align_up(off + M * L * 4, 256);    // room for M rows: the act path stages n <= M states
+    const size_t o_c = off; off = align_up(off + M * L * 4, 256);
     const size_t o_rw = off; off = align_up(off + M * 4, 256);
     const size_t o_dn = off; off = align_up(off + M, 256);
     const size_t o_wt = off; off = align_up(off + M * 4, 256);
     DRL_TRY(adam_learner_init(h, off, M));
+    if (L == 256) DRL_TRY(r2d2_cluster_setup<256>(&h->clusters_fwd, &h->clusters_bwd));
+    if (L == 512) DRL_TRY(r2d2_cluster_setup<512>(&h->clusters_fwd, &h->clusters_bwd));
     for (const LearnerSlot& s : h->slots)
       h->in.push_back(R2In{s.base + o_fr, reinterpret_cast<int32_t*>(s.base + o_pa),
                            reinterpret_cast<int32_t*>(s.base + o_ac), reinterpret_cast<float*>(s.base + o_h),
@@ -629,14 +676,14 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
     DRL_TRY(dev_alloc(h, &b.dq, M * 32));
     DRL_TRY(dev_alloc(h, &b.dmean, M * 32));
     DRL_TRY(dev_alloc(h, &b.dq1, M * kR2H));
-    DRL_TRY(dev_alloc(h, &b.dhout, M * kR2L));
-    DRL_TRY(dev_alloc(h, &b.dz, M * kR2G));
+    DRL_TRY(dev_alloc(h, &b.dhout, M * L));
+    DRL_TRY(dev_alloc(h, &b.dz, M * 4 * L));
     DRL_TRY(alloc_trunk_bwd(h, b, M, A, h->C, true));
     const size_t Nt = h->Nt;
     DRL_TRY(dev_alloc(h, &h->sav, B * Nt));
     DRL_TRY(dev_alloc(h, &h->target_value, B * Nt));
     DRL_TRY(dev_alloc(h, &h->td_dev, B));
-    DRL_TRY(dev_alloc(h, &h->c_last, M * kR2L));
+    DRL_TRY(dev_alloc(h, &h->c_last, M * L));
     DRL_CUDA_CHECK(cudaDeviceSynchronize());
     return DRL_OK;
   }();
@@ -701,6 +748,10 @@ int drl::r2d2_params_snapshot(drl_r2d2* h, int device, int num_action, int chann
               channels);
     return DRL_ERR_INVALID;
   }
+  if (h->L != kR2L) {
+    set_error("sync: the learner has lstm_size %d, the policy engine %d", h->L, kR2L);
+    return DRL_ERR_INVALID;
+  }
   return learner_params_snapshot(h, kName, device, dst_stream, dst, ev_ready, ev_copied);
 }
 
@@ -757,12 +808,12 @@ int drl_r2d2_act(drl_r2d2* h, int32_t n, const uint8_t* state, const int32_t* pr
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   DRL_TRY(stage_into(h, in, h->compute, n, 1, state, previous_action, nullptr, h_in, c_in, nullptr, nullptr, nullptr));
   in.done = nullptr;                                     // a single step: nothing is carried
-  DRL_TRY(r2_forward(h->streams(), h->pl, h->params, h->wi, in, h->act, h->c_last, n, 1, h->mode, h->images_stale,
+  DRL_TRY(r2_forward(h, h->streams(), h->params, h->wi, in, h->act, h->c_last, n, 1, h->mode, h->images_stale,
                      h->images_stale, false, nullptr));
   h->images_stale = false;
   if (q_value) DRL_CUDA_CHECK(cudaMemcpyAsync(q_value, h->act.q, (size_t)n * h->A * 4, cudaMemcpyDeviceToHost, h->compute));
-  if (h_out) DRL_CUDA_CHECK(cudaMemcpyAsync(h_out, h->act.hout, (size_t)n * kR2L * 4, cudaMemcpyDeviceToHost, h->compute));
-  if (c_out) DRL_CUDA_CHECK(cudaMemcpyAsync(c_out, h->c_last, (size_t)n * kR2L * 4, cudaMemcpyDeviceToHost, h->compute));
+  if (h_out) DRL_CUDA_CHECK(cudaMemcpyAsync(h_out, h->act.hout, (size_t)n * h->L * 4, cudaMemcpyDeviceToHost, h->compute));
+  if (c_out) DRL_CUDA_CHECK(cudaMemcpyAsync(c_out, h->c_last, (size_t)n * h->L * 4, cudaMemcpyDeviceToHost, h->compute));
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   h->last_n = 0;
   return DRL_OK;
@@ -797,13 +848,13 @@ int drl_r2d2_read_buffer(drl_r2d2* h, const char* name, float* host_dst, int64_t
   if (!name || !host_dst) { set_error("null argument"); return DRL_ERR_INVALID; }
   DRL_CUDA_CHECK(cudaSetDevice(h->device));
   if (h->last_n < 1) { set_error("read_buffer: no step or td_error call has run"); return DRL_ERR_STATE; }
-  const size_t M = (size_t)h->last_n * h->S, A = h->A;
+  const size_t M = (size_t)h->last_n * h->S, A = h->A, L = h->L;
   const NamedBuffer tab[] = {
       {"a1", h->act.a1, M * 400 * 32}, {"a2", h->act.a2, M * 81 * 64}, {"a3", h->act.a3, M * Geo::FLAT},
       {"emb", h->act.table, A * Geo::EMB}, {"e1", h->act.e1, A * Geo::EMB}, {"q1", h->act.q1, M * kR2H},
-      {"hout", h->act.hout, M * kR2L}, {"hin", h->act.hin, M * kR2L}, {"cin", h->act.cin, M * kR2L},
-      {"gates", h->act.gates, M * kR2G}, {"dz", h->bwd.dz, M * kR2G}, {"dhout", h->bwd.dhout, M * kR2L},
-      {"zx", h->act.zx, M * kR2G}, {"tc", h->act.tc, M * kR2L}, {"q", h->act.q, M * A},
+      {"hout", h->act.hout, M * L}, {"hin", h->act.hin, M * L}, {"cin", h->act.cin, M * L},
+      {"gates", h->act.gates, M * 4 * L}, {"dz", h->bwd.dz, M * 4 * L}, {"dhout", h->bwd.dhout, M * L},
+      {"zx", h->act.zx, M * 4 * L}, {"tc", h->act.tc, M * L}, {"q", h->act.q, M * A},
       {"dq", h->bwd.dq, M * 32}, {"dmean", h->bwd.dmean, M * 32}, {"dq1", h->bwd.dq1, M * kR2H},
       {"du", h->bwd.du, M * Geo::EMB}, {"da3", h->bwd.da3, M * Geo::FLAT}, {"da2", h->bwd.da2, M * 81 * 64},
       {"da1", h->bwd.da1, M * 400 * 32}};
@@ -820,7 +871,7 @@ int drl_debug_r2d2_launch_plan(int32_t B, int32_t S, int32_t C, int32_t mode, in
     return DRL_ERR_INVALID;
   }
   const int M = B * S;
-  out[0] = plan_r2_x(M, mode).splits;
+  out[0] = plan_r2_x(M, mode, kR2G).splits;
   out[1] = C == 1 ? plan_conv1_wgrad_c1(M).splits : plan_conv1_wgrad(M, mode).splits;
   out[2] = plan_conv2_wgrad(M, mode).splits;
   out[3] = plan_conv3_wgrad(M, mode).splits;
@@ -834,5 +885,14 @@ int drl_r2d2_profile_step(drl_r2d2* h, int32_t slot, char* names, int64_t names_
 int drl_r2d2_last_step_ms(drl_r2d2* h, float* ms) { return learner_last_step_ms(h, kName, ms); }
 int drl_r2d2_stream(drl_r2d2* h, void** stream) { return learner_stream(h, kName, stream); }
 int drl_r2d2_launches_per_step(const drl_r2d2* h, int32_t* n) { return learner_launches_per_step(h, kName, n); }
+
+int drl_r2d2_recurrence_clusters(const drl_r2d2* h, int32_t* cluster_size, int32_t* max_fwd, int32_t* max_bwd) {
+  DRL_TRY(check_handle(h, kName));
+  if (!cluster_size || !max_fwd || !max_bwd) { set_error("null argument"); return DRL_ERR_INVALID; }
+  *cluster_size = h->L == kR2L ? 0 : h->L / 32;
+  *max_fwd = h->clusters_fwd;
+  *max_bwd = h->clusters_bwd;
+  return DRL_OK;
+}
 
 }  // extern "C"

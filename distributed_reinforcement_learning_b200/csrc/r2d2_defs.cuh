@@ -9,28 +9,30 @@
 
 namespace drl {
 
-constexpr int kR2L = 64;                 // lstm_size (config.json:93): the recurrence kernels keep W_h (L x 4L) on chip
+// lstm_size of config.json:93: the width of the policy engine, recorder and device queue, and the learner width whose
+// recurrence runs one CTA per sequence (r2d2_lstm_fwd_kernel); the learner also takes 256 and 512 (r2d2_cluster.cuh)
+constexpr int kR2L = 64;
 constexpr int kR2G = 4 * kR2L;           // 256 gate columns
 constexpr int kR2H = 128;                // dense width between the LSTM and the two output streams (model/r2d2_lstm.py:50)
 constexpr int kR2Cat = Geo::FLAT + Geo::EMB;   // 3392 rows of the LSTM kernel that multiply the step input
 
 struct R2Layout : TrunkLayout {
   int64_t lstm_w, lstm_b, q1_w, q1_b, value_w, value_b, mean_w, mean_b;
-  void init(int num_action, int channels) {
+  void init(int num_action, int channels, int L = kR2L) {
     A = num_action; C = channels;
     const int64_t sizes[] = {
         8 * 8 * (int64_t)C * 32, 32, 4 * 4 * 32 * 64, 64, 3 * 3 * 64 * 64, 64,
         (int64_t)A * 256, 256, 256 * 256, 256,
-        (int64_t)(kR2Cat + kR2L) * kR2G, kR2G,
-        (int64_t)kR2L * kR2H, kR2H, (int64_t)kR2H * A, A, kR2H, 1};
+        (int64_t)(kR2Cat + L) * 4 * L, 4 * L,
+        (int64_t)L * kR2H, kR2H, (int64_t)kR2H * A, A, kR2H, 1};
     int64_t* const named[] = {&conv1_w, &conv1_b, &conv2_w, &conv2_b, &conv3_w, &conv3_b, &emb1_w, &emb1_b, &emb2_w,
                               &emb2_b, &lstm_w, &lstm_b, &q1_w, &q1_b, &value_w, &value_b, &mean_w, &mean_b};
     set(sizes, named);
   }
 };
 
-// drl_r2d2_policy_sync_from_learner: learner_params_snapshot of an R2D2 learner whose network has num_action actions and
-// `channels` input channels (DRL_ERR_INVALID otherwise)
+// drl_r2d2_policy_sync_from_learner: learner_params_snapshot of an R2D2 learner whose network has num_action actions,
+// `channels` input channels and lstm_size kR2L, the policy engine's (DRL_ERR_INVALID otherwise)
 int r2d2_params_snapshot(drl_r2d2* h, int device, int num_action, int channels, cudaStream_t dst_stream, float* dst,
                          cudaEvent_t ev_ready, cudaEvent_t ev_copied);
 
@@ -64,6 +66,8 @@ struct R2In {              // one staged minibatch, caller's batch-major layout
 struct drl_r2d2 : drl::AdamLearner {
   drl_r2d2_config cfg{};
   int S = 0, A = 0, C = 1, Nt = 0;
+  int L = drl::kR2L;                    // lstm_size: 64, 256 or 512
+  int clusters_fwd = 0, clusters_bwd = 0;   // L > 64: clusters of the recurrence kernels the device places at once
   size_t frame = 0;
   drl::R2Layout pl{};
   drl::R2Acts act{}, tact{};

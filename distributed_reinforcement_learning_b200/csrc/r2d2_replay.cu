@@ -36,9 +36,10 @@ struct R2SeqRows {
 };
 
 // Block (i, t) copies frame t of row src_row into row dst_row as 16-byte vectors (frame16 = 84 * 84 * C / 16 of them:
-// 441 or 1,764), and thread 0 the step's four scalars; block (i, 0) also copies the row's h0 and c0 (L / 4 vectors each).
+// 441 or 1,764), and thread 0 the step's four scalars; block (i, 0) also copies the row's h0 and c0 (L / 4 vectors each,
+// L = lstm_size).
 __device__ __forceinline__ void copy_seq_step(const R2SeqRows& src, int64_t src_row, const R2SeqRows& dst,
-                                              int64_t dst_row, int S, int frame16) {
+                                              int64_t dst_row, int S, int frame16, int L) {
   const int t = blockIdx.y;
   const size_t fs = ((size_t)src_row * S + t) * frame16, fd = ((size_t)dst_row * S + t) * frame16;
   const uint4* __restrict__ s4 = reinterpret_cast<const uint4*>(src.frames) + fs;
@@ -51,28 +52,29 @@ __device__ __forceinline__ void copy_seq_step(const R2SeqRows& src, int64_t src_
     dst.reward[dof] = src.reward[so];
     dst.done[dof] = src.done[so];
   }
-  if (t == 0 && threadIdx.x < 2 * (kR2L / 4)) {
-    const int k = threadIdx.x % (kR2L / 4);
-    const float* s = threadIdx.x < kR2L / 4 ? src.h0 : src.c0;
-    float* d = threadIdx.x < kR2L / 4 ? dst.h0 : dst.c0;
-    reinterpret_cast<float4*>(d + (size_t)dst_row * kR2L)[k] = reinterpret_cast<const float4*>(s + (size_t)src_row * kR2L)[k];
-  }
+  if (t == 0)
+    for (int i = threadIdx.x; i < 2 * (L / 4); i += blockDim.x) {
+      const int k = i % (L / 4);
+      const float* s = i < L / 4 ? src.h0 : src.c0;
+      float* d = i < L / 4 ? dst.h0 : dst.c0;
+      reinterpret_cast<float4*>(d + (size_t)dst_row * L)[k] = reinterpret_cast<const float4*>(s + (size_t)src_row * L)[k];
+    }
 }
 
 // Ingest: the n sequences of the ingest block (rows 0..n-1) into the storage rows (first + i) mod capacity.  Grid (n, S).
 __global__ void __launch_bounds__(256) replay_store_seq_kernel(const R2SeqRows in, int64_t first, int64_t capacity,
-                                                                const R2SeqRows mem, int S, int frame16) {
+                                                                const R2SeqRows mem, int S, int frame16, int L) {
   kernel_prologue();
-  copy_seq_step(in, blockIdx.x, mem, (first + blockIdx.x) % capacity, S, frame16);
+  copy_seq_step(in, blockIdx.x, mem, (first + blockIdx.x) % capacity, S, frame16, L);
 }
 
 // The minibatch of a training step: the sampled storage rows data_index[0, B) into a learner slot's views (rows 0..B-1),
 // in the layout drl_r2d2_stage writes.  The importance weights are written by the sample kernel.  Grid (B, S).
 __global__ void __launch_bounds__(256) replay_gather_seq_kernel(const int64_t* __restrict__ data_index,
                                                                  const R2SeqRows mem, const R2SeqRows out, int S,
-                                                                 int frame16) {
+                                                                 int frame16, int L) {
   kernel_prologue();
-  copy_seq_step(mem, data_index[blockIdx.x], out, blockIdx.x, S, frame16);
+  copy_seq_step(mem, data_index[blockIdx.x], out, blockIdx.x, S, frame16, L);
 }
 
 }  // namespace drl
@@ -86,13 +88,13 @@ constexpr const char* kName = "r2d2 replay";
 // caller's priorities when given)
 struct IngestLayout {
   size_t fr, pa, ac, h, c, rw, dn, er, bytes;
-  IngestLayout(size_t n, size_t S, size_t frame) {
+  IngestLayout(size_t n, size_t S, size_t frame, size_t L) {
     size_t off = 0;
     fr = off; off = align_up(off + n * S * frame, 256);
     pa = off; off = align_up(off + n * S * 4, 256);
     ac = off; off = align_up(off + n * S * 4, 256);
-    h = off; off = align_up(off + n * kR2L * 4, 256);
-    c = off; off = align_up(off + n * kR2L * 4, 256);
+    h = off; off = align_up(off + n * L * 4, 256);
+    c = off; off = align_up(off + n * L * 4, 256);
     rw = off; off = align_up(off + n * S * 4, 256);
     dn = off; off = align_up(off + n * S, 256);
     er = off; off = align_up(off + n * 8, 256);
@@ -104,7 +106,7 @@ struct IngestLayout {
 
 // the sum tree, the ordering and the sample / update state are the shared core's (replay_core.cuh)
 struct drl_r2d2_replay : ReplayCore {
-  int S = 0, C = 1, A = 0;
+  int S = 0, C = 1, A = 0, L = kR2L;    // L: lstm_size, the width of a record's h0 / c0
   size_t frame = 0;                    // bytes of one 84x84xC frame
   // the sequences, zero-initialised: a leaf past n_entries reached through float drift gathers a defined record
   R2SeqRows mem{};
@@ -121,9 +123,9 @@ int check_learner(const drl_r2d2_replay* r, const drl_r2d2* h) {
     set_error("r2d2 replay: the learner is on device %d, the memory on device %d", h->device, r->device);
     return DRL_ERR_INVALID;
   }
-  if (h->S != r->S || h->C != r->C || h->A != r->A) {
-    set_error("r2d2 replay: the learner has seq_len %d, %d channels and num_action %d, the memory %d, %d and %d", h->S,
-              h->C, h->A, r->S, r->C, r->A);
+  if (h->S != r->S || h->C != r->C || h->A != r->A || h->L != r->L) {
+    set_error("r2d2 replay: the learner has seq_len %d, %d channels, num_action %d and lstm_size %d, the memory %d, %d, "
+              "%d and %d", h->S, h->C, h->A, h->L, r->S, r->C, r->A, r->L);
     return DRL_ERR_INVALID;
   }
   return DRL_OK;
@@ -141,8 +143,17 @@ extern "C" {
 
 int drl_r2d2_replay_create(int32_t device, int64_t capacity, int32_t seq_len, int32_t channels, int32_t num_action,
                            drl_r2d2_replay** out) {
+  return drl_r2d2_replay_create_lstm(device, capacity, seq_len, channels, num_action, kR2L, out);
+}
+
+int drl_r2d2_replay_create_lstm(int32_t device, int64_t capacity, int32_t seq_len, int32_t channels, int32_t num_action,
+                                int32_t lstm_size, drl_r2d2_replay** out) {
   if (!out) { set_error("null argument"); return DRL_ERR_INVALID; }
   *out = nullptr;
+  if (lstm_size != kR2L && lstm_size != 256 && lstm_size != 512) {
+    set_error("r2d2 replay: lstm_size must be 64, 256 or 512 (got %d)", lstm_size);
+    return DRL_ERR_INVALID;
+  }
   if (seq_len < 2) { set_error("r2d2 replay: seq_len must be >= 2 (got %d)", seq_len); return DRL_ERR_INVALID; }
   if (channels != 1 && channels != 4) { set_error("r2d2 replay: channels must be 1 or 4 (got %d)", channels); return DRL_ERR_INVALID; }
   if (num_action < 2 || num_action > 32) { set_error("r2d2 replay: num_action must be in [2, 32] (got %d)", num_action); return DRL_ERR_INVALID; }
@@ -152,6 +163,7 @@ int drl_r2d2_replay_create(int32_t device, int64_t capacity, int32_t seq_len, in
   r->S = seq_len;
   r->C = channels;
   r->A = num_action;
+  r->L = lstm_size;
   r->frame = (size_t)Geo::IH * Geo::IW * channels;
   int rc = [&]() -> int {
     const size_t C = (size_t)capacity, S = (size_t)seq_len;
@@ -160,8 +172,8 @@ int drl_r2d2_replay_create(int32_t device, int64_t capacity, int32_t seq_len, in
     DRL_TRY(dev_alloc(r, &m.frames, C * S * r->frame));
     DRL_TRY(dev_alloc(r, &m.pa, C * S));
     DRL_TRY(dev_alloc(r, &m.action, C * S));
-    DRL_TRY(dev_alloc(r, &m.h0, C * kR2L));
-    DRL_TRY(dev_alloc(r, &m.c0, C * kR2L));
+    DRL_TRY(dev_alloc(r, &m.h0, C * lstm_size));
+    DRL_TRY(dev_alloc(r, &m.c0, C * lstm_size));
     DRL_TRY(dev_alloc(r, &m.reward, C * S));
     DRL_TRY(dev_alloc(r, &m.done, C * S));
     DRL_CUDA_CHECK(cudaDeviceSynchronize());
@@ -206,15 +218,15 @@ int drl_r2d2_replay_add(drl_r2d2_replay* r, drl_r2d2* learner, int32_t n, const 
       return DRL_ERR_INVALID;
     }
   DRL_CUDA_CHECK(cudaSetDevice(r->device));
-  const IngestLayout L(n, S, r->frame);
+  const IngestLayout L(n, S, r->frame, r->L);
   DRL_TRY(replay_ensure_ingest(r, L.bytes));
   uint8_t* h = r->ingest.h;
   const size_t ns = (size_t)n * S;
   memcpy(h + L.fr, state, ns * r->frame);
   memcpy(h + L.pa, previous_action, ns * 4);
   memcpy(h + L.ac, action, ns * 4);
-  memcpy(h + L.h, h0, (size_t)n * kR2L * 4);
-  memcpy(h + L.c, c0, (size_t)n * kR2L * 4);
+  memcpy(h + L.h, h0, (size_t)n * r->L * 4);
+  memcpy(h + L.c, c0, (size_t)n * r->L * 4);
   memcpy(h + L.rw, reward, ns * 4);
   memcpy(h + L.dn, done, ns);
   if (error) memcpy(h + L.er, error, (size_t)n * 8);
@@ -234,7 +246,7 @@ int drl_r2d2_replay_add(drl_r2d2_replay* r, drl_r2d2* learner, int32_t n, const 
   }
   prof_mark(s, "replay_store_seq");
   DRL_CUDA_CHECK((launch_k(replay_store_seq_kernel, dim3(n, S), 256, 0, s, rows, r->cursor, r->capacity, r->mem, S,
-                           (int)(r->frame / 16))));
+                           (int)(r->frame / 16), r->L)));
   DRL_TRY(replay_launch_update(r, s, n, nullptr, r->cursor, error ? reinterpret_cast<const double*>(d + L.er) : nullptr,
                                error ? nullptr : learner->td_dev));
   DRL_TRY(replay_end(r, s));
@@ -256,6 +268,10 @@ int drl_r2d2_replay_add_from_queue(drl_r2d2_replay* r, drl_r2d2* learner, drl_r2
     if (q->S != r->S || q->C != r->C || q->A != r->A) {
       set_error("r2d2 replay add_from_queue: the queue has seq_len %d, %d channels and num_action %d, the memory %d, %d "
                 "and %d", q->S, q->C, q->A, r->S, r->C, r->A);
+      return DRL_ERR_INVALID;
+    }
+    if (r->L != kR2L) {
+      set_error("r2d2 replay add_from_queue: the queue stores lstm_size %d states, the memory %d", kR2L, r->L);
       return DRL_ERR_INVALID;
     }
     if (q->batch > learner->B) {
@@ -289,7 +305,7 @@ int drl_r2d2_replay_add_from_queue(drl_r2d2_replay* r, drl_r2d2* learner, drl_r2
     learner->last_n = n;
     prof_mark(s, "replay_store_seq");
     DRL_CUDA_CHECK((launch_k(replay_store_seq_kernel, dim3(n, S), 256, 0, s, rows, r->cursor, r->capacity, r->mem, S,
-                             (int)(r->frame / 16))));
+                             (int)(r->frame / 16), r->L)));
     return replay_launch_update(r, s, n, nullptr, r->cursor, nullptr, learner->td_dev);
   }();
   // the queue slot goes back to the producers either way (their copies into it wait for its release event)
@@ -315,7 +331,7 @@ int drl_r2d2_replay_step_async(drl_r2d2_replay* r, drl_r2d2* learner, int32_t sl
   return replay_step(r, learner, slot, u01, const_cast<float*>(in.weight), learner->td_dev, [&](cudaStream_t s) -> int {
     prof_mark(s, "replay_gather_seq");
     DRL_CUDA_CHECK((launch_k(replay_gather_seq_kernel, dim3(B, r->S), 256, 0, s, r->d_data_index, r->mem, out, r->S,
-                             (int)(r->frame / 16))));
+                             (int)(r->frame / 16), r->L)));
     return DRL_OK;
   });
 }
@@ -350,8 +366,9 @@ int drl_r2d2_replay_read(drl_r2d2_replay* r, int64_t data_index, int32_t n, uint
   if (state) DRL_CUDA_CHECK(cp(state, mem.frames + i * S * r->frame, m * S * r->frame));
   if (previous_action) DRL_CUDA_CHECK(cp(previous_action, mem.pa + i * S, m * S * 4));
   if (action) DRL_CUDA_CHECK(cp(action, mem.action + i * S, m * S * 4));
-  if (h0) DRL_CUDA_CHECK(cp(h0, mem.h0 + i * kR2L, m * kR2L * 4));
-  if (c0) DRL_CUDA_CHECK(cp(c0, mem.c0 + i * kR2L, m * kR2L * 4));
+  const size_t L = (size_t)r->L;
+  if (h0) DRL_CUDA_CHECK(cp(h0, mem.h0 + i * L, m * L * 4));
+  if (c0) DRL_CUDA_CHECK(cp(c0, mem.c0 + i * L, m * L * 4));
   if (reward) DRL_CUDA_CHECK(cp(reward, mem.reward + i * S, m * S * 4));
   if (done) DRL_CUDA_CHECK(cp(done, mem.done + i * S, m * S));
   return DRL_OK;

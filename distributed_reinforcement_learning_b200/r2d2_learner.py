@@ -74,6 +74,13 @@ class NativeR2D2Learner(AdamLearnerHandle):
         N.check(N.lib.drl_r2d2_act(self._h, n, N.ptr(st), N.ptr(pa), N.ptr(hh), N.ptr(cc), N.ptr(q), N.ptr(ho), N.ptr(co)))
         return q, ho, co
 
+    def recurrence_clusters(self):
+        """-> (CTAs per cluster, clusters of the forward / BPTT recurrence the device places at once); (0, 0, 0) at
+        lstm_size 64, whose recurrence runs one CTA per sequence."""
+        v = [C.c_int32() for _ in range(3)]
+        N.check(N.lib.drl_r2d2_recurrence_clusters(self._h, *[C.byref(x) for x in v]))
+        return tuple(int(x.value) for x in v)
+
     def taps(self, n=None):
         n = self.B if n is None else int(n)
         mq = np.empty((n, self.S, self.A), np.float32)

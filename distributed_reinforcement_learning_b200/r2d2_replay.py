@@ -8,7 +8,8 @@ on the GPU beside a ``NativeR2D2Learner``: ingest with the learner's |td| of a w
 sampling, the minibatch gather into a staging slot and the priority update from the step's |td| run as kernels on the
 learner's compute stream.  The host draws the uniforms (the reference's ``random.random()``) and keeps the control
 flow.  Same constants and arithmetic as ``Memory``: for the same uniforms it samples the same indices (DESIGN.md
-section 11).  A record keeps step 0 of the stored (h, c), the only step the learner reads.
+section 11).  A record keeps step 0 of the stored (h, c), the only step the learner reads, as ``lstm_size`` floats each
+(64, 256 or 512: the width of the learners it serves).
 """
 import ctypes as C
 
@@ -16,18 +17,15 @@ import numpy as np
 
 from . import _native as N
 
-LSTM = 64
-
-
 class NativeR2D2Replay:
 
-    def __init__(self, capacity, seq_len=15, num_action=4, input_shape=(84, 84, 1), device=0):
+    def __init__(self, capacity, seq_len=15, num_action=4, input_shape=(84, 84, 1), device=0, lstm_size=64):
         self.capacity, self.device = int(capacity), int(device)
-        self.S, self.A = int(seq_len), int(num_action)
+        self.S, self.A, self.L = int(seq_len), int(num_action), int(lstm_size)
         self.input_shape = tuple(int(x) for x in input_shape)
         self._h = C.c_void_p()
-        N.check(N.lib.drl_r2d2_replay_create(self.device, self.capacity, self.S, self.input_shape[-1], self.A,
-                                             C.byref(self._h)))
+        N.check(N.lib.drl_r2d2_replay_create_lstm(self.device, self.capacity, self.S, self.input_shape[-1], self.A,
+                                                  self.L, C.byref(self._h)))
         self._n_last = 0            # draws of the most recent sample / step
 
     # ---- lifetime ----------------------------------------------------------------
@@ -63,13 +61,13 @@ class NativeR2D2Replay:
     # ---- data path ---------------------------------------------------------------
     def add(self, learner, state, previous_action, action, h0, c0, reward, done, error=None):
         """Memory.add of n sequences in order: state [n, S, H, W, C], previous_action / action / reward / done [n, S],
-        h0 / c0 [n, 64] (step 0 of the stored states).  error=None: the priorities are ``learner``'s |td| of these
+        h0 / c0 [n, lstm_size] (step 0 of the stored states).  error=None: the priorities are ``learner``'s |td| of these
         sequences, computed on the device (n <= learner.B); otherwise ``error`` [n] (learner may be None)."""
         n, S = int(np.asarray(state).shape[0]), self.S
         arrs = (N.as_c(state, np.uint8, (n, S) + self.input_shape, "state"),
                 N.as_c(previous_action, np.int32, (n, S), "previous_action"),
                 N.as_c(action, np.int32, (n, S), "action"),
-                N.as_c(h0, np.float32, (n, LSTM), "h0"), N.as_c(c0, np.float32, (n, LSTM), "c0"),
+                N.as_c(h0, np.float32, (n, self.L), "h0"), N.as_c(c0, np.float32, (n, self.L), "c0"),
                 N.as_c(reward, np.float32, (n, S), "reward"),
                 N.as_c(N.as_u8(done), np.uint8, (n, S), "done"))
         err = None if error is None else N.as_c(error, np.float64, (n,), "error")
@@ -115,11 +113,11 @@ class NativeR2D2Replay:
         return ti, pr, w
 
     def read(self, data_index, n=1):
-        """Rows [data_index, data_index + n) of the storage as a dict of arrays (h0 / c0 [n, 64])."""
+        """Rows [data_index, data_index + n) of the storage as a dict of arrays (h0 / c0 [n, lstm_size])."""
         n, S = int(n), self.S
         out = dict(state=np.empty((n, S) + self.input_shape, np.uint8),
                    previous_action=np.empty((n, S), np.int32), action=np.empty((n, S), np.int32),
-                   h0=np.empty((n, LSTM), np.float32), c0=np.empty((n, LSTM), np.float32),
+                   h0=np.empty((n, self.L), np.float32), c0=np.empty((n, self.L), np.float32),
                    reward=np.empty((n, S), np.float32), done=np.empty((n, S), np.uint8))
         N.check(N.lib.drl_r2d2_replay_read(self._h, int(data_index), n,
                                            *[N.ptr(out[k]) for k in ("state", "previous_action", "action", "h0", "c0",

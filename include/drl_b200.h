@@ -363,7 +363,8 @@ int drl_r2d2_policy_set_params(drl_r2d2_policy* h, const float* host_flat, int64
 int drl_r2d2_policy_get_params(drl_r2d2_policy* h, float* host_flat, int64_t n);
 /* parameter_sync without a host round trip: the learner's main parameters after all work enqueued on it so far (a step
  * in flight included), copied device to device on the policy's stream; the learner's next update waits for the copy.
- * The learner must be on the same device and have the same num_action and channels (DRL_ERR_INVALID otherwise).
+ * The learner must be on the same device and have the same num_action and channels, and lstm_size 64
+ * (DRL_ERR_INVALID otherwise).
  * Returns without waiting for the copy. */
 int drl_r2d2_policy_sync_from_learner(drl_r2d2_policy* h, struct drl_r2d2* learner);
 /* Agent.get_action (agent/r2d2.py:171-191) for n <= max_batch environments.  state u8 [n,H,W,C]; previous_action i32
@@ -998,7 +999,9 @@ typedef struct drl_r2d2_config {
   int32_t burn_in;            /* loss window starts here (config.json:96), 0 <= burn_in <= S - 2         */
   int32_t height, width, channels; /* 84, 84, 1 (config.json:91) or 84, 84, 4                            */
   int32_t num_action;         /* A, 2..32                                                                */
-  int32_t lstm_size;          /* 64 -- only this size is supported (config.json:93)                      */
+  int32_t lstm_size;          /* 64 (config.json:93), 256 or 512; others -> DRL_ERR_INVALID. 256 and 512 run the
+                                 recurrence on a thread-block cluster of lstm_size / 32 CTAs; the policy engine
+                                 only syncs from a 64-wide learner                                       */
   float discount_factor;      /* agent/r2d2.py:62                                                        */
   float learning_rate;        /* 1e-4 (agent/r2d2.py:91)                                                 */
   int32_t device;
@@ -1065,26 +1068,33 @@ int drl_r2d2_profile_step(drl_r2d2* h, int32_t slot, char* names, int64_t names_
 int drl_r2d2_last_step_ms(drl_r2d2* h, float* ms);
 int drl_r2d2_stream(drl_r2d2* h, void** stream);
 int drl_r2d2_launches_per_step(const drl_r2d2* h, int32_t* n);
+/* The recurrence's placement: CTAs per cluster (lstm_size / 32; 0 at lstm_size 64, which runs one CTA per sequence)
+ * and how many clusters of the forward / BPTT kernel the device places at once (cudaOccupancyMaxActiveClusters at
+ * create time; each launch uses at most that many, one per 8 (L = 256) or 4 (L = 512) sequences). */
+int drl_r2d2_recurrence_clusters(const drl_r2d2* h, int32_t* cluster_size, int32_t* max_fwd, int32_t* max_bwd);
 
 /* ------------------------------------------------------------------------------------------
  * R2D2 prioritized sequence replay memory on the device (DESIGN.md section 11): buffer_queue.Memory with one
  * stored-state sequence per record in HBM (state u8 [S,84,84,C]; previous_action, action i32 [S]; reward f32 [S]; done
- * u8 [S]; h0, c0 f32 [64], step 0 of the stored states, the only step the learner reads; zero-initialised), the float64
+ * u8 [S]; h0, c0 f32 [L], step 0 of the stored states, the only step the learner reads; zero-initialised), the float64
  * sum tree on the device, and the learner loop of train_r2d2.py:87-165 -- ingest, sample, minibatch gather, step,
  * priority update -- as kernels on the learner's compute stream.  The sum tree, its constants and arithmetic and the
  * sample / update / last_sample / total / size / beta calls behave as drl_apex_replay_*'s.  The memory outlives any
- * learner: every call that uses one takes a drl_r2d2* on the memory's device with the memory's seq_len, channels and
- * num_action, and orders itself after the memory's previous work on whichever stream that ran.
+ * learner: every call that uses one takes a drl_r2d2* on the memory's device with the memory's seq_len, channels,
+ * num_action and lstm_size L, and orders itself after the memory's previous work on whichever stream that ran.
  * ------------------------------------------------------------------------------------------ */
 typedef struct drl_r2d2_replay drl_r2d2_replay;
-/* capacity in [2, 2^31], seq_len >= 2, channels 1 or 4, num_action in [2, 32].  Device memory per sequence:
- * S * (7,056 C + 13) + 512 bytes: 106,547 B at S = 15, C = 1 (10.7 GB at the reference's capacity 1e5), 424,067 B at
- * C = 4 (42.4 GB). */
+/* capacity in [2, 2^31], seq_len >= 2, channels 1 or 4, num_action in [2, 32]; lstm_size L = 64.  Device memory per
+ * sequence: S * (7,056 C + 13) + 8 L bytes: 106,547 B at S = 15, C = 1, L = 64 (10.7 GB at the reference's capacity
+ * 1e5), 424,067 B at C = 4 (42.4 GB). */
 int drl_r2d2_replay_create(int32_t device, int64_t capacity, int32_t seq_len, int32_t channels, int32_t num_action,
                            drl_r2d2_replay** out);
+/* drl_r2d2_replay_create for lstm_size L in {64, 256, 512} (others -> DRL_ERR_INVALID). */
+int drl_r2d2_replay_create_lstm(int32_t device, int64_t capacity, int32_t seq_len, int32_t channels, int32_t num_action,
+                                int32_t lstm_size, drl_r2d2_replay** out);
 int drl_r2d2_replay_destroy(drl_r2d2_replay* r);
 /* Memory.add for n sequences in order at the write cursor (wrapping); the arguments are drl_r2d2_td_error's (h0, c0
- * [n, 64]).  error == NULL: the priorities are the learner's |td| of these sequences (agent/r2d2.py:97-130, all n in
+ * [n, L]).  error == NULL: the priorities are the learner's |td| of these sequences (agent/r2d2.py:97-130, all n in
  * one pass), computed on the device and never copied to the host; then 1 <= n <= the learner's batch.  Otherwise
  * error [n] are the caller's and learner may be NULL.  Every previous_action and action must be in [0, num_action).
  * Does not wait for the learner's compute stream. */
@@ -1099,7 +1109,7 @@ int drl_r2d2_replay_add(drl_r2d2_replay* r, drl_r2d2* learner, int32_t n, const 
  * (timeout_ms < 0: forever; DRL_ERR_TIMEOUT with nothing changed otherwise), then, on the learner's compute stream, the
  * learner's |td| of the batch read from the queue slot, the store and the priority update; the slot goes back to the
  * producers after them, also when enqueueing fails.  The queue's seq_len, channels, num_action and device must be the
- * memory's and its batch at most the learner's (DRL_ERR_INVALID).  Does not wait for the learner's compute stream. */
+ * memory's, the memory's lstm_size the queue's 64, and the queue's batch at most the learner's (DRL_ERR_INVALID).  Does not wait for the learner's compute stream. */
 int drl_r2d2_replay_add_from_queue(drl_r2d2_replay* r, drl_r2d2* learner, drl_r2d2_queue* queue, int32_t timeout_ms);
 int drl_r2d2_replay_step_async(drl_r2d2_replay* r, drl_r2d2* learner, int32_t slot, const double* u01);
 /* As drl_apex_replay_sample / _update / _last_sample. */
