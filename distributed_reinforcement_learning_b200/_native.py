@@ -141,7 +141,7 @@ def _load():
         "drl_debug_trace": (C.c_int, [vp]),
         "drl_debug_launch_plan": (C.c_int, [i32, i32, i32, vp]),
         "drl_debug_apex_launch_plan": (C.c_int, [i32, i32, vp]),
-        "drl_debug_r2d2_launch_plan": (C.c_int, [i32, i32, i32, i32, vp]),
+        "drl_debug_r2d2_launch_plan": (C.c_int, [i32, i32, i32, i32, i32, vp]),
         "drl_debug_gemm16_residency": (C.c_int, [vp]),
         "drl_debug_gemm16_local_bytes": (C.c_int, [vp]),
         "drl_learner_last_step_ms": (C.c_int, [vp, C.POINTER(f32)]),

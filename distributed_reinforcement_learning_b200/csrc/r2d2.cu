@@ -861,20 +861,23 @@ int drl_r2d2_read_buffer(drl_r2d2* h, const char* name, float* host_dst, int64_t
   return read_named_buffer(h, tab, sizeof(tab) / sizeof(tab[0]), name, host_dst, n);
 }
 
-// The launch plan of an R2D2 step over B sequences of S steps of C-channel frames in math mode `mode` (M = B*S rows,
-// all of which receive gradient), read by the per-kernel tests to assert which edges a case reaches: out[0] = split-K
-// count of lstm_x_fwd, out[1..3] = split-K count of the conv1 / conv2 / conv3 weight gradients (conv1: the
-// single-channel plan when C == 1).
-int drl_debug_r2d2_launch_plan(int32_t B, int32_t S, int32_t C, int32_t mode, int32_t* out) {
-  if (!out || B < 1 || S < 1 || (C != 1 && C != 4) || mode < 1 || mode > 2) {
-    set_error("r2d2_launch_plan: need out, B >= 1, S >= 1, C 1 or 4, mode 1 or 2");
+// The launch plan of an R2D2 step over B sequences of S steps of C-channel frames in math mode `mode` at width
+// `lstm_size` (M = B*S rows, all of which receive gradient), read by the per-kernel tests to assert which edges a case
+// reaches: out[0] = split-K count of lstm_x_fwd (N = 4 lstm_size), out[1..3] = split-K count of the conv1 / conv2 /
+// conv3 weight gradients (conv1: the single-channel plan when C == 1), out[4] = sequences per cluster pass of the
+// recurrence (R2Clu<L>::R; 0 at 64, which runs one CTA per sequence).
+int drl_debug_r2d2_launch_plan(int32_t B, int32_t S, int32_t C, int32_t mode, int32_t lstm_size, int32_t* out) {
+  if (!out || B < 1 || S < 1 || (C != 1 && C != 4) || mode < 1 || mode > 2 ||
+      (lstm_size != kR2L && lstm_size != 256 && lstm_size != 512)) {
+    set_error("r2d2_launch_plan: need out, B >= 1, S >= 1, C 1 or 4, mode 1 or 2, lstm_size 64, 256 or 512");
     return DRL_ERR_INVALID;
   }
   const int M = B * S;
-  out[0] = plan_r2_x(M, mode, kR2G).splits;
+  out[0] = plan_r2_x(M, mode, 4 * lstm_size).splits;
   out[1] = C == 1 ? plan_conv1_wgrad_c1(M).splits : plan_conv1_wgrad(M, mode).splits;
   out[2] = plan_conv2_wgrad(M, mode).splits;
   out[3] = plan_conv3_wgrad(M, mode).splits;
+  out[4] = lstm_size == 256 ? R2Clu<256>::R : lstm_size == 512 ? R2Clu<512>::R : 0;
   return DRL_OK;
 }
 

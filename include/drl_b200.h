@@ -195,9 +195,10 @@ int drl_debug_launch_plan(int32_t B, int32_t T, int32_t mode, int32_t* out);
  * conv3 weight gradients. */
 int drl_debug_apex_launch_plan(int32_t B, int32_t mode, int32_t* out);
 /* Test aid: the launch plan of an R2D2 step over B sequences of S steps of C-channel frames (M = B*S rows) in math
- * mode 1 or 2: out[0] = split-K count of the LSTM input contraction (lstm_x_fwd), out[1..3] = split-K count of the
- * conv1 / conv2 / conv3 weight gradients (conv1: the single-channel plan when C == 1). */
-int drl_debug_r2d2_launch_plan(int32_t B, int32_t S, int32_t C, int32_t mode, int32_t* out);
+ * mode 1 or 2 at lstm_size 64, 256 or 512 (others -> DRL_ERR_INVALID): out[0] = split-K count of the LSTM input
+ * contraction (lstm_x_fwd, N = 4 lstm_size), out[1..3] = split-K count of the conv1 / conv2 / conv3 weight gradients
+ * (conv1: the single-channel plan when C == 1), out[4] = sequences per cluster pass of the recurrence (0 at 64). */
+int drl_debug_r2d2_launch_plan(int32_t B, int32_t S, int32_t C, int32_t mode, int32_t lstm_size, int32_t* out);
 /* Test aid: CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor at the launch's block size and dynamic shared
  * memory) of the math-mode-5 kernels sized for two per SM: out[0] / out[1] = conv2 / conv3 forward, out[2] = conv2
  * data gradient. */

@@ -29,10 +29,10 @@ def gpu_masks(eng, B, S, A):
             "emb": torch.from_numpy(eng.read_buffer("emb", A * 256).reshape(A, 256) > 0)}
 
 
-def make_batch(B, S, A, C, seed, done_rate=None, done_ends=False):
-    """rt.make_sequences, optionally with its dones redrawn at ``done_rate`` and, with ``done_ends``, forced at the
-    first and the last step of every sequence."""
-    b = rt.make_sequences(B, S=S, A=A, input_shape=(84, 84, C), seed=seed)
+def make_batch(B, S, A, C, seed, done_rate=None, done_ends=False, L=64):
+    """rt.make_sequences (h, c of width ``L``), optionally with its dones redrawn at ``done_rate`` and, with
+    ``done_ends``, forced at the first and the last step of every sequence."""
+    b = rt.make_sequences(B, S=S, A=A, L=L, input_shape=(84, 84, C), seed=seed)
     if done_rate is not None:
         b["done"] = np.random.default_rng(seed + 7919).random((B, S)) < done_rate
     if done_ends:

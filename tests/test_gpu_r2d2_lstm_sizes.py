@@ -216,8 +216,9 @@ def _run_loop(agent, device, records, iters, seed, batch, capacity=64):
     return out
 
 
-def test_device_replay_at_512_samples_the_host_memory(native):
-    L, S, bi, B = 512, 6, 2, 4
+def _device_replay_samples_the_host_memory(L):
+    """The device replay memory at width L samples the same indices as the host Memory and gives identical losses."""
+    S, bi, B = 6, 2, 4
     rng = np.random.default_rng(3)
     records = []
     for _ in range(4):
@@ -225,10 +226,18 @@ def test_device_replay_at_512_samples_the_host_memory(native):
         q["h"] = np.repeat(q["h"][:, :1], S, 1)
         q["c"] = np.repeat(q["c"][:, :1], S, 1)
         records.append(q)
-    host = _run_loop(_agent("r2d2_lstm512_host", L, S, bi), False, records, 10, 7, B)
-    dev = _run_loop(_agent("r2d2_lstm512_dev", L, S, bi), True, records, 10, 7, B)
+    host = _run_loop(_agent("r2d2_lstm%d_host" % L, L, S, bi), False, records, 10, 7, B)
+    dev = _run_loop(_agent("r2d2_lstm%d_dev" % L, L, S, bi), True, records, 10, 7, B)
     assert len(host["idx"]) == 8 and host["idx"] == dev["idx"]
     assert host["loss"] == dev["loss"]
+
+
+def test_device_replay_at_512_samples_the_host_memory(native):
+    _device_replay_samples_the_host_memory(512)
+
+
+def test_device_replay_at_256_samples_the_host_memory(native):
+    _device_replay_samples_the_host_memory(256)
 
 
 def test_replay_storage_and_width_checks(native):

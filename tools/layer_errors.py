@@ -5,7 +5,7 @@ the policy engines; the same checks as tests/test_gpu_layer_local.py, tests/test
 tests/test_gpu_policy_layer_local.py).  A performance change can show with it which kernel's error moved.
 
     python tools/layer_errors.py --mode 5 --B 32 --T 20 --A 18 --regime init [--regime trained ...]
-    python tools/layer_errors.py --family r2d2 --mode 2 --B 16 --T 80 --burn-in 40 --A 4 --C 1
+    python tools/layer_errors.py --family r2d2 --mode 2 --B 16 --T 80 --burn-in 40 --A 4 --C 1 [--lstm-size 512]
     python tools/layer_errors.py --family apex --mode 2 --B 32 --A 18 [--regime ties]
     python tools/layer_errors.py --family impala_policy --n 64 --A 18 [--regime peaked]
     python tools/layer_errors.py --family r2d2_policy --n 9 --A 4 --C 4 [--regime saturated]
@@ -36,6 +36,7 @@ def main():
     ap.add_argument("--burn-in", type=int, default=40, help="r2d2 only")
     ap.add_argument("--A", type=int, default=18)
     ap.add_argument("--C", type=int, default=1, help="r2d2 frame channels")
+    ap.add_argument("--lstm-size", type=int, default=64, choices=alp.R2_SIZES, help="r2d2 only")
     ap.add_argument("--n", type=int, default=64, help="rows of the act (policy families)")
     ap.add_argument("--regime", action="append")
     a = ap.parse_args()
@@ -59,12 +60,12 @@ def main():
     if a.family in ("impala", "r2d2"):
         shape["T"] = a.T
     if a.family == "r2d2":
-        shape.update(burn_in=a.burn_in, C=a.C)
+        shape.update(burn_in=a.burn_in, C=a.C, lstm_size=a.lstm_size)
     for regime in a.regime or ["init"]:
         if a.family == "impala":
             rows, facts = lp.run_case(mode, a.B, a.T, a.A, regime)
         elif a.family == "r2d2":
-            rows, facts = alp.run_r2d2_case(mode, a.B, a.T, a.burn_in, a.A, a.C, regime)
+            rows, facts = alp.run_r2d2_case(mode, a.B, a.T, a.burn_in, a.A, a.C, regime, L=a.lstm_size)
         else:
             rows, facts = alp.run_apex_case(a.family, mode, a.B, a.A, regime)
         for r in rows:
