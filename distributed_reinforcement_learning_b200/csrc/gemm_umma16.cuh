@@ -26,55 +26,16 @@
 //                     atom (g = mn / 64, kg = k / 8) at (kg * (ROWS / 64) + g) * 1024: LBO = 1024, SBO = (ROWS/64)*1024;
 //                     a K = 16 slice j covers k-groups 2j, 2j+1 and starts at 2 j SBO   (cute: make_gmma_desc<Major::MN>);
 //   * uint8 operands (the frames) are exact in fp16: one plane, two products, 16 bytes -> 16 halves with PRMT + HSUB2;
-//   * pre-tiled weight images are always K-major (retile_b16_kernel), whatever the weight's own layout.
+//   * pre-tiled weight images are always K-major (retile_b16_kernel), whatever the weight's own layout;
+//   * an A operand over a 16-bit plane (PlaneA, loaders.cuh: K-major, next to a pre-tiled B) is not gathered at all: the
+//     producers cp.async its hi and lo chunks into the stage and arrive on the full barrier when the copies land.
 #pragma once
 #include "gemm_umma.cuh"
+#include "split16.cuh"
 
 namespace drl {
 namespace umma16 {
 
-struct BF16 {
-  static constexpr uint32_t kFormat = 1;
-  static constexpr bool kBf16 = true;
-  __device__ static __forceinline__ uint32_t pack2(float lo_elem, float hi_elem) {
-    uint32_t r;
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));   // d = {a (upper), b (lower)}
-    return r;
-  }
-  __device__ static __forceinline__ float2 unpack2(uint32_t p) {
-    return make_float2(__uint_as_float(p << 16), __uint_as_float(p & 0xffff0000u));
-  }
-};
-struct F16 {
-  static constexpr uint32_t kFormat = 0;
-  static constexpr bool kBf16 = false;
-  __device__ static __forceinline__ uint32_t pack2(float lo_elem, float hi_elem) {
-    uint32_t r;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
-    return r;
-  }
-  __device__ static __forceinline__ float2 unpack2(uint32_t p) {
-    float2 f;
-    asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.f32.f16 %0, l;\n\tcvt.f32.f16 %1, h;\n\t}"
-        : "=f"(f.x), "=f"(f.y) : "r"(p));
-    return f;
-  }
-};
-
-// 8 consecutive fp32 values -> 8 hi halves + 8 lo halves (element i in the low/high half of word i/2, memory order)
-template <class F>
-__device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& hi, uint4& lo) {
-  const float x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-  uint32_t h[4], l[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    h[i] = F::pack2(x[2 * i], x[2 * i + 1]);
-    const float2 hf = F::unpack2(h[i]);
-    l[i] = F::pack2(x[2 * i] - hf.x, x[2 * i + 1] - hf.y);
-  }
-  hi = make_uint4(h[0], h[1], h[2], h[3]);
-  lo = make_uint4(l[0], l[1], l[2], l[3]);
-}
 // 4 bytes -> 4 fp16 (exact): PRMT builds 0x64bb = 1024 + b, one HSUB2 per pair removes the 1024
 __device__ __forceinline__ uint2 u8x4_to_h4(uint32_t w) {
   uint32_t p0 = __byte_perm(w, 0x64646464u, 0x4140), p1 = __byte_perm(w, 0x64646464u, 0x4342);
@@ -90,7 +51,24 @@ __device__ __forceinline__ void mma16(float (&d)[N / 2], uint64_t adesc, uint64_
   wg::Wg16<N, F::kBf16, TA, TB>::mma(d, adesc, bdesc, accumulate);
 }
 
+// 16 bytes global -> shared without registers; bytes = 0 fills the chunk with zeros
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, uint32_t bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(umma::smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes)
+               : "memory");
+}
+// one arrival on `bar` once every cp.async this thread issued so far has landed (counts against the barrier's own count)
+__device__ __forceinline__ void cp_async_arrive_noinc(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(umma::smem_u32(bar)) : "memory");
+}
+
 }  // namespace umma16
+
+// An A loader may declare `kPlane` (PlaneA, loaders.cuh): its operand is a 16-bit [hi | lo] plane in global memory, and
+// the producers copy its 16-byte chunks into the stages with cp.async instead of gathering fp32 into registers.
+template <class L, class = void>
+struct loader_plane : std::false_type {};
+template <class L>
+struct loader_plane<L, std::void_t<decltype(L::kPlane)>> : std::bool_constant<L::kPlane> {};
 
 // One 16-bit operand plane of a stage: ROWS x 64 elements = ROWS x 128 bytes.
 template <int ROWS, bool KMAJOR>
@@ -201,6 +179,8 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
   constexpr bool A16 = loader_vec16<AL>::value;              // uint8 operand fetched 16 elements per 128-bit load
   static_assert(!AEX || A16, "exact (uint8) operands use the 16-wide raw loads");
   constexpr bool LWB = BPT && Cfg::LW;
+  constexpr bool APL = loader_plane<AL>::value;              // A copied from a 16-bit plane (cp.async)
+  static_assert(!APL || (BPT && !EP::kColSum), "a plane A operand pairs with a pre-tiled B");
   // units per sub-tile: 8 elements of the contiguous dimension (16 for the raw uint8 loads)
   constexpr int NUA = BM * SUBK / (A16 ? 16 : 8), NUB = BN * SUBK / 8;
   constexpr int UA = NUA / NPROD, UB = BPT ? 1 : NUB / NPROD;
@@ -237,104 +217,30 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
   if (warp < Cfg::PW) {
     // ================= PRODUCERS =================
     if constexpr (Cfg::PREG > 0) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PREG));
-    // per-unit state: up to two Row handles (MN-major units span two 4-element loader groups), element offset inside
-    // the sub-tile along K, and the byte offset of the unit's 16-byte chunk inside the plane for sub-tile 0
-    typename AL::Row arow[UA][AR];
-    typename BL::Row brow[UB][2];
-    int a_k[UA], a_o[UA], b_k[UB], b_o[UB];
+    if constexpr (APL) {
+      // A from its plane: unit = (row r, 16-byte chunk c of the stage's K = 64), 8 lanes per row (128 contiguous bytes of
+      // hi and of lo for a row's K tile), UP rows per thread.  A stage's chunks are all in flight at once: the prefetch
+      // depth is the pipeline's STAGES, and no register holds operand data.
+      constexpr int UP = BM * (BK / 8) / NPROD;
+      static_assert(BM * (BK / 8) % NPROD == 0, "chunks must divide among the producer threads");
+      const int c = tid & 7;
+      typename AL::Row prow[UP];
+      int poff[UP];
 #pragma unroll
-    for (int i = 0; i < UA; ++i) {
-      const int u = tid + i * NPROD;
-      if constexpr (A16) {
-        if (AK) {     // unit = (row, 16-k half of the 32-k sub-tile); lanes = consecutive rows
-          const int r = u % BM, half = u / BM;
-          arow[i][0] = al.row(z, (m0 + r < M) ? m0 + r : -1);
-          a_k[i] = half * 16;
-          a_o[i] = r;
-        } else {      // unit = (k, 16 consecutive mn)
-          const int kk = u % SUBK, q16 = u / SUBK;
-          arow[i][0] = al.row(z, (m0 + q16 * 16 < M) ? m0 + q16 * 16 : -1);
-          a_k[i] = kk;
-          a_o[i] = q16 * 16;
-        }
-      } else if (AK) {
-        // 4 lanes cover one row's 32 k (128 contiguous bytes of fp32); rows are visited in the order 0,4,1,5,2,6,3,7
-        // within each group of 8 so that the two rows of a store phase (8 lanes) differ in bit 2 of (row & 7): their
-        // chunks then fall into different halves of the 128-byte bank window (conflict-free 16-byte stores)
-        const int c4 = u & 3, rs = (u >> 2) & 7, r = (u >> 5) * 8 + ((rs & 1) << 2) + (rs >> 1);
-        arow[i][0] = al.row(z, (m0 + r < M) ? m0 + r : -1);
-        a_k[i] = c4 * 8;
-        a_o[i] = r;
-      } else {
-        const int q = u % (BM / 8), kk = u / (BM / 8);
-        arow[i][0] = al.row(z, (m0 + q * 8 < M) ? m0 + q * 8 : -1);
-        arow[i][1] = al.row(z, (m0 + q * 8 + 4 < M) ? m0 + q * 8 + 4 : -1);
-        a_k[i] = kk;
-        a_o[i] = q * 8;
+      for (int i = 0; i < UP; ++i) {
+        const int r = (tid >> 3) + i * (NPROD / 8);
+        prow[i] = al.row(z, (m0 + r < M) ? m0 + r : -1);
+        poff[i] = TA::chunk_off(r, c * 8);
       }
-    }
-#pragma unroll
-    for (int i = 0; i < UB; ++i) {
-      const int u = tid + i * NPROD;
-      if constexpr (BPT) {
-        b_k[i] = 0; b_o[i] = 0;
-      } else if (BKc) {
-        const int c4 = u & 3, rs = (u >> 2) & 7, r = (u >> 5) * 8 + ((rs & 1) << 2) + (rs >> 1);
-        brow[i][0] = bl.row(z, (n0 + r < N) ? n0 + r : -1);
-        b_k[i] = c4 * 8;
-        b_o[i] = r;
-      } else {
-        const int q = u % (BN / 8), kk = u / (BN / 8);
-        brow[i][0] = bl.row(z, (n0 + q * 8 < N) ? n0 + q * 8 : -1);
-        brow[i][1] = bl.row(z, (n0 + q * 8 + 4 < N) ? n0 + q * 8 + 4 : -1);
-        b_k[i] = kk;
-        b_o[i] = q * 8;
-      }
-    }
-    float4 csum[UB][2];
-#pragma unroll
-    for (int i = 0; i < UB; ++i) { csum[i][0] = zero4(); csum[i][1] = zero4(); }
-
-    // gather sub-tile g (K range [k0 + 32 g, +32)) into registers
-    auto gload = [&](int g, ARaw (&ra)[UA][AR], float4 (&rb)[UB][2]) {
-      const int kb = k0 + g * SUBK;
-      if (tid == 0) TR(600 + g);
-#pragma unroll
-      for (int i = 0; i < UA; ++i) {
-        const int k = kb + a_k[i];
-        if constexpr (A16) {
-          ra[i][0] = (k < k1) ? al.load_raw16(arow[i][0], k) : make_uint4(0u, 0u, 0u, 0u);
-        } else if (AK) {
-          ra[i][0] = (k < k1) ? al.load(arow[i][0], k) : zero4();
-          ra[i][1] = (k + 4 < k1) ? al.load(arow[i][0], k + 4) : zero4();
-        } else {
-          ra[i][0] = (k < k1) ? al.load(arow[i][0], k) : zero4();
-          ra[i][1] = (k < k1) ? al.load(arow[i][1], k) : zero4();
-        }
-      }
-      if constexpr (!BPT) {
-#pragma unroll
-        for (int i = 0; i < UB; ++i) {
-          const int k = kb + b_k[i];
-          if (BKc) {
-            rb[i][0] = (k < k1) ? bl.load(brow[i][0], k) : zero4();
-            rb[i][1] = (k + 4 < k1) ? bl.load(brow[i][0], k + 4) : zero4();
-          } else {
-            rb[i][0] = (k < k1) ? bl.load(brow[i][0], k) : zero4();
-            rb[i][1] = (k < k1) ? bl.load(brow[i][1], k) : zero4();
-          }
-        }
-      }
-    };
-    // convert sub-tile g and store it into its stage; the second sub-tile of a stage publishes the stage
-    auto publish = [&](int g, const ARaw (&ra)[UA][AR], const float4 (&rb)[UB][2]) {
-      const int t = g >> 1, sub = g & 1;
-      const int s = t % STAGES;
-      uint8_t* st = smem + s * SM::STAGE_BYTES;
-      if (sub == 0) {
+      const uint16_t* hi = al.plane;
+      const uint16_t* lo = al.plane + al.count;
+#pragma unroll 1
+      for (int t = 0; t < ntiles; ++t) {
+        const int s = t % STAGES;
         umma::mbar_wait(&empty[s], ((t / STAGES) & 1) ^ 1);
-        if (tid == 0) TR(1000 + g);
-        if constexpr (BPT && !LWB) {
+        if (tid == 0) TR(1000 + 2 * t);
+        uint8_t* st = smem + s * SM::STAGE_BYTES;
+        if constexpr (!LWB) {
           if (tid == 0) {
             const int kt = (k0 + t * BK) / BK;
             umma::mbar_expect_tx(&full[s], 2 * SM::B_BYTES);
@@ -342,96 +248,216 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
                            2 * SM::B_BYTES, &full[s]);
           }
         }
-      }
-      const int ksub = sub * SUBK;   // element offset of this sub-tile inside the stage's K = 64
+        const int k = k0 + t * BK + c * 8;
 #pragma unroll
+        for (int i = 0; i < UP; ++i) {
+          const long long e = (k < k1) ? al.chunk(prow[i], k) : -1ll;
+          const uint32_t bytes = e >= 0 ? 16u : 0u;
+          const size_t o = e >= 0 ? (size_t)e : 0;
+          umma16::cp_async16(st + poff[i], hi + o, bytes);
+          umma16::cp_async16(st + OFF_ALO + poff[i], lo + o, bytes);
+        }
+        umma16::cp_async_arrive_noinc(&full[s]);
+        if (tid == 0) TR(2000 + 2 * t + 1);
+      }
+      asm volatile("cp.async.wait_all;" ::: "memory");
+    } else {
+      // per-unit state: up to two Row handles (MN-major units span two 4-element loader groups), element offset inside
+      // the sub-tile along K, and the byte offset of the unit's 16-byte chunk inside the plane for sub-tile 0
+      typename AL::Row arow[UA][AR];
+      typename BL::Row brow[UB][2];
+      int a_k[UA], a_o[UA], b_k[UB], b_o[UB];
+  #pragma unroll
       for (int i = 0; i < UA; ++i) {
+        const int u = tid + i * NPROD;
         if constexpr (A16) {
-          const uint2 h0 = umma16::u8x4_to_h4(ra[i][0].x), h1 = umma16::u8x4_to_h4(ra[i][0].y);
-          const uint2 h2 = umma16::u8x4_to_h4(ra[i][0].z), h3 = umma16::u8x4_to_h4(ra[i][0].w);
-          const int o0 = AK ? TA::chunk_off(a_o[i], ksub + a_k[i]) : TA::chunk_off(a_o[i], ksub + a_k[i]);
-          const int o1 = AK ? TA::chunk_off(a_o[i], ksub + a_k[i] + 8) : TA::chunk_off(a_o[i] + 8, ksub + a_k[i]);
-          *reinterpret_cast<uint4*>(st + o0) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-          *reinterpret_cast<uint4*>(st + o1) = make_uint4(h2.x, h2.y, h3.x, h3.y);
+          if (AK) {     // unit = (row, 16-k half of the 32-k sub-tile); lanes = consecutive rows
+            const int r = u % BM, half = u / BM;
+            arow[i][0] = al.row(z, (m0 + r < M) ? m0 + r : -1);
+            a_k[i] = half * 16;
+            a_o[i] = r;
+          } else {      // unit = (k, 16 consecutive mn)
+            const int kk = u % SUBK, q16 = u / SUBK;
+            arow[i][0] = al.row(z, (m0 + q16 * 16 < M) ? m0 + q16 * 16 : -1);
+            a_k[i] = kk;
+            a_o[i] = q16 * 16;
+          }
+        } else if (AK) {
+          // 4 lanes cover one row's 32 k (128 contiguous bytes of fp32); rows are visited in the order 0,4,1,5,2,6,3,7
+          // within each group of 8 so that the two rows of a store phase (8 lanes) differ in bit 2 of (row & 7): their
+          // chunks then fall into different halves of the 128-byte bank window (conflict-free 16-byte stores)
+          const int c4 = u & 3, rs = (u >> 2) & 7, r = (u >> 5) * 8 + ((rs & 1) << 2) + (rs >> 1);
+          arow[i][0] = al.row(z, (m0 + r < M) ? m0 + r : -1);
+          a_k[i] = c4 * 8;
+          a_o[i] = r;
         } else {
-          uint4 h, l;
-          umma16::split8<AF>(ra[i][0], ra[i][1], h, l);
-          const int off = TA::chunk_off(a_o[i], ksub + a_k[i]);
-          *reinterpret_cast<uint4*>(st + off) = h;
-          *reinterpret_cast<uint4*>(st + OFF_ALO + off) = l;
+          const int q = u % (BM / 8), kk = u / (BM / 8);
+          arow[i][0] = al.row(z, (m0 + q * 8 < M) ? m0 + q * 8 : -1);
+          arow[i][1] = al.row(z, (m0 + q * 8 + 4 < M) ? m0 + q * 8 + 4 : -1);
+          a_k[i] = kk;
+          a_o[i] = q * 8;
         }
       }
-      if constexpr (!BPT) {
-#pragma unroll
-        for (int i = 0; i < UB; ++i) {
-          uint4 h, l;
-          umma16::split8<BF>(rb[i][0], rb[i][1], h, l);
-          const int off = TB::chunk_off(b_o[i], ksub + b_k[i]);
-          *reinterpret_cast<uint4*>(st + OFF_BHI + off) = h;
-          *reinterpret_cast<uint4*>(st + OFF_BLO + off) = l;
-          if (kColSum) {
-            csum[i][0].x += rb[i][0].x; csum[i][0].y += rb[i][0].y; csum[i][0].z += rb[i][0].z; csum[i][0].w += rb[i][0].w;
-            csum[i][1].x += rb[i][1].x; csum[i][1].y += rb[i][1].y; csum[i][1].z += rb[i][1].z; csum[i][1].w += rb[i][1].w;
+  #pragma unroll
+      for (int i = 0; i < UB; ++i) {
+        const int u = tid + i * NPROD;
+        if constexpr (BPT) {
+          b_k[i] = 0; b_o[i] = 0;
+        } else if (BKc) {
+          const int c4 = u & 3, rs = (u >> 2) & 7, r = (u >> 5) * 8 + ((rs & 1) << 2) + (rs >> 1);
+          brow[i][0] = bl.row(z, (n0 + r < N) ? n0 + r : -1);
+          b_k[i] = c4 * 8;
+          b_o[i] = r;
+        } else {
+          const int q = u % (BN / 8), kk = u / (BN / 8);
+          brow[i][0] = bl.row(z, (n0 + q * 8 < N) ? n0 + q * 8 : -1);
+          brow[i][1] = bl.row(z, (n0 + q * 8 + 4 < N) ? n0 + q * 8 + 4 : -1);
+          b_k[i] = kk;
+          b_o[i] = q * 8;
+        }
+      }
+      float4 csum[UB][2];
+  #pragma unroll
+      for (int i = 0; i < UB; ++i) { csum[i][0] = zero4(); csum[i][1] = zero4(); }
+
+      // gather sub-tile g (K range [k0 + 32 g, +32)) into registers
+      auto gload = [&](int g, ARaw (&ra)[UA][AR], float4 (&rb)[UB][2]) {
+        const int kb = k0 + g * SUBK;
+        if (tid == 0) TR(600 + g);
+  #pragma unroll
+        for (int i = 0; i < UA; ++i) {
+          const int k = kb + a_k[i];
+          if constexpr (A16) {
+            ra[i][0] = (k < k1) ? al.load_raw16(arow[i][0], k) : make_uint4(0u, 0u, 0u, 0u);
+          } else if (AK) {
+            ra[i][0] = (k < k1) ? al.load(arow[i][0], k) : zero4();
+            ra[i][1] = (k + 4 < k1) ? al.load(arow[i][0], k + 4) : zero4();
+          } else {
+            ra[i][0] = (k < k1) ? al.load(arow[i][0], k) : zero4();
+            ra[i][1] = (k < k1) ? al.load(arow[i][1], k) : zero4();
+          }
+        }
+        if constexpr (!BPT) {
+  #pragma unroll
+          for (int i = 0; i < UB; ++i) {
+            const int k = kb + b_k[i];
+            if (BKc) {
+              rb[i][0] = (k < k1) ? bl.load(brow[i][0], k) : zero4();
+              rb[i][1] = (k + 4 < k1) ? bl.load(brow[i][0], k + 4) : zero4();
+            } else {
+              rb[i][0] = (k < k1) ? bl.load(brow[i][0], k) : zero4();
+              rb[i][1] = (k < k1) ? bl.load(brow[i][1], k) : zero4();
+            }
+          }
+        }
+      };
+      // convert sub-tile g and store it into its stage; the second sub-tile of a stage publishes the stage
+      auto publish = [&](int g, const ARaw (&ra)[UA][AR], const float4 (&rb)[UB][2]) {
+        const int t = g >> 1, sub = g & 1;
+        const int s = t % STAGES;
+        uint8_t* st = smem + s * SM::STAGE_BYTES;
+        if (sub == 0) {
+          umma::mbar_wait(&empty[s], ((t / STAGES) & 1) ^ 1);
+          if (tid == 0) TR(1000 + g);
+          if constexpr (BPT && !LWB) {
+            if (tid == 0) {
+              const int kt = (k0 + t * BK) / BK;
+              umma::mbar_expect_tx(&full[s], 2 * SM::B_BYTES);
+              umma::bulk_g2s(st + OFF_BHI, bl.image + ((size_t)blockIdx.y * bl.ktiles + kt) * (size_t)(2 * SM::B_BYTES),
+                             2 * SM::B_BYTES, &full[s]);
+            }
+          }
+        }
+        const int ksub = sub * SUBK;   // element offset of this sub-tile inside the stage's K = 64
+  #pragma unroll
+        for (int i = 0; i < UA; ++i) {
+          if constexpr (A16) {
+            const uint2 h0 = umma16::u8x4_to_h4(ra[i][0].x), h1 = umma16::u8x4_to_h4(ra[i][0].y);
+            const uint2 h2 = umma16::u8x4_to_h4(ra[i][0].z), h3 = umma16::u8x4_to_h4(ra[i][0].w);
+            const int o0 = AK ? TA::chunk_off(a_o[i], ksub + a_k[i]) : TA::chunk_off(a_o[i], ksub + a_k[i]);
+            const int o1 = AK ? TA::chunk_off(a_o[i], ksub + a_k[i] + 8) : TA::chunk_off(a_o[i] + 8, ksub + a_k[i]);
+            *reinterpret_cast<uint4*>(st + o0) = make_uint4(h0.x, h0.y, h1.x, h1.y);
+            *reinterpret_cast<uint4*>(st + o1) = make_uint4(h2.x, h2.y, h3.x, h3.y);
+          } else {
+            uint4 h, l;
+            umma16::split8<AF>(ra[i][0], ra[i][1], h, l);
+            const int off = TA::chunk_off(a_o[i], ksub + a_k[i]);
+            *reinterpret_cast<uint4*>(st + off) = h;
+            *reinterpret_cast<uint4*>(st + OFF_ALO + off) = l;
+          }
+        }
+        if constexpr (!BPT) {
+  #pragma unroll
+          for (int i = 0; i < UB; ++i) {
+            uint4 h, l;
+            umma16::split8<BF>(rb[i][0], rb[i][1], h, l);
+            const int off = TB::chunk_off(b_o[i], ksub + b_k[i]);
+            *reinterpret_cast<uint4*>(st + OFF_BHI + off) = h;
+            *reinterpret_cast<uint4*>(st + OFF_BLO + off) = l;
+            if (kColSum) {
+              csum[i][0].x += rb[i][0].x; csum[i][0].y += rb[i][0].y; csum[i][0].z += rb[i][0].z; csum[i][0].w += rb[i][0].w;
+              csum[i][1].x += rb[i][1].x; csum[i][1].y += rb[i][1].y; csum[i][1].z += rb[i][1].z; csum[i][1].w += rb[i][1].w;
+            }
+          }
+        }
+        if (sub == 1) {
+          umma::fence_proxy_async();
+          umma::mbar_arrive(&full[s]);
+        }
+        if (tid == 0) TR(2000 + g);
+      };
+
+      // register prefetch ring, in sub-tiles, within Cfg::PF_REGS registers
+      constexpr int RPS = 4 * UA * AR + (BPT ? 0 : 8 * UB);      // registers one gathered sub-tile occupies
+      constexpr int PF0 = Cfg::PFD > 0 ? Cfg::PFD : (A16 ? 4 : (BPT ? 3 : 2));
+      constexpr int PFR = Cfg::PF_REGS;
+      constexpr int PF = (PF0 * RPS <= PFR) ? PF0 : (PFR / RPS >= 1 ? PFR / RPS : 1);
+      const int nsub = 2 * ntiles;
+      ARaw ra[PF][UA][AR];
+      float4 rb[PF][UB][2];
+  #pragma unroll
+      for (int d = 0; d < PF - 1; ++d)
+        if (d < nsub) gload(d, ra[d], rb[d]);
+  #pragma unroll 1
+      for (int g0 = 0; g0 < nsub; g0 += PF) {
+  #pragma unroll
+        for (int u = 0; u < PF; ++u) {
+          const int g = g0 + u;
+          if (g < nsub) {
+            if (g + PF - 1 < nsub) gload(g + PF - 1, ra[(u + PF - 1) % PF], rb[(u + PF - 1) % PF]);
+            publish(g, ra[u], rb[u]);
           }
         }
       }
-      if (sub == 1) {
-        umma::fence_proxy_async();
-        umma::mbar_arrive(&full[s]);
-      }
-      if (tid == 0) TR(2000 + g);
-    };
 
-    // register prefetch ring, in sub-tiles, within Cfg::PF_REGS registers
-    constexpr int RPS = 4 * UA * AR + (BPT ? 0 : 8 * UB);      // registers one gathered sub-tile occupies
-    constexpr int PF0 = Cfg::PFD > 0 ? Cfg::PFD : (A16 ? 4 : (BPT ? 3 : 2));
-    constexpr int PFR = Cfg::PF_REGS;
-    constexpr int PF = (PF0 * RPS <= PFR) ? PF0 : (PFR / RPS >= 1 ? PFR / RPS : 1);
-    const int nsub = 2 * ntiles;
-    ARaw ra[PF][UA][AR];
-    float4 rb[PF][UB][2];
-#pragma unroll
-    for (int d = 0; d < PF - 1; ++d)
-      if (d < nsub) gload(d, ra[d], rb[d]);
-#pragma unroll 1
-    for (int g0 = 0; g0 < nsub; g0 += PF) {
-#pragma unroll
-      for (int u = 0; u < PF; ++u) {
-        const int g = g0 + u;
-        if (g < nsub) {
-          if (g + PF - 1 < nsub) gload(g + PF - 1, ra[(u + PF - 1) % PF], rb[(u + PF - 1) % PF]);
-          publish(g, ra[u], rb[u]);
+      // bias-gradient row: column sums of B (dY, exact fp32 values) over this CTA's K range, fixed order
+      if (kColSum && blockIdx.x == 0) {
+        // a thread's units all have q = tid % (BN / 8) (NPROD is a multiple of BN / 8): 8 columns per thread
+        float4 a0 = zero4(), a1 = zero4();
+  #pragma unroll
+        for (int i = 0; i < UB; ++i) {
+          a0.x += csum[i][0].x; a0.y += csum[i][0].y; a0.z += csum[i][0].z; a0.w += csum[i][0].w;
+          a1.x += csum[i][1].x; a1.y += csum[i][1].y; a1.z += csum[i][1].z; a1.w += csum[i][1].w;
+        }
+        cs_scratch[2 * tid] = a0;
+        cs_scratch[2 * tid + 1] = a1;
+        asm volatile("bar.sync 1, %0;" ::"n"(NPROD) : "memory");
+        if (tid < BN / 4) {     // thread handles 4 columns: q = tid / 2, half = tid & 1
+          const int q = tid >> 1, half = tid & 1;
+          float4 tot = zero4();
+          for (int j = q; j < NPROD; j += BN / 8) {
+            const float4 v = cs_scratch[2 * j + half];
+            tot.x += v.x; tot.y += v.y; tot.z += v.z; tot.w += v.w;
+          }
+          const int n = n0 + q * 8 + half * 4;
+          if (n < N) ep.store_colsum(z, n, tot.x);
+          if (n + 1 < N) ep.store_colsum(z, n + 1, tot.y);
+          if (n + 2 < N) ep.store_colsum(z, n + 2, tot.z);
+          if (n + 3 < N) ep.store_colsum(z, n + 3, tot.w);
         }
       }
-    }
 
-    // bias-gradient row: column sums of B (dY, exact fp32 values) over this CTA's K range, fixed order
-    if (kColSum && blockIdx.x == 0) {
-      // a thread's units all have q = tid % (BN / 8) (NPROD is a multiple of BN / 8): 8 columns per thread
-      float4 a0 = zero4(), a1 = zero4();
-#pragma unroll
-      for (int i = 0; i < UB; ++i) {
-        a0.x += csum[i][0].x; a0.y += csum[i][0].y; a0.z += csum[i][0].z; a0.w += csum[i][0].w;
-        a1.x += csum[i][1].x; a1.y += csum[i][1].y; a1.z += csum[i][1].z; a1.w += csum[i][1].w;
-      }
-      cs_scratch[2 * tid] = a0;
-      cs_scratch[2 * tid + 1] = a1;
-      asm volatile("bar.sync 1, %0;" ::"n"(NPROD) : "memory");
-      if (tid < BN / 4) {     // thread handles 4 columns: q = tid / 2, half = tid & 1
-        const int q = tid >> 1, half = tid & 1;
-        float4 tot = zero4();
-        for (int j = q; j < NPROD; j += BN / 8) {
-          const float4 v = cs_scratch[2 * j + half];
-          tot.x += v.x; tot.y += v.y; tot.z += v.z; tot.w += v.w;
-        }
-        const int n = n0 + q * 8 + half * 4;
-        if (n < N) ep.store_colsum(z, n, tot.x);
-        if (n + 1 < N) ep.store_colsum(z, n + 1, tot.y);
-        if (n + 2 < N) ep.store_colsum(z, n + 2, tot.z);
-        if (n + 3 < N) ep.store_colsum(z, n + 3, tot.w);
-      }
     }
-
   } else if (warp >= Cfg::PW + 8) {
     // ================= B LOADER (warp PW+8, Cfg::LW) =================
     if constexpr (LWB) {
@@ -465,6 +491,7 @@ gemm_umma16_kernel(const AL al, const BL bl, const EP ep, int M, int N, int K, i
     for (int t = 0; t < ntiles; ++t) {
       const int s = t % STAGES;
       umma::mbar_wait(&full[s], (t / STAGES) & 1);
+      if constexpr (APL) umma::fence_proxy_async();   // the plane chunks were written by cp.async (generic proxy)
       if (ct == 0) TR(3000 + t);
       const uint32_t st = umma::smem_u32(smem + s * SM::STAGE_BYTES);
       const uint64_t a_hi = umma::desc_at(da_base, st + a_off), a_lo = umma::desc_at(da_base, st + OFF_ALO + a_off);

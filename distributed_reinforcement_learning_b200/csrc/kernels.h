@@ -105,6 +105,10 @@ struct TrunkActs {
   float* a3;             // [M,3136]
   float* e1;             // [A,256]  relu(emb1)
   float* table;          // [A,256]  action-embedding table
+  // math mode 5: 16-bit [hi | lo] planes of a1 / a2 (Plane16, split16.cuh), written beside them by conv1_fwd / conv2_fwd
+  // and read by conv2_fwd / conv3_fwd; 2 x 2 bytes per element, nullptr where not kept
+  uint16_t* a1p = nullptr;
+  uint16_t* a2p = nullptr;
 };
 struct TrunkBwd {
   float* da3;            // [Mb,3136]
@@ -117,21 +121,29 @@ struct TrunkBwd {
   float* wg_part2;       // split-K partial slabs for the conv1 weight gradient (main stream)
   float* dcol = nullptr; // [Mb*81, 512] (conv2) / [Mb*49, 576] (conv3): per-output-pixel tap gradients before col2im
                          // (math modes 2 and 3; math mode 5 computes the conv data gradients without it)
+  // math mode 5: 16-bit planes of da3 / da2, written beside them by lstm_dgrad / conv3_dgrad and read by conv3_dgrad /
+  // conv2_dgrad (as TrunkActs::a1p)
+  uint16_t* da3p = nullptr;
+  uint16_t* da2p = nullptr;
 };
 // floats of wg_part / wg_part2 for Mb rows of C-channel frames: the largest split-K slab set of the conv weight gradients
 // in any math mode, at least the scratch of emb_backward
 size_t trunk_partial_floats(int Mb, int C);
 template <class H>
-int alloc_trunk_acts(H* h, TrunkActs& a, size_t M, size_t A) {
+int alloc_trunk_acts(H* h, TrunkActs& a, size_t M, size_t A, bool planes = false) {
   DRL_TRY(dev_alloc(h, &a.a1, M * 400 * 32));
   DRL_TRY(dev_alloc(h, &a.a2, M * 81 * 64));
   DRL_TRY(dev_alloc(h, &a.a3, M * Geo::FLAT));
   DRL_TRY(dev_alloc(h, &a.e1, A * Geo::EMB));
   DRL_TRY(dev_alloc(h, &a.table, A * Geo::EMB));
+  if (planes) {
+    DRL_TRY(dev_alloc(h, &a.a1p, 2 * M * 400 * 32));
+    DRL_TRY(dev_alloc(h, &a.a2p, 2 * M * 81 * 64));
+  }
   return DRL_OK;
 }
 template <class H>
-int alloc_trunk_bwd(H* h, TrunkBwd& b, size_t Mb, size_t A, int C, bool dcol) {
+int alloc_trunk_bwd(H* h, TrunkBwd& b, size_t Mb, size_t A, int C, bool dcol, bool planes = false) {
   DRL_TRY(dev_alloc(h, &b.da3, Mb * Geo::FLAT));
   DRL_TRY(dev_alloc(h, &b.du, Mb * Geo::EMB));
   DRL_TRY(dev_alloc(h, &b.dpre2, A * Geo::EMB));
@@ -142,6 +154,10 @@ int alloc_trunk_bwd(H* h, TrunkBwd& b, size_t Mb, size_t A, int C, bool dcol) {
   DRL_TRY(dev_alloc(h, &b.wg_part, wg));
   DRL_TRY(dev_alloc(h, &b.wg_part2, wg));
   if (dcol) DRL_TRY(dev_alloc(h, &b.dcol, Mb * 81 * 512));
+  if (planes) {
+    DRL_TRY(dev_alloc(h, &b.da3p, 2 * Mb * Geo::FLAT));
+    DRL_TRY(dev_alloc(h, &b.da2p, 2 * Mb * 81 * 64));
+  }
   return DRL_OK;
 }
 
@@ -235,10 +251,12 @@ size_t lstm_image_bytes(int which, int M, int Mb);
 int forward_launch_count();
 int backward_launch_count();
 // the IMPALA policy engine's convolutions (policy.cu): the math-mode-5 conv1 / conv2 / conv3 forward of net_forward over
-// n single frames on one stream, and the build of its conv2 / conv3 weight images (WeightImages slots 1 and 2 sizes)
+// n single frames on one stream, and the build of its conv2 / conv3 weight images (WeightImages slots 1 and 2 sizes);
+// a1p / a2p: the 16-bit planes of a1 / a2 (TrunkActs::a1p) for n rows
 int conv_images16(cudaStream_t s, const ParamLayout& pl, const float* params, uint8_t* img_conv2, uint8_t* img_conv3);
 int conv_forward16(cudaStream_t s, const ParamLayout& pl, const float* params, const uint8_t* img_conv2,
-                   const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3);
+                   const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3,
+                   uint16_t* a1p, uint16_t* a2p);
 // the Ape-X / A3C and R2D2 policy engines' convolutions (apex_policy.cu, r2d2_policy.cu; defined in r2d2.cu, whose
 // learner instantiates both channel counts): the math-mode-2 conv_forward_tf32 of layer_defs.cuh over n single frames
 // of pl.C channels, and conv_images_tf32

@@ -34,6 +34,11 @@ using Conv2DB = ConvDgradB<32, 64, 2, 4, 4>;
 using Conv2DE = EpConvDx<20, 20, 32, 2, 10, 10>;
 using Conv2DBm = ConvDgradBMerged<32, 64, 2, 4, 4>;     // math mode 5: the four parity classes as one GEMM, N = 128
 using Conv2DEm = EpConvDxMerged<20, 20, 32, 2, 10, 10>;
+// math mode 5: the same A operands read from the 16-bit planes of a1 / a2 / da3 / da2 (cp.async, no fp32 gather)
+using Conv2AP = PlaneA<Conv2A>;
+using Conv3AP = PlaneA<Conv3A>;
+using Conv3DAP = PlaneA<Conv3DA>;
+using Conv2DAP = PlaneA<Conv2DA>;
 
 // Every tensor-core configuration has two consumer warpgroups (256 threads) whose wgmma accumulators hold BN / 2 fp32
 // registers per thread, next to the producer warps, in one CTA per SM unless MINB says otherwise: BN = 256 (128
@@ -53,8 +58,9 @@ using U256L = U256;                    // (no loader warp: the same configuratio
 // other is an O(0.1) weight.
 using Fmt16 = umma16::BF16;     // every GEMM whose operands are fp32 activations / gradients / weights
 // Two CTAs per SM (MINB = 2, 106 KB of shared memory each): one CTA's pipeline fill and epilogue overlap the other's main
-// loop.  512 threads x 64 registers, split by role: 8 producer warps (the gathers are latency-bound) keep PREG registers and
-// issue the weight image's bulk copy themselves, the consumer warpgroups take the rest.
+// loop.  512 threads x 64 registers, split by role: 8 producer warps keep PREG registers and issue the weight image's bulk
+// copy themselves, the consumer warpgroups take the rest.  Fed from planes (PlaneA), the producers only compute addresses
+// and issue cp.async; the register prefetch ring of the fp32 gather path does not apply.
 using X64L2 = Umma16Cfg<64, 2, 2, 8, 0, Fmt16, Fmt16, 0, false, 56>;  // conv2 / conv3 fwd: 48 KB per K = 64 stage; producers
                                                                      // 56 (a prefetch ring of 2 sub-tiles), consumers 72
 using X64W8x2 = Umma16Cfg<64, 2, 1, 8, 0, Fmt16, Fmt16>;     // conv2 / conv3 weight gradients (both operands gathered)
@@ -63,13 +69,13 @@ using XH = Umma16Cfg<64, 4, 1, 8, 0, Fmt16, Fmt16>;          // head layers (K =
 using BK256 = Bulk16Cfg<256, 2>;       // 96 KB per stage (A 32 KB + B 64 KB), 2 stages
 using X256L = Umma16Cfg<256, 2, 1, 4, 0, Fmt16, Fmt16>;      // lstm fwd: 96 KB per stage
 using X128D = Umma16Cfg<128, 3, 1, 8, 1, Fmt16, Fmt16>;      // lstm data gradient: 64 KB per stage
-// conv data gradients (pre-tiled B, one K tile of 64 co per filter tap): per-tap partial sums added in tap order, the
-// rounding of the dCol GEMM + col2im of math modes 2 and 3.
-using X64T = Umma16Cfg<64, 2, 1, 8, 1, Fmt16, Fmt16, 0, true>;    // conv3: K = 9 taps x 64 co, N = 64 ci
-// conv2: K = 4 taps x 64 co, N = 4 parity classes x 32 ci, as two N tiles of (py, px = 0..1) x 32 ci, two CTAs per SM as
-// X64L2 (each N tile gathers the dY taps itself: ~59 MB more L2 reads at B = 32, T = 20).  The second register set (64
-// per consumer thread) leaves the producers 48 registers: no register prefetch beyond the sub-tile in flight.  (conv3's
-// data gradient measured slower this way, 0.070 -> 0.072 ms on an H100 SXM at 700 W, and keeps X64T.)
+// conv data gradients (pre-tiled B, one K tile of 64 co per filter tap, A copied from the da3 / da2 planes): per-tap
+// partial sums added in tap order, the rounding of the dCol GEMM + col2im of math modes 2 and 3.  Two CTAs per SM as
+// X64L2; the second register set (64 per consumer thread) leaves the producers 48 registers, which the plane copies'
+// addresses fit.  conv3: K = 9 taps x 64 co, N = 64 ci.  conv2: K = 4 taps x 64 co, N = 4 parity classes x 32 ci, as two
+// N tiles of (py, px = 0..1) x 32 ci (each N tile copies the dY taps itself: ~59 MB more L2 reads at B = 32, T = 20).
+// (conv3's data gradient with the fp32 register gather measured slower at two CTAs per SM than at one, 0.070 -> 0.072
+// ms; fed from its plane it measured faster, 0.057 -> 0.052 ms, on an H100 SXM at 700 W.)
 using X64T2 = Umma16Cfg<64, 2, 2, 8, 0, Fmt16, Fmt16, 0, true, 48>;
 
 // math mode 3 (experimental): the persistent, fully warp-specialised variant of each tensor-core configuration

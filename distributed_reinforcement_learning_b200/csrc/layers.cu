@@ -102,9 +102,9 @@ extern "C" int drl_debug_gemm16_residency(int32_t* out) {
   if (drl_device_count() < 1) { set_error("CUDA device not available (no CPU fallback)"); return DRL_ERR_CUDA; }
   using FwdB = PretiledB<PlainB>;
   using FwdE = EpBiasAct<true, true>;
-  DRL_TRY((umma16_resident_ctas<X64L2, Conv2A, FwdB, FwdE>(out + 0)));
-  DRL_TRY((umma16_resident_ctas<X64L2, Conv3A, FwdB, FwdE>(out + 1)));
-  DRL_TRY((umma16_resident_ctas<X64T2, Conv2DA, PretiledB<Conv2DBm>, Conv2DEm>(out + 2)));
+  DRL_TRY((umma16_resident_ctas<X64L2, Conv2AP, FwdB, FwdE>(out + 0)));
+  DRL_TRY((umma16_resident_ctas<X64L2, Conv3AP, FwdB, FwdE>(out + 1)));
+  DRL_TRY((umma16_resident_ctas<X64T2, Conv2DAP, PretiledB<Conv2DBm>, Conv2DEm>(out + 2)));
   return DRL_OK;
 }
 
@@ -217,19 +217,22 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
   // attention_CNN (model/impala_actor_critic.py:6-10): u8 frames -> a1 [M,20,20,32] -> a2 [M,9,9,64] -> a3 [M,7,7,64]
   // = flatten HWC [M,3136]; conv2 waits for its weight image, conv3 for its own in math mode 5
   if (m16) {
+    // a1 and a2 are written with their 16-bit planes, from which conv2 / conv3 copy their A tiles
+    const size_t n1 = (size_t)M * 400 * 32, n2 = (size_t)M * 81 * 64;
     prof_mark(s, "conv1_fwd");
-    DRL_TRY(launch_conv1_fwd_tma(s, in.frames, M, map, P + pl.conv1_w, EpConv1{act.a1, 32, P + pl.conv1_b}));
+    DRL_TRY(launch_conv1_fwd_tma(s, in.frames, M, map, P + pl.conv1_w,
+                                 EpConv1{act.a1, 32, P + pl.conv1_b, Plane16{act.a1p, n1}}));
     ++n;
     if (retile && st.par) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[7], 0));
     {
-      Conv2A al{act.a1, map};
+      Conv2AP al{Conv2A{act.a1, map}, act.a1, act.a1p, n1};
       PretiledB<PlainB> blp{wi.img[1], 512 / 64};
-      EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
+      EpBiasAct<true, true> ep{act.a2, 64, 0, P + pl.conv2_b, 0, 1.0f, Plane16{act.a2p, n2}};
       GEMM16("conv2_fwd", X64L2, al, blp, ep, M * 81, 64, 512, 1, 512, 0);
     }
     if (c3_event) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[4], 0));
     {
-      Conv3A al{act.a2, map};
+      Conv3AP al{Conv3A{act.a2, map}, act.a2, act.a2p, n2};
       PretiledB<PlainB> blp{wi.img[2], 576 / 64};
       EpBiasAct<true, true> ep{act.a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
       GEMM16("conv3_fwd", X64L2, al, blp, ep, M * 49, 64, 576, 1, 576, 0);
@@ -297,17 +300,19 @@ int conv_images16(cudaStream_t s, const ParamLayout& pl, const float* P, uint8_t
 }
 
 int conv_forward16(cudaStream_t s, const ParamLayout& pl, const float* P, const uint8_t* img_conv2,
-                   const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3) {
+                   const uint8_t* img_conv3, const uint8_t* frames, int n, float* a1, float* a2, float* a3,
+                   uint16_t* a1p, uint16_t* a2p) {
   const RowMap map{n, 1};
-  DRL_TRY(launch_conv1_fwd_tma(s, frames, n, map, P + pl.conv1_w, EpConv1{a1, 32, P + pl.conv1_b}));
+  const size_t n1 = (size_t)n * 400 * 32, n2 = (size_t)n * 81 * 64;
+  DRL_TRY(launch_conv1_fwd_tma(s, frames, n, map, P + pl.conv1_w, EpConv1{a1, 32, P + pl.conv1_b, Plane16{a1p, n1}}));
   {
-    Conv2A al{a1, map};
+    Conv2AP al{Conv2A{a1, map}, a1, a1p, n1};
     PretiledB<PlainB> blp{img_conv2, 512 / 64};
-    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f};
+    EpBiasAct<true, true> ep{a2, 64, 0, P + pl.conv2_b, 0, 1.0f, Plane16{a2p, n2}};
     DRL_TRY((launch_gemm_umma16<X64L2>(s, al, blp, ep, n * 81, 64, 512, 1, 512, 0)));
   }
   {
-    Conv3A al{a2, map};
+    Conv3AP al{Conv3A{a2, map}, a2, a2p, n2};
     PretiledB<PlainB> blp{img_conv3, 576 / 64};
     EpBiasAct<true, true> ep{a3, 64, 0, P + pl.conv3_b, 0, 1.0f};
     DRL_TRY((launch_gemm_umma16<X64L2>(s, al, blp, ep, n * 49, 64, 576, 1, 576, 0)));
@@ -338,10 +343,10 @@ static int conv_backward16(const Streams& st, const ParamLayout& pl, const Weigh
     // gather form: rows = input pixels, K = 9 taps x 64 output channels (taps outside the output are zero), ReLU mask of
     // a2 in the epilogue; each tap's partial sum is rounded to fp32 and the taps are added in (ky, kx) order, as
     // col2im_conv3 adds the dCol of math modes 2 and 3: the same da2, bit for bit
-    Conv3DA al{bw.da3};
+    Conv3DAP al{Conv3DA{bw.da3}, bw.da3, bw.da3p, (size_t)Mb * Geo::FLAT};
     PretiledB<Conv3DB> blp{wi.img[5], 576 / 64};
-    Conv3DE ep{bw.da2, act.a2};
-    GEMM16("conv3_dgrad", X64T, al, blp, ep, Mb * 81, 64, 576, 1, 576, 0);
+    Conv3DE ep{bw.da2, act.a2, Plane16{bw.da2p, (size_t)Mb * 81 * 64}};
+    GEMM16("conv3_dgrad", X64T2, al, blp, ep, Mb * 81, 64, 576, 1, 576, 0);
   }
   DRL_TRY(fork_to_side(st, 5));
   s = st.par ? st.side : st.main;
@@ -359,7 +364,7 @@ static int conv_backward16(const Streams& st, const ParamLayout& pl, const Weigh
     // merged-phase gather form: row = the 2 x 2 block of input pixels (2i + py, 2j + px); all four parity classes read
     // the same dY taps (i - a, j - b), so K = (a, b, co) = 256 and N = (py, px, ci) = 128, in two N tiles (py = 0, 1);
     // ReLU mask of a1 in the epilogue; per-tap partial sums added in (a, b) order, as in col2im_conv2
-    Conv2DA al{bw.da2};
+    Conv2DAP al{Conv2DA{bw.da2}, bw.da2, bw.da2p, (size_t)Mb * 81 * 64};
     PretiledB<Conv2DBm> blp{wi.img[6], 256 / 64};
     Conv2DEm ep{{bw.da1, act.a1}};
     GEMM16("conv2_dgrad", X64T2, al, blp, ep, Mb * 100, 128, 256, 1, 256, 0);
@@ -480,7 +485,7 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
   {  // d[a3 | emb] = dz W[:3392]^T  (h0, c0 are fed data: no gradient, agent/impala.py:38-39)
     PlainA al{bw.dz, Geo::G4, 0};
     PlainBT bl{P + pl.lstm_w, Geo::G4, 0};
-    EpLstmDx ep{bw.da3, act.a3, bw.du};
+    EpLstmDx ep{bw.da3, act.a3, bw.du, Plane16{bw.da3p, (size_t)Mb * Geo::FLAT}};   // plane: math mode 5 only
     PretiledB<PlainBT> blp{wi.img[4], m16 ? Geo::G4 / 64 : Geo::G4 / 32};
     if (m16) GEMM16("lstm_dgrad", X128D, al, blp, ep, Mb, Geo::FLAT + Geo::EMB, Geo::G4, 1, Geo::G4, 0);
     else GEMM_W("lstm_dgrad", CfgMid, U128L, al, bl, blp, ep, Mb, Geo::FLAT + Geo::EMB, Geo::G4, 1, Geo::G4, 0);

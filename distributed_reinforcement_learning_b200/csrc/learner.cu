@@ -234,7 +234,7 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
       DRL_CUDA_CHECK(cudaMemcpy(h->ms, ones.data(), NP * sizeof(float), cudaMemcpyHostToDevice));
     }
     Acts& a = h->act;
-    DRL_TRY(alloc_trunk_acts(h, a, M, A));
+    DRL_TRY(alloc_trunk_acts(h, a, M, A, h->mode == 5));
     DRL_TRY(dev_alloc(h, &a.zpart, (size_t)kLstmSplits * M * Geo::G4));
     DRL_TRY(dev_alloc(h, &a.gates, M * Geo::G4));
     DRL_TRY(dev_alloc(h, &a.c1, M * Geo::L));
@@ -256,7 +256,7 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     DRL_TRY(dev_alloc(h, &b.dhid1, 2 * Mb * Geo::HID));
     DRL_TRY(dev_alloc(h, &b.dh_part, 2 * Mb * Geo::L));
     DRL_TRY(dev_alloc(h, &b.dz, Mb * Geo::G4));
-    DRL_TRY(alloc_trunk_bwd(h, b, Mb, A, Geo::IC, h->mode != 5));
+    DRL_TRY(alloc_trunk_bwd(h, b, Mb, A, Geo::IC, h->mode != 5, h->mode == 5));
     b.wg_part_floats = trunk_partial_floats((int)Mb, Geo::IC);
     DRL_TRY(dev_alloc(h, &b.emb_scratch, (size_t)16 * 32 * 256));
     {
@@ -646,7 +646,12 @@ int drl_learner_read_buffer(drl_learner* h, const char* name, float* host_dst, i
       {"dlogits", h->bwd.dlogits, Mb * 32}, {"dv", h->bwd.dv, Mb * 32}, {"dhid2", h->bwd.dhid2, 2 * Mb * Geo::HID},
       {"dhid1", h->bwd.dhid1, 2 * Mb * Geo::HID}, {"dh_part", h->bwd.dh_part, 2 * Mb * Geo::L},
       {"dz", h->bwd.dz, Mb * Geo::G4}, {"da3", h->bwd.da3, Mb * Geo::FLAT}, {"du", h->bwd.du, Mb * Geo::EMB},
-      {"da2", h->bwd.da2, Mb * 81 * 64}, {"da1", h->bwd.da1, Mb * 400 * 32}};
+      {"da2", h->bwd.da2, Mb * 81 * 64}, {"da1", h->bwd.da1, Mb * 400 * 32},
+      // math mode 5's 16-bit planes, [hi | lo] bf16 (2 x 2 bytes per element: the buffer's count in 4-byte words)
+      {"a1_plane", reinterpret_cast<float*>(h->act.a1p), M * 400 * 32},
+      {"a2_plane", reinterpret_cast<float*>(h->act.a2p), M * 81 * 64},
+      {"da3_plane", reinterpret_cast<float*>(h->bwd.da3p), Mb * Geo::FLAT},
+      {"da2_plane", reinterpret_cast<float*>(h->bwd.da2p), Mb * 81 * 64}};
   return read_named_buffer(h, tab, sizeof(tab) / sizeof(tab[0]), name, host_dst, n);
 }
 

@@ -445,6 +445,7 @@ int read_named_buffer(LearnerCore* h, const NamedBuffer* tab, int ntab, const ch
     const NamedBuffer& e = tab[i];
     if (strcmp(e.name, name) != 0) continue;
     if ((size_t)n != e.count) { set_error("read_buffer(%s): expected %zu floats, got %lld", name, e.count, (long long)n); return DRL_ERR_INVALID; }
+    if (e.p == nullptr) { set_error("read_buffer(%s): not kept in this math mode", name); return DRL_ERR_INVALID; }
     DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
     DRL_CUDA_CHECK(cudaMemcpy(host_dst, e.p, e.count * sizeof(float), cudaMemcpyDeviceToHost));
     return DRL_OK;

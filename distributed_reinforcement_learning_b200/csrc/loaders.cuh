@@ -6,6 +6,7 @@
 // [B,T,...] layout and are addressed through the (t,b) -> b*T+t remap.
 #pragma once
 #include "common.cuh"
+#include "split16.cuh"
 
 namespace drl {
 
@@ -57,11 +58,16 @@ struct ConvFwdA {
     r.base = x + (size_t)simg * (IH * IW * C) + ((oy * S) * IW + ox * S) * C;
     return r;
   }
-  __device__ __forceinline__ float4 load(const Row& r, int k) const {
-    if (r.base == nullptr) return zero4();
+  // address of element k of row r (nullptr: the row is out of range); a run of KW*C elements along k is contiguous
+  __device__ __forceinline__ const T* addr(const Row& r, int k) const {
+    if (r.base == nullptr) return nullptr;
     const int ky = k / (KW * C);
     const int rr = k - ky * (KW * C);
-    const T* p = r.base + ky * (IW * C) + rr;
+    return r.base + ky * (IW * C) + rr;
+  }
+  __device__ __forceinline__ float4 load(const Row& r, int k) const {
+    const T* p = addr(r, k);
+    if (p == nullptr) return zero4();
     if constexpr (sizeof(T) == 1) {
       return u8x4_to_f4(__ldg(reinterpret_cast<const uchar4*>(p)));
     } else {
@@ -139,14 +145,19 @@ struct ConvDgradA {
     r.xx = p - r.yy * RW;
     return r;
   }
-  __device__ __forceinline__ float4 load(const Row& r, int k) const {
-    if (r.img < 0) return zero4();
+  // address of element k of row r (nullptr: row out of range or tap outside the output: zero); CO elements per tap
+  __device__ __forceinline__ const float* addr(const Row& r, int k) const {
+    if (r.img < 0) return nullptr;
     const int tap = k / CO;
     const int co = k - tap * CO;
     const int jy = tap / TW, jx = tap - jy * TW;
     const int oy = r.yy - jy, ox = r.xx - jx;
-    if (oy < 0 || oy >= OH || ox < 0 || ox >= OW) return zero4();
-    return __ldg(reinterpret_cast<const float4*>(dy + ((size_t)(r.img * OH + oy) * OW + ox) * CO + co));
+    if (oy < 0 || oy >= OH || ox < 0 || ox >= OW) return nullptr;
+    return dy + ((size_t)(r.img * OH + oy) * OW + ox) * CO + co;
+  }
+  __device__ __forceinline__ float4 load(const Row& r, int k) const {
+    const float* p = addr(r, k);
+    return p ? __ldg(reinterpret_cast<const float4*>(p)) : zero4();
   }
 };
 // Matching B operand: B(k=(tap,co), n=ci) = W[ky, kx, ci, co], contiguous along co (= along k).
@@ -182,6 +193,28 @@ struct ConvDgradBMerged {
   using Row = typename ConvDgradB<CI, CO, S, KH, KW>::Row;
   __device__ __forceinline__ Row row(int, int n) const { return n < 0 ? b.row(0, -1) : b.row(n / CI, n % CI); }
   __device__ __forceinline__ float4 load(const Row& r, int k) const { return b.load(r, k); }
+};
+
+// A K-major A operand read from the 16-bit plane (Plane16) of the fp32 buffer `base` that loader L gathers from: the same
+// rows and the same gather addresses as L, as element indices into the plane.  gemm_umma16_kernel copies each 16-byte
+// chunk (8 consecutive k: L's contiguous runs along k are multiples of 8 long) of hi and of lo straight into the stage
+// with cp.async: no operand registers, no conversion, and the bits of the fp32 path.
+template <class L>
+struct PlaneA {
+  static_assert(L::kContigK, "plane operands are K-major");
+  static constexpr bool kContigK = true;
+  static constexpr bool kPlane = true;
+  L l;
+  const float* base;        // the fp32 buffer L reads
+  const uint16_t* plane;    // its [hi | lo] plane
+  size_t count;             // elements of the buffer (offset of the lo half)
+  using Row = typename L::Row;
+  __device__ __forceinline__ Row row(int z, int m) const { return l.row(z, m); }
+  // element index of the chunk [k, k + 8) of row r (k a multiple of 8), or -1: zero
+  __device__ __forceinline__ long long chunk(const Row& r, int k) const {
+    const float* p = l.addr(r, k);
+    return p ? (long long)(p - base) : -1ll;
+  }
 };
 
 // --------------------------------------------------------------------------------------------
@@ -371,6 +404,7 @@ struct EpBiasAct {
   float* c; int ldc; size_t sz;
   const float* bias; size_t sbias;
   float scale;
+  Plane16 plane{};   // optional 16-bit plane of c
   template <int V>
   __device__ __forceinline__ void store(int z, int m, int n, const float (&v)[V]) const {
     float o[V];
@@ -381,8 +415,13 @@ struct EpBiasAct {
       o[j] = RELU ? fmaxf(t, 0.f) : t;
     }
     const size_t off = z * sz + (size_t)m * ldc + n;
-    if constexpr (V == 4) *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
-    else c[off] = o[0];
+    if constexpr (V == 4) {
+      *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
+      plane.store4(off, o[0], o[1], o[2], o[3]);
+    } else {
+      c[off] = o[0];
+      plane.store1(off, o[0]);
+    }
   }
   // hoisted-bias form used by the tensor-core epilogues (epilogue_store_32x32)
   __device__ __forceinline__ float4 bias4(int z, int n) const {
@@ -398,6 +437,7 @@ struct EpBiasAct {
     }
     const size_t off = z * sz + (size_t)m * ldc + n;
     *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
+    plane.store4(off, o[0], o[1], o[2], o[3]);
   }
   __device__ __forceinline__ void store_colsum(int, int, float) const {}
 };
@@ -416,14 +456,20 @@ struct EpConv1 {
   static constexpr bool kColSum = false;
   float* c; int ldc;
   const float* bias;
+  Plane16 plane{};   // optional 16-bit plane of c
   template <int V>
   __device__ __forceinline__ void store(int, int m, int n, const float (&v)[V]) const {
     float o[V];
 #pragma unroll
     for (int j = 0; j < V; ++j) o[j] = fmaxf(div255(v[j]) + __ldg(bias + n + j), 0.f);
     const size_t off = (size_t)m * ldc + n;
-    if constexpr (V == 4) *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
-    else c[off] = o[0];
+    if constexpr (V == 4) {
+      *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
+      plane.store4(off, o[0], o[1], o[2], o[3]);
+    } else {
+      c[off] = o[0];
+      plane.store1(off, o[0]);
+    }
   }
   __device__ __forceinline__ float4 bias4(int, int n) const { return __ldg(reinterpret_cast<const float4*>(bias + n)); }
   __device__ __forceinline__ void store4b(int, int m, int n, const float (&v)[4], const float4& b) const {
@@ -433,6 +479,7 @@ struct EpConv1 {
     for (int j = 0; j < 4; ++j) o[j] = fmaxf(div255(v[j]) + bb[j], 0.f);
     const size_t off = (size_t)m * ldc + n;
     *reinterpret_cast<float4*>(c + off) = make_float4(o[0], o[1], o[2], o[3]);
+    plane.store4(off, o[0], o[1], o[2], o[3]);
   }
   __device__ __forceinline__ void store_colsum(int, int, float) const {}
 };
@@ -485,14 +532,17 @@ struct EpReluMask {
 struct EpLstmDx {
   static constexpr bool kColSum = false;
   float* da3; const float* a3; float* du;
+  Plane16 plane{};   // optional 16-bit plane of da3
   template <int V>
   __device__ __forceinline__ void store(int, int m, int n, const float (&v)[V]) const {
     if constexpr (V == 4) {          // FLAT and EMB are multiples of 4: a 4-group never straddles the boundary
       if (n < Geo::FLAT) {
         const size_t o = (size_t)m * Geo::FLAT + n;
         const float4 a = __ldg(reinterpret_cast<const float4*>(a3 + o));
-        *reinterpret_cast<float4*>(da3 + o) = make_float4(a.x > 0.f ? v[0] : 0.f, a.y > 0.f ? v[1] : 0.f,
-                                                          a.z > 0.f ? v[2] : 0.f, a.w > 0.f ? v[3] : 0.f);
+        const float4 d = make_float4(a.x > 0.f ? v[0] : 0.f, a.y > 0.f ? v[1] : 0.f, a.z > 0.f ? v[2] : 0.f,
+                                     a.w > 0.f ? v[3] : 0.f);
+        *reinterpret_cast<float4*>(da3 + o) = d;
+        plane.store4(o, d.x, d.y, d.z, d.w);
       } else {
         *reinterpret_cast<float4*>(du + (size_t)m * Geo::EMB + (n - Geo::FLAT)) = make_float4(v[0], v[1], v[2], v[3]);
       }
@@ -503,7 +553,9 @@ struct EpLstmDx {
       const int nn = n + j;
       if (nn < Geo::FLAT) {
         const size_t o = (size_t)m * Geo::FLAT + nn;
-        da3[o] = (__ldg(a3 + o) > 0.f) ? v[j] : 0.f;
+        const float d = (__ldg(a3 + o) > 0.f) ? v[j] : 0.f;
+        da3[o] = d;
+        plane.store1(o, d);
       } else {
         du[(size_t)m * Geo::EMB + (nn - Geo::FLAT)] = v[j];
       }
@@ -516,6 +568,7 @@ template <int IH, int IW, int CI, int S, int RH, int RW>
 struct EpConvDx {
   static constexpr bool kColSum = false;
   float* dx; const float* act;
+  Plane16 plane{};   // optional 16-bit plane of dx
   template <int V>
   __device__ __forceinline__ void store(int z, int m, int n, const float (&v)[V]) const {
     const int img = m / (RH * RW);
@@ -525,11 +578,17 @@ struct EpConvDx {
     const size_t o = ((size_t)(img * IH + yy * S + py) * IW + (xx * S + px)) * CI + n;
     if constexpr (V == 4) {          // CI is a multiple of 4 and n a multiple of 4: 16-byte aligned
       const float4 a = __ldg(reinterpret_cast<const float4*>(act + o));
-      *reinterpret_cast<float4*>(dx + o) = make_float4(a.x > 0.f ? v[0] : 0.f, a.y > 0.f ? v[1] : 0.f,
-                                                       a.z > 0.f ? v[2] : 0.f, a.w > 0.f ? v[3] : 0.f);
+      const float4 d = make_float4(a.x > 0.f ? v[0] : 0.f, a.y > 0.f ? v[1] : 0.f, a.z > 0.f ? v[2] : 0.f,
+                                   a.w > 0.f ? v[3] : 0.f);
+      *reinterpret_cast<float4*>(dx + o) = d;
+      plane.store4(o, d.x, d.y, d.z, d.w);
     } else {
 #pragma unroll
-      for (int j = 0; j < V; ++j) dx[o + j] = (__ldg(act + o + j) > 0.f) ? v[j] : 0.f;
+      for (int j = 0; j < V; ++j) {
+        const float d = (__ldg(act + o + j) > 0.f) ? v[j] : 0.f;
+        dx[o + j] = d;
+        plane.store1(o + j, d);
+      }
     }
   }
   __device__ __forceinline__ void store_colsum(int, int, float) const {}

@@ -312,7 +312,8 @@ int enqueue_forward(drl_policy* h, int n, const PolicyOutRows& out, drl_policy_r
   cudaStream_t s = h->stream;
   const int32_t* pa = reinterpret_cast<const int32_t*>(h->d_in + l.pa);
   const float* h0 = reinterpret_cast<const float*>(h->d_in + l.h0);
-  DRL_TRY(conv_forward16(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3));
+  DRL_TRY(conv_forward16(s, pl, P, h->img_conv2, h->img_conv3, h->d_in + l.frames, n, h->a1, h->a2, h->a3,
+                         h->a1p, h->a2p));
   DRL_TRY((launch_policy_lstm<Geo::L, kLSplits>(s, h->a3, h->table, pa, h0, P + pl.lstm_w, h->zpart, n)));
   HeadArgs a;
   a.zpart = h->zpart;

@@ -58,6 +58,8 @@ int policy_core_init(PolicyCore* h, int (*set_attributes)(), size_t zpart_floats
     DRL_TRY(dev_alloc(h, &h->a1, MB * 400 * 32));
     DRL_TRY(dev_alloc(h, &h->a2, MB * 81 * 64));
     DRL_TRY(dev_alloc(h, &h->a3, MB * Geo::FLAT));
+    DRL_TRY(dev_alloc(h, &h->a1p, 2 * MB * 400 * 32));
+    DRL_TRY(dev_alloc(h, &h->a2p, 2 * MB * 81 * 64));
     DRL_TRY(dev_alloc(h, &h->zpart, zpart_floats));
     DRL_TRY(dev_alloc(h, &h->d_in, in_bytes));
     DRL_CUDA_CHECK(cudaHostAlloc((void**)&h->h_in, in_bytes, cudaHostAllocDefault));

@@ -45,6 +45,7 @@ struct PolicyCore {
   float* e1 = nullptr;           // [A,256] relu(emb1), scratch of emb_forward
   float* table = nullptr;        // [A,256] action-embedding table (depends on the parameters only)
   float *a1 = nullptr, *a2 = nullptr, *a3 = nullptr;   // conv activations of max_batch rows
+  uint16_t *a1p = nullptr, *a2p = nullptr;              // 16-bit planes of a1 / a2 (conv_forward16)
   float* zpart = nullptr;        // split-K partial sums of the family's first skinny GEMM
   uint8_t* d_in = nullptr;       // device input block (the family's layout)
   uint8_t* h_in = nullptr;       // pinned staging of the same block
