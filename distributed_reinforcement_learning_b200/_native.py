@@ -32,7 +32,8 @@ class LearnerConfig(C.Structure):
                 ("end_learning_rate", C.c_float), ("learning_frame", C.c_double),
                 ("baseline_loss_coef", C.c_float), ("entropy_coef", C.c_float),
                 ("gradient_clip_norm", C.c_float), ("reward_clipping", C.c_int32), ("device", C.c_int32),
-                ("num_slots", C.c_int32), ("use_cuda_graph", C.c_int32), ("math_mode", C.c_int32)]
+                ("num_slots", C.c_int32), ("use_cuda_graph", C.c_int32), ("math_mode", C.c_int32),
+                ("recurrent", C.c_int32)]
 
 
 class StepOut(C.Structure):

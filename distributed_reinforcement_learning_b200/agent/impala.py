@@ -53,6 +53,7 @@ class Agent:
         self.reward_clipping = reward_clipping
         self.model_name = model_name
         self.learner_name = learner_name
+        self.recurrent = False         # set_recurrent
         self.device = int(os.environ.get("LOCAL_RANK", "0"))
         # the whole step is one CUDA graph by default (the benchmarked path); DRL_B200_CUDA_GRAPH=0 launches eagerly
         self.use_cuda_graph = os.environ.get("DRL_B200_CUDA_GRAPH", "1") != "0"
@@ -94,10 +95,24 @@ class Agent:
                 end_learning_rate=self.end_learning_rate, learning_frame=self.learning_frame,
                 baseline_loss_coef=self.baseline_loss_coef, entropy_coef=self.entropy_coef,
                 gradient_clip_norm=self.gradient_clip_norm, reward_clipping=self.reward_clipping,
-                device=self.device, num_slots=2, use_cuda_graph=self.use_cuda_graph)
+                device=self.device, num_slots=2, use_cuda_graph=self.use_cuda_graph, recurrent=self.recurrent)
             self._engine.set_params(self._params)
             self._engine.set_opt_state(self._ms, self._step)
         return self._engine
+
+    def set_recurrent(self, recurrent=True):
+        """Choose how ``train`` / ``train_from_queue`` treat the LSTM (the constructor keeps the reference's 14
+        arguments).  False (the default) trains as the reference does: one LSTM step from each step's recorded (h, c).
+        True unrolls the LSTM through each trajectory with BPTT, restarting from the recorded state after every done
+        (NativeLearner(recurrent=True), DESIGN.md section 21).  Parameters, RMSProp state and checkpoints are the same in
+        both modes: switching keeps them and rebuilds the learner engine at the next step."""
+        with self._lock:
+            recurrent = bool(recurrent)
+            if recurrent != self.recurrent and self._engine is not None:
+                self._pull_state()
+                self._engine.close()
+                self._engine = None
+            self.recurrent = recurrent
 
     # ---- reference API ---------------------------------------------------------------
     def save_weights(self, path):

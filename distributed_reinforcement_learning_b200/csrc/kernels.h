@@ -174,6 +174,10 @@ struct Acts : TrunkActs { // forward activations, time-major rows m = t*B + b, M
   float* value;          // [M]
   // math mode 5, bulk-fed lstm_wgrad (gemm_bulk16.cuh): x^T = [a3|emb|h0]^T as a 16-bit operand image
   uint8_t* img_xt = nullptr;   // x^T : rows = features (3648) x K = Mb rows -- A operand of lstm_wgrad
+  // recurrent mode only (Recurrence): the summed input half of the pre-activation and the state each step read
+  float* zx = nullptr;         // [M,1024] [a3 | emb] W[:3392]
+  float* hin = nullptr;        // [M,256]
+  float* cin = nullptr;        // [M,256]
 };
 
 struct Bwd : TrunkBwd {  // backward workspace, Mb = B*(T-2) rows
@@ -241,11 +245,20 @@ struct Streams {
   cudaEvent_t ev_lstm_grads = nullptr;   // backward: recorded on the side stream once the head and LSTM weight gradients
                                          // are in the bucket (the early part of the peer exchange waits for it)
 };
+// The IMPALA learner's recurrent mode (drl_learner_config.recurrent = 1): the LSTM runs through the T steps of each
+// trajectory on the cluster kernels of r2d2_cluster.cuh (RESTART variant), which the device places this many clusters of
+// at once.  Zero clusters: the stored-state mode, one LSTM step per row from the recorded (h, c).
+struct Recurrence {
+  int clusters_fwd = 0, clusters_bwd = 0;
+  bool on() const { return clusters_fwd > 0; }
+};
+// Create-time set-up of the recurrent mode's kernels (dynamic shared memory, occupancy); DRL_ERR_CUDA if no cluster fits
+int impala_recurrence_setup(Recurrence* rec);
 // mode: 1 = FP32-FFMA gather-GEMM, 2 = wgmma 3xTF32 gather-GEMM for the large contractions
 int net_forward(const Streams& st, const ParamLayout& pl, const float* params, const WeightImages& wi, const Inputs& in,
-                const Acts& act, int B, int T, int mode, bool retile);
+                const Acts& act, int B, int T, int mode, bool retile, const Recurrence& rec);
 int net_backward(const Streams& st, const ParamLayout& pl, const float* params, const WeightImages& wi, float* grads,
-                 const Inputs& in, const Acts& act, const Bwd& bwd, int B, int T, int mode);
+                 const Inputs& in, const Acts& act, const Bwd& bwd, int B, int T, int mode, const Recurrence& rec);
 // bytes of the operand images of the bulk-fed lstm_wgrad: which = 1 x^T (K = Mb), 3 dz^T (K = Mb)
 size_t lstm_image_bytes(int which, int M, int Mb);
 int forward_launch_count();

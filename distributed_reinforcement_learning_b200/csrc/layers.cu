@@ -5,8 +5,40 @@
 // mode 1) or the wgmma 3xTF32 tensor-core core (gemm_umma.cuh, math mode 2) -- same loaders and
 // epilogues.  Outside math mode 5 the small head layers (M x 256 x 256) use the FFMA core.
 #include "layer_defs.cuh"
+#include "r2d2_cluster.cuh"
 
 namespace drl {
+
+// ------------------------------------------------------------------------------------------
+// Recurrent mode (Recurrence, kernels.h; DESIGN.md section 21): the LSTM of each trajectory runs through its T steps
+// on the cluster kernels of r2d2_cluster.cuh at L = 256, RESTART variant: step 0 and every step after a done start from
+// the state the actor recorded for it, every other step from the previous step's output.  The BPTT walks the T - 2
+// steps that receive loss gradient (the time-major prefix of Mb = B (T - 2) rows) and carries nothing across a done.
+// ------------------------------------------------------------------------------------------
+using ImpClu = R2Clu<Geo::L>;
+
+__global__ void __launch_bounds__(ImpClu::T, 1) impala_lstm_fwd_cluster_kernel(
+    const float* __restrict__ zx, const float* __restrict__ bias, const float* __restrict__ Wh,
+    const float* __restrict__ h0, const float* __restrict__ c0, const uint8_t* __restrict__ done,
+    float* __restrict__ gates, float* __restrict__ tc, float* __restrict__ hout, float* __restrict__ hin,
+    float* __restrict__ cin, float* __restrict__ c_last, int B, int T) {
+  lstm_fwd_cluster_body<Geo::L, true>(zx, bias, Wh, h0, c0, done, gates, tc, hout, hin, cin, c_last, B, T);
+}
+
+__global__ void __launch_bounds__(ImpClu::T, 1) impala_lstm_bwd_cluster_kernel(
+    const float* __restrict__ dh_part, size_t part_stride, const float* __restrict__ gates,
+    const float* __restrict__ tc, const float* __restrict__ cin, const float* __restrict__ Wh,
+    const uint8_t* __restrict__ done, float* __restrict__ dz, int B, int T) {
+  lstm_bwd_cluster_body<Geo::L, true>(dh_part, part_stride, gates, tc, cin, Wh, done, dz, B, T - 2, T);
+}
+
+int impala_recurrence_setup(Recurrence* rec) {
+  return lstm_cluster_setup<Geo::L>(impala_lstm_fwd_cluster_kernel, impala_lstm_bwd_cluster_kernel, &rec->clusters_fwd,
+                                    &rec->clusters_bwd);
+}
+
+// one cluster per R = 8 trajectories, up to what the device places at once
+static int recurrence_grid(int B, int max_clusters) { return std::min(cdiv(B, ImpClu::R), max_clusters) * ImpClu::CL; }
 
 void FlatLayout::set(int n, const int64_t* sizes, int64_t* const* named) {
   num_tensors = n;
@@ -167,7 +199,7 @@ int net_retile(cudaStream_t, cudaStream_t s_rest, const ParamLayout& pl, const f
 }
 
 int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const WeightImages& wi, const Inputs& in,
-                const Acts& act, int B, int T, int mode, bool retile) {
+                const Acts& act, int B, int T, int mode, bool retile, const Recurrence& rec) {
   const int M = B * T;
   const RowMap map{B, T};
   int n = 0, nsplit = 4;
@@ -244,21 +276,34 @@ int net_forward(const Streams& st, const ParamLayout& pl, const float* P, const 
   }
   if (late_images) DRL_CUDA_CHECK(cudaStreamWaitEvent(st.main, st.ev[1], 0));
   else DRL_TRY(join_from_side(st, 1));
-  // LSTM pre-activation z = [a3 | emb | h0] W  (split-K partial sums; bias added in the gate kernel) (:18-25)
+  // LSTM pre-activation z = [a3 | emb | h0] W  (split-K partial sums; bias added in the gate kernel) (:18-25).
+  // Recurrent mode: only the K = 3392 input rows, [a3 | emb] W[:3392]; the h rows multiply inside the recurrence.
   {
     LstmA al{act.a3, act.table, in.pa, in.h0, map};
     PlainB bl{P + pl.lstm_w, Geo::G4, 0};
     EpRaw<false> ep{act.zpart, Geo::G4, (size_t)M * Geo::G4, 1.0f, 0, Geo::G4};
     // FFMA: 4 splits of 57 x 16.  Tensor cores: 128 x 256 tiles -> 5 x 4 output tiles x 7 splits of 17 x 32 (B = 32, T = 20)
+    // Recurrent mode (math modes 2 and 5): 7 splits of 512 = 8 K tiles of 64 or 16 of 32 (the last 320)
     nsplit = (mode >= 2) ? 7 : 4;
-    const int kchunk = m16 ? 576 : (mode >= 2) ? 544 : Geo::XK / 4;      // 16-bit: 9 K tiles of 64 per split
+    const int K = rec.on() ? Geo::FLAT + Geo::EMB : Geo::XK;
+    const int kchunk = rec.on() ? 512 : m16 ? 576 : (mode >= 2) ? 544 : Geo::XK / 4;   // 16-bit: 9 K tiles of 64 per split
     PretiledB<PlainB> blp{wi.img[3], m16 ? Geo::XK / 64 : Geo::XK / 32};
-    if (m16) GEMM16("lstm_fwd", X256L, al, blp, ep, M, Geo::G4, Geo::XK, nsplit, kchunk, kchunk);
-    else GEMM_W("lstm_fwd", CfgMid, U256L, al, bl, blp, ep, M, Geo::G4, Geo::XK, nsplit, kchunk, kchunk);
+    if (m16) GEMM16("lstm_fwd", X256L, al, blp, ep, M, Geo::G4, K, nsplit, kchunk, kchunk);
+    else GEMM_W("lstm_fwd", CfgMid, U256L, al, bl, blp, ep, M, Geo::G4, K, nsplit, kchunk, kchunk);
   }
-  KERNEL("lstm_gates_fwd",
-         lstm_gates_forward(s, act.zpart, nsplit, P + pl.lstm_b, in.c0, act.gates, act.c1, act.tc1, act.h1, M, B,
-                            T), 1);
+  if (rec.on()) {
+    KERNEL("lstm_x_reduce", splitk_reduce(s, act.zpart, (size_t)M * Geo::G4, nsplit, act.zx, (size_t)M * Geo::G4), 1);
+    prof_mark(s, "lstm_unroll_fwd");
+    DRL_CUDA_CHECK(launch_cluster_k(impala_lstm_fwd_cluster_kernel, ImpClu::CL, recurrence_grid(B, rec.clusters_fwd),
+                                    ImpClu::T, ImpClu::kFwdSmem, s, act.zx, P + pl.lstm_b,
+                                    P + pl.lstm_w + (size_t)(Geo::FLAT + Geo::EMB) * Geo::G4, in.h0, in.c0, in.done,
+                                    act.gates, act.tc1, act.h1, act.hin, act.cin, act.c1, B, T));
+    ++n;
+  } else {
+    KERNEL("lstm_gates_fwd",
+           lstm_gates_forward(s, act.zpart, nsplit, P + pl.lstm_b, in.c0, act.gates, act.c1, act.tc1, act.h1, M, B,
+                              T), 1);
+  }
   // heads (fully_connected, :27-30,40-41): z = 0 actor, z = 1 critic
   const size_t head_stride = (size_t)(pl.critic1_w - pl.actor1_w);
   if (late_images) {
@@ -381,7 +426,7 @@ static int conv_backward16(const Streams& st, const ParamLayout& pl, const Weigh
 }
 
 int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const WeightImages& wi, float* G,
-                 const Inputs& in, const Acts& act, const Bwd& bw, int B, int T, int mode) {
+                 const Inputs& in, const Acts& act, const Bwd& bw, int B, int T, int mode, const Recurrence& rec) {
   const bool m16 = mode == 5;
   cudaStream_t s = st.main;
   const cudaStream_t side = st.par ? st.side : st.main;
@@ -401,7 +446,11 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     // small head kernels
     DRL_TRY(fork_to_side(st, 0));
     prof_mark(side, "lstm_xt_image");
-    DRL_TRY((launch_retile_t16<128, Fmt16>(side, LstmAT{act.a3, act.table, in.pa, in.h0, map}, Geo::XK, Mb, act.img_xt)));
+    if (rec.on())
+      DRL_TRY((launch_retile_t16<128, Fmt16>(side, LstmHinAT{act.a3, act.table, in.pa, act.hin, map, Geo::L}, Geo::XK, Mb,
+                                             act.img_xt)));
+    else
+      DRL_TRY((launch_retile_t16<128, Fmt16>(side, LstmAT{act.a3, act.table, in.pa, in.h0, map}, Geo::XK, Mb, act.img_xt)));
     ++n;
   }
   // dlogits / dv / dhid2 are ready: three weight gradients can start beside the chain (on the second side lane if any)
@@ -454,8 +503,17 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
     else GEMM_FFMA_KS("heads_l1_dgrad", CfgSmall, 4, al, bl, ep, Mb, Geo::L, Geo::HID, 2, Geo::HID, 0);
   }
   // ---- LSTM cell ---------------------------------------------------------------------------
-  KERNEL("lstm_gates_bwd",
-         lstm_gates_backward(s, bw.dh_part, (size_t)Mb * Geo::L, act.gates, act.tc1, in.c0, bw.dz, Mb, B, T), 1);
+  if (rec.on()) {
+    prof_mark(s, "lstm_unroll_bwd");
+    DRL_CUDA_CHECK(launch_cluster_k(impala_lstm_bwd_cluster_kernel, ImpClu::CL, recurrence_grid(B, rec.clusters_bwd),
+                                    ImpClu::T, ImpClu::kBwdSmem, s, bw.dh_part, (size_t)Mb * Geo::L, act.gates, act.tc1,
+                                    act.cin, P + pl.lstm_w + (size_t)(Geo::FLAT + Geo::EMB) * Geo::G4, in.done, bw.dz, B,
+                                    T));
+    ++n;
+  } else {
+    KERNEL("lstm_gates_bwd",
+           lstm_gates_backward(s, bw.dh_part, (size_t)Mb * Geo::L, act.gates, act.tc1, in.c0, bw.dz, Mb, B, T), 1);
+  }
   DRL_TRY(fork_to_side(st, 3));
   s = side;
   {  // d lstm kernel [3648(+1), 1024] = x^T dz ; bias gradient = column sums of dz
@@ -471,6 +529,10 @@ int net_backward(const Streams& st, const ParamLayout& pl, const float* P, const
       DRL_TRY((launch_gemm_bulk16<BK256>(s, ImageOp{act.img_xt, ktm}, ImageOp{bw.img_dzt, ktm}, epw, Geo::XK, Geo::G4, Mb,
                                          1, Mb, 0)));
       n += 3;
+    } else if (rec.on()) {
+      LstmHinAT al{act.a3, act.table, in.pa, act.hin, map, Geo::L};
+      EpRaw<true> ep{G + pl.lstm_w, Geo::G4, 0, 1.0f, Geo::XK, Geo::G4};
+      GEMM("lstm_wgrad", CfgBig, U256, al, bl, ep, Geo::XK, Geo::G4, Mb, 1, Mb, 0);
     } else {
       LstmAT al{act.a3, act.table, in.pa, in.h0, map};
       EpRaw<true> ep{G + pl.lstm_w, Geo::G4, 0, 1.0f, Geo::XK, Geo::G4};

@@ -32,6 +32,7 @@ struct drl_learner : LearnerCore {
   WeightImages wimg{};
   VtraceOut vt{};
   OptState opt{};
+  Recurrence rec{};          // recurrent mode (cfg.recurrent = 1): cluster counts of the recurrence kernels
   // gradient exchange over NVLink peer memory (peer.cu); off until drl_learner_peer_import
   bool peer_on = false;
   int peer_nblk = 132 * 4;
@@ -68,7 +69,7 @@ Streams streams_of(const drl_learner* h) {
 // retile = true: (re)build the weight images first.  A training step always does (the parameters changed in the
 // previous apply); the forward-only entry points only when the images are stale.
 int enqueue_forward(drl_learner* h, const Inputs& in, int B, int T, bool retile) {
-  return net_forward(streams_of(h), h->pl, h->params, h->wimg, in, h->act, B, T, h->mode, retile);
+  return net_forward(streams_of(h), h->pl, h->params, h->wimg, in, h->act, B, T, h->mode, retile, h->rec);
 }
 
 int fwd_bwd(LearnerCore* core, int slot, int* launches) {
@@ -86,7 +87,8 @@ int fwd_bwd(LearnerCore* core, int slot, int* launches) {
                           h->T, h->A));
   }
   NvtxRange r("drl:backward");
-  DRL_TRY(net_backward(streams_of(h), h->pl, h->params, h->wimg, h->grads, in, h->act, h->bwd, h->B, h->T, h->mode));
+  DRL_TRY(net_backward(streams_of(h), h->pl, h->params, h->wimg, h->grads, in, h->act, h->bwd, h->B, h->T, h->mode,
+                       h->rec));
   if (launches) *launches += forward_launch_count() + 1 + backward_launch_count();   // + the V-trace/loss kernel
   return DRL_OK;
 }
@@ -191,6 +193,14 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
               "or 5 (wgmma with 16-bit split operands)");
     return DRL_ERR_INVALID;
   }
+  if (cfg->recurrent != 0 && cfg->recurrent != 1) {
+    set_error("recurrent must be 0 (one LSTM step from each step's recorded state) or 1 (unroll through the trajectory)");
+    return DRL_ERR_INVALID;
+  }
+  if (cfg->recurrent && (cfg->math_mode == 1 || cfg->math_mode == 3)) {
+    set_error("recurrent = 1 runs in math mode 5 (default) or 2; math mode %d is not supported with it", cfg->math_mode);
+    return DRL_ERR_INVALID;
+  }
   if (drl_device_count() <= cfg->device) { set_error("CUDA device %d not available (no CPU fallback)", cfg->device); return DRL_ERR_CUDA; }
 
   drl_learner* h = new drl_learner();
@@ -245,6 +255,12 @@ int drl_learner_create(const drl_learner_config* cfg, drl_learner** out) {
     DRL_TRY(dev_alloc(h, &a.logits, M * A));
     DRL_TRY(dev_alloc(h, &a.policy, M * A));
     DRL_TRY(dev_alloc(h, &a.value, M));
+    if (cfg->recurrent) {
+      DRL_TRY(impala_recurrence_setup(&h->rec));
+      DRL_TRY(dev_alloc(h, &a.zx, M * Geo::G4));
+      DRL_TRY(dev_alloc(h, &a.hin, M * Geo::L));
+      DRL_TRY(dev_alloc(h, &a.cin, M * Geo::L));
+    }
     if (h->mode == 5) {
       DRL_TRY(dev_alloc(h, &a.img_xt, lstm_image_bytes(1, (int)M, (int)Mb)));
       DRL_TRY(dev_alloc(h, &h->bwd.img_dzt, lstm_image_bytes(3, (int)M, (int)Mb)));
@@ -645,7 +661,9 @@ int drl_learner_read_buffer(drl_learner* h, const char* name, float* host_dst, i
       {"logits", h->act.logits, M * A}, {"policy", h->act.policy, M * A}, {"value", h->act.value, M},
       {"dlogits", h->bwd.dlogits, Mb * 32}, {"dv", h->bwd.dv, Mb * 32}, {"dhid2", h->bwd.dhid2, 2 * Mb * Geo::HID},
       {"dhid1", h->bwd.dhid1, 2 * Mb * Geo::HID}, {"dh_part", h->bwd.dh_part, 2 * Mb * Geo::L},
-      {"dz", h->bwd.dz, Mb * Geo::G4}, {"da3", h->bwd.da3, Mb * Geo::FLAT}, {"du", h->bwd.du, Mb * Geo::EMB},
+      {"dz", h->bwd.dz, Mb * Geo::G4}, {"hin", h->act.hin, M * Geo::L}, {"cin", h->act.cin, M * Geo::L},
+      {"hout", h->rec.on() ? h->act.h1 : nullptr, M * Geo::L}, {"tc", h->rec.on() ? h->act.tc1 : nullptr, M * Geo::L},
+      {"da3", h->bwd.da3, Mb * Geo::FLAT}, {"du", h->bwd.du, Mb * Geo::EMB},
       {"da2", h->bwd.da2, Mb * 81 * 64}, {"da1", h->bwd.da1, Mb * 400 * 32},
       // math mode 5's 16-bit planes, [hi | lo] bf16 (2 x 2 bytes per element: the buffer's count in 4-byte words)
       {"a1_plane", reinterpret_cast<float*>(h->act.a1p), M * 400 * 32},
@@ -662,7 +680,8 @@ int drl_learner_act(drl_learner* h, int32_t n, const uint8_t* state, const int32
   if (n < 1 || n > h->M) { set_error("act: n must be in [1, %d]", h->M); return DRL_ERR_INVALID; }
   if (!state || !previous_action || !h_in || !c_in) { set_error("act: null input pointer"); return DRL_ERR_INVALID; }
   DRL_TRY(set_device(h));
-  // reuse staging slot 0 as an [n, 1] batch (B = n, T = 1 makes the time-major/batch-major remap the identity)
+  // reuse staging slot 0 as an [n, 1] batch (B = n, T = 1 makes the time-major/batch-major remap the identity); one
+  // LSTM step from the given state in either mode
   const Inputs& in = h->in[0];
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->compute));
   DRL_CUDA_CHECK(cudaStreamSynchronize(h->copy));
@@ -674,7 +693,8 @@ int drl_learner_act(drl_learner* h, int32_t n, const uint8_t* state, const int32
   DRL_CUDA_CHECK(cp(in.h0, h_in, (size_t)n * Geo::L * 4));
   DRL_CUDA_CHECK(cp(in.c0, c_in, (size_t)n * Geo::L * 4));
   h->slots[0].has_data = false;   // the slot no longer holds a training batch
-  DRL_TRY(enqueue_forward(h, in, n, 1, h->images_stale));
+  DRL_TRY(net_forward(streams_of(h), h->pl, h->params, h->wimg, in, h->act, n, 1, h->mode, h->images_stale,
+                      Recurrence{}));
   h->images_stale = false;
   if (policy) DRL_CUDA_CHECK(cudaMemcpyAsync(policy, h->act.policy, (size_t)n * h->A * 4, cudaMemcpyDeviceToHost, h->compute));
   if (h_out) DRL_CUDA_CHECK(cudaMemcpyAsync(h_out, h->act.h1, (size_t)n * Geo::L * 4, cudaMemcpyDeviceToHost, h->compute));

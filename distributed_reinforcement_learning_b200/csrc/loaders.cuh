@@ -266,6 +266,22 @@ struct LstmAT {  // transposed view for dW = X^T dz : index i = feature (contigu
     return __ldg(reinterpret_cast<const float4*>(p));
   }
 };
+// [x | h_in]^T for the LSTM kernel gradient of an unrolled LSTM (the R2D2 learner; the IMPALA learner's recurrent mode):
+// feature index i < 3392 -> [a3 | emb] (as LstmAT), else h_in, the state the recurrence read (device, time-major [M, L])
+struct LstmHinAT {
+  static constexpr bool kContigK = false;
+  const float* e; const float* table; const int* pa; const float* hin; RowMap map; int L;
+  struct Row { int i; };
+  __device__ __forceinline__ Row row(int, int i) const { Row r; r.i = i; return r; }
+  __device__ __forceinline__ float4 load(const Row& r, int m) const {
+    if (r.i < 0) return zero4();
+    const float* p;
+    if (r.i < Geo::FLAT) p = e + (size_t)m * Geo::FLAT + r.i;
+    else if (r.i < Geo::FLAT + Geo::EMB) p = table + (size_t)__ldg(pa + map.src(m)) * Geo::EMB + (r.i - Geo::FLAT);
+    else p = hin + (size_t)m * L + (r.i - Geo::FLAT - Geo::EMB);
+    return __ldg(reinterpret_cast<const float4*>(p));
+  }
+};
 
 // --------------------------------------------------------------------------------------------
 // Ape-X dueling network operands (model/apex_value.py:22-41): both streams read

@@ -26,21 +26,6 @@
 
 namespace drl {
 
-// [x | h_in]^T for the LSTM kernel gradient: feature index i < 3392 -> [a3 | emb] (as LstmAT), else h_in (device, time-major)
-struct R2XhAT {
-  static constexpr bool kContigK = false;
-  const float* e; const float* table; const int* pa; const float* hin; RowMap map; int L;
-  struct Row { int i; };
-  __device__ __forceinline__ Row row(int, int i) const { Row r; r.i = i; return r; }
-  __device__ __forceinline__ float4 load(const Row& r, int m) const {
-    if (r.i < 0) return zero4();
-    const float* p;
-    if (r.i < Geo::FLAT) p = e + (size_t)m * Geo::FLAT + r.i;
-    else if (r.i < kR2Cat) p = table + (size_t)__ldg(pa + map.src(m)) * Geo::EMB + (r.i - Geo::FLAT);
-    else p = hin + (size_t)m * L + (r.i - kR2Cat);
-    return __ldg(reinterpret_cast<const float4*>(p));
-  }
-};
 // step input [a3 | emb[prev_action]] with the (t,b) -> (b,t) remap of prev_action (K = 3392)
 struct R2XA {
   static constexpr bool kContigK = true;
@@ -507,7 +492,7 @@ static int r2_backward(const drl_r2d2* h, const Streams& st, const float* P, con
   DRL_TRY(fork_to_side(st, 3));
   s = side;
   {  // d lstm kernel [3392 + L (+1), 4L] = [x | h_in]^T dz ; bias gradient = column sums of dz
-    R2XhAT al{act.a3, act.table, in.pa, act.hin, map, L};
+    LstmHinAT al{act.a3, act.table, in.pa, act.hin, map, L};
     PlainB bl{bw.dz, NG, 0};
     EpRaw<true> ep{G + pl.lstm_w, NG, 0, 1.0f, kR2Cat + L, NG};
     GEMM("lstm_wgrad", CfgBig, U256, al, bl, ep, kR2Cat + L, NG, M, 1, M, 0);

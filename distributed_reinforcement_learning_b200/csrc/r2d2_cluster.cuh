@@ -1,6 +1,7 @@
 // r2d2_cluster.cuh -- the R2D2 LSTM recurrence at lstm_size 256 and 512 (r2d2.cu keeps r2d2_lstm_fwd_kernel /
 // r2d2_lstm_bwd_kernel for 64): the same contracts, with W_h (L x 4L fp32: 1 MB at 256, 4 MB at 512) spread over a
 // thread-block cluster of CL = L / 32 CTAs (8, portable; 16, non-portable) so that it stays on chip for all S steps.
+// The IMPALA learner's recurrent mode (layers.cu) runs the same bodies at 256 in their RESTART variant.
 //
 // CTA `rank` of a cluster owns hidden units [32 rank, 32 rank + 32) and their four gate columns (i, j, f, o): 128 local
 // columns c, global column (c / 32) L + 32 rank + c % 32, so the cell update of a unit never leaves its CTA.  It holds
@@ -47,8 +48,12 @@ struct R2Clu {
 
 // Forward: as r2d2_lstm_fwd_kernel (zx [M, 4L] already holds the split-K sum; rows m = t B + b).  Grid: a multiple of
 // CL CTAs of T threads, cluster (CL, 1, 1), R2Clu<L>::kFwdSmem bytes of dynamic shared memory.
-template <int L>
-__global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_fwd_cluster_kernel(
+// RESTART = false (R2D2): h0 / c0 are [B, L], and done (optional, [B, S]) zeroes the state entering step t + 1.
+// RESTART = true (the IMPALA learner's recurrent mode): h0 / c0 are the states the actor recorded for every step, [B, S, L]
+// batch-major, and done [B, S] is required: after done[b, t] step t + 1 starts from the recorded (h0, c0)[b, t + 1]
+// instead of (h_t, c_t); nothing is zeroed.
+template <int L, bool RESTART>
+__device__ __forceinline__ void lstm_fwd_cluster_body(
     const float* __restrict__ zx, const float* __restrict__ bias, const float* __restrict__ Wh,
     const float* __restrict__ h0, const float* __restrict__ c0, const uint8_t* __restrict__ done,
     float* __restrict__ gates, float* __restrict__ tc, float* __restrict__ hout, float* __restrict__ hin,
@@ -81,10 +86,10 @@ __global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_fwd_cluster_kernel(
     const int b0 = ch * R;
     for (int i = tid; i < R * L; i += T) {
       const int b = b0 + i / L;
-      hbuf[i] = b < B ? h0[(size_t)b * L + i % L] : 0.f;
+      hbuf[i] = b < B ? h0[(RESTART ? (size_t)b * S : (size_t)b) * L + i % L] : 0.f;
     }
     float c_reg = 0.f;
-    if (cell && b0 + cr < B) c_reg = c0[(size_t)(b0 + cr) * L + cu];
+    if (cell && b0 + cr < B) c_reg = c0[(RESTART ? (size_t)(b0 + cr) * S : (size_t)(b0 + cr)) * L + cu];
     __syncthreads();
     for (int t = 0; t < S; ++t) {
       const float* hb = hbuf + (t & 1) * R * L;
@@ -96,7 +101,18 @@ __global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_fwd_cluster_kernel(
         zin[i] = b < B ? bias[g] + zx[((size_t)t * B + b) * G + g] : 0.f;
       }
       const bool live = cell && b0 + cr < B;
-      const float keep = (live && done && done[(size_t)(b0 + cr) * S + t]) ? 0.f : 1.f;
+      const float keep = (!RESTART && live && done && done[(size_t)(b0 + cr) * S + t]) ? 0.f : 1.f;
+      // RESTART: step t + 1 starts from the recorded (h_rec, c_rec); read here, before the product, like zin
+      bool restart = false;
+      float h_rec = 0.f, c_rec = 0.f;
+      if constexpr (RESTART) {
+        if (live && t + 1 < S && done[(size_t)(b0 + cr) * S + t]) {
+          restart = true;
+          const size_t r = ((size_t)(b0 + cr) * S + t + 1) * L + cu;
+          h_rec = h0[r];
+          c_rec = c0[r];
+        }
+      }
       float acc[R];
 #pragma unroll
       for (int r = 0; r < R; ++r) acc[r] = 0.f;
@@ -154,10 +170,10 @@ __global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_fwd_cluster_kernel(
           hout[o] = h;
           if (c_last) c_last[o] = cv;
         }
-        c_reg = cv * keep;
+        c_reg = RESTART ? (restart ? c_rec : cv) : cv * keep;
         if (t + 1 < S) {
           float* dst = hbuf + ((t + 1) & 1) * R * L + cr * L + cu;
-          const float hk2 = h * keep;
+          const float hk2 = RESTART ? (restart ? h_rec : h) : h * keep;
 #pragma unroll
           for (int q = 0; q < K::CL; ++q) *cluster.map_shared_rank(dst, q) = hk2;
         }
@@ -167,13 +183,25 @@ __global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_fwd_cluster_kernel(
   }
 }
 
-// BPTT: as r2d2_lstm_bwd_kernel (dhout, gates, tc, cin, done -> dz [M, 4L]).  Thread k (< L) holds row k of the CTA's
-// slice, W_h[k, its 128 columns].  Grid and cluster as the forward, R2Clu<L>::kBwdSmem bytes of dynamic shared memory.
 template <int L>
-__global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_bwd_cluster_kernel(
-    const float* __restrict__ dhout, const float* __restrict__ gates, const float* __restrict__ tc,
+__global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_fwd_cluster_kernel(
+    const float* __restrict__ zx, const float* __restrict__ bias, const float* __restrict__ Wh,
+    const float* __restrict__ h0, const float* __restrict__ c0, const uint8_t* __restrict__ done,
+    float* __restrict__ gates, float* __restrict__ tc, float* __restrict__ hout, float* __restrict__ hin,
+    float* __restrict__ cin, float* __restrict__ c_last, int B, int S) {
+  lstm_fwd_cluster_body<L, false>(zx, bias, Wh, h0, c0, done, gates, tc, hout, hin, cin, c_last, B, S);
+}
+
+// BPTT: as r2d2_lstm_bwd_kernel (dhout, gates, tc, cin, done -> dz [M, 4L]) over S steps; done is [B, dstride].  Thread
+// k (< L) holds row k of the CTA's slice, W_h[k, its 128 columns].  Grid and cluster as the forward, R2Clu<L>::kBwdSmem
+// bytes of dynamic shared memory.  A done step carries nothing back from the next one, whether the forward zeroed the
+// state after it (R2D2) or restarted from a recorded one (RESTART).  RESTART: dL/dh_out is the sum of two partials,
+// dhout[m] + dhout[dh_stride + m] (the IMPALA actor and critic heads), added in that order.
+template <int L, bool RESTART>
+__device__ __forceinline__ void lstm_bwd_cluster_body(
+    const float* __restrict__ dhout, size_t dh_stride, const float* __restrict__ gates, const float* __restrict__ tc,
     const float* __restrict__ cin, const float* __restrict__ Wh, const uint8_t* __restrict__ done,
-    float* __restrict__ dz, int B, int S) {
+    float* __restrict__ dz, int B, int S, int dstride) {
   using K = R2Clu<L>;
   constexpr int NC = K::NC, R = K::R, G = K::G, CL = K::CL;
   kernel_prologue();
@@ -208,10 +236,11 @@ __global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_bwd_cluster_kernel(
           m = (size_t)t * B + b;
           const float* g = gates + m * G + cu;
           dho = dhout[m * L + cu];
+          if constexpr (RESTART) dho += dhout[dh_stride + m * L + cu];
           si = g[0]; tj = g[L]; sf = g[2 * L]; so = g[3 * L];
           tcv = tc[m * L + cu];
           cprev = cin[m * L + cu];
-          keep = done[(size_t)b * S + t] ? 0.f : 1.f;
+          keep = done[(size_t)b * dstride + t] ? 0.f : 1.f;
         }
         float dh_next = 0.f;
         if (t + 1 < S) {
@@ -270,6 +299,14 @@ __global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_bwd_cluster_kernel(
   }
 }
 
+template <int L>
+__global__ void __launch_bounds__(R2Clu<L>::T, 1) r2d2_lstm_bwd_cluster_kernel(
+    const float* __restrict__ dhout, const float* __restrict__ gates, const float* __restrict__ tc,
+    const float* __restrict__ cin, const float* __restrict__ Wh, const uint8_t* __restrict__ done,
+    float* __restrict__ dz, int B, int S) {
+  lstm_bwd_cluster_body<L, false>(dhout, 0, gates, tc, cin, Wh, done, dz, B, S, S);
+}
+
 // cudaLaunchKernelEx with a (cl, 1, 1) cluster: capturable into a CUDA graph like launch_k
 template <class... KA, class... A>
 inline cudaError_t launch_cluster_k(void (*kern)(KA...), int cl, dim3 grid, dim3 block, size_t smem, cudaStream_t s,
@@ -289,14 +326,12 @@ inline cudaError_t launch_cluster_k(void (*kern)(KA...), int cl, dim3 grid, dim3
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KA>(args)...);
 }
 
-// Create-time set-up of the two kernels at width L (outside any capture): the dynamic shared memory and, at CL = 16,
-// the non-portable cluster size; then how many clusters of the planned shape the device places at once (0: none ->
-// the caller fails the create rather than let a step wait forever).
-template <int L>
-int r2d2_cluster_setup(int* max_fwd, int* max_bwd) {
+// Create-time set-up of a forward / BPTT kernel pair at width L (outside any capture): the dynamic shared memory and, at
+// CL = 16, the non-portable cluster size; then how many clusters of the planned shape the device places at once (0:
+// none -> the caller fails the create rather than let a step wait forever).
+template <int L, class KF, class KB>
+int lstm_cluster_setup(KF kf, KB kb, int* max_fwd, int* max_bwd) {
   using K = R2Clu<L>;
-  auto kf = r2d2_lstm_fwd_cluster_kernel<L>;
-  auto kb = r2d2_lstm_bwd_cluster_kernel<L>;
   DRL_CUDA_CHECK(cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K::kFwdSmem));
   DRL_CUDA_CHECK(cudaFuncSetAttribute(kb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K::kBwdSmem));
   if (K::CL > 8) {
@@ -325,6 +360,11 @@ int r2d2_cluster_setup(int* max_fwd, int* max_bwd) {
     return DRL_ERR_CUDA;
   }
   return DRL_OK;
+}
+
+template <int L>
+int r2d2_cluster_setup(int* max_fwd, int* max_bwd) {
+  return lstm_cluster_setup<L>(r2d2_lstm_fwd_cluster_kernel<L>, r2d2_lstm_bwd_cluster_kernel<L>, max_fwd, max_bwd);
 }
 
 }  // namespace drl

@@ -26,7 +26,10 @@ class NativeLearner(LearnerHandle):
                  discount_factor=0.99, start_learning_rate=0.0006, end_learning_rate=0.0,
                  learning_frame=1000000000, baseline_loss_coef=1.0, entropy_coef=0.05,
                  gradient_clip_norm=40.0, reward_clipping="abs_one", device=0, num_slots=2,
-                 use_cuda_graph=True, math_mode=0):
+                 use_cuda_graph=True, math_mode=0, recurrent=False):
+        """recurrent=True: the LSTM runs through the T steps of each trajectory from the recorded state of step 0,
+        restarting from the recorded state after every done step, with BPTT over the unroll (DESIGN.md section 21);
+        False: the reference's learner, one LSTM step from every step's recorded state."""
         if reward_clipping not in N.REWARD_CLIPPING:
             raise ValueError("reward_clipping must be one of %s" % sorted(N.REWARD_CLIPPING))   # utils.py:45
         h, w, c = input_shape
@@ -36,7 +39,8 @@ class NativeLearner(LearnerHandle):
         cfg = N.LearnerConfig(self.B, self.T, h, w, c, self.A, self.L, discount_factor, start_learning_rate,
                               end_learning_rate, float(learning_frame), baseline_loss_coef, entropy_coef,
                               gradient_clip_norm, N.REWARD_CLIPPING[reward_clipping], self.device, int(num_slots),
-                              int(bool(use_cuda_graph)), int(math_mode))
+                              int(bool(use_cuda_graph)), int(math_mode), int(bool(recurrent)))
+        self.recurrent = bool(recurrent)
         self._create(cfg, self.device, num_slots)
         self._peer = False
         self._no_collective = False          # diagnostic only (bench.py --collective none)

@@ -52,7 +52,7 @@ typedef struct drl_learner_config {
   int32_t trajectory;         /* T, 3..32 (config.json:136)                                      */
   int32_t height, width, channels; /* 84,84,4 -- only this geometry is supported (config.json:133) */
   int32_t num_action;         /* A, 2..32 (config.json:134)                                     */
-  int32_t lstm_size;          /* 256 -- only this size is supported (config.json:137)           */
+  int32_t lstm_size;          /* 256 -- only this size is supported (config.json:137); see also `recurrent` */
   float discount_factor;      /* agent/impala.py:51                                             */
   float start_learning_rate;  /* agent/impala.py:96                                             */
   float end_learning_rate;
@@ -67,6 +67,16 @@ typedef struct drl_learner_config {
   int32_t math_mode;          /* 0 = default (5); 1 = FP32 FFMA; 2 = wgmma 3xTF32; 3 = same, persistent kernels;
                                  5 = wgmma on bf16 hi/lo split operands (three products, fp32-grade) + bulk-fed
                                  LSTM weight gradient; any other value (4 included) is DRL_ERR_INVALID */
+  int32_t recurrent;          /* 0 = the reference's learner: every step is one LSTM step from the (h, c) the actor
+                                 recorded for it, no gradient through time.  1 = the LSTM runs through the T steps of
+                                 each trajectory from the recorded state of step 0; after a done step the next step
+                                 restarts from its recorded state; BPTT over the T - 2 steps with loss gradient, not
+                                 across a done; the recorded states get no gradient (DESIGN.md section 21).  Same
+                                 parameters, checkpoints and entry points; drl_learner_act stays one step.  Math
+                                 modes 5 (default) and 2 only (1 and 3 -> DRL_ERR_INVALID).  The recurrent mode adds
+                                 the named buffers "hin", "cin" (state each step read), "hout", "tc" (tanh c) for
+                                 drl_learner_read_buffer.  Any other value -> DRL_ERR_INVALID, before any device
+                                 lookup. */
 } drl_learner_config;
 
 /* Results of one step: the 4 floats Agent.train returns (agent/impala.py:144-148) + grad norm. */
