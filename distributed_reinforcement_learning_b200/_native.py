@@ -71,7 +71,8 @@ class R2d2Config(C.Structure):
     _fields_ = [("batch", C.c_int32), ("seq_len", C.c_int32), ("burn_in", C.c_int32), ("height", C.c_int32),
                 ("width", C.c_int32), ("channels", C.c_int32), ("num_action", C.c_int32), ("lstm_size", C.c_int32),
                 ("discount_factor", C.c_float), ("learning_rate", C.c_float), ("device", C.c_int32),
-                ("num_slots", C.c_int32), ("use_cuda_graph", C.c_int32), ("math_mode", C.c_int32)]
+                ("num_slots", C.c_int32), ("use_cuda_graph", C.c_int32), ("math_mode", C.c_int32),
+                ("n_step", C.c_int32), ("priority_rule", C.c_int32), ("priority_eta", C.c_float)]
 
 
 class R2d2Out(C.Structure):

@@ -15,6 +15,8 @@ the learner branch of ``train_r2d2.py:87-165`` runs on it unchanged, with the TF
                        as one device-resident step -> (loss, td_error)
   Agent.main_q_value_test / target_q_value_test   agent/r2d2.py:193-217
   Agent.save_weights / load_weights (new) both scopes and the Adam state in one .npz, as apex.Agent's
+  Agent.set_n_step / set_priority_eta (new) the R2D2 paper's n-step targets and mixed max / mean priorities
+                       (DESIGN.md section 22); switching keeps the parameters and the Adam state
 """
 import os
 import random
@@ -54,6 +56,7 @@ class Agent:
         self._slot = 0
         self._last = {}
         self._train_calls = 0
+        self.n_step, self.priority_eta = 1, None     # set_n_step / set_priority_eta
         self._lock = threading.RLock()   # actor threads sync from / act on this agent while the learner thread trains
         _AGENTS[model_name] = self
 
@@ -84,9 +87,40 @@ class Agent:
             self._engine = NativeR2D2Learner(
                 batch=batch, seq_len=self.seq_len, burn_in=self.burn_in, num_action=self.num_action,
                 lstm_size=self.lstm_size, input_shape=tuple(self.input_shape), discount_factor=self.discount_factor,
-                device=self.device, num_slots=2, use_cuda_graph=self.use_cuda_graph)
+                device=self.device, num_slots=2, use_cuda_graph=self.use_cuda_graph, n_step=self.n_step,
+                priority_eta=self.priority_eta)
             self._push_state()
         return self._engine
+
+    def _rebuild_with(self, **kw):
+        """Apply learner settings that live in the engine's configuration: the next call rebuilds the engine with
+        the parameters, target network and Adam state it had."""
+        with self._lock:
+            if any(getattr(self, k) != v for k, v in kw.items()) and self._engine is not None:
+                self._pull_state()
+                self._engine.close()
+                self._engine = None
+            for k, v in kw.items():
+                setattr(self, k, v)
+
+    def set_n_step(self, n):
+        """Train on n-step double-Q targets (the R2D2 paper uses n = 5; 1, the default, is the reference's one-step
+        target).  The constructor keeps the reference's 12 arguments.  1 <= n <= seq_len - burn_in - 1."""
+        n = int(n)
+        if not 1 <= n <= self.seq_len - self.burn_in - 1:
+            raise ValueError("n_step must be in [1, seq_len - burn_in - 1 = %d] (got %d)"
+                             % (self.seq_len - self.burn_in - 1, n))
+        self._rebuild_with(n_step=n)
+
+    def set_priority_eta(self, eta):
+        """Give each sequence the priority eta max_t |td| + (1 - eta) mean_t |td| (the R2D2 paper uses 0.9); None, the
+        default, keeps the reference's |mean_t td|.  It applies to train's td_error, get_td_error and the priorities
+        of a DeviceMemory."""
+        if eta is not None:
+            eta = float(eta)
+            if not 0.0 <= eta <= 1.0:
+                raise ValueError("priority_eta must be None or in [0, 1] (got %r)" % eta)
+        self._rebuild_with(priority_eta=eta)
 
     @staticmethod
     def _u8(state):

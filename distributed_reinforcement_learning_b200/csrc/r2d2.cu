@@ -248,6 +248,11 @@ __global__ void __launch_bounds__(kR2H) r2d2_out_bwd_kernel(const float* __restr
 //   loss = mean_b w_b mean_i (target - sav)^2 ; td[b] = |mean_i (target - sav)|
 // The two rescalings are evaluated in float64: h^-1 subtracts 1 from sqrt(1 + 4 eps (..)) ~ 1.002, which costs float32
 // three digits.  One block; a warp owns sequences b = warp, warp + 8, ...; all reductions in a fixed order.
+// NSTEP (r2d2_td_nstep_kernel, DESIGN.md section 22): the n-step double-Q target over k = min(n, S - 1 - t) steps,
+//   G = sum_{j<k} (prod_{l<j} D_{t+l}) r[t+j] + (prod_{l<k} D_{t+l}) h^-1(target_q[t+k][argmax main_q[t+k]]),
+//   D = gamma (1 - done), target = h(G), all in float64; and, when `mixed`, the priority
+//   td[b] = eta max_i |diff| + (1 - eta) mean_i |diff| instead of |mean_i diff|.  At k = 1 the target expression is the
+//   one-step one term for term (G = r exactly), so n = 1 reproduces its bits.
 // ------------------------------------------------------------------------------------------
 struct R2TdArgs {
   const float* mq; const float* tq;            // [M, A] time-major
@@ -267,7 +272,8 @@ __device__ __forceinline__ double r2_hinv(double x) {
   const double r = (sqrt(1.0 + 4.0 * 1e-3 * (fabs(x) + 1.0 + 1e-3)) - 1.0) / (2.0 * 1e-3);
   return s * (r * r - 1.0);
 }
-__global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
+template <bool NSTEP>
+__device__ __forceinline__ void r2d2_td_body(const R2TdArgs& a, int n, bool mixed, float eta) {
   kernel_prologue();
   __shared__ float red[8];
   const int Nt = a.S - a.burn_in - 1;
@@ -285,27 +291,45 @@ __global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
   float wloss = 0.f;
   for (int b = warp; b < a.B; b += 8) {
     const float w = a.weight ? a.weight[b] : 1.0f;
-    float sdiff = 0.f, ssq = 0.f;
+    float sdiff = 0.f, ssq = 0.f, sabs = 0.f, mabs = 0.f;
     for (int i = lane; i < Nt; i += 32) {
       const int t = a.burn_in + i;
       const size_t m = (size_t)t * a.B + b, mn = (size_t)(t + 1) * a.B + b;
+      // NSTEP: the bootstrap row is t + k, the horizon k = min(n, S - 1 - t) cut at the last step of the sequence
+      const size_t mb = NSTEP ? (size_t)(t + min(n, a.S - 1 - t)) * a.B + b : mn;
       const int act = a.action[(size_t)b * a.S + t];
       float best = -INFINITY;
       int arg = 0;
       for (int k = 0; k < a.A; ++k) {
-        const float v = a.mq[mn * a.A + k];
+        const float v = a.mq[mb * a.A + k];
         if (v > best) { best = v; arg = k; }
       }
       const bool act_ok = act >= 0 && act < a.A;            // tf.one_hot: an out-of-range action selects nothing
       const float sav = act_ok ? a.mq[m * a.A + act] : 0.f;
-      const float nsav = a.tq[mn * a.A + arg];
-      const double disc = a.done[(size_t)b * a.S + t] ? 0.0 : (double)a.discount;
-      const float target = (float)r2_h(r2_hinv((double)nsav) * disc + (double)a.reward[(size_t)b * a.S + t]);
+      const float nsav = a.tq[mb * a.A + arg];
+      float target;
+      if constexpr (NSTEP) {
+        const size_t r0 = (size_t)b * a.S + t;
+        const int hz = min(n, a.S - 1 - t);
+        double ret = 0.0, disc = 1.0;        // sum_{j<k} (prod_{l<j} D) r[t+j], then prod_{l<k} D
+        for (int j = 0; j < hz; ++j) {
+          ret += disc * (double)a.reward[r0 + j];
+          disc *= a.done[r0 + j] ? 0.0 : (double)a.discount;
+        }
+        target = (float)r2_h(r2_hinv((double)nsav) * disc + ret);
+      } else {
+        const double disc = a.done[(size_t)b * a.S + t] ? 0.0 : (double)a.discount;
+        target = (float)r2_h(r2_hinv((double)nsav) * disc + (double)a.reward[(size_t)b * a.S + t]);
+      }
       const float diff = target - sav;
       a.sav[(size_t)b * Nt + i] = sav;
       a.target_value[(size_t)b * Nt + i] = target;
       sdiff += diff;
       ssq += diff * diff;
+      if (NSTEP && mixed) {
+        sabs += fabsf(diff);
+        mabs = fmaxf(mabs, fabsf(diff));
+      }
       if (a.dq) {
         const float g = -2.0f * w * diff / ((float)Nt * (float)a.B);
         if (act_ok) {
@@ -316,8 +340,12 @@ __global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
     }
     sdiff = warp_sum(sdiff);
     ssq = warp_sum(ssq);
+    if (NSTEP && mixed) {
+      sabs = warp_sum(sabs);
+      mabs = warp_max(mabs);
+    }
     if (lane == 0) {
-      const float td = fabsf(sdiff / (float)Nt);
+      const float td = (NSTEP && mixed) ? eta * mabs + (1.0f - eta) * (sabs / (float)Nt) : fabsf(sdiff / (float)Nt);
       a.td_dev[b] = td;
       if (a.td_host) a.td_host[b] = td;
       wloss += w * (ssq / (float)Nt);
@@ -333,6 +361,13 @@ __global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
       *a.loss = s / (float)a.B;
     }
   }
+}
+__global__ void __launch_bounds__(256) r2d2_td_kernel(R2TdArgs a) {
+  r2d2_td_body<false>(a, 1, false, 0.f);
+}
+// n >= 1; mixed: the priority rule eta max |diff| + (1 - eta) mean |diff| (eta in [0, 1]), otherwise |mean diff|
+__global__ void __launch_bounds__(256) r2d2_td_nstep_kernel(R2TdArgs a, int n, int mixed, float eta) {
+  r2d2_td_body<true>(a, n, mixed != 0, eta);
 }
 
 
@@ -545,7 +580,12 @@ int drl::enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, flo
   a.dq = train ? h->bwd.dq : nullptr; a.dmean = train ? h->bwd.dmean : nullptr;
   a.loss = train ? h->loss : nullptr;
   prof_mark(h->compute, "td_target_loss");
-  DRL_CUDA_CHECK((launch_k(r2d2_td_kernel, 1, 256, 0, h->compute, a)));
+  const int n_step = std::max(h->cfg.n_step, 1);
+  if (n_step > 1 || h->cfg.priority_rule == 1)
+    DRL_CUDA_CHECK((launch_k(r2d2_td_nstep_kernel, 1, 256, 0, h->compute, a, n_step, h->cfg.priority_rule,
+                             h->cfg.priority_eta)));
+  else
+    DRL_CUDA_CHECK((launch_k(r2d2_td_kernel, 1, 256, 0, h->compute, a)));
   if (launches) *launches += 1;
   return DRL_OK;
 }
@@ -620,6 +660,19 @@ int drl_r2d2_create(const drl_r2d2_config* cfg, drl_r2d2** out) {
     return DRL_ERR_INVALID;
   }
   if (cfg->math_mode < 0 || cfg->math_mode > 2) { set_error("math_mode must be 0 (default), 1 (FP32 FFMA) or 2 (wgmma 3xTF32)"); return DRL_ERR_INVALID; }
+  const int Nt = cfg->seq_len - cfg->burn_in - 1;
+  if (cfg->n_step < 0 || cfg->n_step > Nt) {
+    set_error("n_step must be 0 or 1 (one-step targets) or at most seq_len - burn_in - 1 = %d (got %d)", Nt, cfg->n_step);
+    return DRL_ERR_INVALID;
+  }
+  if (cfg->priority_rule != 0 && cfg->priority_rule != 1) {
+    set_error("priority_rule must be 0 (|mean td|) or 1 (eta max |td| + (1 - eta) mean |td|) (got %d)", cfg->priority_rule);
+    return DRL_ERR_INVALID;
+  }
+  if (cfg->priority_rule == 1 && !(cfg->priority_eta >= 0.0f && cfg->priority_eta <= 1.0f)) {
+    set_error("priority_eta must be finite and in [0, 1] (got %g)", (double)cfg->priority_eta);
+    return DRL_ERR_INVALID;
+  }
   if (drl_device_count() <= cfg->device) { set_error("CUDA device %d not available (no CPU fallback)", cfg->device); return DRL_ERR_CUDA; }
   drl_r2d2* h = new drl_r2d2();
   h->cfg = *cfg;

@@ -80,8 +80,8 @@ namespace drl {
 
 // both unrolls (main and target scope) + TD kernel over the nb sequences held by `in` on the compute stream (the target
 // unroll on its own stream pair when the step runs parallel); train = also the head gradients and the loss.  Writes
-// |mean_t(target - q)| per sequence to td_dev and, when td_host is not null, to td_host.  Adds the launches to
-// *launches unless it is null.
+// the per-sequence priority (|mean_t(target - q)|, or the mixed max / mean rule of cfg.priority_rule) to td_dev and, when
+// td_host is not null, to td_host.  Adds the launches to *launches unless it is null.
 int enqueue_forward_td(drl_r2d2* h, const R2In& in, int nb, bool train, float* td_host, int* launches);
 
 }  // namespace drl

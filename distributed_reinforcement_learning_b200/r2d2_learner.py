@@ -3,7 +3,8 @@
 ``step`` is ``r2d2.Agent.train`` (agent/r2d2.py:132-159) minus the Python/TF session: the stored-state LSTM unroll of
 the main and the target scope over seq_len steps, double-Q targets with value-function rescaling over the
 post-burn-in window, the weighted loss, BPTT through all steps of the main scope and TF1 Adam; it returns the new
-priorities |mean_t(target - q)|.
+priorities |mean_t(target - q)|.  ``n_step`` and ``priority_eta`` select the R2D2 paper's n-step targets and mixed
+max / mean priorities instead.
 """
 import ctypes as C
 
@@ -17,14 +18,21 @@ class NativeR2D2Learner(AdamLearnerHandle):
     family = "r2d2"
 
     def __init__(self, batch, seq_len=15, burn_in=7, num_action=4, lstm_size=64, input_shape=(84, 84, 1),
-                 discount_factor=0.997, learning_rate=1e-4, device=0, num_slots=2, use_cuda_graph=False, math_mode=0):
+                 discount_factor=0.997, learning_rate=1e-4, device=0, num_slots=2, use_cuda_graph=False, math_mode=0,
+                 n_step=1, priority_eta=None):
+        """n_step > 1: the R2D2 paper's n-step double-Q target, the horizon cut at the end of each sequence (1 <= n <=
+        seq_len - burn_in - 1); 1: the reference's one-step target.  priority_eta: None gives each sequence the
+        reference's priority |mean_t td|; a value in [0, 1] gives eta max_t |td| + (1 - eta) mean_t |td| (the paper
+        uses 0.9), for every |td| the learner returns and the device replay memory stores (DESIGN.md section 22)."""
         h, w, c = input_shape
         self.B, self.S, self.bi, self.A, self.L = int(batch), int(seq_len), int(burn_in), int(num_action), int(lstm_size)
         self.Nt = self.S - self.bi - 1
         self.input_shape = (int(h), int(w), int(c))
         self.device = int(device)
         cfg = N.R2d2Config(self.B, self.S, self.bi, h, w, c, self.A, self.L, discount_factor, learning_rate,
-                           self.device, int(num_slots), int(bool(use_cuda_graph)), int(math_mode))
+                           self.device, int(num_slots), int(bool(use_cuda_graph)), int(math_mode), int(n_step),
+                           0 if priority_eta is None else 1, 0.0 if priority_eta is None else float(priority_eta))
+        self.n_step, self.priority_eta = int(n_step), priority_eta
         self._create(cfg, self.device, num_slots)
 
     def main_to_target(self):

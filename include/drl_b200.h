@@ -1019,6 +1019,17 @@ typedef struct drl_r2d2_config {
   int32_t num_slots;
   int32_t use_cuda_graph;
   int32_t math_mode;          /* 0 = default (2); 1 = FP32 FFMA; 2 = wgmma 3xTF32 for the large contractions */
+  int32_t n_step;             /* 0 or 1 = the reference's one-step double-Q target (agent/r2d2.py:62-88).  n in
+                                 [2, seq_len - burn_in - 1] = the R2D2 paper's n-step target: window t bootstraps from
+                                 step t + k, k = min(n, seq_len - 1 - t), through the discounted rewards r[t..t+k-1]; a
+                                 done inside the horizon cuts every later reward and the bootstrap (DESIGN.md section
+                                 22).  Negative or larger values -> DRL_ERR_INVALID, before any device lookup. */
+  int32_t priority_rule;      /* the per-sequence |td| of drl_r2d2_step / _wait / _td_error and of the device replay
+                                 memory's priorities: 0 = |mean_t td| (agent/r2d2.py:154-157); 1 = the R2D2 paper's
+                                 priority_eta max_t |td| + (1 - priority_eta) mean_t |td|.  Other values ->
+                                 DRL_ERR_INVALID, before any device lookup.  The loss is the same under both rules. */
+  float priority_eta;         /* read when priority_rule = 1 (the paper uses 0.9): finite and in [0, 1], otherwise
+                                 DRL_ERR_INVALID, before any device lookup */
 } drl_r2d2_config;
 
 typedef struct drl_r2d2_out {
